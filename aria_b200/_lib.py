@@ -83,6 +83,9 @@ SIGNATURES = {
     "aria_ep_dispatch": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp]),
     "aria_attention_fwd": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64, i32, f32, i32, vp, i64, vp]),
     "aria_attention_fwd_workspace_bytes": (i64, [i32, i32, i32, i32, i32, i32]),
+    "aria_attention_fwd_lse": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64, i32, f32, i32, vp, i64, vp]),
+    "aria_attention_bwd_workspace_bytes": (i64, [i32, i32, i32, i32, i32]),
+    "aria_attention_bwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, vp, i64, vp]),
     "aria_attention_decode": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i64, i64, i64, i64, f32, vp, i64, vp]),
     "aria_attention_decode_workspace_bytes": (i64, [i32, i32, i32]),
 }
@@ -109,7 +112,7 @@ def load():
 
 
 # kernels launched per C-ABI call (for bench.py's `gpu_launches`; memsets are not counted)
-KERNELS_PER_CALL = {"router_topk": 2, "attention_decode": 2, "moe_block_fwd": 9}
+KERNELS_PER_CALL = {"router_topk": 2, "attention_decode": 2, "attention_bwd": 3, "moe_block_fwd": 9}
 launch_count = 0
 
 

@@ -35,11 +35,13 @@ struct AttnParams {
   float scale_log2;
   const uint8_t* key_mask;  // [B, Tk] 1 = masked out
   __nv_bfloat16* out;       // [B, Tq, H*out_hd]
+  float* lse;               // [B, H, Tq] natural-log logsumexp of scale * q.k (LSE instantiations only)
   int n_q_tiles;
 };
 
-// HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM)
-template <int HD, bool CAUSAL>
+// HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM); LSE: also store the row logsumexp
+// (what the backward needs to recompute P)
+template <int HD, bool CAUSAL, bool LSE>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -206,6 +208,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     l_lo += __shfl_xor_sync(0xffffffffu, l_lo, o_);
     l_hi += __shfl_xor_sync(0xffffffffu, l_hi, o_);
   }
+  if constexpr (LSE) {
+    // sum_k 2^(s_k - m) = l for ANY m (the lazy max included), so log2-sum-exp2 = m + log2 l; -inf for a row that sees no key
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int hrow = 0; hrow < 2; ++hrow) {
+        const int q = r_lo + 8 * hrow;
+        const float l = hrow ? l_hi : l_lo, m = hrow ? m_hi : m_lo;
+        if (q < p.Tq) p.lse[static_cast<int64_t>(bh) * p.Tq + q] = l > 0.f ? (m + log2f(l)) * 0.6931471805599453f : -INFINITY;
+      }
+    }
+  }
   const int64_t ld = static_cast<int64_t>(p.H) * p.out_hd;
 #pragma unroll
   for (int hrow = 0; hrow < 2; ++hrow) {
@@ -329,31 +342,20 @@ static int make_tmap_heads(CUtensorMap* tm, const void* ptr, int T, int H, int B
   return make_tmap_bf16(tm, ptr, 4, dims, str, box);
 }
 
-template <int HD, bool CAUSAL>
+template <int HD, bool CAUSAL, bool LSE>
 static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, int64_t grid,
                        cudaStream_t stream) {
-  auto kern = attn_fwd_kernel<HD, CAUSAL>;
+  auto kern = attn_fwd_kernel<HD, CAUSAL, LSE>;
   static bool attr_set[kMaxDevices] = {};
   if (ensure_dynamic_smem(attr_set, kern, AT_SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
   kern<<<static_cast<int>(grid), AT_THREADS, AT_SMEM, stream>>>(tmQ, tmK, tmV, p);
   return check_launch("attn_fwd_kernel");
 }
 
-}  // namespace aria
-
-using namespace aria;
-
-extern "C" int64_t aria_attention_fwd_workspace_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk, int32_t out_hd, int32_t causal) {
-  (void)B; (void)H; (void)Tq; (void)Tk; (void)out_hd; (void)causal;
-  return 0;  // one CTA per (batch, head, 128 queries): no partial results to merge
-}
-
-extern "C" int aria_attention_fwd(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask, int32_t B,
-                                  int32_t H, int32_t Tq, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h,
-                                  int64_t kv_stride_b, int64_t kv_stride_h, int32_t out_hd, float scale, int32_t causal,
-                                  void* workspace, int64_t workspace_bytes, aria_stream_t stream_) {
-  (void)workspace; (void)workspace_bytes;
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// aria_attention_fwd and aria_attention_fwd_lse: one launcher, the logsumexp store is a compile-time flag of the same kernel
+static int attention_fwd(const void* q, const void* k, const void* v, void* out, float* lse, const uint8_t* key_mask, int32_t B,
+                         int32_t H, int32_t Tq, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
+                         int64_t kv_stride_h, int32_t out_hd, float scale, int32_t causal, cudaStream_t stream) {
   ARIA_CHECK_ARG(q && k && v && out);
   ARIA_CHECK_ARG(B > 0 && H > 0 && Tq > 0 && Tk > 0 && Tk >= (causal ? Tq : 0));
   ARIA_CHECK_ARG(out_hd > 0 && out_hd <= AT_D && out_hd % 8 == 0);
@@ -374,11 +376,44 @@ extern "C" int aria_attention_fwd(const void* q, const void* k, const void* v, v
   p.scale_log2 = scale * 1.4426950408889634f;
   p.key_mask = key_mask;
   p.out = static_cast<__nv_bfloat16*>(out);
+  p.lse = lse;
   p.n_q_tiles = (Tq + AT_BM - 1) / AT_BM;
   const int64_t grid = static_cast<int64_t>(B) * H * p.n_q_tiles;
   ARIA_CHECK_ARG(grid < (1ll << 31));
-  if (out_hd <= 80) return causal ? launch_attn<80, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<80, false>(tmQ, tmK, tmV, p, grid, stream);
-  return causal ? launch_attn<128, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<128, false>(tmQ, tmK, tmV, p, grid, stream);
+  if (lse) {
+    if (out_hd <= 80) return causal ? launch_attn<80, true, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<80, false, true>(tmQ, tmK, tmV, p, grid, stream);
+    return causal ? launch_attn<128, true, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<128, false, true>(tmQ, tmK, tmV, p, grid, stream);
+  }
+  if (out_hd <= 80) return causal ? launch_attn<80, true, false>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<80, false, false>(tmQ, tmK, tmV, p, grid, stream);
+  return causal ? launch_attn<128, true, false>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<128, false, false>(tmQ, tmK, tmV, p, grid, stream);
+}
+
+}  // namespace aria
+
+using namespace aria;
+
+extern "C" int64_t aria_attention_fwd_workspace_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk, int32_t out_hd, int32_t causal) {
+  (void)B; (void)H; (void)Tq; (void)Tk; (void)out_hd; (void)causal;
+  return 0;  // one CTA per (batch, head, 128 queries): no partial results to merge
+}
+
+extern "C" int aria_attention_fwd(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask, int32_t B,
+                                  int32_t H, int32_t Tq, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h,
+                                  int64_t kv_stride_b, int64_t kv_stride_h, int32_t out_hd, float scale, int32_t causal,
+                                  void* workspace, int64_t workspace_bytes, aria_stream_t stream_) {
+  (void)workspace; (void)workspace_bytes;
+  return attention_fwd(q, k, v, out, nullptr, key_mask, B, H, Tq, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, out_hd,
+                       scale, causal, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int aria_attention_fwd_lse(const void* q, const void* k, const void* v, void* out, float* lse, const uint8_t* key_mask,
+                                      int32_t B, int32_t H, int32_t Tq, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h,
+                                      int64_t kv_stride_b, int64_t kv_stride_h, int32_t out_hd, float scale, int32_t causal,
+                                      void* workspace, int64_t workspace_bytes, aria_stream_t stream_) {
+  (void)workspace; (void)workspace_bytes;
+  ARIA_CHECK_ARG(lse);
+  return attention_fwd(q, k, v, out, lse, key_mask, B, H, Tq, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, out_hd,
+                       scale, causal, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int64_t aria_attention_decode_workspace_bytes(int32_t B, int32_t H, int32_t Tk) {

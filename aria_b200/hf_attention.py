@@ -9,9 +9,11 @@ for a purely causal batch and the 2-D padding mask otherwise).  The module keeps
 
     prefill / chunked prefill (Tq > 1)  -> aria_attention_fwd   (causal, queries are the last Tq positions of Tk keys)
     decode (Tq == 1)                    -> aria_attention_decode (split-KV streaming kernel)
+    training (Tq > 1, q/k/v need grad)  -> attention_train.AttentionFunction: aria_attention_fwd_lse, and aria_attention_bwd
+                                           in the backward (works under gradient checkpointing with use_reentrant=False)
 
-Padded batches: the 2-D padding mask becomes the kernels' key mask (prefill and decode).
-No fallback: MHA with head_dim 128, bf16, CUDA, no dropout, no autograd — anything else raises.
+Padded batches: the 2-D padding mask becomes the kernels' key mask (prefill, decode and the backward).
+No fallback: MHA with head_dim 128, bf16, CUDA, no dropout, no decode under autograd — anything else raises.
 (Our own mirror `aria_b200.moe_lm.AriaAttention` fuses q/k/v + RoPE + the cache write into the projection GEMM and is what
 bench.py times; this seam exists so that an unmodified HF/reference model can switch the core by changing one config string.)
 """
@@ -22,6 +24,7 @@ from typing import Optional
 import torch
 
 from . import ops
+from .attention_train import AttentionFunction
 
 IMPL_KEY = "aria_b200"
 
@@ -33,8 +36,9 @@ def aria_b200_attention_forward(module, query: torch.Tensor, key: torch.Tensor, 
     (attn_output [B, Tq, H, 128], None) — the contract of transformers' attention interface."""
     if dropout:
         raise NotImplementedError("aria_b200 attention: dropout is not supported (inference / frozen-attention path)")
-    if torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad):
-        raise RuntimeError("aria_b200 attention: inference-only core (no autograd through the kernel); run under torch.no_grad()")
+    train = torch.is_grad_enabled() and (query.requires_grad or key.requires_grad or value.requires_grad)
+    if train and query.shape[2] == 1:
+        raise RuntimeError("aria_b200 attention: decode (one query) has no backward; run it under torch.no_grad()")
     if is_causal is False or getattr(module, "is_causal", True) is False:
         raise NotImplementedError("aria_b200 attention: only causal self-attention goes through this seam")
     B, H, Tq, hd = query.shape
@@ -59,6 +63,9 @@ def aria_b200_attention_forward(module, query: torch.Tensor, key: torch.Tensor, 
     v = value.contiguous()
     if k.stride() != v.stride():
         v = v.clone(memory_format=torch.contiguous_format)
+    if train:
+        out = AttentionFunction.apply(query.contiguous(), k, v, scale, True, key_mask)                  # [B, Tq, H*128]
+        return out.view(B, Tq, H, hd), None
     if Tq == 1:
         out = ops.attention_decode(query.reshape(B, H, hd).contiguous(), k, v, Tk, scale, key_mask=key_mask)   # [B, H*128]
         return out.view(B, 1, H, hd), None

@@ -539,15 +539,21 @@ def add_pos_embedding(x: torch.Tensor, pos_ids: torch.Tensor, table: torch.Tenso
 
 
 # ------------------------------------------------------------------------------------------- attention
-def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tq: int, Tk: int, scale: float, causal: bool,
-              out_hd: int = 128, key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """q [B,H,>=Tq,128], k/v [B,H,>=Tk,128] head-major (first Tq/Tk rows used) -> out [B, Tq, H*out_hd].
-    Token rows must be 128 contiguous bf16 at a row stride of 128 (a slice q[:, :, pos0:] of a staging buffer is fine)."""
+def _attn_qkv_check(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, what: str):
     for t in (q, k, v):
         if not (t.is_cuda and t.dtype == bf16 and t.dim() == 4 and t.stride(-1) == 1 and t.stride(-2) == 128 and t.data_ptr() % 16 == 0):
-            raise RuntimeError("attention: q/k/v must be CUDA bf16 [B,H,T,128] with 128-element token rows (16-byte aligned)")
-    B, H = q.shape[0], q.shape[1]
+            raise RuntimeError(f"{what}: q/k/v must be CUDA bf16 [B,H,T,128] with 128-element token rows (16-byte aligned)")
     assert q.shape[-1] == 128 and k.shape[-1] == 128 and k.stride() == v.stride()
+
+
+def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tq: int, Tk: int, scale: float, causal: bool,
+              out_hd: int = 128, key_mask: Optional[torch.Tensor] = None, return_lse: bool = False):
+    """q [B,H,>=Tq,128], k/v [B,H,>=Tk,128] head-major (first Tq/Tk rows used) -> out [B, Tq, H*out_hd].
+    Token rows must be 128 contiguous bf16 at a row stride of 128 (a slice q[:, :, pos0:] of a staging buffer is fine).
+    return_lse=True -> (out, lse): lse [B, H, Tq] fp32 is the natural-log logsumexp of scale * q.k over the visible keys
+    (-inf for a row that sees none), what `attention_bwd` needs; `out` is bit-identical to the return_lse=False call."""
+    _attn_qkv_check(q, k, v, "attention")
+    B, H = q.shape[0], q.shape[1]
     assert q.shape[2] >= Tq and k.shape[2] >= Tk
     out = torch.empty((B, Tq, H * out_hd), dtype=bf16, device=q.device)
     if key_mask is not None:
@@ -557,10 +563,47 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tq: int, Tk: in
     ws_bytes = lib.aria_attention_fwd_workspace_bytes(B, H, Tq, Tk, out_hd, int(causal))
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device) if ws_bytes > 0 else None
     with torch.cuda.device(q.device):
+        if return_lse:
+            lse = torch.empty((B, H, Tq), dtype=torch.float32, device=q.device)
+            L.check(lib.aria_attention_fwd_lse(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(key_mask), B, H, Tq, Tk, q.stride(0),
+                                               q.stride(1), k.stride(0), k.stride(1), out_hd, scale, int(causal), _p(ws), ws_bytes,
+                                               _stream(q)), "attention_fwd")
+            return out, lse
         L.check(lib.aria_attention_fwd(_p(q), _p(k), _p(v), _p(out), _p(key_mask), B, H, Tq, Tk, q.stride(0), q.stride(1),
                                        k.stride(0), k.stride(1), out_hd, scale, int(causal), _p(ws), ws_bytes, _stream(q)),
                 "attention_fwd")
     return out
+
+
+def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                  Tq: int, Tk: int, scale: float, causal: bool, key_mask: Optional[torch.Tensor] = None):
+    """Backward of `attention(..., return_lse=True)` (head dim 128): q [B,H,>=Tq,128], k/v [B,H,>=Tk,128] as in the forward,
+    out / dout [B, Tq, H*128] token-major, lse [B, H, Tq] -> (dq [B,H,Tq,128], dk [B,H,Tk,128], dv [B,H,Tk,128]) bf16.
+    dk and dv are bit-reproducible; dq's last bits depend on the order of fp32 atomic additions."""
+    _attn_qkv_check(q, k, v, "attention_bwd")
+    B, H = q.shape[0], q.shape[1]
+    assert q.shape[2] >= Tq and k.shape[2] >= Tk
+    _chk(out), _chk(dout), _chk(lse, torch.float32, align=4)
+    assert out.shape == (B, Tq, H * 128) and dout.shape == out.shape and lse.shape == (B, H, Tq)
+    if key_mask is not None:
+        _chk(key_mask, torch.uint8)
+        assert key_mask.shape == (B, Tk)
+    dq = torch.empty((B, H, Tq, 128), dtype=bf16, device=q.device)
+    dk = torch.empty((B, H, Tk, 128), dtype=bf16, device=q.device)
+    dv = torch.empty_like(dk)
+    lib = L.load()
+    ws_bytes = lib.aria_attention_bwd_workspace_bytes(B, H, Tq, Tk, int(causal))
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    # the kernel reads q with q's strides and writes dq with the same strides; k/v/dk/dv likewise share theirs
+    if q.stride() != dq.stride():
+        q = q[:, :, :Tq].contiguous()
+    if k.stride() != dk.stride():
+        k, v = k[:, :, :Tk].contiguous(), v[:, :, :Tk].contiguous()
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_bwd(_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(dq), _p(dk), _p(dv), _p(key_mask),
+                                       B, H, Tq, Tk, q.stride(0), q.stride(1), k.stride(0), k.stride(1), scale, int(causal),
+                                       _p(ws), ws_bytes, _stream(q)), "attention_bwd")
+    return dq, dk, dv
 
 
 def attention_decode(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tk: int, scale: float,

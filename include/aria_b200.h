@@ -263,6 +263,24 @@ int aria_attention_fwd(const void* q, const void* k, const void* v, void* out, c
 /* Scratch bytes aria_attention_fwd wants in `workspace` (0 for this build: one CTA per (batch, head, 128 queries), no partial
  * results to merge).  workspace may be NULL. */
 int64_t aria_attention_fwd_workspace_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk, int32_t out_hd, int32_t causal);
+/* aria_attention_fwd that also writes lse [B, H, Tq] fp32: the natural-log logsumexp of scale * q.k over the keys the row sees,
+ * -inf for a row that sees none (e.g. a left-padded query row).  `out` is bit-identical to aria_attention_fwd's (same kernel). */
+int aria_attention_fwd_lse(const void* q, const void* k, const void* v, void* out, float* lse, const uint8_t* key_mask,
+                           int32_t B, int32_t H, int32_t Tq, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h,
+                           int64_t kv_stride_b, int64_t kv_stride_h, int32_t out_hd, float scale, int32_t causal,
+                           void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* Backward of aria_attention_fwd for head_dim 128, with the forward's (Tq <= Tk, causal, key_mask) conventions:
+ *   q, dq [B, H, Tq, 128] at the q strides; k, v, dk, dv [B, H, Tk, 128] at the kv strides (head-major, 128-element rows);
+ *   out, dout [B, Tq, H*128] token-major (the forward's output layout); lse from aria_attention_fwd_lse.
+ *   dq = scale * dS k, dk = scale * dS^T q, dv = P^T dout with P = exp(scale * q k^T - lse), dS = P o (dout v^T - rowsum(dout o out)).
+ * A query row with lse = -inf contributes nothing; a key that is masked out or that no query sees gets dk = dv = 0.
+ * dk and dv are bit-reproducible; dq is summed over key tiles with fp32 atomics, so its last bits depend on their order.
+ * workspace: aria_attention_bwd_workspace_bytes(...) bytes, 16-byte aligned.  Three kernel launches. */
+int64_t aria_attention_bwd_workspace_bytes(int32_t B, int32_t H, int32_t Tq, int32_t Tk, int32_t causal);
+int aria_attention_bwd(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
+                       void* dq, void* dk, void* dv, const uint8_t* key_mask, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
+                       int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
+                       int32_t causal, void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 /* Single-token decode against a KV cache (HBM-bound, split-KV): q element (b,h,:) at q + b*q_stride_b + h*q_stride_h
  * (128 contiguous bf16), cache [B,H,Tk_max,128], out [B, H*128].  workspace: B*H*splits*(128+2) floats.
  * key_mask [B, Tk] uint8 or NULL: 1 = key is masked OUT (padded batch: the HF 2-D attention_mask inverted). */
