@@ -4,12 +4,15 @@
 //     S = Q K^T   (A = Q tile, B = K tile, both K-major SW128 in shared memory, S accumulates in registers)
 //     O += P V    (A = P, bf16, straight from the registers that held S; B = V tile consumed MN-major — V is [keys, d] with d
 //                  contiguous, exactly the HF cache layout — O accumulates in registers)
-//   warpgroup 0: TMA producer (Q once, K/V through a two-stage ring); warpgroups 1-2: 64 query rows each, fp32 online
-//   softmax on the fragments (four threads share a row: max / sum over two shuffles) and the final normalise + store.
+//   warpgroup 0: TMA producer (Q once, K/V through a ring of separately released K and V slots); warpgroups 1-2: 64 query
+//   rows each, fp32 online softmax on the fragments (four threads share a row: max / sum over two shuffles) and the final
+//   normalise + store.  The two consumer warpgroups take turns issuing their wgmmas (ping-pong on named barriers), so one
+//   runs its softmax while the other's products run; at HD = 80 each also issues S_{j+1} with PV_j before its softmax.
 //   One CTA per (batch, head, 128 queries); causal launches visit the heaviest query tiles first.
 // Replaces flash_attn_func / SDPA behind LLAMA_ATTENTION_CLASSES (aria/model/moe_lm.py:594) and the
 // Idefics2 / nn.MultiheadAttention attention of the ViT + projector (vision_encoder.py:120, projector.py:93), whose
-// 72-wide heads live in 128-wide rows: QK contracts HD = 80 columns (5 k-steps), PV produces all 128 and only out_hd are stored.
+// 72-wide heads live in 128-wide rows: at HD = 80 only columns 0-79 of K and V are loaded (a 64-column SW128 box plus a
+// 16-column SW32 box), QK contracts 80 columns (5 k-steps) and PV produces 80 (m64n64 + m64n16); out_hd of them are stored.
 // Scores and softmax statistics stay fp32.  The running row max is raised lazily, only when it grows by more than 2^8: P then
 // lies in [0, 256] and is rounded to bf16 at that scale, which measured closer to transformers' eager attention (the reference
 // of the ViT path) than rounding P relative to the exact running max, and it skips most rescales of O.
@@ -23,11 +26,23 @@ namespace aria {
 constexpr int AT_BM = 128;   // queries per CTA
 constexpr int AT_BN = 128;   // keys per step
 constexpr int AT_D = 128;    // head dim (row width of q / k / v)
-constexpr int AT_TILE = AT_BM * AT_D * 2;  // 32 KB
+constexpr int AT_TILE = AT_BM * AT_D * 2;  // 32 KB: the Q tile, and one K or V ring slot at HD = 128
 constexpr int AT_HALF = AT_TILE / 2;       // one SW128 column chunk: [128 rows][64 bf16]
-constexpr int AT_STAGES = 2;
 constexpr int AT_THREADS = 384;            // producer warpgroup + two consumer warpgroups
-constexpr int AT_SMEM = 1024 + AT_TILE /*Q*/ + AT_STAGES * 2 * AT_TILE /*K, V*/ + 256;
+constexpr uint32_t AT_BAR_TURN = 1;        // named barriers 1, 2: consumer warpgroup 0 / 1 may issue its wgmmas
+
+// Per head-dim layout.  HD = 128: a K (or V) ring slot is two SW128 column chunks.  HD = 80: the SW128 chunk of columns
+// 0-63 plus a [128 keys][16] SW32 tile of columns 64-79, 20 KB instead of 32, which leaves room for a four-stage ring.
+template <int HD>
+struct AttnCfg {
+  static constexpr int KV_TILE = HD == 80 ? AT_HALF + AT_BN * 32 : AT_TILE;
+  static constexpr int STAGES = HD == 80 ? 4 : 2;
+  static constexpr int NO = HD == 80 ? 80 : 128;  // output columns PV produces
+  // S_{j+1} in flight during the softmax of block j needs a second score fragment; at HD = 128 it does not fit beside the
+  // 64-register O without spills, so that path runs the ping-pong alone
+  static constexpr bool INTRA = HD == 80;
+  static constexpr int SMEM = 1024 + AT_TILE /*Q*/ + STAGES * 2 * KV_TILE /*K, V*/ + 256;
+};
 
 struct AttnParams {
   int B, H, Tq, Tk;
@@ -40,21 +55,24 @@ struct AttnParams {
 };
 
 // HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM); LSE: also store the row logsumexp
-// (what the backward needs to recompute P)
+// (what the backward needs to recompute P).  tmK16 / tmV16: 16-column SW32 boxes of columns 64-79 (HD = 80 only).
 template <int HD, bool CAUSAL, bool LSE>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmK16,
+                const __grid_constant__ CUtensorMap tmV16, const AttnParams p) {
+  constexpr int S = AttnCfg<HD>::STAGES, KVT = AttnCfg<HD>::KV_TILE, NO = AttnCfg<HD>::NO;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;                            // [2 chunks][128 rows][64]
-  uint8_t* sK = sQ + AT_TILE;                    // [STAGES][32 KB]
-  uint8_t* sV = sK + AT_STAGES * AT_TILE;        // [STAGES][32 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + AT_STAGES * AT_TILE);
+  uint8_t* sK = sQ + AT_TILE;                    // [STAGES][KV_TILE]
+  uint8_t* sV = sK + S * KVT;                    // [STAGES][KV_TILE]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + S * KVT);
   uint64_t* q_full = bars;                       // [1]
   uint64_t* k_full = bars + 1;                   // [STAGES]
-  uint64_t* v_full = k_full + AT_STAGES;         // [STAGES]
-  uint64_t* kv_empty = v_full + AT_STAGES;       // [STAGES], one arrival per consumer warp
+  uint64_t* v_full = k_full + S;                 // [STAGES]
+  uint64_t* k_empty = v_full + S;                // [STAGES], one arrival per consumer warp
+  uint64_t* v_empty = k_empty + S;               // [STAGES], one arrival per consumer warp
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
   const int BH = p.B * p.H;
@@ -70,11 +88,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     prefetch_tmap(&tmQ);
     prefetch_tmap(&tmK);
     prefetch_tmap(&tmV);
+    if (HD == 80) {
+      prefetch_tmap(&tmK16);
+      prefetch_tmap(&tmV16);
+    }
     mbar_init(q_full, 1);
-    for (int i = 0; i < AT_STAGES; ++i) {
+    for (int i = 0; i < S; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 8);
+      mbar_init(&k_empty[i], 8);
+      mbar_init(&v_empty[i], 8);
     }
     fence_mbar_init();
   }
@@ -87,21 +110,27 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       mbar_arrive_expect_tx(q_full, AT_TILE);
       tma_load_4d(sQ, &tmQ, q_full, 0, q0, h, b);
       tma_load_4d(sQ + AT_HALF, &tmQ, q_full, 64, q0, h, b);
+      // K slots are freed once both warpgroups hold S_j, V slots after PV_j: the K loads run ahead of the V loads
       for (int j = 0; j < n_kv; ++j) {
-        const int s = j % AT_STAGES;
-        mbar_wait(&kv_empty[s], ((j / AT_STAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(&k_full[s], AT_TILE);
-        tma_load_4d(sK + s * AT_TILE, &tmK, &k_full[s], 0, j * AT_BN, h, b);
-        tma_load_4d(sK + s * AT_TILE + AT_HALF, &tmK, &k_full[s], 64, j * AT_BN, h, b);
-        mbar_arrive_expect_tx(&v_full[s], AT_TILE);
-        tma_load_4d(sV + s * AT_TILE, &tmV, &v_full[s], 0, j * AT_BN, h, b);
-        tma_load_4d(sV + s * AT_TILE + AT_HALF, &tmV, &v_full[s], 64, j * AT_BN, h, b);
+        const int s = j % S;
+        const uint32_t ph = ((j / S) & 1) ^ 1;
+        mbar_wait(&k_empty[s], ph);
+        mbar_arrive_expect_tx(&k_full[s], KVT);
+        tma_load_4d(sK + s * KVT, &tmK, &k_full[s], 0, j * AT_BN, h, b);
+        tma_load_4d(sK + s * KVT + AT_HALF, HD == 80 ? &tmK16 : &tmK, &k_full[s], 64, j * AT_BN, h, b);
+        mbar_wait(&v_empty[s], ph);
+        mbar_arrive_expect_tx(&v_full[s], KVT);
+        tma_load_4d(sV + s * KVT, &tmV, &v_full[s], 0, j * AT_BN, h, b);
+        tma_load_4d(sV + s * KVT + AT_HALF, HD == 80 ? &tmV16 : &tmV, &v_full[s], 64, j * AT_BN, h, b);
       }
     }
     return;
   }
 
   // =========================== consumer warpgroup cw: query rows [q0 + 64 cw, +64) ===========================
+  // FlashAttention-3 schedule.  Inside a warpgroup, S_j = Q K_j^T is issued together with PV_{j-1}, and the softmax of block
+  // j runs while PV_{j-1} is in flight.  Across the two warpgroups, named barriers hand the right to issue back and forth
+  // (ping-pong), so one warpgroup's products run while the other does its softmax.
   setmaxnreg_inc<240>();
   const int cw = wg - 1;
   const int r_lo = q0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's two rows: r_lo and r_lo + 8
@@ -109,31 +138,52 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int kq = 2 * (lane & 3);                                  // key / column offset of this thread in an 8-wide block
   const uint8_t* km = p.key_mask ? p.key_mask + static_cast<int64_t>(b) * p.Tk : nullptr;
   const uint32_t sQa = smem_u32(sQ) + cw * 64 * 128, sKa = smem_u32(sK), sVa = smem_u32(sV);
+  const uint32_t my_turn = AT_BAR_TURN + cw, other_turn = AT_BAR_TURN + (cw ^ 1);
   // K-major k-step kk (16 columns of the head): chunk kk / 4, +32 B per step inside the chunk
   auto kmaj_off = [](int kk) { return static_cast<uint32_t>((kk >> 2) * AT_HALF + (kk & 3) * 32); };
-  // V MN-major: LBO = 16 KB between the two 64-column chunks, SBO = 1024 (8 keys), +2048 B per 16 keys
-  const uint64_t dV0 = make_smem_desc(sVa, AT_HALF, 1024);
 
-  float o[64];
+  float o[NO / 2];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  for (int i = 0; i < NO / 2; ++i) o[i] = 0.f;
   float m_lo = -INFINITY, m_hi = -INFINITY, l_lo = 0.f, l_hi = 0.f;
-  mbar_wait(q_full, 0);
+  float sc[64];       // scores of the newest block, then its P (fp32)
+  uint32_t pa[8][4];  // P of the previous block as the A operand of PV: k-step kk = {row lo keys +0/+1, row hi, lo +8/+9, hi}
+  float f_lo = 1.f, f_hi = 1.f;
 
-  for (int j = 0; j < n_kv; ++j) {
-    const int s = j % AT_STAGES;
-    const uint32_t ph = (j / AT_STAGES) & 1;
-    float sc[64];
-    mbar_wait(&k_full[s], ph);
-    wgmma_fence();
+  // S = Q K^T over the K tile in ring slot s.  HD = 80: k-steps 0-3 on the SW128 chunk, k-step 4 (columns 64-79) with K
+  // from its SW32 tile; Q keeps both SW128 chunks.
+  auto issue_qk = [&](int s) {
+    const uint32_t kt = sKa + s * KVT;
+    constexpr int KS = HD == 80 ? 4 : HD / 16;
 #pragma unroll
-    for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_m64n128_ss<0, 0>(sc, make_smem_desc(sQa + kmaj_off(kk), 16, 1024),
-                             make_smem_desc(sKa + s * AT_TILE + kmaj_off(kk), 16, 1024), kk ? 1u : 0u);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(sc);
-
+    for (int kk = 0; kk < KS; ++kk)
+      wgmma_m64n128_ss<0, 0>(sc, make_smem_desc(sQa + kmaj_off(kk), 16, 1024), make_smem_desc(kt + kmaj_off(kk), 16, 1024),
+                             kk ? 1u : 0u);
+    if constexpr (HD == 80)
+      wgmma_m64n128_ss<0, 0>(sc, make_smem_desc(sQa + kmaj_off(4), 16, 1024), make_smem_desc_sw32(kt + AT_HALF, 256), 1u);
+  };
+  // O += P V over the V tile in ring slot s, V consumed MN-major.  HD = 128: m64n128 over both SW128 chunks (LBO = 16 KB
+  // between them, SBO = 1024 per 8 keys, +2048 B per 16 keys).  HD = 80: m64n64 on the SW128 chunk (o[0..31]) and
+  // m64n16 on the SW32 tile (o[32..39]; SBO = 256 per 8 keys, +512 B per 16 keys).
+  auto issue_pv = [&](int s) {
+    const uint32_t vt = sVa + s * KVT;
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+      if constexpr (HD == 80) {
+        wgmma_m64n64_rs<1>(*reinterpret_cast<float(*)[32]>(&o[0]), pa[kk], make_smem_desc(vt + kk * 2048, AT_HALF, 1024));
+        wgmma_m64n16_rs<1>(*reinterpret_cast<float(*)[8]>(&o[32]), pa[kk], make_smem_desc_sw32(vt + AT_HALF + kk * 512, 256));
+      } else {
+        wgmma_m64n128_rs<1>(o, pa[kk], make_smem_desc(vt + kk * 2048, AT_HALF, 1024));
+      }
+    }
+  };
+  auto release = [&](uint64_t* bar) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar);
+  };
+  // Online softmax of block j on sc, in place (sc becomes P in fp32).  Returns whether the row max was raised; O must then
+  // be scaled by f_lo / f_hi before PV_j, which is done once PV_{j-1} has landed.
+  auto softmax = [&](int j) -> bool {
     const int k0 = j * AT_BN;
     const bool need_mask = (k0 + AT_BN > p.Tk) || (CAUSAL && (k0 + AT_BN - 1 > pos_off + q0 + cw * 64)) || km != nullptr;
     if (need_mask) {  // rare path (diagonal / tail / padded keys): -inf on dead keys
@@ -163,24 +213,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const float mc_lo = fmaxf(m_lo, mx_lo * p.scale_log2), mc_hi = fmaxf(m_hi, mx_hi * p.scale_log2);
     const bool up_lo = (mc_lo - m_lo > 8.0f) || (m_lo == -INFINITY && mc_lo > -INFINITY);
     const bool up_hi = (mc_hi - m_hi > 8.0f) || (m_hi == -INFINITY && mc_hi > -INFINITY);
-    if (__any_sync(0xffffffffu, up_lo || up_hi)) {
-      const float f_lo = !up_lo ? 1.f : (m_lo == -INFINITY ? 0.f : fast_ex2(m_lo - mc_lo));
-      const float f_hi = !up_hi ? 1.f : (m_hi == -INFINITY ? 0.f : fast_ex2(m_hi - mc_hi));
+    const bool rescale = __any_sync(0xffffffffu, up_lo || up_hi);
+    if (rescale) {
+      f_lo = !up_lo ? 1.f : (m_lo == -INFINITY ? 0.f : fast_ex2(m_lo - mc_lo));
+      f_hi = !up_hi ? 1.f : (m_hi == -INFINITY ? 0.f : fast_ex2(m_hi - mc_hi));
       if (up_lo) m_lo = mc_lo;
       if (up_hi) m_hi = mc_hi;
       l_lo *= f_lo;
       l_hi *= f_hi;
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
-        o[4 * jj] *= f_lo;
-        o[4 * jj + 1] *= f_lo;
-        o[4 * jj + 2] *= f_hi;
-        o[4 * jj + 3] *= f_hi;
-      }
     }
     const float neg_lo = (m_lo == -INFINITY) ? 0.f : -m_lo, neg_hi = (m_hi == -INFINITY) ? 0.f : -m_hi;
-    // P as the A operand of the PV product: k-step kk (keys 16 kk..) = {row lo keys +0/+1, row hi, row lo keys +8/+9, row hi}
-    uint32_t pa[8][4];
 #pragma unroll
     for (int kk = 0; kk < 8; ++kk) {
 #pragma unroll
@@ -189,18 +231,108 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const float x0 = fast_ex2(fmaf(sc[8 * kk + 2 * r], p.scale_log2, hi ? neg_hi : neg_lo));
         const float x1 = fast_ex2(fmaf(sc[8 * kk + 2 * r + 1], p.scale_log2, hi ? neg_hi : neg_lo));
         if (hi) l_hi += x0 + x1; else l_lo += x0 + x1;
-        pa[kk][r] = pack_bf16(x0, x1);
+        sc[8 * kk + 2 * r] = x0;
+        sc[8 * kk + 2 * r + 1] = x1;
       }
     }
-    mbar_wait(&v_full[s], ph);
-    wgmma_fence();
+    return rescale;
+  };
+  auto rescale_o = [&]() {
 #pragma unroll
-    for (int kk = 0; kk < 8; ++kk) wgmma_m64n128_rs<1>(o, pa[kk], dV0 + ((s * AT_TILE + kk * 2048) >> 4));
+    for (int jj = 0; jj < NO / 8; ++jj) {
+      o[4 * jj] *= f_lo;
+      o[4 * jj + 1] *= f_lo;
+      o[4 * jj + 2] *= f_hi;
+      o[4 * jj + 3] *= f_hi;
+    }
+  };
+  auto pack_p = [&]() {
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) pa[kk][r] = pack_bf16(sc[8 * kk + 2 * r], sc[8 * kk + 2 * r + 1]);
+    }
+  };
+
+  mbar_wait(q_full, 0);
+  if (cw == 1) named_bar_arrive(other_turn, 256);  // warpgroup 0 issues first
+
+  if constexpr (!AttnCfg<HD>::INTRA) {
+    // HD = 128: ping-pong only.  S_j and PV_j are issued in turns of their own and each is waited for before the next step.
+    for (int j = 0; j < n_kv; ++j) {
+      const int s = j % S;
+      const uint32_t ph = (j / S) & 1;
+      mbar_wait(&k_full[s], ph);
+      named_bar_sync(my_turn, 256);
+      wgmma_fence();
+      issue_qk(s);
+      wgmma_commit();
+      named_bar_arrive(other_turn, 256);
+      wgmma_wait<0>();
+      fence_regs(sc);
+      release(&k_empty[s]);
+      if (softmax(j)) rescale_o();
+      pack_p();
+      mbar_wait(&v_full[s], ph);
+      named_bar_sync(my_turn, 256);
+      wgmma_fence();
+      issue_pv(s);
+      wgmma_commit();
+      if (cw == 0 || j + 1 < n_kv) named_bar_arrive(other_turn, 256);  // warpgroup 1 issues last: no turn to hand back
+      wgmma_wait<0>();
+      fence_regs(o);
+      release(&v_empty[s]);
+    }
+  } else {
+    // block 0: S_0 alone (O is still zero, nothing to rescale)
+    mbar_wait(&k_full[0], 0);
+    named_bar_sync(my_turn, 256);
+    wgmma_fence();
+    issue_qk(0);
     wgmma_commit();
+    named_bar_arrive(other_turn, 256);
     wgmma_wait<0>();
-    fence_regs(o);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&kv_empty[s]);
+    fence_regs(sc);
+    release(&k_empty[0]);
+    softmax(0);
+    pack_p();
+
+    for (int j = 1; j < n_kv; ++j) {
+      const int s = j % S, sp = (j - 1) % S;
+      mbar_wait(&k_full[s], (j / S) & 1);
+      mbar_wait(&v_full[sp], ((j - 1) / S) & 1);
+      named_bar_sync(my_turn, 256);
+      wgmma_fence();
+      issue_qk(s);
+      wgmma_commit();
+      issue_pv(sp);
+      wgmma_commit();
+      named_bar_arrive(other_turn, 256);
+      wgmma_wait<1>();  // S_j has landed, PV_{j-1} may still run
+      fence_regs(sc);
+      release(&k_empty[s]);
+      const bool rescale = softmax(j);
+      wgmma_wait<0>();
+      fence_regs(o);
+      fence_regs(sc);  // P_j is packed into pa only after PV_{j-1} has read the old pa
+      release(&v_empty[sp]);
+      if (rescale) rescale_o();
+      pack_p();
+    }
+
+    // last block: PV alone
+    {
+      const int sp = (n_kv - 1) % S;
+      mbar_wait(&v_full[sp], ((n_kv - 1) / S) & 1);
+      named_bar_sync(my_turn, 256);
+      wgmma_fence();
+      issue_pv(sp);
+      wgmma_commit();
+      if (cw == 0) named_bar_arrive(other_turn, 256);  // warpgroup 1 issues last: there is no turn left to hand back
+      wgmma_wait<0>();
+      fence_regs(o);
+      release(&v_empty[sp]);
+    }
   }
 
 #pragma unroll
@@ -228,7 +360,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const float inv_l = l > 0.f ? 1.0f / l : 0.f;
     __nv_bfloat16* orow = p.out + (static_cast<int64_t>(b) * p.Tq + q) * ld + h * p.out_hd;
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
+    for (int jj = 0; jj < NO / 8; ++jj) {
       if (8 * jj < p.out_hd)
         *reinterpret_cast<uint32_t*>(orow + 8 * jj + kq) = pack_bf16(o[4 * jj + 2 * hrow] * inv_l, o[4 * jj + 2 * hrow + 1] * inv_l);
     }
@@ -335,20 +467,23 @@ __global__ void __launch_bounds__(128) attn_decode_merge(const float* __restrict
   out[static_cast<int64_t>(bh) * AT_D + d] = __float2bfloat16_rn(L > 0.f ? A / L : 0.f);
 }
 
-static int make_tmap_heads(CUtensorMap* tm, const void* ptr, int T, int H, int B, int64_t stride_b, int64_t stride_h) {
+// box of [128 rows][cols] per (head, batch): 64 columns with SW128, or the 16-column SW32 box of the HD = 80 path
+static int make_tmap_heads(CUtensorMap* tm, const void* ptr, int T, int H, int B, int64_t stride_b, int64_t stride_h,
+                           uint32_t cols = 64, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
   uint64_t dims[4] = {static_cast<uint64_t>(AT_D), static_cast<uint64_t>(T), static_cast<uint64_t>(H), static_cast<uint64_t>(B)};
   uint64_t str[3] = {static_cast<uint64_t>(AT_D) * 2, static_cast<uint64_t>(stride_h) * 2, static_cast<uint64_t>(stride_b) * 2};
-  uint32_t box[4] = {64, 128, 1, 1};
-  return make_tmap_bf16(tm, ptr, 4, dims, str, box);
+  uint32_t box[4] = {cols, 128, 1, 1};
+  return make_tmap_bf16_swz(tm, ptr, 4, dims, str, box, swizzle);
 }
 
 template <int HD, bool CAUSAL, bool LSE>
-static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const AttnParams& p, int64_t grid,
-                       cudaStream_t stream) {
+static int launch_attn(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmK16,
+                       const CUtensorMap& tmV16, const AttnParams& p, int64_t grid, cudaStream_t stream) {
   auto kern = attn_fwd_kernel<HD, CAUSAL, LSE>;
+  constexpr int smem = AttnCfg<HD>::SMEM;
   static bool attr_set[kMaxDevices] = {};
-  if (ensure_dynamic_smem(attr_set, kern, AT_SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
-  kern<<<static_cast<int>(grid), AT_THREADS, AT_SMEM, stream>>>(tmQ, tmK, tmV, p);
+  if (ensure_dynamic_smem(attr_set, kern, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  kern<<<static_cast<int>(grid), AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, tmK16, tmV16, p);
   return check_launch("attn_fwd_kernel");
 }
 
@@ -360,13 +495,22 @@ static int attention_fwd(const void* q, const void* k, const void* v, void* out,
   ARIA_CHECK_ARG(B > 0 && H > 0 && Tq > 0 && Tk > 0 && Tk >= (causal ? Tq : 0));
   ARIA_CHECK_ARG(out_hd > 0 && out_hd <= AT_D && out_hd % 8 == 0);
   ARIA_CHECK_ARG(q_stride_b % 8 == 0 && q_stride_h % 8 == 0 && kv_stride_b % 8 == 0 && kv_stride_h % 8 == 0);
-  CUtensorMap tmQ, tmK, tmV;
+  CUtensorMap tmQ, tmK, tmV, tmK16, tmV16;
   int rc = make_tmap_heads(&tmQ, q, Tq, H, B, q_stride_b, q_stride_h);
   if (rc) return rc;
   rc = make_tmap_heads(&tmK, k, Tk, H, B, kv_stride_b, kv_stride_h);
   if (rc) return rc;
   rc = make_tmap_heads(&tmV, v, Tk, H, B, kv_stride_b, kv_stride_h);
   if (rc) return rc;
+  if (out_hd <= 80) {  // columns 64-79 of K and V
+    rc = make_tmap_heads(&tmK16, k, Tk, H, B, kv_stride_b, kv_stride_h, 16, CU_TENSOR_MAP_SWIZZLE_32B);
+    if (rc) return rc;
+    rc = make_tmap_heads(&tmV16, v, Tk, H, B, kv_stride_b, kv_stride_h, 16, CU_TENSOR_MAP_SWIZZLE_32B);
+    if (rc) return rc;
+  } else {  // unused at HD = 128
+    tmK16 = tmK;
+    tmV16 = tmV;
+  }
   AttnParams p{};
   p.B = B;
   p.H = H;
@@ -380,12 +524,14 @@ static int attention_fwd(const void* q, const void* k, const void* v, void* out,
   p.n_q_tiles = (Tq + AT_BM - 1) / AT_BM;
   const int64_t grid = static_cast<int64_t>(B) * H * p.n_q_tiles;
   ARIA_CHECK_ARG(grid < (1ll << 31));
+#define ARIA_ATTN_LAUNCH(HD, C, L) launch_attn<HD, C, L>(tmQ, tmK, tmV, tmK16, tmV16, p, grid, stream)
   if (lse) {
-    if (out_hd <= 80) return causal ? launch_attn<80, true, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<80, false, true>(tmQ, tmK, tmV, p, grid, stream);
-    return causal ? launch_attn<128, true, true>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<128, false, true>(tmQ, tmK, tmV, p, grid, stream);
+    if (out_hd <= 80) return causal ? ARIA_ATTN_LAUNCH(80, true, true) : ARIA_ATTN_LAUNCH(80, false, true);
+    return causal ? ARIA_ATTN_LAUNCH(128, true, true) : ARIA_ATTN_LAUNCH(128, false, true);
   }
-  if (out_hd <= 80) return causal ? launch_attn<80, true, false>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<80, false, false>(tmQ, tmK, tmV, p, grid, stream);
-  return causal ? launch_attn<128, true, false>(tmQ, tmK, tmV, p, grid, stream) : launch_attn<128, false, false>(tmQ, tmK, tmV, p, grid, stream);
+  if (out_hd <= 80) return causal ? ARIA_ATTN_LAUNCH(80, true, false) : ARIA_ATTN_LAUNCH(80, false, false);
+  return causal ? ARIA_ATTN_LAUNCH(128, true, false) : ARIA_ATTN_LAUNCH(128, false, false);
+#undef ARIA_ATTN_LAUNCH
 }
 
 }  // namespace aria
