@@ -6,9 +6,13 @@
 // with one group, of the nn.Linear layers (dW[out,in] = dY^T X).  Both operands are consumed MN-major straight from the
 // row-major activation tensors (wgmma transpose bits set for A and B): no transposes are materialised.
 //
-// Ragged groups: group row offsets must be multiples of 16 (the training-mode dispatcher pads each expert's block with
-// zero rows).  TMA always fetches 64-row slabs; for the last slab of a group only the 16-row k-steps that lie inside
-// the group are issued, so rows of the next expert that share the slab are never multiplied.
+// Ragged groups: group row offsets are any non-decreasing values.  TMA fetches 64-row slabs starting at the group's first
+// row; for the last slab of a group only the 16-row k-steps that reach into the group are issued, so whole k-steps of the
+// next group that share the slab are never multiplied.  When a group's row count is not a multiple of 16, its last
+// k-step also holds the first rows of the next group (or rows past the last group): before that k-step's MMAs each
+// consumer warpgroup zeroes those rows in its own 64-column A chunk, so they contribute 0 * B.  In the MN-major SW128
+// layout a contraction row is one whole 128-byte line, so the swizzle does not move rows.  16-aligned groups (what the
+// training dispatcher's row_align = 16 produces) take no zeroing and issue exactly the same MMAs.
 #include "gemm_common.cuh"
 
 namespace aria {
@@ -16,7 +20,7 @@ namespace aria {
 struct WgradParams {
   int Md, Nd, G;
   int n_src;            // row groups are (source, g) pairs, source-major: offs has n_src*G+1 entries and out[g] sums over sources
-  const int32_t* offs;  // [G+1], multiples of 16 (last = total rows, any)
+  const int32_t* offs;  // [n_src*G+1], non-decreasing
   __nv_bfloat16* out;   // [G, Md, Nd]
 };
 
@@ -53,10 +57,10 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     mi = r / nt;
     ni = r - mi * nt;
   };
-  // rows of (source s, group g): start row and number of 16-row k-steps
-  auto span = [&](int s, int g, int& r0, int& ksteps) {
+  // rows of (source s, group g): start row and row count
+  auto span = [&](int s, int g, int& r0, int& n) {
     r0 = p.offs[s * p.G + g];
-    ksteps = (p.offs[s * p.G + g + 1] - r0 + 15) / 16;
+    n = p.offs[s * p.G + g + 1] - r0;
   };
 
   if (wg == 0) {
@@ -68,9 +72,9 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         int g, mi, ni;
         decode(t, g, mi, ni);
         for (int src = 0; src < p.n_src; ++src) {
-          int r0, ksteps;
-          span(src, g, r0, ksteps);
-          const int slabs = (ksteps + 3) / 4;
+          int r0, n;
+          span(src, g, r0, n);
+          const int slabs = (n + 63) / 64;
           for (int s = 0; s < slabs; ++s) {
             mbar_wait(&empty_bar[stage], phase ^ 1);
             uint8_t* sa = smem + stage * WG_STAGE_BYTES;
@@ -106,14 +110,24 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       for (int i = 0; i < WG_BN / 2; ++i) acc[i] = 0.f;  // an empty group stores zeros
       int prev = -1;
       for (int src = 0; src < p.n_src; ++src) {
-        int r0, ksteps;
-        span(src, g, r0, ksteps);
-        const int slabs = (ksteps + 3) / 4;
+        int r0, n;
+        span(src, g, r0, n);
+        const int slabs = (n + 63) / 64;
         for (int s = 0; s < slabs; ++s) {
           mbar_wait(&full_bar[stage], phase);
           const uint64_t da = dA0 + stage * (WG_STAGE_BYTES >> 4), db = dB0 + stage * (WG_STAGE_BYTES >> 4);
-          // the last slab of a group: only the 16-row k-steps inside the group (rows of the next group share the slab)
-          const int kmax = min(4, ksteps - s * 4);
+          // the last slab of a group: only the 16-row k-steps that reach into the group (rows of the next group share the slab)
+          const int valid = n - s * 64;                 // rows of this group in the slab (> 0)
+          const int kmax = min(4, (valid + 15) >> 4);
+          if (valid < 16 * kmax) {
+            // partial last k-step: zero A rows [valid, 16 * kmax) of this warpgroup's chunk (one 128-byte line per row);
+            // the proxy fence orders these generic stores before the wgmma reads and before TMA refills the slot
+            uint4* ca = reinterpret_cast<uint4*>(smem + stage * WG_STAGE_BYTES + cw * 8192);
+            for (int i = valid * 8 + tid; i < kmax * 128; i += 128) ca[i] = make_uint4(0u, 0u, 0u, 0u);
+            fence_proxy_async_smem();
+            if (cw == 0) named_bar_sync(1, 128);    // literal ids: ptxas reserves 3 hardware barriers, not all 16
+            else named_bar_sync(2, 128);
+          }
           wgmma_fence();
           for (int k = 0; k < kmax; ++k) wgmma_m64n128_ss<1, 1>(acc, da + k * (2048 >> 4), db + k * (2048 >> 4), 1u);
           wgmma_commit();

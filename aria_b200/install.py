@@ -8,34 +8,43 @@ Seams (SURVEY.md §8b):
   3. decoder-layer attention (moe_lm.py:594)                -> `AriaAttention`-style forward on the module's own q/k/v/o_proj
   4. `Idefics2EncoderLayer.forward` (vision_encoder.py:120) -> fused ViT layer
 
-(1) and (2) are wired by `install()`; (3) is `aria_b200.hf_attention.register()` (an implementation key for transformers'
+(1) and (2) are wired by `install()` — inference-only by default, differentiable with `install(..., trainable=True)`; (3) is `aria_b200.hf_attention.register()` (an implementation key for transformers'
 attention interface — the module keeps its projections, RoPE and HF Cache); (4) is `install_vit()` (per-layer forward on the
 HF module's own parameters; the embeddings / mask creation around it stay HF's).
 There is no CPU fallback: the patched modules require CUDA bf16 tensors.
 """
 from __future__ import annotations
 
+import sys
 import types
 
 import torch
+from torch import nn
 
+from . import lora as _lora
 from . import moe_lm as _m
+from . import moe_train as _t
 from . import ops
 
 
 def _reject_autograd(what: str, module, *tensors):
     """The seams below are the INFERENCE path: their outputs come straight from the C ABI and carry no grad_fn, so under
     autograd they would silently cut the graph (and drop the training-mode router losses, moe_lm.py:257-272).  Refuse
-    instead of training with wrong gradients; fine-tuning goes through aria_b200.moe_train / aria_b200.lora."""
+    instead of training with wrong gradients; `install(..., trainable=True)` binds the differentiable MoE seams."""
     if torch.is_grad_enabled() and (module.training or any(t is not None and t.requires_grad for t in tensors)):
         raise RuntimeError(f"aria_b200.install: {what} is inference-only (no autograd through the fused kernels); call it under "
-                           "torch.no_grad() with the module in eval() mode, or use aria_b200.moe_train / aria_b200.lora to train")
+                           "torch.no_grad() with the module in eval() mode (install(..., trainable=True) binds differentiable MoE seams)")
 
 
 def _moe_forward(self, hidden_states: torch.Tensor) -> torch.Tensor:
     """Replacement for the reference `MoELayer.forward` (moe_lm.py:548-577) — and for transformers' own `AriaTextMoELayer.forward`,
     which has the same sub-modules with `router` an nn.Linear — using the module's own parameters."""
     _reject_autograd("MoELayer.forward", self, hidden_states)
+    return _moe_block(self, hidden_states)
+
+
+def _moe_block(self, hidden_states: torch.Tensor) -> torch.Tensor:
+    """The inference MoE block on the module's own (plain) parameters."""
     cfg = getattr(self.router, "config", None) or self.config
     shape = hidden_states.shape
     x = hidden_states.reshape(-1, shape[-1]).contiguous()
@@ -56,6 +65,118 @@ def _moe_forward(self, hidden_states: torch.Tensor) -> torch.Tensor:
     y = ops.grouped_gemm(h, self.experts.fc2.weight, offsets)
     shared = _m.join_side(forked, x)
     return ops.unpermute_combine(y, dest, scores, shared).view(shape)
+
+
+# ------------------------------------------------------------------------------------------------ trainable MoE seam
+def _plain_weight(mod):
+    """Weight of an unwrapped bias-free projection (nn.Linear, or the reference's TopKRouter), else None (e.g. peft-wrapped)."""
+    if type(mod) is nn.Linear and mod.bias is None:
+        return mod.weight
+    if type(mod).__name__ == "TopKRouter" and not hasattr(mod, "base_layer"):
+        return mod.weight
+    return None
+
+
+def _lora_parts(fc):
+    """For an expert GEMM wrapped like the reference's `GroupedGemmLoraLayer` (aria/lora/layers.py:30-152: `base_layer`,
+    `lora_A`, `lora_B`, `scaling`, `active_adapters`): (base weight, A [E, in, r], B [E, r, out], scaling), or
+    (base weight, None, None, None) when no adapter is active (disabled or merged).  None for a plain GroupedGEMM."""
+    if not all(hasattr(fc, a) for a in ("base_layer", "lora_A", "lora_B", "scaling", "active_adapters")):
+        return None
+    base = fc.base_layer.weight
+    if getattr(fc, "disable_adapters", False) or getattr(fc, "merged", False):
+        return base, None, None, None
+    active = [a for a in fc.active_adapters if a in fc.lora_A]
+    if len(active) > 1:
+        raise NotImplementedError(f"aria_b200.install: {len(active)} active LoRA adapters on one expert GEMM; one is supported")
+    if not active:
+        return base, None, None, None
+    name = active[0]
+    drop = getattr(fc, "lora_dropout", None)
+    if drop is not None and name in drop and float(getattr(drop[name], "p", 0.0)) > 0.0:
+        raise NotImplementedError("aria_b200.install: lora_dropout > 0 is not supported on the expert GEMMs")
+    if getattr(fc, "use_dora", {}).get(name, False):
+        raise NotImplementedError("aria_b200.install: DoRA is not supported on the expert GEMMs")
+    a, b = fc.lora_A[name].weight, fc.lora_B[name].weight
+    if a.shape[-1] > _lora.R_PAD:
+        raise NotImplementedError(f"aria_b200.install: LoRA rank {a.shape[-1]} > {_lora.R_PAD} on the expert GEMMs")
+    return base, a, b, float(fc.scaling[name])
+
+
+def _expert_gemm(fc, a, offsets):
+    parts = _lora_parts(fc)
+    w = fc.weight if parts is None else parts[0]
+    if parts is not None and parts[1] is not None:
+        return _lora._LoraGroupedGemm.apply(a, w, parts[1], parts[2], offsets, parts[3])
+    return _t.GroupedGemmFunction.apply(a, w, offsets)
+
+
+def _router_losses(self):
+    """(loss_coeffs, scale holder) of the training-mode router losses (moe_lm.py:257-272): the reference `MoELayer` in train()
+    mode gets its router config's coefficients and ITS module's `MoEAuxLossAutoScaler` (train.py sets the scale on that class);
+    transformers' `AriaTextMoELayer` has no router losses."""
+    router = self.router
+    cfg = getattr(router, "config", None)
+    if not self.training or type(self).__name__ != "MoELayer" or cfg is None or not hasattr(cfg, "moe_z_loss_coeff"):
+        return None, None
+    holder = getattr(sys.modules.get(type(router).__module__), "MoEAuxLossAutoScaler", None)
+    if holder is None:
+        raise RuntimeError(f"aria_b200.install: no MoEAuxLossAutoScaler next to {type(router).__module__}.TopKRouter")
+    return (float(cfg.moe_z_loss_coeff), float(cfg.moe_aux_loss_coeff)), holder
+
+
+def _moe_plain(self):
+    """True when router, experts and shared experts are all unwrapped: the layer is one MoELayerFunction."""
+    se = self.shared_experts
+    return (_plain_weight(self.router) is not None and all(_plain_weight(m) is not None for m in (se.gate_proj, se.up_proj, se.down_proj))
+            and all(_lora_parts(f) is None and getattr(f, "weight", None) is not None for f in (self.experts.fc1, self.experts.fc2)))
+
+
+def _moe_composed(self, x2: torch.Tensor, k: int, coeffs, holder) -> torch.Tensor:
+    """The MoE block from per-stage autograd functions, for wrapped sub-modules: LoRA-wrapped expert GEMMs run
+    `lora._LoraGroupedGemm`; a wrapped router or shared-expert projection runs through its module."""
+    se = self.shared_experts
+    wr = _plain_weight(self.router)
+    logits = _t.LinearFunction.apply(x2, wr) if wr is not None else self.router(x2)
+    scores, idx, counts = _t.TopKFunction.apply(logits, k, coeffs, holder)
+    offsets, dest, src = ops.build_permutation(idx, counts, row_align=16)
+    xp = _t.PermuteFunction.apply(x2, src, dest, k)
+    y = _expert_gemm(self.experts.fc2, _lora.swiglu(_expert_gemm(self.experts.fc1, xp, offsets)), offsets)
+    ws = [_plain_weight(m) for m in (se.gate_proj, se.up_proj, se.down_proj)]
+    if all(w is not None for w in ws):
+        shared = _t.LinearFunction.apply(_lora.swiglu(_t.LinearFunction.apply(x2, ws[0], ws[1])), ws[2])
+    else:
+        shared = se(x2)
+    return _t.CombineFunction.apply(y, dest, scores, shared.reshape(x2.shape).contiguous())
+
+
+def _moe_train_forward(self, hidden_states: torch.Tensor) -> torch.Tensor:
+    """Replacement for `MoELayer.forward` / `AriaTextMoELayer.forward` bound by `install(..., trainable=True)`.
+      - no gradient needed (no_grad, or nothing requires grad): the inference path — for unwrapped sub-modules the same
+        `ops.moe_block_fwd` call as `install()`;
+      - otherwise one `moe_train.MoELayerFunction` on the module's own parameters (16-row-aligned permutation, our router,
+        explicit backward), with the reference's router losses in train() mode; wrapped sub-modules (LoRA experts, a
+        peft-wrapped router or shared-expert projection) run the same stages as separate autograd functions.
+    Frozen parameters get no gradient and cost no kernel."""
+    if getattr(self, "expert_parallel", None) is not None:
+        raise NotImplementedError("aria_b200.install(trainable=True): expert-parallel MoE layers run their own path "
+                                  "(aria_b200.expert_parallel); install the trainable seam without expert parallelism")
+    plain = _moe_plain(self)                 # raises for unsupported adapters before any kernel runs
+    train = torch.is_grad_enabled() and (hidden_states.requires_grad or any(p.requires_grad for p in self.parameters()))
+    if not train and plain:
+        return _moe_block(self, hidden_states)
+    if not hidden_states.is_cuda:
+        raise RuntimeError("aria_b200.install(trainable=True): the MoE training path needs CUDA tensors (there is no CPU path)")
+    if hidden_states.dtype != torch.bfloat16:
+        raise RuntimeError(f"aria_b200.install(trainable=True): expected bf16 hidden states, got {hidden_states.dtype}")
+    cfg = getattr(self.router, "config", None) or self.config
+    coeffs, holder = _router_losses(self)
+    if plain:
+        se = self.shared_experts
+        return _t.MoELayerFunction.apply(hidden_states, self.router.weight, self.experts.fc1.weight, self.experts.fc2.weight,
+                                         se.gate_proj.weight, se.up_proj.weight, se.down_proj.weight, cfg.moe_topk, coeffs, holder)
+    shape = hidden_states.shape
+    return _moe_composed(self, hidden_states.reshape(-1, shape[-1]).contiguous(), cfg.moe_topk, coeffs, holder).view(shape)
 
 
 def _vit_layer_forward(self, hidden_states: torch.Tensor, attention_mask=None, *args, **kwargs):
@@ -111,15 +232,20 @@ def install_vit(model) -> int:
     return n
 
 
-def install(model, reference_moe_lm_module=None) -> int:
+def install(model, reference_moe_lm_module=None, trainable: bool = False) -> int:
     """Patch every reference `MoELayer` inside `model` (and, if given, the reference module's global `experts_gemm`).
-    Returns the number of layers patched.  Idempotent."""
+    Returns the number of layers patched.  Idempotent.
+    trainable=False: the inference seams (they refuse autograd).  trainable=True: the MoE layers run `_moe_train_forward`
+    (differentiable, router losses in train() mode; inference unchanged) and `experts_gemm` becomes the differentiable
+    `moe_train.experts_gemm_train`."""
+    fwd = _moe_train_forward if trainable else _moe_forward
     n = 0
     for mod in model.modules():
         if type(mod).__name__ in ("MoELayer", "AriaTextMoELayer") and hasattr(mod, "router") and hasattr(mod, "experts") \
                 and hasattr(mod, "shared_experts"):
-            mod.forward = types.MethodType(_moe_forward, mod)
+            mod.forward = types.MethodType(fwd, mod)
             n += 1
     if reference_moe_lm_module is not None:
-        reference_moe_lm_module.experts_gemm = _m.experts_gemm  # seam 1: GroupedGEMM.forward calls the module global
+        # seam 1: GroupedGEMM.forward calls the module global
+        reference_moe_lm_module.experts_gemm = _t.experts_gemm_train if trainable else _m.experts_gemm
     return n

@@ -15,7 +15,8 @@ costs two extra launches forward.  Backward (adapters and input only; the base w
     dB = (x A s)^T dy      `aria_grouped_wgrad`          dh = dy B^T          `aria_gemm` B_GNK (weight read transposed)
     dA = s * x^T dh        `aria_grouped_wgrad`          dx = dy W^T + dh (A s)^T
 
-Group rows must start on multiples of 16 (the training dispatcher's `row_align=16`), as for every wgrad here.
+Group rows may start at any row (`aria_grouped_wgrad` handles densely packed groups); the training dispatcher's
+`row_align=16` blocks take its cheaper aligned path.
 Parity: the oracle's restatement is pinned bit-exactly to the unmodified reference layer, loaded under a stand-in for the two
 peft symbols it imports (oracle/ref_loader.py `load_reference_lora`, tests/test_oracle_vs_reference.py) and through
 tests/golden/lora_grouped_gemm_*.pt on the GPU.

@@ -10,7 +10,9 @@ gradient is an explicit kernel:
 
 Router losses: with `router_losses=True` (the reference's `self.training` branch, moe_lm.py:257-258,271-272) the z-loss and
 load-balancing-loss gradients (moe_lm.py:84-166) are added to dlogits by `aria_router_aux_bwd`, scaled by
-`MoEAuxLossAutoScaler.main_loss_backward_scale`; the default (False) is eval-mode routing, which is what BASELINE cfg 5 times.
+`MoEAuxLossAutoScaler.main_loss_backward_scale` of `loss_scale_source` (read at backward time, as the reference's autograd
+function does; default: aria_b200.moe_lm's holder — the trainable seam passes the reference module's own class); the default
+(False) is eval-mode routing, which is what BASELINE cfg 5 times.
 Gradients are bf16 tensors accumulated in fp32 inside the tensor-core kernels.
 """
 from __future__ import annotations
@@ -23,7 +25,7 @@ from . import ops
 
 class MoELayerFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w_router, fc1, fc2, gate_w, up_w, down_w, topk: int, loss_coeffs=None):
+    def forward(ctx, x, w_router, fc1, fc2, gate_w, up_w, down_w, topk: int, loss_coeffs=None, loss_scale_source=None):
         shape = x.shape
         x2 = x.reshape(-1, shape[-1]).contiguous()
         E = w_router.shape[0]
@@ -42,6 +44,7 @@ class MoELayerFunction(torch.autograd.Function):
         ctx.save_for_backward(x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, offsets, dest, xp, h1, h, y, hs1, hs)
         ctx.topk = topk
         ctx.loss_coeffs = loss_coeffs
+        ctx.loss_scale_source = loss_scale_source
         if loss_coeffs is not None:  # keep what the loss gradients need: the bf16 logits and tokens_per_expert
             ctx.router_logits, ctx.counts = _logits, counts
         ctx.shape = shape
@@ -54,35 +57,54 @@ class MoELayerFunction(torch.autograd.Function):
         Is = gate_w.shape[0]
         T = x2.shape[0]
         do = dout.reshape(-1, d).contiguous()
+        # a gradient nobody needs (frozen weight, input without requires_grad) is neither computed nor launched; the ones
+        # computed run the same kernels in the same order as when every gradient is needed
+        need_x, need_r, need_fc1, need_fc2, need_gate, need_up, need_down = ctx.needs_input_grad[:7]
         dense = torch.tensor([0, T], dtype=torch.int32, device=do.device)  # one 16-aligned "group" for dense wgrads
+        d_router = d_fc1 = d_fc2 = d_gate = d_up = d_down = dx = None
         # ---- routed experts
         dy, dscores = ops.combine_bwd(do, y, dest, scores)
-        d_fc2 = ops.grouped_wgrad(h, dy, offsets)                             # [E, I, d]
-        dh = ops.grouped_gemm_nt(dy, fc2, offsets)                            # dy @ fc2[e].T -> [rows, I]
-        dh1 = ops.swiglu_bwd(h1, dh)
-        d_fc1 = ops.grouped_wgrad(xp, dh1, offsets)                           # [E, d, 2I]
-        dxp = ops.grouped_gemm_nt(dh1, fc1, offsets)                          # [rows, d]
+        if need_fc2:
+            d_fc2 = ops.grouped_wgrad(h, dy, offsets)                         # [E, I, d]
+        if need_x or need_fc1:
+            dh = ops.grouped_gemm_nt(dy, fc2, offsets)                        # dy @ fc2[e].T -> [rows, I]
+            dh1 = ops.swiglu_bwd(h1, dh)
+            if need_fc1:
+                d_fc1 = ops.grouped_wgrad(xp, dh1, offsets)                   # [E, d, 2I]
+            if need_x:
+                dxp = ops.grouped_gemm_nt(dh1, fc1, offsets)                  # [rows, d]
         # ---- shared expert (out += shared: its upstream gradient is dout itself)
-        d_down = ops.grouped_wgrad(do, hs, dense)[0]                          # [d, Is]
-        dhs = ops.matmul_kn(do, down_w)                                       # do @ down_w  ([d, Is] read as K x N)
-        dhs1 = ops.swiglu_bwd(hs1, dhs)                                       # [T, 2 Is] = [d gate | d up]
-        d_gate = ops.grouped_wgrad(dhs1[:, :Is], x2, dense)[0]                # [Is, d]
-        d_up = ops.grouped_wgrad(dhs1[:, Is:], x2, dense)[0]
-        dx = ops.matmul_kn(dhs1[:, :Is], gate_w)
-        dx = ops.matmul_kn(dhs1[:, Is:], up_w, residual=dx)
+        if need_down:
+            d_down = ops.grouped_wgrad(do, hs, dense)[0]                      # [d, Is]
+        if need_x or need_gate or need_up:
+            dhs = ops.matmul_kn(do, down_w)                                   # do @ down_w  ([d, Is] read as K x N)
+            dhs1 = ops.swiglu_bwd(hs1, dhs)                                   # [T, 2 Is] = [d gate | d up]
+            if need_gate:
+                d_gate = ops.grouped_wgrad(dhs1[:, :Is], x2, dense)[0]        # [Is, d]
+            if need_up:
+                d_up = ops.grouped_wgrad(dhs1[:, Is:], x2, dense)[0]
+            if need_x:
+                dx = ops.matmul_kn(dhs1[:, :Is], gate_w)
+                dx = ops.matmul_kn(dhs1[:, Is:], up_w, residual=dx)
         # ---- router
-        dlogits = ops.router_bwd(dscores, scores, idx, E)                     # [T, E]
-        if ctx.loss_coeffs is not None:
-            from .moe_lm import MoEAuxLossAutoScaler
-            z_c, aux_c = ctx.loss_coeffs
-            ops.router_aux_bwd(ctx.router_logits, ctx.counts, dlogits, ctx.topk, z_c, aux_c,
-                               MoEAuxLossAutoScaler.main_loss_backward_scale)
-        d_router = ops.grouped_wgrad(dlogits, x2, dense)[0]                   # [E, d]
-        dx = ops.matmul_kn(dlogits, w_router, residual=dx)
+        if need_x or need_r:
+            dlogits = ops.router_bwd(dscores, scores, idx, E)                 # [T, E]
+            if ctx.loss_coeffs is not None:
+                src = ctx.loss_scale_source
+                if src is None:
+                    from .moe_lm import MoEAuxLossAutoScaler as src
+                z_c, aux_c = ctx.loss_coeffs
+                ops.router_aux_bwd(ctx.router_logits, ctx.counts, dlogits, ctx.topk, z_c, aux_c,
+                                   float(src.main_loss_backward_scale))
+            if need_r:
+                d_router = ops.grouped_wgrad(dlogits, x2, dense)[0]           # [E, d]
+            if need_x:
+                dx = ops.matmul_kn(dlogits, w_router, residual=dx)
         # ---- un-permute: dx[t] += sum_j dxp[dest[t, j]]
-        ones = torch.ones_like(scores)
-        dx = ops.unpermute_combine(dxp, dest, ones, dx)
-        return dx.view(ctx.shape), d_router, d_fc1, d_fc2, d_gate, d_up, d_down, None, None
+        if need_x:
+            ones = torch.ones_like(scores)
+            dx = ops.unpermute_combine(dxp, dest, ones, dx).view(ctx.shape)
+        return dx, d_router, d_fc1, d_fc2, d_gate, d_up, d_down, None, None, None
 
 
 def moe_layer_train(layer, hidden_states: torch.Tensor, router_losses: bool = False) -> torch.Tensor:
@@ -93,3 +115,114 @@ def moe_layer_train(layer, hidden_states: torch.Tensor, router_losses: bool = Fa
     return MoELayerFunction.apply(hidden_states, layer.router.weight, layer.experts.fc1.weight, layer.experts.fc2.weight,
                                   layer.shared_experts.gate_proj.weight, layer.shared_experts.up_proj.weight,
                                   layer.shared_experts.down_proj.weight, cfg.moe_topk, coeffs)
+
+
+# ------------------------------------------------------------------------------------------------ trainable seams
+class GroupedGemmFunction(torch.autograd.Function):
+    """Differentiable `gmm`: out[rows of e] = a[rows of e] @ w[e] over any int32 row offsets [E+1] (densely packed, as the
+    reference's dispatcher produces them, or 16-aligned).  Backward: da = dy @ w[e].T (`aria_gemm`, weight read transposed
+    in place), dw = a.T @ dy per group (`aria_grouped_wgrad`); each only when its input requires grad."""
+
+    @staticmethod
+    def forward(ctx, a, w, offsets):
+        ctx.save_for_backward(a, w, offsets)
+        return ops.grouped_gemm(a, w, offsets)
+
+    @staticmethod
+    def backward(ctx, dy):
+        a, w, offsets = ctx.saved_tensors
+        dy = dy.contiguous()
+        da = ops.grouped_gemm_nt(dy, w, offsets) if ctx.needs_input_grad[0] else None
+        dw = ops.grouped_wgrad(a, dy, offsets) if ctx.needs_input_grad[1] else None
+        return da, dw, None
+
+
+def experts_gemm_train(input: torch.Tensor, weight: torch.Tensor, tokens_per_expert: torch.Tensor) -> torch.Tensor:
+    """Trainable drop-in for `grouped_gemm.ops.gmm(a, b, batch_sizes)` (seam 1, moe_lm.py:431-443): same contract as
+    `aria_b200.moe_lm.experts_gemm` (counts [E] in any integer dtype on CPU or GPU, or int32 device offsets [E+1]), and
+    the result carries a grad_fn when `input` or `weight` requires grad."""
+    from .moe_lm import _as_offsets
+    off = _as_offsets(tokens_per_expert, weight.shape[0], input.device)
+    if torch.is_grad_enabled() and (input.requires_grad or weight.requires_grad):
+        return GroupedGemmFunction.apply(input, weight, off)
+    return ops.grouped_gemm(input, weight, off)
+
+
+class LinearFunction(torch.autograd.Function):
+    """x @ [W0 | W1 | ...].T in one GEMM (nn.Linear weights [N, K], equal N); backward as MoELayerFunction's shared expert:
+    dW_i = dy_i.T @ x (`aria_grouped_wgrad`, one dense group), dx = sum_i dy_i @ W_i (`aria_gemm`, weight in place)."""
+
+    @staticmethod
+    def forward(ctx, x, *weights):
+        ctx.save_for_backward(x, *weights)
+        return ops.linear_multi(x, list(weights))
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, *weights = ctx.saved_tensors
+        dy = dy.contiguous()
+        N = weights[0].shape[0]
+        dense = torch.tensor([0, x.shape[0]], dtype=torch.int32, device=x.device)
+        dws, dx = [], None
+        for i, w in enumerate(weights):
+            seg = dy[:, i * N:(i + 1) * N]
+            dws.append(ops.grouped_wgrad(seg, x, dense)[0] if ctx.needs_input_grad[1 + i] else None)
+            if ctx.needs_input_grad[0]:
+                dx = ops.matmul_kn(seg, w, residual=dx)
+        return (dx, *dws)
+
+
+class TopKFunction(torch.autograd.Function):
+    """Router top-k + softmax over given logits [T, E] (`aria_route_from_logits`) -> (scores [T, k] bf16, idx, counts).
+    Backward: dlogits = top-k softmax backward (`aria_router_bwd`) + the training-mode router-loss gradients when
+    `loss_coeffs` is set (`aria_router_aux_bwd`, scaled by `loss_scale_source.main_loss_backward_scale`)."""
+
+    @staticmethod
+    def forward(ctx, logits, topk: int, loss_coeffs=None, loss_scale_source=None):
+        logits = logits.contiguous()
+        scores, idx, counts = ops.route_from_logits(logits, topk)
+        ctx.save_for_backward(logits, scores, idx, counts)
+        ctx.topk, ctx.loss_coeffs, ctx.loss_scale_source = topk, loss_coeffs, loss_scale_source
+        ctx.mark_non_differentiable(idx, counts)
+        return scores, idx, counts
+
+    @staticmethod
+    def backward(ctx, dscores, _didx, _dcounts):
+        logits, scores, idx, counts = ctx.saved_tensors
+        dlogits = ops.router_bwd(dscores.float().contiguous(), scores, idx, logits.shape[1])
+        if ctx.loss_coeffs is not None:
+            z_c, aux_c = ctx.loss_coeffs
+            ops.router_aux_bwd(logits, counts, dlogits, ctx.topk, z_c, aux_c, float(ctx.loss_scale_source.main_loss_backward_scale))
+        return dlogits, None, None, None
+
+
+class PermuteFunction(torch.autograd.Function):
+    """Token rows into expert order (`aria_permute_rows`, pad rows zero); backward sums each token's k copies
+    (`aria_unpermute_combine` with unit scores)."""
+
+    @staticmethod
+    def forward(ctx, x, src, dest, topk: int):
+        ctx.save_for_backward(dest)
+        ctx.topk = topk
+        return ops.permute_rows(x, src)
+
+    @staticmethod
+    def backward(ctx, dxp):
+        (dest,) = ctx.saved_tensors
+        ones = torch.ones((dest.numel() // ctx.topk, ctx.topk), dtype=torch.bfloat16, device=dxp.device)
+        return ops.unpermute_combine(dxp.contiguous(), dest, ones), None, None, None
+
+
+class CombineFunction(torch.autograd.Function):
+    """out[t] = sum_j scores[t, j] * y[dest[t, j]] + shared[t] (`aria_unpermute_combine`); backward `aria_combine_bwd`."""
+
+    @staticmethod
+    def forward(ctx, y, dest, scores, shared):
+        ctx.save_for_backward(y, dest, scores)
+        return ops.unpermute_combine(y, dest, scores, shared)
+
+    @staticmethod
+    def backward(ctx, dout):
+        y, dest, scores = ctx.saved_tensors
+        dy, dscores = ops.combine_bwd(dout.contiguous(), y, dest, scores)
+        return dy, None, dscores.to(scores.dtype), dout

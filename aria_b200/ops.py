@@ -224,9 +224,9 @@ def matmul_kn(a: torch.Tensor, w_kn: torch.Tensor, residual: Optional[torch.Tens
 
 
 def grouped_wgrad(a: torch.Tensor, b: torch.Tensor, offsets: torch.Tensor, num_sources: int = 1) -> torch.Tensor:
-    """out[g] = a[rows of g].T @ b[rows of g]; a [rows, Md], b [rows, Nd] (row strides allowed), offsets [G+1] int32 with
-    16-aligned entries -> out [G, Md, Nd] bf16 (fp32 accumulation).  num_sources=S: offsets [S*G+1] over
-    (source, g) row groups, out[g] sums over the sources."""
+    """out[g] = a[rows of g].T @ b[rows of g]; a [rows, Md], b [rows, Nd] (row strides allowed), offsets [G+1] int32,
+    non-decreasing, any alignment (16-aligned groups take no extra work) -> out [G, Md, Nd] bf16 (fp32 accumulation); an
+    empty group gives zeros.  num_sources=S: offsets [S*G+1] over (source, g) row groups, out[g] sums over the sources."""
     for t in (a, b):
         if not (t.is_cuda and t.dtype == bf16 and t.stride(1) == 1 and t.data_ptr() % 16 == 0):
             raise RuntimeError("grouped_wgrad: operands must be CUDA bf16 with contiguous rows")

@@ -105,7 +105,10 @@ int aria_grouped_gemm(const void* a, const void* b, void* out, const int32_t* gr
 
 /* Weight gradient of a (grouped) linear layer — backward of gmm / F.linear:
  *   out[g, m, n] = sum_{r in group g} a[r, m] * b[r, n]   a [rows, md] (row stride lda), b [rows, nd] (ldb), out [G, md, nd] bf16.
- * group_offsets: device int32 row offsets, each a multiple of 16 (aria_build_permutation with row_align = 16).
+ * group_offsets: device int32 row offsets, non-decreasing, any values (densely packed groups as the reference's dispatcher
+ * produces them, or the 16-aligned blocks of aria_build_permutation with row_align = 16).  Rows past the last offset are
+ * never multiplied into a result.  When a group's row count is not a multiple of 16, the (up to 15) rows of b that follow
+ * it are multiplied by zeros, so they must be finite (rows past `rows` are read as zeros).
  * num_sources = 1: offsets[G+1].  num_sources = S > 1 (expert parallelism): rows are grouped (source rank, g),
  * source-major, offsets[S*G+1], and out[g] sums the S partial products — no separate reduction pass. */
 int aria_grouped_wgrad(const void* a, int64_t lda, const void* b, int64_t ldb, void* out, const int32_t* group_offsets,
