@@ -37,7 +37,6 @@ class GemmDesc(C.Structure):
         ("head_dim", i32), ("head_ld", i32), ("rows_per_batch", i32), ("pos0", i32),
         ("stride_b", i64), ("stride_h", i64),
         ("rope_mask", i32), ("rope_cos", vp), ("rope_sin", vp), ("position_ids", vp),
-        ("dbg_lbo", i32), ("dbg_sbo", i32), ("dbg_kadv", i32),
         ("group_counts", vp), ("a_rows", i64), ("out_group_base", vp), ("out_group_row0", vp),
     ]
 
@@ -76,10 +75,7 @@ SIGNATURES = {
     "aria_ipc_export": (i32, [vp, vp, vp]),
     "aria_ipc_open": (i32, [vp, vp]),
     "aria_ipc_close": (i32, [vp]),
-    "aria_ep_publish_counts": (i32, [vp, vp, i32, i32, i32, vp]),
     "aria_peer_barrier": (i32, [vp, i32, i32, vp, vp]),
-    "aria_ep_layout": (i32, [vp, i32, i32, i32, vp, vp, vp, vp]),
-    "aria_scatter_rows_grouped": (i32, [vp, vp, vp, i32, vp, i32, vp, i32, i64, vp]),
     "aria_ep_dispatch": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, vp]),
     "aria_attention_fwd": (i32, [vp, vp, vp, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64, i32, f32, i32, vp, i64, vp]),
     "aria_attention_fwd_workspace_bytes": (i64, [i32, i32, i32, i32, i32, i32]),

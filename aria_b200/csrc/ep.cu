@@ -1,27 +1,15 @@
 // Expert-parallel exchange over NVLink peer memory (no NCCL, no host sync): every rank owns an arena that all peers map
 // (aria_b200/peer.py); the kernels below store straight into the peers' arenas through NVSwitch.
 //
-//   ep_publish_counts      my per-expert counts -> row `rank` of counts_all in every peer's arena
-//   peer_barrier           device-side all-ranks barrier on flags in the arenas (release/acquire at system scope)
-//   ep_layout              from counts_all [W,E]: receive offsets of my (source rank, local expert) groups, the row base of
-//                          each of my expert blocks inside its owner's receive buffer, and the row base each received
-//                          group came from (for the way back)
-//   scatter_rows_grouped   FUSED permute + dispatch: gathers token rows in expert order and stores them directly into the
-//                          owning rank's receive buffer (and, on the way back, expert outputs into the source rank's
-//                          buffer at their original sorted position)
+//   peer_barrier   device-side all-ranks barrier on flags in the arenas (release/acquire at system scope)
+//   ep_dispatch    FUSED permute + dispatch: gathers token rows in expert order and stores them directly into the owning
+//                  rank's fixed-capacity receive regions, and publishes each block's (count, first sorted row) to the owner
+// The way back needs no kernel here: the fc2 grouped GEMM's epilogue stores into the source ranks' buffers (csrc/gemm.cu).
 // Replaces the all-to-all of Megatron's dispatcher that the reference stripped out (aria/model/moe_lm.py:296-297).
 #include "common.cuh"
 #include "ptx.cuh"
 
 namespace aria {
-
-__global__ void ep_publish_counts_kernel(const int32_t* __restrict__ counts, const uint64_t* __restrict__ peer_counts, int rank,
-                                         int W, int E) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= W * E) return;
-  const int p = i / E, e = i - p * E;
-  reinterpret_cast<int32_t*>(peer_counts[p])[rank * E + e] = counts[e];
-}
 
 // The epoch lives in device memory and is advanced by the kernel itself, so a CUDA graph that captured the barrier replays
 // correctly (every rank executes the same sequence of barriers, so the counters stay in step).
@@ -45,63 +33,6 @@ __global__ void peer_barrier_kernel(const uint64_t* __restrict__ peer_flags, int
       __trap();
     }
   } while (v < epoch);
-}
-
-// Single block.  counts_all[s][e] = rows rank s sends to global expert e.
-__global__ void ep_layout_kernel(const int32_t* __restrict__ counts_all, int rank, int W, int E, int32_t* __restrict__ roff,
-                                 int32_t* __restrict__ send_base, int32_t* __restrict__ ret_base) {
-  const int E_loc = E / W;
-  if (threadIdx.x == 0) {
-    // my receive buffer: groups ordered (source rank, local expert)
-    int a = 0;
-    for (int s = 0; s < W; ++s)
-      for (int e = 0; e < E_loc; ++e) {
-        roff[s * E_loc + e] = a;
-        a += counts_all[s * E + rank * E_loc + e];
-      }
-    roff[W * E_loc] = a;
-  }
-  // where my block for global expert e starts inside its owner's receive buffer
-  for (int e = threadIdx.x; e < E; e += blockDim.x) {
-    const int p = e / E_loc, el = e - p * E_loc;
-    int a = 0;
-    for (int s = 0; s < rank; ++s)
-      for (int x = 0; x < E_loc; ++x) a += counts_all[s * E + p * E_loc + x];
-    for (int x = 0; x < el; ++x) a += counts_all[rank * E + p * E_loc + x];
-    send_base[e] = a;
-  }
-  // where the rows of received group (s, el) sit in rank s's expert-sorted order (= its local offsets)
-  for (int g = threadIdx.x; g < W * E_loc; g += blockDim.x) {
-    const int s = g / E_loc, el = g - s * E_loc;
-    int a = 0;
-    for (int x = 0; x < rank * E_loc + el; ++x) a += counts_all[s * E + x];
-    ret_base[g] = a;
-  }
-}
-
-// Row i of group g (goff[g] <= i < goff[g+1]) goes to rank g / group_div, row dst_row_base[g] + (i - goff[g]) of that
-// rank's buffer (peer_bufs[rank] = address as mapped on THIS GPU).  Source row = rows[src_token ? src_token[i] : i].
-__global__ void __launch_bounds__(256) scatter_rows_grouped_kernel(const uint4* __restrict__ rows, const int32_t* __restrict__ src_token,
-                                                                   const int32_t* __restrict__ goff, int G,
-                                                                   const int32_t* __restrict__ dst_row_base, int group_div,
-                                                                   const uint64_t* __restrict__ peer_bufs, int vec_per_row) {
-  __shared__ int s_off[1025];
-  for (int i = threadIdx.x; i <= G; i += blockDim.x) s_off[i] = goff[i];
-  __syncthreads();
-  const int total = s_off[G];
-  const int lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
-  for (int r = blockIdx.x * wpb + (threadIdx.x >> 5); r < total; r += gridDim.x * wpb) {
-    int lo = 0, hi = G;  // group of row r: last g with s_off[g] <= r
-    while (hi - lo > 1) {
-      const int mid = (lo + hi) >> 1;
-      if (s_off[mid] <= r) lo = mid; else hi = mid;
-    }
-    const int g = lo;
-    uint4* dst = reinterpret_cast<uint4*>(peer_bufs[g / group_div]) +
-                 static_cast<int64_t>(dst_row_base[g] + (r - s_off[g])) * vec_per_row;
-    const uint4* src = rows + static_cast<int64_t>(src_token ? src_token[r] : r) * vec_per_row;
-    for (int v = lane; v < vec_per_row; v += 32) dst[v] = __ldg(src + v);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -170,39 +101,9 @@ extern "C" int aria_ep_dispatch(const void* x, const int32_t* src_token, const i
   return check_launch("ep_dispatch_kernel");
 }
 
-extern "C" int aria_ep_publish_counts(const int32_t* counts, const uint64_t* peer_counts, int32_t rank, int32_t W, int32_t E,
-                                      aria_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  ARIA_CHECK_ARG(counts && peer_counts && W >= 1 && E >= 1 && rank >= 0 && rank < W);
-  ep_publish_counts_kernel<<<(W * E + 255) / 256, 256, 0, stream>>>(counts, peer_counts, rank, W, E);
-  return check_launch("ep_publish_counts_kernel");
-}
-
 extern "C" int aria_peer_barrier(const uint64_t* peer_flags, int32_t rank, int32_t W, int32_t* epoch_dev, aria_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   ARIA_CHECK_ARG(peer_flags && epoch_dev && W >= 1 && W <= 32 && rank >= 0 && rank < W);
   peer_barrier_kernel<<<1, 32, 0, stream>>>(peer_flags, rank, W, epoch_dev);
   return check_launch("peer_barrier_kernel");
-}
-
-extern "C" int aria_ep_layout(const int32_t* counts_all, int32_t rank, int32_t W, int32_t E, int32_t* roff, int32_t* send_base,
-                              int32_t* ret_base, aria_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  ARIA_CHECK_ARG(counts_all && roff && send_base && ret_base && W >= 1 && E % W == 0);
-  ep_layout_kernel<<<1, 256, 0, stream>>>(counts_all, rank, W, E, roff, send_base, ret_base);
-  return check_launch("ep_layout_kernel");
-}
-
-extern "C" int aria_scatter_rows_grouped(const void* rows, const int32_t* src_token, const int32_t* group_offsets, int32_t G,
-                                         const int32_t* dst_row_base, int32_t group_div, const uint64_t* peer_bufs, int32_t d,
-                                         int64_t max_rows, aria_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  ARIA_CHECK_ARG(rows && group_offsets && dst_row_base && peer_bufs && G >= 1 && G <= 1024 && group_div >= 1 && d % 8 == 0);
-  int64_t blocks = (max_rows + 7) / 8;
-  const int64_t cap = static_cast<int64_t>(sm_count()) * 8;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  scatter_rows_grouped_kernel<<<static_cast<int>(blocks), 256, 0, stream>>>(static_cast<const uint4*>(rows), src_token, group_offsets, G,
-                                                                          dst_row_base, group_div, peer_bufs, d / 8);
-  return check_launch("scatter_rows_grouped_kernel");
 }

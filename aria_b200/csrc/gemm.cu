@@ -123,9 +123,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     setmaxnreg_inc<232>();
     const int cw = wg - 1;
     const int tid = threadIdx.x & 127;
-    const uint32_t b_lbo = p.dbg_lbo ? p.dbg_lbo : (B_MN ? 64 * BK * 2 : 16);
-    const uint32_t b_sbo = p.dbg_sbo ? p.dbg_sbo : 1024;
-    const uint32_t b_kadv = (p.dbg_kadv ? p.dbg_kadv : (B_MN ? 16 * 128 : 32)) >> 4;
+    constexpr uint32_t b_lbo = B_MN ? 64 * BK * 2 : 16;
+    constexpr uint32_t b_sbo = 1024;
+    constexpr uint32_t b_kadv = (B_MN ? 16 * 128 : 32) >> 4;
     // descriptors of stage 0 / k-step 0; the start-address field is (addr >> 4) in the low 14 bits and shared-memory
     // addresses stay below 2^18, so adding (byte offset >> 4) never carries into the next field
     const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
@@ -258,9 +258,6 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
   p.rope_cos = static_cast<const __nv_bfloat16*>(d->rope_cos);
   p.rope_sin = static_cast<const __nv_bfloat16*>(d->rope_sin);
   p.position_ids = d->position_ids;
-  p.dbg_lbo = d->dbg_lbo;
-  p.dbg_sbo = d->dbg_sbo;
-  p.dbg_kadv = d->dbg_kadv;
 
   // ---- tile shape selection: 128-wide tiles; the 72-dim ViT heads (n = 1152 = 8 x 144) take 144-wide tiles of whole heads
   const int64_t n_out_total = d->n * (swiglu ? 1 : d->n_seg);
@@ -341,5 +338,5 @@ extern "C" int aria_grouped_gemm(const void* a, const void* b, void* out, const 
   return aria_gemm(&d, stream);
 }
 
-extern "C" int aria_abi_version(void) { return 2; }
+extern "C" int aria_abi_version(void) { return 3; }
 extern "C" const char* aria_build_arch(void) { return "sm_90a"; }

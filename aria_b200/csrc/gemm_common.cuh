@@ -47,7 +47,6 @@ struct GemmParams {
   const __nv_bfloat16* rope_cos;
   const __nv_bfloat16* rope_sin;
   const int32_t* position_ids;
-  int dbg_lbo, dbg_sbo, dbg_kadv;
 };
 
 ARIA_DEVICE int weight_block(const GemmParams& p, int grp) {

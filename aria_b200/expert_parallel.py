@@ -53,6 +53,35 @@ class CudaBackend:
         return ops.unpermute_combine(y, dest, scores, shared)
 
 
+def exchange_plan(counts: torch.Tensor, group, row_align: int = 1):
+    """The NCCL exchange plan of one layer from my per-expert row counts [E] (rows sorted by global expert id, so by
+    destination rank): all-to-all of the per-(rank, local expert) counts, then the one host sync per layer (NCCL's
+    all-to-all-v takes host split sizes).  row_align > 1: every expert block is sent padded to a multiple of it (the
+    training layout, so the received groups stay 16-aligned).  Returns (recv_counts int64 [W*E_loc] on the counts'
+    device, groups ordered (source rank, local expert); rows sent to each rank; rows received from each rank)."""
+    send_counts = counts.to(torch.int64)
+    if row_align > 1:
+        send_counts = (send_counts + row_align - 1) // row_align * row_align
+    send_counts = send_counts.view(dist.get_world_size(group), -1)
+    recv_counts = torch.empty_like(send_counts)
+    dist.all_to_all_single(recv_counts, send_counts, group=group)
+    return recv_counts.reshape(-1), send_counts.sum(1).tolist(), recv_counts.sum(1).tolist()
+
+
+def exchange_rows(rows: torch.Tensor, plan, group, back: bool = False, out=None) -> torch.Tensor:
+    """All-to-all-v of rows along `plan` (from `exchange_plan`).  Forward: the first rows the plan sends (expert order) go
+    to the owners of their experts; returns the received rows, grouped (source rank, local expert).  back=True: the
+    reverse, rows laid out as received go back to their source ranks, into the first rows of `out` (the rows past them,
+    e.g. zeroed pads, are left as they are); returns `out`."""
+    _, send, recv = plan
+    if back:
+        dist.all_to_all_single(out[:sum(send)], rows, output_split_sizes=send, input_split_sizes=recv, group=group)
+        return out
+    out = torch.empty((sum(recv), rows.shape[1]), dtype=rows.dtype, device=rows.device)
+    dist.all_to_all_single(out, rows[:sum(send)], output_split_sizes=recv, input_split_sizes=send, group=group)
+    return out
+
+
 class ExpertParallelMoE:
     """Expert-parallel `MoELayer.forward` (moe_lm.py:548-577) for one layer.
 
@@ -60,7 +89,7 @@ class ExpertParallelMoE:
     slice [E/W, ...]; router and shared-expert weights are replicated."""
 
     def __init__(self, weights: dict, num_experts: int, topk: int, group=None, backend=None, transport=None):
-        """transport: a `PeerTransport` -> the exchange runs over NVLink peer memory with our own kernels (fused
+        """transport: a `FusedPeerTransport` -> the exchange runs over NVLink peer memory with our own kernels (fused
         permute+dispatch, device-side barriers, no host sync); None -> NCCL all-to-all-v (needs one host sync)."""
         self.transport = transport
         self.w = weights
@@ -85,85 +114,27 @@ class ExpertParallelMoE:
         return out
 
     def forward(self, x: torch.Tensor) -> torch.Tensor:
-        if isinstance(self.transport, FusedPeerTransport):
-            return _ep_forward_fused(self, x)
         if self.transport is not None:
-            return _ep_forward_p2p(self, x)
+            return _ep_forward_fused(self, x)
         shape = x.shape
         x2 = x.reshape(-1, shape[-1])
-        be, W, E_loc = self.backend, self.W, self.E_loc
+        be = self.backend
         scores, idx, counts = be.router(x2, self.w["router.weight"], self.k)
         permuted, dest = be.permute(x2, idx, counts)  # rows sorted by global expert id == by destination rank
-
-        # per-(destination rank, local expert) counts -> everyone learns what it will receive
-        send_counts = counts.to(torch.int64).view(W, E_loc)
-        recv_counts = torch.empty_like(send_counts)  # [source rank, local expert]
-        dist.all_to_all_single(recv_counts, send_counts, group=self.group)
-        send_host = send_counts.sum(1).tolist()  # the one host sync per layer (NCCL split sizes live on the host)
-        recv_host = recv_counts.sum(1).tolist()
-
-        recv_rows = torch.empty((sum(recv_host), x2.shape[1]), dtype=x2.dtype, device=x2.device)
-        dist.all_to_all_single(recv_rows, permuted, output_split_sizes=recv_host, input_split_sizes=send_host,
-                               group=self.group)
+        plan = exchange_plan(counts, self.group)
+        recv_rows = exchange_rows(permuted, plan, self.group)
         # shared expert is local work that overlaps with the exchange on the GPU (separate NCCL stream)
         shared = be.shared(x2, self.w["shared_experts.gate_proj.weight"], self.w["shared_experts.up_proj.weight"],
                            self.w["shared_experts.down_proj.weight"])
-        y_recv = be.grouped_mlp(recv_rows, self.w["experts.fc1.weight"], self.w["experts.fc2.weight"],
-                                recv_counts.reshape(-1).contiguous(), E_loc)
-        y = torch.empty_like(permuted)
-        dist.all_to_all_single(y, y_recv, output_split_sizes=send_host, input_split_sizes=recv_host, group=self.group)
+        y_recv = be.grouped_mlp(recv_rows, self.w["experts.fc1.weight"], self.w["experts.fc2.weight"], plan[0], self.E_loc)
+        y = exchange_rows(y_recv, plan, self.group, back=True, out=torch.empty_like(permuted))
         return be.combine(y, dest, scores, shared).view(shape)
 
     __call__ = forward
 
 
-class PeerTransport:
-    """NVLink peer-memory transport for the expert-parallel exchange (no NCCL, no host sync, CUDA-graph friendly).
-    One arena per rank, mapped by every peer (aria_b200/peer.py):
-
-        counts_all [W, E] int32 | flags [W] int32 | recv_x [cap_rows, d] bf16 | ret_y [T_max*k, d] bf16
-
-    cap_rows = W * T_max * k covers the worst case of every token of every rank routed to one rank's experts."""
-
-    def __init__(self, T_max: int, hidden: int, num_experts: int, topk: int, device, group=None):
-        from .peer import PeerArena
-        self.group = group
-        self.W = dist.get_world_size(group)
-        self.rank = dist.get_rank(group)
-        self.E, self.k, self.d = num_experts, topk, hidden
-        self.E_loc = num_experts // self.W
-        self.cap_rows = self.W * T_max * topk
-        self.ret_rows = T_max * topk
-        al = lambda n: (n + 1023) // 1024 * 1024
-        self.off_counts = 0
-        self.off_flags = al(self.W * num_experts * 4)
-        self.off_recv = self.off_flags + al(self.W * 4)
-        self.off_ret = self.off_recv + al(self.cap_rows * hidden * 2)
-        total = self.off_ret + al(self.ret_rows * hidden * 2)
-        self.arena = PeerArena(total, device, group)
-        dev = torch.device(device)
-        mk = lambda off: torch.tensor([self.arena.ptr(r, off) for r in range(self.W)], dtype=torch.int64, device=dev)
-        self.p_counts, self.p_flags, self.p_recv, self.p_ret = mk(self.off_counts), mk(self.off_flags), mk(self.off_recv), mk(self.off_ret)
-        self.counts_all = self.arena.local_view(self.off_counts, (self.W, num_experts), torch.int32)
-        self.recv_x = self.arena.local_view(self.off_recv, (self.cap_rows, hidden), torch.bfloat16)
-        self.ret_y = self.arena.local_view(self.off_ret, (self.ret_rows, hidden), torch.bfloat16)
-        self.roff = torch.zeros(self.W * self.E_loc + 1, dtype=torch.int32, device=dev)
-        self.send_base = torch.zeros(num_experts, dtype=torch.int32, device=dev)
-        self.ret_base = torch.zeros(self.W * self.E_loc, dtype=torch.int32, device=dev)
-        self.epoch = torch.zeros(1, dtype=torch.int32, device=dev)  # device-side barrier counter (graph-replay safe)
-        self.device = dev
-
-    def barrier(self):
-        from . import _lib as L
-        import ctypes as C
-        with torch.cuda.device(self.device):
-            L.check(L.load().aria_peer_barrier(C.c_void_p(self.p_flags.data_ptr()), self.rank, self.W,
-                                               C.c_void_p(self.epoch.data_ptr()),
-                                               C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), "peer_barrier")
-
-
 class FusedPeerTransport:
-    """Round-2 exchange (csrc/ep.cu "Fused exchange"): fixed-capacity receive regions, the dispatch fused into the permute
+    """NVLink peer-memory exchange (csrc/ep.cu): fixed-capacity receive regions, the dispatch fused into the permute
     kernel, the return path fused into the fc2 GEMM epilogue, two device-side barriers per layer, no host sync, CUDA-graph
     friendly.  Arena of every rank (mapped by all peers):
 
@@ -205,7 +176,13 @@ class FusedPeerTransport:
         self.epoch = torch.zeros(1, dtype=torch.int32, device=dev)
         self.device = dev
 
-    barrier = PeerTransport.barrier
+    def barrier(self):
+        from . import _lib as L
+        import ctypes as C
+        with torch.cuda.device(self.device):
+            L.check(L.load().aria_peer_barrier(C.c_void_p(self.p_flags.data_ptr()), self.rank, self.W,
+                                               C.c_void_p(self.epoch.data_ptr()),
+                                               C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), "peer_barrier")
 
 
 def _ep_forward_fused(self, x: torch.Tensor) -> torch.Tensor:
@@ -243,129 +220,16 @@ def _ep_forward_fused(self, x: torch.Tensor) -> torch.Tensor:
     return ops.unpermute_combine(tr.ret_y, dest, scores, shared).view(shape)
 
 
-def _ep_forward_p2p(self, x: torch.Tensor) -> torch.Tensor:
-    """ExpertParallelMoE.forward over NVLink peer memory: the permute kernel stores each expert-sorted row directly into the
-    owning rank's receive buffer (fused permute + dispatch), and expert outputs are stored straight back into the source
-    rank's buffer at their sorted position; three device-side barriers per layer, zero host syncs."""
-    import ctypes as C
-    from . import _lib as L
-    from . import ops
-    tr = self.transport
-    lib = L.load()
-    shape = x.shape
-    x2 = x.reshape(-1, shape[-1]).contiguous()
-    T = x2.shape[0]
-    assert T * self.k <= tr.ret_rows, "PeerTransport was sized for fewer tokens"
-    stream = lambda: C.c_void_p(torch.cuda.current_stream(x2.device).cuda_stream)
-    vp = lambda t: C.c_void_p(t.data_ptr())
-    scores, idx, counts, _ = ops.router_topk(x2, self.w["router.weight"], self.k)
-    offsets, dest, src = ops.build_permutation(idx, counts)
-    with torch.cuda.device(x2.device):
-        L.check(lib.aria_ep_publish_counts(vp(counts), vp(tr.p_counts), tr.rank, tr.W, tr.E, stream()), "ep_publish_counts")
-        tr.barrier()
-        L.check(lib.aria_ep_layout(vp(tr.counts_all), tr.rank, tr.W, tr.E, vp(tr.roff), vp(tr.send_base), vp(tr.ret_base),
-                                   stream()), "ep_layout")
-        # fused permute + dispatch: expert-sorted token rows -> the owners' receive buffers, over NVLink
-        L.check(lib.aria_scatter_rows_grouped(vp(x2), vp(src), vp(offsets), tr.E, vp(tr.send_base), tr.E_loc, vp(tr.p_recv),
-                                              tr.d, T * self.k, stream()), "scatter_rows_grouped")
-        # local shared expert while the rows are in flight on the other GPUs
-        shared = ops.linear(ops.linear_swiglu(x2, self.w["shared_experts.gate_proj.weight"],
-                                              self.w["shared_experts.up_proj.weight"]), self.w["shared_experts.down_proj.weight"])
-        tr.barrier()
-        h = ops.grouped_gemm(tr.recv_x, self.w["experts.fc1.weight"], tr.roff, swiglu=True, group_mod=tr.E_loc)
-        y_recv = ops.grouped_gemm(h, self.w["experts.fc2.weight"], tr.roff, group_mod=tr.E_loc)
-        # way back: expert outputs -> the source ranks' buffers at their original sorted rows
-        L.check(lib.aria_scatter_rows_grouped(vp(y_recv), None, vp(tr.roff), tr.W * tr.E_loc, vp(tr.ret_base), tr.E_loc,
-                                              vp(tr.p_ret), tr.d, tr.cap_rows, stream()), "scatter_rows_grouped")
-        tr.barrier()
-    return ops.unpermute_combine(tr.ret_y, dest, scores, shared).view(shape)
-
-
 def exchange_bytes_per_layer(tokens_per_rank: int, topk: int, hidden: int, world: int) -> float:
     """Expected bytes a rank sends per direction per layer: (W-1)/W of its k*T rows leave the rank (SURVEY.md §8e)."""
     return tokens_per_rank * topk * hidden * 2 * (world - 1) / world
 
 
-# ----------------------------------------------------------------------------------------------------------------------
-# Training path (BASELINE cfg 5: expert-parallel forward + backward).  CUDA only.
-class _EPMoEFunction(torch.autograd.Function):
-    """Expert-parallel MoE layer with explicit backward.  Forward = the exchange above with the training-mode layout
-    (every expert block padded to a multiple of 16 rows on the SENDER, so the (source rank, expert) groups on the receiver
-    are 16-aligned and feed the ragged wgrad GEMM directly).  Backward mirrors it: grad rows take the same two all-to-alls
-    in reverse; expert weight grads stay on the owning rank (no all-reduce); router / shared-expert grads are per-rank
-    partial sums (the usual data-parallel all-reduce is left to the caller, as in the reference's DP/ZeRO setup)."""
-
-    @staticmethod
-    def forward(ctx, x, w_router, fc1, fc2, gate_w, up_w, down_w, topk, group):
-        from . import ops
-        W = dist.get_world_size(group)
-        E = w_router.shape[0]
-        E_loc = E // W
-        shape = x.shape
-        x2 = x.reshape(-1, shape[-1]).contiguous()
-        scores, idx, counts, _ = ops.router_topk(x2, w_router, topk)
-        offsets, dest, src = ops.build_permutation(idx, counts, row_align=16)
-        xp = ops.permute_rows(x2, src)
-        padded = ((counts.to(torch.int64) + 15) // 16) * 16           # rows sent per expert (incl. zero pads)
-        send_counts = padded.view(W, E_loc)
-        recv_counts = torch.empty_like(send_counts)
-        dist.all_to_all_single(recv_counts, send_counts, group=group)
-        send_host = send_counts.sum(1).tolist()
-        recv_host = recv_counts.sum(1).tolist()
-        n_send = sum(send_host)
-        xr = torch.empty((sum(recv_host), x2.shape[1]), dtype=x2.dtype, device=x2.device)
-        dist.all_to_all_single(xr, xp[:n_send], output_split_sizes=recv_host, input_split_sizes=send_host, group=group)
-        roff = ops.offsets_from_counts(recv_counts.reshape(-1).contiguous())
-        h1 = ops.grouped_gemm(xr, fc1, roff, group_mod=E_loc)
-        h = ops.swiglu_fwd(h1)
-        yr = ops.grouped_gemm(h, fc2, roff, group_mod=E_loc)
-        y = torch.zeros_like(xp)
-        dist.all_to_all_single(y[:n_send], yr, output_split_sizes=send_host, input_split_sizes=recv_host, group=group)
-        hs1 = ops.linear_multi(x2, [gate_w, up_w])
-        hs = ops.swiglu_fwd(hs1)
-        shared = ops.linear(hs, down_w)
-        out = ops.unpermute_combine(y, dest, scores, shared)
-        ctx.save_for_backward(x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, dest, y, xr, h1, h, roff, hs1, hs)
-        ctx.meta = (shape, send_host, recv_host, n_send, E_loc, group, xp.shape[0])
-        return out.view(shape)
-
-    @staticmethod
-    def backward(ctx, dout):
-        from . import ops
-        (x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, dest, y, xr, h1, h, roff, hs1, hs) = ctx.saved_tensors
-        shape, send_host, recv_host, n_send, E_loc, group, rows_pad = ctx.meta
-        E, d = w_router.shape
-        Is = gate_w.shape[0]
-        T = x2.shape[0]
-        do = dout.reshape(-1, d).contiguous()
-        dense = torch.tensor([0, T], dtype=torch.int32, device=do.device)
-        dy, dscores = ops.combine_bwd(do, y, dest, scores)
-        dyr = torch.empty_like(xr)
-        dist.all_to_all_single(dyr, dy[:n_send], output_split_sizes=recv_host, input_split_sizes=send_host, group=group)
-        W = len(send_host)
-        d_fc2 = ops.grouped_wgrad(h, dyr, roff, num_sources=W)   # sums the W (source rank) row blocks of each local expert
-        dh = ops.grouped_gemm_nt(dyr, fc2, roff, group_mod=E_loc)
-        dh1 = ops.swiglu_bwd(h1, dh)
-        d_fc1 = ops.grouped_wgrad(xr, dh1, roff, num_sources=W)
-        dxr = ops.grouped_gemm_nt(dh1, fc1, roff, group_mod=E_loc)
-        dxp = torch.zeros((rows_pad, d), dtype=dxr.dtype, device=dxr.device)
-        dist.all_to_all_single(dxp[:n_send], dxr, output_split_sizes=send_host, input_split_sizes=recv_host, group=group)
-        d_down = ops.grouped_wgrad(do, hs, dense)[0]
-        dhs = ops.matmul_kn(do, down_w)
-        dhs1 = ops.swiglu_bwd(hs1, dhs)
-        d_gate = ops.grouped_wgrad(dhs1[:, :Is], x2, dense)[0]
-        d_up = ops.grouped_wgrad(dhs1[:, Is:], x2, dense)[0]
-        dx = ops.matmul_kn(dhs1[:, :Is], gate_w)
-        dx = ops.matmul_kn(dhs1[:, Is:], up_w, residual=dx)
-        dlogits = ops.router_bwd(dscores, scores, idx, E)
-        d_router = ops.grouped_wgrad(dlogits, x2, dense)[0]
-        dx = ops.matmul_kn(dlogits, w_router, residual=dx)
-        dx = ops.unpermute_combine(dxp, dest, torch.ones_like(scores), dx)
-        return dx.view(shape), d_router, d_fc1, d_fc2, d_gate, d_up, d_down, None, None
-
-
 def ep_moe_layer_train(x, w: dict, topk: int, group=None):
-    """Differentiable expert-parallel MoE layer; `w` as in ExpertParallelMoE (expert weights = this rank's slice)."""
-    return _EPMoEFunction.apply(x, w["router.weight"], w["experts.fc1.weight"], w["experts.fc2.weight"],
-                                w["shared_experts.gate_proj.weight"], w["shared_experts.up_proj.weight"],
-                                w["shared_experts.down_proj.weight"], topk, group)
+    """Differentiable expert-parallel MoE layer (BASELINE cfg 5): `moe_train.MoELayerFunction` over `group` (default: the
+    world), eval-mode routing; `w` as in ExpertParallelMoE (expert weights = this rank's slice)."""
+    from .moe_train import MoELayerFunction
+    return MoELayerFunction.apply(x, w["router.weight"], w["experts.fc1.weight"], w["experts.fc2.weight"],
+                                  w["shared_experts.gate_proj.weight"], w["shared_experts.up_proj.weight"],
+                                  w["shared_experts.down_proj.weight"], topk, None, None,
+                                  dist.group.WORLD if group is None else group)

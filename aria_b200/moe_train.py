@@ -13,6 +13,11 @@ load-balancing-loss gradients (moe_lm.py:84-166) are added to dlogits by `aria_r
 `MoEAuxLossAutoScaler.main_loss_backward_scale` of `loss_scale_source` (read at backward time, as the reference's autograd
 function does; default: aria_b200.moe_lm's holder — the trainable seam passes the reference module's own class); the default
 (False) is eval-mode routing, which is what BASELINE cfg 5 times.
+Expert parallelism: with a process `group` (`expert_parallel.ep_moe_layer_train`, what BASELINE cfg 5 times) this rank holds
+only its slice of the experts and the same launches run with the all-to-alls inserted: the 16-padded expert blocks go to their
+owners between the permute and fc1 and come back into a zeroed buffer between fc2 and the combine; backward sends dy to the
+owners before the fc2 wgrad/dgrad and brings dxp back before the un-permute.  Expert weight grads stay on the owning rank;
+router and shared-expert grads are per-rank partial sums (the usual data-parallel all-reduce is left to the caller).
 Gradients are bf16 tensors accumulated in fp32 inside the tensor-core kernels.
 """
 from __future__ import annotations
@@ -21,38 +26,49 @@ import torch
 
 from . import _lib as L
 from . import ops
+from .expert_parallel import exchange_plan, exchange_rows
 
 
 class MoELayerFunction(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, w_router, fc1, fc2, gate_w, up_w, down_w, topk: int, loss_coeffs=None, loss_scale_source=None):
+    def forward(ctx, x, w_router, fc1, fc2, gate_w, up_w, down_w, topk: int, loss_coeffs=None, loss_scale_source=None,
+                group=None):
         shape = x.shape
         x2 = x.reshape(-1, shape[-1]).contiguous()
-        E = w_router.shape[0]
-        I = fc2.shape[1]
         scores, idx, counts, _logits = ops.router_topk(x2, w_router, topk)
         offsets, dest, src = ops.build_permutation(idx, counts, row_align=16)
         xp = ops.permute_rows(x2, src)                       # [rows_pad, d], pad rows zero
-        h1 = ops.grouped_gemm(xp, fc1, offsets)              # [rows_pad, 2I]
+        # the expert GEMMs' rows xe and offsets: every row here, or under a group the rows all ranks sent to my experts,
+        # grouped by (source rank, local expert) (16-aligned: each expert block is sent with its pad rows)
+        xe, off, plan, group_mod = xp, offsets, None, 0
+        if group is not None:
+            plan = exchange_plan(counts, group, row_align=16)
+            xe = exchange_rows(xp, plan, group)
+            off = ops.offsets_from_counts(plan[0])
+            group_mod = fc1.shape[0]
+        h1 = ops.grouped_gemm(xe, fc1, off, group_mod=group_mod)   # [rows, 2I]
         h = ops.swiglu_fwd(h1)
-        y = ops.grouped_gemm(h, fc2, offsets)                # [rows_pad, d]
+        y = ops.grouped_gemm(h, fc2, off, group_mod=group_mod)     # [rows, d]
+        if group is not None:
+            y = exchange_rows(y, plan, group, back=True, out=torch.zeros_like(xp))
         # shared expert: gate|up in one GEMM (two B segments), unfused glu so that the pre-activation is kept
         hs1 = ops.linear_multi(x2, [gate_w, up_w])
         hs = ops.swiglu_fwd(hs1)
         shared = ops.linear(hs, down_w)
         out = ops.unpermute_combine(y, dest, scores, shared)
-        ctx.save_for_backward(x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, offsets, dest, xp, h1, h, y, hs1, hs)
+        ctx.save_for_backward(x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, off, dest, xe, h1, h, y, hs1, hs)
         ctx.topk = topk
         ctx.loss_coeffs = loss_coeffs
         ctx.loss_scale_source = loss_scale_source
         if loss_coeffs is not None:  # keep what the loss gradients need: the bf16 logits and tokens_per_expert
             ctx.router_logits, ctx.counts = _logits, counts
-        ctx.shape = shape
+        ctx.shape, ctx.plan, ctx.group = shape, plan, group
         return out.view(shape)
 
     @staticmethod
     def backward(ctx, dout):
-        (x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, offsets, dest, xp, h1, h, y, hs1, hs) = ctx.saved_tensors
+        (x2, w_router, fc1, fc2, gate_w, up_w, down_w, scores, idx, off, dest, xe, h1, h, y, hs1, hs) = ctx.saved_tensors
+        plan, group = ctx.plan, ctx.group
         E, d = w_router.shape
         Is = gate_w.shape[0]
         T = x2.shape[0]
@@ -60,19 +76,26 @@ class MoELayerFunction(torch.autograd.Function):
         # a gradient nobody needs (frozen weight, input without requires_grad) is neither computed nor launched; the ones
         # computed run the same kernels in the same order as when every gradient is needed
         need_x, need_r, need_fc1, need_fc2, need_gate, need_up, need_down = ctx.needs_input_grad[:7]
+        # every rank must issue the exchanges (collectives), so under a group the routed data-gradient chain always runs
+        need_dxp = need_x or group is not None
+        group_mod, num_sources = (0, 1) if group is None else (fc1.shape[0], len(plan[1]))
         dense = torch.tensor([0, T], dtype=torch.int32, device=do.device)  # one 16-aligned "group" for dense wgrads
         d_router = d_fc1 = d_fc2 = d_gate = d_up = d_down = dx = None
         # ---- routed experts
         dy, dscores = ops.combine_bwd(do, y, dest, scores)
+        if group is not None:
+            dy = exchange_rows(dy, plan, group)                                # to the experts' owners
         if need_fc2:
-            d_fc2 = ops.grouped_wgrad(h, dy, offsets)                         # [E, I, d]
-        if need_x or need_fc1:
-            dh = ops.grouped_gemm_nt(dy, fc2, offsets)                        # dy @ fc2[e].T -> [rows, I]
+            d_fc2 = ops.grouped_wgrad(h, dy, off, num_sources=num_sources)    # [E, I, d]
+        if need_dxp or need_fc1:
+            dh = ops.grouped_gemm_nt(dy, fc2, off, group_mod=group_mod)       # dy @ fc2[e].T -> [rows, I]
             dh1 = ops.swiglu_bwd(h1, dh)
             if need_fc1:
-                d_fc1 = ops.grouped_wgrad(xp, dh1, offsets)                   # [E, d, 2I]
-            if need_x:
-                dxp = ops.grouped_gemm_nt(dh1, fc1, offsets)                  # [rows, d]
+                d_fc1 = ops.grouped_wgrad(xe, dh1, off, num_sources=num_sources)  # [E, d, 2I]
+            if need_dxp:
+                dxp = ops.grouped_gemm_nt(dh1, fc1, off, group_mod=group_mod)  # [rows, d]
+                if group is not None:
+                    dxp = exchange_rows(dxp, plan, group, back=True, out=torch.zeros_like(y))
         # ---- shared expert (out += shared: its upstream gradient is dout itself)
         if need_down:
             d_down = ops.grouped_wgrad(do, hs, dense)[0]                      # [d, Is]
@@ -104,7 +127,7 @@ class MoELayerFunction(torch.autograd.Function):
         if need_x:
             ones = torch.ones_like(scores)
             dx = ops.unpermute_combine(dxp, dest, ones, dx).view(ctx.shape)
-        return dx, d_router, d_fc1, d_fc2, d_gate, d_up, d_down, None, None, None
+        return dx, d_router, d_fc1, d_fc2, d_gate, d_up, d_down, None, None, None, None
 
 
 def moe_layer_train(layer, hidden_states: torch.Tensor, router_losses: bool = False) -> torch.Tensor:

@@ -106,7 +106,7 @@ def linear_swiglu(x: torch.Tensor, gate_w: torch.Tensor, up_w: torch.Tensor) -> 
 
 
 def grouped_gemm(a: torch.Tensor, b: torch.Tensor, offsets: torch.Tensor, swiglu: bool = False,
-                 dbg=(0, 0, 0), group_mod: int = 0, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 group_mod: int = 0, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out[off[e]:off[e+1]] = a[off[e]:off[e+1]] @ b[e] (+ residual); b [E, K, N] (GroupedGEMM.weight, moe_lm.py:465).
     swiglu=True fuses `glu` (moe_lm.py:505-507): b has 2I columns, out has I."""
     _chk(a), _chk(b), _chk(offsets, torch.int32)
@@ -128,7 +128,6 @@ def grouped_gemm(a: torch.Tensor, b: torch.Tensor, offsets: torch.Tensor, swiglu
         assert not swiglu and residual.shape == out.shape
         _chk(residual)
         d.residual, d.ldr = residual.data_ptr(), N
-    d.dbg_lbo, d.dbg_sbo, d.dbg_kadv = dbg
     _run_gemm(d, a, "grouped_gemm")
     return out
 

@@ -79,8 +79,6 @@ typedef struct aria_gemm_desc {
   const void* rope_cos;    /* [max_pos, head_dim] bf16 tables (aria_rope_table)                          */
   const void* rope_sin;
   const int32_t* position_ids; /* [m] or NULL (then position = pos0 + token)                              */
-  /* debug overrides of the B operand's wgmma shared-memory descriptor fields (0 = default); bring-up only */
-  int32_t dbg_lbo, dbg_sbo, dbg_kadv;
   /* Expert parallelism over NVLink peer memory (fused compute + collective, SURVEY.md §8e):
    *   group_counts  non-NULL: group g = rows [group_offsets[g], group_offsets[g] + group_counts[g]) — fixed-capacity
    *                 regions a peer GPU fills without knowing the other senders' counts; a_rows = rows of the A buffer
@@ -231,17 +229,8 @@ int aria_ipc_close(void* base);
 /* Expert-parallel exchange over NVLink peer memory (aria_b200/csrc/ep.cu): replaces the all-to-all the reference's
  * dispatcher lost (moe_lm.py:296-297).  `peer_*` arrays are device arrays of W addresses (one per rank, as mapped on THIS
  * GPU).  All calls are asynchronous and need no host sync. */
-int aria_ep_publish_counts(const int32_t* counts, const uint64_t* peer_counts, int32_t rank, int32_t W, int32_t E,
-                           aria_stream_t stream);                      /* my counts[E] -> counts_all[rank][:] on every rank */
 int aria_peer_barrier(const uint64_t* peer_flags, int32_t rank, int32_t W, int32_t* epoch_dev /* device counter, advanced by the call */,
                       aria_stream_t stream);
-int aria_ep_layout(const int32_t* counts_all, int32_t rank, int32_t W, int32_t E, int32_t* roff, int32_t* send_base,
-                   int32_t* ret_base, aria_stream_t stream);          /* roff[W*E/W+1], send_base[E], ret_base[W*E/W] */
-/* Fused permute + dispatch (and the way back): row i of group g -> rank g/group_div, row dst_row_base[g] + i - off[g];
- * source row = rows[src_token ? src_token[i] : i].  max_rows only sizes the grid. */
-int aria_scatter_rows_grouped(const void* rows, const int32_t* src_token, const int32_t* group_offsets, int32_t G,
-                              const int32_t* dst_row_base, int32_t group_div, const uint64_t* peer_bufs, int32_t d,
-                              int64_t max_rows, aria_stream_t stream);
 /* Fused exchange (fixed-capacity regions; see csrc/ep.cu): gathers the token rows in expert order (src_token / offsets from
  * aria_build_permutation) and stores each into region (e % E_loc, rank) = index (e % E_loc) * W + rank of owner e / E_loc — peer_recv[p] = rank p's receive
  * buffer [W*E_loc][cap][d] as mapped on this GPU — and publishes per-block (row count, first sorted row) into the owners'

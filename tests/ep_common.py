@@ -81,16 +81,13 @@ def ep_worker(rank, world, port, backend_name, device_kind, tc, T, dtype_name, r
     shard = {k: v.to(dev) for k, v in ExpertParallelMoE.shard_state(full, rank, world).items()}
     backend = OracleBackend(tc["moe_topk"]) if backend_name == "oracle" else None
     transport = None
-    if backend_name == "p2p":
-        from aria_b200.expert_parallel import PeerTransport
-        transport = PeerTransport(T + 3 * world, tc["hidden_size"], tc["moe_num_experts"], tc["moe_topk"], dev)
     if backend_name == "fused":
         from aria_b200.expert_parallel import FusedPeerTransport
         transport = FusedPeerTransport(T + 3 * world, tc["hidden_size"], tc["moe_intermediate_size"], tc["moe_num_experts"],
                                        tc["moe_topk"], dev)
     ep = ExpertParallelMoE(shard, tc["moe_num_experts"], tc["moe_topk"], backend=backend, transport=transport)
     got = ep(x.to(dev)).float().cpu()
-    if backend_name in ("p2p", "fused"):  # a second layer through the same arena (buffer reuse across layers) must agree too
+    if backend_name == "fused":  # a second layer through the same arena (buffer reuse across layers) must agree too
         got2 = ep(x.to(dev)).float().cpu()
         assert torch.equal(got, got2)
     if device_kind == "cuda":

@@ -40,7 +40,7 @@ def _counts(offsets):
     return (offsets[1:] - offsets[:-1]).long()
 
 
-def grouped_gemm(a, b, offsets, swiglu=False, dbg=(0, 0, 0), group_mod=0, residual=None):
+def grouped_gemm(a, b, offsets, swiglu=False, group_mod=0, residual=None):
     assert not group_mod
     y = O.sequential_gemm(a, b, _counts(offsets))
     if swiglu:

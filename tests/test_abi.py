@@ -32,8 +32,9 @@ def test_exports_every_declared_symbol(lib):
         assert s in _lib.SIGNATURES, f"{s} has no ctypes signature in aria_b200/_lib.py"
 
 
-def test_version_and_arch(lib):
-    assert lib.aria_abi_version() == 2
+def test_abi_version_3_and_arch(lib):
+    """Version 3: `aria_gemm_desc_t` without the descriptor debug fields, and 41 entries (no round-1 peer transport)."""
+    assert lib.aria_abi_version() == 3
     assert lib.aria_build_arch() == b"sm_90a"
 
 

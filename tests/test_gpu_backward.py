@@ -86,6 +86,55 @@ def test_moe_layer_forward_backward_vs_oracle_autograd(T, E, k, d, I):
         assert _rel_l2(p_.grad, sd32[n].grad) <= tol, n
 
 
+def _one_rank_ep_worker(rank, port, tc, T, result_dir):
+    """ep_moe_layer_train on a one-rank NCCL group and MoELayerFunction without a group, on the same inputs."""
+    import os
+    import sys
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    if root not in sys.path:
+        sys.path.insert(0, root)
+    import torch.distributed as dist
+    from aria_b200.expert_parallel import ep_moe_layer_train
+    from aria_b200.moe_train import MoELayerFunction
+    from oracle import configs as C
+    os.environ["MASTER_ADDR"] = "127.0.0.1"
+    os.environ["MASTER_PORT"] = str(port)
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(dev)
+    dist.init_process_group("nccl", rank=0, world_size=1, device_id=dev)
+    gen = torch.Generator().manual_seed(5)
+    sd = {n: v.bfloat16().to(dev) for n, v in C.moe_layer_state(tc, gen).items()}
+    x = torch.randn(T, tc["hidden_size"], generator=gen).bfloat16().to(dev)
+    gout = torch.randn(T, tc["hidden_size"], generator=gen).bfloat16().to(dev)
+    names = ["router.weight", "experts.fc1.weight", "experts.fc2.weight", "shared_experts.gate_proj.weight",
+             "shared_experts.up_proj.weight", "shared_experts.down_proj.weight"]
+    runs = []
+    for ep in (True, False):
+        w = {n: sd[n].clone().requires_grad_(True) for n in names}
+        xg = x.clone().requires_grad_(True)
+        with torch.enable_grad():
+            out = (ep_moe_layer_train(xg, w, tc["moe_topk"]) if ep else
+                   MoELayerFunction.apply(xg, *[w[n] for n in names], tc["moe_topk"]))
+            out.backward(gout)
+        runs.append({"out": out.detach(), "dx": xg.grad, **{n: w[n].grad for n in names}})
+    torch.cuda.synchronize()
+    torch.save({k: torch.equal(runs[0][k], runs[1][k]) for k in runs[0]}, os.path.join(result_dir, "equal.pt"))
+    dist.destroy_process_group()
+
+
+def test_one_rank_expert_parallel_layer_is_bit_identical_to_single_device():
+    """BASELINE cfg 5 on one GPU: the expert-parallel layer over a one-rank group runs the single-device kernels on the
+    same rows (group_mod = E over E groups picks weight block g, as group_mod = 0 does), so every output is bit-equal."""
+    import tempfile
+    import torch.multiprocessing as mp
+    from ep_common import free_port
+    tc = dict(hidden_size=256, moe_num_experts=64, moe_topk=6, moe_intermediate_size=128, moe_num_shared_experts=2)
+    with tempfile.TemporaryDirectory() as tmp:
+        mp.spawn(_one_rank_ep_worker, args=(free_port(), tc, 300, tmp), nprocs=1, join=True)
+        equal = torch.load(f"{tmp}/equal.pt")
+    assert len(equal) == 8 and all(equal.values()), equal
+
+
 def test_wgrad_two_cta_path_and_sources():
     """Many output tiles of large weight matrices (more tiles than SMs), plus the expert-parallel
     `num_sources` accumulation (offsets over (source, group) pairs, out[g] sums the sources)."""

@@ -12,8 +12,8 @@ pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
-# NCCL all-to-all-v / round-1 NVLink peer-memory kernels / fused exchange (dispatch in the permute kernel, return in the fc2 epilogue)
-@pytest.mark.parametrize("transport", ["cuda", "p2p", "fused"])
+# NCCL all-to-all-v / NVLink peer-memory exchange (dispatch in the permute kernel, return in the fc2 epilogue)
+@pytest.mark.parametrize("transport", ["cuda", "fused"])
 @pytest.mark.parametrize("E,k,T,d,I", [(8, 2, 50, 256, 128), (64, 6, 1024, 2560, 1664)])
 def test_ep_forward_two_gpus(E, k, T, d, I, transport):
     tc = dict(hidden_size=d, moe_num_experts=E, moe_topk=k, moe_intermediate_size=I, moe_num_shared_experts=2)

@@ -97,7 +97,7 @@ def _stand_in_ops(monkeypatch):
     def from_counts(c):
         return torch.cat([torch.zeros(1, dtype=torch.int64), c.cumsum(0)]).to(torch.int32)
 
-    def grouped_gemm(a, b, off, swiglu=False, dbg=(0, 0, 0), group_mod=0, residual=None):
+    def grouped_gemm(a, b, off, swiglu=False, group_mod=0, residual=None):
         o, out = offs(off), torch.zeros(a.shape[0], b.shape[2], dtype=a.dtype)
         for e in range(b.shape[0]):
             out[o[e]:o[e + 1]] = (a[o[e]:o[e + 1]].float() @ b[e].float()).to(a.dtype)

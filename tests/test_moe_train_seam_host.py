@@ -1,5 +1,6 @@
 """CPU: host logic of the trainable MoE seams — which path `install(..., trainable=True)` takes in each mode, its refusals, the
-router-loss scale plumbing and the `needs_input_grad` skipping of the backward kernels.  The kernels are replaced by shape-only
+router-loss scale plumbing, the `needs_input_grad` skipping of the backward kernels and the MoE layer's launch sequence with and
+without expert parallelism.  The kernels are replaced by shape-only
 recorders (zeros of the right shape; every call logged), or by the oracle-backed stand-ins of tests/standin_ops.py for the
 inference path; the arithmetic is covered on the GPU by tests/test_gpu_moe_train_seam.py."""
 import os
@@ -27,16 +28,19 @@ class Recorder:
 
     def __init__(self):
         self.calls = []
+        self.seq = []             # the calls with the expert-grouping arguments, e.g. "grouped_gemm group_mod=4"
         self.loss_scales = []
 
-    def _log(self, name):
+    def _log(self, name, **kw):
         self.calls.append(name)
+        self.seq.append(" ".join([name] + [f"{k}={v}" for k, v in kw.items()]))
 
     def router_topk(self, x, w, k):
         self._log("router_topk")
         T, E = x.shape[0], w.shape[0]
         idx = (torch.arange(T * k) % E).view(T, k).to(torch.int32)
-        return torch.zeros(T, k, dtype=bf16), idx, torch.zeros(E, dtype=torch.int32), torch.zeros(T, E, dtype=bf16)
+        counts = torch.bincount(idx.flatten().long(), minlength=E).to(torch.int32)
+        return torch.zeros(T, k, dtype=bf16), idx, counts, torch.zeros(T, E, dtype=bf16)
 
     def build_permutation(self, idx, counts, row_align=1):
         self._log("build_permutation")
@@ -49,16 +53,20 @@ class Recorder:
         self._log("permute_rows")
         return torch.zeros(src.numel(), x.shape[1], dtype=bf16)
 
-    def grouped_gemm(self, a, b, off, swiglu=False, residual=None, **_):
-        self._log("grouped_gemm")
+    def offsets_from_counts(self, counts):
+        self._log("offsets_from_counts")
+        return torch.zeros(counts.numel() + 1, dtype=torch.int32)
+
+    def grouped_gemm(self, a, b, off, swiglu=False, group_mod=0, residual=None):
+        self._log("grouped_gemm", group_mod=group_mod)
         return torch.zeros(a.shape[0], b.shape[2] // (2 if swiglu else 1), dtype=bf16)
 
-    def grouped_gemm_nt(self, a, b, off, residual=None, **_):
-        self._log("grouped_gemm_nt")
+    def grouped_gemm_nt(self, a, b, off, group_mod=0, residual=None):
+        self._log("grouped_gemm_nt", group_mod=group_mod)
         return torch.zeros(a.shape[0], b.shape[1], dtype=bf16)
 
     def grouped_wgrad(self, a, b, off, num_sources=1):
-        self._log("grouped_wgrad")
+        self._log("grouped_wgrad", num_sources=num_sources)
         return torch.zeros((off.numel() - 1) // num_sources, a.shape[1], b.shape[1], dtype=bf16)
 
     def swiglu_fwd(self, h1):
@@ -148,6 +156,66 @@ def test_loss_scale_is_read_from_the_given_holder_at_backward_time(rec, monkeypa
     holder.main_loss_backward_scale = 3.0
     scores.float().sum().backward()
     assert rec.loss_scales == [(0.25, 0.5, 3.0)]
+
+
+_FWD = ["router_topk", "build_permutation", "permute_rows", "grouped_gemm group_mod=0", "swiglu_fwd", "grouped_gemm group_mod=0",
+        "linear_multi", "swiglu_fwd", "linear", "unpermute_combine"]
+_BWD = ["combine_bwd", "grouped_wgrad num_sources=1", "grouped_gemm_nt group_mod=0", "swiglu_bwd", "grouped_wgrad num_sources=1",
+        "grouped_gemm_nt group_mod=0", "grouped_wgrad num_sources=1", "matmul_kn", "swiglu_bwd", "grouped_wgrad num_sources=1",
+        "grouped_wgrad num_sources=1", "matmul_kn", "matmul_kn", "router_bwd", "grouped_wgrad num_sources=1", "matmul_kn",
+        "unpermute_combine"]
+# one rank over E=4 experts: the same launches with the exchange steps inserted and the expert GEMMs over (source, expert) groups
+_EP_FWD = ["router_topk", "build_permutation", "permute_rows", "all_to_all_single", "all_to_all_single", "offsets_from_counts",
+           "grouped_gemm group_mod=4", "swiglu_fwd", "grouped_gemm group_mod=4", "all_to_all_single", "linear_multi", "swiglu_fwd",
+           "linear", "unpermute_combine"]
+_EP_BWD = ["combine_bwd", "all_to_all_single", "grouped_wgrad num_sources=1", "grouped_gemm_nt group_mod=4", "swiglu_bwd",
+           "grouped_wgrad num_sources=1", "grouped_gemm_nt group_mod=4", "all_to_all_single", "grouped_wgrad num_sources=1",
+           "matmul_kn", "swiglu_bwd", "grouped_wgrad num_sources=1", "grouped_wgrad num_sources=1", "matmul_kn", "matmul_kn",
+           "router_bwd", "grouped_wgrad num_sources=1", "matmul_kn", "unpermute_combine"]
+
+
+def test_moe_layer_launch_sequence_with_and_without_expert_parallelism(rec, monkeypatch, tmp_path):
+    """The full sequence of kernel calls of the MoE layer's forward and backward, single-device and through
+    `ep_moe_layer_train` on a one-rank gloo group (the all-to-alls logged where they are issued)."""
+    import torch.distributed as dist
+    from aria_b200 import moe_train
+    from aria_b200.expert_parallel import ep_moe_layer_train
+    args = [t.requires_grad_(True) for t in _block_args()]
+    out = moe_train.MoELayerFunction.apply(*args, 2)
+    assert rec.seq == _FWD
+    rec.seq.clear()
+    out.sum().backward()
+    assert rec.seq == _BWD
+    real = dist.all_to_all_single
+
+    def all_to_all_single(*a, **kw):
+        rec._log("all_to_all_single")
+        return real(*a, **kw)
+
+    monkeypatch.setattr(dist, "all_to_all_single", all_to_all_single)
+    dist.init_process_group("gloo", init_method=f"file://{tmp_path}/store", rank=0, world_size=1)
+    try:
+        args = [t.detach().requires_grad_(True) for t in _block_args()]
+        w = dict(zip(["router.weight", "experts.fc1.weight", "experts.fc2.weight", "shared_experts.gate_proj.weight",
+                      "shared_experts.up_proj.weight", "shared_experts.down_proj.weight"], args[1:]))
+        rec.seq.clear()
+        out = ep_moe_layer_train(args[0], w, 2)
+        assert rec.seq == _EP_FWD
+        rec.seq.clear()
+        out.sum().backward()
+        assert rec.seq == _EP_BWD
+        assert all(t.grad is not None for t in args)
+        # skipped gradients under a group: only the wgrads and the local kernels go; the exchanges and the routed
+        # data-gradient chain between them are collective work every rank issues
+        for t in args:
+            t.requires_grad_(t is w["experts.fc2.weight"])
+        out = ep_moe_layer_train(args[0], w, 2)
+        rec.seq.clear()
+        out.sum().backward()
+        assert rec.seq == ["combine_bwd", "all_to_all_single", "grouped_wgrad num_sources=1", "grouped_gemm_nt group_mod=4",
+                           "swiglu_bwd", "grouped_gemm_nt group_mod=4", "all_to_all_single"]
+    finally:
+        dist.destroy_process_group()
 
 
 def test_differentiable_gmm_skips_unneeded_gradients(rec):
