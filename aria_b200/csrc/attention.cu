@@ -18,6 +18,7 @@
 // of the ViT path) than rounding P relative to the exact running max, and it skips most rescales of O.
 //
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
+// aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -370,20 +371,27 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // ------------------------------------------------------------------------------------------------
 // Decode: one query per (b,h); block = 4 warps over a contiguous chunk of keys; each lane owns 4 dims.
 // Partial (m, l, acc[128]) per (b,h,split) -> workspace; a second kernel merges the splits.
+// DEVLEN: the key count of row b is the device value lens[b] (at most Tk = T_max, the cache rows the grid is sized for) and
+// the key mask has the row stride mask_stride.  A split that starts past lens[b] sees no key and writes (m = -inf, l = 0,
+// acc = 0); the merge reads the first ceil(lens[b] / DEC_SPLIT_KEYS) splits only, so row b is bit-identical to the host-length
+// launch with Tk = lens[b].
 constexpr int DEC_SPLIT_KEYS = 256;
 
+template <bool DEVLEN>
 __global__ void __launch_bounds__(128) attn_decode_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                                                            const __nv_bfloat16* __restrict__ vc, const uint8_t* __restrict__ key_mask,
                                                            float* __restrict__ ws, int H, int Tk,
                                                            int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
-                                                           int64_t kv_stride_h, float scale_log2, int splits) {
+                                                           int64_t kv_stride_h, float scale_log2, int splits,
+                                                           const int32_t* __restrict__ lens, int mask_stride) {
   const int bh = blockIdx.x, split = blockIdx.y;
   const int b = bh / H, h = bh % H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int k_begin = split * DEC_SPLIT_KEYS, k_end = min(Tk, k_begin + DEC_SPLIT_KEYS);
+  const int len = DEVLEN ? min(lens[b], Tk) : Tk;
+  const int k_begin = split * DEC_SPLIT_KEYS, k_end = min(len, k_begin + DEC_SPLIT_KEYS);
   const __nv_bfloat16* kbase = kc + b * kv_stride_b + h * kv_stride_h;
   const __nv_bfloat16* vbase = vc + b * kv_stride_b + h * kv_stride_h;
-  const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(b) * Tk : nullptr;
+  const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(b) * (DEVLEN ? mask_stride : Tk) : nullptr;
   const uint2 qv = *reinterpret_cast<const uint2*>(q + b * q_stride_b + h * q_stride_h + lane * 4);
   const float q0 = bf16_lo(qv.x) * scale_log2, q1 = bf16_hi(qv.x) * scale_log2, q2 = bf16_lo(qv.y) * scale_log2,
               q3 = bf16_hi(qv.y) * scale_log2;
@@ -452,13 +460,16 @@ __global__ void __launch_bounds__(128) attn_decode_partial(const __nv_bfloat16* 
   }
 }
 
-__global__ void __launch_bounds__(128) attn_decode_merge(const float* __restrict__ ws, __nv_bfloat16* __restrict__ out, int splits) {
+template <bool DEVLEN>
+__global__ void __launch_bounds__(128) attn_decode_merge(const float* __restrict__ ws, __nv_bfloat16* __restrict__ out, int splits,
+                                                         const int32_t* __restrict__ lens, int H) {
   const int bh = blockIdx.x, d = threadIdx.x;
   const float* base = ws + static_cast<int64_t>(bh) * splits * (AT_D + 2);
+  const int n = DEVLEN ? min(splits, (lens[bh / H] + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS) : splits;
   float M = -INFINITY;
-  for (int s = 0; s < splits; ++s) M = fmaxf(M, base[s * (AT_D + 2) + AT_D]);
+  for (int s = 0; s < n; ++s) M = fmaxf(M, base[s * (AT_D + 2) + AT_D]);
   float L = 0.f, A = 0.f;
-  for (int s = 0; s < splits; ++s) {
+  for (int s = 0; s < n; ++s) {
     const float ms = base[s * (AT_D + 2) + AT_D];
     const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - M);
     L += base[s * (AT_D + 2) + AT_D + 1] * f;
@@ -575,11 +586,34 @@ extern "C" int aria_attention_decode(const void* q, const void* k, const void* v
   ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(B, H, Tk));
   const int splits = (Tk + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
   dim3 grid(B * H, splits);
-  attn_decode_partial<<<grid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k),
-                                                static_cast<const __nv_bfloat16*>(v), key_mask, static_cast<float*>(workspace), H, Tk,
-                                                q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, scale * 1.4426950408889634f, splits);
+  attn_decode_partial<false><<<grid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k),
+                                                       static_cast<const __nv_bfloat16*>(v), key_mask, static_cast<float*>(workspace), H, Tk,
+                                                       q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, scale * 1.4426950408889634f,
+                                                       splits, nullptr, 0);
   int rc = check_launch("attn_decode_partial");
   if (rc) return rc;
-  attn_decode_merge<<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits);
+  attn_decode_merge<false><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
+                                                      nullptr, H);
+  return check_launch("attn_decode_merge");
+}
+
+extern "C" int aria_attention_decode_devlen(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask,
+                                            int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t H, int32_t T_max,
+                                            int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h,
+                                            float scale, void* workspace, int64_t workspace_bytes, aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && k && v && out && lens && workspace && B > 0 && H > 0 && T_max > 0 && q_stride_b % 4 == 0 && q_stride_h % 4 == 0);
+  ARIA_CHECK_ARG(!key_mask || (key_mask_stride >= T_max && key_mask_stride < (1ll << 31)));
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(B, H, T_max));
+  const int splits = (T_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
+  dim3 grid(B * H, splits);
+  attn_decode_partial<true><<<grid, 128, 0, stream>>>(static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k),
+                                                      static_cast<const __nv_bfloat16*>(v), key_mask, static_cast<float*>(workspace), H,
+                                                      T_max, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h,
+                                                      scale * 1.4426950408889634f, splits, lens, static_cast<int>(key_mask_stride));
+  int rc = check_launch("attn_decode_partial");
+  if (rc) return rc;
+  attn_decode_merge<true><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
+                                                     lens, H);
   return check_launch("attn_decode_merge");
 }

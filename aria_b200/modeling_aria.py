@@ -226,11 +226,62 @@ class AriaForConditionalGeneration(nn.Module):
         return model_inputs
 
     @torch.no_grad()
-    def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None):
-        """Greedy decoding (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365):
-        prefill with the image, then one token per step against the KV cache (pixel inputs only at step 0).
-        attention_mask [B, T]: LEFT-padded batches of ragged prompts (the HF generation convention); positions are derived
-        from it as GenerationMixin does."""
+    def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None, *,
+                 do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
+                 pad_token_id=None, seed: int = 0, poll_every: int = 8):
+        """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
+
+        Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
+        captured decode step (GraphedDecode: embedding -> layers -> norm -> lm_head -> sample -> advance), all positions on the
+        device.  attention_mask [B, T]: LEFT-padded batches of ragged prompts (the HF generation convention); positions are
+        derived from it as GenerationMixin does.
+        do_sample=False: argmax (ties to the lowest id).  do_sample=True: transformers' TemperatureLogitsWarper ->
+        TopKLogitsWarper (top_k <= 1024, 0 = off) -> TopPLogitsWarper -> softmax -> multinomial, drawn with Philox noise keyed
+        by `seed` (reproducible; not torch's generator stream).  top_k = 0 with top_p < 1 is not supported.
+        eos_token_id: an id or up to 8 ids; a row that emits one is finished and emits pad_token_id (default: the first EOS
+        id) from then on, and generation stops once every row is finished, trimmed as GenerationMixin trims it.  The host
+        looks at the finished flag every `poll_every` tokens; the result does not depend on it.
+        Returns [B, T + generated] int64 on the model's device (prompt ids first)."""
+        B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
+                                                   top_p, eos_token_id, pad_token_id, seed, poll_every)
+        dev = self.device
+        if dev.type != "cuda":
+            if do_sample or eos:
+                raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
+            return self._generate_stepwise(input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask)
+        if do_sample:
+            sampling = (float(temperature), int(top_k), float(top_p), int(seed))
+        else:
+            sampling = (0.0, 0, 1.0, 0)
+        # rows are device-driven, so one captured step serves every prompt length of the same 256-row bucket
+        T_max = -(-(T + max_new_tokens) // 256) * 256
+        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev)
+        g = getattr(self, "_decode_graph", None)
+        if g is None or g.key != key:
+            self._decode_graph = g = None   # release the old graph and cache before building the new one
+            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad)
+        mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
+        inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
+                                                    attention_mask=mask, num_logits_to_keep=1)
+        g.cache.seq_len = 0
+        inputs["past_key_values"] = g.cache
+        out = self.forward(**inputs)
+        g.start(T, mask)
+        g.sample_and_advance(out.logits[:, -1])
+        n = 0                                   # decode steps replayed
+        while n < max_new_tokens - 1:
+            if eos and n % poll_every == 0 and g.done():
+                break
+            g.graph.replay()
+            n += 1
+        g.cache.seq_len = T + n
+        done = int(g.done_step.item())          # synchronises; -1 when no EOS stopped the batch
+        L = done + 1 if done >= 0 else max_new_tokens
+        return torch.cat([input_ids.to(dev), g.out_tokens[:, :L]], dim=1)
+
+    def _generate_stepwise(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask):
+        """Greedy decoding through the public step API, one forward(past_key_values=...) per token: what generate() does
+        on a device without CUDA graphs, i.e. the torch stand-ins of `ops` that the host-logic tests swap in."""
         B, T = input_ids.shape
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
@@ -244,9 +295,132 @@ class AriaForConditionalGeneration(nn.Module):
             if mask is not None:
                 mask = torch.cat([mask, torch.ones(B, 1, dtype=torch.long)], dim=1)
             inputs = self.prepare_inputs_for_generation(all_ids, cache, attention_mask=mask, num_logits_to_keep=1)
-            step = self.forward(**inputs)
-            tokens.append(step.logits[:, -1].float().argmax(-1))
+            tokens.append(self.forward(**inputs).logits[:, -1].float().argmax(-1))
         return torch.cat([input_ids.to(tokens[0].device), torch.stack(tokens, 1)], dim=1)
+
+    @staticmethod
+    def _check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k, top_p, eos_token_id,
+                             pad_token_id, seed, poll_every):
+        """All of generate()'s argument checks, on the host, before any device work -> (B, T, eos ids tuple, pad id)."""
+        import math
+        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
+            raise ValueError(f"input_ids must be [B, T] with B, T >= 1, got {tuple(input_ids.shape)}")
+        B, T = input_ids.shape
+        if B > 1024:
+            raise NotImplementedError("generate(): at most 1024 rows per batch")
+        if not isinstance(max_new_tokens, int) or max_new_tokens < 1:
+            raise ValueError(f"max_new_tokens must be a positive int, got {max_new_tokens!r}")
+        if attention_mask is not None and tuple(attention_mask.shape) != (B, T):
+            raise ValueError(f"attention_mask must be [B, T] = {(B, T)}, got {tuple(attention_mask.shape)}")
+        if not isinstance(poll_every, int) or poll_every < 1:
+            raise ValueError(f"poll_every must be a positive int, got {poll_every!r}")
+        if not isinstance(seed, int) or not 0 <= seed < 2 ** 64:
+            raise ValueError(f"seed must be an int in [0, 2**64), got {seed!r}")
+        if do_sample:
+            if not (isinstance(temperature, (int, float)) and math.isfinite(temperature) and temperature > 0):
+                raise ValueError(f"temperature must be a strictly positive float, got {temperature!r}")
+            if not isinstance(top_k, int) or top_k < 0:
+                raise ValueError(f"top_k must be a non-negative int, got {top_k!r}")
+            if top_k > 1024:
+                raise NotImplementedError("top_k > 1024 is not supported by the sampling kernel")
+            if not (isinstance(top_p, (int, float)) and 0 < top_p <= 1):
+                raise ValueError(f"top_p must be a float in (0, 1], got {top_p!r}")
+            if top_k == 0 and top_p < 1:
+                raise NotImplementedError("top-p without top-k (a full-vocabulary nucleus) is not supported")
+        eos = () if eos_token_id is None else (eos_token_id,) if isinstance(eos_token_id, int) else tuple(eos_token_id)
+        if len(eos) > 8 or not all(isinstance(e, int) for e in eos):
+            raise ValueError(f"eos_token_id must be an int or at most 8 ints, got {eos_token_id!r}")
+        if pad_token_id is None:
+            pad_token_id = eos[0] if eos else 0
+        if not isinstance(pad_token_id, int):
+            raise ValueError(f"pad_token_id must be an int, got {pad_token_id!r}")
+        return B, T, eos, pad_token_id
+
+
+class GraphedDecode:
+    """One decode step captured as a CUDA graph and replayed token after token (AriaForConditionalGeneration.generate).
+
+    The step is embedding -> every layer (AriaMoELMForCausalLM.decode_step) -> norm -> lm_head -> sample_tokens ->
+    decode_advance.  Nothing in it is a host integer: the step's input ids, RoPE positions, cache rows and key counts
+    (`state`), the RNG offset, the finished flags, the step index and the output tokens all live in static device buffers,
+    and decode_advance moves them on at the end of every replay.  The KV cache belongs to the graph: generate() prefills
+    into it with forward(past_key_values=g.cache), then calls start() and sample_and_advance() for the first token.
+    `logits` is the last replayed step's logits [B, 1, V]."""
+
+    def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad):
+        from .moe_lm import DecodeState
+        dev = model.device
+        lm = model.language_model
+        c = lm.config
+        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev)
+        self.model, self.B, self.T_max = model, B, T_max
+        self.sampling, self.eos, self.pad = sampling, eos, pad
+        self.cache = lm.new_cache(B, T_max, dev)
+        self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
+        self.rope = lm.model.rope_tables(T_max, dev)   # held here: the graph reads these tables
+        self.ids = torch.zeros(B, 1, dtype=torch.int64, device=dev)
+        self.next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.rng_offset = torch.zeros(1, dtype=torch.int64, device=dev)   # read as uint64 by the kernels
+        self.step = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.done_step = torch.full((1,), -1, dtype=torch.int32, device=dev)
+        self.finished = torch.zeros(B, dtype=torch.uint8, device=dev)
+        self.out_tokens = torch.zeros(B, max_new_tokens, dtype=torch.int64, device=dev)
+        self.done_host = torch.full((1,), -1, dtype=torch.int32).pin_memory()
+        self.event = torch.cuda.Event()
+        self.dev = dev
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):               # warm-up (its cache rows and state are reset by start())
+            self._step()
+        cur.wait_stream(side)
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.logits = self._step()
+
+    def _step(self):
+        lm = self.model.language_model
+        emb = ops.embedding(self.ids, lm.get_input_embeddings().weight)
+        logits = lm.decode_step(emb, self.cache, self.state, self.rope)
+        self.sample_and_advance(logits[:, -1])
+        return logits
+
+    def sample_and_advance(self, logits: torch.Tensor):
+        """Sample from logits [B, V] into next_ids, then advance the state (also the eager first token after the prefill)."""
+        t, k, p, seed = self.sampling
+        ops.sample_tokens(logits, t, k, p, seed, self.rng_offset, out=self.next_ids)
+        st = self.state
+        ops.decode_advance(self.next_ids, self.ids, self.out_tokens, self.step, st.rope_pos, st.write_pos, st.kv_len,
+                           self.rng_offset, self.finished, self.done_step, self.eos, self.pad)
+        self.done_host.copy_(self.done_step, non_blocking=True)
+
+    def start(self, T: int, mask: Optional[torch.Tensor]):
+        """Reset the state for a prompt of T tokens (mask: host [B, T] padding mask or None) already prefilled into
+        self.cache.  The values are those of the last prompt token: the advance after the first sample moves them on."""
+        B = self.B
+        if mask is None:
+            last = torch.full((B,), T - 1, dtype=torch.int32)
+        else:
+            last = (mask.sum(-1) - 1).to(torch.int32)
+        km = torch.zeros(B, self.T_max, dtype=torch.uint8)
+        if mask is not None:
+            km[:, :T] = (mask == 0).to(torch.uint8)
+        st = self.state
+        st.rope_pos.copy_(last)
+        st.write_pos.fill_(T - 1)
+        st.kv_len.fill_(T)
+        st.key_mask.copy_(km)
+        self.rng_offset.zero_()
+        self.step.zero_()
+        self.done_step.fill_(-1)
+        self.finished.zero_()
+        self.done_host.fill_(-1)
+
+    def done(self) -> bool:
+        """Whether every row has finished, from the pinned copy of done_step (waits for the work queued so far)."""
+        self.event.record(torch.cuda.current_stream(self.dev))
+        self.event.synchronize()
+        return int(self.done_host[0]) >= 0
 
 
 class GraphedPrefill:

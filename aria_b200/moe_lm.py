@@ -305,6 +305,21 @@ class KVCache:
         self.T_max = T_max
 
 
+class DecodeState:
+    """Device-resident positions of a decode step that is captured once and replayed token after token
+    (modeling_aria.GraphedDecode): nothing in the step reads `KVCache.seq_len` or any other host integer.
+    The step's token has RoPE position rope_pos[b], its k/v land in cache row write_pos[b], and it attends to cache rows
+    [0, kv_len[b]) minus the padded prompt keys of key_mask (1 = masked out).  aria_decode_advance moves all three on."""
+
+    def __init__(self, B, H, T_max, device):
+        i32 = dict(dtype=torch.int32, device=device)
+        self.rope_pos = torch.zeros(B, **i32)
+        self.write_pos = torch.zeros(B, **i32)
+        self.kv_len = torch.ones(B, **i32)
+        self.key_mask = torch.zeros(B, T_max, dtype=torch.uint8, device=device)
+        self.qkv = torch.empty(3, B, H, 1, 128, dtype=bf16, device=device)  # staging rows of the step's q, k, v
+
+
 class AriaAttention(nn.Module):
     """What `LLAMA_ATTENTION_CLASSES[config._attn_implementation]` provides at moe_lm.py:594: MHA, no bias,
     rotate-half RoPE, causal, KV cache.  q/k/v projections + RoPE + cache write are ONE GEMM launch."""
@@ -345,6 +360,21 @@ class AriaAttention(nn.Module):
             o = ops.attention(q[:, :, pos0:], kc, vc, T, Tk, scale, causal=True, key_mask=key_mask)
         return ops.linear(o, self.o_proj.weight, residual=residual)
 
+    def decode_step(self, hidden_states, cache: KVCache, rope, state: DecodeState, residual=None):
+        """One token per row with every position on the device (graph-replayable): the fused projection writes q, k, v
+        to the state's staging rows (RoPE at state.rope_pos), kv_append moves k, v into the cache at state.write_pos, and
+        the decode attention reads state.kv_len keys.  Same kernels and arithmetic as forward() at T = 1."""
+        B, T, d = hidden_states.shape
+        H, hd = self.num_heads, self.head_dim
+        kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
+        q, k, v = state.qkv[0], state.qkv[1], state.qkv[2]
+        cos, sin = rope
+        ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3, [q, k, v], hd, 1,
+                      pos0=0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=state.rope_pos)
+        ops.kv_append(k[:, :, 0], v[:, :, 0], kc, vc, state.write_pos)
+        o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
+        return ops.linear(o, self.o_proj.weight, residual=residual)
+
 
 class MoEDecoderLayer(nn.Module):
     """moe_lm.py:580-602: x + attn(rms(x)); h + moe(rms(h)).  The MoE residual add is deferred into the next
@@ -365,6 +395,16 @@ class MoEDecoderLayer(nn.Module):
         else:
             h, x = self.input_layernorm(x, residual=pending)
         x = self.self_attn(h, cache, rope, residual=x, key_mask=key_mask, position_ids=position_ids)
+        h = self.post_attention_layernorm(x)
+        return x, self.mlp(h)
+
+    def decode_step(self, x, pending, cache, rope, state: DecodeState):
+        """forward() for one token per row, positions from `state` (AriaAttention.decode_step)."""
+        if pending is None:
+            h = self.input_layernorm(x)
+        else:
+            h, x = self.input_layernorm(x, residual=pending)
+        x = self.self_attn.decode_step(h, cache, rope, state, residual=x)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
@@ -399,6 +439,14 @@ class AriaMoELMModel(nn.Module):
             x, pending = layer(x, pending, cache, rope, key_mask, position_ids)
         cache.seq_len += T
         return x, pending  # final residual add happens inside the final norm
+
+    def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
+        """One token per row through every layer with the positions of `state`; `cache.seq_len` is neither read nor
+        written (the caller owns it).  `rope`: the tables of rope_tables(cache.T_max), computed outside any graph capture."""
+        x, pending = inputs_embeds, None
+        for layer in self.layers:
+            x, pending = layer.decode_step(x, pending, cache, rope, state)
+        return x, pending
 
 
 class AriaMoELMForCausalLM(nn.Module):
@@ -445,3 +493,9 @@ class AriaMoELMForCausalLM(nn.Module):
             pending = pending[:, -num_logits_to_keep:, :].contiguous()
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h), cache
+
+    def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
+        """inputs_embeds [B, 1, d] -> logits [B, 1, V] for one decode step driven by device positions (graph-replayable)."""
+        x, pending = self.model.decode_step(inputs_embeds, cache, state, rope)
+        h, _ = self.model.norm(x, residual=pending)
+        return self.lm_head(h)

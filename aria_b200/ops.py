@@ -624,3 +624,93 @@ def attention_decode(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tk: int,
         L.check(lib.aria_attention_decode(_p(q), _p(k), _p(v), _p(out), _p(key_mask), B, H, Tk, q.stride(0), q.stride(1), k.stride(0),
                                           k.stride(1), scale, _p(ws), ws_bytes, _stream(q)), "attention_decode")
     return out
+
+
+def attention_decode_devlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, lens: torch.Tensor, scale: float,
+                            key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """attention_decode with the key count of each row on the device: row b sees cache rows [0, lens[b]) (lens int32 [B]).
+    Cache k/v [B,H,T_max,128]; key_mask [B, >=T_max] uint8 (1 = masked out; any row stride).  Row b is bit-identical to
+    attention_decode(..., Tk=lens[b]); nothing reads the host value of lens, so one captured launch serves every step."""
+    _chk(k), _chk(v), _chk(lens, torch.int32, align=4)
+    if not (q.is_cuda and q.dtype == bf16 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
+        raise RuntimeError("attention_decode_devlen: q must be a CUDA bf16 tensor with a contiguous last dim")
+    B, H, T_max = q.shape[0], q.shape[1], k.shape[2]
+    assert lens.shape == (B,) and k.shape[:2] == (B, H)
+    lib = L.load()
+    ws_bytes = lib.aria_attention_decode_workspace_bytes(B, H, T_max)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    out = torch.empty((B, H * 128), dtype=bf16, device=q.device)
+    mask_stride = 0
+    if key_mask is not None:
+        if not (key_mask.is_cuda and key_mask.dtype == torch.uint8 and key_mask.stride(-1) == 1 and key_mask.shape[0] == B
+                and key_mask.shape[1] >= T_max):
+            raise RuntimeError("attention_decode_devlen: key_mask must be CUDA uint8 [B, >= T_max] with contiguous rows")
+        mask_stride = key_mask.stride(0)
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_decode_devlen(_p(q), _p(k), _p(v), _p(out), _p(key_mask), mask_stride, _p(lens), B, H, T_max,
+                                                 q.stride(0), q.stride(1), k.stride(0), k.stride(1), scale, _p(ws), ws_bytes,
+                                                 _stream(q)), "attention_decode_devlen")
+    return out
+
+
+# ------------------------------------------------------------------------------------------- generation
+def sample_tokens(logits: torch.Tensor, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
+                  rng_offset: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
+                  probs_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Next token per row of bf16 logits [B, V] (contiguous last dim, any row stride, 0 repeats one row): transformers'
+    temperature -> top-k -> top-p -> softmax -> multinomial on an fp32 copy; temperature 0 = greedy argmax (lowest id on ties).
+    rng_offset: device int64 [1] read as the uint64 Philox offset (None: 0).  out: int64 [B] (allocated when None).
+    probs_out: fp32 [B, V], receives the final distribution (zero outside the kept set).  See aria_sample_tokens."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(-1) == 1):
+        raise RuntimeError("sample_tokens: logits must be CUDA bf16 [B, V] with a contiguous last dim")
+    B, V = logits.shape
+    if out is None:
+        out = torch.empty((B,), dtype=torch.int64, device=logits.device)
+    _chk(out, torch.int64, align=8)
+    assert out.shape == (B,)
+    if rng_offset is not None:
+        _chk(rng_offset, torch.int64, align=8)
+    if probs_out is not None:
+        _chk(probs_out, torch.float32, align=4)
+        assert probs_out.shape == (B, V)
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_sample_tokens(_p(logits), logits.stride(0), _p(out), _p(probs_out), B, V, float(temperature),
+                                            int(top_k), float(top_p), int(seed) & (2 ** 64 - 1), _p(rng_offset), _stream(logits)),
+                "sample_tokens")
+    return out
+
+
+def kv_append(k_new: torch.Tensor, v_new: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos: torch.Tensor):
+    """k_cache[b, :, pos[b]] = k_new[b], v_cache[b, :, pos[b]] = v_new[b]; k_new / v_new [B, H, 128] (any strides with 128
+    contiguous elements), caches [B, H, T_max, 128], pos int32 [B] on the device."""
+    _chk(k_cache), _chk(v_cache), _chk(pos, torch.int32, align=4)
+    for t in (k_new, v_new):
+        if not (t.is_cuda and t.dtype == bf16 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0):
+            raise RuntimeError("kv_append: new rows must be CUDA bf16 with a contiguous, 16-byte aligned last dim")
+    assert k_new.stride() == v_new.stride() and k_cache.stride() == v_cache.stride()
+    B, H, T_max = k_cache.shape[0], k_cache.shape[1], k_cache.shape[2]
+    assert k_new.shape == (B, H, 128) and v_new.shape == (B, H, 128) and pos.shape == (B,)
+    with torch.cuda.device(k_cache.device):
+        L.check(L.load().aria_kv_append(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_cache), _p(v_cache),
+                                        k_cache.stride(0), k_cache.stride(1), _p(pos), B, H, T_max, _stream(k_cache)), "kv_append")
+
+
+def decode_advance(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: torch.Tensor, step: torch.Tensor,
+                   rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor, rng_offset: torch.Tensor,
+                   finished: torch.Tensor, done_step: torch.Tensor, eos_token_ids: Sequence[int] = (), pad_token_id: int = 0):
+    """One launch after sample_tokens: out_tokens[:, step] <- next_ids (pad for finished rows), ids_in <- the same tokens,
+    EOS bookkeeping (finished, done_step), positions / step / rng offset + 1.  Every argument is a device tensor; the EOS ids
+    (at most 8) and the pad id are baked into the launch.  See aria_decode_advance."""
+    B = next_ids.numel()
+    for t, dt in ((next_ids, torch.int64), (ids_in, torch.int64), (out_tokens, torch.int64), (step, torch.int32),
+                  (rope_pos, torch.int32), (write_pos, torch.int32), (kv_len, torch.int32), (rng_offset, torch.int64),
+                  (finished, torch.uint8), (done_step, torch.int32)):
+        _chk(t, dt, align=1)
+    assert ids_in.numel() == B and out_tokens.shape[0] == B and finished.numel() == B and rope_pos.numel() == B
+    eos = list(eos_token_ids)
+    arr = (C.c_int64 * max(1, len(eos)))(*eos)
+    with torch.cuda.device(next_ids.device):
+        L.check(L.load().aria_decode_advance(_p(next_ids), _p(ids_in), _p(out_tokens), out_tokens.shape[1], _p(step), _p(rope_pos),
+                                             _p(write_pos), _p(kv_len), _p(rng_offset), _p(finished), _p(done_step),
+                                             C.cast(arr, C.c_void_p), len(eos), int(pad_token_id), B, _stream(next_ids)),
+                "decode_advance")

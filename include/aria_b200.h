@@ -280,6 +280,47 @@ int aria_attention_decode(const void* q, const void* k, const void* v, void* out
                           int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
                           void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 int64_t aria_attention_decode_workspace_bytes(int32_t B, int32_t H, int32_t Tk);
+/* aria_attention_decode with the key count of each row in DEVICE memory (one captured decode step replayed token after token):
+ * row b attends to cache rows [0, min(lens[b], T_max)), lens = int32 [B].  key_mask [B, T_max] uint8 at row stride
+ * key_mask_stride (>= T_max) or NULL.  The grid covers T_max; the result of row b is bit-identical to aria_attention_decode's
+ * with Tk = lens[b].  Rows at or past lens[b] are never read.  workspace: aria_attention_decode_workspace_bytes(B, H, T_max). */
+int aria_attention_decode_devlen(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask,
+                                 int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t H, int32_t T_max,
+                                 int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
+                                 void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * Generation: sampling, KV append, decode-state advance (one decode step has no host integer in it)
+ * ------------------------------------------------------------------------------------------------ */
+/* Next token of each row from bf16 logits [B, V] (row r at logits + r * logits_stride elements; stride 0 repeats one row),
+ * following transformers' warper chain on an fp32 copy: TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper ->
+ * softmax -> multinomial, written to next_ids [B] int64.
+ *   temperature == 0: greedy, argmax with ties to the lowest id (torch.argmax); top_k / top_p are then not applied.
+ *   top_k in [1, 1024] keeps every logit >= the k-th largest (ties kept); 0 = off.  top_p in (0, 1]: HF's rule over the top-k
+ *   survivors (ascending cumulative probability <= 1 - top_p removed, the largest always kept; boundary ties removed lowest id
+ *   first).  top_k == 0 with top_p < 1 (a full-vocabulary nucleus) returns ARIA_ERR_UNSUPPORTED.
+ *   Sampling is Gumbel-max with Philox4x32-10 noise keyed by `seed`, counter (vocabulary index, row, *rng_offset): the same
+ *   seed and offset give the same tokens; it is NOT torch's generator stream.  rng_offset: device uint64, or NULL for 0.
+ *   probs_out [B, V] fp32 or NULL: the final normalised distribution (zero outside the kept set; one-hot when greedy).
+ * B <= 2^20, V <= 2^24.  One CTA of 1024 threads per row. */
+int aria_sample_tokens(const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out, int32_t B, int32_t V,
+                       float temperature, int32_t top_k, float top_p, uint64_t seed, const uint64_t* rng_offset,
+                       aria_stream_t stream);
+/* Copy the new k and v rows k_new / v_new [B, H, 128] (element strides new_stride_b / new_stride_h) into the caches
+ * [B, H, T_max, 128] (strides cache_stride_b / cache_stride_h) at the device row pos[b] (int32 [B]); a row outside
+ * [0, T_max) is not written.  Strides must be multiples of 8 elements. */
+int aria_kv_append(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_cache, void* v_cache,
+                   int64_t cache_stride_b, int64_t cache_stride_h, const int32_t* pos, int32_t B, int32_t H, int32_t T_max,
+                   aria_stream_t stream);
+/* Decode-state advance after aria_sample_tokens, one launch (B <= 1024), all state in device memory:
+ *   t = *step; tok[b] = finished[b] ? pad_token_id : next_ids[b]; out_tokens[b * max_steps + t] = tok[b] (if t < max_steps);
+ *   ids_in[b] = tok[b]; finished[b] |= tok[b] is one of eos_ids (HOST array of n_eos <= 8 ids, copied at the call);
+ *   ++rope_pos[b], ++write_pos[b], ++kv_len[b]; *step = t + 1; *rng_offset += 1;
+ *   and when n_eos > 0, every row is finished and *done_step < 0: *done_step = t (GenerationMixin stops after that token). */
+int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int64_t* out_tokens, int32_t max_steps, int32_t* step,
+                        int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len, uint64_t* rng_offset, uint8_t* finished,
+                        int32_t* done_step, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t B,
+                        aria_stream_t stream);
 
 #ifdef __cplusplus
 }
