@@ -44,15 +44,16 @@ inline PFN_encodeTiled get_encode_fn() {
 }
 
 // bf16 tensor map, 128B swizzle (or the given one), zero OOB fill.  dims/strides innermost-first; strides[i] is the byte stride
-// of dim i+1 (rank-1 entries).
+// of dim i+1 (rank-1 entries).  `dtype`: UINT8 for the e4m3 expert weights (fp8 grouped GEMM).
 inline int make_tmap_bf16_swz(CUtensorMap* tm, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                              const uint32_t* box, CUtensorMapSwizzle swizzle);
+                              const uint32_t* box, CUtensorMapSwizzle swizzle,
+                              CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 inline int make_tmap_bf16(CUtensorMap* tm, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                           const uint32_t* box) {
   return make_tmap_bf16_swz(tm, ptr, rank, dims, strides_bytes, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 inline int make_tmap_bf16_swz(CUtensorMap* tm, const void* ptr, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
-                              const uint32_t* box, CUtensorMapSwizzle swizzle) {
+                              const uint32_t* box, CUtensorMapSwizzle swizzle, CUtensorMapDataType dtype) {
   PFN_encodeTiled enc = get_encode_fn();
   if (!enc) {
     fprintf(stderr, "aria_b200: cuTensorMapEncodeTiled unavailable\n");
@@ -77,12 +78,12 @@ inline int make_tmap_bf16_swz(CUtensorMap* tm, const void* ptr, int rank, const 
     cudaFree(0);
     ctx_bound = true;
   }
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
+  CUresult r = enc(tm, dtype, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r == CUDA_ERROR_INVALID_CONTEXT || r == CUDA_ERROR_NOT_INITIALIZED) {  // e.g. the context was popped by another library
     cudaFree(0);
-    r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
+    r = enc(tm, dtype, rank, const_cast<void*>(ptr), gdim, gstr, bx, es,
             CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   }
@@ -101,6 +102,15 @@ inline int make_tmap_2d(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64
   uint64_t str[1] = {row_stride_bytes};
   uint32_t box[2] = {box_inner, box_outer};
   return make_tmap_bf16(tm, ptr, 2, dims, str, box);
+}
+
+// byte tensor map without swizzle (e4m3 weights as UINT8; 16-byte rows of the box land contiguously)
+inline int make_tmap_2d_u8(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
+                           uint32_t box_inner, uint32_t box_outer) {
+  uint64_t dims[2] = {inner, outer};
+  uint64_t str[1] = {row_stride_bytes};
+  uint32_t box[2] = {box_inner, box_outer};
+  return make_tmap_bf16_swz(tm, ptr, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_DATA_TYPE_UINT8);
 }
 
 // Per-device state: one process may drive several GPUs (the reference's device_map="auto", aria/inference.py:55-57), and

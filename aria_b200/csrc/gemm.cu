@@ -1,4 +1,6 @@
 // Persistent wgmma GEMM (M=128 x N=BN tiles, two consumer warpgroups of 64 rows each).  See gemm_common.cuh for the design.
+#include <cuda_fp8.h>
+
 #include "gemm_common.cuh"
 
 namespace aria {
@@ -6,9 +8,34 @@ namespace aria {
 // four k-blocks in flight: the ring takes what the fp32 staging tile of the epilogue leaves of the 227 KB per block
 constexpr int GEMM_STAGES = 4;
 constexpr int acc_ld(int BN) { return BN + 4; }  // staging row stride (floats): 16-byte aligned rows, spread over the banks
-template <int BN>
+// fp8 B (B_FP8): TMA lands the e4m3 boxes in a ring of their own, the producer warpgroup's three idle warps widen them to bf16
+// in the SW128 layout of the bf16 ring, and the wgmma sequence is unchanged.  Three landing slots fit beside the four bf16
+// stages and the fp32 staging tile (DESIGN §3); a fourth would not.
+constexpr int FP8_LAND_STAGES = 3;
+constexpr int FP8_CONVERT_WARPS = 3;
+template <int BN, bool B_FP8 = false>
 constexpr int gemm_smem_bytes() {
-  return 1024 /*align*/ + GEMM_STAGES * (A_STAGE_BYTES + BN * BK * 2) + BM * acc_ld(BN) * 4 + 256 /*barriers*/;
+  return 1024 /*align*/ + GEMM_STAGES * (A_STAGE_BYTES + BN * BK * 2) + BM * acc_ld(BN) * 4 + 256 /*barriers*/ +
+         (B_FP8 ? FP8_LAND_STAGES * BN * BK : 0);
+}
+static_assert(gemm_smem_bytes<128, true>() <= 232448, "fp8 landing ring must fit the opt-in shared memory of a block");
+
+// 16 e4m3 values (one 16-byte landing chunk, columns in address order) -> 16 bf16 in two 16-byte chunks; every e4m3 value,
+// subnormals and -0 included, is exact in fp16, fp32 and bf16
+ARIA_DEVICE void e4m3x16_to_bf16(const uint4 v, uint4& lo, uint4& hi) {
+  const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t o[8];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w[i] >> (16 * h)), __NV_E4M3);
+      const float2 f = __half22float2(__half2(hr));
+      o[2 * i + h] = pack_bf16(f.x, f.y);
+    }
+  }
+  lo = make_uint4(o[0], o[1], o[2], o[3]);
+  hi = make_uint4(o[4], o[5], o[6], o[7]);
 }
 
 template <int BN, bool B_MN>
@@ -17,7 +44,7 @@ ARIA_DEVICE void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) 
   else wgmma_m64n144_ss<0, B_MN ? 1 : 0>(acc, da, db, 1u);
 }
 
-template <int BN, bool B_MN, int EPI>
+template <int BN, bool B_MN, int EPI, bool B_FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
             const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
@@ -27,12 +54,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   constexpr int ACC_LD = acc_ld(BN);
   constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
   static_assert(BN == 128 || BN == 144, "tile widths with a wgmma wrapper");
+  static_assert(!B_FP8 || (B_MN && BN == 128 && EPI != ARIA_EPI_HEADS), "fp8 B: grouped [G, K, N] weights, 128-wide tiles");
+  constexpr int LAND_BYTES = BN * BK;  // one k-block of fp8 B: BN/64 boxes of 64 k-rows x 64 bytes, unswizzled
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [BM][ACC_LD] fp32 accumulator staging
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + BM * ACC_LD);
   uint64_t* empty_bar = full_bar + STAGES;
+  // B_FP8: e4m3 landing ring after the barrier block; land_full completes on the TMA bytes, land_empty once per converter warp
+  uint64_t* land_full = empty_bar + STAGES;
+  uint64_t* land_empty = land_full + FP8_LAND_STAGES;
+  uint8_t* land = reinterpret_cast<uint8_t*>(stg + BM * ACC_LD) + 256;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -44,8 +77,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(&tmB1);
     if (p.n_seg > 2) prefetch_tmap(&tmB2);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
+      // B_FP8: a stage is full once A has landed AND every converter warp has written its share of B
+      mbar_init(&full_bar[i], B_FP8 ? 1 + FP8_CONVERT_WARPS : 1);
       mbar_init(&empty_bar[i], CONSUMER_WARPS);
+    }
+    if constexpr (B_FP8) {
+      for (int i = 0; i < FP8_LAND_STAGES; ++i) {
+        mbar_init(&land_full[i], 1);
+        mbar_init(&land_empty[i], FP8_CONVERT_WARPS);
+      }
     }
     fence_mbar_init();
   }
@@ -64,6 +104,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       TileSched sched;
       sched.init(p, n_tiles);
       uint32_t stage = 0, phase = 0;
+      uint32_t lstage = 0, lphase = 0;  // B_FP8 landing ring
       for (int t = blockIdx.x;; t += gridDim.x) {
         int grp, m_idx, n_idx, row0, rows;
         if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
@@ -88,9 +129,32 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           const uint32_t sa = smem_base + stage * STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
           mbar_wait_addr(empty0 + stage * 8, phase ^ 1);
-          mbar_arrive_expect_tx_addr(fb, STAGE_BYTES);
+          mbar_arrive_expect_tx_addr(fb, B_FP8 ? A_STAGE_BYTES : STAGE_BYTES);
           tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
-          if constexpr (B_MN) {
+          if constexpr (B_FP8) {
+            // the e4m3 boxes go to the landing ring; the converters widen them into this stage's B slot.  That slot is free:
+            // the converters see this k-block only after the empty-barrier wait above.
+            const uint32_t lf = smem_u32(land_full) + lstage * 8;
+            mbar_wait_addr(smem_u32(land_empty) + lstage * 8, lphase ^ 1);
+            mbar_arrive_expect_tx_addr(lf, LAND_BYTES);
+            const int krow = b_c0 + kb * BK;
+            constexpr int CH = BN / 64;
+#pragma unroll
+            for (int c = 0; c < CH; ++c) {
+              int ncol;
+              if constexpr (EPI == ARIA_EPI_SWIGLU) {
+                constexpr int HALF = CH / 2;
+                ncol = (c < HALF) ? (n_idx * OUT_BN + c * 64) : (p.N + n_idx * OUT_BN + (c - HALF) * 64);
+              } else {
+                ncol = n_idx * BN + c * 64;
+              }
+              tma_load_2d_addr(smem_u32(land) + lstage * LAND_BYTES + c * (64 * BK), &tmB0, lf, ncol, krow);
+            }
+            if (++lstage == FP8_LAND_STAGES) {
+              lstage = 0;
+              lphase ^= 1;
+            }
+          } else if constexpr (B_MN) {
             // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n (8 KB), BN/64 boxes per stage
             const int krow = b_c0 + kb * BK;
             constexpr int CH = BN / 64;
@@ -114,6 +178,50 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1;
+          }
+        }
+      }
+    } else if constexpr (B_FP8) {
+      if (warp > 0) {
+        // ============ converters (warps 1-3): e4m3 landing slot -> bf16 B slot of the same k-block, SW128 MN-major ============
+        // Chunk i of a landing slot is 16 fp8 columns: box i / 256, k-row (i / 4) % 64, columns 16 (i % 4) +[0, 16).  Widened,
+        // they are the 16-byte chunks 2 (i % 4) and 2 (i % 4) + 1 of that 128-byte bf16 row, stored at chunk j ^ (row % 8)
+        // as TMA's 128-byte swizzle would have placed them.
+        const int ct = threadIdx.x - 32;
+        TileSched sched;
+        sched.init(p, n_tiles);
+        uint32_t stage = 0, phase = 0, lstage = 0, lphase = 0;
+        for (int t = blockIdx.x;; t += gridDim.x) {
+          int grp, m_idx, n_idx, row0, rows;
+          if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+          for (int kb = 0; kb < k_blocks; ++kb) {
+            mbar_wait_addr(smem_u32(land_full) + lstage * 8, lphase);
+            const uint8_t* src = land + lstage * LAND_BYTES;
+            uint8_t* dst = smem + stage * STAGE_BYTES + A_STAGE_BYTES;
+#pragma unroll 1
+            for (int i = ct; i < LAND_BYTES / 16; i += FP8_CONVERT_WARPS * 32) {
+              const uint4 v = *reinterpret_cast<const uint4*>(src + i * 16);
+              uint4 lo, hi;
+              e4m3x16_to_bf16(v, lo, hi);
+              const int r = (i >> 2) & 63, j = 2 * (i & 3);
+              uint8_t* row = dst + (i >> 8) * (64 * BK * 2) + r * 128;
+              *reinterpret_cast<uint4*>(row + ((j ^ (r & 7)) << 4)) = lo;
+              *reinterpret_cast<uint4*>(row + (((j + 1) ^ (r & 7)) << 4)) = hi;
+            }
+            fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads
+            __syncwarp();
+            if (lane == 0) {
+              mbar_arrive(&full_bar[stage]);
+              mbar_arrive(&land_empty[lstage]);
+            }
+            if (++stage == STAGES) {
+              stage = 0;
+              phase ^= 1;
+            }
+            if (++lstage == FP8_LAND_STAGES) {
+              lstage = 0;
+              lphase ^= 1;
+            }
           }
         }
       }
@@ -142,6 +250,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      // B_FP8: the scales of this thread's accumulator columns (8 j + frag_col, +1), fetched while the k-loop runs
+      float2 bsc[BN / 8];
+      if constexpr (B_FP8) {
+        const int ncols = EPI == ARIA_EPI_SWIGLU ? 2 * p.N : p.N;
+        const float* srow = p.b_scale + static_cast<int64_t>(weight_block(p, grp)) * ncols;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          int col;
+          if constexpr (EPI == ARIA_EPI_SWIGLU)  // gate columns [0, OUT_BN) of the tile, then the up columns
+            col = (8 * j < OUT_BN) ? n_idx * OUT_BN + 8 * j + frag_col : p.N + n_idx * OUT_BN + 8 * j - OUT_BN + frag_col;
+          else
+            col = n_idx * BN + 8 * j + frag_col;
+          bsc[j] = col < ncols ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
+        }
+      }
       // one k-block's wgmma group stays in flight while the next one is issued; a stage is released once its group retired
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
@@ -168,8 +291,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         float* d0 = stg + frag_row * ACC_LD + 8 * j + frag_col;
-        *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        if constexpr (B_FP8) {  // per-column weight scale on the fp32 accumulator, before any rounding of the epilogue
+          *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j] * bsc[j].x, acc[4 * j + 1] * bsc[j].y);
+          *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) = make_float2(acc[4 * j + 2] * bsc[j].x, acc[4 * j + 3] * bsc[j].y);
+        } else {
+          *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
       }
       named_bar_sync(1 + cw, 128);
       const int r_in_grp = m_idx * BM + epi_row;
@@ -180,11 +308,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
-template <int BN, bool B_MN, int EPI>
+template <int BN, bool B_MN, int EPI, bool B_FP8 = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap* tmB, const GemmParams& p, int max_tiles,
                        cudaStream_t stream) {
-  constexpr int SMEM = gemm_smem_bytes<BN>();
-  auto kern = gemm_kernel<BN, B_MN, EPI>;
+  constexpr int SMEM = gemm_smem_bytes<BN, B_FP8>();
+  auto kern = gemm_kernel<BN, B_MN, EPI, B_FP8>;
   static bool attr_set[kMaxDevices] = {};
   if (ensure_dynamic_smem(attr_set, kern, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
   int grid = sm_count();
@@ -198,8 +326,8 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap* tmB, const Gem
 
 using namespace aria;
 
-extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
-  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+// aria_gemm, and aria_grouped_gemm_fp8 with b_scale != NULL (then d->b[0] is e4m3 and the GKN layout is the only one)
+static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_t stream) {
   ARIA_CHECK_ARG(d != nullptr);
   ARIA_CHECK_ARG(d->a && d->b[0] && d->out[0]);
   ARIA_CHECK_ARG(d->m >= 0 && d->n > 0 && d->k > 0);
@@ -258,6 +386,7 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
   p.rope_cos = static_cast<const __nv_bfloat16*>(d->rope_cos);
   p.rope_sin = static_cast<const __nv_bfloat16*>(d->rope_sin);
   p.position_ids = d->position_ids;
+  p.b_scale = b_scale;
 
   // ---- tile shape selection: 128-wide tiles; the 72-dim ViT heads (n = 1152 = 8 x 144) take 144-wide tiles of whole heads
   const int64_t n_out_total = d->n * (swiglu ? 1 : d->n_seg);
@@ -283,7 +412,8 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
   if (b_mn) {
     const uint64_t ncols = swiglu ? 2 * d->n : d->n;
     const uint64_t n_weights = d->group_mod > 0 ? d->group_mod : (d->group_mod < 0 ? d->num_groups / (-d->group_mod) : d->num_groups);
-    rc = make_tmap_2d(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols * 2, 64, BK);
+    rc = b_scale ? make_tmap_2d_u8(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols, 64, BK)
+                 : make_tmap_2d(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols * 2, 64, BK);
     if (rc) return rc;
     tmB[1] = tmB[0];
     tmB[2] = tmB[0];
@@ -305,7 +435,11 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
   int64_t max_tiles = n_tiles * m_tiles_ub;
   if (max_tiles > (1 << 30)) max_tiles = 1 << 30;
 
-#define ARIA_LAUNCH(BN_, MN_, EPI_) return launch_gemm<BN_, MN_, EPI_>(tmA, tmB, p, static_cast<int>(max_tiles), stream)
+#define ARIA_LAUNCH(BN_, MN_, EPI_, ...) return launch_gemm<BN_, MN_, EPI_, ##__VA_ARGS__>(tmA, tmB, p, static_cast<int>(max_tiles), stream)
+  if (b_scale) {
+    if (swiglu) ARIA_LAUNCH(128, true, ARIA_EPI_SWIGLU, true);
+    ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR, true);
+  }
   if (d->epilogue == ARIA_EPI_HEADS) {
     if (BN == 128) ARIA_LAUNCH(128, false, ARIA_EPI_HEADS);
     ARIA_LAUNCH(144, false, ARIA_EPI_HEADS);
@@ -317,6 +451,10 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream_) {
   if (b_mn) ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR);
   ARIA_LAUNCH(128, false, ARIA_EPI_LINEAR);
 #undef ARIA_LAUNCH
+}
+
+extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream) {
+  return gemm_run(d, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int aria_grouped_gemm(const void* a, const void* b, void* out, const int32_t* group_offsets, int64_t rows,
@@ -336,6 +474,31 @@ extern "C" int aria_grouped_gemm(const void* a, const void* b, void* out, const 
   d.out[0] = out;
   d.ldo = n;
   return aria_gemm(&d, stream);
+}
+
+extern "C" int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const float* b_scale, void* out,
+                                     const int32_t* group_offsets, int64_t rows, int64_t k, int64_t n, int32_t num_groups,
+                                     int32_t epilogue, aria_stream_t stream) {
+  ARIA_CHECK_ARG(a && b_fp8 && b_scale && out && group_offsets);
+  ARIA_CHECK_ARG(rows >= 0 && k > 0 && n > 0 && k % BK == 0 && n % 64 == 0 && num_groups >= 1);
+  ARIA_CHECK_ARG(epilogue == ARIA_EPI_LINEAR || epilogue == ARIA_EPI_SWIGLU);
+  ARIA_CHECK_ARG((reinterpret_cast<uintptr_t>(a) & 15) == 0 && (reinterpret_cast<uintptr_t>(b_fp8) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(b_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0);
+  aria_gemm_desc_t d{};
+  d.a = a;
+  d.lda = k;
+  d.m = rows;
+  d.n = n;
+  d.k = k;
+  d.b[0] = b_fp8;
+  d.n_seg = 1;
+  d.b_layout = ARIA_B_GKN;
+  d.num_groups = num_groups;
+  d.group_offsets = group_offsets;
+  d.epilogue = epilogue;
+  d.out[0] = out;
+  d.ldo = n;
+  return gemm_run(&d, b_scale, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int aria_abi_version(void) { return 3; }

@@ -47,6 +47,7 @@ struct GemmParams {
   const __nv_bfloat16* rope_cos;
   const __nv_bfloat16* rope_sin;
   const int32_t* position_ids;
+  const float* b_scale;  // fp8 B (gemm_kernel<.., B_FP8 = true>): [G, B columns] fp32 scale of each weight column
 };
 
 ARIA_DEVICE int weight_block(const GemmParams& p, int grp) {

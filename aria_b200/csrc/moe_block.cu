@@ -62,17 +62,12 @@ cudaEvent_t* branch_events() {
   return ev[dev];
 }
 
-}  // namespace
-
-extern "C" int64_t aria_moe_block_fwd_workspace_bytes(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared) {
-  if (T <= 0 || d <= 0 || E <= 0 || k <= 0 || I <= 0 || I_shared < 0) return ARIA_ERR_BAD_ARG;
-  return carve(T, d, E, k, I, I_shared).total;
-}
-
-extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const void* gate_w,
-                                  const void* up_w, const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k,
-                                  int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
-                                  int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
+// The whole block.  fc1_scale / fc2_scale NULL: bf16 expert weights; given: fc1_w / fc2_w are e4m3 with per-(expert, column)
+// fp32 scales and the two expert GEMMs are aria_grouped_gemm_fp8.  Every other launch is the same.
+int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
+                  const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T, int32_t d,
+                  int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
+                  int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
   if (!x || !w_router || !fc1_w || !fc2_w || !out || !workspace) return ARIA_ERR_BAD_ARG;
   if (T <= 0 || d <= 0 || E <= 0 || E > 64 || k <= 0 || k > 8 || k > E || I <= 0 || I_shared < 0) return ARIA_ERR_BAD_ARG;
   if (I_shared > 0 && (!gate_w || !up_w || !down_w)) return ARIA_ERR_BAD_ARG;
@@ -130,7 +125,11 @@ extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const voi
   }
   if ((rc = aria_build_permutation(idx, counts, offsets, dest, src, T, E, k, 1, stream))) return rc;
   if ((rc = aria_permute_rows(x, src, at(ws.permuted), R, d, stream))) return rc;
-  {
+  if (fc1_scale) {
+    if ((rc = aria_grouped_gemm_fp8(at(ws.permuted), fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, stream)))
+      return rc;
+    if ((rc = aria_grouped_gemm_fp8(at(ws.h), fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, stream))) return rc;
+  } else {
     aria_gemm_desc_t g;
     memset(&g, 0, sizeof(g));
     g.a = at(ws.permuted); g.lda = d; g.m = R; g.n = I; g.k = d;
@@ -157,4 +156,34 @@ extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const voi
     shared = at(ws.shared);
   }
   return aria_unpermute_combine(at(ws.y), dest, at(ws.scores), shared, out, T, d, k, stream);
+}
+
+}  // namespace
+
+extern "C" int64_t aria_moe_block_fwd_workspace_bytes(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared) {
+  if (T <= 0 || d <= 0 || E <= 0 || k <= 0 || I <= 0 || I_shared < 0) return ARIA_ERR_BAD_ARG;
+  return carve(T, d, E, k, I, I_shared).total;
+}
+
+extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const void* gate_w,
+                                  const void* up_w, const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k,
+                                  int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
+                                  int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
+  return moe_block_run(x, w_router, fc1_w, fc2_w, nullptr, nullptr, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
+                       forced_top_idx, workspace, workspace_bytes, stream, side_stream);
+}
+
+extern "C" int aria_moe_block_fwd_fp8(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w,
+                                      const float* fc1_scale, const float* fc2_scale, const void* gate_w, const void* up_w,
+                                      const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
+                                      int32_t I_shared, const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes,
+                                      aria_stream_t stream, aria_stream_t side_stream) {
+  // the expert GEMMs' constraints are checked here too, so that nothing is launched for a block that would fail half-way
+  if (!fc1_scale || !fc2_scale) return ARIA_ERR_BAD_ARG;
+  if (d <= 0 || I <= 0 || d % 64 != 0 || I % 64 != 0) return ARIA_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(fc1_w) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_w) & 15) != 0 ||
+      (reinterpret_cast<uintptr_t>(fc1_scale) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_scale) & 15) != 0)
+    return ARIA_ERR_BAD_ARG;
+  return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
+                       forced_top_idx, workspace, workspace_bytes, stream, side_stream);
 }

@@ -238,6 +238,9 @@ def install(model, reference_moe_lm_module=None, trainable: bool = False) -> int
     trainable=False: the inference seams (they refuse autograd).  trainable=True: the MoE layers run `_moe_train_forward`
     (differentiable, router losses in train() mode; inference unchanged) and `experts_gemm` becomes the differentiable
     `moe_train.experts_gemm_train`."""
+    if trainable and any(type(mod) is _m.Fp8GroupedGEMM for mod in model.modules()):
+        raise NotImplementedError("aria_b200.install(trainable=True): fp8 expert weights are inference-only; install the "
+                                  "trainable seam on the bf16 model")
     fwd = _moe_train_forward if trainable else _moe_forward
     n = 0
     for mod in model.modules():

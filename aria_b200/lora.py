@@ -27,7 +27,7 @@ import torch
 from torch import nn
 
 from . import ops
-from .moe_lm import GroupedGEMM, _as_offsets
+from .moe_lm import Fp8GroupedGEMM, GroupedGEMM, _as_offsets
 
 R_PAD = 128
 
@@ -118,6 +118,9 @@ def inject_lora(model: nn.Module, target_modules, r: int = 8, lora_alpha: int = 
     Returns the names wrapped.  Other module types in the list are left alone (their LoRA is peft's stock Linear path)."""
     wanted, done = set(target_modules), []
     for name, mod in list(model.named_modules()):
+        if name in wanted and type(mod) is Fp8GroupedGEMM:
+            raise NotImplementedError(f"LoRA on fp8 expert weights ({name}) is not supported: inject the adapters into the "
+                                      "bf16 model")
         if name in wanted and type(mod) is GroupedGEMM:
             parent = model.get_submodule(name.rsplit(".", 1)[0]) if "." in name else model
             setattr(parent, name.rsplit(".", 1)[-1], GroupedGemmLoraLayer(mod, adapter_name, r=r, lora_alpha=lora_alpha))
@@ -132,6 +135,8 @@ class GroupedGemmLoraLayer(nn.Module):
     def __init__(self, base_layer: GroupedGEMM, adapter_name: str = "default", r: int = 8, lora_alpha: int = 32,
                  lora_dropout: float = 0.0):
         super().__init__()
+        if type(base_layer) is Fp8GroupedGEMM:
+            raise NotImplementedError("LoRA on fp8 expert weights is not supported: wrap the bf16 GroupedGEMM")
         if r <= 0:
             raise ValueError(f"`r` should be a positive integer value but the value passed is {r}")   # layers.py:74-77
         if r > R_PAD or r % 8:

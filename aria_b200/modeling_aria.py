@@ -98,6 +98,9 @@ class AriaForConditionalGeneration(nn.Module):
         GEMM epilogue).  Every rank must then call forward() in lock-step with its own tokens."""
         import torch.distributed as dist
         from .expert_parallel import ExpertParallelMoE, FusedPeerTransport
+        if any(layer.mlp.experts.is_fp8() for layer in self.language_model.model.layers):
+            raise NotImplementedError("enable_expert_parallel: the experts are quantized to fp8; expert parallelism runs on "
+                                      "bf16 expert weights")
         t = self.config.text_config
         W, r = dist.get_world_size(group), dist.get_rank(group)
         tr = FusedPeerTransport(max_tokens, t.hidden_size, t.moe_intermediate_size, t.moe_num_experts, t.moe_topk, self.device, group)
@@ -112,6 +115,40 @@ class AriaForConditionalGeneration(nn.Module):
             m.expert_parallel = ExpertParallelMoE(w, t.moe_num_experts, t.moe_topk, group=group, transport=tr)
         self._ep_transport = tr
         return tr
+
+    @torch.no_grad()
+    def quantize_experts_fp8(self):
+        """Quantize every MoE layer's routed experts (`experts.fc1` / `experts.fc2`) to weight-only fp8 in place: e4m3 weights
+        with one fp32 scale per (expert, output column), Fp8GroupedGEMM.  It halves the bytes of the routed experts, which are
+        most of the model and most of what a decode step reads.  Layer by layer, so the peak is the bf16 model plus one
+        layer's fp8 copy; the bf16 expert tensors are freed.  Attention, shared experts, router, lm_head and the ViT stay bf16.
+        A second call changes nothing.  Returns the model.
+        Raises ValueError for non-finite expert weights and NotImplementedError under expert parallelism, both before
+        anything changes.  The captured decode graph of generate() is dropped (it holds the bf16 weight pointers); a
+        GraphedPrefill built before the call must be rebuilt."""
+        from .moe_lm import Fp8GroupedGEMM, GroupedGEMM
+        mlps = [layer.mlp for layer in self.language_model.model.layers]
+        if any(m.expert_parallel is not None for m in mlps):
+            raise NotImplementedError("quantize_experts_fp8: expert parallelism is enabled; it runs on bf16 expert weights")
+        todo = []
+        for i, m in enumerate(mlps):
+            if m.experts.is_fp8():
+                continue
+            for name in ("fc1", "fc2"):
+                fc = getattr(m.experts, name)
+                if type(fc) is not GroupedGEMM:
+                    raise NotImplementedError(f"quantize_experts_fp8: layer {i} experts.{name} is a {type(fc).__name__} "
+                                              "(e.g. LoRA-wrapped), not a plain GroupedGEMM")
+                if not bool(torch.isfinite(fc.weight).all()):
+                    raise ValueError(f"quantize_experts_fp8: layer {i} experts.{name}.weight has non-finite values")
+            todo.append(m.experts)
+        if not todo:
+            return self
+        self._decode_graph = None
+        for experts in todo:
+            for name in ("fc1", "fc2"):
+                setattr(experts, name, Fp8GroupedGEMM.from_grouped_gemm(getattr(experts, name)))   # drops the bf16 module
+        return self
 
     @property
     def device(self):

@@ -179,6 +179,47 @@ class GroupedGEMM(nn.Module):
         return experts_gemm(input, self.weight, tokens_per_expert)
 
 
+def _reject_fp8_grad(x: torch.Tensor):
+    """The fp8 expert weights are an inference format: there is no backward through them."""
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise RuntimeError("aria_b200: fp8 expert weights are inference-only, but the input requires grad; run under "
+                           "torch.no_grad(), or train on the bf16 model")
+
+
+class Fp8GroupedGEMM(nn.Module):
+    """GroupedGEMM with weight-only fp8 expert weights (AriaForConditionalGeneration.quantize_experts_fp8): `weight`
+    [groups, in_features, out_features] torch.float8_e4m3fn and `weight_scale` [groups, out_features] fp32, one scale per
+    (expert, output column).  Activations stay bf16; the kernel widens the weights to bf16 in shared memory and applies the
+    scale to the fp32 accumulator.  Both are frozen parameters, so a quantized model saves and reloads through its state
+    dict (`...fc1.weight`, `...fc1.weight_scale`)."""
+
+    def __init__(self, in_features, out_features, groups, device=None, weight=None, weight_scale=None):
+        super().__init__()
+        self.in_features = in_features
+        self.out_features = out_features
+        self.groups = groups
+        if weight is None:
+            weight = torch.empty(groups, in_features, out_features, dtype=torch.float8_e4m3fn, device=device)
+        if weight_scale is None:
+            weight_scale = torch.empty(groups, out_features, dtype=torch.float32, device=device)
+        if weight.shape != (groups, in_features, out_features) or weight.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"weight must be [{groups}, {in_features}, {out_features}] float8_e4m3fn")
+        if weight_scale.shape != (groups, out_features) or weight_scale.dtype != torch.float32:
+            raise ValueError(f"weight_scale must be [{groups}, {out_features}] float32")
+        self.weight = nn.Parameter(weight, requires_grad=False)
+        self.weight_scale = nn.Parameter(weight_scale, requires_grad=False)
+
+    @classmethod
+    def from_grouped_gemm(cls, m: "GroupedGEMM") -> "Fp8GroupedGEMM":
+        q, scale = ops.quantize_fp8_cols(m.weight.detach())
+        return cls(m.in_features, m.out_features, m.groups, weight=q, weight_scale=scale)
+
+    def forward(self, input, tokens_per_expert):
+        _reject_fp8_grad(input)
+        return ops.grouped_gemm_fp8(input, self.weight, self.weight_scale,
+                                    _as_offsets(tokens_per_expert, self.groups, input.device))
+
+
 class GroupedMLP(nn.Module):
     """moe_lm.py:487-525: fc1 -> glu (first half gate, second half up) -> fc2.  The glu is fused into fc1's
     epilogue with the reference's bf16 rounding points."""
@@ -189,8 +230,19 @@ class GroupedMLP(nn.Module):
         self.fc1 = GroupedGEMM(config.hidden_size, config.moe_intermediate_size * 2, config.moe_num_experts, device)
         self.fc2 = GroupedGEMM(config.moe_intermediate_size, config.hidden_size, config.moe_num_experts, device)
 
+    def is_fp8(self) -> bool:
+        """Whether fc1 / fc2 hold fp8 weights (Fp8GroupedGEMM); one quantized without the other is an error."""
+        f1, f2 = type(self.fc1) is Fp8GroupedGEMM, type(self.fc2) is Fp8GroupedGEMM
+        if f1 != f2:
+            raise RuntimeError("GroupedMLP: fc1 and fc2 must both be fp8 (Fp8GroupedGEMM) or both not")
+        return f1
+
     def forward(self, permuted_tokens, tokens_per_expert):
         off = _as_offsets(tokens_per_expert, self.fc1.groups, permuted_tokens.device)
+        if self.is_fp8():
+            _reject_fp8_grad(permuted_tokens)
+            h = ops.grouped_gemm_fp8(permuted_tokens, self.fc1.weight, self.fc1.weight_scale, off, swiglu=True)
+            return ops.grouped_gemm_fp8(h, self.fc2.weight, self.fc2.weight_scale, off)
         if type(self.fc1) is GroupedGEMM and type(self.fc2) is GroupedGEMM:
             h = ops.grouped_gemm(permuted_tokens, self.fc1.weight, off, swiglu=True)
             return ops.grouped_gemm(h, self.fc2.weight, off)
@@ -274,14 +326,19 @@ class MoELayer(nn.Module):
     def forward(self, hidden_states: torch.Tensor) -> torch.Tensor:
         if self.expert_parallel is not None:
             return self.expert_parallel(hidden_states)
-        if (hidden_states.is_cuda and type(self.experts.fc1) is GroupedGEMM and type(self.experts.fc2) is GroupedGEMM
+        fp8 = self.experts.is_fp8()
+        if fp8:
+            _reject_fp8_grad(hidden_states)
+        if (hidden_states.is_cuda and (fp8 or (type(self.experts.fc1) is GroupedGEMM and type(self.experts.fc2) is GroupedGEMM))
                 and os.environ.get("ARIA_MOE_BLOCK", "1") != "0"):   # =0: one C-ABI call per kernel (bench.py's per-kernel table)
             # the whole block behind one C-ABI call (csrc/moe_block.cu); shared experts on the side stream of this device
             x = hidden_states.reshape(-1, hidden_states.shape[-1])
             se = self.shared_experts
-            out = ops.moe_block_fwd(x, self.router.weight, self.experts.fc1.weight, self.experts.fc2.weight, se.gate_proj.weight,
+            fc1, fc2 = self.experts.fc1, self.experts.fc2
+            out = ops.moe_block_fwd(x, self.router.weight, fc1.weight, fc2.weight, se.gate_proj.weight,
                                     se.up_proj.weight, se.down_proj.weight, self.router.config.moe_topk,
-                                    forced_top_idx=self.router.forced_top_indices, side_stream=_side_stream(x.device))
+                                    forced_top_idx=self.router.forced_top_indices, side_stream=_side_stream(x.device),
+                                    fc1_scale=fc1.weight_scale if fp8 else None, fc2_scale=fc2.weight_scale if fp8 else None)
             return out.view(hidden_states.shape)
         # module-by-module path (adapter-wrapped experts, CPU stand-in ops of the host-logic tests)
         forked = shared_expert_overlapped(lambda: self.shared_experts(hidden_states), hidden_states)

@@ -132,6 +132,40 @@ def grouped_gemm(a: torch.Tensor, b: torch.Tensor, offsets: torch.Tensor, swiglu
     return out
 
 
+def quantize_fp8_cols(w: torch.Tensor):
+    """Per-(expert, output column) e4m3 quantisation of GroupedGEMM weights w [E, K, N] bf16 -> (q [E, K, N]
+    torch.float8_e4m3fn, scale [E, N] fp32): scale = amax over K / 448 (an all-zero column gets 1), q = e4m3(w / scale),
+    bit for bit `(w.float() / scale).to(torch.float8_e4m3fn)`."""
+    _chk(w)
+    if w.dim() != 3:
+        raise ValueError(f"expected [E, K, N] expert weights, got {tuple(w.shape)}")
+    E, K, N = w.shape
+    q = torch.empty((E, K, N), dtype=torch.float8_e4m3fn, device=w.device)
+    scale = torch.empty((E, N), dtype=torch.float32, device=w.device)
+    with torch.cuda.device(w.device):
+        L.check(L.load().aria_quantize_fp8_cols(_p(w), _p(q), _p(scale), E, K, N, _stream(w)), "quantize_fp8_cols")
+    return q, scale
+
+
+def grouped_gemm_fp8(a: torch.Tensor, q: torch.Tensor, scale: torch.Tensor, offsets: torch.Tensor,
+                     swiglu: bool = False) -> torch.Tensor:
+    """grouped_gemm with e4m3 weights q [E, K, N_b] (float8_e4m3fn) and per-column scales scale [E, N_b] fp32: the fp32
+    accumulator of column c of expert e is multiplied by scale[e, c] before the epilogue rounds it.  swiglu=True: N_b = 2I
+    (gate then up, each column with its own scale), out [rows, I]."""
+    _chk(a), _chk(q, torch.float8_e4m3fn), _chk(scale, torch.float32), _chk(offsets, torch.int32)
+    rows, K = a.shape
+    E, Kb, Nb = q.shape
+    if Kb != K or scale.shape != (E, Nb) or offsets.numel() != E + 1:
+        raise ValueError(f"grouped_gemm_fp8: a {tuple(a.shape)}, q {tuple(q.shape)}, scale {tuple(scale.shape)}, "
+                         f"offsets {offsets.numel()} do not fit together")
+    N = Nb // 2 if swiglu else Nb
+    out = torch.empty((rows, N), dtype=bf16, device=a.device)
+    with torch.cuda.device(a.device):
+        L.check(L.load().aria_grouped_gemm_fp8(_p(a), _p(q), _p(scale), _p(out), _p(offsets), rows, K, N, E,
+                                               L.EPI_SWIGLU if swiglu else L.EPI_LINEAR, _stream(a)), "grouped_gemm_fp8")
+    return out
+
+
 def grouped_gemm_regions(a_buf: torch.Tensor, b: torch.Tensor, starts: torch.Tensor, counts: torch.Tensor, rows_hint: int,
                          swiglu: bool = False, group_mod: int = 0, out: Optional[torch.Tensor] = None,
                          out_group_base: Optional[torch.Tensor] = None, out_group_row0: Optional[torch.Tensor] = None,
@@ -430,12 +464,22 @@ def unpermute_combine(y: torch.Tensor, dest_row: torch.Tensor, scores: torch.Ten
 
 def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, fc2_w: torch.Tensor, gate_w: Optional[torch.Tensor],
                   up_w: Optional[torch.Tensor], down_w: Optional[torch.Tensor], k: int,
-                  forced_top_idx: Optional[torch.Tensor] = None, side_stream: Optional[torch.cuda.Stream] = None) -> torch.Tensor:
-    """MoELayer.forward (moe_lm.py:548-577) as one C-ABI call (`aria_moe_block_fwd`): x [T, d] -> [T, d]."""
-    _chk(x), _chk(w_router), _chk(fc1_w), _chk(fc2_w)
+                  forced_top_idx: Optional[torch.Tensor] = None, side_stream: Optional[torch.cuda.Stream] = None,
+                  fc1_scale: Optional[torch.Tensor] = None, fc2_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """MoELayer.forward (moe_lm.py:548-577) as one C-ABI call (`aria_moe_block_fwd`): x [T, d] -> [T, d].
+    With fc1_scale [E, 2I] / fc2_scale [E, d] fp32, fc1_w / fc2_w are e4m3 (quantize_fp8_cols) and the call is
+    `aria_moe_block_fwd_fp8`."""
+    fp8 = fc1_scale is not None or fc2_scale is not None
+    if fp8 and (fc1_scale is None or fc2_scale is None):
+        raise ValueError("moe_block_fwd: give both fc1_scale and fc2_scale, or neither")
+    wdt = torch.float8_e4m3fn if fp8 else bf16
+    _chk(x), _chk(w_router), _chk(fc1_w, wdt), _chk(fc2_w, wdt)
     T, d = x.shape
     E, I = fc2_w.shape[0], fc2_w.shape[1]
     assert w_router.shape == (E, d) and fc1_w.shape == (E, d, 2 * I) and fc2_w.shape == (E, I, d)
+    if fp8:
+        _chk(fc1_scale, torch.float32), _chk(fc2_scale, torch.float32)
+        assert fc1_scale.shape == (E, 2 * I) and fc2_scale.shape == (E, d)
     Is = 0
     if gate_w is not None:
         _chk(gate_w), _chk(up_w), _chk(down_w)
@@ -448,10 +492,15 @@ def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, 
     nbytes = lib.aria_moe_block_fwd_workspace_bytes(T, d, E, k, I, Is)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     out = torch.empty((T, d), dtype=bf16, device=x.device)
+    side = C.c_void_p(side_stream.cuda_stream) if side_stream is not None else None
     with torch.cuda.device(x.device):
-        L.check(lib.aria_moe_block_fwd(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(gate_w), _p(up_w), _p(down_w), _p(out), T, d, E, k,
-                                       I, Is, _p(forced_top_idx), _p(ws), nbytes, _stream(x),
-                                       C.c_void_p(side_stream.cuda_stream) if side_stream is not None else None), "moe_block_fwd")
+        if fp8:
+            L.check(lib.aria_moe_block_fwd_fp8(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(fc1_scale), _p(fc2_scale), _p(gate_w),
+                                               _p(up_w), _p(down_w), _p(out), T, d, E, k, I, Is, _p(forced_top_idx), _p(ws), nbytes,
+                                               _stream(x), side), "moe_block_fwd_fp8")
+        else:
+            L.check(lib.aria_moe_block_fwd(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(gate_w), _p(up_w), _p(down_w), _p(out), T, d,
+                                           E, k, I, Is, _p(forced_top_idx), _p(ws), nbytes, _stream(x), side), "moe_block_fwd")
     return out
 
 

@@ -101,6 +101,21 @@ int aria_gemm(const aria_gemm_desc_t* desc, aria_stream_t stream);
 int aria_grouped_gemm(const void* a, const void* b, void* out, const int32_t* group_offsets, int64_t rows,
                       int64_t k, int64_t n, int32_t num_groups, aria_stream_t stream);
 
+/* FP8 expert weights (weight-only, e4m3 with one fp32 scale per (expert, output column); activations stay bf16).
+ *
+ * aria_quantize_fp8_cols: w [G, K, N] bf16 (GroupedGEMM.weight layout) ->
+ *   scale [G, N] fp32 = max_k |w[g,k,n]| / 448 (IEEE division; an all-zero column gets 1),
+ *   q [G, K, N] e4m3 = w / scale, round to nearest even, saturating — bit for bit (w.float() / scale).to(float8_e4m3fn).
+ *   K % 64 == 0, N % 64 == 0; w, q, scale 16-byte aligned.
+ *
+ * aria_grouped_gemm_fp8: aria_grouped_gemm with e4m3 weights b_fp8 [G, k, N_b] and scales b_scale [G, N_b]:
+ *   epilogue ARIA_EPI_LINEAR (N_b = n) or ARIA_EPI_SWIGLU (N_b = 2n, gate then up, out [rows, n]).  The result is aria_gemm's
+ *   with ARIA_B_GKN weights q.to(bf16), except that the fp32 accumulator of column c of group g is multiplied by
+ *   b_scale[g, c] before the epilogue's first bf16 rounding; every rounding point is the same.  k % 64 == 0, n % 64 == 0. */
+int aria_quantize_fp8_cols(const void* w, void* q, float* scale, int32_t G, int64_t K, int64_t N, aria_stream_t stream);
+int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const float* b_scale, void* out, const int32_t* group_offsets,
+                          int64_t rows, int64_t k, int64_t n, int32_t num_groups, int32_t epilogue, aria_stream_t stream);
+
 /* Weight gradient of a (grouped) linear layer — backward of gmm / F.linear:
  *   out[g, m, n] = sum_{r in group g} a[r, m] * b[r, n]   a [rows, md] (row stride lda), b [rows, nd] (ldb), out [G, md, nd] bf16.
  * group_offsets: device int32 row offsets, non-decreasing, any values (densely packed groups as the reference's dispatcher
@@ -165,6 +180,12 @@ int aria_moe_block_fwd(const void* x, const void* w_router, const void* fc1_w, c
                        const void* up_w, const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
                        int32_t I_shared, const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes,
                        aria_stream_t stream, aria_stream_t side_stream);
+/* The same block with e4m3 expert weights: fc1_w [E, d, 2I] / fc2_w [E, I, d] from aria_quantize_fp8_cols, with their scales
+ * fc1_scale [E, 2I] / fc2_scale [E, d]; the expert GEMMs are aria_grouped_gemm_fp8.  d % 64 == 0, I % 64 == 0.  Same workspace. */
+int aria_moe_block_fwd_fp8(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
+                           const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
+                           int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx,
+                           void* workspace, int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream);
 
 /* ---- backward of the MoE block (BASELINE cfg 5; autograd through moe_lm.py:548-577) ---- */
 /* h = bf16(bf16(silu(g)) * u) with g = h1[:, :I], u = h1[:, I:]  (unfused `glu`, moe_lm.py:505-507; training keeps h1). */
