@@ -54,10 +54,13 @@ SIGNATURES = {
     "aria_build_permutation": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, i32, vp]),
     "aria_quantize_fp8_cols": (i32, [vp, vp, vp, i32, i64, i64, vp]),
     "aria_grouped_gemm_fp8": (i32, [vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]),
+    "aria_permute_quantize_fp8_rows": (i32, [vp, vp, vp, vp, i64, i32, vp]),
+    "aria_grouped_gemm_w8a8": (i32, [vp, vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]),
     "aria_grouped_wgrad": (i32, [vp, i64, vp, i64, vp, vp, i64, i64, i64, i32, i32, vp]),
     "aria_moe_block_fwd_workspace_bytes": (i64, [i64, i32, i32, i32, i32, i32]),
     "aria_moe_block_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
     "aria_moe_block_fwd_fp8": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
+    "aria_moe_block_fwd_w8a8": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
     "aria_swiglu_fwd": (i32, [vp, vp, i64, i32, vp]),
     "aria_swiglu_bwd": (i32, [vp, vp, vp, i64, i32, vp]),
     "aria_combine_bwd": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, i32, vp]),
@@ -116,7 +119,7 @@ def load():
 
 # kernels launched per C-ABI call (for bench.py's `gpu_launches`; memsets are not counted)
 KERNELS_PER_CALL = {"router_topk": 2, "attention_decode": 2, "attention_decode_devlen": 2, "attention_bwd": 3, "moe_block_fwd": 9, "moe_block_fwd_fp8": 9,
-                    "quantize_fp8_cols": 2}
+                    "moe_block_fwd_w8a8": 10, "quantize_fp8_cols": 2}
 launch_count = 0
 
 

@@ -308,6 +308,160 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 }
 
+// W8A8 grouped GEMM: e4m3 A [rows, K] with one fp32 scale per row, e4m3 B [G * N_b, K] (K-major: fp8 wgmma has no transpose)
+// with one per (group, column).  The pipeline, tile scheduler and epilogues are gemm_kernel's; a k-block is 128 fp8 elements,
+// one 128-byte SW128 row, so the A and B stages keep their 16 KB and the K-major descriptors are the bf16 ones.  The tensor
+// core's fp8 accumulation keeps ~14 bits, so each k-block is accumulated on its own (`part`) and promoted into the fp32
+// accumulator before the next one starts; the other consumer warpgroup keeps the tensor cores busy during that wait.
+constexpr int W8_BK = 128;
+static_assert(BM * W8_BK == A_STAGE_BYTES, "W8A8 A stage = bf16 A stage");
+
+template <int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
+                 const float* __restrict__ a_scale) {
+  constexpr int BN = 128;
+  constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * W8_BK;
+  constexpr int STAGES = GEMM_STAGES;
+  constexpr int ACC_LD = acc_ld(BN);
+  constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;
+  static_assert(EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_SWIGLU, "W8A8: expert GEMM epilogues");
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + BM * ACC_LD);
+  uint64_t* empty_bar = full_bar + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], CONSUMER_WARPS);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int n_tiles = (p.N + OUT_BN - 1) / OUT_BN;
+  const int k_blocks = p.K / W8_BK;
+  const uint32_t smem_base = smem_u32(smem);
+  const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+
+  if (wg == 0) {
+    // =========================== TMA producer ===========================
+    setmaxnreg_dec<40>();
+    if (warp == 0 && elect_one()) {
+      TileSched sched;
+      sched.init(p, n_tiles);
+      uint32_t stage = 0, phase = 0;
+      for (int t = blockIdx.x;; t += gridDim.x) {
+        int grp, m_idx, n_idx, row0, rows;
+        if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+        const int a_row = row0 + m_idx * BM;
+        // B rows of the two 64-row boxes: (group, column c) is row group * N_b + c; SwiGLU takes the gate and the up box
+        int b_r0, b_r1;
+        if constexpr (EPI == ARIA_EPI_SWIGLU) {
+          b_r0 = weight_block(p, grp) * 2 * p.N + n_idx * OUT_BN;
+          b_r1 = b_r0 + p.N;
+        } else {
+          b_r0 = weight_block(p, grp) * p.N + n_idx * BN;
+          b_r1 = b_r0 + 64;
+        }
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          const uint32_t fb = full0 + stage * 8;
+          const uint32_t sa = smem_base + stage * STAGE_BYTES;
+          const uint32_t sb = sa + A_STAGE_BYTES;
+          mbar_wait_addr(empty0 + stage * 8, phase ^ 1);
+          mbar_arrive_expect_tx_addr(fb, STAGE_BYTES);
+          tma_load_2d_addr(sa, &tmA, fb, kb * W8_BK, a_row);
+          tma_load_2d_addr(sb, &tmB, fb, kb * W8_BK, b_r0);
+          tma_load_2d_addr(sb + 64 * W8_BK, &tmB, fb, kb * W8_BK, b_r1);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+  } else {
+    // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    const int tid = threadIdx.x & 127;
+    const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
+    const uint64_t db0 = make_smem_desc(smem_base + A_STAGE_BYTES, 16, 1024);
+    const int frag_row = cw * 64 + (tid >> 5) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
+    const int epi_row = cw * 64 + (tid & 63), half = tid >> 6;
+    TileSched sched;
+    sched.init(p, n_tiles);
+    uint32_t stage = 0, phase = 0;
+    float part[BN / 2];  // one k-block's tensor-core sum (the first wgmma of a k-block overwrites it)
+    for (int t = blockIdx.x;; t += gridDim.x) {
+      int grp, m_idx, n_idx, row0, rows;
+      if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      // column scales of this thread's accumulator columns (8 j + frag_col, +1) and row scales of its two fragment rows (rows
+      // past the group's end are computed but never stored; the index is clamped to the buffer)
+      float2 bsc[BN / 8];
+      {
+        const int ncols = EPI == ARIA_EPI_SWIGLU ? 2 * p.N : p.N;
+        const float* srow = p.b_scale + static_cast<int64_t>(weight_block(p, grp)) * ncols;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          int col;
+          if constexpr (EPI == ARIA_EPI_SWIGLU)
+            col = (8 * j < OUT_BN) ? n_idx * OUT_BN + 8 * j + frag_col : p.N + n_idx * OUT_BN + 8 * j - OUT_BN + frag_col;
+          else
+            col = n_idx * BN + 8 * j + frag_col;
+          bsc[j] = col < ncols ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
+        }
+      }
+      const int ar = row0 + m_idx * BM + frag_row;
+      const float as0 = __ldg(a_scale + min(ar, p.M - 1)), as1 = __ldg(a_scale + min(ar + 8, p.M - 1));
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait_addr(full0 + stage * 8, phase);
+        const uint64_t da = da0 + stage * (STAGE_BYTES >> 4);
+        const uint64_t db = db0 + stage * (STAGE_BYTES >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < W8_BK / 32; ++k) wgmma_m64n128k32_e4m3_ss(part, da + k * 2, db + k * 2, k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(part);
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+
+      named_bar_sync(1 + cw, 128);  // the previous tile's epilogue has finished reading this warpgroup's staging rows
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {  // both scales on the fp32 accumulator, before any rounding of the epilogue
+        float* d0 = stg + frag_row * ACC_LD + 8 * j + frag_col;
+        *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j] * as0 * bsc[j].x, acc[4 * j + 1] * as0 * bsc[j].y);
+        *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) =
+            make_float2(acc[4 * j + 2] * as1 * bsc[j].x, acc[4 * j + 3] * as1 * bsc[j].y);
+      }
+      named_bar_sync(1 + cw, 128);
+      const int r_in_grp = m_idx * BM + epi_row;
+      const bool row_ok = r_in_grp < rows;
+      const int64_t grow = static_cast<int64_t>(row0) + r_in_grp;
+      epilogue_tile<BN, EPI>(p, stg + epi_row * ACC_LD, p.N, n_idx, grow, row_ok, half, grp, r_in_grp);
+    }
+  }
+}
+
 template <int BN, bool B_MN, int EPI, bool B_FP8 = false>
 static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap* tmB, const GemmParams& p, int max_tiles,
                        cudaStream_t stream) {
@@ -499,6 +653,59 @@ extern "C" int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const flo
   d.out[0] = out;
   d.ldo = n;
   return gemm_run(&d, b_scale, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, const void* b_fp8_nk, const float* b_scale,
+                                      void* out, const int32_t* group_offsets, int64_t rows, int64_t k, int64_t n,
+                                      int32_t num_groups, int32_t epilogue, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(a_fp8 && a_scale && b_fp8_nk && b_scale && out && group_offsets);
+  ARIA_CHECK_ARG(rows >= 0 && rows < (int64_t(1) << 31) && k > 0 && n > 0 && k % W8_BK == 0 && n % 64 == 0 && num_groups >= 1);
+  ARIA_CHECK_ARG(k <= (1 << 30) && n <= (1 << 29) && static_cast<int64_t>(num_groups) * n * 2 < (int64_t(1) << 31));
+  ARIA_CHECK_ARG(epilogue == ARIA_EPI_LINEAR || epilogue == ARIA_EPI_SWIGLU);
+  ARIA_CHECK_ARG((reinterpret_cast<uintptr_t>(a_fp8) & 15) == 0 && (reinterpret_cast<uintptr_t>(b_fp8_nk) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(b_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(a_scale) & 3) == 0);
+  if (rows == 0) return ARIA_OK;
+  const bool swiglu = epilogue == ARIA_EPI_SWIGLU;
+  GemmParams p{};
+  p.M = static_cast<int>(rows);
+  p.N = static_cast<int>(n);
+  p.K = static_cast<int>(k);
+  p.num_groups = num_groups;
+  p.group_offsets = group_offsets;
+  p.n_seg = 1;
+  p.out[0] = static_cast<__nv_bfloat16*>(out);
+  p.ldo = n;
+  p.rows_per_batch = p.M;
+  p.b_scale = b_scale;
+
+  // UINT8 maps, 128-byte swizzle: a box row is one 128-element k-block
+  CUtensorMap tmA, tmB;
+  const uint64_t a_dims[2] = {static_cast<uint64_t>(k), static_cast<uint64_t>(rows)}, b_rows = static_cast<uint64_t>(num_groups) * (swiglu ? 2 * n : n);
+  const uint64_t b_dims[2] = {static_cast<uint64_t>(k), b_rows}, stride[1] = {static_cast<uint64_t>(k)};
+  const uint32_t a_box[2] = {W8_BK, BM}, b_box[2] = {W8_BK, 64};
+  int rc = make_tmap_bf16_swz(&tmA, a_fp8, 2, a_dims, stride, a_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  if (rc) return rc;
+  rc = make_tmap_bf16_swz(&tmB, b_fp8_nk, 2, b_dims, stride, b_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  if (rc) return rc;
+
+  const int64_t n_tiles = (n + (swiglu ? 63 : 127)) / (swiglu ? 64 : 128);
+  int64_t max_tiles = n_tiles * ((rows + BM - 1) / BM + num_groups);
+  if (max_tiles > (1 << 30)) max_tiles = 1 << 30;
+  int grid = sm_count();
+  if (max_tiles < grid) grid = static_cast<int>(max_tiles);
+  constexpr int SMEM = gemm_smem_bytes<128>();
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (swiglu) {
+    static bool attr_set[kMaxDevices] = {};
+    if (ensure_dynamic_smem(attr_set, gemm_w8a8_kernel<ARIA_EPI_SWIGLU>, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
+    gemm_w8a8_kernel<ARIA_EPI_SWIGLU><<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB, p, a_scale);
+  } else {
+    static bool attr_set[kMaxDevices] = {};
+    if (ensure_dynamic_smem(attr_set, gemm_w8a8_kernel<ARIA_EPI_LINEAR>, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
+    gemm_w8a8_kernel<ARIA_EPI_LINEAR><<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB, p, a_scale);
+  }
+  return check_launch("gemm_w8a8_kernel");
 }
 
 extern "C" int aria_abi_version(void) { return 3; }

@@ -62,11 +62,28 @@ cudaEvent_t* branch_events() {
   return ev[dev];
 }
 
+// W8A8 keeps the workspace of the other modes: the e4m3 rows and scales of fc1's input go to the `permuted` region (R d 2
+// bytes), those of h to the same region once fc1 has consumed the first ones (R I bytes, hence I <= 2 d), and h's row
+// scales to the `src` region, dead after the gather (R 4 bytes: at I = 2 d the rows of h fill `permuted`).
+struct W8a8Ws {
+  int64_t xq, xs, hq, hs;
+};
+inline int64_t al16(int64_t n) { return (n + 15) / 16 * 16; }
+bool w8a8_fits(int64_t R, int32_t d, int32_t I, const BlockWs& ws, W8a8Ws& o) {
+  o.xq = ws.permuted;
+  o.xs = ws.permuted + al16(R * d);
+  o.hq = ws.permuted;
+  o.hs = ws.src;
+  const int64_t permuted_bytes = ws.h - ws.permuted, src_bytes = ws.logits - ws.src;
+  return al16(R * d) + R * 4 <= permuted_bytes && R * I <= permuted_bytes && R * 4 <= src_bytes;
+}
+
 // The whole block.  fc1_scale / fc2_scale NULL: bf16 expert weights; given: fc1_w / fc2_w are e4m3 with per-(expert, column)
-// fp32 scales and the two expert GEMMs are aria_grouped_gemm_fp8.  Every other launch is the same.
+// fp32 scales and the two expert GEMMs are aria_grouped_gemm_fp8, or with w8a8 aria_grouped_gemm_w8a8 on K-major weights
+// ([E, 2I, d] / [E, d, I]) and row-quantised activations.  Every other launch is the same.
 int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
-                  const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T, int32_t d,
-                  int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
+                  const float* fc2_scale, bool w8a8, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
+                  int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
                   int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
   if (!x || !w_router || !fc1_w || !fc2_w || !out || !workspace) return ARIA_ERR_BAD_ARG;
   if (T <= 0 || d <= 0 || E <= 0 || E > 64 || k <= 0 || k > 8 || k > E || I <= 0 || I_shared < 0) return ARIA_ERR_BAD_ARG;
@@ -74,6 +91,8 @@ int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const 
   if ((reinterpret_cast<uintptr_t>(workspace) & 15) != 0) return ARIA_ERR_BAD_ARG;
   const BlockWs ws = carve(T, d, E, k, I, I_shared);
   if (workspace_bytes < ws.total) return ARIA_ERR_BAD_ARG;
+  W8a8Ws q{};
+  if (w8a8 && !w8a8_fits(T * k, d, I, ws, q)) return ARIA_ERR_BAD_ARG;
   uint8_t* base = static_cast<uint8_t*>(workspace);
   auto at = [&](int64_t off) { return static_cast<void*>(base + off); };
   int32_t* idx = static_cast<int32_t*>(at(ws.idx));
@@ -124,8 +143,16 @@ int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const 
     if ((rc = aria_router_topk(x, w_router, at(ws.logits), idx, at(ws.scores), counts, T, d, E, k, stream))) return rc;
   }
   if ((rc = aria_build_permutation(idx, counts, offsets, dest, src, T, E, k, 1, stream))) return rc;
-  if ((rc = aria_permute_rows(x, src, at(ws.permuted), R, d, stream))) return rc;
-  if (fc1_scale) {
+  if (w8a8) {
+    float* xs = static_cast<float*>(at(q.xs));
+    float* hs = static_cast<float*>(at(q.hs));
+    if ((rc = aria_permute_quantize_fp8_rows(x, src, at(q.xq), xs, R, d, stream))) return rc;
+    if ((rc = aria_grouped_gemm_w8a8(at(q.xq), xs, fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, stream))) return rc;
+    if ((rc = aria_permute_quantize_fp8_rows(at(ws.h), nullptr, at(q.hq), hs, R, I, stream))) return rc;
+    if ((rc = aria_grouped_gemm_w8a8(at(q.hq), hs, fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, stream))) return rc;
+  } else if ((rc = aria_permute_rows(x, src, at(ws.permuted), R, d, stream))) {
+    return rc;
+  } else if (fc1_scale) {
     if ((rc = aria_grouped_gemm_fp8(at(ws.permuted), fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, stream)))
       return rc;
     if ((rc = aria_grouped_gemm_fp8(at(ws.h), fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, stream))) return rc;
@@ -169,7 +196,7 @@ extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const voi
                                   const void* up_w, const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k,
                                   int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
                                   int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
-  return moe_block_run(x, w_router, fc1_w, fc2_w, nullptr, nullptr, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
+  return moe_block_run(x, w_router, fc1_w, fc2_w, nullptr, nullptr, false, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
                        forced_top_idx, workspace, workspace_bytes, stream, side_stream);
 }
 
@@ -184,6 +211,22 @@ extern "C" int aria_moe_block_fwd_fp8(const void* x, const void* w_router, const
   if ((reinterpret_cast<uintptr_t>(fc1_w) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_w) & 15) != 0 ||
       (reinterpret_cast<uintptr_t>(fc1_scale) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_scale) & 15) != 0)
     return ARIA_ERR_BAD_ARG;
-  return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
+  return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, false, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
                        forced_top_idx, workspace, workspace_bytes, stream, side_stream);
+}
+
+extern "C" int aria_moe_block_fwd_w8a8(const void* x, const void* w_router, const void* fc1_w_nk, const void* fc2_w_nk,
+                                       const float* fc1_scale, const float* fc2_scale, const void* gate_w, const void* up_w,
+                                       const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
+                                       int32_t I_shared, const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes,
+                                       aria_stream_t stream, aria_stream_t side_stream) {
+  // the expert GEMMs' and quantizer's constraints are checked here too, so that nothing is launched for a block that would
+  // fail half-way
+  if (!fc1_scale || !fc2_scale) return ARIA_ERR_BAD_ARG;
+  if (d <= 0 || I <= 0 || d % 128 != 0 || I % 128 != 0 || d > 4096 || I > 4096 || I > 2 * d) return ARIA_ERR_BAD_ARG;
+  if ((reinterpret_cast<uintptr_t>(fc1_w_nk) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_w_nk) & 15) != 0 ||
+      (reinterpret_cast<uintptr_t>(fc1_scale) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_scale) & 15) != 0)
+    return ARIA_ERR_BAD_ARG;
+  return moe_block_run(x, w_router, fc1_w_nk, fc2_w_nk, fc1_scale, fc2_scale, true, gate_w, up_w, down_w, out, T, d, E, k, I,
+                       I_shared, forced_top_idx, workspace, workspace_bytes, stream, side_stream);
 }

@@ -1,5 +1,6 @@
 // aria_quantize_fp8_cols: per-(expert, output column) e4m3 quantisation of the routed-expert weights (GroupedGEMM.weight,
-// [G, K, N] bf16, N contiguous) for the fp8-weight grouped GEMM (gemm.cu, aria_grouped_gemm_fp8).
+// [G, K, N] bf16, N contiguous) for the fp8-weight grouped GEMMs (gemm.cu, aria_grouped_gemm_fp8 / _w8a8).
+// aria_permute_quantize_fp8_rows: the same formula per row of the activations, for aria_grouped_gemm_w8a8.
 //
 //   scale[g, n] = max_k |w[g, k, n]| / 448        (fp32, IEEE division; an all-zero column gets scale 1)
 //   q[g, k, n]  = e4m3(w[g, k, n] / scale[g, n])  (IEEE division, round to nearest even, saturating)
@@ -83,7 +84,74 @@ __global__ void __launch_bounds__(256) cast_e4m3_kernel(const __nv_bfloat16* __r
   }
 }
 
+// 8 bf16 (one 16-byte chunk) / scale -> 8 e4m3 codes, low byte first; IEEE division, round to nearest even, saturating
+__device__ __forceinline__ uint2 cast8_e4m3(const uint4 v, float s) {
+  const uint32_t u[4] = {v.x, v.y, v.z, v.w};
+  uint32_t packed[2] = {0u, 0u};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float x0 = __fdiv_rn(__uint_as_float(u[j] << 16), s);
+    const float x1 = __fdiv_rn(__uint_as_float(u[j] & 0xFFFF0000u), s);
+    const uint32_t pair = __nv_cvt_float2_to_fp8x2(make_float2(x0, x1), __NV_SATFINITE, __NV_E4M3);
+    packed[j >> 1] |= (pair & 0xFFFFu) << (16 * (j & 1));
+  }
+  return make_uint2(packed[0], packed[1]);
+}
+
+// Per-row e4m3 quantisation of the activations of the W8A8 expert GEMMs, fused with the token gather:
+//   scale[r] = max |x[src(r)]| / 448 (1 for an all-zero row),  q[r] = e4m3(x[src(r)] / scale[r])
+// src(r) = src_token[r], or r without a gather.  One warp per row; the row stays in registers between the amax and the cast, so
+// every source byte is read once.
+constexpr int QROW_MAX_VEC = 16;  // 16-byte chunks per lane: d <= 32 * 16 * 8 = 4096
+
+__global__ void __launch_bounds__(256) permute_quantize_rows_kernel(const uint4* __restrict__ x, const int32_t* __restrict__ src_token,
+                                                                    uint8_t* __restrict__ q, float* __restrict__ scale,
+                                                                    int64_t rows, int vec_per_row) {
+  const int lane = threadIdx.x & 31;
+  const int wpb = blockDim.x >> 5;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * wpb + (threadIdx.x >> 5); r < rows;
+       r += static_cast<int64_t>(gridDim.x) * wpb) {
+    const int64_t st = src_token ? src_token[r] : r;  // st < 0: alignment pad row of the training layout, quantised as zeros
+    uint4 v[QROW_MAX_VEC];
+    float m = 0.f;
+#pragma unroll
+    for (int i = 0; i < QROW_MAX_VEC; ++i) {
+      const int c = lane + 32 * i;
+      v[i] = (st >= 0 && c < vec_per_row) ? __ldg(x + st * vec_per_row + c) : make_uint4(0, 0, 0, 0);
+      const uint32_t u[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        m = fmaxf(m, fmaxf(fabsf(__uint_as_float(u[j] << 16)), fabsf(__uint_as_float(u[j] & 0xFFFF0000u))));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    const float s = m > 0.f ? __fdiv_rn(m, E4M3_MAX) : 1.f;
+    if (lane == 0) scale[r] = s;
+    uint2* dst = reinterpret_cast<uint2*>(q + r * vec_per_row * 8);
+#pragma unroll
+    for (int i = 0; i < QROW_MAX_VEC; ++i) {
+      const int c = lane + 32 * i;
+      if (c < vec_per_row) dst[c] = cast8_e4m3(v[i], s);
+    }
+  }
+}
+
 }  // namespace
+
+extern "C" int aria_permute_quantize_fp8_rows(const void* x, const int32_t* src_token, void* q, float* scale, int64_t rows,
+                                              int32_t d, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(x && q && scale);
+  ARIA_CHECK_ARG(rows >= 0 && d > 0 && d % 8 == 0 && d <= 32 * QROW_MAX_VEC * 8);
+  ARIA_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(q) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(scale) & 3) == 0);
+  if (rows == 0) return ARIA_OK;
+  int64_t blocks = (rows + 7) / 8;
+  const int64_t cap = static_cast<int64_t>(aria::sm_count()) * 16;
+  if (blocks > cap) blocks = cap;
+  permute_quantize_rows_kernel<<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const uint4*>(x), src_token, static_cast<uint8_t*>(q), scale, rows, d / 8);
+  return aria::check_launch("permute_quantize_rows_kernel");
+}
 
 extern "C" int aria_quantize_fp8_cols(const void* w, void* q, float* scale, int32_t G, int64_t K, int64_t N,
                                       aria_stream_t stream_) {

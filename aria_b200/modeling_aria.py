@@ -117,22 +117,30 @@ class AriaForConditionalGeneration(nn.Module):
         return tr
 
     @torch.no_grad()
-    def quantize_experts_fp8(self):
-        """Quantize every MoE layer's routed experts (`experts.fc1` / `experts.fc2`) to weight-only fp8 in place: e4m3 weights
-        with one fp32 scale per (expert, output column), Fp8GroupedGEMM.  It halves the bytes of the routed experts, which are
-        most of the model and most of what a decode step reads.  Layer by layer, so the peak is the bf16 model plus one
-        layer's fp8 copy; the bf16 expert tensors are freed.  Attention, shared experts, router, lm_head and the ViT stay bf16.
-        A second call changes nothing.  Returns the model.
-        Raises ValueError for non-finite expert weights and NotImplementedError under expert parallelism, both before
-        anything changes.  The captured decode graph of generate() is dropped (it holds the bf16 weight pointers); a
-        GraphedPrefill built before the call must be rebuilt."""
+    def quantize_experts_fp8(self, activations: str = "bf16"):
+        """Quantize every MoE layer's routed experts (`experts.fc1` / `experts.fc2`) to fp8 in place: e4m3 weights with one
+        fp32 scale per (expert, output column), Fp8GroupedGEMM.  It halves the bytes of the routed experts, which are most of
+        the model and most of what a decode step reads.  Layer by layer, so the peak is the bf16 model plus one layer's fp8
+        copy; the bf16 expert tensors are freed.  Attention, shared experts, router, lm_head and the ViT stay bf16.
+        `activations`: "bf16" keeps the activations in bf16 (weight-only, W8A16); "fp8" also quantizes the expert GEMMs'
+        inputs to e4m3 with one scale per row (W8A8, the fp8 tensor cores).  W8A8 rounds the activations as well, so it is
+        an explicit choice, never made by row count.  Both modes hold the same codes, scales and state dict; a model
+        quantized in one mode is switched to the other by re-laying out its codes, without re-quantizing.  A call in the
+        mode the model is already in changes nothing.  Returns the model.
+        Raises ValueError for an unknown mode or non-finite expert weights and NotImplementedError under expert
+        parallelism, all before anything changes.  The captured decode graph of generate() is dropped (it holds the old
+        weight pointers); a GraphedPrefill built before the call must be rebuilt."""
         from .moe_lm import Fp8GroupedGEMM, GroupedGEMM
+        if activations not in ("bf16", "fp8"):
+            raise ValueError(f"quantize_experts_fp8: activations must be 'bf16' or 'fp8', got {activations!r}")
         mlps = [layer.mlp for layer in self.language_model.model.layers]
         if any(m.expert_parallel is not None for m in mlps):
             raise NotImplementedError("quantize_experts_fp8: expert parallelism is enabled; it runs on bf16 expert weights")
-        todo = []
+        todo, relayout = [], []
         for i, m in enumerate(mlps):
             if m.experts.is_fp8():
+                if m.experts.fp8_activations() != (activations == "fp8"):
+                    relayout.append(m.experts)
                 continue
             for name in ("fc1", "fc2"):
                 fc = getattr(m.experts, name)
@@ -142,12 +150,17 @@ class AriaForConditionalGeneration(nn.Module):
                 if not bool(torch.isfinite(fc.weight).all()):
                     raise ValueError(f"quantize_experts_fp8: layer {i} experts.{name}.weight has non-finite values")
             todo.append(m.experts)
-        if not todo:
+        if not todo and not relayout:
             return self
         self._decode_graph = None
         for experts in todo:
             for name in ("fc1", "fc2"):
-                setattr(experts, name, Fp8GroupedGEMM.from_grouped_gemm(getattr(experts, name)))   # drops the bf16 module
+                fc = Fp8GroupedGEMM.from_grouped_gemm(getattr(experts, name))
+                setattr(experts, name, fc)              # drops the bf16 module
+                fc.set_activations(activations)         # re-laid out after the bf16 weights are gone: the same peak
+        for experts in relayout:
+            for name in ("fc1", "fc2"):
+                getattr(experts, name).set_activations(activations)
         return self
 
     @property

@@ -187,14 +187,21 @@ def _reject_fp8_grad(x: torch.Tensor):
 
 
 class Fp8GroupedGEMM(nn.Module):
-    """GroupedGEMM with weight-only fp8 expert weights (AriaForConditionalGeneration.quantize_experts_fp8): `weight`
+    """GroupedGEMM with fp8 expert weights (AriaForConditionalGeneration.quantize_experts_fp8): `weight`
     [groups, in_features, out_features] torch.float8_e4m3fn and `weight_scale` [groups, out_features] fp32, one scale per
-    (expert, output column).  Activations stay bf16; the kernel widens the weights to bf16 in shared memory and applies the
-    scale to the fp32 accumulator.  Both are frozen parameters, so a quantized model saves and reloads through its state
-    dict (`...fc1.weight`, `...fc1.weight_scale`)."""
+    (expert, output column).  Both are frozen parameters, so a quantized model saves and reloads through its state dict
+    (`...fc1.weight`, `...fc1.weight_scale`).
+    `activations` is the mode:
+      "bf16"  weight-only (W8A16): the kernel widens the weights to bf16 in shared memory.
+      "fp8"   W8A8: the input is quantized per row (ops.permute_quantize_fp8) and both operands go to the fp8 tensor cores.
+              fp8 wgmma reads K-major operands only, so `weight` is then the transpose(1, 2) view of a contiguous
+              [groups, out_features, in_features] buffer: same shape, codes and state dict as in "bf16" mode, other strides.
+    Both scales multiply the fp32 accumulator before the epilogue rounds it."""
 
-    def __init__(self, in_features, out_features, groups, device=None, weight=None, weight_scale=None):
+    def __init__(self, in_features, out_features, groups, device=None, weight=None, weight_scale=None, activations="bf16"):
         super().__init__()
+        if activations not in ("bf16", "fp8"):
+            raise ValueError(f"activations must be 'bf16' or 'fp8', got {activations!r}")
         self.in_features = in_features
         self.out_features = out_features
         self.groups = groups
@@ -206,18 +213,34 @@ class Fp8GroupedGEMM(nn.Module):
             raise ValueError(f"weight must be [{groups}, {in_features}, {out_features}] float8_e4m3fn")
         if weight_scale.shape != (groups, out_features) or weight_scale.dtype != torch.float32:
             raise ValueError(f"weight_scale must be [{groups}, {out_features}] float32")
+        self.activations = "bf16"
         self.weight = nn.Parameter(weight, requires_grad=False)
         self.weight_scale = nn.Parameter(weight_scale, requires_grad=False)
+        self.set_activations(activations)
 
     @classmethod
     def from_grouped_gemm(cls, m: "GroupedGEMM") -> "Fp8GroupedGEMM":
         q, scale = ops.quantize_fp8_cols(m.weight.detach())
         return cls(m.in_features, m.out_features, m.groups, weight=q, weight_scale=scale)
 
+    def set_activations(self, activations: str) -> None:
+        """Switch between W8A16 ("bf16") and W8A8 ("fp8") by re-laying out the existing codes; nothing is re-quantized."""
+        if activations not in ("bf16", "fp8"):
+            raise ValueError(f"activations must be 'bf16' or 'fp8', got {activations!r}")
+        w = self.weight.detach()
+        if activations == "fp8" and not w.transpose(1, 2).is_contiguous():
+            self.weight = nn.Parameter(w.transpose(1, 2).contiguous().transpose(1, 2), requires_grad=False)
+        elif activations == "bf16" and not w.is_contiguous():
+            self.weight = nn.Parameter(w.contiguous(), requires_grad=False)
+        self.activations = activations
+
     def forward(self, input, tokens_per_expert):
         _reject_fp8_grad(input)
-        return ops.grouped_gemm_fp8(input, self.weight, self.weight_scale,
-                                    _as_offsets(tokens_per_expert, self.groups, input.device))
+        off = _as_offsets(tokens_per_expert, self.groups, input.device)
+        if self.activations == "fp8":
+            aq, a_scale = ops.permute_quantize_fp8(input)
+            return ops.grouped_gemm_w8a8(aq, a_scale, self.weight, self.weight_scale, off)
+        return ops.grouped_gemm_fp8(input, self.weight, self.weight_scale, off)
 
 
 class GroupedMLP(nn.Module):
@@ -237,10 +260,24 @@ class GroupedMLP(nn.Module):
             raise RuntimeError("GroupedMLP: fc1 and fc2 must both be fp8 (Fp8GroupedGEMM) or both not")
         return f1
 
+    def fp8_activations(self) -> bool:
+        """Whether fc1 / fc2 are W8A8 (Fp8GroupedGEMM with activations="fp8"); the two must be in the same mode."""
+        if not self.is_fp8():
+            return False
+        a1, a2 = self.fc1.activations, self.fc2.activations
+        if a1 != a2:
+            raise RuntimeError(f"GroupedMLP: fc1 ({a1}) and fc2 ({a2}) must quantize their activations alike")
+        return a1 == "fp8"
+
     def forward(self, permuted_tokens, tokens_per_expert):
         off = _as_offsets(tokens_per_expert, self.fc1.groups, permuted_tokens.device)
         if self.is_fp8():
             _reject_fp8_grad(permuted_tokens)
+            if self.fp8_activations():
+                xq, xs = ops.permute_quantize_fp8(permuted_tokens)
+                h = ops.grouped_gemm_w8a8(xq, xs, self.fc1.weight, self.fc1.weight_scale, off, swiglu=True)
+                hq, hs = ops.permute_quantize_fp8(h)
+                return ops.grouped_gemm_w8a8(hq, hs, self.fc2.weight, self.fc2.weight_scale, off)
             h = ops.grouped_gemm_fp8(permuted_tokens, self.fc1.weight, self.fc1.weight_scale, off, swiglu=True)
             return ops.grouped_gemm_fp8(h, self.fc2.weight, self.fc2.weight_scale, off)
         if type(self.fc1) is GroupedGEMM and type(self.fc2) is GroupedGEMM:
@@ -338,7 +375,8 @@ class MoELayer(nn.Module):
             out = ops.moe_block_fwd(x, self.router.weight, fc1.weight, fc2.weight, se.gate_proj.weight,
                                     se.up_proj.weight, se.down_proj.weight, self.router.config.moe_topk,
                                     forced_top_idx=self.router.forced_top_indices, side_stream=_side_stream(x.device),
-                                    fc1_scale=fc1.weight_scale if fp8 else None, fc2_scale=fc2.weight_scale if fp8 else None)
+                                    fc1_scale=fc1.weight_scale if fp8 else None, fc2_scale=fc2.weight_scale if fp8 else None,
+                                    w8a8=self.experts.fp8_activations())
             return out.view(hidden_states.shape)
         # module-by-module path (adapter-wrapped experts, CPU stand-in ops of the host-logic tests)
         forked = shared_expert_overlapped(lambda: self.shared_experts(hidden_states), hidden_states)

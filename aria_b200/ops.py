@@ -166,6 +166,54 @@ def grouped_gemm_fp8(a: torch.Tensor, q: torch.Tensor, scale: torch.Tensor, offs
     return out
 
 
+def permute_quantize_fp8(x: torch.Tensor, src_token: Optional[torch.Tensor] = None):
+    """Per-row e4m3 quantisation of activations x [*, d] bf16, gathered through src_token [rows] int32 when given ->
+    (q [rows, d] torch.float8_e4m3fn, scale [rows] fp32): scale = amax of the row / 448 (an all-zero row gets 1),
+    q = e4m3(row / scale), bit for bit `(x.float() / scale[:, None]).to(torch.float8_e4m3fn)`."""
+    _chk(x)
+    if x.dim() != 2:
+        raise ValueError(f"expected [rows, d] activations, got {tuple(x.shape)}")
+    rows, d = x.shape
+    if src_token is not None:
+        _chk(src_token, torch.int32, align=4)
+        rows = src_token.numel()
+    q = torch.empty((rows, d), dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        L.check(L.load().aria_permute_quantize_fp8_rows(_p(x), _p(src_token), _p(q), _p(scale), rows, d, _stream(x)),
+                "permute_quantize_fp8")
+    return q, scale
+
+
+def _kmajor(weight: torch.Tensor) -> torch.Tensor:
+    """The [E, N, K] e4m3 buffer behind a W8A8 expert weight, the [E, K, N] parameter's transpose(1, 2) view."""
+    if weight.dim() != 3 or not weight.transpose(1, 2).is_contiguous():
+        raise ValueError("W8A8 expert weights must be the transpose(1, 2) view of a contiguous [E, N, K] buffer "
+                         "(quantize_experts_fp8(activations=\"fp8\"))")
+    return _chk(weight.transpose(1, 2), torch.float8_e4m3fn)
+
+
+def grouped_gemm_w8a8(aq: torch.Tensor, a_scale: torch.Tensor, weight: torch.Tensor, weight_scale: torch.Tensor,
+                      offsets: torch.Tensor, swiglu: bool = False) -> torch.Tensor:
+    """grouped_gemm with e4m3 activations aq [rows, K] (per-row scales a_scale [rows], permute_quantize_fp8) and e4m3 weights
+    weight [E, K, N_b] (K-major storage, see _kmajor) with per-column scales weight_scale [E, N_b]: the fp32 accumulator is
+    multiplied by a_scale[row] * weight_scale[e, col] before the epilogue rounds it.  swiglu=True: N_b = 2I, out [rows, I]."""
+    _chk(aq, torch.float8_e4m3fn), _chk(a_scale, torch.float32, align=4), _chk(weight_scale, torch.float32)
+    _chk(offsets, torch.int32)
+    b = _kmajor(weight)
+    rows, K = aq.shape
+    E, Kb, Nb = weight.shape
+    if Kb != K or a_scale.shape != (rows,) or weight_scale.shape != (E, Nb) or offsets.numel() != E + 1:
+        raise ValueError(f"grouped_gemm_w8a8: aq {tuple(aq.shape)}, a_scale {tuple(a_scale.shape)}, weight {tuple(weight.shape)}, "
+                         f"weight_scale {tuple(weight_scale.shape)}, offsets {offsets.numel()} do not fit together")
+    N = Nb // 2 if swiglu else Nb
+    out = torch.empty((rows, N), dtype=bf16, device=aq.device)
+    with torch.cuda.device(aq.device):
+        L.check(L.load().aria_grouped_gemm_w8a8(_p(aq), _p(a_scale), _p(b), _p(weight_scale), _p(out), _p(offsets), rows, K, N, E,
+                                                L.EPI_SWIGLU if swiglu else L.EPI_LINEAR, _stream(aq)), "grouped_gemm_w8a8")
+    return out
+
+
 def grouped_gemm_regions(a_buf: torch.Tensor, b: torch.Tensor, starts: torch.Tensor, counts: torch.Tensor, rows_hint: int,
                          swiglu: bool = False, group_mod: int = 0, out: Optional[torch.Tensor] = None,
                          out_group_base: Optional[torch.Tensor] = None, out_group_row0: Optional[torch.Tensor] = None,
@@ -465,15 +513,23 @@ def unpermute_combine(y: torch.Tensor, dest_row: torch.Tensor, scores: torch.Ten
 def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, fc2_w: torch.Tensor, gate_w: Optional[torch.Tensor],
                   up_w: Optional[torch.Tensor], down_w: Optional[torch.Tensor], k: int,
                   forced_top_idx: Optional[torch.Tensor] = None, side_stream: Optional[torch.cuda.Stream] = None,
-                  fc1_scale: Optional[torch.Tensor] = None, fc2_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+                  fc1_scale: Optional[torch.Tensor] = None, fc2_scale: Optional[torch.Tensor] = None,
+                  w8a8: bool = False) -> torch.Tensor:
     """MoELayer.forward (moe_lm.py:548-577) as one C-ABI call (`aria_moe_block_fwd`): x [T, d] -> [T, d].
     With fc1_scale [E, 2I] / fc2_scale [E, d] fp32, fc1_w / fc2_w are e4m3 (quantize_fp8_cols) and the call is
-    `aria_moe_block_fwd_fp8`."""
+    `aria_moe_block_fwd_fp8`; with w8a8=True as well, the weights are K-major (see grouped_gemm_w8a8), the activations are
+    quantized per row too and the call is `aria_moe_block_fwd_w8a8`."""
     fp8 = fc1_scale is not None or fc2_scale is not None
     if fp8 and (fc1_scale is None or fc2_scale is None):
         raise ValueError("moe_block_fwd: give both fc1_scale and fc2_scale, or neither")
+    if w8a8 and not fp8:
+        raise ValueError("moe_block_fwd: w8a8 needs the fp8 weight scales")
     wdt = torch.float8_e4m3fn if fp8 else bf16
-    _chk(x), _chk(w_router), _chk(fc1_w, wdt), _chk(fc2_w, wdt)
+    _chk(x), _chk(w_router)
+    if w8a8:
+        _kmajor(fc1_w), _kmajor(fc2_w)
+    else:
+        _chk(fc1_w, wdt), _chk(fc2_w, wdt)
     T, d = x.shape
     E, I = fc2_w.shape[0], fc2_w.shape[1]
     assert w_router.shape == (E, d) and fc1_w.shape == (E, d, 2 * I) and fc2_w.shape == (E, I, d)
@@ -494,7 +550,11 @@ def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, 
     out = torch.empty((T, d), dtype=bf16, device=x.device)
     side = C.c_void_p(side_stream.cuda_stream) if side_stream is not None else None
     with torch.cuda.device(x.device):
-        if fp8:
+        if w8a8:
+            L.check(lib.aria_moe_block_fwd_w8a8(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(fc1_scale), _p(fc2_scale),
+                                                _p(gate_w), _p(up_w), _p(down_w), _p(out), T, d, E, k, I, Is, _p(forced_top_idx),
+                                                _p(ws), nbytes, _stream(x), side), "moe_block_fwd_w8a8")
+        elif fp8:
             L.check(lib.aria_moe_block_fwd_fp8(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(fc1_scale), _p(fc2_scale), _p(gate_w),
                                                _p(up_w), _p(down_w), _p(out), T, d, E, k, I, Is, _p(forced_top_idx), _p(ws), nbytes,
                                                _stream(x), side), "moe_block_fwd_fp8")

@@ -116,6 +116,25 @@ int aria_quantize_fp8_cols(const void* w, void* q, float* scale, int32_t G, int6
 int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const float* b_scale, void* out, const int32_t* group_offsets,
                           int64_t rows, int64_t k, int64_t n, int32_t num_groups, int32_t epilogue, aria_stream_t stream);
 
+/* FP8 activations and weights (W8A8) for the routed experts.
+ *
+ * aria_permute_quantize_fp8_rows: x [*, d] bf16 -> q [rows, d] e4m3, scale [rows] fp32, row r taken from x[src_token[r]]
+ *   (x[r] when src_token is NULL; src_token[r] < 0 gives a zero row):
+ *   scale[r] = max |x_row| / 448 (IEEE division; an all-zero row gets 1), q = e4m3(x_row / scale[r]), round to nearest even,
+ *   saturating — bit for bit (x.float() / scale[:, None]).to(float8_e4m3fn).  d % 8 == 0, d <= 4096; x, q 16-byte aligned.
+ *
+ * aria_grouped_gemm_w8a8: out[off[g]:off[g+1]] = epilogue(a[rows of g] . b[g]^T * a_scale[row] * b_scale[g, col]), with
+ *   a_fp8 [rows, k] e4m3 and a_scale [rows] from aria_permute_quantize_fp8_rows, b_fp8_nk [G, N_b, k] e4m3 (K-major: the
+ *   transpose of the [G, k, N_b] weights of aria_quantize_fp8_cols, same codes) and b_scale [G, N_b].  Epilogue ARIA_EPI_LINEAR
+ *   (N_b = n) or ARIA_EPI_SWIGLU (N_b = 2n, gate then up, out [rows, n]).  Both scales multiply the fp32 accumulator before the
+ *   epilogue's first bf16 rounding; every rounding point after that is aria_gemm's.  The tensor cores accumulate one
+ *   128-element k-block at a time, which is then added to an fp32 accumulator.  k % 128 == 0, n % 64 == 0. */
+int aria_permute_quantize_fp8_rows(const void* x, const int32_t* src_token, void* q, float* scale, int64_t rows, int32_t d,
+                                   aria_stream_t stream);
+int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, const void* b_fp8_nk, const float* b_scale, void* out,
+                           const int32_t* group_offsets, int64_t rows, int64_t k, int64_t n, int32_t num_groups, int32_t epilogue,
+                           aria_stream_t stream);
+
 /* Weight gradient of a (grouped) linear layer — backward of gmm / F.linear:
  *   out[g, m, n] = sum_{r in group g} a[r, m] * b[r, n]   a [rows, md] (row stride lda), b [rows, nd] (ldb), out [G, md, nd] bf16.
  * group_offsets: device int32 row offsets, non-decreasing, any values (densely packed groups as the reference's dispatcher
@@ -186,6 +205,14 @@ int aria_moe_block_fwd_fp8(const void* x, const void* w_router, const void* fc1_
                            const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
                            int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx,
                            void* workspace, int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream);
+/* The same block with W8A8 experts: fc1_w_nk [E, 2I, d] / fc2_w_nk [E, d, I] are the K-major e4m3 weights (the transposes of
+ * aria_quantize_fp8_cols' codes) with the scales fc1_scale [E, 2I] / fc2_scale [E, d].  The gathered tokens and h are
+ * quantised per row (aria_permute_quantize_fp8_rows) and the expert GEMMs are aria_grouped_gemm_w8a8.
+ * d % 128 == 0, I % 128 == 0, d and I <= 4096, I <= 2 d.  Same workspace. */
+int aria_moe_block_fwd_w8a8(const void* x, const void* w_router, const void* fc1_w_nk, const void* fc2_w_nk, const float* fc1_scale,
+                            const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
+                            int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx,
+                            void* workspace, int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream);
 
 /* ---- backward of the MoE block (BASELINE cfg 5; autograd through moe_lm.py:548-577) ---- */
 /* h = bf16(bf16(silu(g)) * u) with g = h1[:, :I], u = h1[:, I:]  (unfused `glu`, moe_lm.py:505-507; training keeps h1). */
