@@ -96,21 +96,14 @@ inline int make_tmap_bf16_swz(CUtensorMap* tm, const void* ptr, int rank, const 
   return ARIA_OK;
 }
 
+// Row-major 2-D tensor map; e4m3 operands are UINT8 maps
 inline int make_tmap_2d(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                        uint32_t box_inner, uint32_t box_outer) {
+                        uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B,
+                        CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
   uint64_t dims[2] = {inner, outer};
   uint64_t str[1] = {row_stride_bytes};
   uint32_t box[2] = {box_inner, box_outer};
-  return make_tmap_bf16(tm, ptr, 2, dims, str, box);
-}
-
-// byte tensor map without swizzle (e4m3 weights as UINT8; 16-byte rows of the box land contiguously)
-inline int make_tmap_2d_u8(CUtensorMap* tm, const void* ptr, uint64_t inner, uint64_t outer, uint64_t row_stride_bytes,
-                           uint32_t box_inner, uint32_t box_outer) {
-  uint64_t dims[2] = {inner, outer};
-  uint64_t str[1] = {row_stride_bytes};
-  uint32_t box[2] = {box_inner, box_outer};
-  return make_tmap_bf16_swz(tm, ptr, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  return make_tmap_bf16_swz(tm, ptr, 2, dims, str, box, swizzle, dtype);
 }
 
 // Per-device state: one process may drive several GPUs (the reference's device_map="auto", aria/inference.py:55-57), and
@@ -141,5 +134,24 @@ inline cudaError_t ensure_dynamic_smem(bool* flags, Kernel kern, int bytes) {
   else fprintf(stderr, "aria_b200: cudaFuncSetAttribute(smem=%d) failed: %s\n", bytes, cudaGetErrorString(e));
   return e;
 }
+
+// Launches a persistent kernel: one CTA per SM, fewer when there are fewer than `max_tiles` tiles, with `smem` bytes of
+// dynamic shared memory.  Each kernel instantiates this template once, so each has its own opt-in flags.
+template <auto kernel, typename... Args>
+inline int launch_persistent(const char* name, int threads, int smem, int64_t max_tiles, cudaStream_t stream,
+                             const Args&... args) {
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  int grid = sm_count();
+  if (max_tiles < grid) grid = static_cast<int>(max_tiles);
+  if (grid < 1) grid = 1;
+  kernel<<<grid, threads, smem, stream>>>(args...);
+  return check_launch(name);
+}
+
+// Grouped expert GEMM (gemm.cu): out[rows, n] = a[rows, k] x b[g] for the rows of group g (`offsets`), b = [groups, k, n]
+// bf16, or e4m3 with one fp32 scale per (group, column) when b_scale is given.  `epilogue`: LINEAR or SWIGLU.
+int grouped_gemm(const void* a, const void* b, const float* b_scale, void* out, const int32_t* offsets, int64_t rows,
+                 int64_t k, int64_t n, int32_t groups, int32_t epilogue, cudaStream_t stream);
 
 }  // namespace aria

@@ -7,7 +7,6 @@ namespace aria {
 
 // four k-blocks in flight: the ring takes what the fp32 staging tile of the epilogue leaves of the 227 KB per block
 constexpr int GEMM_STAGES = 4;
-constexpr int acc_ld(int BN) { return BN + 4; }  // staging row stride (floats): 16-byte aligned rows, spread over the banks
 // fp8 B (B_FP8): TMA lands the e4m3 boxes in a ring of their own, the producer warpgroup's three idle warps widen them to bf16
 // in the SW128 layout of the bf16 ring, and the wgmma sequence is unchanged.  Three landing slots fit beside the four bf16
 // stages and the fp32 staging tile (DESIGN §3); a fourth would not.
@@ -57,15 +56,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   static_assert(!B_FP8 || (B_MN && BN == 128 && EPI != ARIA_EPI_HEADS), "fp8 B: grouped [G, K, N] weights, 128-wide tiles");
   constexpr int LAND_BYTES = BN * BK;  // one k-block of fp8 B: BN/64 boxes of 64 k-rows x 64 bytes, unswizzled
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_1024();
   float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [BM][ACC_LD] fp32 accumulator staging
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + BM * ACC_LD);
-  uint64_t* empty_bar = full_bar + STAGES;
-  // B_FP8: e4m3 landing ring after the barrier block; land_full completes on the TMA bytes, land_empty once per converter warp
-  uint64_t* land_full = empty_bar + STAGES;
-  uint64_t* land_empty = land_full + FP8_LAND_STAGES;
-  uint8_t* land = reinterpret_cast<uint8_t*>(stg + BM * ACC_LD) + 256;
+  const BarrierRing<STAGES> bar(stg + BM * ACC_LD);
+  // B_FP8: e4m3 landing ring after the barrier block; its full barriers complete on the TMA bytes, its empty ones once per
+  // converter warp
+  const BarrierRing<FP8_LAND_STAGES> land_bar(bar.empty + STAGES);
+  uint8_t* land = reinterpret_cast<uint8_t*>(bar.full) + 256;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -76,17 +73,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     prefetch_tmap(&tmB0);
     if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(&tmB1);
     if (p.n_seg > 2) prefetch_tmap(&tmB2);
-    for (int i = 0; i < STAGES; ++i) {
-      // B_FP8: a stage is full once A has landed AND every converter warp has written its share of B
-      mbar_init(&full_bar[i], B_FP8 ? 1 + FP8_CONVERT_WARPS : 1);
-      mbar_init(&empty_bar[i], CONSUMER_WARPS);
-    }
-    if constexpr (B_FP8) {
-      for (int i = 0; i < FP8_LAND_STAGES; ++i) {
-        mbar_init(&land_full[i], 1);
-        mbar_init(&land_empty[i], FP8_CONVERT_WARPS);
-      }
-    }
+    // B_FP8: a stage is full once A has landed AND every converter warp has written its share of B
+    bar.init(B_FP8 ? 1 + FP8_CONVERT_WARPS : 1, CONSUMER_WARPS);
+    if constexpr (B_FP8) land_bar.init(1, FP8_CONVERT_WARPS);
     fence_mbar_init();
   }
   __syncthreads();
@@ -95,7 +84,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int n_tiles = (n_out_total + OUT_BN - 1) / OUT_BN;
   const int k_blocks = (p.K + BK - 1) / BK;
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+  const uint32_t full0 = smem_u32(bar.full), empty0 = smem_u32(bar.empty);
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
@@ -103,8 +92,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (warp == 0 && elect_one()) {
       TileSched sched;
       sched.init(p, n_tiles);
-      uint32_t stage = 0, phase = 0;
-      uint32_t lstage = 0, lphase = 0;  // B_FP8 landing ring
+      RingPos<STAGES> rp;
+      RingPos<FP8_LAND_STAGES> lp;  // B_FP8 landing ring
       for (int t = blockIdx.x;; t += gridDim.x) {
         int grp, m_idx, n_idx, row0, rows;
         if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
@@ -125,60 +114,36 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           b_c0 = col - seg * p.N + bgrp * p.b_group_rows;
         }
         for (int kb = 0; kb < k_blocks; ++kb) {
-          const uint32_t fb = full0 + stage * 8;
-          const uint32_t sa = smem_base + stage * STAGE_BYTES;
+          const uint32_t fb = full0 + rp.stage * 8;
+          const uint32_t sa = smem_base + rp.stage * STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
-          mbar_wait_addr(empty0 + stage * 8, phase ^ 1);
+          mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
           mbar_arrive_expect_tx_addr(fb, B_FP8 ? A_STAGE_BYTES : STAGE_BYTES);
           tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
-          if constexpr (B_FP8) {
-            // the e4m3 boxes go to the landing ring; the converters widen them into this stage's B slot.  That slot is free:
-            // the converters see this k-block only after the empty-barrier wait above.
-            const uint32_t lf = smem_u32(land_full) + lstage * 8;
-            mbar_wait_addr(smem_u32(land_empty) + lstage * 8, lphase ^ 1);
-            mbar_arrive_expect_tx_addr(lf, LAND_BYTES);
+          if constexpr (B_MN) {
+            // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n, BN/64 boxes per stage
+            uint32_t dst = sb, box_bytes = 64 * BK * 2, bar_addr = fb;
+            if constexpr (B_FP8) {
+              // the e4m3 boxes go to the landing ring; the converters widen them into this stage's B slot.  That slot is
+              // free: the converters see this k-block only after the empty-barrier wait above.
+              bar_addr = smem_u32(land_bar.full) + lp.stage * 8;
+              mbar_wait_addr(smem_u32(land_bar.empty) + lp.stage * 8, lp.phase ^ 1);
+              mbar_arrive_expect_tx_addr(bar_addr, LAND_BYTES);
+              dst = smem_u32(land) + lp.stage * LAND_BYTES;
+              box_bytes = 64 * BK;
+            }
             const int krow = b_c0 + kb * BK;
-            constexpr int CH = BN / 64;
 #pragma unroll
-            for (int c = 0; c < CH; ++c) {
-              int ncol;
-              if constexpr (EPI == ARIA_EPI_SWIGLU) {
-                constexpr int HALF = CH / 2;
-                ncol = (c < HALF) ? (n_idx * OUT_BN + c * 64) : (p.N + n_idx * OUT_BN + (c - HALF) * 64);
-              } else {
-                ncol = n_idx * BN + c * 64;
-              }
-              tma_load_2d_addr(smem_u32(land) + lstage * LAND_BYTES + c * (64 * BK), &tmB0, lf, ncol, krow);
-            }
-            if (++lstage == FP8_LAND_STAGES) {
-              lstage = 0;
-              lphase ^= 1;
-            }
-          } else if constexpr (B_MN) {
-            // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n (8 KB), BN/64 boxes per stage
-            const int krow = b_c0 + kb * BK;
-            constexpr int CH = BN / 64;
-#pragma unroll
-            for (int c = 0; c < CH; ++c) {
-              int ncol;
-              if constexpr (EPI == ARIA_EPI_SWIGLU) {
-                constexpr int HALF = CH / 2;
-                ncol = (c < HALF) ? (n_idx * OUT_BN + c * 64) : (p.N + n_idx * OUT_BN + (c - HALF) * 64);
-              } else {
-                ncol = n_idx * BN + c * 64;
-              }
-              tma_load_2d_addr(sb + c * (64 * BK * 2), &tmB0, fb, ncol, krow);
-            }
+            for (int c = 0; c < BN / 64; ++c)
+              tma_load_2d_addr(dst + c * box_bytes, &tmB0, bar_addr, tile_b_col<BN, EPI>(c * 64, n_idx, p.N), krow);
+            if constexpr (B_FP8) lp.next();
           } else if constexpr (EPI == ARIA_EPI_SWIGLU) {
             tma_load_2d_addr(sb, tb0, fb, kb * BK, b_c0);
             tma_load_2d_addr(sb + (BN / 2) * BK * 2, tb1, fb, kb * BK, b_c1);
           } else {
             tma_load_2d_addr(sb, tb0, fb, kb * BK, b_c0);
           }
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          rp.next();
         }
       }
     } else if constexpr (B_FP8) {
@@ -190,14 +155,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int ct = threadIdx.x - 32;
         TileSched sched;
         sched.init(p, n_tiles);
-        uint32_t stage = 0, phase = 0, lstage = 0, lphase = 0;
+        RingPos<STAGES> rp;
+        RingPos<FP8_LAND_STAGES> lp;
         for (int t = blockIdx.x;; t += gridDim.x) {
           int grp, m_idx, n_idx, row0, rows;
           if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
           for (int kb = 0; kb < k_blocks; ++kb) {
-            mbar_wait_addr(smem_u32(land_full) + lstage * 8, lphase);
-            const uint8_t* src = land + lstage * LAND_BYTES;
-            uint8_t* dst = smem + stage * STAGE_BYTES + A_STAGE_BYTES;
+            mbar_wait_addr(smem_u32(land_bar.full) + lp.stage * 8, lp.phase);
+            const uint8_t* src = land + lp.stage * LAND_BYTES;
+            uint8_t* dst = smem + rp.stage * STAGE_BYTES + A_STAGE_BYTES;
 #pragma unroll 1
             for (int i = ct; i < LAND_BYTES / 16; i += FP8_CONVERT_WARPS * 32) {
               const uint4 v = *reinterpret_cast<const uint4*>(src + i * 16);
@@ -211,17 +177,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             fence_proxy_async_smem();  // generic-proxy stores -> visible to the wgmma (async proxy) reads
             __syncwarp();
             if (lane == 0) {
-              mbar_arrive(&full_bar[stage]);
-              mbar_arrive(&land_empty[lstage]);
+              mbar_arrive(&bar.full[rp.stage]);
+              mbar_arrive(&land_bar.empty[lp.stage]);
             }
-            if (++stage == STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-            if (++lstage == FP8_LAND_STAGES) {
-              lstage = 0;
-              lphase ^= 1;
-            }
+            rp.next();
+            lp.next();
           }
         }
       }
@@ -230,7 +190,6 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
     setmaxnreg_inc<232>();
     const int cw = wg - 1;
-    const int tid = threadIdx.x & 127;
     constexpr uint32_t b_lbo = B_MN ? 64 * BK * 2 : 16;
     constexpr uint32_t b_sbo = 1024;
     constexpr uint32_t b_kadv = (B_MN ? 16 * 128 : 32) >> 4;
@@ -238,72 +197,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // addresses stay below 2^18, so adding (byte offset >> 4) never carries into the next field
     const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
     const uint64_t db0 = make_smem_desc(smem_base + A_STAGE_BYTES, b_lbo, b_sbo);
-    // this thread's place in the wgmma accumulator fragment, and the row it finishes in the epilogue
-    const int frag_row = cw * 64 + (tid >> 5) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
-    const int epi_row = cw * 64 + (tid & 63), half = tid >> 6;
+    const ConsumerThread ct = consumer_thread(cw, lane);
     TileSched sched;
     sched.init(p, n_tiles);
-    uint32_t stage = 0, phase = 0;
+    RingPos<STAGES> rp;
     for (int t = blockIdx.x;; t += gridDim.x) {
       int grp, m_idx, n_idx, row0, rows;
       if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      // B_FP8: the scales of this thread's accumulator columns (8 j + frag_col, +1), fetched while the k-loop runs
       float2 bsc[BN / 8];
-      if constexpr (B_FP8) {
-        const int ncols = EPI == ARIA_EPI_SWIGLU ? 2 * p.N : p.N;
-        const float* srow = p.b_scale + static_cast<int64_t>(weight_block(p, grp)) * ncols;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          int col;
-          if constexpr (EPI == ARIA_EPI_SWIGLU)  // gate columns [0, OUT_BN) of the tile, then the up columns
-            col = (8 * j < OUT_BN) ? n_idx * OUT_BN + 8 * j + frag_col : p.N + n_idx * OUT_BN + 8 * j - OUT_BN + frag_col;
-          else
-            col = n_idx * BN + 8 * j + frag_col;
-          bsc[j] = col < ncols ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
-        }
-      }
+      if constexpr (B_FP8) load_col_scales<BN, EPI>(p, grp, n_idx, ct.frag_col, bsc);
       // one k-block's wgmma group stays in flight while the next one is issued; a stage is released once its group retired
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait_addr(full0 + stage * 8, phase);
-        const uint64_t da = da0 + stage * (STAGE_BYTES >> 4);
-        const uint64_t db = db0 + stage * (STAGE_BYTES >> 4);
+        mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+        const uint64_t da = da0 + rp.stage * (STAGE_BYTES >> 4);
+        const uint64_t db = db0 + rp.stage * (STAGE_BYTES >> 4);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) wgmma_tile_k16<BN, B_MN>(acc, da + k * 2, db + k * b_kadv);
         wgmma_commit();
         wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = static_cast<int>(stage);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
+        prev = static_cast<int>(rp.stage);
+        rp.next();
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-
-      named_bar_sync(1 + cw, 128);  // the previous tile's epilogue has finished reading this warpgroup's staging rows
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        float* d0 = stg + frag_row * ACC_LD + 8 * j + frag_col;
-        if constexpr (B_FP8) {  // per-column weight scale on the fp32 accumulator, before any rounding of the epilogue
-          *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j] * bsc[j].x, acc[4 * j + 1] * bsc[j].y);
-          *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) = make_float2(acc[4 * j + 2] * bsc[j].x, acc[4 * j + 3] * bsc[j].y);
-        } else {
-          *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      named_bar_sync(1 + cw, 128);
-      const int r_in_grp = m_idx * BM + epi_row;
-      const bool row_ok = r_in_grp < rows;
-      const int64_t grow = static_cast<int64_t>(row0) + r_in_grp;
-      epilogue_tile<BN, EPI>(p, stg + epi_row * ACC_LD, n_out_total, n_idx, grow, row_ok, half, grp, r_in_grp);
+      if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
+      stage_and_epilogue<BN, EPI, B_FP8 ? AccScale::COL : AccScale::NONE>(p, stg, ct, acc, bsc, 1.f, 1.f, n_out_total, grp,
+                                                                           m_idx, n_idx, row0, rows);
     }
   }
 }
@@ -327,11 +252,9 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;
   static_assert(EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_SWIGLU, "W8A8: expert GEMM epilogues");
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_1024();
   float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stg + BM * ACC_LD);
-  uint64_t* empty_bar = full_bar + STAGES;
+  const BarrierRing<STAGES> bar(stg + BM * ACC_LD);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -340,10 +263,7 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CONSUMER_WARPS);
-    }
+    bar.init(1, CONSUMER_WARPS);
     fence_mbar_init();
   }
   __syncthreads();
@@ -351,7 +271,7 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int n_tiles = (p.N + OUT_BN - 1) / OUT_BN;
   const int k_blocks = p.K / W8_BK;
   const uint32_t smem_base = smem_u32(smem);
-  const uint32_t full0 = smem_u32(full_bar), empty0 = smem_u32(empty_bar);
+  const uint32_t full0 = smem_u32(bar.full), empty0 = smem_u32(bar.empty);
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
@@ -359,7 +279,7 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (warp == 0 && elect_one()) {
       TileSched sched;
       sched.init(p, n_tiles);
-      uint32_t stage = 0, phase = 0;
+      RingPos<STAGES> rp;
       for (int t = blockIdx.x;; t += gridDim.x) {
         int grp, m_idx, n_idx, row0, rows;
         if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
@@ -374,18 +294,15 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           b_r1 = b_r0 + 64;
         }
         for (int kb = 0; kb < k_blocks; ++kb) {
-          const uint32_t fb = full0 + stage * 8;
-          const uint32_t sa = smem_base + stage * STAGE_BYTES;
+          const uint32_t fb = full0 + rp.stage * 8;
+          const uint32_t sa = smem_base + rp.stage * STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
-          mbar_wait_addr(empty0 + stage * 8, phase ^ 1);
+          mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
           mbar_arrive_expect_tx_addr(fb, STAGE_BYTES);
           tma_load_2d_addr(sa, &tmA, fb, kb * W8_BK, a_row);
           tma_load_2d_addr(sb, &tmB, fb, kb * W8_BK, b_r0);
           tma_load_2d_addr(sb + 64 * W8_BK, &tmB, fb, kb * W8_BK, b_r1);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          rp.next();
         }
       }
     }
@@ -393,14 +310,12 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
     setmaxnreg_inc<232>();
     const int cw = wg - 1;
-    const int tid = threadIdx.x & 127;
     const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
     const uint64_t db0 = make_smem_desc(smem_base + A_STAGE_BYTES, 16, 1024);
-    const int frag_row = cw * 64 + (tid >> 5) * 16 + (lane >> 2), frag_col = 2 * (lane & 3);
-    const int epi_row = cw * 64 + (tid & 63), half = tid >> 6;
+    const ConsumerThread ct = consumer_thread(cw, lane);
     TileSched sched;
     sched.init(p, n_tiles);
-    uint32_t stage = 0, phase = 0;
+    RingPos<STAGES> rp;
     float part[BN / 2];  // one k-block's tensor-core sum (the first wgmma of a k-block overwrites it)
     for (int t = blockIdx.x;; t += gridDim.x) {
       int grp, m_idx, n_idx, row0, rows;
@@ -408,79 +323,101 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      // column scales of this thread's accumulator columns (8 j + frag_col, +1) and row scales of its two fragment rows (rows
-      // past the group's end are computed but never stored; the index is clamped to the buffer)
       float2 bsc[BN / 8];
-      {
-        const int ncols = EPI == ARIA_EPI_SWIGLU ? 2 * p.N : p.N;
-        const float* srow = p.b_scale + static_cast<int64_t>(weight_block(p, grp)) * ncols;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          int col;
-          if constexpr (EPI == ARIA_EPI_SWIGLU)
-            col = (8 * j < OUT_BN) ? n_idx * OUT_BN + 8 * j + frag_col : p.N + n_idx * OUT_BN + 8 * j - OUT_BN + frag_col;
-          else
-            col = n_idx * BN + 8 * j + frag_col;
-          bsc[j] = col < ncols ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
-        }
-      }
-      const int ar = row0 + m_idx * BM + frag_row;
+      load_col_scales<BN, EPI>(p, grp, n_idx, ct.frag_col, bsc);
+      // row scales of the fragment's two rows (rows past the group's end are computed but never stored; the index is clamped
+      // to the buffer)
+      const int ar = row0 + m_idx * BM + ct.frag_row;
       const float as0 = __ldg(a_scale + min(ar, p.M - 1)), as1 = __ldg(a_scale + min(ar + 8, p.M - 1));
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait_addr(full0 + stage * 8, phase);
-        const uint64_t da = da0 + stage * (STAGE_BYTES >> 4);
-        const uint64_t db = db0 + stage * (STAGE_BYTES >> 4);
+        mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+        const uint64_t da = da0 + rp.stage * (STAGE_BYTES >> 4);
+        const uint64_t db = db0 + rp.stage * (STAGE_BYTES >> 4);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < W8_BK / 32; ++k) wgmma_m64n128k32_e4m3_ss(part, da + k * 2, db + k * 2, k > 0 ? 1u : 0u);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(part);
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (lane == 0) mbar_arrive(&bar.empty[rp.stage]);
 #pragma unroll
         for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        rp.next();
       }
-
-      named_bar_sync(1 + cw, 128);  // the previous tile's epilogue has finished reading this warpgroup's staging rows
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {  // both scales on the fp32 accumulator, before any rounding of the epilogue
-        float* d0 = stg + frag_row * ACC_LD + 8 * j + frag_col;
-        *reinterpret_cast<float2*>(d0) = make_float2(acc[4 * j] * as0 * bsc[j].x, acc[4 * j + 1] * as0 * bsc[j].y);
-        *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) =
-            make_float2(acc[4 * j + 2] * as1 * bsc[j].x, acc[4 * j + 3] * as1 * bsc[j].y);
-      }
-      named_bar_sync(1 + cw, 128);
-      const int r_in_grp = m_idx * BM + epi_row;
-      const bool row_ok = r_in_grp < rows;
-      const int64_t grow = static_cast<int64_t>(row0) + r_in_grp;
-      epilogue_tile<BN, EPI>(p, stg + epi_row * ACC_LD, p.N, n_idx, grow, row_ok, half, grp, r_in_grp);
+      stage_and_epilogue<BN, EPI, AccScale::ROW_COL>(p, stg, ct, acc, bsc, as0, as1, p.N, grp, m_idx, n_idx, row0, rows);
     }
   }
-}
-
-template <int BN, bool B_MN, int EPI, bool B_FP8 = false>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap* tmB, const GemmParams& p, int max_tiles,
-                       cudaStream_t stream) {
-  constexpr int SMEM = gemm_smem_bytes<BN, B_FP8>();
-  auto kern = gemm_kernel<BN, B_MN, EPI, B_FP8>;
-  static bool attr_set[kMaxDevices] = {};
-  if (ensure_dynamic_smem(attr_set, kern, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
-  int grid = sm_count();
-  if (max_tiles < grid) grid = max_tiles;
-  if (grid < 1) grid = 1;
-  kern<<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB[0], tmB[1], tmB[2], p);
-  return check_launch("gemm_kernel");
 }
 
 }  // namespace aria
 
 using namespace aria;
 
-// aria_gemm, and aria_grouped_gemm_fp8 with b_scale != NULL (then d->b[0] is e4m3 and the GKN layout is the only one)
+static GemmParams gemm_params(const aria_gemm_desc_t* d, const float* b_scale) {
+  const bool swiglu = d->epilogue == ARIA_EPI_SWIGLU;
+  GemmParams p{};
+  p.M = static_cast<int>(d->m);
+  p.N = static_cast<int>(d->n);
+  p.K = static_cast<int>(d->k);
+  p.num_groups = d->num_groups;
+  p.group_offsets = d->group_offsets;
+  p.group_counts = d->group_counts;
+  p.out_group_base = static_cast<const uint64_t*>(d->out_group_base);
+  p.out_group_row0 = d->out_group_row0;
+  p.group_mod = d->group_mod;
+  p.b_group_rows = d->b_layout == ARIA_B_GNK ? static_cast<int>(d->n) : 0;
+  p.n_seg = swiglu ? 1 : d->n_seg;
+  p.act = d->act;
+  for (int i = 0; i < 3; ++i) {
+    p.bias[i] = static_cast<const __nv_bfloat16*>(d->bias[i]);
+    p.out[i] = static_cast<__nv_bfloat16*>(d->out[i]);
+  }
+  p.residual = static_cast<const __nv_bfloat16*>(d->residual);
+  p.ldr = d->ldr;
+  p.ldo = d->ldo;
+  p.head_dim = d->head_dim;
+  p.head_ld = d->head_ld;
+  p.rows_per_batch = d->rows_per_batch > 0 ? d->rows_per_batch : static_cast<int>(d->m);
+  p.pos0 = d->pos0;
+  p.stride_b = d->stride_b;
+  p.stride_h = d->stride_h;
+  p.rope_mask = d->rope_mask;
+  p.rope_cos = static_cast<const __nv_bfloat16*>(d->rope_cos);
+  p.rope_sin = static_cast<const __nv_bfloat16*>(d->rope_sin);
+  p.position_ids = d->position_ids;
+  p.b_scale = b_scale;
+  return p;
+}
+
+// out[rows, n] = a[rows, k] x weight block g of b, for the rows of group g
+static aria_gemm_desc_t grouped_desc(const void* a, const void* b, void* out, const int32_t* offsets, int64_t rows, int64_t k,
+                                     int64_t n, int32_t groups, int32_t epilogue) {
+  aria_gemm_desc_t d{};
+  d.a = a;
+  d.lda = k;
+  d.m = rows;
+  d.n = n;
+  d.k = k;
+  d.b[0] = b;
+  d.n_seg = 1;
+  d.b_layout = ARIA_B_GKN;
+  d.num_groups = groups;
+  d.group_offsets = offsets;
+  d.epilogue = epilogue;
+  d.out[0] = out;
+  d.ldo = n;
+  return d;
+}
+
+// Tiles of a launch at most: n-tiles x (m-tiles of all rows + one partial m-tile for each of `groups` groups)
+static int64_t max_tiles(const aria_gemm_desc_t* d, int BN, int64_t groups) {
+  const bool swiglu = d->epilogue == ARIA_EPI_SWIGLU;
+  const int out_bn = swiglu ? BN / 2 : BN;
+  const int64_t n_out_total = d->n * (swiglu ? 1 : d->n_seg);
+  return (n_out_total + out_bn - 1) / out_bn * ((d->m + BM - 1) / BM + groups);
+}
+
+// aria_gemm, and grouped_gemm with b_scale != NULL (then d->b[0] is e4m3 and the GKN layout is the only one)
 static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_t stream) {
   ARIA_CHECK_ARG(d != nullptr);
   ARIA_CHECK_ARG(d->a && d->b[0] && d->out[0]);
@@ -510,40 +447,7 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   if (d->out_group_base) ARIA_CHECK_ARG(d->out_group_row0 != nullptr && d->epilogue == ARIA_EPI_LINEAR && d->group_offsets != nullptr);
   ARIA_CHECK_ARG(d->a_rows == 0 || d->a_rows >= d->m);
 
-  GemmParams p{};
-  p.M = static_cast<int>(d->m);
-  p.N = static_cast<int>(d->n);
-  p.K = static_cast<int>(d->k);
-  p.num_groups = d->num_groups;
-  p.group_offsets = d->group_offsets;
-  p.group_counts = d->group_counts;
-  p.out_group_base = static_cast<const uint64_t*>(d->out_group_base);
-  p.out_group_row0 = d->out_group_row0;
-  p.group_mod = d->group_mod;
-  p.b_group_rows = b_gnk ? static_cast<int>(d->n) : 0;
-  p.n_seg = swiglu ? 1 : d->n_seg;
-  p.act = d->act;
-  for (int i = 0; i < 3; ++i) {
-    p.bias[i] = static_cast<const __nv_bfloat16*>(d->bias[i]);
-    p.out[i] = static_cast<__nv_bfloat16*>(d->out[i]);
-  }
-  p.residual = static_cast<const __nv_bfloat16*>(d->residual);
-  p.ldr = d->ldr;
-  p.ldo = d->ldo;
-  p.head_dim = d->head_dim;
-  p.head_ld = d->head_ld;
-  p.rows_per_batch = d->rows_per_batch > 0 ? d->rows_per_batch : static_cast<int>(d->m);
-  p.pos0 = d->pos0;
-  p.stride_b = d->stride_b;
-  p.stride_h = d->stride_h;
-  p.rope_mask = d->rope_mask;
-  p.rope_cos = static_cast<const __nv_bfloat16*>(d->rope_cos);
-  p.rope_sin = static_cast<const __nv_bfloat16*>(d->rope_sin);
-  p.position_ids = d->position_ids;
-  p.b_scale = b_scale;
-
   // ---- tile shape selection: 128-wide tiles; the 72-dim ViT heads (n = 1152 = 8 x 144) take 144-wide tiles of whole heads
-  const int64_t n_out_total = d->n * (swiglu ? 1 : d->n_seg);
   int BN = 128;
   if (d->epilogue == ARIA_EPI_HEADS) {
     ARIA_CHECK_ARG(d->head_dim > 0 && d->head_dim % 8 == 0 && d->head_ld >= d->head_dim && d->n % d->head_dim == 0);
@@ -566,7 +470,9 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   if (b_mn) {
     const uint64_t ncols = swiglu ? 2 * d->n : d->n;
     const uint64_t n_weights = d->group_mod > 0 ? d->group_mod : (d->group_mod < 0 ? d->num_groups / (-d->group_mod) : d->num_groups);
-    rc = b_scale ? make_tmap_2d_u8(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols, 64, BK)
+    // fp8: byte map without swizzle, the 64-byte rows of a box land contiguously for the converters
+    rc = b_scale ? make_tmap_2d(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols, 64, BK, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                CU_TENSOR_MAP_DATA_TYPE_UINT8)
                  : make_tmap_2d(&tmB[0], d->b[0], ncols, n_weights * d->k, ncols * 2, 64, BK);
     if (rc) return rc;
     tmB[1] = tmB[0];
@@ -583,13 +489,12 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
     }
   }
 
-  const int out_bn = swiglu ? BN / 2 : BN;
-  const int64_t n_tiles = (n_out_total + out_bn - 1) / out_bn;
-  const int64_t m_tiles_ub = (d->m + BM - 1) / BM + (d->num_groups > 1 ? d->num_groups : 0);
-  int64_t max_tiles = n_tiles * m_tiles_ub;
-  if (max_tiles > (1 << 30)) max_tiles = 1 << 30;
-
-#define ARIA_LAUNCH(BN_, MN_, EPI_, ...) return launch_gemm<BN_, MN_, EPI_, ##__VA_ARGS__>(tmA, tmB, p, static_cast<int>(max_tiles), stream)
+  const GemmParams p = gemm_params(d, b_scale);
+  const int64_t tiles = max_tiles(d, BN, d->num_groups > 1 ? d->num_groups : 0);
+#define ARIA_LAUNCH(BN_, MN_, EPI_, ...)                                                                                     \
+  return launch_persistent<gemm_kernel<BN_, MN_, EPI_, ##__VA_ARGS__>>("gemm_kernel", GEMM_THREADS,                          \
+                                                                       gemm_smem_bytes<BN_, ##__VA_ARGS__>(), tiles, stream, \
+                                                                       tmA, tmB[0], tmB[1], tmB[2], p)
   if (b_scale) {
     if (swiglu) ARIA_LAUNCH(128, true, ARIA_EPI_SWIGLU, true);
     ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR, true);
@@ -611,23 +516,16 @@ extern "C" int aria_gemm(const aria_gemm_desc_t* d, aria_stream_t stream) {
   return gemm_run(d, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int aria::grouped_gemm(const void* a, const void* b, const float* b_scale, void* out, const int32_t* offsets, int64_t rows,
+                       int64_t k, int64_t n, int32_t groups, int32_t epilogue, cudaStream_t stream) {
+  const aria_gemm_desc_t d = grouped_desc(a, b, out, offsets, rows, k, n, groups, epilogue);
+  return gemm_run(&d, b_scale, stream);
+}
+
 extern "C" int aria_grouped_gemm(const void* a, const void* b, void* out, const int32_t* group_offsets, int64_t rows,
                                  int64_t k, int64_t n, int32_t num_groups, aria_stream_t stream) {
-  aria_gemm_desc_t d{};
-  d.a = a;
-  d.lda = k;
-  d.m = rows;
-  d.n = n;
-  d.k = k;
-  d.b[0] = b;
-  d.n_seg = 1;
-  d.b_layout = ARIA_B_GKN;
-  d.num_groups = num_groups;
-  d.group_offsets = group_offsets;
-  d.epilogue = ARIA_EPI_LINEAR;
-  d.out[0] = out;
-  d.ldo = n;
-  return aria_gemm(&d, stream);
+  return grouped_gemm(a, b, nullptr, out, group_offsets, rows, k, n, num_groups, ARIA_EPI_LINEAR,
+                      reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const float* b_scale, void* out,
@@ -638,21 +536,8 @@ extern "C" int aria_grouped_gemm_fp8(const void* a, const void* b_fp8, const flo
   ARIA_CHECK_ARG(epilogue == ARIA_EPI_LINEAR || epilogue == ARIA_EPI_SWIGLU);
   ARIA_CHECK_ARG((reinterpret_cast<uintptr_t>(a) & 15) == 0 && (reinterpret_cast<uintptr_t>(b_fp8) & 15) == 0 &&
                  (reinterpret_cast<uintptr_t>(b_scale) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0);
-  aria_gemm_desc_t d{};
-  d.a = a;
-  d.lda = k;
-  d.m = rows;
-  d.n = n;
-  d.k = k;
-  d.b[0] = b_fp8;
-  d.n_seg = 1;
-  d.b_layout = ARIA_B_GKN;
-  d.num_groups = num_groups;
-  d.group_offsets = group_offsets;
-  d.epilogue = epilogue;
-  d.out[0] = out;
-  d.ldo = n;
-  return gemm_run(&d, b_scale, reinterpret_cast<cudaStream_t>(stream));
+  return grouped_gemm(a, b_fp8, b_scale, out, group_offsets, rows, k, n, num_groups, epilogue,
+                      reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, const void* b_fp8_nk, const float* b_scale,
@@ -667,45 +552,25 @@ extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, c
                  (reinterpret_cast<uintptr_t>(a_scale) & 3) == 0);
   if (rows == 0) return ARIA_OK;
   const bool swiglu = epilogue == ARIA_EPI_SWIGLU;
-  GemmParams p{};
-  p.M = static_cast<int>(rows);
-  p.N = static_cast<int>(n);
-  p.K = static_cast<int>(k);
-  p.num_groups = num_groups;
-  p.group_offsets = group_offsets;
-  p.n_seg = 1;
-  p.out[0] = static_cast<__nv_bfloat16*>(out);
-  p.ldo = n;
-  p.rows_per_batch = p.M;
-  p.b_scale = b_scale;
+  const aria_gemm_desc_t d = grouped_desc(a_fp8, b_fp8_nk, out, group_offsets, rows, k, n, num_groups, epilogue);
+  const GemmParams p = gemm_params(&d, b_scale);
 
   // UINT8 maps, 128-byte swizzle: a box row is one 128-element k-block
   CUtensorMap tmA, tmB;
-  const uint64_t a_dims[2] = {static_cast<uint64_t>(k), static_cast<uint64_t>(rows)}, b_rows = static_cast<uint64_t>(num_groups) * (swiglu ? 2 * n : n);
-  const uint64_t b_dims[2] = {static_cast<uint64_t>(k), b_rows}, stride[1] = {static_cast<uint64_t>(k)};
-  const uint32_t a_box[2] = {W8_BK, BM}, b_box[2] = {W8_BK, 64};
-  int rc = make_tmap_bf16_swz(&tmA, a_fp8, 2, a_dims, stride, a_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  int rc = make_tmap_2d(&tmA, a_fp8, k, rows, k, W8_BK, BM, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
   if (rc) return rc;
-  rc = make_tmap_bf16_swz(&tmB, b_fp8_nk, 2, b_dims, stride, b_box, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  rc = make_tmap_2d(&tmB, b_fp8_nk, k, num_groups * (swiglu ? 2 * n : n), k, W8_BK, 64, CU_TENSOR_MAP_SWIZZLE_128B,
+                    CU_TENSOR_MAP_DATA_TYPE_UINT8);
   if (rc) return rc;
 
-  const int64_t n_tiles = (n + (swiglu ? 63 : 127)) / (swiglu ? 64 : 128);
-  int64_t max_tiles = n_tiles * ((rows + BM - 1) / BM + num_groups);
-  if (max_tiles > (1 << 30)) max_tiles = 1 << 30;
-  int grid = sm_count();
-  if (max_tiles < grid) grid = static_cast<int>(max_tiles);
+  const int64_t tiles = max_tiles(&d, 128, num_groups);
   constexpr int SMEM = gemm_smem_bytes<128>();
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (swiglu) {
-    static bool attr_set[kMaxDevices] = {};
-    if (ensure_dynamic_smem(attr_set, gemm_w8a8_kernel<ARIA_EPI_SWIGLU>, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
-    gemm_w8a8_kernel<ARIA_EPI_SWIGLU><<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB, p, a_scale);
-  } else {
-    static bool attr_set[kMaxDevices] = {};
-    if (ensure_dynamic_smem(attr_set, gemm_w8a8_kernel<ARIA_EPI_LINEAR>, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
-    gemm_w8a8_kernel<ARIA_EPI_LINEAR><<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB, p, a_scale);
-  }
-  return check_launch("gemm_w8a8_kernel");
+  if (swiglu)
+    return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_SWIGLU>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA,
+                                                                 tmB, p, a_scale);
+  return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_LINEAR>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB,
+                                                              p, a_scale);
 }
 
 extern "C" int aria_abi_version(void) { return 3; }

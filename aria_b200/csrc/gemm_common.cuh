@@ -23,6 +23,7 @@ constexpr int BK = 64;
 constexpr int A_STAGE_BYTES = BM * BK * 2;  // 16 KB
 constexpr int GEMM_THREADS = 384;  // warpgroup 0 TMA producer, warpgroups 1-2 MMA + epilogue (64 rows each)
 constexpr int CONSUMER_WARPS = 8;
+constexpr int acc_ld(int BN) { return BN + 4; }  // staging row stride (floats): 16-byte aligned rows, spread over the banks
 
 struct GemmParams {
   int M, N, K;  // N = output columns per segment
@@ -47,11 +48,75 @@ struct GemmParams {
   const __nv_bfloat16* rope_cos;
   const __nv_bfloat16* rope_sin;
   const int32_t* position_ids;
-  const float* b_scale;  // fp8 B (gemm_kernel<.., B_FP8 = true>): [G, B columns] fp32 scale of each weight column
+  const float* b_scale;  // fp8 B (gemm_kernel<.., B_FP8 = true>, gemm_w8a8_kernel): [G, B columns] fp32 scale of each weight column
 };
 
 ARIA_DEVICE int weight_block(const GemmParams& p, int grp) {
   return p.group_mod > 0 ? grp % p.group_mod : (p.group_mod < 0 ? grp / (-p.group_mod) : grp);
+}
+
+// The dynamic shared memory from its first 1024-byte boundary: the SW128 swizzle pattern repeats every 1024 bytes
+ARIA_DEVICE uint8_t* smem_1024() {
+  extern __shared__ uint8_t smem_raw[];
+  return reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+}
+
+// full / empty mbarrier pairs of a STAGES-slot ring at `at`: full[i] completes when slot i holds its data, empty[i] when its
+// readers have released it.  init() runs on one thread before the block's first barrier.
+template <int STAGES>
+struct BarrierRing {
+  uint64_t* full;
+  uint64_t* empty;
+  ARIA_DEVICE explicit BarrierRing(void* at) : full(static_cast<uint64_t*>(at)), empty(full + STAGES) {}
+  ARIA_DEVICE void init(uint32_t full_arrivals, uint32_t empty_arrivals) const {
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], full_arrivals);
+      mbar_init(&empty[i], empty_arrivals);
+    }
+  }
+};
+
+// A reader's or writer's position in a STAGES-slot ring: the slot, and the barrier phase it waits for there
+template <int STAGES>
+struct RingPos {
+  uint32_t stage = 0, phase = 0;
+  ARIA_DEVICE void next() {
+    const bool wrap = ++stage == STAGES;
+    stage = wrap ? 0 : stage;
+    phase ^= wrap;
+  }
+};
+
+// Column of B that column x of tile n_idx multiplies: BN consecutive columns, or for SwiGLU the gate columns
+// [n_idx BN/2, +BN/2), then the matching up columns, N further on
+template <int BN, int EPI>
+ARIA_DEVICE int tile_b_col(int x, int n_idx, int N) {
+  constexpr int OUT_BN = BN / 2;
+  if constexpr (EPI == ARIA_EPI_SWIGLU) return x < OUT_BN ? n_idx * OUT_BN + x : N + n_idx * OUT_BN + x - OUT_BN;
+  else return n_idx * BN + x;
+}
+
+// A consumer thread: its place in the wgmma accumulator fragment of its warpgroup's 64 rows (cw: warpgroup 1 or 2 -> 0 / 1),
+// and the row it finishes in the epilogue with its `half` of the columns
+struct ConsumerThread {
+  int cw, frag_row, frag_col, epi_row, half;
+};
+ARIA_DEVICE ConsumerThread consumer_thread(int cw, int lane) {
+  const int tid = threadIdx.x & 127;
+  return {cw, cw * 64 + (tid >> 5) * 16 + (lane >> 2), 2 * (lane & 3), cw * 64 + (tid & 63), tid >> 6};
+}
+
+// The scales of this thread's accumulator columns (8 j + frag_col, +1) in tile n_idx of group grp, fetched while the k-loop
+// runs; columns past the weight's end get 0
+template <int BN, int EPI>
+ARIA_DEVICE void load_col_scales(const GemmParams& p, int grp, int n_idx, int frag_col, float2 (&bsc)[BN / 8]) {
+  const int ncols = EPI == ARIA_EPI_SWIGLU ? 2 * p.N : p.N;
+  const float* srow = p.b_scale + static_cast<int64_t>(weight_block(p, grp)) * ncols;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int col = tile_b_col<BN, EPI>(8 * j, n_idx, p.N) + frag_col;
+    bsc[j] = col < ncols ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
+  }
 }
 
 // Monotonic decoder of the persistent tile index -> (group, m-tile, n-tile).  Tiles are ordered group-major,
@@ -367,6 +432,38 @@ ARIA_DEVICE void epilogue_tile(const GemmParams& p, const float* acc, const int 
       }
     }
   }
+}
+
+// Scales applied to the fp32 accumulator as it is staged, before any rounding of the epilogue: none, per B column, or per A
+// row and then per B column
+enum class AccScale { NONE, COL, ROW_COL };
+
+// The end of a consumer warpgroup's tile: stage its fp32 accumulator rows in `stg` ([BM][acc_ld(BN)]), scaled by the column
+// scales `bsc` (load_col_scales) and the row scales of the fragment's two rows `as0` / `as1` as SCALE says, then run the
+// epilogue on this thread's row.
+template <int BN, int EPI, AccScale SCALE>
+ARIA_DEVICE void stage_and_epilogue(const GemmParams& p, float* stg, const ConsumerThread& ct, const float (&acc)[BN / 2],
+                                    const float2 (&bsc)[BN / 8], float as0, float as1, int n_out_total, int grp, int m_idx,
+                                    int n_idx, int row0, int rows) {
+  constexpr int ACC_LD = acc_ld(BN);
+  auto scaled = [](float a, float as, float bs) {
+    if constexpr (SCALE == AccScale::ROW_COL) return a * as * bs;
+    else if constexpr (SCALE == AccScale::COL) return a * bs;
+    else return a;
+  };
+  named_bar_sync(1 + ct.cw, 128);  // the previous tile's epilogue has finished reading this warpgroup's staging rows
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    float* d0 = stg + ct.frag_row * ACC_LD + 8 * j + ct.frag_col;
+    *reinterpret_cast<float2*>(d0) = make_float2(scaled(acc[4 * j], as0, bsc[j].x), scaled(acc[4 * j + 1], as0, bsc[j].y));
+    *reinterpret_cast<float2*>(d0 + 8 * ACC_LD) =
+        make_float2(scaled(acc[4 * j + 2], as1, bsc[j].x), scaled(acc[4 * j + 3], as1, bsc[j].y));
+  }
+  named_bar_sync(1 + ct.cw, 128);
+  const int r_in_grp = m_idx * BM + ct.epi_row;
+  const bool row_ok = r_in_grp < rows;
+  const int64_t grow = static_cast<int64_t>(row0) + r_in_grp;
+  epilogue_tile<BN, EPI>(p, stg + ct.epi_row * ACC_LD, n_out_total, n_idx, grow, row_ok, ct.half, grp, r_in_grp);
 }
 
 }  // namespace aria

@@ -30,19 +30,14 @@ constexpr int WG_STAGE_BYTES = 64 * BM * 2 + 64 * WG_BN * 2;  // A slab [64 rows
 
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const WgradParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + WG_STAGES * WG_STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + WG_STAGES;
+  uint8_t* smem = smem_1024();
+  const BarrierRing<WG_STAGES> bar(smem + WG_STAGES * WG_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
-    for (int i = 0; i < WG_STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], CONSUMER_WARPS);
-    }
+    bar.init(1, CONSUMER_WARPS);
     fence_mbar_init();
   }
   __syncthreads();
@@ -66,8 +61,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (warp == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos<WG_STAGES> rp;
       for (int t = blockIdx.x; t < total; t += gridDim.x) {
         int g, mi, ni;
         decode(t, g, mi, ni);
@@ -76,19 +70,17 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           span(src, g, r0, n);
           const int slabs = (n + 63) / 64;
           for (int s = 0; s < slabs; ++s) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + stage * WG_STAGE_BYTES;
+            mbar_wait(&bar.empty[rp.stage], rp.phase ^ 1);
+            uint8_t* sa = smem + rp.stage * WG_STAGE_BYTES;
             uint8_t* sb = sa + 64 * BM * 2;
-            mbar_arrive_expect_tx(&full_bar[stage], WG_STAGE_BYTES);
+            uint64_t* fb = &bar.full[rp.stage];
+            mbar_arrive_expect_tx(fb, WG_STAGE_BYTES);
             const int row = r0 + s * 64;
 #pragma unroll
-            for (int c = 0; c < BM / 64; ++c) tma_load_2d(sa + c * 8192, &tmA, &full_bar[stage], mi * BM + c * 64, row);
+            for (int c = 0; c < BM / 64; ++c) tma_load_2d(sa + c * 8192, &tmA, fb, mi * BM + c * 64, row);
 #pragma unroll
-            for (int c = 0; c < WG_BN / 64; ++c) tma_load_2d(sb + c * 8192, &tmB, &full_bar[stage], ni * WG_BN + c * 64, row);
-            if (++stage == WG_STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
+            for (int c = 0; c < WG_BN / 64; ++c) tma_load_2d(sb + c * 8192, &tmB, fb, ni * WG_BN + c * 64, row);
+            rp.next();
           }
         }
       }
@@ -99,9 +91,8 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
     // both operands MN-major: A = 64-column chunk cw of the slab (this warpgroup's 64 m), B = both 64-column chunks (LBO 8 KB)
     const uint64_t dA0 = make_smem_desc(smem_u32(smem) + cw * 8192, 8192, 1024);  // stage 0, k-step 0; later ones are + (bytes >> 4)
     const uint64_t dB0 = make_smem_desc(smem_u32(smem) + 64 * BM * 2, 8192, 1024);
-    const int m_frag = cw * 64 + (tid >> 5) * 16 + (lane >> 2), n_frag = 2 * (lane & 3);
-    int stage = 0;
-    uint32_t phase = 0;
+    const ConsumerThread ct = consumer_thread(cw, lane);
+    RingPos<WG_STAGES> rp;
     for (int t = blockIdx.x; t < total; t += gridDim.x) {
       int g, mi, ni;
       decode(t, g, mi, ni);
@@ -114,15 +105,15 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
         span(src, g, r0, n);
         const int slabs = (n + 63) / 64;
         for (int s = 0; s < slabs; ++s) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint64_t da = dA0 + stage * (WG_STAGE_BYTES >> 4), db = dB0 + stage * (WG_STAGE_BYTES >> 4);
+          mbar_wait(&bar.full[rp.stage], rp.phase);
+          const uint64_t da = dA0 + rp.stage * (WG_STAGE_BYTES >> 4), db = dB0 + rp.stage * (WG_STAGE_BYTES >> 4);
           // the last slab of a group: only the 16-row k-steps that reach into the group (rows of the next group share the slab)
           const int valid = n - s * 64;                 // rows of this group in the slab (> 0)
           const int kmax = min(4, (valid + 15) >> 4);
           if (valid < 16 * kmax) {
             // partial last k-step: zero A rows [valid, 16 * kmax) of this warpgroup's chunk (one 128-byte line per row);
             // the proxy fence orders these generic stores before the wgmma reads and before TMA refills the slot
-            uint4* ca = reinterpret_cast<uint4*>(smem + stage * WG_STAGE_BYTES + cw * 8192);
+            uint4* ca = reinterpret_cast<uint4*>(smem + rp.stage * WG_STAGE_BYTES + cw * 8192);
             for (int i = valid * 8 + tid; i < kmax * 128; i += 128) ca[i] = make_uint4(0u, 0u, 0u, 0u);
             fence_proxy_async_smem();
             if (cw == 0) named_bar_sync(1, 128);    // literal ids: ptxas reserves 3 hardware barriers, not all 16
@@ -132,26 +123,23 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
           for (int k = 0; k < kmax; ++k) wgmma_m64n128_ss<1, 1>(acc, da + k * (2048 >> 4), db + k * (2048 >> 4), 1u);
           wgmma_commit();
           wgmma_wait<1>();
-          if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-          prev = stage;
-          if (++stage == WG_STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
+          if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
+          prev = static_cast<int>(rp.stage);
+          rp.next();
         }
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int m = mi * BM + m_frag + 8 * h;
+        const int m = mi * BM + ct.frag_row + 8 * h;
         if (m >= p.Md) continue;
         __nv_bfloat16* orow = p.out + (static_cast<int64_t>(g) * p.Md + m) * p.Nd + ni * WG_BN;
 #pragma unroll
         for (int j = 0; j < WG_BN / 8; ++j) {
           if (ni * WG_BN + 8 * j + 8 <= p.Nd)
-            *reinterpret_cast<uint32_t*>(orow + 8 * j + n_frag) = pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            *reinterpret_cast<uint32_t*>(orow + 8 * j + ct.frag_col) = pack_bf16(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
         }
       }
     }
@@ -182,11 +170,6 @@ extern "C" int aria_grouped_wgrad(const void* a, int64_t lda, const void* b, int
   p.offs = group_offsets;
   p.out = static_cast<__nv_bfloat16*>(out);
   constexpr int SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
-  static bool attr_set[kMaxDevices] = {};
-  if (ensure_dynamic_smem(attr_set, wgrad_kernel, SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
-  const int64_t total = static_cast<int64_t>(num_groups) * ((md + BM - 1) / BM) * ((nd + WG_BN - 1) / WG_BN);
-  int grid = sm_count();
-  if (total < grid) grid = static_cast<int>(total);
-  wgrad_kernel<<<grid, GEMM_THREADS, SMEM, stream>>>(tmA, tmB, p);
-  return check_launch("wgrad_kernel");
+  const int64_t tiles = static_cast<int64_t>(num_groups) * ((md + BM - 1) / BM) * ((nd + WG_BN - 1) / WG_BN);
+  return launch_persistent<wgrad_kernel>("wgrad_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB, p);
 }

@@ -2,7 +2,7 @@
 //
 //   router GEMM + top-k + softmax + histogram (moe_lm.py:190-201, 261-269)  -> aria_router_topk
 //   stable counting sort by expert            (moe_lm.py:313-334)           -> aria_build_permutation, aria_permute_rows
-//   fc1 grouped GEMM + glu, fc2 grouped GEMM  (moe_lm.py:467-525)           -> aria_gemm x 2 (device-resident offsets: no
+//   fc1 grouped GEMM + glu, fc2 grouped GEMM  (moe_lm.py:467-525)           -> grouped_gemm x 2 (device-resident offsets: no
 //                                                                              tokens_per_expert.cpu() sync, moe_lm.py:478)
 //   shared experts                            (moe_lm.py:368-395)           -> aria_gemm x 2 on `side_stream` when given: the
 //                                                                              branch is independent until the final add
@@ -79,7 +79,7 @@ bool w8a8_fits(int64_t R, int32_t d, int32_t I, const BlockWs& ws, W8a8Ws& o) {
 }
 
 // The whole block.  fc1_scale / fc2_scale NULL: bf16 expert weights; given: fc1_w / fc2_w are e4m3 with per-(expert, column)
-// fp32 scales and the two expert GEMMs are aria_grouped_gemm_fp8, or with w8a8 aria_grouped_gemm_w8a8 on K-major weights
+// fp32 scales and the two expert GEMMs run the fp8-weight grouped GEMM, or with w8a8 aria_grouped_gemm_w8a8 on K-major weights
 // ([E, 2I, d] / [E, d, I]) and row-quantised activations.  Every other launch is the same.
 int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
                   const float* fc2_scale, bool w8a8, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
@@ -150,26 +150,11 @@ int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const 
     if ((rc = aria_grouped_gemm_w8a8(at(q.xq), xs, fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, stream))) return rc;
     if ((rc = aria_permute_quantize_fp8_rows(at(ws.h), nullptr, at(q.hq), hs, R, I, stream))) return rc;
     if ((rc = aria_grouped_gemm_w8a8(at(q.hq), hs, fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, stream))) return rc;
-  } else if ((rc = aria_permute_rows(x, src, at(ws.permuted), R, d, stream))) {
-    return rc;
-  } else if (fc1_scale) {
-    if ((rc = aria_grouped_gemm_fp8(at(ws.permuted), fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, stream)))
+  } else {  // bf16 weights, or e4m3 ones with their scales
+    if ((rc = aria_permute_rows(x, src, at(ws.permuted), R, d, stream))) return rc;
+    if ((rc = aria::grouped_gemm(at(ws.permuted), fc1_w, fc1_scale, at(ws.h), offsets, R, d, I, E, ARIA_EPI_SWIGLU, s_main)))
       return rc;
-    if ((rc = aria_grouped_gemm_fp8(at(ws.h), fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, stream))) return rc;
-  } else {
-    aria_gemm_desc_t g;
-    memset(&g, 0, sizeof(g));
-    g.a = at(ws.permuted); g.lda = d; g.m = R; g.n = I; g.k = d;
-    g.b[0] = fc1_w; g.n_seg = 1; g.b_layout = ARIA_B_GKN; g.num_groups = E; g.group_offsets = offsets;
-    g.epilogue = ARIA_EPI_SWIGLU;
-    g.out[0] = at(ws.h); g.ldo = I;
-    if ((rc = aria_gemm(&g, stream))) return rc;
-    memset(&g, 0, sizeof(g));
-    g.a = at(ws.h); g.lda = I; g.m = R; g.n = d; g.k = I;
-    g.b[0] = fc2_w; g.n_seg = 1; g.b_layout = ARIA_B_GKN; g.num_groups = E; g.group_offsets = offsets;
-    g.epilogue = ARIA_EPI_LINEAR;
-    g.out[0] = at(ws.y); g.ldo = d;
-    if ((rc = aria_gemm(&g, stream))) return rc;
+    if ((rc = aria::grouped_gemm(at(ws.h), fc2_w, fc2_scale, at(ws.y), offsets, R, I, d, E, ARIA_EPI_LINEAR, s_main))) return rc;
   }
 
   // ---- join + combine (+ shared)
