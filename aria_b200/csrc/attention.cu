@@ -19,7 +19,11 @@
 //
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
+// aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
+#include <type_traits>
+
 #include "common.cuh"
+#include "fp8.cuh"
 #include "ptx.cuh"
 
 namespace aria {
@@ -375,60 +379,135 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 // the key mask has the row stride mask_stride.  A split that starts past lens[b] sees no key and writes (m = -inf, l = 0,
 // acc = 0); the merge reads the first ceil(lens[b] / DEC_SPLIT_KEYS) splits only, so row b is bit-identical to the host-length
 // launch with Tk = lens[b].
+// KV_FP8: k / v are e4m3 codes [B, H, T_max, 128] with one fp32 scale per (row, head, token) at k_scale / v_scale (strides
+// sc_stride_b / sc_stride_h).  A lane widens its 4 codes per key exactly; the key scale multiplies the reduced dot product and
+// the value weight is pw * v_scale.  Split size, warp -> key assignment and update order are the bf16 kernel's, so with
+// power-of-two scales (both products exact) the result is bit-identical to the bf16 kernel run on the tensors code * scale.
 constexpr int DEC_SPLIT_KEYS = 256;
 
-template <bool DEVLEN>
-__global__ void __launch_bounds__(128) attn_decode_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
-                                                           const __nv_bfloat16* __restrict__ vc, const uint8_t* __restrict__ key_mask,
-                                                           float* __restrict__ ws, int H, int Tk,
-                                                           int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
-                                                           int64_t kv_stride_h, float scale_log2, int splits,
-                                                           const int32_t* __restrict__ lens, int mask_stride) {
+template <bool DEVLEN, bool KV_FP8, typename KV = std::conditional_t<KV_FP8, uint8_t, __nv_bfloat16>>
+__device__ __forceinline__ void decode_partial(const __nv_bfloat16* __restrict__ q, const KV* __restrict__ kc,
+                                               const KV* __restrict__ vc, const float* __restrict__ k_scale,
+                                               const float* __restrict__ v_scale, const uint8_t* __restrict__ key_mask,
+                                               float* __restrict__ ws, int H, int Tk, int64_t q_stride_b, int64_t q_stride_h,
+                                               int64_t kv_stride_b, int64_t kv_stride_h, int64_t sc_stride_b, int64_t sc_stride_h,
+                                               float scale_log2, int splits, const int32_t* __restrict__ lens, int mask_stride) {
   const int bh = blockIdx.x, split = blockIdx.y;
   const int b = bh / H, h = bh % H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int len = DEVLEN ? min(lens[b], Tk) : Tk;
   const int k_begin = split * DEC_SPLIT_KEYS, k_end = min(len, k_begin + DEC_SPLIT_KEYS);
-  const __nv_bfloat16* kbase = kc + b * kv_stride_b + h * kv_stride_h;
-  const __nv_bfloat16* vbase = vc + b * kv_stride_b + h * kv_stride_h;
+  const KV* kbase = kc + b * kv_stride_b + h * kv_stride_h;
+  const KV* vbase = vc + b * kv_stride_b + h * kv_stride_h;
   const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(b) * (DEVLEN ? mask_stride : Tk) : nullptr;
   const uint2 qv = *reinterpret_cast<const uint2*>(q + b * q_stride_b + h * q_stride_h + lane * 4);
   const float q0 = bf16_lo(qv.x) * scale_log2, q1 = bf16_hi(qv.x) * scale_log2, q2 = bf16_lo(qv.y) * scale_log2,
               q3 = bf16_hi(qv.y) * scale_log2;
   float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  for (int k0 = k_begin + warp * 4; k0 < k_end; k0 += 16) {
-    float s[4];
-    uint2 vv[4];
-    bool live[4];
+  if constexpr (!KV_FP8) {
+    for (int k0 = k_begin + warp * 4; k0 < k_end; k0 += 16) {
+      float s[4];
+      uint2 vv[4];
+      bool live[4];
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int kk = k0 + u;
-      live[u] = kk < k_end && !(km && km[kk]);
-      if (live[u]) {
-        const uint2 kv = __ldg(reinterpret_cast<const uint2*>(kbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
-        vv[u] = __ldg(reinterpret_cast<const uint2*>(vbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
-        s[u] = q0 * bf16_lo(kv.x) + q1 * bf16_hi(kv.x) + q2 * bf16_lo(kv.y) + q3 * bf16_hi(kv.y);
-      } else {
-        s[u] = 0.f;
-        vv[u] = make_uint2(0, 0);
+      for (int u = 0; u < 4; ++u) {
+        const int kk = k0 + u;
+        live[u] = kk < k_end && !(km && km[kk]);
+        if (live[u]) {
+          const uint2 kv = __ldg(reinterpret_cast<const uint2*>(kbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
+          vv[u] = __ldg(reinterpret_cast<const uint2*>(vbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
+          s[u] = q0 * bf16_lo(kv.x) + q1 * bf16_hi(kv.x) + q2 * bf16_lo(kv.y) + q3 * bf16_hi(kv.y);
+        } else {
+          s[u] = 0.f;
+          vv[u] = make_uint2(0, 0);
+        }
+      }
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        if (live[u]) {
+          const float m_new = fmaxf(m, s[u]);
+          const float f = exp2f(m - m_new), pw = exp2f(s[u] - m_new);
+          l = l * f + pw;
+          a0 = a0 * f + pw * bf16_lo(vv[u].x);
+          a1 = a1 * f + pw * bf16_hi(vv[u].x);
+          a2 = a2 * f + pw * bf16_lo(vv[u].y);
+          a3 = a3 * f + pw * bf16_hi(vv[u].y);
+          m = m_new;
+        }
       }
     }
+  } else {
+    const float* ksb = k_scale + b * sc_stride_b + h * sc_stride_h;
+    const float* vsb = v_scale + b * sc_stride_b + h * sc_stride_h;
+    // A lane reads 4 + 4 bytes per key, half of what the bf16 loop reads, so the loads of step k0 + 16 are issued before the
+    // arithmetic of step k0 to keep as many bytes in flight per warp.
+    uint32_t kn[4], vn[4];
+    float ksn[4], vsn[4];
+    bool ln[4];
+    auto load = [&](int k0) {
 #pragma unroll
-    for (int o = 16; o; o >>= 1) {
+      for (int u = 0; u < 4; ++u) {
+        const int kk = k0 + u;
+        ln[u] = kk < k_end && !(km && km[kk]);
+        if (ln[u]) {
+          kn[u] = __ldg(reinterpret_cast<const uint32_t*>(kbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
+          vn[u] = __ldg(reinterpret_cast<const uint32_t*>(vbase + static_cast<int64_t>(kk) * AT_D + lane * 4));
+          ksn[u] = __ldg(ksb + kk);
+          vsn[u] = __ldg(vsb + kk);
+        } else {
+          kn[u] = vn[u] = 0u;
+          ksn[u] = vsn[u] = 0.f;
+        }
+      }
+    };
+    load(k_begin + warp * 4);
+    for (int k0 = k_begin + warp * 4; k0 < k_end; k0 += 16) {
+      uint32_t kq[4], vq[4];
+      float ks[4], vs[4], s[4];
+      bool live[4];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
-    }
+      for (int u = 0; u < 4; ++u) {
+        kq[u] = kn[u];
+        vq[u] = vn[u];
+        ks[u] = ksn[u];
+        vs[u] = vsn[u];
+        live[u] = ln[u];
+      }
+      load(k0 + 16);
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      if (live[u]) {
-        const float m_new = fmaxf(m, s[u]);
-        const float f = exp2f(m - m_new), pw = exp2f(s[u] - m_new);
-        l = l * f + pw;
-        a0 = a0 * f + pw * bf16_lo(vv[u].x);
-        a1 = a1 * f + pw * bf16_hi(vv[u].x);
-        a2 = a2 * f + pw * bf16_lo(vv[u].y);
-        a3 = a3 * f + pw * bf16_hi(vv[u].y);
-        m = m_new;
+      for (int u = 0; u < 4; ++u) {
+        if (live[u]) {
+          const float4 c = e4m3x4_to_float4(kq[u]);
+          s[u] = q0 * c.x + q1 * c.y + q2 * c.z + q3 * c.w;
+        } else {
+          s[u] = 0.f;
+        }
+      }
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        if (live[u]) {
+          const float su = s[u] * ks[u];
+          const float m_new = fmaxf(m, su);
+          const float f = exp2f(m - m_new), pw = exp2f(su - m_new);
+          const float pv = pw * vs[u];
+          const float4 c = e4m3x4_to_float4(vq[u]);
+          l = l * f + pw;
+          a0 = a0 * f + pv * c.x;
+          a1 = a1 * f + pv * c.y;
+          a2 = a2 * f + pv * c.z;
+          a3 = a3 * f + pv * c.w;
+          m = m_new;
+        }
       }
     }
   }
@@ -458,6 +537,29 @@ __global__ void __launch_bounds__(128) attn_decode_partial(const __nv_bfloat16* 
     o[AT_D] = M;
     o[AT_D + 1] = L;
   }
+}
+
+template <bool DEVLEN>
+__global__ void __launch_bounds__(128) attn_decode_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
+                                                           const __nv_bfloat16* __restrict__ vc, const uint8_t* __restrict__ key_mask,
+                                                           float* __restrict__ ws, int H, int Tk,
+                                                           int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
+                                                           int64_t kv_stride_h, float scale_log2, int splits,
+                                                           const int32_t* __restrict__ lens, int mask_stride) {
+  decode_partial<DEVLEN, false>(q, kc, vc, nullptr, nullptr, key_mask, ws, H, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, 0,
+                                0, scale_log2, splits, lens, mask_stride);
+}
+
+template <bool DEVLEN>
+__global__ void __launch_bounds__(128) attn_decode_partial_fp8(const __nv_bfloat16* __restrict__ q, const uint8_t* __restrict__ kc,
+                                                               const uint8_t* __restrict__ vc, const float* __restrict__ k_scale,
+                                                               const float* __restrict__ v_scale, const uint8_t* __restrict__ key_mask,
+                                                               float* __restrict__ ws, int H, int Tk, int64_t q_stride_b,
+                                                               int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h,
+                                                               int64_t sc_stride_b, int64_t sc_stride_h, float scale_log2, int splits,
+                                                               const int32_t* __restrict__ lens, int mask_stride) {
+  decode_partial<DEVLEN, true>(q, kc, vc, k_scale, v_scale, key_mask, ws, H, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h,
+                               sc_stride_b, sc_stride_h, scale_log2, splits, lens, mask_stride);
 }
 
 template <bool DEVLEN>
@@ -616,4 +718,50 @@ extern "C" int aria_attention_decode_devlen(const void* q, const void* k, const 
   attn_decode_merge<true><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
                                                      lens, H);
   return check_launch("attn_decode_merge");
+}
+
+// The fp8 entries check what the bf16 ones check, plus the scales, and e4m3 cache strides in multiples of 16 codes (16-byte rows)
+template <bool DEVLEN>
+static int attention_decode_fp8(const void* q, const void* k, const void* v, const float* k_scale, const float* v_scale, void* out,
+                                const uint8_t* key_mask, int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t H,
+                                int32_t Tk, int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h,
+                                int64_t scale_stride_b, int64_t scale_stride_h, float scale, void* workspace,
+                                int64_t workspace_bytes, cudaStream_t stream) {
+  ARIA_CHECK_ARG(q && k && v && k_scale && v_scale && out && workspace && (!DEVLEN || lens));
+  ARIA_CHECK_ARG(B > 0 && H > 0 && Tk > 0 && q_stride_b % 4 == 0 && q_stride_h % 4 == 0);
+  ARIA_CHECK_ARG(kv_stride_b % 16 == 0 && kv_stride_h % 16 == 0 && scale_stride_b >= 0 && scale_stride_h >= 0);
+  ARIA_CHECK_ARG(!DEVLEN || !key_mask || (key_mask_stride >= Tk && key_mask_stride < (1ll << 31)));
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(B, H, Tk));
+  const int splits = (Tk + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
+  dim3 grid(B * H, splits);
+  attn_decode_partial_fp8<DEVLEN><<<grid, 128, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const uint8_t*>(k), static_cast<const uint8_t*>(v), k_scale, v_scale, key_mask,
+      static_cast<float*>(workspace), H, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, scale_stride_b, scale_stride_h,
+      scale * 1.4426950408889634f, splits, lens, static_cast<int>(key_mask_stride));
+  int rc = check_launch("attn_decode_partial_fp8");
+  if (rc) return rc;
+  attn_decode_merge<DEVLEN><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
+                                                       lens, H);
+  return check_launch("attn_decode_merge");
+}
+
+extern "C" int aria_attention_decode_fp8(const void* q, const void* k, const void* v, const float* k_scale, const float* v_scale,
+                                         void* out, const uint8_t* key_mask, int32_t B, int32_t H, int32_t Tk, int64_t q_stride_b,
+                                         int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, int64_t scale_stride_b,
+                                         int64_t scale_stride_h, float scale, void* workspace, int64_t workspace_bytes,
+                                         aria_stream_t stream_) {
+  return attention_decode_fp8<false>(q, k, v, k_scale, v_scale, out, key_mask, 0, nullptr, B, H, Tk, q_stride_b, q_stride_h,
+                                     kv_stride_b, kv_stride_h, scale_stride_b, scale_stride_h, scale, workspace, workspace_bytes,
+                                     reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int aria_attention_decode_devlen_fp8(const void* q, const void* k, const void* v, const float* k_scale, const float* v_scale,
+                                                void* out, const uint8_t* key_mask, int64_t key_mask_stride, const int32_t* lens,
+                                                int32_t B, int32_t H, int32_t T_max, int64_t q_stride_b, int64_t q_stride_h,
+                                                int64_t kv_stride_b, int64_t kv_stride_h, int64_t scale_stride_b,
+                                                int64_t scale_stride_h, float scale, void* workspace, int64_t workspace_bytes,
+                                                aria_stream_t stream_) {
+  return attention_decode_fp8<true>(q, k, v, k_scale, v_scale, out, key_mask, key_mask_stride, lens, B, H, T_max, q_stride_b,
+                                    q_stride_h, kv_stride_b, kv_stride_h, scale_stride_b, scale_stride_h, scale, workspace,
+                                    workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
 }

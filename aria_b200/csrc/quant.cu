@@ -14,12 +14,15 @@
 
 #include "../../include/aria_b200.h"
 #include "common.cuh"
+#include "fp8.cuh"
 
 namespace {
 
+using aria::cast8_e4m3;
+using aria::E4M3_MAX;
+
 constexpr int AMAX_TX = 32;  // threads across the columns of a block (8 columns each: one 16-byte load per row)
 constexpr int AMAX_TY = 8;   // row slices of a block, reduced through shared memory
-constexpr float E4M3_MAX = 448.f;
 
 __global__ void __launch_bounds__(AMAX_TX * AMAX_TY) col_amax_kernel(const __nv_bfloat16* __restrict__ w, float* __restrict__ scale,
                                                                      int K, int N) {
@@ -82,20 +85,6 @@ __global__ void __launch_bounds__(256) cast_e4m3_kernel(const __nv_bfloat16* __r
     }
     *reinterpret_cast<uint2*>(q + row * N + c0) = make_uint2(packed[0], packed[1]);
   }
-}
-
-// 8 bf16 (one 16-byte chunk) / scale -> 8 e4m3 codes, low byte first; IEEE division, round to nearest even, saturating
-__device__ __forceinline__ uint2 cast8_e4m3(const uint4 v, float s) {
-  const uint32_t u[4] = {v.x, v.y, v.z, v.w};
-  uint32_t packed[2] = {0u, 0u};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float x0 = __fdiv_rn(__uint_as_float(u[j] << 16), s);
-    const float x1 = __fdiv_rn(__uint_as_float(u[j] & 0xFFFF0000u), s);
-    const uint32_t pair = __nv_cvt_float2_to_fp8x2(make_float2(x0, x1), __NV_SATFINITE, __NV_E4M3);
-    packed[j >> 1] |= (pair & 0xFFFFu) << (16 * (j & 1));
-  }
-  return make_uint2(packed[0], packed[1]);
 }
 
 // Per-row e4m3 quantisation of the activations of the W8A8 expert GEMMs, fused with the token gather:

@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .moe_lm import AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16
+from .moe_lm import KV_CACHE_DTYPES, AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16
 from .projector import AriaProjector
 from .vision_encoder import AriaVisionConfig, AriaVisionModel
 
@@ -175,8 +175,11 @@ class AriaForConditionalGeneration(nn.Module):
                 use_cache: Optional[bool] = None, output_attentions: Optional[bool] = None,
                 output_hidden_states: Optional[bool] = None, return_dict: Optional[bool] = None,
                 cache_position: Optional[torch.Tensor] = None, num_logits_to_keep: int = 0,
-                max_cache_len: Optional[int] = None, input_ids_host: Optional[torch.Tensor] = None) -> AriaCausalLMOutputWithPast:
-        """Same arguments as the reference forward (modeling_aria.py:194-210); `max_cache_len` / `input_ids_host` are ours.
+                max_cache_len: Optional[int] = None, input_ids_host: Optional[torch.Tensor] = None,
+                kv_cache_dtype: Optional[str] = None) -> AriaCausalLMOutputWithPast:
+        """Same arguments as the reference forward (modeling_aria.py:194-210); `max_cache_len` / `input_ids_host` /
+        `kv_cache_dtype` are ours.  `max_cache_len` and `kv_cache_dtype` ("bf16" or "fp8", default bf16) shape the KV cache
+        forward() creates when no past_key_values is given; a kv_cache_dtype that disagrees with a given cache is a ValueError.
 
         input_ids / pixel_values / pixel_mask may be HOST tensors (pinned for async copies): they are copied to
         the device on the current stream; image-token bookkeeping is then done on the host copy (no device sync).
@@ -191,6 +194,11 @@ class AriaForConditionalGeneration(nn.Module):
         path), return_dict=False."""
         if output_attentions or output_hidden_states:
             raise NotImplementedError("aria_b200: attention weights / per-layer hidden states are not materialised by the fused path")
+        if kv_cache_dtype is not None:
+            if kv_cache_dtype not in KV_CACHE_DTYPES:
+                raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
+            if past_key_values is not None and past_key_values.dtype != kv_cache_dtype:
+                raise ValueError(f"kv_cache_dtype={kv_cache_dtype!r} disagrees with the given {past_key_values.dtype} past_key_values")
         if return_dict is False:
             raise NotImplementedError("aria_b200: tuple outputs are not supported (return_dict=False)")
         if cache_position is not None and past_key_values is not None and int(cache_position.reshape(-1)[0]) != past_key_values.seq_len:
@@ -223,7 +231,7 @@ class AriaForConditionalGeneration(nn.Module):
         B, T, _ = inputs_embeds.shape
         cache = past_key_values
         if cache is None:
-            cache = self.language_model.new_cache(B, max_cache_len or T, dev)
+            cache = self.language_model.new_cache(B, max_cache_len or T, dev, kv_cache_dtype or "bf16")
         key_mask = None
         if attention_mask is not None:
             if attention_mask.shape != (B, cache.seq_len + T):
@@ -278,7 +286,7 @@ class AriaForConditionalGeneration(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None, *,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
-                 pad_token_id=None, seed: int = 0, poll_every: int = 8):
+                 pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16"):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -291,13 +299,17 @@ class AriaForConditionalGeneration(nn.Module):
         eos_token_id: an id or up to 8 ids; a row that emits one is finished and emits pad_token_id (default: the first EOS
         id) from then on, and generation stops once every row is finished, trimmed as GenerationMixin trims it.  The host
         looks at the finished flag every `poll_every` tokens; the result does not depend on it.
+        kv_cache_dtype: "bf16", or "fp8" for e4m3 keys and values with one scale per (row, head, token) (KVCache): the prefill
+        still attends in bf16, every decode step reads the fp8 cache.  GPU only.
         Returns [B, T + generated] int64 on the model's device (prompt ids first)."""
         B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
-                                                   top_p, eos_token_id, pad_token_id, seed, poll_every)
+                                                   top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype)
         dev = self.device
         if dev.type != "cuda":
             if do_sample or eos:
                 raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
+            if kv_cache_dtype == "fp8":
+                raise NotImplementedError("aria_b200: the fp8 KV cache runs on the GPU only")
             return self._generate_stepwise(input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask)
         if do_sample:
             sampling = (float(temperature), int(top_k), float(top_p), int(seed))
@@ -305,11 +317,11 @@ class AriaForConditionalGeneration(nn.Module):
             sampling = (0.0, 0, 1.0, 0)
         # rows are device-driven, so one captured step serves every prompt length of the same 256-row bucket
         T_max = -(-(T + max_new_tokens) // 256) * 256
-        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev)
+        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
         if g is None or g.key != key:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
-            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad)
+            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype)
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
                                                     attention_mask=mask, num_logits_to_keep=1)
@@ -350,7 +362,7 @@ class AriaForConditionalGeneration(nn.Module):
 
     @staticmethod
     def _check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k, top_p, eos_token_id,
-                             pad_token_id, seed, poll_every):
+                             pad_token_id, seed, poll_every, kv_cache_dtype="bf16"):
         """All of generate()'s argument checks, on the host, before any device work -> (B, T, eos ids tuple, pad id)."""
         import math
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -366,6 +378,8 @@ class AriaForConditionalGeneration(nn.Module):
             raise ValueError(f"poll_every must be a positive int, got {poll_every!r}")
         if not isinstance(seed, int) or not 0 <= seed < 2 ** 64:
             raise ValueError(f"seed must be an int in [0, 2**64), got {seed!r}")
+        if kv_cache_dtype not in KV_CACHE_DTYPES:
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
         if do_sample:
             if not (isinstance(temperature, (int, float)) and math.isfinite(temperature) and temperature > 0):
                 raise ValueError(f"temperature must be a strictly positive float, got {temperature!r}")
@@ -397,15 +411,16 @@ class GraphedDecode:
     into it with forward(past_key_values=g.cache), then calls start() and sample_and_advance() for the first token.
     `logits` is the last replayed step's logits [B, 1, V]."""
 
-    def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad):
+    def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
+                 kv_cache_dtype: str = "bf16"):
         from .moe_lm import DecodeState
         dev = model.device
         lm = model.language_model
         c = lm.config
-        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev)
+        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, kv_cache_dtype)
         self.model, self.B, self.T_max = model, B, T_max
         self.sampling, self.eos, self.pad = sampling, eos, pad
-        self.cache = lm.new_cache(B, T_max, dev)
+        self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
         self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
         self.rope = lm.model.rope_tables(T_max, dev)   # held here: the graph reads these tables
         self.ids = torch.zeros(B, 1, dtype=torch.int64, device=dev)

@@ -388,14 +388,34 @@ class MoELayer(nn.Module):
         return self.token_dispatcher.token_unpermutation(expert_output, scores, shared_expert_output)
 
 
-class KVCache:
-    """Static per-layer KV cache in the HF layout [B, H, T_max, head_dim] (modeling_aria.py:49-50)."""
+KV_CACHE_DTYPES = ("bf16", "fp8")
 
-    def __init__(self, n_layers, B, H, T_max, hd, device):
+
+class KVCache:
+    """Static per-layer KV cache in the HF layout [B, H, T_max, head_dim] (modeling_aria.py:49-50).
+
+    dtype "bf16": k[l] / v[l] are bf16.
+    dtype "fp8":  k[l] / v[l] are float8_e4m3fn codes and k_scale[l] / v_scale[l] fp32 [B, H, T_max], one scale per
+                  (row, head, token): scale = amax / 448, code = e4m3(x / scale) (ops.kv_store_fp8).  There is no calibration
+                  data to fix a static scale, and a dynamic scale per 128 values keeps an outlier to its own token and head
+                  for 4 bytes in 132.  One bf16 staging pair k_stage / v_stage [B, H, T_max, head_dim], shared by all layers and
+                  with the strides of `q`, receives the q/k/v projection's k and v rows before they are quantized; a
+                  multi-token forward() attends to it in bf16 (AriaAttention.forward)."""
+
+    def __init__(self, n_layers, B, H, T_max, hd, device, dtype="bf16"):
+        if dtype not in KV_CACHE_DTYPES:
+            raise ValueError(f"KV cache dtype must be 'bf16' or 'fp8', got {dtype!r}")
+        self.dtype = dtype
         # rows >= seq_len are never read (the attention TMA maps cover the valid rows only), so no zero-fill
-        self.k = [torch.empty(B, H, T_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
-        self.v = [torch.empty(B, H, T_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+        kv_dt = torch.float8_e4m3fn if dtype == "fp8" else bf16
+        self.k = [torch.empty(B, H, T_max, hd, dtype=kv_dt, device=device) for _ in range(n_layers)]
+        self.v = [torch.empty(B, H, T_max, hd, dtype=kv_dt, device=device) for _ in range(n_layers)]
         self.q = torch.empty(B, H, T_max, hd, dtype=bf16, device=device)  # rows [seq_len, seq_len+T) used per step
+        if dtype == "fp8":
+            self.k_scale = [torch.empty(B, H, T_max, dtype=torch.float32, device=device) for _ in range(n_layers)]
+            self.v_scale = [torch.empty(B, H, T_max, dtype=torch.float32, device=device) for _ in range(n_layers)]
+            self.k_stage = torch.empty_like(self.q)
+            self.v_stage = torch.empty_like(self.q)
         self.seq_len = 0
         self.T_max = T_max
 
@@ -445,10 +465,27 @@ class AriaAttention(nn.Module):
         kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q = cache.q  # staging buffer with the cache's strides: the fused epilogue scatters q, k, v with one stride pair
         cos, sin = rope
+        fp8 = cache.dtype == "fp8"
+        k_out, v_out = (cache.k_stage, cache.v_stage) if fp8 else (kc, vc)
         ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3,
-                      [q, kc, vc], hd, T, pos0=pos0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=position_ids)
+                      [q, k_out, v_out], hd, T, pos0=pos0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=position_ids)
         Tk = pos0 + T
         scale = hd ** -0.5
+        if fp8:
+            # fp8 cache: a single token is quantized into the cache and attends to it (as decode_step does); a multi-token
+            # step attends in bf16 to the staging pair, holding the dequantized cached rows and its own rows, which are
+            # quantized into the cache afterwards.  A one-chunk prefill thus gives the bf16 cache's logits bit for bit.
+            ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
+            k_st, v_st = cache.k_stage, cache.v_stage
+            if T == 1:
+                ops.kv_store_fp8(k_st[:, :, pos0:Tk], v_st[:, :, pos0:Tk], kc, vc, ks, vs, pos0)
+                o = ops.attention_decode(q[:, :, pos0, :], kc, vc, Tk, scale, key_mask=key_mask, k_scale=ks, v_scale=vs).view(B, 1, d)
+            else:
+                if pos0 > 0:
+                    ops.kv_load_fp8(kc, vc, ks, vs, k_st, v_st, pos0)
+                o = ops.attention(q[:, :, pos0:], k_st, v_st, T, Tk, scale, causal=True, key_mask=key_mask)
+                ops.kv_store_fp8(k_st[:, :, pos0:Tk], v_st[:, :, pos0:Tk], kc, vc, ks, vs, pos0)
+            return ops.linear(o, self.o_proj.weight, residual=residual)
         if T == 1:
             o = ops.attention_decode(q[:, :, pos0, :], kc, vc, Tk, scale, key_mask=key_mask).view(B, 1, d)  # strided view, no copy
         else:  # prefill, or a multi-token continuation (chunked prefill): the queries are the last T of Tk positions
@@ -466,6 +503,12 @@ class AriaAttention(nn.Module):
         cos, sin = rope
         ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3, [q, k, v], hd, 1,
                       pos0=0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=state.rope_pos)
+        if cache.dtype == "fp8":
+            ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
+            ops.kv_append_fp8(k[:, :, 0], v[:, :, 0], kc, vc, ks, vs, state.write_pos)
+            o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask, k_scale=ks,
+                                            v_scale=vs).view(B, 1, d)
+            return ops.linear(o, self.o_proj.weight, residual=residual)
         ops.kv_append(k[:, :, 0], v[:, :, 0], kc, vc, state.write_pos)
         o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
         return ops.linear(o, self.o_proj.weight, residual=residual)
@@ -554,9 +597,14 @@ class AriaMoELMForCausalLM(nn.Module):
         self.vocab_size = config.vocab_size
         self.lm_head = Linear(config.hidden_size, config.vocab_size, device=device)
 
-    def new_cache(self, B, T_max, device):
+    def new_cache(self, B, T_max, device, kv_cache_dtype="bf16"):
+        """A KVCache for B rows of T_max tokens; kv_cache_dtype "fp8" stores K/V as e4m3 with per-token scales (CUDA only)."""
+        if kv_cache_dtype not in KV_CACHE_DTYPES:
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
+        if kv_cache_dtype == "fp8" and torch.device(device).type != "cuda":
+            raise NotImplementedError("aria_b200: the fp8 KV cache runs on the GPU only")
         c = self.config
-        return KVCache(c.num_hidden_layers, B, c.num_attention_heads, T_max, c.head_dim, device)
+        return KVCache(c.num_hidden_layers, B, c.num_attention_heads, T_max, c.head_dim, device, kv_cache_dtype)
 
     # moe_lm.py:663-679: the routers read the coefficients from the shared config object (used by moe_train's router losses)
     def set_z_loss_coeff(self, z_loss_coeff: float):

@@ -714,13 +714,38 @@ def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.
     return dq, dk, dv
 
 
+fp8 = torch.float8_e4m3fn
+
+
+def _fp8_cache_check(k: torch.Tensor, v: torch.Tensor, k_scale: Optional[torch.Tensor], v_scale: Optional[torch.Tensor],
+                     what: str):
+    """An fp8 KV cache: e4m3 k / v [B, H, T_max, 128] with 16-byte rows and fp32 scales k_scale / v_scale [B, H, T_max]."""
+    if k_scale is None or v_scale is None:
+        raise ValueError(f"{what}: an fp8 (float8_e4m3fn) cache needs k_scale= and v_scale=")
+    for t in (k, v):
+        if not (t.is_cuda and t.dtype == fp8 and t.dim() == 4 and t.shape[-1] == 128 and t.stride(-1) == 1 and t.stride(-2) == 128
+                and t.data_ptr() % 16 == 0):
+            raise RuntimeError(f"{what}: fp8 k/v must be CUDA float8_e4m3fn [B,H,T_max,128] with 128-code rows (16-byte aligned)")
+    for t in (k_scale, v_scale):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.shape == k.shape[:3] and t.stride(-1) == 1):
+            raise RuntimeError(f"{what}: k_scale / v_scale must be CUDA float32 [B,H,T_max] with contiguous rows")
+    if k.stride() != v.stride() or k_scale.stride() != v_scale.stride() or v.shape != k.shape:
+        raise RuntimeError(f"{what}: k and v (and their scales) must share shape and strides")
+
+
 def attention_decode(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tk: int, scale: float,
-                     key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     key_mask: Optional[torch.Tensor] = None, k_scale: Optional[torch.Tensor] = None,
+                     v_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q [B,H,128] (any strides with a contiguous last dim, e.g. a row of the q staging buffer), cache k/v
-    [B,H,T_max,128] -> out [B, H*128].  key_mask [B, Tk] uint8, 1 = masked out (padded batch)."""
-    _chk(k), _chk(v)
+    [B,H,T_max,128] -> out [B, H*128].  key_mask [B, Tk] uint8, 1 = masked out (padded batch).
+    With an fp8 cache (k.dtype float8_e4m3fn) k_scale / v_scale [B,H,T_max] fp32 are required and the fp8 kernel runs."""
     if not (q.is_cuda and q.dtype == bf16 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
         raise RuntimeError("attention_decode: q must be a CUDA bf16 tensor with a contiguous last dim")
+    is_fp8 = k.dtype == fp8
+    if is_fp8:
+        _fp8_cache_check(k, v, k_scale, v_scale, "attention_decode")
+    else:
+        _chk(k), _chk(v)
     B, H = q.shape[0], q.shape[1]
     lib = L.load()
     ws_bytes = lib.aria_attention_decode_workspace_bytes(B, H, Tk)
@@ -730,17 +755,29 @@ def attention_decode(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, Tk: int,
         _chk(key_mask, torch.uint8)
         assert key_mask.shape == (B, Tk)
     with torch.cuda.device(q.device):
-        L.check(lib.aria_attention_decode(_p(q), _p(k), _p(v), _p(out), _p(key_mask), B, H, Tk, q.stride(0), q.stride(1), k.stride(0),
-                                          k.stride(1), scale, _p(ws), ws_bytes, _stream(q)), "attention_decode")
+        if is_fp8:
+            L.check(lib.aria_attention_decode_fp8(_p(q), _p(k), _p(v), _p(k_scale), _p(v_scale), _p(out), _p(key_mask), B, H, Tk,
+                                                  q.stride(0), q.stride(1), k.stride(0), k.stride(1), k_scale.stride(0),
+                                                  k_scale.stride(1), scale, _p(ws), ws_bytes, _stream(q)), "attention_decode_fp8")
+        else:
+            L.check(lib.aria_attention_decode(_p(q), _p(k), _p(v), _p(out), _p(key_mask), B, H, Tk, q.stride(0), q.stride(1),
+                                              k.stride(0), k.stride(1), scale, _p(ws), ws_bytes, _stream(q)), "attention_decode")
     return out
 
 
 def attention_decode_devlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, lens: torch.Tensor, scale: float,
-                            key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+                            key_mask: Optional[torch.Tensor] = None, k_scale: Optional[torch.Tensor] = None,
+                            v_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """attention_decode with the key count of each row on the device: row b sees cache rows [0, lens[b]) (lens int32 [B]).
     Cache k/v [B,H,T_max,128]; key_mask [B, >=T_max] uint8 (1 = masked out; any row stride).  Row b is bit-identical to
-    attention_decode(..., Tk=lens[b]); nothing reads the host value of lens, so one captured launch serves every step."""
-    _chk(k), _chk(v), _chk(lens, torch.int32, align=4)
+    attention_decode(..., Tk=lens[b]); nothing reads the host value of lens, so one captured launch serves every step.
+    With an fp8 cache (k.dtype float8_e4m3fn) k_scale / v_scale [B,H,T_max] fp32 are required and the fp8 kernel runs."""
+    is_fp8 = k.dtype == fp8
+    if is_fp8:
+        _fp8_cache_check(k, v, k_scale, v_scale, "attention_decode_devlen")
+    else:
+        _chk(k), _chk(v)
+    _chk(lens, torch.int32, align=4)
     if not (q.is_cuda and q.dtype == bf16 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
         raise RuntimeError("attention_decode_devlen: q must be a CUDA bf16 tensor with a contiguous last dim")
     B, H, T_max = q.shape[0], q.shape[1], k.shape[2]
@@ -756,9 +793,15 @@ def attention_decode_devlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, l
             raise RuntimeError("attention_decode_devlen: key_mask must be CUDA uint8 [B, >= T_max] with contiguous rows")
         mask_stride = key_mask.stride(0)
     with torch.cuda.device(q.device):
-        L.check(lib.aria_attention_decode_devlen(_p(q), _p(k), _p(v), _p(out), _p(key_mask), mask_stride, _p(lens), B, H, T_max,
-                                                 q.stride(0), q.stride(1), k.stride(0), k.stride(1), scale, _p(ws), ws_bytes,
-                                                 _stream(q)), "attention_decode_devlen")
+        if is_fp8:
+            L.check(lib.aria_attention_decode_devlen_fp8(_p(q), _p(k), _p(v), _p(k_scale), _p(v_scale), _p(out), _p(key_mask),
+                                                         mask_stride, _p(lens), B, H, T_max, q.stride(0), q.stride(1), k.stride(0),
+                                                         k.stride(1), k_scale.stride(0), k_scale.stride(1), scale, _p(ws), ws_bytes,
+                                                         _stream(q)), "attention_decode_devlen_fp8")
+        else:
+            L.check(lib.aria_attention_decode_devlen(_p(q), _p(k), _p(v), _p(out), _p(key_mask), mask_stride, _p(lens), B, H, T_max,
+                                                     q.stride(0), q.stride(1), k.stride(0), k.stride(1), scale, _p(ws), ws_bytes,
+                                                     _stream(q)), "attention_decode_devlen")
     return out
 
 
@@ -802,6 +845,61 @@ def kv_append(k_new: torch.Tensor, v_new: torch.Tensor, k_cache: torch.Tensor, v
     with torch.cuda.device(k_cache.device):
         L.check(L.load().aria_kv_append(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_cache), _p(v_cache),
                                         k_cache.stride(0), k_cache.stride(1), _p(pos), B, H, T_max, _stream(k_cache)), "kv_append")
+
+
+def _bf16_rows_check(ts, what: str):
+    for t in ts:
+        if not (t.is_cuda and t.dtype == bf16 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0
+                and (t.dim() == 3 or t.stride(-2) == 128)):
+            raise RuntimeError(f"{what}: bf16 rows must be CUDA bf16 with 128 contiguous, 16-byte aligned elements per row")
+    if ts[0].stride() != ts[1].stride() or ts[0].shape != ts[1].shape:
+        raise RuntimeError(f"{what}: the k and v rows must share shape and strides")
+
+
+def kv_store_fp8(k_src: torch.Tensor, v_src: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Tensor,
+                 v_scale: torch.Tensor, row0: int):
+    """Quantise bf16 rows k_src / v_src [B, H, n, 128] (row stride 128, e.g. rows of the staging pair) into fp8 cache rows
+    [row0, row0 + n): one fp32 scale per (row, head, token) = amax / 448 (1 for an all-zero row), codes e4m3(x / scale), bit for
+    bit `(x.float() / scale[..., None]).to(torch.float8_e4m3fn)`."""
+    _fp8_cache_check(k_cache, v_cache, k_scale, v_scale, "kv_store_fp8")
+    _bf16_rows_check((k_src, v_src), "kv_store_fp8")
+    B, H, T_max = k_cache.shape[:3]
+    n = k_src.shape[2]
+    if k_src.shape != (B, H, n, 128) or not 0 <= row0 <= T_max - n:
+        raise ValueError(f"kv_store_fp8: rows {tuple(k_src.shape)} at row {row0} do not fit a cache of {tuple(k_cache.shape)}")
+    with torch.cuda.device(k_cache.device):
+        L.check(L.load().aria_kv_store_fp8(_p(k_src), _p(v_src), k_src.stride(0), k_src.stride(1), _p(k_cache), _p(v_cache),
+                                           _p(k_scale), _p(v_scale), k_cache.stride(0), k_cache.stride(1), k_scale.stride(0),
+                                           k_scale.stride(1), row0, n, B, H, T_max, _stream(k_cache)), "kv_store_fp8")
+
+
+def kv_append_fp8(k_new: torch.Tensor, v_new: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Tensor,
+                  v_scale: torch.Tensor, pos: torch.Tensor):
+    """kv_append for the fp8 cache: quantise k_new / v_new [B, H, 128] into cache row pos[b] (int32 [B] on the device) with the
+    quantiser of kv_store_fp8, so the row gets the same codes and scale as kv_store_fp8 would give it."""
+    _fp8_cache_check(k_cache, v_cache, k_scale, v_scale, "kv_append_fp8")
+    _bf16_rows_check((k_new, v_new), "kv_append_fp8")
+    _chk(pos, torch.int32, align=4)
+    B, H, T_max = k_cache.shape[:3]
+    assert k_new.shape == (B, H, 128) and pos.shape == (B,)
+    with torch.cuda.device(k_cache.device):
+        L.check(L.load().aria_kv_append_fp8(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_cache), _p(v_cache),
+                                            _p(k_scale), _p(v_scale), k_cache.stride(0), k_cache.stride(1), k_scale.stride(0),
+                                            k_scale.stride(1), _p(pos), B, H, T_max, _stream(k_cache)), "kv_append_fp8")
+
+
+def kv_load_fp8(k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor, k_out: torch.Tensor,
+                v_out: torch.Tensor, n: int):
+    """Dequantise fp8 cache rows [0, n) into bf16 k_out / v_out [B, H, >= n, 128] (row stride 128): bf16(code.float() * scale)."""
+    _fp8_cache_check(k_cache, v_cache, k_scale, v_scale, "kv_load_fp8")
+    _bf16_rows_check((k_out, v_out), "kv_load_fp8")
+    B, H, T_max = k_cache.shape[:3]
+    if k_out.shape[:2] != (B, H) or k_out.shape[2] < n or not 0 < n <= T_max:
+        raise ValueError(f"kv_load_fp8: {n} rows of a cache of {tuple(k_cache.shape)} do not fit {tuple(k_out.shape)}")
+    with torch.cuda.device(k_cache.device):
+        L.check(L.load().aria_kv_load_fp8(_p(k_cache), _p(v_cache), _p(k_scale), _p(v_scale), k_cache.stride(0), k_cache.stride(1),
+                                          k_scale.stride(0), k_scale.stride(1), _p(k_out), _p(v_out), k_out.stride(0),
+                                          k_out.stride(1), n, B, H, T_max, _stream(k_cache)), "kv_load_fp8")
 
 
 def decode_advance(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: torch.Tensor, step: torch.Tensor,

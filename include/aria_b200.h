@@ -336,6 +336,21 @@ int aria_attention_decode_devlen(const void* q, const void* k, const void* v, vo
                                  int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t H, int32_t T_max,
                                  int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
                                  void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* aria_attention_decode / aria_attention_decode_devlen over an fp8 KV cache: k, v are e4m3 codes [B,H,T_max,128] (element = byte
+ * strides kv_stride_b / kv_stride_h, multiples of 16), k_scale / v_scale fp32 [B,H,T_max] at scale_stride_b / scale_stride_h, one
+ * scale per (row, head, token): key t of (b, h) is code * scale.  The key scale multiplies the reduced dot product q.code and the
+ * value weight is p * v_scale.  Same split size, key assignment and update order as the bf16 kernels, so with power-of-two
+ * scales the output is bit-identical to the bf16 entry run on the bf16 tensors code * scale.  Same workspace query, same
+ * key_mask / lens contracts (rows at or past lens[b] are never read). */
+int aria_attention_decode_fp8(const void* q, const void* k, const void* v, const float* k_scale, const float* v_scale, void* out,
+                              const uint8_t* key_mask, int32_t B, int32_t H, int32_t Tk, int64_t q_stride_b, int64_t q_stride_h,
+                              int64_t kv_stride_b, int64_t kv_stride_h, int64_t scale_stride_b, int64_t scale_stride_h, float scale,
+                              void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+int aria_attention_decode_devlen_fp8(const void* q, const void* k, const void* v, const float* k_scale, const float* v_scale,
+                                     void* out, const uint8_t* key_mask, int64_t key_mask_stride, const int32_t* lens, int32_t B,
+                                     int32_t H, int32_t T_max, int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
+                                     int64_t kv_stride_h, int64_t scale_stride_b, int64_t scale_stride_h, float scale,
+                                     void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Generation: sampling, KV append, decode-state advance (one decode step has no host integer in it)
@@ -360,6 +375,26 @@ int aria_sample_tokens(const void* logits, int64_t logits_stride, int64_t* next_
 int aria_kv_append(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_cache, void* v_cache,
                    int64_t cache_stride_b, int64_t cache_stride_h, const int32_t* pos, int32_t B, int32_t H, int32_t T_max,
                    aria_stream_t stream);
+/* fp8 KV cache: e4m3 codes k_cache / v_cache [B, H, T_max, 128] (element = byte strides cache_stride_b / cache_stride_h, multiples
+ * of 16) and fp32 scales k_scale / v_scale [B, H, T_max] (strides scale_stride_b / scale_stride_h), one per (row, head, token):
+ *   scale = max |x| / 448 (IEEE division; an all-zero row gets 1), code = e4m3(x / scale) (round to nearest even, saturating),
+ * bit for bit (x.float() / scale[..., None]).to(torch.float8_e4m3fn).  bf16 sources / outputs have 128-element rows at strides
+ * that are multiples of 8 elements.  The store and the append share one device quantiser, so a row gets the same bits from both.
+ * aria_kv_store_fp8: source rows [0, n_rows) ([B, H, n_rows, 128]) -> cache rows [row0, row0 + n_rows) (row0 + n_rows <= T_max). */
+int aria_kv_store_fp8(const void* k_src, const void* v_src, int64_t src_stride_b, int64_t src_stride_h, void* k_cache, void* v_cache,
+                      float* k_scale, float* v_scale, int64_t cache_stride_b, int64_t cache_stride_h, int64_t scale_stride_b,
+                      int64_t scale_stride_h, int32_t row0, int32_t n_rows, int32_t B, int32_t H, int32_t T_max, aria_stream_t stream);
+/* aria_kv_append for the fp8 cache: k_new / v_new [B, H, 128] -> cache row pos[b] (device int32 [B]); a row outside [0, T_max)
+ * is not written. */
+int aria_kv_append_fp8(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_cache, void* v_cache,
+                       float* k_scale, float* v_scale, int64_t cache_stride_b, int64_t cache_stride_h, int64_t scale_stride_b,
+                       int64_t scale_stride_h, const int32_t* pos, int32_t B, int32_t H, int32_t T_max, aria_stream_t stream);
+/* Dequantise cache rows [0, n_rows) (n_rows <= T_max) into bf16 k_out / v_out [B, H, >= n_rows, 128]: bf16(code * scale), the
+ * fp32 product rounded to nearest even. */
+int aria_kv_load_fp8(const void* k_cache, const void* v_cache, const float* k_scale, const float* v_scale, int64_t cache_stride_b,
+                     int64_t cache_stride_h, int64_t scale_stride_b, int64_t scale_stride_h, void* k_out, void* v_out,
+                     int64_t out_stride_b, int64_t out_stride_h, int32_t n_rows, int32_t B, int32_t H, int32_t T_max,
+                     aria_stream_t stream);
 /* Decode-state advance after aria_sample_tokens, one launch (B <= 1024), all state in device memory:
  *   t = *step; tok[b] = finished[b] ? pad_token_id : next_ids[b]; out_tokens[b * max_steps + t] = tok[b] (if t < max_steps);
  *   ids_in[b] = tok[b]; finished[b] |= tok[b] is one of eos_ids (HOST array of n_eos <= 8 ids, copied at the call);
