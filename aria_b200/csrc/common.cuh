@@ -149,6 +149,43 @@ inline int launch_persistent(const char* name, int threads, int smem, int64_t ma
   return check_launch(name);
 }
 
+// Launches a persistent kernel as clusters of two CTAs along x (one CTA per SM): as many clusters as the device holds at once,
+// fewer when there are fewer than `max_pairs` tile pairs.  How many fit is asked once per device: a GPC with an odd number of
+// free SMs can leave one of them out.
+template <auto kernel, typename... Args>
+inline int launch_persistent_pairs(const char* name, int threads, int smem, int64_t max_pairs, cudaStream_t stream,
+                                   const Args&... args) {
+  static bool attr_set[kMaxDevices] = {};
+  static int max_clusters[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  cudaLaunchAttribute attr{};
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(2);
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  const int dev = current_device();
+  if (!max_clusters[dev]) {
+    int n = 0;
+    const cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kernel, &cfg);
+    if (e != cudaSuccess || n < 1) {
+      fprintf(stderr, "aria_b200: cudaOccupancyMaxActiveClusters(%s) = %d: %s\n", name, n, cudaGetErrorString(e));
+      return ARIA_ERR_CUDA;
+    }
+    max_clusters[dev] = n;
+  }
+  const int64_t clusters = max_pairs < max_clusters[dev] ? (max_pairs > 1 ? max_pairs : 1) : max_clusters[dev];
+  cfg.gridDim = dim3(static_cast<unsigned>(2 * clusters));
+  cudaLaunchKernelEx(&cfg, kernel, args...);  // its error, if any, is the one check_launch reads
+  return check_launch(name);
+}
+
 // Grouped expert GEMM (gemm.cu): out[rows, n] = a[rows, k] x b[g] for the rows of group g (`offsets`), b = [groups, k, n]
 // bf16, or e4m3 with one fp32 scale per (group, column) when b_scale is given.  `epilogue`: LINEAR or SWIGLU.
 int grouped_gemm(const void* a, const void* b, const float* b_scale, void* out, const int32_t* offsets, int64_t rows,

@@ -12,6 +12,8 @@ constexpr int GEMM_STAGES = 4;
 // stages and the fp32 staging tile (DESIGN §3); a fourth would not.
 constexpr int FP8_LAND_STAGES = 3;
 constexpr int FP8_CONVERT_WARPS = 3;
+// Fewest rows of a dense LINEAR GEMM that runs as CTA pairs (gemm_run)
+constexpr int PAIR_MIN_ROWS = 2048;
 template <int BN, bool B_FP8 = false>
 constexpr int gemm_smem_bytes() {
   return 1024 /*align*/ + GEMM_STAGES * (A_STAGE_BYTES + BN * BK * 2) + BM * acc_ld(BN) * 4 + 256 /*barriers*/ +
@@ -37,13 +39,29 @@ ARIA_DEVICE void e4m3x16_to_bf16(const uint4 v, uint4& lo, uint4& hi) {
   hi = make_uint4(o[4], o[5], o[6], o[7]);
 }
 
+// The persistent loop of a CTA: tiles blockIdx.x, + gridDim.x, ...  PAIR: both CTAs of a cluster walk the same pair indices,
+// so their trip counts are identical, and the scheduler's n-tiles are n-pairs
+template <bool PAIR> ARIA_DEVICE int first_tile() { return PAIR ? blockIdx.x >> 1 : blockIdx.x; }
+template <bool PAIR> ARIA_DEVICE int tile_step() { return PAIR ? gridDim.x >> 1 : gridDim.x; }
+template <bool PAIR> ARIA_DEVICE int pair_sched_n(int n_tiles) { return PAIR ? (n_tiles + 1) / 2 : n_tiles; }
+
 template <int BN, bool B_MN>
 ARIA_DEVICE void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
   if constexpr (BN == 128) wgmma_m64n128_ss<0, B_MN ? 1 : 0>(acc, da, db, 1u);
   else wgmma_m64n144_ss<0, B_MN ? 1 : 0>(acc, da, db, 1u);
 }
 
-template <int BN, bool B_MN, int EPI, bool B_FP8 = false>
+// PAIR: the kernel runs as clusters of two CTAs that take n-tiles 2 j and 2 j + 1 of the same m-tile (pair j).  Each CTA loads
+// one 64-row half of the shared A tile and multicasts it into both CTAs' ring; each loads its own B.  Per CTA and k-block that
+// is (64 + BN) x 64 instead of (128 + BN) x 64 elements from L2.  Protocol (DESIGN §3):
+//   * full[s] of each CTA expects the whole stage, its own B and both A halves; its producer's expect_tx is the one arrival
+//     (the peer's half may land first).
+//   * empty[s] of each CTA counts the consumer warps of BOTH CTAs: no producer multicasts into a slot its peer still reads.
+//   * with an odd n-tile count the last pair's second tile is a phantom: its CTA loads and multicasts its A half, waits for
+//     and releases every stage like the others, and loads no B, issues no MMA and stores nothing.
+//   * cluster barriers after the barrier init (before any remote access) and before exit (no CTA leaves while its peer can
+//     still write its shared memory or arrive on its barriers).
+template <int BN, bool B_MN, int EPI, bool B_FP8 = false, bool PAIR = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
             const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
@@ -54,6 +72,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
   static_assert(BN == 128 || BN == 144, "tile widths with a wgmma wrapper");
   static_assert(!B_FP8 || (B_MN && BN == 128 && EPI != ARIA_EPI_HEADS), "fp8 B: grouped [G, K, N] weights, 128-wide tiles");
+  static_assert(!PAIR || (!B_MN && !B_FP8), "CTA pairs: dense K-major bf16 B");
   constexpr int LAND_BYTES = BN * BK;  // one k-block of fp8 B: BN/64 boxes of 64 k-rows x 64 bytes, unswizzled
 
   uint8_t* smem = smem_1024();
@@ -74,11 +93,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(&tmB1);
     if (p.n_seg > 2) prefetch_tmap(&tmB2);
     // B_FP8: a stage is full once A has landed AND every converter warp has written its share of B
-    bar.init(B_FP8 ? 1 + FP8_CONVERT_WARPS : 1, CONSUMER_WARPS);
+    bar.init(B_FP8 ? 1 + FP8_CONVERT_WARPS : 1, PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
     if constexpr (B_FP8) land_bar.init(1, FP8_CONVERT_WARPS);
     fence_mbar_init();
   }
-  __syncthreads();
+  if constexpr (PAIR) cluster_sync();
+  else __syncthreads();
 
   const int n_out_total = p.N * (EPI == ARIA_EPI_SWIGLU ? 1 : p.n_seg);  // output columns overall
   const int n_tiles = (n_out_total + OUT_BN - 1) / OUT_BN;
@@ -90,14 +110,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     // =========================== TMA producer ===========================
     setmaxnreg_dec<40>();
     if (warp == 0 && elect_one()) {
+      const uint32_t rank = PAIR ? cluster_ctarank() : 0;
       TileSched sched;
-      sched.init(p, n_tiles);
+      sched.init(p, pair_sched_n<PAIR>(n_tiles));
       RingPos<STAGES> rp;
       RingPos<FP8_LAND_STAGES> lp;  // B_FP8 landing ring
-      for (int t = blockIdx.x;; t += gridDim.x) {
+      for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
         int grp, m_idx, n_idx, row0, rows;
         if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+        if constexpr (PAIR) n_idx = 2 * n_idx + rank;
+        const bool phantom = PAIR && n_idx >= n_tiles;
         const int a_row = row0 + m_idx * BM;
+        // PAIR: this CTA's half of the A tile; a half wholly past the last row is never read back, so the box is moved onto
+        // the first half rather than issued out of bounds
+        const int a_half_row = a_row + (m_idx * BM + static_cast<int>(rank) * (BM / 2) < rows ? rank * (BM / 2) : 0);
         const int bgrp = weight_block(p, grp);
         // B coordinates of this tile (k-invariant part)
         int b_c0 = 0, b_c1 = 0;          // K-major: row (n) coordinate of the two boxes; MN-major: base k row
@@ -118,8 +144,17 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           const uint32_t sa = smem_base + rp.stage * STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
           mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
-          mbar_arrive_expect_tx_addr(fb, B_FP8 ? A_STAGE_BYTES : STAGE_BYTES);
-          tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
+          if constexpr (PAIR) {
+            mbar_arrive_expect_tx_addr(fb, phantom ? A_STAGE_BYTES : STAGE_BYTES);
+            tma_load_2d_multicast_addr(sa + rank * (A_STAGE_BYTES / 2), &tmA, fb, kb * BK, a_half_row, 0b11);
+            if (phantom) {
+              rp.next();
+              continue;
+            }
+          } else {
+            mbar_arrive_expect_tx_addr(fb, B_FP8 ? A_STAGE_BYTES : STAGE_BYTES);
+            tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
+          }
           if constexpr (B_MN) {
             // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n, BN/64 boxes per stage
             uint32_t dst = sb, box_bytes = 64 * BK * 2, bar_addr = fb;
@@ -198,12 +233,31 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
     const uint64_t db0 = make_smem_desc(smem_base + A_STAGE_BYTES, b_lbo, b_sbo);
     const ConsumerThread ct = consumer_thread(cw, lane);
+    const uint32_t rank = PAIR ? cluster_ctarank() : 0;
     TileSched sched;
-    sched.init(p, n_tiles);
+    sched.init(p, pair_sched_n<PAIR>(n_tiles));
     RingPos<STAGES> rp;
-    for (int t = blockIdx.x;; t += gridDim.x) {
+    // a stage is released to this CTA's producer and, PAIR, to the peer's, whose A half also lands in it
+    auto release = [&](int s) {
+      if (lane == 0) {
+        mbar_arrive(&bar.empty[s]);
+        if constexpr (PAIR) mbar_arrive_cluster(&bar.empty[s], rank ^ 1);
+      }
+    };
+    for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
       int grp, m_idx, n_idx, row0, rows;
       if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+      if constexpr (PAIR) {
+        n_idx = 2 * n_idx + rank;
+        if (n_idx >= n_tiles) {  // phantom tile: consume every stage the peer's multicast fills, compute nothing
+          for (int kb = 0; kb < k_blocks; ++kb) {
+            mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+            release(rp.stage);
+            rp.next();
+          }
+          continue;
+        }
+      }
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -220,17 +274,18 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         for (int k = 0; k < BK / 16; ++k) wgmma_tile_k16<BN, B_MN>(acc, da + k * 2, db + k * b_kadv);
         wgmma_commit();
         wgmma_wait<1>();
-        if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
+        if (prev >= 0) release(prev);
         prev = static_cast<int>(rp.stage);
         rp.next();
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (prev >= 0 && lane == 0) mbar_arrive(&bar.empty[prev]);
+      if (prev >= 0) release(prev);
       stage_and_epilogue<BN, EPI, B_FP8 ? AccScale::COL : AccScale::NONE>(p, stg, ct, acc, bsc, 1.f, 1.f, n_out_total, grp,
                                                                            m_idx, n_idx, row0, rows);
     }
   }
+  if constexpr (PAIR) cluster_sync();
 }
 
 // W8A8 grouped GEMM: e4m3 A [rows, K] with one fp32 scale per row, e4m3 B [G * N_b, K] (K-major: fp8 wgmma has no transpose)
@@ -462,10 +517,16 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
     if (d->n_seg > 1 && !swiglu) ARIA_CHECK_ARG(d->n % BN == 0);
   }
 
+  // Dense bf16 LINEAR GEMMs with nn.Linear weights and at least PAIR_MIN_ROWS rows run as CTA pairs that share their A tile
+  // (gemm_kernel<.., PAIR>).  Measured on an H100 SXM at 700 W (DESIGN §6): the ViT's 4,900-row o_proj / fc1 / fc2 gain
+  // 3-12 %, while the LM's 768-row GEMMs and the 144-wide HEADS tiles lose 5-16 %, so those keep the one-CTA kernel.
+  const bool pair = !b_scale && d->b_layout == ARIA_B_NK && d->num_groups == 1 && !d->group_offsets &&
+                    d->epilogue == ARIA_EPI_LINEAR && d->m >= PAIR_MIN_ROWS;
+
   CUtensorMap tmA, tmB[3];
   // a_rows: rows of the A buffer when groups live in fixed-capacity regions (m is then the EXPECTED row count that the
-  // kernel-selection heuristics above use; the tensor map must cover the whole buffer)
-  int rc = make_tmap_2d(&tmA, d->a, d->k, d->a_rows > 0 ? d->a_rows : d->m, d->lda * 2, BK, BM);
+  // kernel-selection heuristics above use; the tensor map must cover the whole buffer).  Pairs: one box is a 64-row half.
+  int rc = make_tmap_2d(&tmA, d->a, d->k, d->a_rows > 0 ? d->a_rows : d->m, d->lda * 2, BK, pair ? BM / 2 : BM);
   if (rc) return rc;
   if (b_mn) {
     const uint64_t ncols = swiglu ? 2 * d->n : d->n;
@@ -491,6 +552,11 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
 
   const GemmParams p = gemm_params(d, b_scale);
   const int64_t tiles = max_tiles(d, BN, d->num_groups > 1 ? d->num_groups : 0);
+  if (pair) {
+    const int64_t m_tiles = (d->m + BM - 1) / BM, pairs = (tiles / m_tiles + 1) / 2 * m_tiles;
+    return launch_persistent_pairs<gemm_kernel<128, false, ARIA_EPI_LINEAR, false, true>>(
+        "gemm_kernel", GEMM_THREADS, gemm_smem_bytes<128>(), pairs, stream, tmA, tmB[0], tmB[1], tmB[2], p);
+  }
 #define ARIA_LAUNCH(BN_, MN_, EPI_, ...)                                                                                     \
   return launch_persistent<gemm_kernel<BN_, MN_, EPI_, ##__VA_ARGS__>>("gemm_kernel", GEMM_THREADS,                          \
                                                                        gemm_smem_bytes<BN_, ##__VA_ARGS__>(), tiles, stream, \

@@ -314,123 +314,105 @@ ARIA_DEVICE void epilogue_tile(const GemmParams& p, const float* acc, const int 
         }
       }
     }
-  } else {  // ARIA_EPI_HEADS
+  } else {  // ARIA_EPI_HEADS, a RoPE segment (the others go through heads_store_tile)
     const int col0 = n_idx * BN;
     const int seg = col0 / p.N;
     const int cseg0 = col0 - seg * p.N;
-    const __nv_bfloat16* bias = p.bias[seg];
     const int b = static_cast<int>(grow / p.rows_per_batch);
     const int tok = static_cast<int>(grow - static_cast<int64_t>(b) * p.rows_per_batch);
     __nv_bfloat16* obase = p.out[seg] + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld;
-    const bool rope = (p.rope_mask >> seg) & 1;
-    if (rope) {
-      // head_dim == 128 and BN a multiple of it: the tile holds BN/128 whole heads. rotate-half RoPE with op-by-op
-      // bf16 rounding:  out = bf16(bf16(x*cos) + bf16(rotate_half(x)*sin))
-      const int pos = row_ok ? (p.position_ids ? p.position_ids[grow] : p.pos0 + tok) : 0;
-      const __nv_bfloat16* cs = p.rope_cos + static_cast<int64_t>(pos) * p.head_dim;
-      const __nv_bfloat16* sn = p.rope_sin + static_cast<int64_t>(pos) * p.head_dim;
-      constexpr int NHC = BN / 64;
+    // head_dim == 128 and BN a multiple of it: the tile holds BN/128 whole heads. rotate-half RoPE with op-by-op
+    // bf16 rounding:  out = bf16(bf16(x*cos) + bf16(rotate_half(x)*sin))
+    const int pos = row_ok ? (p.position_ids ? p.position_ids[grow] : p.pos0 + tok) : 0;
+    const __nv_bfloat16* cs = p.rope_cos + static_cast<int64_t>(pos) * p.head_dim;
+    const __nv_bfloat16* sn = p.rope_sin + static_cast<int64_t>(pos) * p.head_dim;
+    constexpr int NHC = BN / 64;
 #pragma unroll 1
-      for (int hc = half * NHC / 2; hc < (half ? NHC : NHC / 2); hc += 1) {
-        // hc enumerates (head-in-tile, 32-column chunk of the low half): hh = hc / 2, c = (hc & 1) * 32
-        const int hh = hc >> 1, c = (hc & 1) * 32;
-        __nv_bfloat16* orow = obase + (cseg0 / p.head_dim + hh) * p.stride_h;
-        const float* th = acc + hh * 128;
-        uint32_t lo[32], hi[32];
-        ld_acc32(th + c, lo);
-        ld_acc32(th + 64 + c, hi);
-        // all 16 table vectors of this chunk are requested before anything waits (they were loaded one group at a time
-        // inside the loop below, each followed by its use)
-        uint4 tc_lo[4], ts_lo[4], tc_hi[4], ts_hi[4];
+    for (int hc = half * NHC / 2; hc < (half ? NHC : NHC / 2); hc += 1) {
+      // hc enumerates (head-in-tile, 32-column chunk of the low half): hh = hc / 2, c = (hc & 1) * 32
+      const int hh = hc >> 1, c = (hc & 1) * 32;
+      __nv_bfloat16* orow = obase + (cseg0 / p.head_dim + hh) * p.stride_h;
+      const float* th = acc + hh * 128;
+      uint32_t lo[32], hi[32];
+      ld_acc32(th + c, lo);
+      ld_acc32(th + 64 + c, hi);
+      // all 16 table vectors of this chunk are requested before anything waits (they were loaded one group at a time
+      // inside the loop below, each followed by its use)
+      uint4 tc_lo[4], ts_lo[4], tc_hi[4], ts_hi[4];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          tc_lo[q] = __ldg(reinterpret_cast<const uint4*>(cs + c + q * 8));
-          ts_lo[q] = __ldg(reinterpret_cast<const uint4*>(sn + c + q * 8));
-          tc_hi[q] = __ldg(reinterpret_cast<const uint4*>(cs + 64 + c + q * 8));
-          ts_hi[q] = __ldg(reinterpret_cast<const uint4*>(sn + 64 + c + q * 8));
-        }
-        if (row_ok) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const uint4 c_lo = tc_lo[q], s_lo = ts_lo[q], c_hi = tc_hi[q], s_hi = ts_hi[q];
-            const uint32_t cl[4] = {c_lo.x, c_lo.y, c_lo.z, c_lo.w}, sl[4] = {s_lo.x, s_lo.y, s_lo.z, s_lo.w};
-            const uint32_t ch[4] = {c_hi.x, c_hi.y, c_hi.z, c_hi.w}, sh[4] = {s_hi.x, s_hi.y, s_hi.z, s_hi.w};
-            float ol[8], oh[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float xl = __uint_as_float(lo[q * 8 + j]);
-              float xh = __uint_as_float(hi[q * 8 + j]);
-              bf16r2(xl, xh);
-              float cosl = (j & 1) ? bf16_hi(cl[j >> 1]) : bf16_lo(cl[j >> 1]);
-              float sinl = (j & 1) ? bf16_hi(sl[j >> 1]) : bf16_lo(sl[j >> 1]);
-              float cosh_ = (j & 1) ? bf16_hi(ch[j >> 1]) : bf16_lo(ch[j >> 1]);
-              float sinh_ = (j & 1) ? bf16_hi(sh[j >> 1]) : bf16_lo(sh[j >> 1]);
-              float a0 = xl * cosl, a1 = -xh * sinl, b0 = xh * cosh_, b1 = xl * sinh_;
-              bf16r2(a0, a1);
-              bf16r2(b0, b1);
-              ol[j] = a0 + a1;
-              oh[j] = b0 + b1;
-            }
-            *reinterpret_cast<uint4*>(orow + c + q * 8) =
-                make_uint4(pack_bf16(ol[0], ol[1]), pack_bf16(ol[2], ol[3]), pack_bf16(ol[4], ol[5]), pack_bf16(ol[6], ol[7]));
-            *reinterpret_cast<uint4*>(orow + 64 + c + q * 8) =
-                make_uint4(pack_bf16(oh[0], oh[1]), pack_bf16(oh[2], oh[3]), pack_bf16(oh[4], oh[5]), pack_bf16(oh[6], oh[7]));
-          }
-        }
+      for (int q = 0; q < 4; ++q) {
+        tc_lo[q] = __ldg(reinterpret_cast<const uint4*>(cs + c + q * 8));
+        ts_lo[q] = __ldg(reinterpret_cast<const uint4*>(sn + c + q * 8));
+        tc_hi[q] = __ldg(reinterpret_cast<const uint4*>(cs + 64 + c + q * 8));
+        ts_hi[q] = __ldg(reinterpret_cast<const uint4*>(sn + 64 + c + q * 8));
       }
-    } else {
-      constexpr int NCH = (BN + 31) / 32, NMAX = NCH - NCH / 2;
-      const int cb = half ? (NCH / 2) * 32 : 0;
-      const int n_my = half ? NCH - NCH / 2 : NCH / 2;
-      // same two-deep pipeline as the LINEAR epilogue: accumulator chunk and bias vectors of chunk i + 1 in flight while chunk i
-      // is converted and scattered to its heads
-      uint32_t v[2][32];
-      uint4 bvq[2][4];
-      auto window = [&](int c) { return (c + 32 <= BN) ? c : BN - 32; };  // BN = 144: the tail re-reads an overlapping window
-      auto issue = [&](int c, int set) {
-        const int cbase = window(c);
-        ld_acc32(acc + cbase, v[set]);
+      if (row_ok) {
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
-          const int cs_ = cseg0 + cbase + q * 8;
-          bvq[set][q] = (bias && cs_ + 8 <= p.N) ? __ldg(reinterpret_cast<const uint4*>(bias + cs_)) : make_uint4(0, 0, 0, 0);
-        }
-      };
-      if (n_my > 0) issue(cb, 0);
+          const uint4 c_lo = tc_lo[q], s_lo = ts_lo[q], c_hi = tc_hi[q], s_hi = ts_hi[q];
+          const uint32_t cl[4] = {c_lo.x, c_lo.y, c_lo.z, c_lo.w}, sl[4] = {s_lo.x, s_lo.y, s_lo.z, s_lo.w};
+          const uint32_t ch[4] = {c_hi.x, c_hi.y, c_hi.z, c_hi.w}, sh[4] = {s_hi.x, s_hi.y, s_hi.z, s_hi.w};
+          float ol[8], oh[8];
 #pragma unroll
-      for (int i = 0; i < NMAX; ++i) {
-        if (i >= n_my) break;
-        const int c = cb + i * 32;
-        const int set = i & 1;
-        if (i + 1 < n_my) issue(c + 32, set ^ 1);
-        const int cbase = window(c);
-        const int qstart = (c + 32 <= BN) ? 0 : (c - cbase) / 8;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          if (q < qstart) continue;
-          const int cs_ = cseg0 + cbase + q * 8;  // column inside the segment
-          if (cs_ + 8 > p.N) continue;
-          float x[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = __uint_as_float(v[set][q * 8 + j]);
-          if (bias) {
-            const uint4 bv = bvq[set][q];
-            const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              x[2 * j] += bf16_lo(bw[j]);
-              x[2 * j + 1] += bf16_hi(bw[j]);
-            }
+          for (int j = 0; j < 8; ++j) {
+            float xl = __uint_as_float(lo[q * 8 + j]);
+            float xh = __uint_as_float(hi[q * 8 + j]);
+            bf16r2(xl, xh);
+            float cosl = (j & 1) ? bf16_hi(cl[j >> 1]) : bf16_lo(cl[j >> 1]);
+            float sinl = (j & 1) ? bf16_hi(sl[j >> 1]) : bf16_lo(sl[j >> 1]);
+            float cosh_ = (j & 1) ? bf16_hi(ch[j >> 1]) : bf16_lo(ch[j >> 1]);
+            float sinh_ = (j & 1) ? bf16_hi(sh[j >> 1]) : bf16_lo(sh[j >> 1]);
+            float a0 = xl * cosl, a1 = -xh * sinl, b0 = xh * cosh_, b1 = xl * sinh_;
+            bf16r2(a0, a1);
+            bf16r2(b0, b1);
+            ol[j] = a0 + a1;
+            oh[j] = b0 + b1;
           }
-          if (row_ok) {
-            const int head = cs_ / p.head_dim;
-            const int d = cs_ - head * p.head_dim;
-            *reinterpret_cast<uint4*>(obase + head * p.stride_h + d) =
-                make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
-          }
+          *reinterpret_cast<uint4*>(orow + c + q * 8) =
+              make_uint4(pack_bf16(ol[0], ol[1]), pack_bf16(ol[2], ol[3]), pack_bf16(ol[4], ol[5]), pack_bf16(ol[6], ol[7]));
+          *reinterpret_cast<uint4*>(orow + 64 + c + q * 8) =
+              make_uint4(pack_bf16(oh[0], oh[1]), pack_bf16(oh[2], oh[3]), pack_bf16(oh[4], oh[5]), pack_bf16(oh[6], oh[7]));
         }
       }
     }
+  }
+}
+
+// A HEADS tile without RoPE: the warpgroup's 64 staged rows (warpgroup cw), bias added, stored into the head-major buffers
+// 16 bytes per thread, with consecutive threads on consecutive 8-column chunks of a row.  Each warp store then covers whole
+// runs of two rows' heads; with one row per thread, every store hit 32 rows head_ld apart (a power-of-two stride), and the ViT
+// q/k/v projection took twice as long as a plain linear of the same shape.  Arithmetic and rounding are unchanged.
+template <int BN>
+ARIA_DEVICE void heads_store_tile(const GemmParams& p, const float* stg, int cw, int m_idx, int n_idx, int row0, int rows) {
+  constexpr int ACC_LD = acc_ld(BN), CH = BN / 8;
+  const int col0 = n_idx * BN;
+  const int seg = col0 / p.N;
+  const int cseg0 = col0 - seg * p.N;
+  const __nv_bfloat16* bias = p.bias[seg];
+  __nv_bfloat16* out = p.out[seg];
+#pragma unroll 1
+  for (int i = threadIdx.x & 127; i < 64 * CH; i += 128) {
+    const int r = cw * 64 + i / CH, c = (i % CH) * 8;
+    const int r_in_grp = m_idx * BM + r;
+    const int cs = cseg0 + c;  // column inside the segment
+    if (r_in_grp >= rows || cs + 8 > p.N) continue;
+    const float4 lo = *reinterpret_cast<const float4*>(stg + r * ACC_LD + c);
+    const float4 hi = *reinterpret_cast<const float4*>(stg + r * ACC_LD + c + 4);
+    float x[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+    if (bias) {
+      const uint4 bv = __ldg(reinterpret_cast<const uint4*>(bias + cs));
+      const uint32_t bw[4] = {bv.x, bv.y, bv.z, bv.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        x[2 * j] += bf16_lo(bw[j]);
+        x[2 * j + 1] += bf16_hi(bw[j]);
+      }
+    }
+    const int grow = row0 + r_in_grp;
+    const int b = grow / p.rows_per_batch, tok = grow - b * p.rows_per_batch;
+    const int head = cs / p.head_dim, d = cs - head * p.head_dim;
+    *reinterpret_cast<uint4*>(out + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld + head * p.stride_h + d) =
+        make_uint4(pack_bf16(x[0], x[1]), pack_bf16(x[2], x[3]), pack_bf16(x[4], x[5]), pack_bf16(x[6], x[7]));
   }
 }
 
@@ -440,7 +422,7 @@ enum class AccScale { NONE, COL, ROW_COL };
 
 // The end of a consumer warpgroup's tile: stage its fp32 accumulator rows in `stg` ([BM][acc_ld(BN)]), scaled by the column
 // scales `bsc` (load_col_scales) and the row scales of the fragment's two rows `as0` / `as1` as SCALE says, then run the
-// epilogue on this thread's row.
+// epilogue on this thread's row (HEADS segments without RoPE: on the warpgroup's rows, heads_store_tile).
 template <int BN, int EPI, AccScale SCALE>
 ARIA_DEVICE void stage_and_epilogue(const GemmParams& p, float* stg, const ConsumerThread& ct, const float (&acc)[BN / 2],
                                     const float2 (&bsc)[BN / 8], float as0, float as1, int n_out_total, int grp, int m_idx,
@@ -460,6 +442,12 @@ ARIA_DEVICE void stage_and_epilogue(const GemmParams& p, float* stg, const Consu
         make_float2(scaled(acc[4 * j + 2], as1, bsc[j].x), scaled(acc[4 * j + 3], as1, bsc[j].y));
   }
   named_bar_sync(1 + ct.cw, 128);
+  if constexpr (EPI == ARIA_EPI_HEADS) {
+    if (!((p.rope_mask >> (n_idx * BN / p.N)) & 1)) {
+      heads_store_tile<BN>(p, stg, ct.cw, m_idx, n_idx, row0, rows);
+      return;
+    }
+  }
   const int r_in_grp = m_idx * BM + ct.epi_row;
   const bool row_ok = r_in_grp < rows;
   const int64_t grow = static_cast<int64_t>(row0) + r_in_grp;

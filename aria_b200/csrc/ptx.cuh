@@ -68,12 +68,41 @@ ARIA_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait_addr(smem
 ARIA_DEVICE void mbar_arrive_expect_tx_addr(uint32_t bar_addr, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar_addr), "r"(bytes) : "memory");
 }
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of this cluster.  Default (.cta) scope: it signals that
+// this thread's reads of a stage are done (a retired wgmma group), which needs no ordering of its memory writes; the .cluster
+// scope form puts a MEMBAR.GPU in front of every arrive, which stalls the consumer warp each k-block.
+ARIA_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n" ::"r"(smem_u32(bar)), "r"(cta)
+      : "memory");
+}
+
+// ---------------------------------------------------------------- thread-block clusters
+ARIA_DEVICE uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// Every thread of every CTA of the cluster; not .aligned, so threads of a warp may reach it on different paths
+ARIA_DEVICE void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 
 // ---------------------------------------------------------------- TMA
 ARIA_DEVICE void tma_load_2d_addr(uint32_t dst, const CUtensorMap* m, uint32_t bar_addr, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same box lands at offset `dst` of every CTA in `cta_mask` and completes its bytes on the mbarrier at `bar_addr` in each
+ARIA_DEVICE void tma_load_2d_multicast_addr(uint32_t dst, const CUtensorMap* m, uint32_t bar_addr, int c0, int c1,
+                                            uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_addr), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 ARIA_DEVICE void prefetch_tmap(const CUtensorMap* m) {
