@@ -15,6 +15,7 @@ ARIA_OK = 0
 B_NK, B_GKN, B_GNK = 0, 1, 2
 EPI_LINEAR, EPI_SWIGLU, EPI_HEADS = 0, 1, 2
 ACT_NONE, ACT_GELU_TANH, ACT_GELU_NEW = 0, 1, 2
+MOE_EXPERTS_BF16, MOE_EXPERTS_FP8, MOE_EXPERTS_W8A8 = 0, 1, 2
 
 _ERR = {-1: "bad argument", -2: "unsupported shape", -3: "CUDA error"}
 
@@ -56,11 +57,15 @@ SIGNATURES = {
     "aria_grouped_gemm_fp8": (i32, [vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]),
     "aria_permute_quantize_fp8_rows": (i32, [vp, vp, vp, vp, i64, i32, vp]),
     "aria_grouped_gemm_w8a8": (i32, [vp, vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]),
+    "aria_gemm_w8a8": (i32, [C.POINTER(GemmDesc), vp, vp, vp]),
     "aria_grouped_wgrad": (i32, [vp, i64, vp, i64, vp, vp, i64, i64, i64, i32, i32, vp]),
     "aria_moe_block_fwd_workspace_bytes": (i64, [i64, i32, i32, i32, i32, i32]),
     "aria_moe_block_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
     "aria_moe_block_fwd_fp8": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
     "aria_moe_block_fwd_w8a8": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
+    "aria_moe_block_fwd_shared_fp8_workspace_bytes": (i64, [i64, i32, i32, i32, i32, i32]),
+    "aria_moe_block_fwd_shared_fp8": (i32, [vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp,
+                                            vp, i64, vp, vp]),
     "aria_swiglu_fwd": (i32, [vp, vp, i64, i32, vp]),
     "aria_swiglu_bwd": (i32, [vp, vp, vp, i64, i32, vp]),
     "aria_combine_bwd": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, i32, vp]),
@@ -71,6 +76,7 @@ SIGNATURES = {
     "aria_permute_rows": (i32, [vp, vp, vp, i64, i32, vp]),
     "aria_unpermute_combine": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, vp]),
     "aria_rmsnorm": (i32, [vp, vp, vp, vp, vp, i64, i32, f32, vp]),
+    "aria_rmsnorm_quantize_fp8": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, f32, vp]),
     "aria_layernorm": (i32, [vp, vp, vp, vp, i64, i32, f32, vp]),
     "aria_rope_table": (i32, [vp, vp, vp, i32, i32, vp]),
     "aria_embedding": (i32, [vp, vp, vp, i64, i32, vp]),
@@ -126,7 +132,10 @@ def load():
 # kernels launched per C-ABI call (for bench.py's `gpu_launches`; memsets are not counted)
 KERNELS_PER_CALL = {"router_topk": 2, "attention_decode": 2, "attention_decode_devlen": 2, "attention_decode_fp8": 2,
                     "attention_decode_devlen_fp8": 2, "attention_bwd": 3, "moe_block_fwd": 9, "moe_block_fwd_fp8": 9,
-                    "moe_block_fwd_w8a8": 10, "quantize_fp8_cols": 2}
+                    "moe_block_fwd_w8a8": 10, "quantize_fp8_cols": 2,
+                    # W8A8 shared experts: two row quantisers join the shared branch's two GEMMs
+                    "moe_block_fwd_bf16_shared_fp8": 11, "moe_block_fwd_fp8_shared_fp8": 11,
+                    "moe_block_fwd_w8a8_shared_fp8": 12}
 launch_count = 0
 
 

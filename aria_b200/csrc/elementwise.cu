@@ -2,6 +2,7 @@
 #include <string.h>
 
 #include "common.cuh"
+#include "fp8.cuh"
 #include "ptx.cuh"
 
 namespace aria {
@@ -78,6 +79,84 @@ __global__ void __launch_bounds__(128) rmsnorm_kernel(const uint4* __restrict__ 
         }
         out[r * vpr + v] = make_uint4(pack_bf16(o[0], o[1]), pack_bf16(o[2], o[3]), pack_bf16(o[4], o[5]), pack_bf16(o[6], o[7]));
       }
+    }
+  }
+}
+
+// rmsnorm_kernel followed by the per-row e4m3 quantiser of quant.cu (permute_quantize_rows_kernel) in one pass: the bf16
+// output row stays in registers, its amax is a second block reduction, and only the codes and the scale are stored.  The
+// arithmetic of both halves is theirs, so the result is bit-identical to the two kernels in sequence.
+template <int MAXV>
+__global__ void __launch_bounds__(128) rmsnorm_quantize_kernel(const uint4* __restrict__ x, const uint4* __restrict__ res,
+                                                               const uint4* __restrict__ w, uint2* __restrict__ q,
+                                                               float* __restrict__ scale, uint4* __restrict__ sum_out,
+                                                               int64_t rows, int vpr, float eps, float inv_d) {
+  __shared__ float red[4], redm[4];
+  const int tid = threadIdx.x;
+  for (int64_t r = blockIdx.x; r < rows; r += gridDim.x) {
+    float h[MAXV][8];
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int v = tid + i * 128;
+      if (v < vpr) {
+        const uint4 a4 = x[r * vpr + v];
+        const uint32_t a[4] = {a4.x, a4.y, a4.z, a4.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          h[i][2 * j] = bf16_lo(a[j]);
+          h[i][2 * j + 1] = bf16_hi(a[j]);
+        }
+        if (res) {
+          const uint4 q2 = res[r * vpr + v];
+          const uint32_t b[4] = {q2.x, q2.y, q2.z, q2.w};
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            h[i][2 * j] = bf16r(h[i][2 * j] + bf16_lo(b[j]));
+            h[i][2 * j + 1] = bf16r(h[i][2 * j + 1] + bf16_hi(b[j]));
+          }
+          if (sum_out)
+            sum_out[r * vpr + v] = make_uint4(pack_bf16(h[i][0], h[i][1]), pack_bf16(h[i][2], h[i][3]),
+                                              pack_bf16(h[i][4], h[i][5]), pack_bf16(h[i][6], h[i][7]));
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) ss += h[i][j] * h[i][j];
+      }
+    }
+    ss = warp_sum(ss);
+    __syncthreads();  // red[] / redm[] free (previous row consumed)
+    if ((tid & 31) == 0) red[tid >> 5] = ss;
+    __syncthreads();
+    ss = red[0] + red[1] + red[2] + red[3];
+    const float rstd = 1.0f / sqrtf(ss * inv_d + eps);
+    uint4 o4[MAXV];  // the bf16 output; o4[i] is set and read under the same v < vpr
+    float m = 0.f;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int v = tid + i * 128;
+      if (v < vpr) {
+        const uint4 wv = __ldg(w + v);
+        const uint32_t a[4] = {wv.x, wv.y, wv.z, wv.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          o[j] = pack_bf16(bf16_lo(a[j]) * bf16r(h[i][2 * j] * rstd), bf16_hi(a[j]) * bf16r(h[i][2 * j + 1] * rstd));
+        o4[i] = make_uint4(o[0], o[1], o[2], o[3]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) m = fmaxf(m, fmaxf(fabsf(__uint_as_float(o[j] << 16)), fabsf(__uint_as_float(o[j] & 0xFFFF0000u))));
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((tid & 31) == 0) redm[tid >> 5] = m;
+    __syncthreads();
+    m = fmaxf(fmaxf(redm[0], redm[1]), fmaxf(redm[2], redm[3]));
+    const float s = m > 0.f ? __fdiv_rn(m, E4M3_MAX) : 1.f;
+    if (tid == 0) scale[r] = s;
+#pragma unroll
+    for (int i = 0; i < MAXV; ++i) {
+      const int v = tid + i * 128;
+      if (v < vpr) q[r * vpr + v] = cast8_e4m3(o4[i], s);
     }
   }
 }
@@ -346,6 +425,31 @@ extern "C" int aria_rmsnorm(const void* x, const void* residual, const void* wei
   else RMS(4);
 #undef RMS
   return check_launch("rmsnorm_kernel");
+}
+
+extern "C" int aria_rmsnorm_quantize_fp8(const void* x, const void* residual, const void* weight, void* q, float* scale,
+                                         void* sum_out, int64_t rows, int32_t d, float eps, aria_stream_t stream_) {
+  auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  ARIA_CHECK_ARG(x && weight && q && scale && d > 0 && d % 8 == 0 && d <= 128 * 8 * 4 && rows >= 0);
+  ARIA_CHECK_ARG(al16(x) && al16(weight) && al16(q) && (reinterpret_cast<uintptr_t>(scale) & 3) == 0);
+  ARIA_CHECK_ARG((!residual || al16(residual)) && (!sum_out || al16(sum_out)));
+  if (rows == 0) return ARIA_OK;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  const int vpr = d / 8;
+  int64_t grid64 = rows;
+  const int64_t cap = static_cast<int64_t>(sm_count()) * 16;
+  if (grid64 > cap) grid64 = cap;
+  const int grid = static_cast<int>(grid64);
+#define RMSQ(MAXV)                                                                                                          \
+  rmsnorm_quantize_kernel<MAXV><<<grid, 128, 0, stream>>>(static_cast<const uint4*>(x), static_cast<const uint4*>(residual), \
+                                                          static_cast<const uint4*>(weight), static_cast<uint2*>(q), scale,   \
+                                                          static_cast<uint4*>(sum_out), rows, vpr, eps, 1.0f / d)
+  if (vpr <= 128) RMSQ(1);
+  else if (vpr <= 256) RMSQ(2);
+  else if (vpr <= 384) RMSQ(3);
+  else RMSQ(4);
+#undef RMSQ
+  return check_launch("rmsnorm_quantize_kernel");
 }
 
 extern "C" int aria_layernorm(const void* x, const void* weight, const void* bias, void* out, int64_t rows, int32_t d,

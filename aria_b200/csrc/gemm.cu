@@ -296,16 +296,45 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 constexpr int W8_BK = 128;
 static_assert(BM * W8_BK == A_STAGE_BYTES, "W8A8 A stage = bf16 A stage");
 
-template <int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
-                 const float* __restrict__ a_scale) {
+// Dense nn.Linear weights (gemm_w8a8_dense_kernel): one [N, K] e4m3 weight and one fp32 scale per output column for each
+// segment s < n_seg (q / k / v, or gate / up for SwiGLU), each behind its own tensor map, so the weights stay separate tensors
+struct W8a8DenseScales {
+  const float* b[3];
+};
+
+// The column scales of this thread's accumulator columns in tile n_idx of a dense launch (load_col_scales of the grouped
+// kernel, per segment): LINEAR / HEADS tiles lie in one segment (n_seg > 1: N % 128 == 0); a SwiGLU tile holds BN/2 gate
+// columns, then the matching up columns.  Columns past N get 0.
+template <int BN, int EPI>
+ARIA_DEVICE void load_dense_col_scales(const GemmParams& p, const W8a8DenseScales& sc, int n_idx, int frag_col,
+                                       float2 (&bsc)[BN / 8]) {
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    int col, seg;
+    if constexpr (EPI == ARIA_EPI_SWIGLU) {
+      seg = 8 * j < BN / 2 ? 0 : 1;
+      col = n_idx * (BN / 2) + 8 * j - seg * (BN / 2) + frag_col;
+    } else {
+      seg = n_idx * BN / p.N;
+      col = n_idx * BN - seg * p.N + 8 * j + frag_col;
+    }
+    const float* srow = seg == 0 ? sc.b[0] : (seg == 1 ? sc.b[1] : sc.b[2]);  // no dynamic index: keeps sc out of local memory
+    bsc[j] = col < p.N ? __ldg(reinterpret_cast<const float2*>(srow + col)) : make_float2(0.f, 0.f);
+  }
+}
+
+// The W8A8 pipeline.  Grouped (DENSE = false): one B map over the [G * N_b, K] expert weights.  DENSE: up to three [N, K]
+// weights (tmB0..2, one per segment), a single group of p.M rows, and every epilogue of gemm_kernel (LINEAR with residual,
+// SWIGLU from separate gate and up weights, HEADS with RoPE).  The k-loop, the tile and the promotion are the same.
+template <int EPI, bool DENSE>
+ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
+                           const GemmParams& p, const float* __restrict__ a_scale, const W8a8DenseScales& dsc) {
   constexpr int BN = 128;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * W8_BK;
   constexpr int STAGES = GEMM_STAGES;
   constexpr int ACC_LD = acc_ld(BN);
   constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;
-  static_assert(EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_SWIGLU, "W8A8: expert GEMM epilogues");
+  static_assert(DENSE || EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_SWIGLU, "W8A8 grouped: expert GEMM epilogues");
 
   uint8_t* smem = smem_1024();
   float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
@@ -316,14 +345,20 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int wg = threadIdx.x >> 7;
 
   if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA);
-    prefetch_tmap(&tmB);
+    prefetch_tmap(tmA);
+    prefetch_tmap(tmB0);
+    if constexpr (DENSE) {
+      if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(tmB1);
+      if (p.n_seg > 2) prefetch_tmap(tmB2);
+    }
     bar.init(1, CONSUMER_WARPS);
     fence_mbar_init();
   }
   __syncthreads();
 
-  const int n_tiles = (p.N + OUT_BN - 1) / OUT_BN;
+  // output columns overall: dense LINEAR / HEADS launches have n_seg segments of N columns
+  const int n_out_total = DENSE ? p.N * (EPI == ARIA_EPI_SWIGLU ? 1 : p.n_seg) : p.N;
+  const int n_tiles = (n_out_total + OUT_BN - 1) / OUT_BN;
   const int k_blocks = p.K / W8_BK;
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t full0 = smem_u32(bar.full), empty0 = smem_u32(bar.empty);
@@ -341,7 +376,20 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int a_row = row0 + m_idx * BM;
         // B rows of the two 64-row boxes: (group, column c) is row group * N_b + c; SwiGLU takes the gate and the up box
         int b_r0, b_r1;
-        if constexpr (EPI == ARIA_EPI_SWIGLU) {
+        const CUtensorMap* tb0 = tmB0;
+        const CUtensorMap* tb1 = tmB0;
+        if constexpr (DENSE) {
+          if constexpr (EPI == ARIA_EPI_SWIGLU) {
+            b_r0 = b_r1 = n_idx * OUT_BN;
+            tb1 = tmB1;
+          } else {
+            const int col = n_idx * BN;
+            const int seg = col / p.N;
+            tb0 = tb1 = seg == 0 ? tmB0 : (seg == 1 ? tmB1 : tmB2);
+            b_r0 = col - seg * p.N;
+            b_r1 = b_r0 + 64;
+          }
+        } else if constexpr (EPI == ARIA_EPI_SWIGLU) {
           b_r0 = weight_block(p, grp) * 2 * p.N + n_idx * OUT_BN;
           b_r1 = b_r0 + p.N;
         } else {
@@ -354,9 +402,9 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const uint32_t sb = sa + A_STAGE_BYTES;
           mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
           mbar_arrive_expect_tx_addr(fb, STAGE_BYTES);
-          tma_load_2d_addr(sa, &tmA, fb, kb * W8_BK, a_row);
-          tma_load_2d_addr(sb, &tmB, fb, kb * W8_BK, b_r0);
-          tma_load_2d_addr(sb + 64 * W8_BK, &tmB, fb, kb * W8_BK, b_r1);
+          tma_load_2d_addr(sa, tmA, fb, kb * W8_BK, a_row);
+          tma_load_2d_addr(sb, tb0, fb, kb * W8_BK, b_r0);
+          tma_load_2d_addr(sb + 64 * W8_BK, tb1, fb, kb * W8_BK, b_r1);
           rp.next();
         }
       }
@@ -379,7 +427,8 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       float2 bsc[BN / 8];
-      load_col_scales<BN, EPI>(p, grp, n_idx, ct.frag_col, bsc);
+      if constexpr (DENSE) load_dense_col_scales<BN, EPI>(p, dsc, n_idx, ct.frag_col, bsc);
+      else load_col_scales<BN, EPI>(p, grp, n_idx, ct.frag_col, bsc);
       // row scales of the fragment's two rows (rows past the group's end are computed but never stored; the index is clamped
       // to the buffer)
       const int ar = row0 + m_idx * BM + ct.frag_row;
@@ -399,9 +448,25 @@ gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
         rp.next();
       }
-      stage_and_epilogue<BN, EPI, AccScale::ROW_COL>(p, stg, ct, acc, bsc, as0, as1, p.N, grp, m_idx, n_idx, row0, rows);
+      stage_and_epilogue<BN, EPI, AccScale::ROW_COL>(p, stg, ct, acc, bsc, as0, as1, n_out_total, grp, m_idx, n_idx, row0,
+                                                     rows);
     }
   }
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
+                 const float* __restrict__ a_scale) {
+  w8a8_body<EPI, false>(&tmA, &tmB, &tmB, &tmB, p, a_scale, W8a8DenseScales{});
+}
+
+template <int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_w8a8_dense_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
+                       const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p,
+                       const float* __restrict__ a_scale, const W8a8DenseScales b_scale) {
+  w8a8_body<EPI, true>(&tmA, &tmB0, &tmB1, &tmB2, p, a_scale, b_scale);
 }
 
 }  // namespace aria
@@ -637,6 +702,59 @@ extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, c
                                                                  tmB, p, a_scale);
   return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_LINEAR>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB,
                                                               p, a_scale);
+}
+
+extern "C" int aria_gemm_w8a8(const aria_gemm_desc_t* d, const float* a_scale, const float* const b_scale[3],
+                              aria_stream_t stream_) {
+  auto al = [](const void* ptr, uintptr_t a) { return (reinterpret_cast<uintptr_t>(ptr) & (a - 1)) == 0; };
+  ARIA_CHECK_ARG(d != nullptr && b_scale != nullptr);
+  ARIA_CHECK_ARG(d->a && d->b[0] && d->out[0] && a_scale && b_scale[0]);
+  ARIA_CHECK_ARG(d->b_layout == ARIA_B_NK && d->num_groups == 1 && d->group_mod == 0 && !d->group_offsets && !d->group_counts &&
+                 !d->out_group_base && d->a_rows == 0);
+  ARIA_CHECK_ARG(d->m >= 0 && d->m < (int64_t(1) << 31) && d->n > 0 && d->k > 0 && d->k <= (1 << 30) && d->n <= (1 << 29));
+  ARIA_CHECK_ARG(d->k % W8_BK == 0 && d->n % 64 == 0 && d->lda >= d->k && d->lda % 16 == 0);
+  ARIA_CHECK_ARG(d->n_seg >= 1 && d->n_seg <= 3);
+  ARIA_CHECK_ARG(d->epilogue == ARIA_EPI_LINEAR || d->epilogue == ARIA_EPI_SWIGLU || d->epilogue == ARIA_EPI_HEADS);
+  ARIA_CHECK_ARG(al(d->a, 16) && al(d->out[0], 16) && al(a_scale, 4));
+  const bool swiglu = d->epilogue == ARIA_EPI_SWIGLU;
+  const int nb = swiglu ? 2 : d->n_seg;  // weights (and scale vectors)
+  if (swiglu) ARIA_CHECK_ARG(d->n_seg == 2);
+  for (int s = 0; s < nb; ++s) ARIA_CHECK_ARG(d->b[s] && b_scale[s] && al(d->b[s], 16) && al(b_scale[s], 16));
+  // LINEAR / HEADS tiles must not straddle two weights
+  if (!swiglu && d->n_seg > 1) ARIA_CHECK_ARG(d->n % 128 == 0);
+  if (d->epilogue == ARIA_EPI_HEADS) {
+    ARIA_CHECK_ARG(d->n % 128 == 0 && d->head_dim > 0 && d->head_dim % 8 == 0 && d->head_ld >= d->head_dim &&
+                   d->n % d->head_dim == 0);
+    if (d->rope_mask) ARIA_CHECK_ARG(d->head_dim == 128 && d->rope_cos && d->rope_sin);
+    for (int s = 0; s < d->n_seg; ++s) ARIA_CHECK_ARG(d->out[s] != nullptr && al(d->out[s], 16));
+  } else {
+    ARIA_CHECK_ARG(d->ldo % 8 == 0 && d->ldo >= (swiglu ? d->n : d->n * d->n_seg));
+  }
+  if (d->residual) ARIA_CHECK_ARG(d->epilogue == ARIA_EPI_LINEAR && al(d->residual, 16) && d->ldr % 8 == 0);
+  if (d->m == 0) return ARIA_OK;
+
+  // UINT8 maps, 128-byte swizzle: a box row is one 128-element k-block; each weight is its own [n, k] map
+  CUtensorMap tmA, tmB[3];
+  int rc = make_tmap_2d(&tmA, d->a, d->k, d->m, d->lda, W8_BK, BM, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  if (rc) return rc;
+  W8a8DenseScales sc{};
+  for (int s = 0; s < 3; ++s) {
+    const int src = s < nb ? s : 0;
+    sc.b[s] = b_scale[src];
+    rc = make_tmap_2d(&tmB[s], d->b[src], d->k, d->n, d->k, W8_BK, 64, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+    if (rc) return rc;
+  }
+  const GemmParams p = gemm_params(d, nullptr);
+  const int64_t tiles = max_tiles(d, 128, 0);
+  constexpr int SMEM = gemm_smem_bytes<128>();
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+#define ARIA_LAUNCH(EPI_)                                                                                                      \
+  return launch_persistent<gemm_w8a8_dense_kernel<EPI_>>("gemm_w8a8_dense_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, \
+                                                          tmB[0], tmB[1], tmB[2], p, a_scale, sc)
+  if (swiglu) ARIA_LAUNCH(ARIA_EPI_SWIGLU);
+  if (d->epilogue == ARIA_EPI_HEADS) ARIA_LAUNCH(ARIA_EPI_HEADS);
+  ARIA_LAUNCH(ARIA_EPI_LINEAR);
+#undef ARIA_LAUNCH
 }
 
 extern "C" int aria_abi_version(void) { return 3; }

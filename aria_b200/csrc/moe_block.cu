@@ -25,9 +25,12 @@ inline int64_t al(int64_t n) { return (n + kAlign - 1) / kAlign * kAlign; }
 
 struct BlockWs {
   int64_t idx, scores, counts, offsets, dest, src, logits, permuted, h, y, hs, shared, total;
+  int64_t sxq, sxs, shq, shs;  // shared_fp8: e4m3 rows and row scales of x and of h for the W8A8 shared experts
 };
 
-BlockWs carve(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t Is) {
+// shared_fp8 appends the shared branch's quantised rows after the regions of the other modes, which keep their offsets and
+// total.  They are the branch's own: it runs on the side stream, concurrently with everything of the routed branch.
+BlockWs carve(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t Is, bool shared_fp8 = false) {
   BlockWs w{};
   int64_t o = 0;
   const int64_t R = T * k;
@@ -43,6 +46,12 @@ BlockWs carve(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t Is)
   w.y = o;        o += al(R * d * 2);
   w.hs = o;       o += al(T * Is * 2);
   w.shared = o;   o += al(T * d * 2);
+  if (shared_fp8) {
+    w.sxq = o;    o += al(T * d);
+    w.sxs = o;    o += al(T * 4);
+    w.shq = o;    o += al(T * Is);
+    w.shs = o;    o += al(T * 4);
+  }
   w.total = o;
   return w;
 }
@@ -78,18 +87,28 @@ bool w8a8_fits(int64_t R, int32_t d, int32_t I, const BlockWs& ws, W8a8Ws& o) {
   return al16(R * d) + R * 4 <= permuted_bytes && R * I <= permuted_bytes && R * 4 <= src_bytes;
 }
 
+// The e4m3 shared-expert weights' column scales (SharedScales::gate == NULL: bf16 shared experts)
+struct SharedScales {
+  const float* gate;
+  const float* up;
+  const float* down;
+};
+
 // The whole block.  fc1_scale / fc2_scale NULL: bf16 expert weights; given: fc1_w / fc2_w are e4m3 with per-(expert, column)
 // fp32 scales and the two expert GEMMs run the fp8-weight grouped GEMM, or with w8a8 aria_grouped_gemm_w8a8 on K-major weights
-// ([E, 2I, d] / [E, d, I]) and row-quantised activations.  Every other launch is the same.
+// ([E, 2I, d] / [E, d, I]) and row-quantised activations.  With shared scales, the shared experts are W8A8 (aria_gemm_w8a8 on
+// row-quantised x and h).  Every other launch is the same.
 int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
                   const float* fc2_scale, bool w8a8, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
                   int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx, void* workspace,
-                  int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream) {
+                  int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream,
+                  const SharedScales& ss = SharedScales{nullptr, nullptr, nullptr}) {
   if (!x || !w_router || !fc1_w || !fc2_w || !out || !workspace) return ARIA_ERR_BAD_ARG;
   if (T <= 0 || d <= 0 || E <= 0 || E > 64 || k <= 0 || k > 8 || k > E || I <= 0 || I_shared < 0) return ARIA_ERR_BAD_ARG;
   if (I_shared > 0 && (!gate_w || !up_w || !down_w)) return ARIA_ERR_BAD_ARG;
   if ((reinterpret_cast<uintptr_t>(workspace) & 15) != 0) return ARIA_ERR_BAD_ARG;
-  const BlockWs ws = carve(T, d, E, k, I, I_shared);
+  const bool shared_fp8 = ss.gate != nullptr;
+  const BlockWs ws = carve(T, d, E, k, I, I_shared, shared_fp8);
   if (workspace_bytes < ws.total) return ARIA_ERR_BAD_ARG;
   W8a8Ws q{};
   if (w8a8 && !w8a8_fits(T * k, d, I, ws, q)) return ARIA_ERR_BAD_ARG;
@@ -109,6 +128,29 @@ int moe_block_run(const void* x, const void* w_router, const void* fc1_w, const 
   const bool fork = I_shared > 0 && s_side != nullptr && s_side != s_main;
   cudaEvent_t* ev = nullptr;
   auto shared_branch = [&](aria_stream_t st) -> int {
+    if (shared_fp8) {
+      // x -> e4m3 rows -> W8A8 SwiGLU (gate | up) -> h -> e4m3 rows -> W8A8 down
+      float* xs = static_cast<float*>(at(ws.sxs));
+      float* hs = static_cast<float*>(at(ws.shs));
+      int r = aria_permute_quantize_fp8_rows(x, nullptr, at(ws.sxq), xs, T, d, st);
+      if (r) return r;
+      aria_gemm_desc_t g;
+      memset(&g, 0, sizeof(g));
+      g.a = at(ws.sxq); g.lda = d; g.m = T; g.n = I_shared; g.k = d;
+      g.b[0] = gate_w; g.b[1] = up_w; g.n_seg = 2; g.b_layout = ARIA_B_NK; g.num_groups = 1;
+      g.epilogue = ARIA_EPI_SWIGLU;
+      g.out[0] = at(ws.hs); g.ldo = I_shared;
+      const float* gu_scale[3] = {ss.gate, ss.up, nullptr};
+      if ((r = aria_gemm_w8a8(&g, xs, gu_scale, st))) return r;
+      if ((r = aria_permute_quantize_fp8_rows(at(ws.hs), nullptr, at(ws.shq), hs, T, I_shared, st))) return r;
+      memset(&g, 0, sizeof(g));
+      g.a = at(ws.shq); g.lda = I_shared; g.m = T; g.n = d; g.k = I_shared;
+      g.b[0] = down_w; g.n_seg = 1; g.b_layout = ARIA_B_NK; g.num_groups = 1;
+      g.epilogue = ARIA_EPI_LINEAR;
+      g.out[0] = at(ws.shared); g.ldo = d;
+      const float* d_scale[3] = {ss.down, nullptr, nullptr};
+      return aria_gemm_w8a8(&g, hs, d_scale, st);
+    }
     aria_gemm_desc_t g;
     memset(&g, 0, sizeof(g));
     g.a = x; g.lda = d; g.m = T; g.n = I_shared; g.k = d;
@@ -185,17 +227,34 @@ extern "C" int aria_moe_block_fwd(const void* x, const void* w_router, const voi
                        forced_top_idx, workspace, workspace_bytes, stream, side_stream);
 }
 
+namespace {
+
+inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// The expert GEMMs' constraints of the fp8-weight and W8A8 modes, checked by the entries so that nothing is launched for a
+// block that would fail half-way
+bool fp8_experts_ok(int32_t d, int32_t I, const void* fc1_w, const void* fc2_w, const float* fc1_scale, const float* fc2_scale) {
+  if (!fc1_scale || !fc2_scale) return false;
+  if (d <= 0 || I <= 0 || d % 64 != 0 || I % 64 != 0) return false;
+  return al16(fc1_w) && al16(fc2_w) && al16(fc1_scale) && al16(fc2_scale);
+}
+
+// ... and of the quantiser in front of them
+bool w8a8_experts_ok(int32_t d, int32_t I, const void* fc1_w_nk, const void* fc2_w_nk, const float* fc1_scale,
+                     const float* fc2_scale) {
+  if (!fc1_scale || !fc2_scale) return false;
+  if (d <= 0 || I <= 0 || d % 128 != 0 || I % 128 != 0 || d > 4096 || I > 4096 || I > 2 * d) return false;
+  return al16(fc1_w_nk) && al16(fc2_w_nk) && al16(fc1_scale) && al16(fc2_scale);
+}
+
+}  // namespace
+
 extern "C" int aria_moe_block_fwd_fp8(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w,
                                       const float* fc1_scale, const float* fc2_scale, const void* gate_w, const void* up_w,
                                       const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
                                       int32_t I_shared, const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes,
                                       aria_stream_t stream, aria_stream_t side_stream) {
-  // the expert GEMMs' constraints are checked here too, so that nothing is launched for a block that would fail half-way
-  if (!fc1_scale || !fc2_scale) return ARIA_ERR_BAD_ARG;
-  if (d <= 0 || I <= 0 || d % 64 != 0 || I % 64 != 0) return ARIA_ERR_BAD_ARG;
-  if ((reinterpret_cast<uintptr_t>(fc1_w) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_w) & 15) != 0 ||
-      (reinterpret_cast<uintptr_t>(fc1_scale) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_scale) & 15) != 0)
-    return ARIA_ERR_BAD_ARG;
+  if (!fp8_experts_ok(d, I, fc1_w, fc2_w, fc1_scale, fc2_scale)) return ARIA_ERR_BAD_ARG;
   return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, false, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
                        forced_top_idx, workspace, workspace_bytes, stream, side_stream);
 }
@@ -205,13 +264,45 @@ extern "C" int aria_moe_block_fwd_w8a8(const void* x, const void* w_router, cons
                                        const void* down_w, void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
                                        int32_t I_shared, const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes,
                                        aria_stream_t stream, aria_stream_t side_stream) {
-  // the expert GEMMs' and quantizer's constraints are checked here too, so that nothing is launched for a block that would
-  // fail half-way
-  if (!fc1_scale || !fc2_scale) return ARIA_ERR_BAD_ARG;
-  if (d <= 0 || I <= 0 || d % 128 != 0 || I % 128 != 0 || d > 4096 || I > 4096 || I > 2 * d) return ARIA_ERR_BAD_ARG;
-  if ((reinterpret_cast<uintptr_t>(fc1_w_nk) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_w_nk) & 15) != 0 ||
-      (reinterpret_cast<uintptr_t>(fc1_scale) & 15) != 0 || (reinterpret_cast<uintptr_t>(fc2_scale) & 15) != 0)
-    return ARIA_ERR_BAD_ARG;
+  if (!w8a8_experts_ok(d, I, fc1_w_nk, fc2_w_nk, fc1_scale, fc2_scale)) return ARIA_ERR_BAD_ARG;
   return moe_block_run(x, w_router, fc1_w_nk, fc2_w_nk, fc1_scale, fc2_scale, true, gate_w, up_w, down_w, out, T, d, E, k, I,
                        I_shared, forced_top_idx, workspace, workspace_bytes, stream, side_stream);
+}
+
+extern "C" int64_t aria_moe_block_fwd_shared_fp8_workspace_bytes(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I,
+                                                                 int32_t I_shared) {
+  if (T <= 0 || d <= 0 || E <= 0 || k <= 0 || I <= 0 || I_shared <= 0) return ARIA_ERR_BAD_ARG;
+  return carve(T, d, E, k, I, I_shared, true).total;
+}
+
+extern "C" int aria_moe_block_fwd_shared_fp8(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w,
+                                             const float* fc1_scale, const float* fc2_scale, int32_t expert_mode,
+                                             const void* gate_w, const void* up_w, const void* down_w, const float* gate_scale,
+                                             const float* up_scale, const float* down_scale, void* out, int64_t T, int32_t d,
+                                             int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx,
+                                             void* workspace, int64_t workspace_bytes, aria_stream_t stream,
+                                             aria_stream_t side_stream) {
+  // the shared GEMMs' and quantisers' constraints (aria_gemm_w8a8: K % 128, N % 64; the row quantiser: d <= 4096)
+  if (!gate_w || !up_w || !down_w || !gate_scale || !up_scale || !down_scale) return ARIA_ERR_BAD_ARG;
+  if (I_shared <= 0 || d <= 0 || d % 128 != 0 || I_shared % 128 != 0 || d > 4096 || I_shared > 4096) return ARIA_ERR_BAD_ARG;
+  if (!al16(gate_w) || !al16(up_w) || !al16(down_w) || !al16(gate_scale) || !al16(up_scale) || !al16(down_scale))
+    return ARIA_ERR_BAD_ARG;
+  if (T >= (int64_t(1) << 31)) return ARIA_ERR_BAD_ARG;
+  const SharedScales ss{gate_scale, up_scale, down_scale};
+  switch (expert_mode) {
+    case ARIA_MOE_EXPERTS_BF16:
+      if (fc1_scale || fc2_scale) return ARIA_ERR_BAD_ARG;
+      return moe_block_run(x, w_router, fc1_w, fc2_w, nullptr, nullptr, false, gate_w, up_w, down_w, out, T, d, E, k, I, I_shared,
+                           forced_top_idx, workspace, workspace_bytes, stream, side_stream, ss);
+    case ARIA_MOE_EXPERTS_FP8:
+      if (!fp8_experts_ok(d, I, fc1_w, fc2_w, fc1_scale, fc2_scale)) return ARIA_ERR_BAD_ARG;
+      return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, false, gate_w, up_w, down_w, out, T, d, E, k, I,
+                           I_shared, forced_top_idx, workspace, workspace_bytes, stream, side_stream, ss);
+    case ARIA_MOE_EXPERTS_W8A8:
+      if (!w8a8_experts_ok(d, I, fc1_w, fc2_w, fc1_scale, fc2_scale)) return ARIA_ERR_BAD_ARG;
+      return moe_block_run(x, w_router, fc1_w, fc2_w, fc1_scale, fc2_scale, true, gate_w, up_w, down_w, out, T, d, E, k, I,
+                           I_shared, forced_top_idx, workspace, workspace_bytes, stream, side_stream, ss);
+    default:
+      return ARIA_ERR_BAD_ARG;
+  }
 }

@@ -101,6 +101,9 @@ class AriaForConditionalGeneration(nn.Module):
         if any(layer.mlp.experts.is_fp8() for layer in self.language_model.model.layers):
             raise NotImplementedError("enable_expert_parallel: the experts are quantized to fp8; expert parallelism runs on "
                                       "bf16 expert weights")
+        if self._dense_fp8_layers():
+            raise NotImplementedError("enable_expert_parallel: the attention projections and shared experts are quantized to "
+                                      "fp8 (quantize_dense_fp8); expert parallelism runs on bf16 dense weights")
         t = self.config.text_config
         W, r = dist.get_world_size(group), dist.get_rank(group)
         tr = FusedPeerTransport(max_tokens, t.hidden_size, t.moe_intermediate_size, t.moe_num_experts, t.moe_topk, self.device, group)
@@ -116,12 +119,64 @@ class AriaForConditionalGeneration(nn.Module):
         self._ep_transport = tr
         return tr
 
+    _DENSE_FP8 = (("self_attn", ("q_proj", "k_proj", "v_proj", "o_proj")),
+                  ("mlp.shared_experts", ("gate_proj", "up_proj", "down_proj")))
+
+    def _dense_fp8_layers(self):
+        """Indices of the LM layers whose attention projections or shared experts are fp8 (Fp8Linear)."""
+        from .moe_lm import Fp8Linear
+        out = []
+        for i, layer in enumerate(self.language_model.model.layers):
+            for owner, names in self._DENSE_FP8:
+                mod = layer.get_submodule(owner)
+                if any(type(getattr(mod, n)) is Fp8Linear for n in names):
+                    out.append(i)
+                    break
+        return out
+
+    @torch.no_grad()
+    def quantize_dense_fp8(self):
+        """Quantize every LM layer's attention projections (q, k, v, o) and shared experts (gate, up, down) to W8A8 in
+        place: e4m3 weights with one fp32 scale per output channel (amax / 448), Fp8Linear.  Their inputs are quantized to
+        e4m3 with one scale per row right before each GEMM (q/k/v: in input_layernorm's kernel, rmsnorm_quantize_fp8).
+        The dense linears are more than half of what a batch-1 W8A8 decode step streams.  lm_head, router, embedding and
+        the ViT stay bf16.  Layer by layer; the bf16 tensors are freed.  Independent of quantize_experts_fp8 (either mode)
+        and of the KV cache dtype.  A second call changes nothing.  Returns the model.
+        Raises NotImplementedError under expert parallelism or for a projection that is not a plain bias-free Linear
+        (e.g. LoRA-wrapped), and ValueError for non-finite weights, all before anything changes.  The captured decode graph
+        of generate() is dropped (it holds the old weight pointers); a GraphedPrefill built before the call must be rebuilt."""
+        from .moe_lm import Fp8Linear, Linear
+        layers = self.language_model.model.layers
+        if any(layer.mlp.expert_parallel is not None for layer in layers):
+            raise NotImplementedError("quantize_dense_fp8: expert parallelism is enabled; it runs on bf16 dense weights")
+        todo = []
+        for i, layer in enumerate(layers):
+            for owner, names in self._DENSE_FP8:
+                mod = layer.get_submodule(owner)
+                for name in names:
+                    lin = getattr(mod, name)
+                    if type(lin) is Fp8Linear:
+                        continue
+                    if type(lin) is not Linear or lin.bias is not None:
+                        raise NotImplementedError(f"quantize_dense_fp8: layer {i} {owner}.{name} is a {type(lin).__name__} "
+                                                  "(e.g. LoRA-wrapped) or has a bias, not a plain bias-free Linear")
+                    if not bool(torch.isfinite(lin.weight).all()):
+                        raise ValueError(f"quantize_dense_fp8: layer {i} {owner}.{name}.weight has non-finite values")
+                    todo.append((mod, name))
+        if not todo:
+            return self
+        self._decode_graph = None
+        for mod, name in todo:
+            setattr(mod, name, Fp8Linear.from_linear(getattr(mod, name)))   # drops the bf16 module
+        return self
+
     @torch.no_grad()
     def quantize_experts_fp8(self, activations: str = "bf16"):
         """Quantize every MoE layer's routed experts (`experts.fc1` / `experts.fc2`) to fp8 in place: e4m3 weights with one
         fp32 scale per (expert, output column), Fp8GroupedGEMM.  It halves the bytes of the routed experts, which are most of
         the model and most of what a decode step reads.  Layer by layer, so the peak is the bf16 model plus one layer's fp8
-        copy; the bf16 expert tensors are freed.  Attention, shared experts, router, lm_head and the ViT stay bf16.
+        copy; the bf16 expert tensors are freed.  Router, lm_head and the ViT stay bf16, and so do attention and the shared
+        experts unless quantize_dense_fp8() is called.
         `activations`: "bf16" keeps the activations in bf16 (weight-only, W8A16); "fp8" also quantizes the expert GEMMs'
         inputs to e4m3 with one scale per row (W8A8, the fp8 tensor cores).  W8A8 rounds the activations as well, so it is
         an explicit choice, never made by row count.  Both modes hold the same codes, scales and state dict; a model

@@ -81,6 +81,54 @@ class Linear(nn.Module):
         return ops.linear(x, self.weight, self.bias, act=act, residual=residual)
 
 
+class Fp8Linear(nn.Module):
+    """Linear with W8A8 weights (AriaForConditionalGeneration.quantize_dense_fp8): `weight` [out, in] torch.float8_e4m3fn,
+    K-major as nn.Linear stores it, and `weight_scale` [out] fp32, one scale per output channel (amax / 448).  Both are frozen
+    parameters, so a quantized model saves and reloads through its state dict (`...q_proj.weight`, `...q_proj.weight_scale`).
+    The input is quantized per row to e4m3 right before the GEMM (ops.permute_quantize_fp8); both scales multiply the fp32
+    accumulator before the epilogue's first bf16 rounding.  Inference only, no bias."""
+
+    def __init__(self, in_features, out_features, device=None, weight=None, weight_scale=None):
+        super().__init__()
+        self.in_features = in_features
+        self.out_features = out_features
+        if weight is None:
+            weight = torch.empty(out_features, in_features, dtype=torch.float8_e4m3fn, device=device)
+        if weight_scale is None:
+            weight_scale = torch.empty(out_features, dtype=torch.float32, device=device)
+        if weight.shape != (out_features, in_features) or weight.dtype != torch.float8_e4m3fn:
+            raise ValueError(f"weight must be [{out_features}, {in_features}] float8_e4m3fn")
+        if weight_scale.shape != (out_features,) or weight_scale.dtype != torch.float32:
+            raise ValueError(f"weight_scale must be [{out_features}] float32")
+        self.weight = nn.Parameter(weight, requires_grad=False)
+        self.weight_scale = nn.Parameter(weight_scale, requires_grad=False)
+
+    @classmethod
+    def from_linear(cls, m: "Linear") -> "Fp8Linear":
+        """e4m3 codes and output-channel scales of a bias-free Linear, bit for bit
+        `(w.float() / scale[:, None]).to(torch.float8_e4m3fn)` with scale = row amax / 448 (the row quantizer on [out, in])."""
+        w = m.weight.detach()
+        q, scale = ops.permute_quantize_fp8(w)
+        return cls(w.shape[1], w.shape[0], weight=q, weight_scale=scale)
+
+    def quantize_input(self, x: torch.Tensor):
+        """x [..., in] bf16 -> (e4m3 rows [rows, in], row scales [rows])."""
+        _reject_fp8_grad(x)
+        return ops.permute_quantize_fp8(x.reshape(-1, x.shape[-1]))
+
+    def forward(self, x, residual=None):
+        xq, xs = self.quantize_input(x)
+        return ops.linear_w8a8(xq, xs, self.weight, self.weight_scale, residual=residual).view(*x.shape[:-1], self.out_features)
+
+
+def _all_fp8(mods, what: str) -> bool:
+    """Whether the Linear modules `mods` are all Fp8Linear; a mix is an error."""
+    f = [type(m) is Fp8Linear for m in mods]
+    if any(f) and not all(f):
+        raise RuntimeError(f"{what}: the projections must all be fp8 (Fp8Linear) or all not")
+    return all(f)
+
+
 class RMSNorm(nn.Module):
     def __init__(self, d, eps, device=None):
         super().__init__()
@@ -301,7 +349,17 @@ class SharedExpertMLP(nn.Module):
         self.up_proj = Linear(self.hidden_size, self.intermediate_size, device=device)
         self.down_proj = Linear(self.intermediate_size, self.hidden_size, device=device)
 
+    def is_fp8(self) -> bool:
+        """Whether gate / up / down are W8A8 (Fp8Linear, AriaForConditionalGeneration.quantize_dense_fp8)."""
+        return _all_fp8((self.gate_proj, self.up_proj, self.down_proj), "SharedExpertMLP")
+
     def forward(self, x):
+        if self.is_fp8():
+            # x -> e4m3 rows -> SwiGLU (gate | up) -> h -> e4m3 rows -> down, the launches of the fused block's shared branch
+            xq, xs = self.gate_proj.quantize_input(x)
+            g, u = self.gate_proj, self.up_proj
+            h = ops.linear_swiglu_w8a8(xq, xs, g.weight, g.weight_scale, u.weight, u.weight_scale)
+            return self.down_proj(h).view(*x.shape[:-1], self.hidden_size)
         h = ops.linear_swiglu(x, self.gate_proj.weight, self.up_proj.weight)
         return ops.linear(h, self.down_proj.weight)
 
@@ -372,11 +430,17 @@ class MoELayer(nn.Module):
             x = hidden_states.reshape(-1, hidden_states.shape[-1])
             se = self.shared_experts
             fc1, fc2 = self.experts.fc1, self.experts.fc2
+            se_fp8 = se.is_fp8()
+            if se_fp8:
+                _reject_fp8_grad(hidden_states)
             out = ops.moe_block_fwd(x, self.router.weight, fc1.weight, fc2.weight, se.gate_proj.weight,
                                     se.up_proj.weight, se.down_proj.weight, self.router.config.moe_topk,
                                     forced_top_idx=self.router.forced_top_indices, side_stream=_side_stream(x.device),
                                     fc1_scale=fc1.weight_scale if fp8 else None, fc2_scale=fc2.weight_scale if fp8 else None,
-                                    w8a8=self.experts.fp8_activations())
+                                    w8a8=self.experts.fp8_activations(),
+                                    gate_scale=se.gate_proj.weight_scale if se_fp8 else None,
+                                    up_scale=se.up_proj.weight_scale if se_fp8 else None,
+                                    down_scale=se.down_proj.weight_scale if se_fp8 else None)
             return out.view(hidden_states.shape)
         # module-by-module path (adapter-wrapped experts, CPU stand-in ops of the host-logic tests)
         forked = shared_expert_overlapped(lambda: self.shared_experts(hidden_states), hidden_states)
@@ -453,9 +517,33 @@ class AriaAttention(nn.Module):
         self.v_proj = Linear(d, d, device=device)
         self.o_proj = Linear(d, d, device=device)
 
-    def forward(self, hidden_states, cache: KVCache, rope, residual=None, key_mask=None, position_ids=None):
+    def is_fp8(self) -> bool:
+        """Whether q / k / v / o are W8A8 (Fp8Linear, AriaForConditionalGeneration.quantize_dense_fp8)."""
+        return _all_fp8((self.q_proj, self.k_proj, self.v_proj, self.o_proj), "AriaAttention")
+
+    def _qkv(self, hidden_states, hq, outs, rows_per_batch, pos0, rope, position_ids):
+        """The fused q/k/v launch.  fp8: hq = (e4m3 rows, row scales) of hidden_states when the caller has them
+        (rmsnorm_quantize_fp8), else they are quantized here."""
+        cos, sin = rope
+        if self.is_fp8():
+            xq, xs = hq if hq is not None else self.q_proj.quantize_input(hidden_states)
+            ws = [self.q_proj, self.k_proj, self.v_proj]
+            ops.qkv_heads_w8a8(xq, xs, [m.weight for m in ws], [m.weight_scale for m in ws], outs, self.head_dim, rows_per_batch,
+                               pos0=pos0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=position_ids)
+            return
+        ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3, outs,
+                      self.head_dim, rows_per_batch, pos0=pos0, rope_mask=0b011, rope_cos=cos, rope_sin=sin,
+                      position_ids=position_ids)
+
+    def _o_proj(self, o, residual):
+        if type(self.o_proj) is Fp8Linear:
+            return self.o_proj(o, residual=residual)
+        return ops.linear(o, self.o_proj.weight, residual=residual)
+
+    def forward(self, hidden_states, cache: KVCache, rope, residual=None, key_mask=None, position_ids=None, hq=None):
         """key_mask [B, pos0+T] uint8, 1 = key masked out (padded batch); position_ids [B*T] int32 RoPE positions
-        (default: cache position pos0 + t, what LlamaModel uses when none are given)."""
+        (default: cache position pos0 + t, what LlamaModel uses when none are given).  With fp8 projections, hidden_states
+        may be the e4m3 rows [B, T, d] with hq = (the same rows, their scales [B*T]) (MoEDecoderLayer: rmsnorm_quantize_fp8)."""
         B, T, d = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
         pos0 = cache.seq_len
@@ -467,8 +555,7 @@ class AriaAttention(nn.Module):
         cos, sin = rope
         fp8 = cache.dtype == "fp8"
         k_out, v_out = (cache.k_stage, cache.v_stage) if fp8 else (kc, vc)
-        ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3,
-                      [q, k_out, v_out], hd, T, pos0=pos0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=position_ids)
+        self._qkv(hidden_states, hq, [q, k_out, v_out], T, pos0, rope, position_ids)
         Tk = pos0 + T
         scale = hd ** -0.5
         if fp8:
@@ -485,14 +572,14 @@ class AriaAttention(nn.Module):
                     ops.kv_load_fp8(kc, vc, ks, vs, k_st, v_st, pos0)
                 o = ops.attention(q[:, :, pos0:], k_st, v_st, T, Tk, scale, causal=True, key_mask=key_mask)
                 ops.kv_store_fp8(k_st[:, :, pos0:Tk], v_st[:, :, pos0:Tk], kc, vc, ks, vs, pos0)
-            return ops.linear(o, self.o_proj.weight, residual=residual)
+            return self._o_proj(o, residual)
         if T == 1:
             o = ops.attention_decode(q[:, :, pos0, :], kc, vc, Tk, scale, key_mask=key_mask).view(B, 1, d)  # strided view, no copy
         else:  # prefill, or a multi-token continuation (chunked prefill): the queries are the last T of Tk positions
             o = ops.attention(q[:, :, pos0:], kc, vc, T, Tk, scale, causal=True, key_mask=key_mask)
-        return ops.linear(o, self.o_proj.weight, residual=residual)
+        return self._o_proj(o, residual)
 
-    def decode_step(self, hidden_states, cache: KVCache, rope, state: DecodeState, residual=None):
+    def decode_step(self, hidden_states, cache: KVCache, rope, state: DecodeState, residual=None, hq=None):
         """One token per row with every position on the device (graph-replayable): the fused projection writes q, k, v
         to the state's staging rows (RoPE at state.rope_pos), kv_append moves k, v into the cache at state.write_pos, and
         the decode attention reads state.kv_len keys.  Same kernels and arithmetic as forward() at T = 1."""
@@ -500,18 +587,16 @@ class AriaAttention(nn.Module):
         H, hd = self.num_heads, self.head_dim
         kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q, k, v = state.qkv[0], state.qkv[1], state.qkv[2]
-        cos, sin = rope
-        ops.qkv_heads(hidden_states, [self.q_proj.weight, self.k_proj.weight, self.v_proj.weight], [None] * 3, [q, k, v], hd, 1,
-                      pos0=0, rope_mask=0b011, rope_cos=cos, rope_sin=sin, position_ids=state.rope_pos)
+        self._qkv(hidden_states, hq, [q, k, v], 1, 0, rope, state.rope_pos)
         if cache.dtype == "fp8":
             ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
             ops.kv_append_fp8(k[:, :, 0], v[:, :, 0], kc, vc, ks, vs, state.write_pos)
             o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask, k_scale=ks,
                                             v_scale=vs).view(B, 1, d)
-            return ops.linear(o, self.o_proj.weight, residual=residual)
+            return self._o_proj(o, residual)
         ops.kv_append(k[:, :, 0], v[:, :, 0], kc, vc, state.write_pos)
         o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
-        return ops.linear(o, self.o_proj.weight, residual=residual)
+        return self._o_proj(o, residual)
 
 
 class MoEDecoderLayer(nn.Module):
@@ -526,23 +611,33 @@ class MoEDecoderLayer(nn.Module):
         self.input_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, device)
         self.post_attention_layernorm = RMSNorm(config.hidden_size, config.rms_norm_eps, device)
 
+    def _attn_input(self, x, pending):
+        """input_layernorm (+ the pending MoE output) -> (h, hq, residual stream).  fp8 attention: h is the e4m3 rows and hq
+        (rows, scales), quantized in the norm's kernel, so no bf16 h is written; else hq is None."""
+        norm = self.input_layernorm
+        if self.self_attn.is_fp8():
+            _reject_fp8_grad(x)
+            if pending is None:
+                hq = ops.rmsnorm_quantize_fp8(x, norm.weight, norm.variance_epsilon)
+            else:
+                *hq, x = ops.rmsnorm_quantize_fp8(x, norm.weight, norm.variance_epsilon, pending)
+            return hq[0], (hq[0].view(-1, hq[0].shape[-1]), hq[1]), x
+        if pending is None:
+            return norm(x), None, x
+        h, x = norm(x, residual=pending)
+        return h, None, x
+
     def forward(self, x, pending, cache, rope, key_mask=None, position_ids=None):
         """x: residual stream; pending: MoE output of the previous layer not yet added (or None)."""
-        if pending is None:
-            h = self.input_layernorm(x)
-        else:
-            h, x = self.input_layernorm(x, residual=pending)
-        x = self.self_attn(h, cache, rope, residual=x, key_mask=key_mask, position_ids=position_ids)
+        h, hq, x = self._attn_input(x, pending)
+        x = self.self_attn(h, cache, rope, residual=x, key_mask=key_mask, position_ids=position_ids, hq=hq)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
     def decode_step(self, x, pending, cache, rope, state: DecodeState):
         """forward() for one token per row, positions from `state` (AriaAttention.decode_step)."""
-        if pending is None:
-            h = self.input_layernorm(x)
-        else:
-            h, x = self.input_layernorm(x, residual=pending)
-        x = self.self_attn.decode_step(h, cache, rope, state, residual=x)
+        h, hq, x = self._attn_input(x, pending)
+        x = self.self_attn.decode_step(h, cache, rope, state, residual=x, hq=hq)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 

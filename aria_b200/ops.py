@@ -214,6 +214,91 @@ def grouped_gemm_w8a8(aq: torch.Tensor, a_scale: torch.Tensor, weight: torch.Ten
     return out
 
 
+def _run_gemm_w8a8(d: L.GemmDesc, a_scale: torch.Tensor, scales: Sequence[torch.Tensor], ref: torch.Tensor, what: str):
+    arr = (C.c_void_p * 3)(*[s.data_ptr() for s in scales], *([None] * (3 - len(scales))))
+    with torch.cuda.device(ref.device):
+        L.check(L.load().aria_gemm_w8a8(C.byref(d), _p(a_scale), C.cast(arr, C.c_void_p), _stream(ref)), what)
+
+
+def _w8a8_operands(xq: torch.Tensor, x_scale: torch.Tensor, weights: Sequence[torch.Tensor], scales: Sequence[torch.Tensor],
+                   what: str):
+    """Checks the e4m3 rows xq [..., K] with row scales x_scale [rows] and the e4m3 nn.Linear weights [N, K] with their
+    output-channel scales [N]; returns (xq as [rows, K], rows, N, K)."""
+    _chk(xq, torch.float8_e4m3fn), _chk(x_scale, torch.float32, align=4)
+    K = xq.shape[-1]
+    x2 = xq.reshape(-1, K)
+    N = weights[0].shape[0]
+    for w, sc in zip(weights, scales):
+        _chk(w, torch.float8_e4m3fn), _chk(sc, torch.float32)
+        if w.shape != (N, K) or sc.shape != (N,):
+            raise ValueError(f"{what}: weight {tuple(w.shape)} / scale {tuple(sc.shape)} do not fit rows of {K} and {N} outputs")
+    if x_scale.shape != (x2.shape[0],):
+        raise ValueError(f"{what}: x_scale {tuple(x_scale.shape)} does not fit {x2.shape[0]} rows")
+    return x2, x2.shape[0], N, K
+
+
+def linear_w8a8(xq: torch.Tensor, x_scale: torch.Tensor, weight: torch.Tensor, weight_scale: torch.Tensor,
+                residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """W8A8 nn.Linear (+ residual): e4m3 rows xq [..., K] with row scales x_scale [rows] (permute_quantize_fp8,
+    rmsnorm_quantize_fp8), e4m3 weight [N, K] with output-channel scales weight_scale [N] -> bf16 [..., N].  The fp32 accumulator
+    is multiplied by x_scale[row] * weight_scale[col] before the first bf16 rounding; the rest is `linear`'s epilogue."""
+    x2, M, N, K = _w8a8_operands(xq, x_scale, [weight], [weight_scale], "linear_w8a8")
+    out = torch.empty((M, N), dtype=bf16, device=xq.device)
+    d = L.GemmDesc()
+    d.a, d.lda, d.m, d.n, d.k = x2.data_ptr(), K, M, N, K
+    d.b[0] = weight.data_ptr()
+    d.n_seg, d.b_layout, d.num_groups = 1, L.B_NK, 1
+    d.epilogue = L.EPI_LINEAR
+    if residual is not None:
+        r2 = _chk(residual).reshape(-1, N)
+        d.residual, d.ldr = r2.data_ptr(), N
+    d.out[0], d.ldo = out.data_ptr(), N
+    _run_gemm_w8a8(d, x_scale, [weight_scale], xq, "linear_w8a8")
+    return out.view(*xq.shape[:-1], N)
+
+
+def linear_swiglu_w8a8(xq: torch.Tensor, x_scale: torch.Tensor, gate_w: torch.Tensor, gate_scale: torch.Tensor,
+                       up_w: torch.Tensor, up_scale: torch.Tensor) -> torch.Tensor:
+    """linear_swiglu with e4m3 operands (see linear_w8a8): silu(gate) * up, each accumulator scaled before rounding."""
+    x2, M, N, K = _w8a8_operands(xq, x_scale, [gate_w, up_w], [gate_scale, up_scale], "linear_swiglu_w8a8")
+    out = torch.empty((M, N), dtype=bf16, device=xq.device)
+    d = L.GemmDesc()
+    d.a, d.lda, d.m, d.n, d.k = x2.data_ptr(), K, M, N, K
+    d.b[0], d.b[1] = gate_w.data_ptr(), up_w.data_ptr()
+    d.n_seg, d.b_layout, d.num_groups = 2, L.B_NK, 1
+    d.epilogue = L.EPI_SWIGLU
+    d.out[0], d.ldo = out.data_ptr(), N
+    _run_gemm_w8a8(d, x_scale, [gate_scale, up_scale], xq, "linear_swiglu_w8a8")
+    return out.view(*xq.shape[:-1], N)
+
+
+def qkv_heads_w8a8(xq: torch.Tensor, x_scale: torch.Tensor, weights: Sequence[torch.Tensor], scales: Sequence[torch.Tensor],
+                   outs: Sequence[torch.Tensor], head_dim: int, rows_per_batch: int, pos0: int = 0, rope_mask: int = 0,
+                   rope_cos: Optional[torch.Tensor] = None, rope_sin: Optional[torch.Tensor] = None,
+                   position_ids: Optional[torch.Tensor] = None):
+    """qkv_heads with e4m3 operands (see linear_w8a8): the q/k/v projections of xq, RoPE, scattered head-major."""
+    x2, M, N, K = _w8a8_operands(xq, x_scale, weights, scales, "qkv_heads_w8a8")
+    d = L.GemmDesc()
+    d.a, d.lda, d.m, d.n, d.k = x2.data_ptr(), K, M, N, K
+    d.n_seg, d.b_layout, d.num_groups = len(weights), L.B_NK, 1
+    d.epilogue = L.EPI_HEADS
+    o0 = outs[0]
+    for s, (w, o) in enumerate(zip(weights, outs)):
+        _chk(o)
+        assert o.shape[1:] == o0.shape[1:] and o.stride() == o0.stride()
+        d.b[s] = w.data_ptr()
+        d.out[s] = o.data_ptr()
+    d.head_dim, d.head_ld = head_dim, o0.shape[-1]
+    d.rows_per_batch, d.pos0 = rows_per_batch, pos0
+    d.stride_b, d.stride_h = o0.stride(0), o0.stride(1)
+    d.rope_mask = rope_mask
+    if rope_mask:
+        d.rope_cos, d.rope_sin = _chk(rope_cos).data_ptr(), _chk(rope_sin).data_ptr()
+    if position_ids is not None:
+        d.position_ids = _chk(position_ids, torch.int32).data_ptr()
+    _run_gemm_w8a8(d, x_scale, scales, xq, "qkv_heads_w8a8")
+
+
 def grouped_gemm_regions(a_buf: torch.Tensor, b: torch.Tensor, starts: torch.Tensor, counts: torch.Tensor, rows_hint: int,
                          swiglu: bool = False, group_mod: int = 0, out: Optional[torch.Tensor] = None,
                          out_group_base: Optional[torch.Tensor] = None, out_group_row0: Optional[torch.Tensor] = None,
@@ -514,11 +599,14 @@ def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, 
                   up_w: Optional[torch.Tensor], down_w: Optional[torch.Tensor], k: int,
                   forced_top_idx: Optional[torch.Tensor] = None, side_stream: Optional[torch.cuda.Stream] = None,
                   fc1_scale: Optional[torch.Tensor] = None, fc2_scale: Optional[torch.Tensor] = None,
-                  w8a8: bool = False) -> torch.Tensor:
+                  w8a8: bool = False, gate_scale: Optional[torch.Tensor] = None, up_scale: Optional[torch.Tensor] = None,
+                  down_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """MoELayer.forward (moe_lm.py:548-577) as one C-ABI call (`aria_moe_block_fwd`): x [T, d] -> [T, d].
     With fc1_scale [E, 2I] / fc2_scale [E, d] fp32, fc1_w / fc2_w are e4m3 (quantize_fp8_cols) and the call is
     `aria_moe_block_fwd_fp8`; with w8a8=True as well, the weights are K-major (see grouped_gemm_w8a8), the activations are
-    quantized per row too and the call is `aria_moe_block_fwd_w8a8`."""
+    quantized per row too and the call is `aria_moe_block_fwd_w8a8`.
+    With gate_scale / up_scale [I_shared] and down_scale [d] fp32, the shared experts' weights are e4m3 nn.Linear weights
+    (W8A8, see linear_w8a8) and the call is `aria_moe_block_fwd_shared_fp8` in the expert mode given by the other arguments."""
     fp8 = fc1_scale is not None or fc2_scale is not None
     if fp8 and (fc1_scale is None or fc2_scale is None):
         raise ValueError("moe_block_fwd: give both fc1_scale and fc2_scale, or neither")
@@ -536,21 +624,37 @@ def moe_block_fwd(x: torch.Tensor, w_router: torch.Tensor, fc1_w: torch.Tensor, 
     if fp8:
         _chk(fc1_scale, torch.float32), _chk(fc2_scale, torch.float32)
         assert fc1_scale.shape == (E, 2 * I) and fc2_scale.shape == (E, d)
+    shared_fp8 = gate_scale is not None or up_scale is not None or down_scale is not None
+    if shared_fp8 and (gate_scale is None or up_scale is None or down_scale is None or gate_w is None):
+        raise ValueError("moe_block_fwd: fp8 shared experts need their weights and all three scales")
     Is = 0
     if gate_w is not None:
-        _chk(gate_w), _chk(up_w), _chk(down_w)
+        sdt = torch.float8_e4m3fn if shared_fp8 else bf16
+        _chk(gate_w, sdt), _chk(up_w, sdt), _chk(down_w, sdt)
         Is = gate_w.shape[0]
         assert gate_w.shape == (Is, d) and up_w.shape == (Is, d) and down_w.shape == (d, Is)
+    if shared_fp8:
+        _chk(gate_scale, torch.float32), _chk(up_scale, torch.float32), _chk(down_scale, torch.float32)
+        assert gate_scale.shape == (Is,) and up_scale.shape == (Is,) and down_scale.shape == (d,)
     if forced_top_idx is not None:
         _chk(forced_top_idx, torch.int32, align=4)
         assert forced_top_idx.shape == (T, k)
     lib = L.load()
-    nbytes = lib.aria_moe_block_fwd_workspace_bytes(T, d, E, k, I, Is)
+    if shared_fp8:
+        nbytes = lib.aria_moe_block_fwd_shared_fp8_workspace_bytes(T, d, E, k, I, Is)
+    else:
+        nbytes = lib.aria_moe_block_fwd_workspace_bytes(T, d, E, k, I, Is)
     ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
     out = torch.empty((T, d), dtype=bf16, device=x.device)
     side = C.c_void_p(side_stream.cuda_stream) if side_stream is not None else None
     with torch.cuda.device(x.device):
-        if w8a8:
+        if shared_fp8:
+            mode, name = (L.MOE_EXPERTS_W8A8, "w8a8") if w8a8 else ((L.MOE_EXPERTS_FP8, "fp8") if fp8 else (L.MOE_EXPERTS_BF16, "bf16"))
+            L.check(lib.aria_moe_block_fwd_shared_fp8(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(fc1_scale), _p(fc2_scale), mode,
+                                                      _p(gate_w), _p(up_w), _p(down_w), _p(gate_scale), _p(up_scale),
+                                                      _p(down_scale), _p(out), T, d, E, k, I, Is, _p(forced_top_idx), _p(ws), nbytes,
+                                                      _stream(x), side), f"moe_block_fwd_{name}_shared_fp8")
+        elif w8a8:
             L.check(lib.aria_moe_block_fwd_w8a8(_p(x), _p(w_router), _p(fc1_w), _p(fc2_w), _p(fc1_scale), _p(fc2_scale),
                                                 _p(gate_w), _p(up_w), _p(down_w), _p(out), T, d, E, k, I, Is, _p(forced_top_idx),
                                                 _p(ws), nbytes, _stream(x), side), "moe_block_fwd_w8a8")
@@ -585,6 +689,24 @@ def rmsnorm(x: torch.Tensor, weight: torch.Tensor, eps: float, residual: Optiona
     with torch.cuda.device(x.device):
         L.check(L.load().aria_rmsnorm(_p(x), _p(residual), _p(weight), _p(out), _p(s), rows, d, eps, _stream(x)), "rmsnorm")
     return out if residual is None else (out, s)
+
+
+def rmsnorm_quantize_fp8(x: torch.Tensor, weight: torch.Tensor, eps: float, residual: Optional[torch.Tensor] = None):
+    """rmsnorm whose bf16 output is quantized per row in the same kernel: returns (q, scale) or, with residual,
+    (q, scale, x + residual); q [..., d] float8_e4m3fn and scale [rows] fp32 are bit for bit
+    permute_quantize_fp8(rmsnorm(x, weight, eps, residual)[0]).  d <= 4096."""
+    _chk(x), _chk(weight)
+    d = x.shape[-1]
+    rows = x.numel() // d
+    q = torch.empty(x.shape, dtype=torch.float8_e4m3fn, device=x.device)
+    scale = torch.empty((rows,), dtype=torch.float32, device=x.device)
+    s = torch.empty_like(x) if residual is not None else None
+    if residual is not None:
+        _chk(residual)
+    with torch.cuda.device(x.device):
+        L.check(L.load().aria_rmsnorm_quantize_fp8(_p(x), _p(residual), _p(weight), _p(q), _p(scale), _p(s), rows, d, eps,
+                                                   _stream(x)), "rmsnorm_quantize_fp8")
+    return (q, scale) if residual is None else (q, scale, s)
 
 
 def layernorm(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, eps: float) -> torch.Tensor:

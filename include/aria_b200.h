@@ -135,6 +135,17 @@ int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, const void* 
                            const int32_t* group_offsets, int64_t rows, int64_t k, int64_t n, int32_t num_groups, int32_t epilogue,
                            aria_stream_t stream);
 
+/* W8A8 dense GEMM for nn.Linear weights: aria_gemm's descriptor (b_layout ARIA_B_NK, num_groups 1, no group offsets or
+ * counts) with a = e4m3 [m, k] (row stride lda, in elements = bytes) and b[s] = e4m3 [n, k] weights, one per segment.
+ * a_scale [m] fp32 is the row scale of a (aria_permute_quantize_fp8_rows or aria_rmsnorm_quantize_fp8); b_scale[s] [n] fp32
+ * the column scales of b[s] (aria_permute_quantize_fp8_rows on the [n, k] weight: one scale per output channel).  The fp32
+ * accumulator of (row r, column c of segment s) is multiplied by a_scale[r] * b_scale[s][c] before the epilogue's first bf16
+ * rounding; every rounding point after that is aria_gemm's.  Epilogues: ARIA_EPI_LINEAR (bias, act, residual), ARIA_EPI_SWIGLU
+ * (n_seg = 2: b[0] = gate, b[1] = up) and ARIA_EPI_HEADS (RoPE at pos0 or position_ids).  k % 128 == 0, n % 64 == 0
+ * (n % 128 == 0 for HEADS and for LINEAR with n_seg > 1); a, out, b[s] and residual 16-byte aligned, b_scale[s] 16-byte
+ * aligned, lda % 16 == 0.  Every argument is checked before any CUDA call. */
+int aria_gemm_w8a8(const aria_gemm_desc_t* desc, const float* a_scale, const float* const b_scale[3], aria_stream_t stream);
+
 /* Weight gradient of a (grouped) linear layer — backward of gmm / F.linear:
  *   out[g, m, n] = sum_{r in group g} a[r, m] * b[r, n]   a [rows, md] (row stride lda), b [rows, nd] (ldb), out [G, md, nd] bf16.
  * group_offsets: device int32 row offsets, non-decreasing, any values (densely packed groups as the reference's dispatcher
@@ -213,6 +224,20 @@ int aria_moe_block_fwd_w8a8(const void* x, const void* w_router, const void* fc1
                             const float* fc2_scale, const void* gate_w, const void* up_w, const void* down_w, void* out, int64_t T,
                             int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared, const int32_t* forced_top_idx,
                             void* workspace, int64_t workspace_bytes, aria_stream_t stream, aria_stream_t side_stream);
+/* The same block with W8A8 shared experts, in any expert mode: expert_mode ARIA_MOE_EXPERTS_BF16 (fc1_scale / fc2_scale NULL,
+ * as aria_moe_block_fwd), _FP8 (as aria_moe_block_fwd_fp8) or _W8A8 (as aria_moe_block_fwd_w8a8).  gate_w / up_w [I_shared, d]
+ * and down_w [d, I_shared] are e4m3 nn.Linear weights with one fp32 scale per output channel, gate_scale / up_scale
+ * [I_shared], down_scale [d].  The shared branch quantises x per row, runs aria_gemm_w8a8 (SwiGLU), quantises h per row and
+ * runs aria_gemm_w8a8 (LINEAR).  I_shared > 0, d and I_shared % 128 == 0 and <= 4096, plus the expert mode's constraints.
+ * workspace: aria_moe_block_fwd_shared_fp8_workspace_bytes(...) bytes, 16-byte aligned. */
+enum { ARIA_MOE_EXPERTS_BF16 = 0, ARIA_MOE_EXPERTS_FP8 = 1, ARIA_MOE_EXPERTS_W8A8 = 2 };
+int64_t aria_moe_block_fwd_shared_fp8_workspace_bytes(int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared);
+int aria_moe_block_fwd_shared_fp8(const void* x, const void* w_router, const void* fc1_w, const void* fc2_w, const float* fc1_scale,
+                                  const float* fc2_scale, int32_t expert_mode, const void* gate_w, const void* up_w,
+                                  const void* down_w, const float* gate_scale, const float* up_scale, const float* down_scale,
+                                  void* out, int64_t T, int32_t d, int32_t E, int32_t k, int32_t I, int32_t I_shared,
+                                  const int32_t* forced_top_idx, void* workspace, int64_t workspace_bytes, aria_stream_t stream,
+                                  aria_stream_t side_stream);
 
 /* ---- backward of the MoE block (BASELINE cfg 5; autograd through moe_lm.py:548-577) ---- */
 /* h = bf16(bf16(silu(g)) * u) with g = h1[:, :I], u = h1[:, I:]  (unfused `glu`, moe_lm.py:505-507; training keeps h1). */
@@ -247,6 +272,11 @@ int aria_router_aux_bwd(const void* logits, const int32_t* counts, void* dlogits
  * If residual != NULL: first h = bf16(x + residual), written to sum_out, and the norm is taken of h. */
 int aria_rmsnorm(const void* x, const void* residual, const void* weight, void* out, void* sum_out, int64_t rows,
                  int32_t d, float eps, aria_stream_t stream);
+/* aria_rmsnorm whose bf16 output row is quantised per row in the same kernel instead of being stored:
+ *   q [rows, d] e4m3, scale [rows] fp32 — bit for bit aria_rmsnorm followed by aria_permute_quantize_fp8_rows (src_token NULL).
+ * residual / sum_out as in aria_rmsnorm.  d % 8 == 0, d <= 4096; x, residual, weight, q, sum_out 16-byte aligned. */
+int aria_rmsnorm_quantize_fp8(const void* x, const void* residual, const void* weight, void* q, float* scale, void* sum_out,
+                              int64_t rows, int32_t d, float eps, aria_stream_t stream);
 /* nn.LayerNorm (Idefics2 encoder layers, projector): out = bf16((x-mean)*rstd*w + b). */
 int aria_layernorm(const void* x, const void* weight, const void* bias, void* out, int64_t rows, int32_t d,
                    float eps, aria_stream_t stream);
