@@ -20,6 +20,7 @@
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
 // aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
+// aria_attention_decode_shared_prefix: n rows per prompt decode against one shared prompt cache plus their own tail caches.
 #include <type_traits>
 
 #include "common.cuh"
@@ -580,6 +581,152 @@ __global__ void __launch_bounds__(128) attn_decode_merge(const float* __restrict
   out[static_cast<int64_t>(bh) * AT_D + d] = __float2bfloat16_rn(L > 0.f ? A / L : 0.f);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Shared-prefix decode: R = G * n rows, row r = g * n + j, attend to the prompt cache of group g (prefix, [G, H, P_max, 128])
+// and then to their own generated rows (tail, [R, H, N_max, 128]).  Row r is bit-identical to the DEVLEN kernels run on the
+// expanded layout: a cache of row r holding the prefix at [0, P_g), masked rows up to S_g = 256 * ceil(P_g / 256) and the tail
+// at [S_g, S_g + tail_len).  That is because every 256-key split of the expanded row is computed here with the same keys, key
+// order and arithmetic:
+//   - prefix splits by attn_decode_prefix_partial, one CTA per (group, head, split), which stages the split's K and V in shared
+//     memory once and runs decode_partial's loop for each of the group's n queries (warp -> key k_begin + 4 warp + 16 i + u, the
+//     same per-key update and the same 4-warp merge), one 4-warp team per query;
+//   - tail splits by the unchanged attn_decode_partial<true> on the tail cache, with lens = tail_lens;
+//   - attn_decode_merge_shared reads the live prefix splits, then the live tail splits, in the order attn_decode_merge reads
+//     the expanded row's splits.
+// Each prompt key and value is read from HBM once per (group, head) and step instead of n times.
+constexpr int SP_TEAMS = 8;                                 // 4-warp teams per prefix CTA
+constexpr int SP_SMEM = 2 * DEC_SPLIT_KEYS * AT_D * 2;      // K and V of one split: 128 KB
+
+__global__ void __launch_bounds__(128 * SP_TEAMS, 1)
+attn_decode_prefix_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
+                           const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ prefix_lens,
+                           const uint8_t* __restrict__ key_mask, int mask_stride, float* __restrict__ ws, int n, int H, int P_max,
+                           int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale_log2,
+                           int splits) {
+  extern __shared__ uint4 sp_smem[];
+  uint4* sK = sp_smem;                                      // [256 keys][16 x 16 B]
+  uint4* sV = sp_smem + DEC_SPLIT_KEYS * (AT_D / 8);
+  __shared__ float sm_m[SP_TEAMS][4], sm_l[SP_TEAMS][4], sm_a[SP_TEAMS][4][AT_D];
+  const int gh = blockIdx.x, split = blockIdx.y;
+  const int g = gh / H, h = gh % H;
+  const int len = min(prefix_lens[g], P_max);
+  const int k_begin = split * DEC_SPLIT_KEYS, k_end = min(len, k_begin + DEC_SPLIT_KEYS);
+  const __nv_bfloat16* kbase = kc + g * kv_stride_b + h * kv_stride_h;
+  const __nv_bfloat16* vbase = vc + g * kv_stride_b + h * kv_stride_h;
+  const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(g) * mask_stride : nullptr;
+  // stage the live keys of the split; masked keys and rows at or past the prefix length are never read
+  for (int i = threadIdx.x; i < (k_end - k_begin) * (AT_D / 8); i += blockDim.x) {
+    const int kk = k_begin + i / (AT_D / 8), c = i % (AT_D / 8);
+    if (km && km[kk]) continue;
+    sK[i] = __ldg(reinterpret_cast<const uint4*>(kbase + static_cast<int64_t>(kk) * AT_D) + c);
+    sV[i] = __ldg(reinterpret_cast<const uint4*>(vbase + static_cast<int64_t>(kk) * AT_D) + c);
+  }
+  __syncthreads();
+  const int team = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const __nv_bfloat16* sKb = reinterpret_cast<const __nv_bfloat16*>(sK);
+  const __nv_bfloat16* sVb = reinterpret_cast<const __nv_bfloat16*>(sV);
+  for (int j = team; j < n; j += SP_TEAMS) {
+    const int r = g * n + j;
+    // decode_partial<DEVLEN, bf16> for row r over keys [k_begin, k_end), with K and V from shared memory
+    const uint2 qv = *reinterpret_cast<const uint2*>(q + r * q_stride_b + h * q_stride_h + lane * 4);
+    const float q0 = bf16_lo(qv.x) * scale_log2, q1 = bf16_hi(qv.x) * scale_log2, q2 = bf16_lo(qv.y) * scale_log2,
+                q3 = bf16_hi(qv.y) * scale_log2;
+    float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+    for (int k0 = k_begin + warp * 4; k0 < k_end; k0 += 16) {
+      float s[4];
+      uint2 vv[4];
+      bool live[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int kk = k0 + u;
+        live[u] = kk < k_end && !(km && km[kk]);
+        if (live[u]) {
+          const uint2 kv = *reinterpret_cast<const uint2*>(sKb + (kk - k_begin) * AT_D + lane * 4);
+          vv[u] = *reinterpret_cast<const uint2*>(sVb + (kk - k_begin) * AT_D + lane * 4);
+          s[u] = q0 * bf16_lo(kv.x) + q1 * bf16_hi(kv.x) + q2 * bf16_lo(kv.y) + q3 * bf16_hi(kv.y);
+        } else {
+          s[u] = 0.f;
+          vv[u] = make_uint2(0, 0);
+        }
+      }
+#pragma unroll
+      for (int o = 16; o; o >>= 1) {
+#pragma unroll
+        for (int u = 0; u < 4; ++u) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        if (live[u]) {
+          const float m_new = fmaxf(m, s[u]);
+          const float f = exp2f(m - m_new), pw = exp2f(s[u] - m_new);
+          l = l * f + pw;
+          a0 = a0 * f + pw * bf16_lo(vv[u].x);
+          a1 = a1 * f + pw * bf16_hi(vv[u].x);
+          a2 = a2 * f + pw * bf16_lo(vv[u].y);
+          a3 = a3 * f + pw * bf16_hi(vv[u].y);
+          m = m_new;
+        }
+      }
+    }
+    // the team's 4-warp merge, as decode_partial's; named barrier 1 + team holds the team's 128 threads
+    if (lane == 0) {
+      sm_m[team][warp] = m;
+      sm_l[team][warp] = l;
+    }
+    sm_a[team][warp][lane * 4 + 0] = a0;
+    sm_a[team][warp][lane * 4 + 1] = a1;
+    sm_a[team][warp][lane * 4 + 2] = a2;
+    sm_a[team][warp][lane * 4 + 3] = a3;
+    named_bar_sync(1 + team, 128);
+    const int d = threadIdx.x & 127;
+    float M = fmaxf(fmaxf(sm_m[team][0], sm_m[team][1]), fmaxf(sm_m[team][2], sm_m[team][3]));
+    float L = 0.f, A = 0.f;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+      const float f = (sm_m[team][w] == -INFINITY) ? 0.f : exp2f(sm_m[team][w] - M);
+      L += sm_l[team][w] * f;
+      A += sm_a[team][w][d] * f;
+    }
+    float* o = ws + ((static_cast<int64_t>(r) * H + h) * splits + split) * (AT_D + 2);
+    o[d] = A;
+    if (d == 0) {
+      o[AT_D] = M;
+      o[AT_D + 1] = L;
+    }
+    named_bar_sync(1 + team, 128);  // the team's next query overwrites sm_*
+  }
+}
+
+// attn_decode_merge over the prefix splits, then the tail splits, of row r = blockIdx.x / H
+__global__ void __launch_bounds__(128) attn_decode_merge_shared(const float* __restrict__ ws_prefix, const float* __restrict__ ws_tail,
+                                                                __nv_bfloat16* __restrict__ out, int prefix_splits, int tail_splits,
+                                                                const int32_t* __restrict__ prefix_lens,
+                                                                const int32_t* __restrict__ tail_lens, int n, int H) {
+  const int rh = blockIdx.x, d = threadIdx.x;
+  const int r = rh / H;
+  const float* bp = ws_prefix + static_cast<int64_t>(rh) * prefix_splits * (AT_D + 2);
+  const float* bt = ws_tail + static_cast<int64_t>(rh) * tail_splits * (AT_D + 2);
+  const int np = min(prefix_splits, (prefix_lens[r / n] + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS);
+  const int nt = min(tail_splits, (tail_lens[r] + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS);
+  float M = -INFINITY;
+  for (int s = 0; s < np; ++s) M = fmaxf(M, bp[s * (AT_D + 2) + AT_D]);
+  for (int s = 0; s < nt; ++s) M = fmaxf(M, bt[s * (AT_D + 2) + AT_D]);
+  float L = 0.f, A = 0.f;
+  for (int s = 0; s < np; ++s) {
+    const float ms = bp[s * (AT_D + 2) + AT_D];
+    const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - M);
+    L += bp[s * (AT_D + 2) + AT_D + 1] * f;
+    A += bp[s * (AT_D + 2) + d] * f;
+  }
+  for (int s = 0; s < nt; ++s) {
+    const float ms = bt[s * (AT_D + 2) + AT_D];
+    const float f = (ms == -INFINITY) ? 0.f : exp2f(ms - M);
+    L += bt[s * (AT_D + 2) + AT_D + 1] * f;
+    A += bt[s * (AT_D + 2) + d] * f;
+  }
+  out[static_cast<int64_t>(rh) * AT_D + d] = __float2bfloat16_rn(L > 0.f ? A / L : 0.f);
+}
+
 // box of [128 rows][cols] per (head, batch): 64 columns with SW128, or the 16-column SW32 box of the HD = 80 path
 static int make_tmap_heads(CUtensorMap* tm, const void* ptr, int T, int H, int B, int64_t stride_b, int64_t stride_h,
                            uint32_t cols = 64, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
@@ -718,6 +865,51 @@ extern "C" int aria_attention_decode_devlen(const void* q, const void* k, const 
   attn_decode_merge<true><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
                                                      lens, H);
   return check_launch("attn_decode_merge");
+}
+
+extern "C" int64_t aria_attention_decode_shared_prefix_workspace_bytes(int32_t G, int32_t n, int32_t H, int32_t P_max, int32_t N_max) {
+  if (G <= 0 || n <= 0 || H <= 0 || P_max <= 0 || N_max <= 0) return -1;
+  const int64_t splits = (P_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS + (N_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
+  return static_cast<int64_t>(G) * n * H * splits * (AT_D + 2) * sizeof(float);
+}
+
+extern "C" int aria_attention_decode_shared_prefix(const void* q, const void* prefix_k, const void* prefix_v, const int32_t* prefix_lens,
+                                                   const uint8_t* prefix_mask, int64_t prefix_mask_stride, const void* tail_k,
+                                                   const void* tail_v, const int32_t* tail_lens, void* out, int32_t G, int32_t n,
+                                                   int32_t H, int32_t P_max, int32_t N_max, int64_t q_stride_b, int64_t q_stride_h,
+                                                   int64_t prefix_stride_b, int64_t prefix_stride_h, int64_t tail_stride_b,
+                                                   int64_t tail_stride_h, float scale, void* workspace, int64_t workspace_bytes,
+                                                   aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && prefix_k && prefix_v && prefix_lens && tail_k && tail_v && tail_lens && out && workspace);
+  ARIA_CHECK_ARG(G > 0 && n > 0 && H > 0 && P_max > 0 && N_max > 0 && static_cast<int64_t>(G) * n * H < (1ll << 31));
+  ARIA_CHECK_ARG(P_max <= 65535 * DEC_SPLIT_KEYS && N_max <= 65535 * DEC_SPLIT_KEYS);  // splits are grid.y
+  ARIA_CHECK_ARG(q_stride_b % 4 == 0 && q_stride_h % 4 == 0);
+  // the prefix CTAs stage 16-byte vectors of each key and value row
+  ARIA_CHECK_ARG(prefix_stride_b % 8 == 0 && prefix_stride_h % 8 == 0 && tail_stride_b % 8 == 0 && tail_stride_h % 8 == 0);
+  ARIA_CHECK_ARG(!prefix_mask || (prefix_mask_stride >= P_max && prefix_mask_stride < (1ll << 31)));
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_shared_prefix_workspace_bytes(G, n, H, P_max, N_max));
+  const int R = G * n;
+  const int p_splits = (P_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS, t_splits = (N_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
+  float* ws_prefix = static_cast<float*>(workspace);
+  float* ws_tail = ws_prefix + static_cast<int64_t>(R) * H * p_splits * (AT_D + 2);
+  const float scale_log2 = scale * 1.4426950408889634f;
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, attn_decode_prefix_partial, SP_SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_decode_prefix_partial<<<dim3(G * H, p_splits), 128 * SP_TEAMS, SP_SMEM, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(prefix_k), static_cast<const __nv_bfloat16*>(prefix_v),
+      prefix_lens, prefix_mask, static_cast<int>(prefix_mask_stride), ws_prefix, n, H, P_max, q_stride_b, q_stride_h, prefix_stride_b,
+      prefix_stride_h, scale_log2, p_splits);
+  int rc = check_launch("attn_decode_prefix_partial");
+  if (rc) return rc;
+  attn_decode_partial<true><<<dim3(R * H, t_splits), 128, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(tail_k), static_cast<const __nv_bfloat16*>(tail_v),
+      nullptr, ws_tail, H, N_max, q_stride_b, q_stride_h, tail_stride_b, tail_stride_h, scale_log2, t_splits, tail_lens, 0);
+  rc = check_launch("attn_decode_partial");
+  if (rc) return rc;
+  attn_decode_merge_shared<<<R * H, 128, 0, stream>>>(ws_prefix, ws_tail, static_cast<__nv_bfloat16*>(out), p_splits, t_splits,
+                                                      prefix_lens, tail_lens, n, H);
+  return check_launch("attn_decode_merge_shared");
 }
 
 // The fp8 entries check what the bf16 ones check, plus the scales, and e4m3 cache strides in multiples of 16 codes (16-byte rows)

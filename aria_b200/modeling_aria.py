@@ -341,7 +341,8 @@ class AriaForConditionalGeneration(nn.Module):
     @torch.no_grad()
     def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None, *,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
-                 pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16"):
+                 pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16",
+                 num_return_sequences: int = 1):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -356,9 +357,15 @@ class AriaForConditionalGeneration(nn.Module):
         looks at the finished flag every `poll_every` tokens; the result does not depend on it.
         kv_cache_dtype: "bf16", or "fp8" for e4m3 keys and values with one scale per (row, head, token) (KVCache): the prefill
         still attends in bf16, every decode step reads the fp8 cache.  GPU only.
-        Returns [B, T + generated] int64 on the model's device (prompt ids first)."""
+        num_return_sequences n > 1 (sampling only, bf16 cache, B * n <= 1024): n continuations of every prompt.  Each prompt goes
+        through the ViT and the prefill once; its n rows then decode against that one prompt cache (SharedPrefixCache), each
+        with its own tail of generated tokens and its own sampling noise (the Philox counter is keyed by row).  Rows are grouped
+        as GenerationMixin groups them: prompt b's rows are b*n .. b*n + n - 1, and its ids are repeated for each of them.
+        Returns [B * n, T + generated] int64 on the model's device (prompt ids first)."""
         B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
-                                                   top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype)
+                                                   top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype,
+                                                   num_return_sequences)
+        n_seq = num_return_sequences
         dev = self.device
         if dev.type != "cuda":
             if do_sample or eos:
@@ -370,13 +377,14 @@ class AriaForConditionalGeneration(nn.Module):
             sampling = (float(temperature), int(top_k), float(top_p), int(seed))
         else:
             sampling = (0.0, 0, 1.0, 0)
-        # rows are device-driven, so one captured step serves every prompt length of the same 256-row bucket
-        T_max = -(-(T + max_new_tokens) // 256) * 256
-        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, kv_cache_dtype)
+        # rows are device-driven, so one captured step serves every prompt length of the same 256-row bucket; with
+        # n_seq > 1 the cache holds the prompts only (their bucket) and the generated tokens go to the tails
+        T_max = -(-(T if n_seq > 1 else T + max_new_tokens) // 256) * 256
+        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
         if g is None or g.key != key:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
-            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype)
+            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype, n_seq)
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
                                                     attention_mask=mask, num_logits_to_keep=1)
@@ -384,17 +392,20 @@ class AriaForConditionalGeneration(nn.Module):
         inputs["past_key_values"] = g.cache
         out = self.forward(**inputs)
         g.start(T, mask)
-        g.sample_and_advance(out.logits[:, -1])
+        first = out.logits[:, -1]
+        g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         n = 0                                   # decode steps replayed
         while n < max_new_tokens - 1:
             if eos and n % poll_every == 0 and g.done():
                 break
             g.graph.replay()
             n += 1
-        g.cache.seq_len = T + n
+        if n_seq == 1:
+            g.cache.seq_len = T + n             # a shared cache keeps the prompt's T; the tails hold the rest
         done = int(g.done_step.item())          # synchronises; -1 when no EOS stopped the batch
         L = done + 1 if done >= 0 else max_new_tokens
-        return torch.cat([input_ids.to(dev), g.out_tokens[:, :L]], dim=1)
+        prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
+        return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
 
     def _generate_stepwise(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask):
         """Greedy decoding through the public step API, one forward(past_key_values=...) per token: what generate() does
@@ -417,7 +428,7 @@ class AriaForConditionalGeneration(nn.Module):
 
     @staticmethod
     def _check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k, top_p, eos_token_id,
-                             pad_token_id, seed, poll_every, kv_cache_dtype="bf16"):
+                             pad_token_id, seed, poll_every, kv_cache_dtype="bf16", num_return_sequences=1):
         """All of generate()'s argument checks, on the host, before any device work -> (B, T, eos ids tuple, pad id)."""
         import math
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -425,6 +436,11 @@ class AriaForConditionalGeneration(nn.Module):
         B, T = input_ids.shape
         if B > 1024:
             raise NotImplementedError("generate(): at most 1024 rows per batch")
+        n = num_return_sequences
+        if not isinstance(n, int) or isinstance(n, bool) or n < 1:
+            raise ValueError(f"num_return_sequences must be a positive int, got {n!r}")
+        if B * n > 1024:
+            raise NotImplementedError(f"generate(): at most 1024 rows per batch, got {B} prompts x {n} sequences")
         if not isinstance(max_new_tokens, int) or max_new_tokens < 1:
             raise ValueError(f"max_new_tokens must be a positive int, got {max_new_tokens!r}")
         if attention_mask is not None and tuple(attention_mask.shape) != (B, T):
@@ -435,6 +451,10 @@ class AriaForConditionalGeneration(nn.Module):
             raise ValueError(f"seed must be an int in [0, 2**64), got {seed!r}")
         if kv_cache_dtype not in KV_CACHE_DTYPES:
             raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
+        if n > 1 and not do_sample:
+            raise ValueError("num_return_sequences > 1 needs do_sample=True: greedy rows of one prompt would all be equal")
+        if n > 1 and kv_cache_dtype == "fp8":
+            raise NotImplementedError("num_return_sequences > 1 shares a bf16 prompt cache; the fp8 KV cache is not supported")
         if do_sample:
             if not (isinstance(temperature, (int, float)) and math.isfinite(temperature) and temperature > 0):
                 raise ValueError(f"temperature must be a strictly positive float, got {temperature!r}")
@@ -464,20 +484,32 @@ class GraphedDecode:
     (`state`), the RNG offset, the finished flags, the step index and the output tokens all live in static device buffers,
     and decode_advance moves them on at the end of every replay.  The KV cache belongs to the graph: generate() prefills
     into it with forward(past_key_values=g.cache), then calls start() and sample_and_advance() for the first token.
-    `logits` is the last replayed step's logits [B, 1, V]."""
+    `logits` is the last replayed step's logits [B, 1, V].
+    group_size n > 1: B prompts decoded n times each.  The cache is a SharedPrefixCache of B prompt rows of T_max (the prompt
+    bucket) and B * n tails of max_new_tokens rounded up to 256; the state, tokens and logits have B * n rows."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
-                 kv_cache_dtype: str = "bf16"):
-        from .moe_lm import DecodeState
+                 kv_cache_dtype: str = "bf16", group_size: int = 1):
+        from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
         dev = model.device
         lm = model.language_model
         c = lm.config
-        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, kv_cache_dtype)
-        self.model, self.B, self.T_max = model, B, T_max
+        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, group_size, kv_cache_dtype)
+        self.group_size = group_size
+        self.T_max = T_max
         self.sampling, self.eos, self.pad = sampling, eos, pad
-        self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
-        self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
-        self.rope = lm.model.rope_tables(T_max, dev)   # held here: the graph reads these tables
+        if group_size == 1:
+            self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
+            self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
+            n_pos = T_max
+        else:
+            N_max = -(-max_new_tokens // 256) * 256
+            self.cache = SharedPrefixCache(c.num_hidden_layers, B, group_size, c.num_attention_heads, T_max, N_max, c.head_dim, dev)
+            self.state = SharedDecodeState(B, group_size, c.num_attention_heads, T_max, dev)
+            n_pos = T_max + N_max
+            B = B * group_size
+        self.model, self.B = model, B
+        self.rope = lm.model.rope_tables(n_pos, dev)   # held here: the graph reads these tables
         self.ids = torch.zeros(B, 1, dtype=torch.int64, device=dev)
         self.next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
         self.rng_offset = torch.zeros(1, dtype=torch.int64, device=dev)   # read as uint64 by the kernels
@@ -517,7 +549,7 @@ class GraphedDecode:
     def start(self, T: int, mask: Optional[torch.Tensor]):
         """Reset the state for a prompt of T tokens (mask: host [B, T] padding mask or None) already prefilled into
         self.cache.  The values are those of the last prompt token: the advance after the first sample moves them on."""
-        B = self.B
+        B = self.B // self.group_size      # prompts
         if mask is None:
             last = torch.full((B,), T - 1, dtype=torch.int32)
         else:
@@ -526,10 +558,18 @@ class GraphedDecode:
         if mask is not None:
             km[:, :T] = (mask == 0).to(torch.uint8)
         st = self.state
-        st.rope_pos.copy_(last)
-        st.write_pos.fill_(T - 1)
-        st.kv_len.fill_(T)
-        st.key_mask.copy_(km)
+        if self.group_size == 1:
+            st.rope_pos.copy_(last)
+            st.write_pos.fill_(T - 1)
+            st.kv_len.fill_(T)
+            st.key_mask.copy_(km)
+        else:
+            # every row of a prompt continues from its last position; its tail is empty until the first advance
+            st.rope_pos.copy_(last.repeat_interleave(self.group_size))
+            st.write_pos.fill_(-1)
+            st.kv_len.fill_(0)
+            st.prefix_lens.fill_(T)
+            st.prefix_mask.copy_(km)
         self.rng_offset.zero_()
         self.step.zero_()
         self.done_step.fill_(-1)

@@ -499,6 +499,32 @@ class DecodeState:
         self.qkv = torch.empty(3, B, H, 1, 128, dtype=bf16, device=device)  # staging rows of the step's q, k, v
 
 
+class SharedPrefixCache(KVCache):
+    """KV cache of G prompts decoded n times each (generate(num_return_sequences=n)): the KVCache of the G prompt rows
+    [G, H, T_max, head_dim], filled once by forward()'s prefill, plus per-layer tail caches tail_k[l] / tail_v[l]
+    [G*n, H, N_max, head_dim] that hold each decoded row's own tokens.  Row r = g * n + j attends to prompt g and then to its
+    tail (ops.attention_decode_shared_prefix), so the prompt's keys and values are stored and read once instead of n times.
+    bf16 only."""
+
+    def __init__(self, n_layers, G, n, H, T_max, N_max, hd, device):
+        super().__init__(n_layers, G, H, T_max, hd, device)
+        self.group_size = n
+        self.N_max = N_max
+        self.tail_k = [torch.empty(G * n, H, N_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+        self.tail_v = [torch.empty(G * n, H, N_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+
+
+class SharedDecodeState(DecodeState):
+    """DecodeState of the R = G * n rows of a SharedPrefixCache: write_pos[r] is the row's tail row and kv_len[r] its tail
+    length; prefix_lens [G] and prefix_mask [G, T_max] (1 = padded prompt key) describe the prompt each group shares."""
+
+    def __init__(self, G, n, H, T_max, device):
+        super().__init__(G * n, H, 0, device)
+        self.key_mask = None
+        self.prefix_lens = torch.zeros(G, dtype=torch.int32, device=device)
+        self.prefix_mask = torch.zeros(G, T_max, dtype=torch.uint8, device=device)
+
+
 class AriaAttention(nn.Module):
     """What `LLAMA_ATTENTION_CLASSES[config._attn_implementation]` provides at moe_lm.py:594: MHA, no bias,
     rotate-half RoPE, causal, KV cache.  q/k/v projections + RoPE + cache write are ONE GEMM launch."""
@@ -588,6 +614,12 @@ class AriaAttention(nn.Module):
         kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q, k, v = state.qkv[0], state.qkv[1], state.qkv[2]
         self._qkv(hidden_states, hq, [q, k, v], 1, 0, rope, state.rope_pos)
+        if isinstance(cache, SharedPrefixCache):
+            tk, tv = cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx]
+            ops.kv_append(k[:, :, 0], v[:, :, 0], tk, tv, state.write_pos)
+            o = ops.attention_decode_shared_prefix(q[:, :, 0], kc, vc, state.prefix_lens, tk, tv, state.kv_len, cache.group_size,
+                                                   hd ** -0.5, prefix_mask=state.prefix_mask).view(B, 1, d)
+            return self._o_proj(o, residual)
         if cache.dtype == "fp8":
             ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
             ops.kv_append_fp8(k[:, :, 0], v[:, :, 0], kc, vc, ks, vs, state.write_pos)

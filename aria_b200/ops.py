@@ -927,6 +927,48 @@ def attention_decode_devlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, l
     return out
 
 
+def attention_decode_shared_prefix(q: torch.Tensor, prefix_k: torch.Tensor, prefix_v: torch.Tensor, prefix_lens: torch.Tensor,
+                                   tail_k: torch.Tensor, tail_v: torch.Tensor, tail_lens: torch.Tensor, group_size: int,
+                                   scale: float, prefix_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Decode attention of R = G * group_size rows that share their group's prompt cache: row r = g * group_size + j attends
+    to prefix rows [0, prefix_lens[g]) of prefix_k / prefix_v [G,H,P_max,128] (minus prefix_mask [G, >= P_max] uint8, 1 = masked
+    out, any row stride), then to its own rows [0, tail_lens[r]) of tail_k / tail_v [R,H,N_max,128].  q [R,H,128] (contiguous
+    last dim, any strides); prefix_lens int32 [G], tail_lens int32 [R] on the device -> out [R, H*128].  Row r is bit-identical
+    to attention_decode_devlen on a cache that holds the prefix at [0, P), masked rows up to S = 256 * ceil(P / 256) and the tail
+    from S on; each prefix key and value is read once per (group, head).  See aria_attention_decode_shared_prefix."""
+    _chk(prefix_k), _chk(prefix_v), _chk(tail_k), _chk(tail_v)
+    _chk(prefix_lens, torch.int32, align=4), _chk(tail_lens, torch.int32, align=4)
+    if not (q.is_cuda and q.dtype == bf16 and q.dim() == 3 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
+        raise RuntimeError("attention_decode_shared_prefix: q must be a CUDA bf16 [R,H,128] tensor with a contiguous last dim")
+    if not isinstance(group_size, int) or group_size < 1:
+        raise ValueError(f"attention_decode_shared_prefix: group_size must be a positive int, got {group_size!r}")
+    R, H = q.shape[0], q.shape[1]
+    G, P_max, N_max = prefix_k.shape[0], prefix_k.shape[2], tail_k.shape[2]
+    if (q.shape[2] != 128 or R != G * group_size or prefix_k.shape != (G, H, P_max, 128) or prefix_v.shape != prefix_k.shape
+            or tail_k.shape != (R, H, N_max, 128) or tail_v.shape != tail_k.shape or prefix_lens.shape != (G,)
+            or tail_lens.shape != (R,)):
+        raise ValueError(f"attention_decode_shared_prefix: q {tuple(q.shape)}, prefix {tuple(prefix_k.shape)}, tail "
+                         f"{tuple(tail_k.shape)}, lens {tuple(prefix_lens.shape)} / {tuple(tail_lens.shape)} do not fit "
+                         f"groups of {group_size}")
+    mask_stride = 0
+    if prefix_mask is not None:
+        if not (prefix_mask.is_cuda and prefix_mask.dtype == torch.uint8 and prefix_mask.dim() == 2
+                and prefix_mask.stride(-1) == 1 and prefix_mask.shape[0] == G and prefix_mask.shape[1] >= P_max):
+            raise RuntimeError("attention_decode_shared_prefix: prefix_mask must be CUDA uint8 [G, >= P_max] with contiguous rows")
+        mask_stride = prefix_mask.stride(0)
+    lib = L.load()
+    ws_bytes = lib.aria_attention_decode_shared_prefix_workspace_bytes(G, group_size, H, P_max, N_max)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    out = torch.empty((R, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_decode_shared_prefix(_p(q), _p(prefix_k), _p(prefix_v), _p(prefix_lens), _p(prefix_mask),
+                                                        mask_stride, _p(tail_k), _p(tail_v), _p(tail_lens), _p(out), G, group_size,
+                                                        H, P_max, N_max, q.stride(0), q.stride(1), prefix_k.stride(0),
+                                                        prefix_k.stride(1), tail_k.stride(0), tail_k.stride(1), scale, _p(ws),
+                                                        ws_bytes, _stream(q)), "attention_decode_shared_prefix")
+    return out
+
+
 # ------------------------------------------------------------------------------------------- generation
 def sample_tokens(logits: torch.Tensor, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
                   rng_offset: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,

@@ -381,6 +381,23 @@ int aria_attention_decode_devlen_fp8(const void* q, const void* k, const void* v
                                      int32_t H, int32_t T_max, int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b,
                                      int64_t kv_stride_h, int64_t scale_stride_b, int64_t scale_stride_h, float scale,
                                      void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* Single-token decode of R = G*n rows in G groups of n (row r = g*n + j) that share a prompt (prefix) cache.  Row r attends to
+ * prefix rows [0, min(prefix_lens[g], P_max)) of prefix_k / prefix_v [G,H,P_max,128] (strides prefix_stride_b / _h) minus the
+ * keys of prefix_mask [G, >= P_max] uint8 (row stride prefix_mask_stride, 1 = masked out; or NULL), then to its own tail rows
+ * [0, min(tail_lens[r], N_max)) of tail_k / tail_v [R,H,N_max,128].  prefix_lens int32 [G] and tail_lens int32 [R] are DEVICE
+ * values (one captured step serves every length); q as aria_attention_decode's with R rows; out [R, H*128].
+ * Result: row r is bit-identical to aria_attention_decode_devlen on the expanded layout, a cache of row r that holds the
+ * prefix at [0, P_g), masked rows [P_g, S_g) with S_g = 256*ceil(P_g/256), the tail at [S_g, S_g + tail_lens[r]), and
+ * lens[r] = S_g + tail_lens[r].  Rows at or past the lengths, and masked prefix rows, are never read.  Each prefix key and value is
+ * read from HBM once per (group, head).  Cache strides are multiples of 8 elements.
+ * workspace: aria_attention_decode_shared_prefix_workspace_bytes(G, n, H, P_max, N_max) (-1 for a non-positive size). */
+int aria_attention_decode_shared_prefix(const void* q, const void* prefix_k, const void* prefix_v, const int32_t* prefix_lens,
+                                        const uint8_t* prefix_mask, int64_t prefix_mask_stride, const void* tail_k, const void* tail_v,
+                                        const int32_t* tail_lens, void* out, int32_t G, int32_t n, int32_t H, int32_t P_max,
+                                        int32_t N_max, int64_t q_stride_b, int64_t q_stride_h, int64_t prefix_stride_b,
+                                        int64_t prefix_stride_h, int64_t tail_stride_b, int64_t tail_stride_h, float scale,
+                                        void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+int64_t aria_attention_decode_shared_prefix_workspace_bytes(int32_t G, int32_t n, int32_t H, int32_t P_max, int32_t N_max);
 
 /* ------------------------------------------------------------------------------------------------
  * Generation: sampling, KV append, decode-state advance (one decode step has no host integer in it)
