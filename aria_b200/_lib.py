@@ -104,7 +104,9 @@ SIGNATURES = {
     "aria_attention_decode_shared_prefix": (i32, [vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i64, i64,
                                                   i64, i64, i64, f32, vp, i64, vp]),
     "aria_attention_decode_shared_prefix_workspace_bytes": (i64, [i32, i32, i32, i32, i32]),
+    "aria_attention_prefill_shared_prefix": (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i64, i64, i64, f32, vp]),
     "aria_kv_append": (i32, [vp, vp, i64, i64, vp, vp, i64, i64, vp, i32, i32, i32, vp]),
+    "aria_kv_scatter_tails": (i32, [vp, vp, i64, vp, vp, i64, i64, vp, i32, i32, i32, i32, i32, vp]),
     "aria_kv_store_fp8": (i32, [vp, vp, i64, i64, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, vp]),
     "aria_kv_append_fp8": (i32, [vp, vp, i64, i64, vp, vp, vp, vp, i64, i64, i64, i64, vp, i32, i32, i32, vp]),
     "aria_kv_load_fp8": (i32, [vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, i64, i32, i32, i32, i32, vp]),

@@ -60,13 +60,77 @@ struct AttnParams {
   int n_q_tiles;
 };
 
+// Suffix prefill over a shared prefix (aria_attention_prefill_shared_prefix): the queries and the suffix keys are B segments
+// packed along one sequence, segment b = rows [cu[b], cu[b + 1]); every query also sees the P keys of one prefix cache.
+struct SharedPrefixParams {
+  const int32_t* cu;  // [n_seg + 1] device segment starts
+  int n_seg;
+  int P;
+};
+
+// The key tiles of one 128-query tile [q0, q_end) of the shared-prefix prefill, in order: the prefix tiles at rows 128 j, then,
+// for each segment present in the query tile, 128-key tiles aligned at the segment's start up to its last query in the tile.
+// The producer and every consumer thread walk the same sequence, one tile per step.
+struct SharedTileWalk {
+  const int32_t* cu;
+  int n_seg, n_pre, q_end;
+  int b, c, e, t;   // current segment, its start / end, tile index inside it
+  int k0, seg_c;    // the current tile: first key row (prefix or packed) and segment start (-1 for a prefix tile)
+
+  __device__ __forceinline__ static int seg_tiles(int c, int e, int q_end) {
+    return e > c ? (min(e, q_end) - 1 - c) / AT_BN + 1 : 0;
+  }
+  __device__ __forceinline__ void init(const SharedPrefixParams& sp, int q0, int q_end_) {
+    cu = sp.cu;
+    n_seg = sp.n_seg;
+    n_pre = (sp.P + AT_BN - 1) / AT_BN;
+    q_end = q_end_;
+    b = packed_segment(cu, n_seg, q0);
+    c = cu[b];
+    e = cu[b + 1];
+    t = -1;
+  }
+  // total tiles (prefix + suffix); reads the segment starts without moving the walk
+  __device__ __forceinline__ int count() const {
+    int n = n_pre, cc = c, ee = e, bb = b;
+    while (bb < n_seg && cc < q_end) {
+      n += seg_tiles(cc, ee, q_end);
+      ++bb;
+      cc = max(ee, cc);
+      ee = bb < n_seg ? cu[bb + 1] : cc;
+    }
+    return n;
+  }
+  // move to tile j (called for j = 0, 1, 2, ... in order)
+  __device__ __forceinline__ void step(int j) {
+    if (j < n_pre) {
+      k0 = j * AT_BN;
+      seg_c = -1;
+      return;
+    }
+    ++t;
+    while (t >= seg_tiles(c, e, q_end) && b < n_seg) {
+      ++b;
+      c = max(e, c);
+      e = b < n_seg ? cu[b + 1] : c;
+      t = 0;
+    }
+    k0 = c + t * AT_BN;
+    seg_c = c;
+  }
+};
+
 // HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM); LSE: also store the row logsumexp
 // (what the backward needs to recompute P).  tmK16 / tmV16: 16-column SW32 boxes of columns 64-79 (HD = 80 only).
-template <int HD, bool CAUSAL, bool LSE>
-__global__ void __launch_bounds__(AT_THREADS, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmK16,
-                const __grid_constant__ CUtensorMap tmV16, const AttnParams p) {
+// SHARED (HD = 128): the shared-prefix suffix prefill; the keys walk the prefix (tmPK / tmPV, rows [0, sp.P)) and then the
+// query tile's segments of the packed suffix (tmK / tmV), SharedTileWalk; a query sees the prefix and its own segment up to
+// itself.  A key masked for a row adds exact zeros to that row, so each row's arithmetic is: the prefix tiles, then its own
+// segment's tiles, whatever else shares its query tile.
+template <int HD, bool CAUSAL, bool LSE, bool SHARED>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                              const CUtensorMap& tmK16, const CUtensorMap& tmV16, const CUtensorMap& tmPK,
+                                              const CUtensorMap& tmPV, const AttnParams& p, const SharedPrefixParams& sp) {
+  static_assert(!SHARED || (HD == 128 && !CAUSAL && !LSE), "the shared-prefix prefill runs at head dim 128 with its own mask");
   constexpr int S = AttnCfg<HD>::STAGES, KVT = AttnCfg<HD>::KV_TILE, NO = AttnCfg<HD>::NO;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -89,6 +153,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int pos_off = p.Tk - p.Tq;
   int n_kv = (p.Tk + AT_BN - 1) / AT_BN;
   if (CAUSAL) n_kv = min(n_kv, (pos_off + min(q0 + AT_BM, p.Tq) - 1) / AT_BN + 1);
+  SharedTileWalk walk;
+  if constexpr (SHARED) {
+    walk.init(sp, q0, min(q0 + AT_BM, p.Tq));
+    n_kv = walk.count();
+  }
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmQ);
@@ -120,6 +189,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       for (int j = 0; j < n_kv; ++j) {
         const int s = j % S;
         const uint32_t ph = ((j / S) & 1) ^ 1;
+        if constexpr (SHARED) {
+          walk.step(j);
+          const CUtensorMap* mk = walk.seg_c < 0 ? &tmPK : &tmK;
+          const CUtensorMap* mv = walk.seg_c < 0 ? &tmPV : &tmV;
+          mbar_wait(&k_empty[s], ph);
+          mbar_arrive_expect_tx(&k_full[s], KVT);
+          tma_load_4d(sK + s * KVT, mk, &k_full[s], 0, walk.k0, h, 0);
+          tma_load_4d(sK + s * KVT + AT_HALF, mk, &k_full[s], 64, walk.k0, h, 0);
+          mbar_wait(&v_empty[s], ph);
+          mbar_arrive_expect_tx(&v_full[s], KVT);
+          tma_load_4d(sV + s * KVT, mv, &v_full[s], 0, walk.k0, h, 0);
+          tma_load_4d(sV + s * KVT + AT_HALF, mv, &v_full[s], 64, walk.k0, h, 0);
+          continue;
+        }
         mbar_wait(&k_empty[s], ph);
         mbar_arrive_expect_tx(&k_full[s], KVT);
         tma_load_4d(sK + s * KVT, &tmK, &k_full[s], 0, j * AT_BN, h, b);
@@ -143,6 +226,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int qpos_lo = pos_off + r_lo, qpos_hi = qpos_lo + 8;
   const int kq = 2 * (lane & 3);                                  // key / column offset of this thread in an 8-wide block
   const uint8_t* km = p.key_mask ? p.key_mask + static_cast<int64_t>(b) * p.Tk : nullptr;
+  int c_lo = 0, c_hi = 0;  // SHARED: segment starts of this thread's two rows
+  if constexpr (SHARED) {
+    c_lo = sp.cu[packed_segment(sp.cu, sp.n_seg, r_lo)];
+    c_hi = sp.cu[packed_segment(sp.cu, sp.n_seg, r_lo + 8)];
+  }
   const uint32_t sQa = smem_u32(sQ) + cw * 64 * 128, sKa = smem_u32(sK), sVa = smem_u32(sV);
   const uint32_t my_turn = AT_BAR_TURN + cw, other_turn = AT_BAR_TURN + (cw ^ 1);
   // K-major k-step kk (16 columns of the head): chunk kk / 4, +32 B per step inside the chunk
@@ -190,17 +278,33 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // Online softmax of block j on sc, in place (sc becomes P in fp32).  Returns whether the row max was raised; O must then
   // be scaled by f_lo / f_hi before PV_j, which is done once PV_{j-1} has landed.
   auto softmax = [&](int j) -> bool {
-    const int k0 = j * AT_BN;
-    const bool need_mask = (k0 + AT_BN > p.Tk) || (CAUSAL && (k0 + AT_BN - 1 > pos_off + q0 + cw * 64)) || km != nullptr;
-    if (need_mask) {  // rare path (diagonal / tail / padded keys): -inf on dead keys
+    if constexpr (SHARED) {
+      // prefix tile: -inf on rows at or past P; suffix tile: -inf unless the key is in the row's segment, at or before it
+      const int k0 = walk.k0, sc_ = walk.seg_c;
+      if (sc_ >= 0 || k0 + AT_BN > sp.P) {
 #pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
+        for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int kc = k0 + 8 * jj + kq + e;
-          const bool gone = kc >= p.Tk || (km && km[kc]);
-          if (gone || (CAUSAL && kc > qpos_lo)) sc[4 * jj + e] = -INFINITY;
-          if (gone || (CAUSAL && kc > qpos_hi)) sc[4 * jj + 2 + e] = -INFINITY;
+          for (int e = 0; e < 2; ++e) {
+            const int kc = k0 + 8 * jj + kq + e;
+            if (sc_ < 0 ? kc >= sp.P : (sc_ != c_lo || kc > r_lo)) sc[4 * jj + e] = -INFINITY;
+            if (sc_ < 0 ? kc >= sp.P : (sc_ != c_hi || kc > r_lo + 8)) sc[4 * jj + 2 + e] = -INFINITY;
+          }
+        }
+      }
+    } else {
+      const int k0 = j * AT_BN;
+      const bool need_mask = (k0 + AT_BN > p.Tk) || (CAUSAL && (k0 + AT_BN - 1 > pos_off + q0 + cw * 64)) || km != nullptr;
+      if (need_mask) {  // rare path (diagonal / tail / padded keys): -inf on dead keys
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int kc = k0 + 8 * jj + kq + e;
+            const bool gone = kc >= p.Tk || (km && km[kc]);
+            if (gone || (CAUSAL && kc > qpos_lo)) sc[4 * jj + e] = -INFINITY;
+            if (gone || (CAUSAL && kc > qpos_hi)) sc[4 * jj + 2 + e] = -INFINITY;
+          }
         }
       }
     }
@@ -268,6 +372,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     for (int j = 0; j < n_kv; ++j) {
       const int s = j % S;
       const uint32_t ph = (j / S) & 1;
+      if constexpr (SHARED) walk.step(j);
       mbar_wait(&k_full[s], ph);
       named_bar_sync(my_turn, 256);
       wgmma_fence();
@@ -371,6 +476,23 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         *reinterpret_cast<uint32_t*>(orow + 8 * jj + kq) = pack_bf16(o[4 * jj + 2 * hrow] * inv_l, o[4 * jj + 2 * hrow + 1] * inv_l);
     }
   }
+}
+
+template <int HD, bool CAUSAL, bool LSE>
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmK16,
+                const __grid_constant__ CUtensorMap tmV16, const AttnParams p) {
+  attn_fwd_body<HD, CAUSAL, LSE, false>(tmQ, tmK, tmV, tmK16, tmV16, tmK, tmV, p, SharedPrefixParams{});
+}
+
+// One CTA per (head, 128 packed queries): tmQ / tmK / tmV map the packed suffix [1, H, S_tot, 128], tmPK / tmPV the prefix
+// cache [1, H, P, 128] (rows past P are outside the map: never read)
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_prefill_shared_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                  const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmPK,
+                                  const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const SharedPrefixParams sp) {
+  attn_fwd_body<128, false, false, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, sp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -820,6 +942,47 @@ extern "C" int aria_attention_fwd_lse(const void* q, const void* k, const void* 
   ARIA_CHECK_ARG(lse);
   return attention_fwd(q, k, v, out, lse, key_mask, B, H, Tq, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h, out_hd,
                        scale, causal, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int aria_attention_prefill_shared_prefix(const void* q, const void* k, const void* v, const void* prefix_k,
+                                                    const void* prefix_v, const int32_t* cu_seqlens, void* out, int32_t B, int32_t H,
+                                                    int32_t S_tot, int32_t P, int32_t P_max, int64_t q_stride_h, int64_t kv_stride_h,
+                                                    int64_t prefix_stride_h, float scale, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(q && k && v && prefix_k && prefix_v && cu_seqlens && out);
+  ARIA_CHECK_ARG(B > 0 && H > 0 && S_tot >= B && P > 0 && P <= P_max);
+  ARIA_CHECK_ARG(q_stride_h >= static_cast<int64_t>(S_tot) * AT_D && kv_stride_h >= static_cast<int64_t>(S_tot) * AT_D &&
+                 prefix_stride_h >= static_cast<int64_t>(P_max) * AT_D);
+  ARIA_CHECK_ARG(q_stride_h % 8 == 0 && kv_stride_h % 8 == 0 && prefix_stride_h % 8 == 0);
+  const int n_q_tiles = (S_tot + AT_BM - 1) / AT_BM;
+  ARIA_CHECK_ARG(static_cast<int64_t>(H) * n_q_tiles < (1ll << 31));
+  // one batch row: its stride is never stepped
+  CUtensorMap tmQ, tmK, tmV, tmPK, tmPV;
+  int rc = make_tmap_heads(&tmQ, q, S_tot, H, 1, q_stride_h * H, q_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmK, k, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmV, v, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPK, prefix_k, P, H, 1, prefix_stride_h * H, prefix_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPV, prefix_v, P, H, 1, prefix_stride_h * H, prefix_stride_h);
+  if (rc) return rc;
+  AttnParams p{};
+  p.B = 1;
+  p.H = H;
+  p.Tq = S_tot;
+  p.Tk = S_tot;
+  p.out_hd = AT_D;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.n_q_tiles = n_q_tiles;
+  const SharedPrefixParams sp{cu_seqlens, B, P};
+  constexpr int smem = AttnCfg<128>::SMEM;
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, attn_prefill_shared_prefix_kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_prefill_shared_prefix_kernel<<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      tmQ, tmK, tmV, tmPK, tmPV, p, sp);
+  return check_launch("attn_prefill_shared_prefix_kernel");
 }
 
 extern "C" int64_t aria_attention_decode_workspace_bytes(int32_t B, int32_t H, int32_t Tk) {

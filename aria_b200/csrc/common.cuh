@@ -191,4 +191,17 @@ inline int launch_persistent_pairs(const char* name, int threads, int smem, int6
 int grouped_gemm(const void* a, const void* b, const float* b_scale, void* out, const int32_t* offsets, int64_t rows,
                  int64_t k, int64_t n, int32_t groups, int32_t epilogue, cudaStream_t stream);
 
+#ifdef __CUDACC__
+// Packed sequences: n_seg segments along one row axis, segment b = rows [cu[b], cu[b + 1]) (cu nondecreasing, device).
+// The segment holding row q: the last b < n_seg with cu[b] <= q.
+__device__ __forceinline__ int packed_segment(const int32_t* cu, int n_seg, int q) {
+  int lo = 0, hi = n_seg - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (cu[mid] <= q) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+#endif
+
 }  // namespace aria

@@ -3,6 +3,7 @@
 //
 // aria_kv_append: copies the step's k and v rows ([B, H, 128] staging rows written by the q/k/v projection) into the cache
 //   at the device row pos[b].
+// aria_kv_scatter_tails: copies the packed suffix k and v rows of a shared-prefix prefill into the n tails of each prompt.
 // aria_decode_advance: after the sampler, feeds next_ids back as the next step's input, records the token, applies
 //   Hugging Face's EOS rule and advances the RoPE positions, the cache rows, the step index and the RNG offset.
 #include <cuda_bf16.h>
@@ -26,6 +27,23 @@ __global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_append_kernel(const __nv_b
   const __nv_bfloat16* src = (is_v ? v_new : k_new) + b * new_sb + h * new_sh;
   __nv_bfloat16* dst = (is_v ? vc : kc) + b * c_sb + h * c_sh + static_cast<int64_t>(p) * 128;
   reinterpret_cast<uint4*>(dst)[j] = reinterpret_cast<const uint4*>(src)[j];
+}
+
+// One CTA per (packed row s, head h): row s of segment b goes to tail row s - cu[b] of rows b * n .. b * n + n - 1
+__global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_scatter_tails_kernel(const __nv_bfloat16* __restrict__ k,
+                                                                           const __nv_bfloat16* __restrict__ v, int64_t src_sh,
+                                                                           __nv_bfloat16* __restrict__ tk, __nv_bfloat16* __restrict__ tv,
+                                                                           int64_t t_sb, int64_t t_sh, const int32_t* __restrict__ cu,
+                                                                           int B, int n, int H, int N_max) {
+  const int s = blockIdx.x / H, h = blockIdx.x % H;
+  const int b = packed_segment(cu, B, s);
+  const int row = s - cu[b];
+  if (row < 0 || row >= N_max) return;  // never past the tails
+  const bool is_v = threadIdx.x >= KV_ROW_VECS;
+  const int j = threadIdx.x % KV_ROW_VECS;
+  const uint4 x = reinterpret_cast<const uint4*>((is_v ? v : k) + h * src_sh + static_cast<int64_t>(s) * 128)[j];
+  __nv_bfloat16* dst = (is_v ? tv : tk) + h * t_sh + static_cast<int64_t>(row) * 128;
+  for (int c = 0; c < n; ++c) reinterpret_cast<uint4*>(dst + static_cast<int64_t>(b * n + c) * t_sb)[j] = x;
 }
 
 constexpr int ADV_MAX_EOS = 8;
@@ -89,6 +107,21 @@ extern "C" int aria_kv_append(const void* k_new, const void* v_new, int64_t new_
       static_cast<const __nv_bfloat16*>(k_new), static_cast<const __nv_bfloat16*>(v_new), new_stride_b, new_stride_h,
       static_cast<__nv_bfloat16*>(k_cache), static_cast<__nv_bfloat16*>(v_cache), cache_stride_b, cache_stride_h, pos, H, T_max);
   return check_launch("kv_append_kernel");
+}
+
+extern "C" int aria_kv_scatter_tails(const void* k, const void* v, int64_t src_stride_h, void* tail_k, void* tail_v,
+                                     int64_t tail_stride_b, int64_t tail_stride_h, const int32_t* cu_seqlens, int32_t B, int32_t n,
+                                     int32_t H, int32_t S_tot, int32_t N_max, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k && v && tail_k && tail_v && cu_seqlens);
+  ARIA_CHECK_ARG(B > 0 && n > 0 && H > 0 && S_tot >= B && N_max > 0);
+  ARIA_CHECK_ARG(static_cast<int64_t>(S_tot) * H < (1ll << 31) && static_cast<int64_t>(B) * n < (1ll << 31));
+  ARIA_CHECK_ARG(src_stride_h >= static_cast<int64_t>(S_tot) * 128 && tail_stride_h >= static_cast<int64_t>(N_max) * 128);
+  ARIA_CHECK_ARG(tail_stride_b >= tail_stride_h * H);  // tails of different rows do not overlap
+  ARIA_CHECK_ARG(src_stride_h % 8 == 0 && tail_stride_b % 8 == 0 && tail_stride_h % 8 == 0);
+  kv_scatter_tails_kernel<<<S_tot * H, 2 * KV_ROW_VECS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), src_stride_h, static_cast<__nv_bfloat16*>(tail_k),
+      static_cast<__nv_bfloat16*>(tail_v), tail_stride_b, tail_stride_h, cu_seqlens, B, n, H, N_max);
+  return check_launch("kv_scatter_tails_kernel");
 }
 
 extern "C" int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int64_t* out_tokens, int32_t max_steps, int32_t* step,

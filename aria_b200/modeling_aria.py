@@ -342,7 +342,7 @@ class AriaForConditionalGeneration(nn.Module):
     def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None, *,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
                  pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16",
-                 num_return_sequences: int = 1):
+                 num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -361,12 +361,26 @@ class AriaForConditionalGeneration(nn.Module):
         through the ViT and the prefill once; its n rows then decode against that one prompt cache (SharedPrefixCache), each
         with its own tail of generated tokens and its own sampling noise (the Philox counter is keyed by row).  Rows are grouped
         as GenerationMixin groups them: prompt b's rows are b*n .. b*n + n - 1, and its ids are repeated for each of them.
+        shared_prefix_len P (bf16 cache, B * n <= 1024): many questions about one image.  The first P real tokens of every row
+        (after its left padding) are one shared prefix that holds every image token, and pixel_values / pixel_mask are that
+        prefix's images, once.  The ViT and the prefix prefill run once; each row's own tokens (its suffix) are prefilled
+        against the prefix cache, packed, and all B * n rows decode against that one prefix cache, each with its own tail.
+        Positions are those GenerationMixin derives from the left-padded mask, and the result is laid out as without it.  One
+        captured step serves every call whose prefix and longest question + max_new_tokens fall in the same 256-row buckets.
         Returns [B * n, T + generated] int64 on the model's device (prompt ids first)."""
         B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
                                                    top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype,
-                                                   num_return_sequences)
+                                                   num_return_sequences, shared_prefix_len)
         n_seq = num_return_sequences
         dev = self.device
+        if shared_prefix_len is not None:
+            ids_host, lens = self._check_shared_prefix(input_ids, attention_mask, shared_prefix_len, self.config.image_token_index,
+                                                       kv_cache_dtype, n_seq)
+            if dev.type != "cuda":
+                raise NotImplementedError("aria_b200: shared_prefix_len runs on the GPU only")
+            sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
+            return self._generate_shared_prefix(input_ids, ids_host, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos,
+                                                pad, poll_every, n_seq, shared_prefix_len)
         if dev.type != "cuda":
             if do_sample or eos:
                 raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
@@ -380,7 +394,7 @@ class AriaForConditionalGeneration(nn.Module):
         # rows are device-driven, so one captured step serves every prompt length of the same 256-row bucket; with
         # n_seq > 1 the cache holds the prompts only (their bucket) and the generated tokens go to the tails
         T_max = -(-(T if n_seq > 1 else T + max_new_tokens) // 256) * 256
-        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, kv_cache_dtype)
+        key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, None, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
         if g is None or g.key != key:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
@@ -394,16 +408,47 @@ class AriaForConditionalGeneration(nn.Module):
         g.start(T, mask)
         first = out.logits[:, -1]
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
-        n = 0                                   # decode steps replayed
-        while n < max_new_tokens - 1:
-            if eos and n % poll_every == 0 and g.done():
-                break
-            g.graph.replay()
-            n += 1
+        n, L = g.run(max_new_tokens, poll_every)
         if n_seq == 1:
             g.cache.seq_len = T + n             # a shared cache keeps the prompt's T; the tails hold the rest
-        done = int(g.done_step.item())          # synchronises; -1 when no EOS stopped the batch
-        L = done + 1 if done >= 0 else max_new_tokens
+        prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
+        return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
+
+    def _generate_shared_prefix(self, input_ids, ids, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos, pad,
+                                poll_every, n_seq, P):
+        """generate(shared_prefix_len=P) on checked arguments (ids: the host copy of input_ids, lens: each row's real length,
+        from _check_shared_prefix): ViT + prefix prefill (forward()) into a SharedPrefixCache of one prompt row, the packed
+        suffix prefill (AriaMoELMModel.prefill_suffixes), the first token from each suffix's last position, then the graphed
+        decode of the B * n rows, one group."""
+        dev = self.device
+        lm = self.language_model
+        B, T = input_ids.shape
+        S = (lens - P).tolist()                      # suffix lengths, >= 1 each (checked)
+        start = (T - lens).tolist()                  # first real token of each row
+        prefix = ids[:1, start[0]:start[0] + P]
+        suffix = torch.cat([ids[b, start[b] + P:] for b in range(B)])[None]
+        cu = torch.tensor([0] + torch.tensor(S).cumsum(0).tolist(), dtype=torch.int32)
+        pos = torch.cat([torch.arange(P, P + s, dtype=torch.int32) for s in S])   # GenerationMixin's cumsum(mask) - 1
+        # the prefix and the tails are bucketed like generate()'s cache: every length in the step is a device value
+        T_max = -(-P // 256) * 256
+        N_max = -(-(max(S) + max_new_tokens) // 256) * 256
+        key = (1, T_max, max_new_tokens, sampling, eos, pad, dev, B * n_seq, N_max, "bf16")
+        g = getattr(self, "_decode_graph", None)
+        if g is None or g.key != key:
+            self._decode_graph = g = None
+            g = self._decode_graph = GraphedDecode(self, 1, T_max, max_new_tokens, sampling, eos, pad, "bf16", B * n_seq,
+                                                   N_max=N_max)
+        g.cache.seq_len = 0
+        self.forward(prefix, pixel_values, pixel_mask, past_key_values=g.cache, num_logits_to_keep=1)
+        cu_dev = cu.to(dev, non_blocking=True)
+        emb = ops.embedding(suffix.to(dev, non_blocking=True), lm.get_input_embeddings().weight)
+        x, pending = lm.model.prefill_suffixes(emb, g.cache, cu_dev, pos.to(dev, non_blocking=True))
+        last = (cu[1:] - 1).to(dev, torch.int64, non_blocking=True)
+        h, _ = lm.model.norm(x[0, last].contiguous(), residual=pending[0, last].contiguous())
+        first = lm.lm_head(h)                       # [B, V]
+        g.start_suffixes(P, S, n_seq)
+        g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
+        _, L = g.run(max_new_tokens, poll_every)
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
         return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
 
@@ -428,18 +473,20 @@ class AriaForConditionalGeneration(nn.Module):
 
     @staticmethod
     def _check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k, top_p, eos_token_id,
-                             pad_token_id, seed, poll_every, kv_cache_dtype="bf16", num_return_sequences=1):
-        """All of generate()'s argument checks, on the host, before any device work -> (B, T, eos ids tuple, pad id)."""
+                             pad_token_id, seed, poll_every, kv_cache_dtype="bf16", num_return_sequences=1, shared_prefix_len=None):
+        """All of generate()'s argument checks, on the host, before any device work -> (B, T, eos ids tuple, pad id).  With a
+        shared_prefix_len the row limit is left to _check_shared_prefix, which generate() runs next: it comes last there."""
         import math
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
             raise ValueError(f"input_ids must be [B, T] with B, T >= 1, got {tuple(input_ids.shape)}")
         B, T = input_ids.shape
-        if B > 1024:
+        rows_checked_here = shared_prefix_len is None
+        if rows_checked_here and B > 1024:
             raise NotImplementedError("generate(): at most 1024 rows per batch")
         n = num_return_sequences
         if not isinstance(n, int) or isinstance(n, bool) or n < 1:
             raise ValueError(f"num_return_sequences must be a positive int, got {n!r}")
-        if B * n > 1024:
+        if rows_checked_here and B * n > 1024:
             raise NotImplementedError(f"generate(): at most 1024 rows per batch, got {B} prompts x {n} sequences")
         if not isinstance(max_new_tokens, int) or max_new_tokens < 1:
             raise ValueError(f"max_new_tokens must be a positive int, got {max_new_tokens!r}")
@@ -475,6 +522,41 @@ class AriaForConditionalGeneration(nn.Module):
             raise ValueError(f"pad_token_id must be an int, got {pad_token_id!r}")
         return B, T, eos, pad_token_id
 
+    @staticmethod
+    def _check_shared_prefix(input_ids, attention_mask, P, image_token_index, kv_cache_dtype, n=1):
+        """generate(shared_prefix_len=P)'s checks after _check_generate_args', in this order: P, the mask, the row lengths, the
+        prefixes, the image tokens (ValueError), the fp8 cache, B * n <= 1024 (NotImplementedError).  One host copy of the ids
+        and of the mask -> (host ids [B, T], the real length of every row, host int64 [B])."""
+        if not isinstance(P, int) or isinstance(P, bool) or P < 1:
+            raise ValueError(f"shared_prefix_len must be a positive int, got {P!r}")
+        B, T = input_ids.shape
+        if attention_mask is None:
+            lens = torch.full((B,), T, dtype=torch.int64)
+        else:
+            m = attention_mask.to("cpu", torch.int64)
+            if not bool(((m == 0) | (m == 1)).all()) or not bool((m[:, 1:] >= m[:, :-1]).all()):
+                raise ValueError("shared_prefix_len needs a left-padded attention_mask (zeros, then ones, in every row)")
+            lens = m.sum(-1)
+        short = (lens <= P).nonzero()
+        if short.numel():
+            b = int(short[0])
+            raise ValueError(f"shared_prefix_len={P}: row {b} has {int(lens[b])} real tokens; every row needs the prefix and at "
+                             "least one token of its own")
+        ids = input_ids.to("cpu")
+        rows = [ids[b, T - int(lens[b]):] for b in range(B)]
+        for b in range(1, B):
+            if not torch.equal(rows[b][:P], rows[0][:P]):
+                raise ValueError(f"shared_prefix_len={P}: the first {P} real tokens of row {b} differ from those of row 0")
+        for b in range(B):
+            if bool((rows[b][P:] == image_token_index).any()):
+                raise ValueError(f"shared_prefix_len={P}: row {b} has an image token after the shared prefix; every image "
+                                 "token must be in the prefix")
+        if kv_cache_dtype == "fp8":
+            raise NotImplementedError("shared_prefix_len shares a bf16 prefix cache; the fp8 KV cache is not supported")
+        if B * n > 1024:
+            raise NotImplementedError(f"generate(): at most 1024 rows per batch, got {B} questions x {n} sequences")
+        return ids, lens
+
 
 class GraphedDecode:
     """One decode step captured as a CUDA graph and replayed token after token (AriaForConditionalGeneration.generate).
@@ -486,24 +568,27 @@ class GraphedDecode:
     into it with forward(past_key_values=g.cache), then calls start() and sample_and_advance() for the first token.
     `logits` is the last replayed step's logits [B, 1, V].
     group_size n > 1: B prompts decoded n times each.  The cache is a SharedPrefixCache of B prompt rows of T_max (the prompt
-    bucket) and B * n tails of max_new_tokens rounded up to 256; the state, tokens and logits have B * n rows."""
+    bucket) and B * n tails of max_new_tokens rounded up to 256; the state, tokens and logits have B * n rows.
+    N_max (generate(shared_prefix_len=...)): a SharedPrefixCache whose tails hold N_max rows (a multiple of 256), each row's
+    own prompt tokens and then its generated ones, for any group size."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
-                 kv_cache_dtype: str = "bf16", group_size: int = 1):
+                 kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None):
         from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
         dev = model.device
         lm = model.language_model
         c = lm.config
-        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, group_size, kv_cache_dtype)
+        self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, group_size, N_max, kv_cache_dtype)
         self.group_size = group_size
         self.T_max = T_max
         self.sampling, self.eos, self.pad = sampling, eos, pad
-        if group_size == 1:
+        if group_size == 1 and N_max is None:
             self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
             self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
             n_pos = T_max
         else:
-            N_max = -(-max_new_tokens // 256) * 256
+            if N_max is None:
+                N_max = -(-max_new_tokens // 256) * 256
             self.cache = SharedPrefixCache(c.num_hidden_layers, B, group_size, c.num_attention_heads, T_max, N_max, c.head_dim, dev)
             self.state = SharedDecodeState(B, group_size, c.num_attention_heads, T_max, dev)
             n_pos = T_max + N_max
@@ -570,11 +655,39 @@ class GraphedDecode:
             st.kv_len.fill_(0)
             st.prefix_lens.fill_(T)
             st.prefix_mask.copy_(km)
+        self._reset()
+
+    def start_suffixes(self, P: int, suffix_lens, n: int):
+        """Reset the state for one prefix of P tokens and B suffixes of suffix_lens (host ints) already prefilled: the prefix
+        into the cache's prompt row, the suffixes into the tails of their n rows each (AriaMoELMModel.prefill_suffixes).
+        Row b * n + j continues from its last suffix token at position P + S_b - 1, tail row S_b - 1."""
+        S = torch.tensor(suffix_lens, dtype=torch.int32).repeat_interleave(n)
+        st = self.state
+        st.rope_pos.copy_(S + (P - 1))
+        st.write_pos.copy_(S - 1)
+        st.kv_len.copy_(S)
+        st.prefix_lens.fill_(P)
+        st.prefix_mask.zero_()
+        self._reset()
+
+    def _reset(self):
         self.rng_offset.zero_()
         self.step.zero_()
         self.done_step.fill_(-1)
         self.finished.zero_()
         self.done_host.fill_(-1)
+
+    def run(self, max_new_tokens: int, poll_every: int):
+        """Replay the step until max_new_tokens tokens are out (the first one is sampled before) or, with EOS ids, every row has
+        finished; the host polls every poll_every steps.  -> (steps replayed, tokens to keep per row)."""
+        n = 0
+        while n < max_new_tokens - 1:
+            if self.eos and n % poll_every == 0 and self.done():
+                break
+            self.graph.replay()
+            n += 1
+        done = int(self.done_step.item())       # synchronises; -1 when no EOS stopped the batch
+        return n, (done + 1 if done >= 0 else max_new_tokens)
 
     def done(self) -> bool:
         """Whether every row has finished, from the pinned copy of done_step (waits for the work queued so far)."""

@@ -630,6 +630,22 @@ class AriaAttention(nn.Module):
         o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
         return self._o_proj(o, residual)
 
+    def prefill_suffixes(self, hidden_states, cache: SharedPrefixCache, rope, cu_seqlens, position_ids, residual=None, hq=None):
+        """Suffixes packed as one [1, S_tot] sequence (AriaMoELMModel.prefill_suffixes) against the prefix held in the cache's
+        rows [0, cache.seq_len): the fused projection writes q, k, v to a staging buffer (RoPE at position_ids), the suffixes
+        attend to the prefix and to themselves (ops.attention_prefill_shared_prefix), and their k, v rows are copied into the
+        tails of each suffix's rows (ops.kv_scatter_tails)."""
+        _, S, d = hidden_states.shape
+        H, hd = self.num_heads, self.head_dim
+        stage = torch.empty(3, 1, H, S, hd, dtype=bf16, device=hidden_states.device)
+        q, k, v = stage[0], stage[1], stage[2]
+        self._qkv(hidden_states, hq, [q, k, v], S, 0, rope, position_ids)
+        o = ops.attention_prefill_shared_prefix(q, k, v, S, cache.k[self.layer_idx], cache.v[self.layer_idx], cache.seq_len,
+                                                cu_seqlens, hd ** -0.5)
+        n = cache.group_size // (cu_seqlens.numel() - 1)    # rows per suffix
+        ops.kv_scatter_tails(k, v, S, cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx], cu_seqlens, n)
+        return self._o_proj(o.view(1, S, d), residual)
+
 
 class MoEDecoderLayer(nn.Module):
     """moe_lm.py:580-602: x + attn(rms(x)); h + moe(rms(h)).  The MoE residual add is deferred into the next
@@ -673,6 +689,13 @@ class MoEDecoderLayer(nn.Module):
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
+    def prefill_suffixes(self, x, pending, cache, rope, cu_seqlens, position_ids):
+        """forward() for packed suffixes over a shared prefix (AriaAttention.prefill_suffixes)."""
+        h, hq, x = self._attn_input(x, pending)
+        x = self.self_attn.prefill_suffixes(h, cache, rope, cu_seqlens, position_ids, residual=x, hq=hq)
+        h = self.post_attention_layernorm(x)
+        return x, self.mlp(h)
+
 
 class AriaMoELMModel(nn.Module):
     """moe_lm.py:605-636."""
@@ -711,6 +734,27 @@ class AriaMoELMModel(nn.Module):
         x, pending = inputs_embeds, None
         for layer in self.layers:
             x, pending = layer.decode_step(x, pending, cache, rope, state)
+        return x, pending
+
+    def prefill_suffixes(self, inputs_embeds, cache: SharedPrefixCache, cu_seqlens, position_ids):
+        """Prefill B suffixes that continue the one prefix already in `cache` (a SharedPrefixCache of one prompt row whose
+        forward() prefill left cache.seq_len = P).  inputs_embeds [1, S_tot, d]: the suffixes packed, suffix b at rows
+        [cu_seqlens[b], cu_seqlens[b+1]) (CUDA int32 [B+1]); position_ids CUDA int32 [S_tot], their RoPE positions.  Each
+        suffix attends to the prefix and to its own earlier rows; its k, v rows land in rows [0, S_b) of the tails
+        b*n .. b*n + n-1 (the cache's one group of B*n rows: n = cache.group_size / B).  The MoE layers see the packed rows as one
+        [1, S_tot] batch.  cache.seq_len is neither read past P nor changed.  Returns (x, pending) as forward() does."""
+        if not isinstance(cache, SharedPrefixCache) or cache.k[0].shape[0] != 1:
+            raise ValueError("prefill_suffixes needs a SharedPrefixCache holding one prefix row")
+        if cache.group_size % (cu_seqlens.numel() - 1):
+            raise ValueError(f"prefill_suffixes: {cu_seqlens.numel() - 1} suffixes do not divide the cache's {cache.group_size} rows")
+        if inputs_embeds.dim() != 3 or inputs_embeds.shape[0] != 1:
+            raise ValueError(f"prefill_suffixes: inputs_embeds must be [1, S_tot, d], got {tuple(inputs_embeds.shape)}")
+        if cache.seq_len < 1:
+            raise ValueError("prefill_suffixes: the cache holds no prefix (seq_len 0)")
+        rope = self.rope_tables(cache.T_max + cache.N_max, inputs_embeds.device)
+        x, pending = inputs_embeds, None
+        for layer in self.layers:
+            x, pending = layer.prefill_suffixes(x, pending, cache, rope, cu_seqlens, position_ids)
         return x, pending
 
 

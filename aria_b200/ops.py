@@ -969,6 +969,64 @@ def attention_decode_shared_prefix(q: torch.Tensor, prefix_k: torch.Tensor, pref
     return out
 
 
+def _packed_check(S_tot: int, cu_seqlens: torch.Tensor, what: str) -> int:
+    """Packed segments: cu_seqlens CUDA int32 [B+1] (B >= 1) and S_tot >= B rows -> B."""
+    _chk(cu_seqlens, torch.int32, align=4)
+    if cu_seqlens.dim() != 1 or cu_seqlens.numel() < 2:
+        raise ValueError(f"{what}: cu_seqlens must be int32 [B+1] with B >= 1, got {tuple(cu_seqlens.shape)}")
+    B = cu_seqlens.numel() - 1
+    if not isinstance(S_tot, int) or S_tot < B:
+        raise ValueError(f"{what}: S_tot must be an int >= B = {B} (every segment has a row), got {S_tot!r}")
+    return B
+
+
+def attention_prefill_shared_prefix(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, S_tot: int, prefix_k: torch.Tensor,
+                                    prefix_v: torch.Tensor, P: int, cu_seqlens: torch.Tensor, scale: float) -> torch.Tensor:
+    """Causal prefill of B suffixes sharing one prefix.  q / k / v [1,H,>=S_tot,128] head-major (first S_tot rows used; 128-element
+    rows as in `attention`) hold the suffixes packed: suffix b is rows [cu_seqlens[b], cu_seqlens[b+1]) (cu_seqlens CUDA int32
+    [B+1], nondecreasing from 0 to S_tot).  prefix_k / prefix_v [1,H,P_max,128]: the prefix is its rows [0, P).  The query at
+    packed row q of suffix b sees the whole prefix and the packed keys [cu_seqlens[b], q] -> out [S_tot, H*128].  With
+    P % 128 == 0, row b is bit-identical to `attention(..., causal=True)` on its own [prefix, suffix b] layout.
+    See aria_attention_prefill_shared_prefix."""
+    _attn_qkv_check(q, k, v, "attention_prefill_shared_prefix")
+    _attn_qkv_check(prefix_k, prefix_v, prefix_v, "attention_prefill_shared_prefix")
+    B = _packed_check(S_tot, cu_seqlens, "attention_prefill_shared_prefix")
+    H, P_max = q.shape[1], prefix_k.shape[2]
+    if q.shape[0] != 1 or q.shape[2] < S_tot or k.shape[:2] != (1, H) or k.shape[2] < S_tot or v.shape != k.shape:
+        raise ValueError(f"attention_prefill_shared_prefix: q {tuple(q.shape)} / k {tuple(k.shape)} must be [1, H, >= {S_tot}, 128]")
+    if prefix_k.shape != (1, H, P_max, 128) or prefix_v.shape != prefix_k.shape or prefix_v.stride() != prefix_k.stride():
+        raise ValueError(f"attention_prefill_shared_prefix: prefix {tuple(prefix_k.shape)} / {tuple(prefix_v.shape)} must be "
+                         f"[1, {H}, P_max, 128] with equal strides")
+    if not isinstance(P, int) or not 1 <= P <= P_max:
+        raise ValueError(f"attention_prefill_shared_prefix: P must be an int in [1, {P_max}], got {P!r}")
+    out = torch.empty((S_tot, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(L.load().aria_attention_prefill_shared_prefix(_p(q), _p(k), _p(v), _p(prefix_k), _p(prefix_v), _p(cu_seqlens),
+                                                              _p(out), B, H, S_tot, P, P_max, q.stride(1), k.stride(1),
+                                                              prefix_k.stride(1), scale, _stream(q)),
+                "attention_prefill_shared_prefix")
+    return out
+
+
+def kv_scatter_tails(k: torch.Tensor, v: torch.Tensor, S_tot: int, tail_k: torch.Tensor, tail_v: torch.Tensor,
+                     cu_seqlens: torch.Tensor, group_size: int):
+    """Copy packed suffix rows k / v [1,H,>=S_tot,128] (segments as in `attention_prefill_shared_prefix`) into the tails
+    tail_k / tail_v [B*group_size, H, N_max, 128]: packed row s of suffix b -> row s - cu_seqlens[b] of tails
+    b*group_size .. b*group_size + group_size - 1.  Tail rows at or past each suffix's length are left as they are."""
+    _attn_qkv_check(k, v, v, "kv_scatter_tails")
+    _chk(tail_k), _chk(tail_v)
+    B = _packed_check(S_tot, cu_seqlens, "kv_scatter_tails")
+    if not isinstance(group_size, int) or group_size < 1:
+        raise ValueError(f"kv_scatter_tails: group_size must be a positive int, got {group_size!r}")
+    H, N_max = k.shape[1], tail_k.shape[2]
+    if k.shape[0] != 1 or k.shape[2] < S_tot or tail_k.shape != (B * group_size, H, N_max, 128) or tail_v.shape != tail_k.shape:
+        raise ValueError(f"kv_scatter_tails: rows {tuple(k.shape)} and tails {tuple(tail_k.shape)} do not fit {B} suffixes x "
+                         f"{group_size} rows of {S_tot} packed rows")
+    with torch.cuda.device(k.device):
+        L.check(L.load().aria_kv_scatter_tails(_p(k), _p(v), k.stride(1), _p(tail_k), _p(tail_v), tail_k.stride(0), tail_k.stride(1),
+                                               _p(cu_seqlens), B, group_size, H, S_tot, N_max, _stream(k)), "kv_scatter_tails")
+
+
 # ------------------------------------------------------------------------------------------- generation
 def sample_tokens(logits: torch.Tensor, temperature: float = 0.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
                   rng_offset: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,

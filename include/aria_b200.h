@@ -398,6 +398,19 @@ int aria_attention_decode_shared_prefix(const void* q, const void* prefix_k, con
                                         int64_t prefix_stride_h, int64_t tail_stride_b, int64_t tail_stride_h, float scale,
                                         void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 int64_t aria_attention_decode_shared_prefix_workspace_bytes(int32_t G, int32_t n, int32_t H, int32_t P_max, int32_t N_max);
+/* Causal prefill of B suffixes that share one prefix (many questions about one image).  The suffixes are packed along one
+ * sequence: q, k, v [1, H, >= S_tot, 128] (head strides q_stride_h / kv_stride_h, 128-element rows), row b's suffix at packed rows
+ * [cu_seqlens[b], cu_seqlens[b+1]) (DEVICE int32 [B+1], nondecreasing from 0 to S_tot, every suffix >= 1 row).  The prefix is
+ * rows [0, P) of prefix_k / prefix_v [1, H, P_max, 128] (head stride prefix_stride_h).  The query at packed row q of suffix b
+ * sees every prefix key (no mask) and the packed keys [cu_seqlens[b], q].  out [S_tot, H*128] bf16 (the o_proj input).
+ * One CTA per (head, 128 packed queries) on aria_attention_fwd's pipeline: the prefix in 128-key tiles from key 0, then each
+ * suffix present in the query tile in 128-key tiles from its own start.  A row's arithmetic is the prefix tiles, then its own
+ * tiles, so with P % 128 == 0 row b is bit-identical to aria_attention_fwd (causal) on its own [prefix, suffix b] layout.
+ * Prefix rows at or past P and packed rows at or past S_tot are never read.  Strides are multiples of 8 elements.  No workspace. */
+int aria_attention_prefill_shared_prefix(const void* q, const void* k, const void* v, const void* prefix_k, const void* prefix_v,
+                                         const int32_t* cu_seqlens, void* out, int32_t B, int32_t H, int32_t S_tot, int32_t P,
+                                         int32_t P_max, int64_t q_stride_h, int64_t kv_stride_h, int64_t prefix_stride_h,
+                                         float scale, aria_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Generation: sampling, KV append, decode-state advance (one decode step has no host integer in it)
@@ -422,6 +435,14 @@ int aria_sample_tokens(const void* logits, int64_t logits_stride, int64_t* next_
 int aria_kv_append(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_cache, void* v_cache,
                    int64_t cache_stride_b, int64_t cache_stride_h, const int32_t* pos, int32_t B, int32_t H, int32_t T_max,
                    aria_stream_t stream);
+/* Copy the packed suffix rows k / v [1, H, >= S_tot, 128] (head stride src_stride_h) of an
+ * aria_attention_prefill_shared_prefix call into the tails tail_k / tail_v [B*n, H, N_max, 128] (strides tail_stride_b /
+ * tail_stride_h): packed row s of suffix b (cu_seqlens as there, DEVICE int32 [B+1]) goes to row s - cu_seqlens[b] of tails
+ * b*n .. b*n + n-1.  Tail rows at or past each suffix's length are not written, nor rows past N_max.  Strides are multiples of 8
+ * elements, and the tails of different rows do not overlap (tail_stride_b >= H * tail_stride_h). */
+int aria_kv_scatter_tails(const void* k, const void* v, int64_t src_stride_h, void* tail_k, void* tail_v, int64_t tail_stride_b,
+                          int64_t tail_stride_h, const int32_t* cu_seqlens, int32_t B, int32_t n, int32_t H, int32_t S_tot,
+                          int32_t N_max, aria_stream_t stream);
 /* fp8 KV cache: e4m3 codes k_cache / v_cache [B, H, T_max, 128] (element = byte strides cache_stride_b / cache_stride_h, multiples
  * of 16) and fp32 scales k_scale / v_scale [B, H, T_max] (strides scale_stride_b / scale_stride_h), one per (row, head, token):
  *   scale = max |x| / 448 (IEEE division; an all-zero row gets 1), code = e4m3(x / scale) (round to nearest even, saturating),
