@@ -21,6 +21,8 @@
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
 // aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
 // aria_attention_decode_shared_prefix: n rows per prompt decode against one shared prompt cache plus their own tail caches.
+// aria_attention_decode_multi: Q consecutive queries per row against its cache (prompt-lookup verification), each query
+//   bit-identical to the devlen kernels.
 #include <type_traits>
 
 #include "common.cuh"
@@ -719,6 +721,82 @@ __global__ void __launch_bounds__(128) attn_decode_merge(const float* __restrict
 constexpr int SP_TEAMS = 8;                                 // 4-warp teams per prefix CTA
 constexpr int SP_SMEM = 2 * DEC_SPLIT_KEYS * AT_D * 2;      // K and V of one split: 128 KB
 
+// decode_partial<DEVLEN, bf16>'s loop and 4-warp merge for one query over keys [k_begin, k_end), run by one 4-warp team with
+// the split's K and V staged in shared memory (rows from k_begin); the partial (acc[128], m, l) goes to o.  Named barrier
+// 1 + team holds the team's 128 threads.  This is attn_decode_prefix_partial's per-query body; that kernel keeps its own copy
+// so that its code stays as it was compiled before.
+__device__ __forceinline__ void decode_team_split(const __nv_bfloat16* __restrict__ qp, const __nv_bfloat16* sKb,
+                                                  const __nv_bfloat16* sVb, const uint8_t* __restrict__ km, int k_begin, int k_end,
+                                                  float scale_log2, int team, float (*sm_m)[4], float (*sm_l)[4],
+                                                  float (*sm_a)[4][AT_D], float* __restrict__ o) {
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const uint2 qv = *reinterpret_cast<const uint2*>(qp + lane * 4);
+  const float q0 = bf16_lo(qv.x) * scale_log2, q1 = bf16_hi(qv.x) * scale_log2, q2 = bf16_lo(qv.y) * scale_log2,
+              q3 = bf16_hi(qv.y) * scale_log2;
+  float m = -INFINITY, l = 0.f, a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
+  for (int k0 = k_begin + warp * 4; k0 < k_end; k0 += 16) {
+    float s[4];
+    uint2 vv[4];
+    bool live[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int kk = k0 + u;
+      live[u] = kk < k_end && !(km && km[kk]);
+      if (live[u]) {
+        const uint2 kv = *reinterpret_cast<const uint2*>(sKb + (kk - k_begin) * AT_D + lane * 4);
+        vv[u] = *reinterpret_cast<const uint2*>(sVb + (kk - k_begin) * AT_D + lane * 4);
+        s[u] = q0 * bf16_lo(kv.x) + q1 * bf16_hi(kv.x) + q2 * bf16_lo(kv.y) + q3 * bf16_hi(kv.y);
+      } else {
+        s[u] = 0.f;
+        vv[u] = make_uint2(0, 0);
+      }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+#pragma unroll
+      for (int u = 0; u < 4; ++u) s[u] += __shfl_xor_sync(0xffffffffu, s[u], o);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (live[u]) {
+        const float m_new = fmaxf(m, s[u]);
+        const float f = exp2f(m - m_new), pw = exp2f(s[u] - m_new);
+        l = l * f + pw;
+        a0 = a0 * f + pw * bf16_lo(vv[u].x);
+        a1 = a1 * f + pw * bf16_hi(vv[u].x);
+        a2 = a2 * f + pw * bf16_lo(vv[u].y);
+        a3 = a3 * f + pw * bf16_hi(vv[u].y);
+        m = m_new;
+      }
+    }
+  }
+  // the team's 4-warp merge, as decode_partial's
+  if (lane == 0) {
+    sm_m[team][warp] = m;
+    sm_l[team][warp] = l;
+  }
+  sm_a[team][warp][lane * 4 + 0] = a0;
+  sm_a[team][warp][lane * 4 + 1] = a1;
+  sm_a[team][warp][lane * 4 + 2] = a2;
+  sm_a[team][warp][lane * 4 + 3] = a3;
+  named_bar_sync(1 + team, 128);
+  const int d = threadIdx.x & 127;
+  float M = fmaxf(fmaxf(sm_m[team][0], sm_m[team][1]), fmaxf(sm_m[team][2], sm_m[team][3]));
+  float L = 0.f, A = 0.f;
+#pragma unroll
+  for (int w = 0; w < 4; ++w) {
+    const float f = (sm_m[team][w] == -INFINITY) ? 0.f : exp2f(sm_m[team][w] - M);
+    L += sm_l[team][w] * f;
+    A += sm_a[team][w][d] * f;
+  }
+  o[d] = A;
+  if (d == 0) {
+    o[AT_D] = M;
+    o[AT_D + 1] = L;
+  }
+  named_bar_sync(1 + team, 128);  // the team's next query overwrites sm_*
+}
+
 __global__ void __launch_bounds__(128 * SP_TEAMS, 1)
 attn_decode_prefix_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
                            const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ prefix_lens,
@@ -816,6 +894,45 @@ attn_decode_prefix_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloa
       o[AT_D + 1] = L;
     }
     named_bar_sync(1 + team, 128);  // the team's next query overwrites sm_*
+  }
+}
+
+// Multi-query decode (prompt-lookup verification): Q queries per (row, head), query i of row b at device key count
+// lens[b * Q + i] (the row's queries are consecutive tokens, so their counts are consecutive).  One CTA per (row, head, 256-key
+// split) stages the live keys of the split once for all Q queries, and min(Q, SP_TEAMS) 4-warp teams run decode_team_split per
+// query: the key assignment, per-key update and 4-warp merge of decode_partial<DEVLEN>.  attn_decode_merge<true> then merges
+// each query's live splits with lens, so query i of row b is bit-identical to aria_attention_decode_devlen at lens[b * Q + i].
+__global__ void __launch_bounds__(128 * SP_TEAMS, 1)
+attn_decode_multi_partial(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kc,
+                          const __nv_bfloat16* __restrict__ vc, const int32_t* __restrict__ lens,
+                          const uint8_t* __restrict__ key_mask, int mask_stride, float* __restrict__ ws, int Q, int H, int T_max,
+                          int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_q, int64_t kv_stride_b, int64_t kv_stride_h,
+                          float scale_log2, int splits) {
+  extern __shared__ uint4 sp_smem[];
+  uint4* sK = sp_smem;
+  uint4* sV = sp_smem + DEC_SPLIT_KEYS * (AT_D / 8);
+  __shared__ float sm_m[SP_TEAMS][4], sm_l[SP_TEAMS][4], sm_a[SP_TEAMS][4][AT_D];
+  const int bh = blockIdx.x, split = blockIdx.y;
+  const int b = bh / H, h = bh % H;
+  int len_max = 0;
+  for (int i = 0; i < Q; ++i) len_max = max(len_max, min(lens[b * Q + i], T_max));
+  const int k_begin = split * DEC_SPLIT_KEYS, k_stage = min(len_max, k_begin + DEC_SPLIT_KEYS);
+  const __nv_bfloat16* kbase = kc + b * kv_stride_b + h * kv_stride_h;
+  const __nv_bfloat16* vbase = vc + b * kv_stride_b + h * kv_stride_h;
+  const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(b) * mask_stride : nullptr;
+  for (int i = threadIdx.x; i < (k_stage - k_begin) * (AT_D / 8); i += blockDim.x) {
+    const int kk = k_begin + i / (AT_D / 8), c = i % (AT_D / 8);
+    if (km && km[kk]) continue;
+    sK[i] = __ldg(reinterpret_cast<const uint4*>(kbase + static_cast<int64_t>(kk) * AT_D) + c);
+    sV[i] = __ldg(reinterpret_cast<const uint4*>(vbase + static_cast<int64_t>(kk) * AT_D) + c);
+  }
+  __syncthreads();
+  const int team = threadIdx.x >> 7, n_teams = blockDim.x >> 7;
+  for (int i = team; i < Q; i += n_teams) {
+    const int k_end = min(min(lens[b * Q + i], T_max), k_begin + DEC_SPLIT_KEYS);
+    decode_team_split(q + b * q_stride_b + h * q_stride_h + i * q_stride_q, reinterpret_cast<const __nv_bfloat16*>(sK),
+                      reinterpret_cast<const __nv_bfloat16*>(sV), km, k_begin, k_end, scale_log2, team, sm_m, sm_l, sm_a,
+                      ws + ((static_cast<int64_t>(b * Q + i) * H + h) * splits + split) * (AT_D + 2));
   }
 }
 
@@ -1027,6 +1144,33 @@ extern "C" int aria_attention_decode_devlen(const void* q, const void* k, const 
   if (rc) return rc;
   attn_decode_merge<true><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
                                                      lens, H);
+  return check_launch("attn_decode_merge");
+}
+
+extern "C" int aria_attention_decode_multi(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask,
+                                           int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t Q, int32_t H,
+                                           int32_t T_max, int64_t q_stride_b, int64_t q_stride_h, int64_t q_stride_q,
+                                           int64_t kv_stride_b, int64_t kv_stride_h, float scale, void* workspace,
+                                           int64_t workspace_bytes, aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && k && v && out && lens && workspace);
+  ARIA_CHECK_ARG(B > 0 && Q > 0 && Q <= 16 && H > 0 && T_max > 0 && static_cast<int64_t>(B) * Q * H < (1ll << 31));
+  ARIA_CHECK_ARG(T_max <= 65535 * DEC_SPLIT_KEYS);  // splits are grid.y
+  ARIA_CHECK_ARG(q_stride_b % 4 == 0 && q_stride_h % 4 == 0 && q_stride_q % 4 == 0);
+  ARIA_CHECK_ARG(kv_stride_b % 8 == 0 && kv_stride_h % 8 == 0);  // the CTAs stage 16-byte vectors of each key and value row
+  ARIA_CHECK_ARG(!key_mask || (key_mask_stride >= T_max && key_mask_stride < (1ll << 31)));
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(B * Q, H, T_max));
+  const int splits = (T_max + DEC_SPLIT_KEYS - 1) / DEC_SPLIT_KEYS;
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, attn_decode_multi_partial, SP_SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_decode_multi_partial<<<dim3(B * H, splits), 128 * min(Q, SP_TEAMS), SP_SMEM, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), lens,
+      key_mask, static_cast<int>(key_mask_stride), static_cast<float*>(workspace), Q, H, T_max, q_stride_b, q_stride_h, q_stride_q,
+      kv_stride_b, kv_stride_h, scale * 1.4426950408889634f, splits);
+  int rc = check_launch("attn_decode_multi_partial");
+  if (rc) return rc;
+  attn_decode_merge<true><<<B * Q * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out),
+                                                         splits, lens, H);
   return check_launch("attn_decode_merge");
 }
 

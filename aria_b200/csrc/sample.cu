@@ -15,6 +15,9 @@
 //     It is not torch's RNG stream.
 //   temperature 0 is greedy: argmax of the logits, ties to the lowest id (torch.argmax's rule).
 // Every sum is reduced in a fixed order, so a row's result depends only on its logits, the seed and the offset.
+//
+// aria_sample_tokens_rows: the same kernel with a noise row and an offset per logits row, so that logits row b * (K + 1) + i
+// of a prompt-lookup verification step draws the noise generation row b draws for its token n_out[b] + i.
 #include <float.h>
 #include <limits.h>
 
@@ -165,7 +168,11 @@ __device__ void find_bin(SampleSmem& sm, int need) {
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParams p) {
+// ROWS (aria_sample_tokens_rows): logits row `row` draws the noise of row noise_rows[row] at offset offsets[row] instead of
+// (row, *p.rng_offset).  Everything else is the same code.
+template <bool ROWS>
+__device__ __forceinline__ void sample_body(const SampleParams p, const int32_t* __restrict__ noise_rows,
+                                            const uint64_t* __restrict__ offsets) {
   __shared__ SampleSmem sm;
   const int tid = threadIdx.x, row = blockIdx.x, V = p.V;
   const uint16_t* x = p.logits + static_cast<int64_t>(row) * p.stride;
@@ -304,7 +311,8 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParam
   }
 
   // ---- Gumbel-max over the kept set; the normalised distribution to probs_out
-  const uint64_t off = p.rng_offset ? *p.rng_offset : 0ull;
+  const uint64_t off = ROWS ? offsets[row] : p.rng_offset ? *p.rng_offset : 0ull;
+  const uint32_t noise_row = ROWS ? static_cast<uint32_t>(noise_rows[row]) : static_cast<uint32_t>(row);
   const float inv_z = 1.f / z_kept;
   float bs = -INFINITY;
   int bi = INT_MAX;
@@ -319,7 +327,7 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParam
     if (keep) {
       const float s = key_to_float(key) / temp;
       pr = expf(s - m) * inv_z;
-      const float g = gumbel(philox_x0(static_cast<uint32_t>(i), static_cast<uint32_t>(row), static_cast<uint32_t>(off),
+      const float g = gumbel(philox_x0(static_cast<uint32_t>(i), noise_row, static_cast<uint32_t>(off),
                                        static_cast<uint32_t>(off >> 32), p.seed_lo, p.seed_hi));
       const float sc = s + g;
       if (arg_better(sc, i, bs, bi)) bs = sc, bi = i;
@@ -330,20 +338,28 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParam
   if (tid == 0) p.next_ids[row] = bi;
 }
 
+__global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParams p) {
+  sample_body<false>(p, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(SP_THREADS, 1) sample_rows_kernel(const SampleParams p, const int32_t* __restrict__ noise_rows,
+                                                                    const uint64_t* __restrict__ offsets) {
+  sample_body<true>(p, noise_rows, offsets);
+}
+
 }  // namespace aria
 
 using namespace aria;
 
-extern "C" int aria_sample_tokens(const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out, int32_t B,
-                                  int32_t V, float temperature, int32_t top_k, float top_p, uint64_t seed,
-                                  const uint64_t* rng_offset, aria_stream_t stream_) {
+// the checks and parameters the two entries share
+static int sample_params(SampleParams& p, const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out, int32_t B,
+                         int32_t V, float temperature, int32_t top_k, float top_p, uint64_t seed, const uint64_t* rng_offset) {
   ARIA_CHECK_ARG(logits && next_ids);
   ARIA_CHECK_ARG(B > 0 && B <= SP_MAX_ROWS && V > 0 && V <= SP_MAX_VOCAB && logits_stride >= 0);
   ARIA_CHECK_ARG(temperature >= 0.f && temperature <= FLT_MAX);  // also rejects NaN and +inf
   ARIA_CHECK_ARG(top_k >= 0 && top_k <= SP_MAX_K);
   ARIA_CHECK_ARG(top_p > 0.f && top_p <= 1.f);
   if (top_k == 0 && top_p < 1.f) return ARIA_ERR_UNSUPPORTED;  // a full-vocabulary nucleus needs a full sort
-  SampleParams p{};
   p.logits = static_cast<const uint16_t*>(logits);
   p.stride = logits_stride;
   p.next_ids = next_ids;
@@ -355,6 +371,26 @@ extern "C" int aria_sample_tokens(const void* logits, int64_t logits_stride, int
   p.seed_lo = static_cast<uint32_t>(seed);
   p.seed_hi = static_cast<uint32_t>(seed >> 32);
   p.rng_offset = rng_offset;
+  return ARIA_OK;
+}
+
+extern "C" int aria_sample_tokens(const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out, int32_t B,
+                                  int32_t V, float temperature, int32_t top_k, float top_p, uint64_t seed,
+                                  const uint64_t* rng_offset, aria_stream_t stream_) {
+  SampleParams p{};
+  const int rc = sample_params(p, logits, logits_stride, next_ids, probs_out, B, V, temperature, top_k, top_p, seed, rng_offset);
+  if (rc) return rc;
   sample_kernel<<<B, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
   return check_launch("sample_kernel");
+}
+
+extern "C" int aria_sample_tokens_rows(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V,
+                                       float temperature, int32_t top_k, float top_p, uint64_t seed, const int32_t* noise_rows,
+                                       const uint64_t* offsets, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(noise_rows && offsets);
+  SampleParams p{};
+  const int rc = sample_params(p, logits, logits_stride, next_ids, nullptr, R, V, temperature, top_k, top_p, seed, nullptr);
+  if (rc) return rc;
+  sample_rows_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p, noise_rows, offsets);
+  return check_launch("sample_rows_kernel");
 }

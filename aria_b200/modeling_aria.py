@@ -342,7 +342,8 @@ class AriaForConditionalGeneration(nn.Module):
     def generate(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, attention_mask=None, *,
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
                  pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16",
-                 num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None):
+                 num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None,
+                 prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -367,12 +368,25 @@ class AriaForConditionalGeneration(nn.Module):
         against the prefix cache, packed, and all B * n rows decode against that one prefix cache, each with its own tail.
         Positions are those GenerationMixin derives from the left-padded mask, and the result is laid out as without it.  One
         captured step serves every call whose prefix and longest question + max_new_tokens fall in the same 256-row buckets.
+        prompt_lookup_num_tokens K (1..15) / max_matching_ngram_size M (1..16, default 2): prompt-lookup decoding, Hugging Face's
+        names.  Every row drafts up to K tokens by matching its last n <= M tokens against its own prompt and output
+        (PromptLookupCandidateGenerator), and one step verifies the row's next token and its drafts (GraphedLookupDecode).  The
+        result is the one generate() gives without these arguments, bit for bit, greedy or sampled: each verified position gets
+        the logits and the sampling noise of the plain step that would emit that token.  Not combined with
+        num_return_sequences > 1, shared_prefix_len or the fp8 KV cache; B * (K + 1) <= 1024; GPU only.  The host waits for every
+        step (poll_every does not apply); the call's counters are in self.prompt_lookup_stats.
         Returns [B * n, T + generated] int64 on the model's device (prompt ids first)."""
         B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
                                                    top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype,
                                                    num_return_sequences, shared_prefix_len)
         n_seq = num_return_sequences
         dev = self.device
+        if prompt_lookup_num_tokens is not None:
+            K, M = self._check_prompt_lookup(B, prompt_lookup_num_tokens, max_matching_ngram_size, n_seq, shared_prefix_len,
+                                             kv_cache_dtype, dev)
+            sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
+            return self._generate_prompt_lookup(input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask, sampling, eos,
+                                                pad, K, M)
         if shared_prefix_len is not None:
             ids_host, lens = self._check_shared_prefix(input_ids, attention_mask, shared_prefix_len, self.config.image_token_index,
                                                        kv_cache_dtype, n_seq)
@@ -452,6 +466,33 @@ class AriaForConditionalGeneration(nn.Module):
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
         return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
 
+    def _generate_prompt_lookup(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask, sampling, eos, pad,
+                                K, M):
+        """generate(prompt_lookup_num_tokens=K) on checked arguments: the eager prefill of generate(), the first token and the first
+        drafts eagerly, then GraphedLookupDecode.run().  The cache bucket also holds the K rows a verify step writes past a row's
+        last token, so no row of a step falls past it; the decode kernels never merge a split past a row's key count, so a larger
+        bucket changes no arithmetic.  Nothing in the graph depends on T itself (the history is T_max long too), so one captured
+        pair of steps serves every prompt length of the same bucket."""
+        dev = self.device
+        B, T = input_ids.shape
+        T_max = -(-(T + max_new_tokens + K) // 256) * 256
+        key = ("lookup", B, T_max, max_new_tokens, sampling, eos, pad, dev, K, M)
+        g = getattr(self, "_decode_graph", None)
+        if g is None or g.key != key:
+            self._decode_graph = g = None
+            g = self._decode_graph = GraphedLookupDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, K, M)
+        mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
+        inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
+                                                    attention_mask=mask, num_logits_to_keep=1)
+        g.cache.seq_len = 0
+        inputs["past_key_values"] = g.cache
+        out = self.forward(**inputs)
+        g.start(input_ids.to("cpu"), mask)
+        g.first(out.logits[:, -1])
+        L = g.run()
+        self.prompt_lookup_stats = g.stats
+        return torch.cat([input_ids.to(dev), g.out_tokens[:, :L]], dim=1)
+
     def _generate_stepwise(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask):
         """Greedy decoding through the public step API, one forward(past_key_values=...) per token: what generate() does
         on a device without CUDA graphs, i.e. the torch stand-ins of `ops` that the host-logic tests swap in."""
@@ -521,6 +562,28 @@ class AriaForConditionalGeneration(nn.Module):
         if not isinstance(pad_token_id, int):
             raise ValueError(f"pad_token_id must be an int, got {pad_token_id!r}")
         return B, T, eos, pad_token_id
+
+    @staticmethod
+    def _check_prompt_lookup(B, K, M, n, shared_prefix_len, kv_cache_dtype, device):
+        """generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=M)'s checks after _check_generate_args', in this order:
+        K, M (ValueError), then num_return_sequences > 1, shared_prefix_len, the fp8 KV cache, a CPU device and B * (K + 1) > 1024
+        (NotImplementedError).  -> (K, M), M defaulting to 2 as in Hugging Face."""
+        if not isinstance(K, int) or isinstance(K, bool) or not 1 <= K <= 15:
+            raise ValueError(f"prompt_lookup_num_tokens must be an int in [1, 15], got {K!r}")
+        M = 2 if M is None else M
+        if not isinstance(M, int) or isinstance(M, bool) or not 1 <= M <= 16:
+            raise ValueError(f"max_matching_ngram_size must be an int in [1, 16], got {M!r}")
+        if n > 1:
+            raise NotImplementedError("prompt_lookup_num_tokens with num_return_sequences > 1 is not supported")
+        if shared_prefix_len is not None:
+            raise NotImplementedError("prompt_lookup_num_tokens with shared_prefix_len is not supported")
+        if kv_cache_dtype == "fp8":
+            raise NotImplementedError("prompt_lookup_num_tokens verifies against a bf16 KV cache; the fp8 KV cache is not supported")
+        if torch.device(device).type != "cuda":
+            raise NotImplementedError("aria_b200: prompt_lookup_num_tokens runs on the GPU only")
+        if B * (K + 1) > 1024:
+            raise NotImplementedError(f"generate(): at most 1024 rows per verify step, got {B} rows x {K + 1} tokens")
+        return K, M
 
     @staticmethod
     def _check_shared_prefix(input_ids, attention_mask, P, image_token_index, kv_cache_dtype, n=1):
@@ -694,6 +757,154 @@ class GraphedDecode:
         self.event.record(torch.cuda.current_stream(self.dev))
         self.event.synchronize()
         return int(self.done_host[0]) >= 0
+
+
+class GraphedLookupDecode:
+    """Prompt-lookup decoding (generate(prompt_lookup_num_tokens=K)) as two captured steps over one KV cache and one
+    LookupDecodeState, replayed until every row is done:
+
+    - the K-wide step: embedding of [B, K + 1] ids (each row's last token, then its drafts) -> every layer
+      (AriaMoELMForCausalLM.verify_step) -> norm -> lm_head -> sample_tokens_rows -> lookup_accept_advance -> ngram_draft;
+    - the 1-wide step: the same with decode_step on [B, 1], for steps where no row has a draft.
+
+    Logits row b * (K + 1) + i draws the Philox noise of generation row b at offset n_out[b] + i, the counter plain generate()
+    uses for that row's token n_out[b] + i.  lookup_accept_advance emits each row's accepted drafts plus one token, stops a row
+    after its first EOS or at max_new_tokens and moves its positions on by the count emitted; rows past their end emit nothing,
+    and out_tokens is pad-filled at start().  After each replay the host reads the pinned status (every row done; any row has a
+    draft) and replays the K-wide step only when some row has a draft: one event wait per step.  `stats`: the last call's steps
+    replayed, K-wide steps, drafted and accepted tokens and tokens emitted."""
+
+    def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad, K: int,
+                 M: int):
+        from .moe_lm import LookupDecodeState
+        dev = model.device
+        lm = model.language_model
+        c = lm.config
+        self.key = ("lookup", B, T_max, max_new_tokens, sampling, eos, pad, dev, K, M)
+        self.model, self.B, self.T_max, self.K, self.M = model, B, T_max, K, M
+        self.max_new = max_new_tokens
+        self.sampling, self.eos, self.pad = sampling, eos, pad
+        self.cache = lm.new_cache(B, T_max, dev)
+        self.state = LookupDecodeState(B, c.num_attention_heads, T_max, K, dev)
+        self.rope = lm.model.rope_tables(T_max, dev)
+        i64, i32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.int32, device=dev)
+        Q = K + 1
+        self.ids1 = torch.zeros(B, 1, **i64)
+        self.idsk = torch.zeros(B, Q, **i64)
+        self.targets1 = torch.zeros(B, **i64)
+        self.targetsk = torch.zeros(B * Q, **i64)
+        self.noise1 = torch.arange(B, **i32)
+        self.noisek = torch.arange(B, **i32).repeat_interleave(Q)
+        self.off1 = torch.zeros(B, **i64)
+        self.offk = torch.zeros(B * Q, **i64)
+        self.draft_len = torch.zeros(B, **i32)
+        self.out_tokens = torch.zeros(B, max_new_tokens, **i64)
+        # a row's history (prompt + output) fits in its cache rows: sized by the bucket, so every prompt length of it is served
+        self.hist = torch.zeros(B, T_max, **i64)
+        self.hist_len = torch.zeros(B, **i32)
+        self.n_out = torch.zeros(B, **i32)
+        self.finished = torch.zeros(B, dtype=torch.uint8, device=dev)
+        self.status = torch.zeros(2, **i32)
+        self.counters = torch.zeros(2, **i64)
+        self.status_host = torch.zeros(2, dtype=torch.int32).pin_memory()
+        self.event = torch.cuda.Event()
+        self.dev = dev
+        self.stats = None
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):               # warm-up (start() resets the cache rows and state it touched)
+            self._step_k()
+            self._step_1()
+        cur.wait_stream(side)
+        self.graph_k = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph_k):
+            self._step_k()
+        self.graph_1 = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph_1):
+            self._step_1()
+
+    def _sample(self, logits, noise, offsets, out):
+        t, k, p, seed = self.sampling
+        ops.sample_tokens_rows(logits, t, k, p, seed, noise, offsets, out=out)
+
+    def _step_k(self):
+        lm = self.model.language_model
+        emb = ops.embedding(self.idsk, lm.get_input_embeddings().weight)
+        logits = lm.verify_step(emb, self.cache, self.state, self.rope)
+        self._sample(logits.view(-1, logits.shape[-1]), self.noisek, self.offk, self.targetsk)
+        self._advance(self.targetsk, self.idsk)
+
+    def _step_1(self):
+        lm = self.model.language_model
+        emb = ops.embedding(self.ids1, lm.get_input_embeddings().weight)
+        logits = lm.decode_step(emb, self.cache, self.state, self.rope)
+        self._sample(logits[:, -1], self.noise1, self.off1, self.targets1)
+        self._advance(self.targets1, self.ids1)
+
+    def _advance(self, targets, step_ids):
+        st = self.state
+        ops.lookup_accept_advance(targets, step_ids, self.draft_len, self.ids1, self.idsk, st.pos_k, st.lens_k, self.off1,
+                                  self.offk, self.out_tokens, self.hist, self.hist_len, self.n_out, self.finished, st.rope_pos,
+                                  st.write_pos, st.kv_len, self.status, self.counters, self.eos)
+        ops.ngram_draft(self.hist, self.hist_len, self.finished, self.n_out, self.max_new, self.idsk[:, 1:], self.draft_len,
+                        self.status[1:], self.K, self.M, self.eos)
+        self.status_host.copy_(self.status, non_blocking=True)
+
+    def start(self, ids: torch.Tensor, mask: Optional[torch.Tensor]):
+        """Reset the state for host prompt ids [B, T] (mask: host [B, T] left-padding mask or None) already prefilled into
+        self.cache: positions of each row's last prompt token, the key mask, and the history = each row's real tokens."""
+        B, T = ids.shape
+        lens = torch.full((B,), T, dtype=torch.int64) if mask is None else mask.sum(-1)
+        hist = torch.zeros(B, self.hist.shape[1], dtype=torch.int64)
+        for b in range(B):
+            n = int(lens[b])
+            hist[b, :n] = ids[b, T - n:]
+        km = torch.zeros(B, self.T_max, dtype=torch.uint8)
+        if mask is not None:
+            km[:, :T] = (mask == 0).to(torch.uint8)
+        st = self.state
+        st.rope_pos.copy_((lens - 1).to(torch.int32))
+        st.write_pos.fill_(T - 1)
+        st.kv_len.fill_(T)
+        st.key_mask.copy_(km)
+        self.hist.copy_(hist)
+        self.hist_len.copy_(lens.to(torch.int32))
+        self.n_out.zero_()
+        self.finished.zero_()
+        self.off1.zero_()
+        self.draft_len.zero_()
+        self.out_tokens.fill_(self.pad)
+        self.status.zero_()
+        self.counters.zero_()
+
+    def first(self, logits: torch.Tensor):
+        """The first token from the prefill's last-position logits [B, V], and the first drafts (eager)."""
+        self._sample(logits, self.noise1, self.off1, self.targets1)
+        self._advance(self.targets1, self.ids1)
+
+    def run(self) -> int:
+        """Replay until every row is finished or has max_new_tokens tokens -> the number of tokens to keep per row: the longest
+        row when every row ended with EOS (GenerationMixin stops after that step), else max_new_tokens."""
+        steps = k_steps = 0
+        while True:
+            self.event.record(torch.cuda.current_stream(self.dev))
+            self.event.synchronize()
+            done, drafted = int(self.status_host[0]), int(self.status_host[1])
+            if done:
+                break
+            if drafted:
+                self.graph_k.replay()
+                k_steps += 1
+            else:
+                self.graph_1.replay()
+            steps += 1
+        n_out = self.n_out.cpu()
+        counters = self.counters.cpu()
+        L = int(n_out.max()) if self.eos and bool(self.finished.cpu().all()) else self.max_new
+        self.stats = {"steps": steps, "k_steps": k_steps, "drafted": int(counters[0]), "accepted": int(counters[1]),
+                      "tokens": int(n_out.sum())}
+        return L
 
 
 class GraphedPrefill:

@@ -525,6 +525,20 @@ class SharedDecodeState(DecodeState):
         self.prefix_mask = torch.zeros(G, T_max, dtype=torch.uint8, device=device)
 
 
+class LookupDecodeState(DecodeState):
+    """DecodeState of prompt-lookup decoding (generate(prompt_lookup_num_tokens=K)): the 1-wide step reads the DecodeState fields
+    as decode_step does; a K-wide verify step runs Q = K + 1 tokens per row, query i of row b at RoPE position pos_k[b*Q + i],
+    cache row write_pos[b] + i and key count lens_k[b*Q + i] (aria_lookup_accept_advance writes both).  qkv_k: the staging rows
+    of the verify step's q, k, v [3, B, H, Q, 128]."""
+
+    def __init__(self, B, H, T_max, K, device):
+        super().__init__(B, H, T_max, device)
+        i32 = dict(dtype=torch.int32, device=device)
+        self.pos_k = torch.zeros(B * (K + 1), **i32)
+        self.lens_k = torch.ones(B * (K + 1), **i32)
+        self.qkv_k = torch.empty(3, B, H, K + 1, 128, dtype=bf16, device=device)
+
+
 class AriaAttention(nn.Module):
     """What `LLAMA_ATTENTION_CLASSES[config._attn_implementation]` provides at moe_lm.py:594: MHA, no bias,
     rotate-half RoPE, causal, KV cache.  q/k/v projections + RoPE + cache write are ONE GEMM launch."""
@@ -630,6 +644,18 @@ class AriaAttention(nn.Module):
         o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
         return self._o_proj(o, residual)
 
+    def verify_step(self, hidden_states, cache: KVCache, rope, state: LookupDecodeState, residual=None, hq=None):
+        """decode_step for Q tokens per row (a prompt-lookup verify step): hidden_states [B, Q, d]; the fused projection writes
+        q, k, v to state.qkv_k (RoPE at state.pos_k), kv_append_rows moves k, v to cache rows write_pos[b] + i, and query i
+        attends to state.lens_k[b*Q + i] keys.  Each query gets the arithmetic decode_step gives that token.  bf16 cache."""
+        B, Q, d = hidden_states.shape
+        kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
+        q, k, v = state.qkv_k[0], state.qkv_k[1], state.qkv_k[2]
+        self._qkv(hidden_states, hq, [q, k, v], Q, 0, rope, state.pos_k)
+        ops.kv_append_rows(k, v, kc, vc, state.write_pos)
+        o = ops.attention_decode_multi(q, kc, vc, state.lens_k, self.head_dim ** -0.5, key_mask=state.key_mask)
+        return self._o_proj(o, residual)
+
     def prefill_suffixes(self, hidden_states, cache: SharedPrefixCache, rope, cu_seqlens, position_ids, residual=None, hq=None):
         """Suffixes packed as one [1, S_tot] sequence (AriaMoELMModel.prefill_suffixes) against the prefix held in the cache's
         rows [0, cache.seq_len): the fused projection writes q, k, v to a staging buffer (RoPE at position_ids), the suffixes
@@ -689,6 +715,13 @@ class MoEDecoderLayer(nn.Module):
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
+    def verify_step(self, x, pending, cache, rope, state: LookupDecodeState):
+        """decode_step for Q tokens per row (AriaAttention.verify_step)."""
+        h, hq, x = self._attn_input(x, pending)
+        x = self.self_attn.verify_step(h, cache, rope, state, residual=x, hq=hq)
+        h = self.post_attention_layernorm(x)
+        return x, self.mlp(h)
+
     def prefill_suffixes(self, x, pending, cache, rope, cu_seqlens, position_ids):
         """forward() for packed suffixes over a shared prefix (AriaAttention.prefill_suffixes)."""
         h, hq, x = self._attn_input(x, pending)
@@ -734,6 +767,13 @@ class AriaMoELMModel(nn.Module):
         x, pending = inputs_embeds, None
         for layer in self.layers:
             x, pending = layer.decode_step(x, pending, cache, rope, state)
+        return x, pending
+
+    def verify_step(self, inputs_embeds, cache: KVCache, state: LookupDecodeState, rope):
+        """decode_step for Q tokens per row, inputs_embeds [B, Q, d], positions from `state` (MoEDecoderLayer.verify_step)."""
+        x, pending = inputs_embeds, None
+        for layer in self.layers:
+            x, pending = layer.verify_step(x, pending, cache, rope, state)
         return x, pending
 
     def prefill_suffixes(self, inputs_embeds, cache: SharedPrefixCache, cu_seqlens, position_ids):
@@ -811,5 +851,12 @@ class AriaMoELMForCausalLM(nn.Module):
     def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
         """inputs_embeds [B, 1, d] -> logits [B, 1, V] for one decode step driven by device positions (graph-replayable)."""
         x, pending = self.model.decode_step(inputs_embeds, cache, state, rope)
+        h, _ = self.model.norm(x, residual=pending)
+        return self.lm_head(h)
+
+    def verify_step(self, inputs_embeds, cache: KVCache, state: LookupDecodeState, rope):
+        """inputs_embeds [B, Q, d] -> logits [B, Q, V]: decode_step for the Q tokens of a prompt-lookup verify step, each row's
+        query i with the logits decode_step gives its token (graph-replayable)."""
+        x, pending = self.model.verify_step(inputs_embeds, cache, state, rope)
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h)

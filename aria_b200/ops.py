@@ -969,6 +969,38 @@ def attention_decode_shared_prefix(q: torch.Tensor, prefix_k: torch.Tensor, pref
     return out
 
 
+def attention_decode_multi(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, lens: torch.Tensor, scale: float,
+                           key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Q consecutive queries per row (prompt-lookup verification): q [B,H,Q,128] (contiguous last dim, any strides), bf16 cache
+    k/v [B,H,T_max,128]; query i of row b sees cache rows [0, lens[b*Q + i]) (lens CUDA int32 [B*Q]) minus key_mask [B, >= T_max]
+    uint8 (1 = masked out, any row stride) -> out [B, Q, H*128].  Query i of row b is bit-identical to
+    attention_decode_devlen(..., lens=lens[b*Q + i]); each key and value is read once per (row, head) for all Q queries."""
+    _chk(k), _chk(v)
+    _chk(lens, torch.int32, align=4)
+    if not (q.is_cuda and q.dtype == bf16 and q.dim() == 4 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
+        raise RuntimeError("attention_decode_multi: q must be a CUDA bf16 [B,H,Q,128] tensor with a contiguous last dim")
+    B, H, Q = q.shape[:3]
+    T_max = k.shape[2]
+    if (q.shape[3] != 128 or k.shape != (B, H, T_max, 128) or v.shape != k.shape or v.stride() != k.stride()
+            or lens.shape != (B * Q,)):
+        raise ValueError(f"attention_decode_multi: q {tuple(q.shape)}, cache {tuple(k.shape)}, lens {tuple(lens.shape)} do not fit")
+    mask_stride = 0
+    if key_mask is not None:
+        if not (key_mask.is_cuda and key_mask.dtype == torch.uint8 and key_mask.dim() == 2 and key_mask.stride(-1) == 1
+                and key_mask.shape[0] == B and key_mask.shape[1] >= T_max):
+            raise RuntimeError("attention_decode_multi: key_mask must be CUDA uint8 [B, >= T_max] with contiguous rows")
+        mask_stride = key_mask.stride(0)
+    lib = L.load()
+    ws_bytes = lib.aria_attention_decode_workspace_bytes(B * Q, H, T_max)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    out = torch.empty((B, Q, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_decode_multi(_p(q), _p(k), _p(v), _p(out), _p(key_mask), mask_stride, _p(lens), B, Q, H, T_max,
+                                                q.stride(0), q.stride(1), q.stride(2), k.stride(0), k.stride(1), scale, _p(ws),
+                                                ws_bytes, _stream(q)), "attention_decode_multi")
+    return out
+
+
 def _packed_check(S_tot: int, cu_seqlens: torch.Tensor, what: str) -> int:
     """Packed segments: cu_seqlens CUDA int32 [B+1] (B >= 1) and S_tot >= B rows -> B."""
     _chk(cu_seqlens, torch.int32, align=4)
@@ -1067,6 +1099,101 @@ def kv_append(k_new: torch.Tensor, v_new: torch.Tensor, k_cache: torch.Tensor, v
     with torch.cuda.device(k_cache.device):
         L.check(L.load().aria_kv_append(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_cache), _p(v_cache),
                                         k_cache.stride(0), k_cache.stride(1), _p(pos), B, H, T_max, _stream(k_cache)), "kv_append")
+
+
+def sample_tokens_rows(logits: torch.Tensor, temperature: float, top_k: int, top_p: float, seed: int, noise_rows: torch.Tensor,
+                       offsets: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample_tokens where logits row r [R, V] draws the Philox noise of row noise_rows[r] (CUDA int32 [R]) at offset
+    offsets[r] (CUDA int64 [R], read as uint64): row r equals sample_tokens on that row with rng_offset = offsets[r] as row
+    noise_rows[r].  out: int64 [R] (allocated when None).  See aria_sample_tokens_rows."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(-1) == 1):
+        raise RuntimeError("sample_tokens_rows: logits must be CUDA bf16 [R, V] with a contiguous last dim")
+    R, V = logits.shape
+    if out is None:
+        out = torch.empty((R,), dtype=torch.int64, device=logits.device)
+    _chk(out, torch.int64, align=8), _chk(noise_rows, torch.int32, align=4), _chk(offsets, torch.int64, align=8)
+    if out.shape != (R,) or noise_rows.shape != (R,) or offsets.shape != (R,):
+        raise ValueError(f"sample_tokens_rows: out / noise_rows / offsets must be [{R}]")
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_sample_tokens_rows(_p(logits), logits.stride(0), _p(out), R, V, float(temperature), int(top_k),
+                                                 float(top_p), int(seed) & (2 ** 64 - 1), _p(noise_rows), _p(offsets),
+                                                 _stream(logits)), "sample_tokens_rows")
+    return out
+
+
+def kv_append_rows(k_new: torch.Tensor, v_new: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, pos: torch.Tensor):
+    """k_cache[b, :, pos[b] + i] = k_new[b, :, i] (and v) for the Q rows of k_new / v_new [B, H, Q, 128] (128 contiguous, 16-byte
+    aligned elements per row); caches [B, H, T_max, 128], pos CUDA int32 [B].  Rows at or past T_max are dropped."""
+    _chk(k_cache), _chk(v_cache), _chk(pos, torch.int32, align=4)
+    for t in (k_new, v_new):
+        if not (t.is_cuda and t.dtype == bf16 and t.dim() == 4 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0):
+            raise RuntimeError("kv_append_rows: new rows must be CUDA bf16 [B, H, Q, 128] with a contiguous, 16-byte aligned last dim")
+    assert k_new.stride() == v_new.stride() and k_cache.stride() == v_cache.stride()
+    B, H, T_max = k_cache.shape[0], k_cache.shape[1], k_cache.shape[2]
+    Q = k_new.shape[2]
+    assert k_new.shape == (B, H, Q, 128) and v_new.shape == k_new.shape and pos.shape == (B,)
+    with torch.cuda.device(k_cache.device):
+        L.check(L.load().aria_kv_append_rows(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), k_new.stride(2), _p(k_cache),
+                                             _p(v_cache), k_cache.stride(0), k_cache.stride(1), _p(pos), B, Q, H, T_max,
+                                             _stream(k_cache)), "kv_append_rows")
+
+
+def _eos_array(eos_token_ids):
+    eos = list(eos_token_ids)
+    return (C.c_int64 * max(1, len(eos)))(*eos), len(eos)    # the caller holds the array across the call
+
+
+def ngram_draft(hist: torch.Tensor, hist_len: torch.Tensor, finished: torch.Tensor, n_out: torch.Tensor, max_new: int,
+                drafts: torch.Tensor, draft_len: torch.Tensor, any_draft: torch.Tensor, K: int, M: int,
+                eos_token_ids: Sequence[int] = ()):
+    """Prompt-lookup drafts of every row (Hugging Face's PromptLookupCandidateGenerator.get_candidates with num_output_tokens=K,
+    max_matching_ngram_size=M) from hist [B, H_max] int64, the first hist_len[b] tokens of row b; then cut to
+    max_new - 1 - n_out[b] tokens, none for a finished row.  Writes drafts [B, >= K] (int64, row stride any; entries past a draft
+    repeat the last token), draft_len int32 [B], and any_draft int32 [>= 1] <- 1 when a row has a draft.  See aria_ngram_draft."""
+    for t, dt in ((hist, torch.int64), (hist_len, torch.int32), (finished, torch.uint8), (n_out, torch.int32),
+                  (draft_len, torch.int32), (any_draft, torch.int32)):
+        _chk(t, dt, align=1)
+    if not (drafts.is_cuda and drafts.dtype == torch.int64):
+        raise RuntimeError("ngram_draft: drafts must be CUDA int64")
+    B = hist.shape[0]
+    if hist.dim() != 2 or drafts.dim() != 2 or drafts.stride(1) != 1 or drafts.shape[0] != B or drafts.shape[1] < K:
+        raise ValueError(f"ngram_draft: hist must be [B, H_max] and drafts [B, >= {K}] with contiguous rows")
+    assert hist_len.shape == (B,) and finished.shape == (B,) and n_out.shape == (B,) and draft_len.shape == (B,)
+    eos, n_eos = _eos_array(eos_token_ids)
+    with torch.cuda.device(hist.device):
+        L.check(L.load().aria_ngram_draft(_p(hist), hist.stride(0), _p(hist_len), _p(finished), _p(n_out), int(max_new), _p(drafts),
+                                          drafts.stride(0), _p(draft_len), _p(any_draft), B, int(K), int(M), C.cast(eos, C.c_void_p), n_eos,
+                                          _stream(hist)), "ngram_draft")
+
+
+def lookup_accept_advance(targets: torch.Tensor, step_ids: torch.Tensor, draft_len: torch.Tensor, ids1: torch.Tensor,
+                          idsk: torch.Tensor, pos_k: torch.Tensor, lens_k: torch.Tensor, off1: torch.Tensor, offk: torch.Tensor,
+                          out_tokens: torch.Tensor, hist: torch.Tensor, hist_len: torch.Tensor, n_out: torch.Tensor,
+                          finished: torch.Tensor, rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor,
+                          status: torch.Tensor, counters: torch.Tensor, eos_token_ids: Sequence[int] = ()):
+    """Accept / emit / advance after a prompt-lookup step of width Q = step_ids.shape[1] (1, or K + 1 = idsk.shape[1]): targets
+    [B*Q] sampled, step_ids [B, Q] the step's input (last token, then the drafts of draft_len [B]).  Emits each live row's accepted
+    drafts plus one token into out_tokens [B, max_new] and hist, applies the EOS rule, moves the positions on and writes the next
+    step's inputs (ids1 [B], idsk[:, 0], pos_k / lens_k int32 and off1 / offk int64 offsets), status int32 [2] (every row done,
+    any draft = 0) and counters int64 [2] (drafts verified, accepted).  See aria_lookup_accept_advance."""
+    i64, i32 = torch.int64, torch.int32
+    for t, dt in ((targets, i64), (step_ids, i64), (draft_len, i32), (ids1, i64), (idsk, i64), (pos_k, i32), (lens_k, i32),
+                  (off1, i64), (offk, i64), (out_tokens, i64), (hist, i64), (hist_len, i32), (n_out, i32),
+                  (finished, torch.uint8), (rope_pos, i32), (write_pos, i32), (kv_len, i32), (status, i32), (counters, i64)):
+        _chk(t, dt, align=1)
+    B, Q = step_ids.shape
+    Kp1 = idsk.shape[1]
+    if (targets.numel() != B * Q or idsk.shape != (B, Kp1) or pos_k.numel() != B * Kp1 or lens_k.numel() != B * Kp1
+            or offk.numel() != B * Kp1 or ids1.numel() != B or off1.numel() != B or out_tokens.shape[0] != B
+            or hist.shape[0] != B or hist.stride(1) != 1 or status.numel() < 2 or counters.numel() < 2):
+        raise ValueError("lookup_accept_advance: the buffers do not fit one another")
+    eos, n_eos = _eos_array(eos_token_ids)
+    with torch.cuda.device(targets.device):
+        L.check(L.load().aria_lookup_accept_advance(_p(targets), _p(step_ids), _p(draft_len), Q, _p(ids1), _p(idsk), Kp1, _p(pos_k),
+                                                    _p(lens_k), _p(off1), _p(offk), _p(out_tokens), out_tokens.shape[1], _p(hist),
+                                                    hist.stride(0), _p(hist_len), _p(n_out), _p(finished), _p(rope_pos),
+                                                    _p(write_pos), _p(kv_len), _p(status), _p(counters), C.cast(eos, C.c_void_p), n_eos, B,
+                                                    _stream(targets)), "lookup_accept_advance")
 
 
 def _bf16_rows_check(ts, what: str):

@@ -473,6 +473,56 @@ int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int64_t* out_t
                         int32_t* done_step, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t B,
                         aria_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Prompt-lookup decoding: a step verifies Q = K + 1 tokens per row (the last token, then K drafts from the row's history)
+ * ------------------------------------------------------------------------------------------------ */
+/* Decode attention of Q consecutive queries per row: q [B, H, Q, 128] (element strides q_stride_b / q_stride_h / q_stride_q,
+ * multiples of 4), cache k / v [B, H, T_max, 128] bf16 (strides kv_stride_b / kv_stride_h, multiples of 8).  Query i of row b sees
+ * cache rows [0, lens[b * Q + i]) (DEVICE int32 [B * Q]) minus key_mask (uint8 [B, >= T_max] at row stride key_mask_stride,
+ * 1 = masked out, or NULL).  out [B, Q, H*128] bf16.  One CTA per (row, head, 256-key split) stages the split's live keys and
+ * values once and serves every query with aria_attention_decode_devlen's per-query arithmetic; the devlen merge follows.  So
+ * query i of row b is bit-identical to aria_attention_decode_devlen at lens = lens[b * Q + i].  Q <= 16.
+ * workspace_bytes >= aria_attention_decode_workspace_bytes(B * Q, H, T_max). */
+int aria_attention_decode_multi(const void* q, const void* k, const void* v, void* out, const uint8_t* key_mask, int64_t key_mask_stride,
+                                const int32_t* lens, int32_t B, int32_t Q, int32_t H, int32_t T_max, int64_t q_stride_b,
+                                int64_t q_stride_h, int64_t q_stride_q, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
+                                void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* aria_kv_append for Q rows per row: k_new / v_new [B, H, Q, 128] (element strides new_stride_b / new_stride_h / new_stride_q) ->
+ * cache rows pos[b] + i (pos DEVICE int32 [B]); rows outside [0, T_max) are not written.  Strides are multiples of 8 elements. */
+int aria_kv_append_rows(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, int64_t new_stride_q,
+                        void* k_cache, void* v_cache, int64_t cache_stride_b, int64_t cache_stride_h, const int32_t* pos, int32_t B,
+                        int32_t Q, int32_t H, int32_t T_max, aria_stream_t stream);
+/* aria_sample_tokens over R logits rows, where row r draws the Philox noise of row noise_rows[r] (DEVICE int32 [R]) at offset
+ * offsets[r] (DEVICE uint64 [R]) instead of (r, *rng_offset).  Same warper chain, same kernel code; no probs output. */
+int aria_sample_tokens_rows(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V, float temperature,
+                            int32_t top_k, float top_p, uint64_t seed, const int32_t* noise_rows, const uint64_t* offsets,
+                            aria_stream_t stream);
+/* Drafts from each row's history hist [B, hist_stride] int64 (its first hist_len[b] entries: the prompt after its left padding,
+ * then the tokens emitted so far), Hugging Face's PromptLookupCandidateGenerator.get_candidates per row: for n = min(M, len - 1)
+ * down to 1, the earliest occurrence of the last n tokens that has a non-empty continuation; the continuation, at most K tokens
+ * and not past the history, cut before its first EOS (HOST array of n_eos <= 8 ids); no match: no draft.  The draft is then cut
+ * to max_new - 1 - n_out[b] tokens (what a step can still emit after the row's next token), and a finished row has none.
+ * Writes drafts [B, K] (row stride draft_stride; entries past a draft repeat the row's last token), draft_len [B], and sets
+ * *any_draft = 1 when a row has a draft (it is never cleared here).  K in [1, 15], M in [1, 16].  One CTA per row. */
+int aria_ngram_draft(const int64_t* hist, int64_t hist_stride, const int32_t* hist_len, const uint8_t* finished, const int32_t* n_out,
+                     int32_t max_new, int64_t* drafts, int64_t draft_stride, int32_t* draft_len, int32_t* any_draft, int32_t B,
+                     int32_t K, int32_t M, const int64_t* eos_ids, int32_t n_eos, aria_stream_t stream);
+/* After aria_sample_tokens_rows on a step of width Q (1, or Kp1 = K + 1 with step_ids [B, Q] = the last token, then the drafts of
+ * draft_len [B]), per row b that is neither finished nor at max_new tokens: a = the number of leading drafts equal to the target
+ * before them (targets [B * Q]); emits targets t_0 .. t_a to out_tokens[b, n_out[b] ...] ([B, max_new]) and to the history,
+ * stopping after the first EOS id (finished[b] = 1) and at max_new tokens; then n_out, hist_len, rope_pos, write_pos and kv_len
+ * move on by the count emitted.  Every row then gets the next step's inputs: ids1[b] and idsk[b * Kp1] = its last token,
+ * pos_k / lens_k [B * Kp1] = rope_pos + i / kv_len + i, off1[b] = n_out[b], offk[b * Kp1 + i] = n_out[b] + i.
+ * status[0] = every row finished or at max_new, status[1] = 0 (aria_ngram_draft sets it); counters[0] += drafts verified,
+ * counters[1] += drafts accepted.  Out tokens are not written past a row's end: the caller fills them with pad first.
+ * B <= 1024, one launch. */
+int aria_lookup_accept_advance(const int64_t* targets, const int64_t* step_ids, const int32_t* draft_len, int32_t Q, int64_t* ids1,
+                               int64_t* idsk, int32_t Kp1, int32_t* pos_k, int32_t* lens_k, uint64_t* off1, uint64_t* offk,
+                               int64_t* out_tokens, int32_t max_new, int64_t* hist, int64_t hist_stride, int32_t* hist_len,
+                               int32_t* n_out, uint8_t* finished, int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len,
+                               int32_t* status, uint64_t* counters, const int64_t* eos_ids, int32_t n_eos, int32_t B,
+                               aria_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
