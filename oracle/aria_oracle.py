@@ -116,7 +116,7 @@ def token_permutation(x: Tensor, top_idx: Tensor, k: int) -> Tuple[Tensor, Tenso
 
 def sequential_gemm(inp: Tensor, weight: Tensor, counts: Tensor) -> Tensor:
     """moe_lm.py:398-428: per-expert matmul over contiguous row groups, weight [E, in, out]."""
-    out = torch.zeros(inp.shape[0], weight.shape[-1], dtype=inp.dtype)
+    out = torch.zeros(inp.shape[0], weight.shape[-1], dtype=inp.dtype, device=inp.device)
     off = 0
     for e in range(weight.shape[0]):
         n = int(counts[e])
@@ -150,7 +150,7 @@ def grouped_mlp(permuted: Tensor, fc1: Tensor, fc2: Tensor, counts: Tensor) -> T
 
 def token_unpermutation(y: Tensor, order: Tensor, scores: Tensor, k: int) -> Tensor:
     """moe_lm.py:336-365: scatter rows back, scale by scores (bf16 multiply), sum over k."""
-    buf = torch.zeros((scores.numel(), y.shape[1]), dtype=y.dtype)
+    buf = torch.zeros((scores.numel(), y.shape[1]), dtype=y.dtype, device=y.device)
     buf.index_copy_(0, order, y)
     buf = buf.reshape(-1, k, y.shape[1])
     buf = buf * scores.unsqueeze(-1)

@@ -1,6 +1,6 @@
 """GPU: MoE block forward+backward (BASELINE cfg 5 unit) against torch autograd through the oracle restatement.
 The oracle runs in fp32 on the bf16-rounded parameters/inputs; our gradients are bf16 with fp32 accumulation, so the
-tolerance is a relative L2 error of 2e-2 per gradient tensor (router-near-tie tokens excluded from dx)."""
+tolerance is a relative L2 error of 2e-2 per gradient tensor (router-near-tie tokens get no upstream gradient)."""
 import pytest
 import torch
 
@@ -48,7 +48,9 @@ def test_grouped_gemm_nt_matches_transposed_weight():
 
 @pytest.mark.parametrize("T,E,k,d,I", [(40, 8, 2, 256, 128), (300, 64, 6, 256, 128)])
 def test_moe_layer_forward_backward_vs_oracle_autograd(T, E, k, d, I):
-    from aria_b200 import moe_lm, moe_train
+    """Near-tie tokens (top-k margin <= 2^-6 of max|logit|) get a zero upstream gradient and every other token must be
+    routed to the oracle's expert set, so all gradients are held to the 2e-2 bar with no routing slack."""
+    from aria_b200 import moe_lm, moe_train, ops
     from oracle import aria_oracle as O
     from oracle import configs as C
     tc = dict(hidden_size=d, moe_num_experts=E, moe_topk=k, moe_intermediate_size=I, moe_num_shared_experts=2)
@@ -56,12 +58,18 @@ def test_moe_layer_forward_backward_vs_oracle_autograd(T, E, k, d, I):
     sd = {n: v.bfloat16() for n, v in C.moe_layer_state(tc, gen).items()}
     x = torch.randn(1, T, d, generator=gen).bfloat16()
     gout = torch.randn(1, T, d, generator=gen).bfloat16()
+    lg = O.router_gating(x.view(T, d).float(), sd["router.weight"].float()).sort(1, descending=True).values
+    safe = ((lg[:, k - 1] - lg[:, k]) / lg.abs().amax(1) > 2 ** -6)
+    assert int(safe.sum()) >= T // 2
+    gout = gout.masked_fill(~safe.view(1, T, 1), 0)
     # oracle: fp32 autograd on the same (bf16-rounded) values
     sd32 = {n: v.float().requires_grad_(True) for n, v in sd.items()}
     x32 = x.float().requires_grad_(True)
     with torch.enable_grad():
         want, parts = O.moe_layer(x32, sd32, k, return_parts=True)
         want.backward(gout.float())
+    _, idx, _, _ = ops.router_topk(x.view(T, d).to(DEV), sd["router.weight"].to(DEV), k)
+    assert torch.equal(idx.cpu().long()[safe].sort(1).values, parts["top_idx"][safe].sort(1).values)
     # ours
     layer = moe_lm.MoELayer(moe_lm.AriaMoELMConfig(**tc), device=DEV)
     layer.load_state_dict({n: v.to(DEV) for n, v in sd.items()}, strict=True)
@@ -71,19 +79,14 @@ def test_moe_layer_forward_backward_vs_oracle_autograd(T, E, k, d, I):
     with torch.enable_grad():
         got = moe_train.moe_layer_train(layer, xg)
         got.backward(gout.to(DEV))
-    lg = parts["logits"].detach().float().sort(1, descending=True).values
-    safe = ((lg[:, k - 1] - lg[:, k]) / lg.abs().amax(1) > 2 ** -6)
-    assert int(safe.sum()) >= T // 2
     assert _rel_l2(got.detach().view(T, d)[safe], want.detach().view(T, d)[safe]) <= 1e-2
-    assert _rel_l2(xg.grad.view(T, d)[safe], x32.grad.view(T, d)[safe]) <= 2e-2
+    assert _rel_l2(xg.grad.view(T, d), x32.grad.view(T, d)) <= 2e-2
     names = {"router.weight": layer.router.weight, "experts.fc1.weight": layer.experts.fc1.weight,
              "experts.fc2.weight": layer.experts.fc2.weight, "shared_experts.gate_proj.weight": layer.shared_experts.gate_proj.weight,
              "shared_experts.up_proj.weight": layer.shared_experts.up_proj.weight,
              "shared_experts.down_proj.weight": layer.shared_experts.down_proj.weight}
-    all_safe = bool(safe.all())
     for n, p_ in names.items():
-        tol = 2e-2 if all_safe else 1.5e-1   # a flipped near-tie token moves a whole row of expert/router gradient
-        assert _rel_l2(p_.grad, sd32[n].grad) <= tol, n
+        assert _rel_l2(p_.grad, sd32[n].grad) <= 2e-2, n
 
 
 def _one_rank_ep_worker(rank, port, tc, T, result_dir):
@@ -159,10 +162,11 @@ def test_wgrad_two_cta_path_and_sources():
             assert _rel_l2(got[e], want) <= 1e-2
 
 
-@pytest.mark.parametrize("T,E,k", [(40, 8, 2), (777, 64, 6), (33, 200, 4)])
+@pytest.mark.parametrize("T,E,k", [(40, 8, 2), (777, 64, 6), (33, 200, 4), (500, 256, 8), (8192, 64, 6)])
 def test_router_aux_loss_kernels_vs_oracle(T, E, k):
     """Training-mode router losses (moe_lm.py:128-166, 203-241): loss values and the gradient they inject, against the
-    oracle's fp32 closed form (pinned to the reference's autograd in tests/test_oracle_vs_reference.py)."""
+    oracle's fp32 closed form (pinned to the reference's autograd in tests/test_oracle_vs_reference.py).  E = 256 is
+    the kernels' AUX_MAX_E; at T = 8192 the loss values sum per-block partials of many blocks."""
     from aria_b200 import ops
     from oracle import aria_oracle as O
     g = torch.Generator().manual_seed(T + E)

@@ -78,9 +78,16 @@ def test_routing_bit_exact(T, E, k):
     assert int(c.sum()) == T * k
 
 
-@pytest.mark.parametrize("T,E,k,d", [(1, 8, 2, 256), (37, 8, 2, 256), (768, 64, 6, 2560), (3001, 64, 6, 512), (5461, 64, 6, 256), (5600, 64, 6, 256)])  # last: > 32768 ids -> the multi-block sort
-def test_permutation_and_combine_bit_exact(T, E, k, d):
-    """stable argsort / index_select / index_copy_ / weighted sum (moe_lm.py:313-365)."""
+_PERM_SHAPES = [(1, 8, 2, 256), (37, 8, 2, 256), (768, 64, 6, 2560), (3001, 64, 6, 512), (5461, 64, 6, 256), (5600, 64, 6, 256)]  # last: > 32768 ids -> the multi-block sort
+
+
+@pytest.mark.parametrize("T,E,k,d,row_align",
+                         [pytest.param(*s, a, id="-".join(map(str, s)) + ("" if a == 1 else f"-align{a}"))
+                          for a in (1, 16) for s in _PERM_SHAPES])
+def test_permutation_and_combine_bit_exact(T, E, k, d, row_align):
+    """stable argsort / index_select / index_copy_ / weighted sum (moe_lm.py:313-365).  row_align=16 is the training
+    layout: expert e's block starts at the sum of the earlier counts each rounded up to 16, its rows are the oracle's
+    stable order shifted by that base, every other slot of `src` is -1 and its permuted row is exactly zero."""
     O, _ = _oracle()
     ops = _ops()
     g = torch.Generator().manual_seed(T + d)
@@ -91,20 +98,32 @@ def test_permutation_and_combine_bit_exact(T, E, k, d):
     s_ref, i_ref, c_ref = O.router_routing(logits, k)
     perm_ref, order = O.token_permutation(x, i_ref, k)
     s, i, c = ops.route_from_logits(logits.to(DEV), k)
-    off, dest, src = ops.build_permutation(i, c)
+    off, dest, src = ops.build_permutation(i, c, row_align=row_align)
     inv = torch.empty_like(order)
     inv[order] = torch.arange(order.numel())
-    assert torch.equal(dest.cpu().long(), inv)
-    assert torch.equal(src.cpu().long(), order // k)
-    assert torch.equal(off.cpu().long(), torch.cat([torch.zeros(1, dtype=torch.long), c_ref.cumsum(0)]))
+    # expert e's rows: dense base (sum of earlier counts) -> aligned base (sum of earlier counts rounded up to row_align)
+    dense0 = torch.cat([torch.zeros(1, dtype=torch.long), c_ref.cumsum(0)])
+    al0 = torch.cat([torch.zeros(1, dtype=torch.long), ((c_ref + row_align - 1) // row_align * row_align).cumsum(0)])
+    eid_flat = i_ref.reshape(-1)
+    dest_ref = inv - dense0[eid_flat] + al0[eid_flat]
+    assert torch.equal(off.cpu().long(), al0)
+    assert torch.equal(dest.cpu().long(), dest_ref)
+    rows = src.numel()
+    assert rows == T * k + E * (row_align - 1)
+    src_ref = torch.full((rows,), -1, dtype=torch.long)
+    src_ref[dest_ref] = torch.arange(T * k) // k
+    assert torch.equal(src.cpu().long(), src_ref)
     p = ops.permute_rows(x.to(DEV), src)
-    assert torch.equal(p.cpu(), perm_ref)
+    p_ref = torch.zeros(rows, d, dtype=torch.bfloat16)
+    p_ref[dest_ref[order]] = perm_ref
+    assert torch.equal(p.cpu(), p_ref)
     # sortedness property: expert id of each permuted row is non-decreasing
     eid = i.reshape(-1)[torch.argsort(dest)].cpu()
     assert bool((eid[1:] >= eid[:-1]).all())
-    y = torch.randn(T * k, d, generator=g).bfloat16()
+    y = torch.randn(rows, d, generator=g).bfloat16()
+    y[src_ref < 0] = float("nan")  # pad rows are never read
     shared = torch.randn(T, d, generator=g).bfloat16()
-    want = O.token_unpermutation(y, order, s_ref, k) + shared
+    want = O.token_unpermutation(y[dest_ref[order]], order, s_ref, k) + shared
     got = ops.unpermute_combine(y.to(DEV), dest, s, shared.to(DEV))
     assert (got.cpu().float() - want.float()).abs().max() <= 2 ** -7 * want.float().abs().max()
     assert float((got.cpu() == want).float().mean()) > 0.999
