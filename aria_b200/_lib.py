@@ -59,6 +59,8 @@ SIGNATURES = {
     "aria_grouped_gemm_w8a8": (i32, [vp, vp, vp, vp, vp, vp, i64, i64, i64, i32, i32, vp]),
     "aria_gemm_w8a8": (i32, [C.POINTER(GemmDesc), vp, vp, vp]),
     "aria_grouped_wgrad": (i32, [vp, i64, vp, i64, vp, vp, i64, i64, i64, i32, i32, vp]),
+    "aria_wgrad_accumulate_f32": (i32, [vp, i64, vp, i64, vp, i64, i64, i64, vp]),
+    "aria_cross_entropy_rows": (i32, [vp, i64, vp, vp, vp, i64, i32, vp]),
     "aria_moe_block_fwd_workspace_bytes": (i64, [i64, i32, i32, i32, i32, i32]),
     "aria_moe_block_fwd": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),
     "aria_moe_block_fwd_fp8": (i32, [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i64, vp, vp]),

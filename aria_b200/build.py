@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libaria_b200.so")
 SOURCES = ["gemm.cu", "gemm_wgrad.cu", "moe_route.cu", "moe_block.cu", "moe_bwd.cu", "ep.cu", "elementwise.cu", "attention.cu",
-           "attention_bwd.cu", "sample.cu", "decode.cu", "quant.cu", "kv_fp8.cu"]
+           "attention_bwd.cu", "sample.cu", "decode.cu", "quant.cu", "kv_fp8.cu", "loss.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

@@ -22,12 +22,17 @@ struct WgradParams {
   int n_src;            // row groups are (source, g) pairs, source-major: offs has n_src*G+1 entries and out[g] sums over sources
   const int32_t* offs;  // [n_src*G+1], non-decreasing
   __nv_bfloat16* out;   // [G, Md, Nd]
+  int rows;             // ACC_F32: one group over rows [0, rows)
+  float* out_f32;       // ACC_F32: [Md, Nd], accumulated into
 };
 
 constexpr int WG_BN = 128;
 constexpr int WG_STAGES = 6;
 constexpr int WG_STAGE_BYTES = 64 * BM * 2 + 64 * WG_BN * 2;  // A slab [64 rows][128 m] + B slab [64 rows][128 n]
 
+// ACC_F32: one group, no offsets array; the epilogue adds the fp32 accumulators into out_f32 instead of storing bf16.  A
+// tile belongs to one CTA, so the read-modify-write needs no atomics.
+template <bool ACC_F32>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const WgradParams p) {
   uint8_t* smem = smem_1024();
@@ -54,8 +59,13 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
   };
   // rows of (source s, group g): start row and row count
   auto span = [&](int s, int g, int& r0, int& n) {
-    r0 = p.offs[s * p.G + g];
-    n = p.offs[s * p.G + g + 1] - r0;
+    if constexpr (ACC_F32) {
+      r0 = 0;
+      n = p.rows;
+    } else {
+      r0 = p.offs[s * p.G + g];
+      n = p.offs[s * p.G + g + 1] - r0;
+    }
   };
 
   if (wg == 0) {
@@ -135,6 +145,20 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CU
       for (int h = 0; h < 2; ++h) {
         const int m = mi * BM + ct.frag_row + 8 * h;
         if (m >= p.Md) continue;
+        if constexpr (ACC_F32) {
+          float* orow = p.out_f32 + static_cast<int64_t>(m) * p.Nd + ni * WG_BN;
+#pragma unroll
+          for (int j = 0; j < WG_BN / 8; ++j) {
+            if (ni * WG_BN + 8 * j + 8 <= p.Nd) {
+              float2* o = reinterpret_cast<float2*>(orow + 8 * j + ct.frag_col);
+              float2 c = *o;
+              c.x += acc[4 * j + 2 * h];
+              c.y += acc[4 * j + 2 * h + 1];
+              *o = c;
+            }
+          }
+          continue;
+        }
         __nv_bfloat16* orow = p.out + (static_cast<int64_t>(g) * p.Md + m) * p.Nd + ni * WG_BN;
 #pragma unroll
         for (int j = 0; j < WG_BN / 8; ++j) {
@@ -171,5 +195,29 @@ extern "C" int aria_grouped_wgrad(const void* a, int64_t lda, const void* b, int
   p.out = static_cast<__nv_bfloat16*>(out);
   constexpr int SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
   const int64_t tiles = static_cast<int64_t>(num_groups) * ((md + BM - 1) / BM) * ((nd + WG_BN - 1) / WG_BN);
-  return launch_persistent<wgrad_kernel>("wgrad_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB, p);
+  return launch_persistent<wgrad_kernel<false>>("wgrad_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB, p);
+}
+
+extern "C" int aria_wgrad_accumulate_f32(const void* a, int64_t lda, const void* b, int64_t ldb, float* out, int64_t rows,
+                                         int64_t md, int64_t nd, aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(a && b && out && rows >= 0 && rows <= INT32_MAX && md > 0 && nd > 0 && md <= INT32_MAX && nd <= INT32_MAX);
+  ARIA_CHECK_ARG(md % 8 == 0 && nd % 8 == 0 && lda % 8 == 0 && ldb % 8 == 0 && lda >= md && ldb >= nd);
+  ARIA_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 7) == 0);
+  if (rows == 0) return ARIA_OK;
+  CUtensorMap tmA, tmB;
+  int rc = make_tmap_2d(&tmA, a, md, rows, lda * 2, 64, 64);
+  if (rc) return rc;
+  rc = make_tmap_2d(&tmB, b, nd, rows, ldb * 2, 64, 64);
+  if (rc) return rc;
+  WgradParams p{};
+  p.Md = static_cast<int>(md);
+  p.Nd = static_cast<int>(nd);
+  p.G = 1;
+  p.n_src = 1;
+  p.rows = static_cast<int>(rows);
+  p.out_f32 = out;
+  constexpr int SMEM = WG_STAGES * WG_STAGE_BYTES + 1024 + 256;
+  const int64_t tiles = ((md + BM - 1) / BM) * ((nd + WG_BN - 1) / WG_BN);
+  return launch_persistent<wgrad_kernel<true>>("wgrad_accumulate_f32_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB, p);
 }

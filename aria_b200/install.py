@@ -7,10 +7,13 @@ Seams (SURVEY.md §8b):
   2. `MoELayer.forward` (moe_lm.py:548-577)                 -> fused router / dispatch / grouped GEMM / combine path
   3. decoder-layer attention (moe_lm.py:594)                -> `AriaAttention`-style forward on the module's own q/k/v/o_proj
   4. `Idefics2EncoderLayer.forward` (vision_encoder.py:120) -> fused ViT layer
+  5. `AriaForConditionalGeneration.forward` (modeling_aria.py:287-323, the loss head) -> `loss.linear_cross_entropy` on the
+     final-norm hidden states: logits only for labelled rows, in chunks, never the [B, T, V] tensor
 
 (1) and (2) are wired by `install()` — inference-only by default, differentiable with `install(..., trainable=True)`; (3) is `aria_b200.hf_attention.register()` (an implementation key for transformers'
 attention interface — the module keeps its projections, RoPE and HF Cache); (4) is `install_vit()` (per-layer forward on the
-HF module's own parameters; the embeddings / mask creation around it stay HF's).
+HF module's own parameters; the embeddings / mask creation around it stay HF's); (5) is `install_loss()` (training forward
+with labels only; every other call runs the original forward).
 There is no CPU fallback: the patched modules require CUDA bf16 tensors.
 """
 from __future__ import annotations
@@ -21,6 +24,7 @@ import types
 import torch
 from torch import nn
 
+from . import loss as _loss
 from . import lora as _lora
 from . import moe_lm as _m
 from . import moe_train as _t
@@ -251,4 +255,82 @@ def install(model, reference_moe_lm_module=None, trainable: bool = False) -> int
     if reference_moe_lm_module is not None:
         # seam 1: GroupedGEMM.forward calls the module global
         reference_moe_lm_module.experts_gemm = _t.experts_gemm_train if trainable else _m.experts_gemm
+    return n
+
+
+# ------------------------------------------------------------------------------------------------ seam 5: the loss head
+def _loss_forward(self, input_ids=None, pixel_values=None, pixel_mask=None, attention_mask=None, position_ids=None,
+                  past_key_values=None, inputs_embeds=None, labels=None, use_cache=None, output_attentions=None,
+                  output_hidden_states=None, return_dict=None, cache_position=None, num_logits_to_keep=0):
+    """Replacement for the reference `AriaForConditionalGeneration.forward` (modeling_aria.py:194-331) bound by
+    `install_loss()`.  A training call (labels given, a gradient needed, every logit requested, a dict output, a plain bias-free
+    nn.Linear lm_head) runs the reference's steps on the model's own submodules up to the language model's final norm, then
+    `loss.linear_cross_entropy` over the reference's rows: position t < T-1 of every sequence predicts labels[:, t+1], kept
+    where attention_mask[:, -(T-1):] != 0 (all positions without a mask), labels == -100 ignored.  It returns the reference's
+    output class with that fp32 loss and `logits=None`.  Every other call runs the original forward unchanged."""
+    kw = dict(input_ids=input_ids, pixel_values=pixel_values, pixel_mask=pixel_mask, attention_mask=attention_mask,
+              position_ids=position_ids, past_key_values=past_key_values, inputs_embeds=inputs_embeds, labels=labels,
+              use_cache=use_cache, output_attentions=output_attentions, output_hidden_states=output_hidden_states,
+              return_dict=return_dict, cache_position=cache_position, num_logits_to_keep=num_logits_to_keep)
+    original = type(self).forward
+    output_attentions = output_attentions if output_attentions is not None else self.config.output_attentions
+    output_hidden_states = output_hidden_states if output_hidden_states is not None else self.config.output_hidden_states
+    return_dict = return_dict if return_dict is not None else self.config.use_return_dict
+    head = self.language_model.lm_head
+    needs_grad = torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters())
+                                              or (inputs_embeds is not None and inputs_embeds.requires_grad))
+    if labels is None or not needs_grad or num_logits_to_keep != 0 or not return_dict or _plain_weight(head) is None:
+        return original(self, **kw)
+    if head.weight.numel() == 0:
+        raise RuntimeError("aria_b200.install_loss: lm_head.weight is empty (a ZeRO-3 partition?); the fused loss reads the "
+                           "whole weight, so gather it first (or train without install_loss)")
+
+    # the reference's steps before the language model (modeling_aria.py:248-283)
+    if inputs_embeds is None:
+        inputs_embeds = self.get_input_embeddings()(input_ids)
+    if pixel_values is not None:
+        image_outputs, image_attn_mask = self.vision_tower(pixel_values, pixel_mask=pixel_mask)
+        image_features = self.multi_modal_projector(image_outputs.last_hidden_state, attn_mask=image_attn_mask)
+        n_image_tokens = (input_ids == self.config.image_token_index).sum().item()
+        n_image_features = image_features.shape[0] * image_features.shape[1]
+        if n_image_tokens != n_image_features:
+            raise ValueError(
+                f"Image features and image tokens do not match: tokens: {n_image_tokens}, features {n_image_features}")
+        special_image_mask = (input_ids == self.config.image_token_index).unsqueeze(-1).expand_as(inputs_embeds)
+        special_image_mask = special_image_mask.to(inputs_embeds.device)
+        image_features = image_features.to(inputs_embeds.device, inputs_embeds.dtype)
+        inputs_embeds = inputs_embeds.masked_scatter(special_image_mask, image_features)
+
+    outputs = self.language_model.model(attention_mask=attention_mask, position_ids=position_ids,
+                                        past_key_values=past_key_values, inputs_embeds=inputs_embeds, use_cache=use_cache,
+                                        output_attentions=output_attentions, output_hidden_states=output_hidden_states,
+                                        return_dict=True, cache_position=cache_position)
+    hidden = outputs[0]
+    B, T, d = hidden.shape
+    # rows of the reference's shift (modeling_aria.py:302-318) as labels: the last position of each sequence and the
+    # positions the attention mask drops are ignored, so the hidden states go in as one [B*T, d] view without a copy
+    shifted = torch.full((B, T), -100, dtype=torch.long, device=hidden.device)
+    shifted[:, :-1] = labels[:, 1:].to(hidden.device)
+    if attention_mask is not None:
+        keep = attention_mask[:, -(T - 1):].to(hidden.device) != 0
+        shifted[:, :-1].masked_fill_(~keep, -100)
+    loss = _loss.linear_cross_entropy(hidden.reshape(B * T, d), head.weight, shifted.view(-1))
+    out_cls = getattr(sys.modules[type(self).__module__], "AriaCausalLMOutputWithPast")
+    return out_cls(loss=loss, logits=None, past_key_values=outputs.past_key_values, hidden_states=outputs.hidden_states,
+                   attentions=outputs.attentions)
+
+
+def install_loss(model) -> int:
+    """Seam 5: patch `forward` of every reference `AriaForConditionalGeneration` inside `model` (what aria/train.py trains) with
+    `_loss_forward`: the training loss from `loss.linear_cross_entropy` instead of full logits and nn.CrossEntropyLoss.
+    transformers' own `models.aria` class and this package's inference mirror are left alone.  Returns the number of models
+    patched.  Idempotent."""
+    n = 0
+    for mod in model.modules():
+        cls = type(mod)
+        if cls.__name__ == "AriaForConditionalGeneration" and not cls.__module__.startswith(("transformers.", "aria_b200.")) \
+                and hasattr(sys.modules.get(cls.__module__), "AriaCausalLMOutputWithPast") \
+                and hasattr(mod, "language_model") and hasattr(mod.language_model, "lm_head"):
+            mod.forward = types.MethodType(_loss_forward, mod)
+            n += 1
     return n

@@ -408,6 +408,43 @@ def grouped_wgrad(a: torch.Tensor, b: torch.Tensor, offsets: torch.Tensor, num_s
     return out
 
 
+def wgrad_accumulate_f32(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out += a.T @ b in fp32, in place; a [rows, Md], b [rows, Nd] bf16 (row strides allowed), out [Md, Nd] fp32 contiguous.
+    The weight gradient of nn.Linear built up over chunks of rows without a bf16 rounding per chunk."""
+    for t in (a, b):
+        if not (t.is_cuda and t.dtype == bf16 and t.stride(1) == 1 and t.data_ptr() % 16 == 0):
+            raise RuntimeError("wgrad_accumulate_f32: operands must be CUDA bf16 with contiguous rows")
+    _chk(out, torch.float32, align=8)
+    rows, Md = a.shape
+    Nd = b.shape[1]
+    assert b.shape[0] == rows and out.shape == (Md, Nd)
+    with torch.cuda.device(a.device):
+        L.check(L.load().aria_wgrad_accumulate_f32(_p(a), a.stride(0), _p(b), b.stride(0), _p(out), rows, Md, Nd, _stream(a)),
+                "wgrad_accumulate_f32")
+    return out
+
+
+def cross_entropy_rows(logits: torch.Tensor, labels: torch.Tensor, grad_scale: torch.Tensor,
+                       loss: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Per-row cross-entropy of bf16 logits [rows, V] (V % 8 == 0, contiguous last dim, row stride a multiple of 8) against
+    int64 labels [rows] in [0, V): returns loss [rows] fp32 (logsumexp - logit[label], softmax in fp32) and overwrites each
+    logits row IN PLACE with (softmax - onehot(label)) * grad_scale in bf16.  grad_scale: device fp32 [1] (no host sync)."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(1) == 1
+            and logits.data_ptr() % 16 == 0):
+        raise RuntimeError("cross_entropy_rows: logits must be CUDA bf16 [rows, V] with contiguous, 16-byte aligned rows")
+    rows, V = logits.shape
+    _chk(labels, torch.int64, align=8), _chk(grad_scale, torch.float32, align=4)
+    assert labels.shape == (rows,) and grad_scale.numel() == 1
+    if loss is None:
+        loss = torch.empty((rows,), dtype=torch.float32, device=logits.device)
+    _chk(loss, torch.float32, align=4)
+    assert loss.shape == (rows,)
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_cross_entropy_rows(_p(logits), logits.stride(0), _p(labels), _p(grad_scale), _p(loss), rows, V,
+                                                 _stream(logits)), "cross_entropy_rows")
+    return loss
+
+
 def swiglu_fwd(h1: torch.Tensor) -> torch.Tensor:
     _chk(h1)
     rows, I2 = h1.shape

@@ -156,6 +156,21 @@ int aria_gemm_w8a8(const aria_gemm_desc_t* desc, const float* a_scale, const flo
  * source-major, offsets[S*G+1], and out[g] sums the S partial products — no separate reduction pass. */
 int aria_grouped_wgrad(const void* a, int64_t lda, const void* b, int64_t ldb, void* out, const int32_t* group_offsets,
                        int64_t rows, int64_t md, int64_t nd, int32_t num_groups, int32_t num_sources, aria_stream_t stream);
+/* One-group weight gradient accumulated in fp32: out[m, n] += sum_{r < rows} a[r, m] * b[r, n]; out [md, nd] fp32, 8-byte
+ * aligned.  The same kernel as aria_grouped_wgrad with an epilogue that adds its fp32 accumulators to out, so a weight gradient
+ * can be built up over chunks of rows without a bf16 rounding per chunk.  Each output tile has one owner: no atomics, and
+ * the result does not depend on the launch.  rows = 0 launches nothing. */
+int aria_wgrad_accumulate_f32(const void* a, int64_t lda, const void* b, int64_t ldb, float* out, int64_t rows, int64_t md,
+                              int64_t nd, aria_stream_t stream);
+
+/* Cross-entropy rows for the fused lm_head loss: for each of `rows` rows of bf16 logits (row stride ld, vocab % 8 == 0,
+ * ld % 8 == 0, logits 16-byte aligned) and its int64 label in [0, vocab):
+ *   loss[r] = logsumexp(logits[r, :]) - logits[r, label[r]]                 (fp32, softmax in fp32)
+ *   logits[r, :] <- (softmax(logits[r, :]) - onehot(label[r])) * (*grad_scale)  (bf16, in place)
+ * grad_scale: DEVICE fp32 scalar (1 / n for a mean, 1 for a sum).  A label outside [0, vocab) gives loss NaN and no one-hot
+ * term (callers check labels first).  One CTA per row; two runs give identical bits. */
+int aria_cross_entropy_rows(void* logits, int64_t ld, const int64_t* labels, const float* grad_scale, float* loss, int64_t rows,
+                            int32_t vocab, aria_stream_t stream);
 
 /* int64 counts (tokens_per_expert as the reference passes it, moe_lm.py:264-269) -> int32 offsets[G+1]. */
 int aria_offsets_from_counts(const int64_t* counts, int32_t* offsets, int32_t num_groups, aria_stream_t stream);
