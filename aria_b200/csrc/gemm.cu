@@ -63,8 +63,9 @@ ARIA_DEVICE void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) 
 //     still write its shared memory or arrive on its barriers).
 template <int BN, bool B_MN, int EPI, bool B_FP8 = false, bool PAIR = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
-            const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA_min,
+            const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
+            const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
   constexpr int B_STAGE_BYTES = BN * BK * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
   constexpr int STAGES = GEMM_STAGES;
@@ -89,6 +90,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
+    if (p.group_offsets) prefetch_tmap(&tmA_min);
     prefetch_tmap(&tmB0);
     if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(&tmB1);
     if (p.n_seg > 2) prefetch_tmap(&tmB2);
@@ -105,6 +107,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int k_blocks = (p.K + BK - 1) / BK;
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t full0 = smem_u32(bar.full), empty0 = smem_u32(bar.empty);
+  // grouped launch: A tiles are loaded and computed only as far as the group's rows reach (tma_load_a_rows)
+  const bool grouped = !PAIR && p.group_offsets != nullptr;
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
@@ -121,6 +125,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if constexpr (PAIR) n_idx = 2 * n_idx + rank;
         const bool phantom = PAIR && n_idx >= n_tiles;
         const int a_row = row0 + m_idx * BM;
+        const int a_rows = grouped ? tile_a_rows(rows, m_idx) : BM;
         // PAIR: this CTA's half of the A tile; a half wholly past the last row is never read back, so the box is moved onto
         // the first half rather than issued out of bounds
         const int a_half_row = a_row + (m_idx * BM + static_cast<int>(rank) * (BM / 2) < rows ? rank * (BM / 2) : 0);
@@ -152,8 +157,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               continue;
             }
           } else {
-            mbar_arrive_expect_tx_addr(fb, B_FP8 ? A_STAGE_BYTES : STAGE_BYTES);
-            tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
+            mbar_arrive_expect_tx_addr(fb, a_rows * (BK * 2) + (B_FP8 ? 0 : B_STAGE_BYTES));
+            tma_load_a_rows(sa, &tmA, &tmA_min, fb, kb * BK, a_row, a_rows);
           }
           if constexpr (B_MN) {
             // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n, BN/64 boxes per stage
@@ -244,19 +249,29 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         if constexpr (PAIR) mbar_arrive_cluster(&bar.empty[s], rank ^ 1);
       }
     };
+    // a tile this warpgroup computes nothing of: it waits for and releases every stage, so the barrier counts hold
+    auto pass_tile = [&] {
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+        release(rp.stage);
+        rp.next();
+      }
+    };
     for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
       int grp, m_idx, n_idx, row0, rows;
       if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
       if constexpr (PAIR) {
         n_idx = 2 * n_idx + rank;
-        if (n_idx >= n_tiles) {  // phantom tile: consume every stage the peer's multicast fills, compute nothing
-          for (int kb = 0; kb < k_blocks; ++kb) {
-            mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
-            release(rp.stage);
-            rp.next();
-          }
+        if (n_idx >= n_tiles) {  // phantom tile: the stages the peer's multicast fills
+          pass_tile();
           continue;
         }
+      }
+      // grouped: no row of the group in rows [64, 128) of the tile, which are then not loaded either.  A whole warpgroup sits
+      // out, so the named barrier of its stage_and_epilogue stays consistent.
+      if (sits_out(grouped && cw == 1 && rows - m_idx * BM <= BM / 2)) {
+        pass_tile();
+        continue;
       }
       float acc[BN / 2];
 #pragma unroll
@@ -323,12 +338,15 @@ ARIA_DEVICE void load_dense_col_scales(const GemmParams& p, const W8a8DenseScale
   }
 }
 
-// The W8A8 pipeline.  Grouped (DENSE = false): one B map over the [G * N_b, K] expert weights.  DENSE: up to three [N, K]
+// The W8A8 pipeline.  Grouped (DENSE = false): one B map over the [G * N_b, K] expert weights; A is loaded as far as the
+// group's rows reach and warpgroup 2 sits out tiles it has no row in, as in gemm_kernel's grouped launches (tmA_min:
+// tma_load_a_rows).  DENSE: up to three [N, K]
 // weights (tmB0..2, one per segment), a single group of p.M rows, and every epilogue of gemm_kernel (LINEAR with residual,
 // SWIGLU from separate gate and up weights, HEADS with RoPE).  The k-loop, the tile and the promotion are the same.
 template <int EPI, bool DENSE>
-ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, const CUtensorMap* tmB1, const CUtensorMap* tmB2,
-                           const GemmParams& p, const float* __restrict__ a_scale, const W8a8DenseScales& dsc) {
+ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmA_min, const CUtensorMap* tmB0, const CUtensorMap* tmB1,
+                           const CUtensorMap* tmB2, const GemmParams& p, const float* __restrict__ a_scale,
+                           const W8a8DenseScales& dsc) {
   constexpr int BN = 128;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + BN * W8_BK;
   constexpr int STAGES = GEMM_STAGES;
@@ -346,6 +364,7 @@ ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, cons
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(tmA);
+    if constexpr (!DENSE) prefetch_tmap(tmA_min);
     prefetch_tmap(tmB0);
     if constexpr (DENSE) {
       if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(tmB1);
@@ -374,6 +393,7 @@ ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, cons
         int grp, m_idx, n_idx, row0, rows;
         if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
         const int a_row = row0 + m_idx * BM;
+        const int a_rows = DENSE ? BM : tile_a_rows(rows, m_idx);  // rows of W8_BK e4m3 = 128 bytes, as the bf16 k-block's
         // B rows of the two 64-row boxes: (group, column c) is row group * N_b + c; SwiGLU takes the gate and the up box
         int b_r0, b_r1;
         const CUtensorMap* tb0 = tmB0;
@@ -401,8 +421,8 @@ ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, cons
           const uint32_t sa = smem_base + rp.stage * STAGE_BYTES;
           const uint32_t sb = sa + A_STAGE_BYTES;
           mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
-          mbar_arrive_expect_tx_addr(fb, STAGE_BYTES);
-          tma_load_2d_addr(sa, tmA, fb, kb * W8_BK, a_row);
+          mbar_arrive_expect_tx_addr(fb, a_rows * W8_BK + BN * W8_BK);
+          tma_load_a_rows(sa, tmA, tmA_min, fb, kb * W8_BK, a_row, a_rows);
           tma_load_2d_addr(sb, tb0, fb, kb * W8_BK, b_r0);
           tma_load_2d_addr(sb + 64 * W8_BK, tb1, fb, kb * W8_BK, b_r1);
           rp.next();
@@ -423,6 +443,15 @@ ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, cons
     for (int t = blockIdx.x;; t += gridDim.x) {
       int grp, m_idx, n_idx, row0, rows;
       if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+      // grouped: no row of the group in rows [64, 128) of the tile (gemm_kernel): wait for and release every stage
+      if (sits_out(!DENSE && cw == 1 && rows - m_idx * BM <= BM / 2)) {
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+          if (lane == 0) mbar_arrive(&bar.empty[rp.stage]);
+          rp.next();
+        }
+        continue;
+      }
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -456,9 +485,9 @@ ARIA_DEVICE void w8a8_body(const CUtensorMap* tmA, const CUtensorMap* tmB0, cons
 
 template <int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p,
-                 const float* __restrict__ a_scale) {
-  w8a8_body<EPI, false>(&tmA, &tmB, &tmB, &tmB, p, a_scale, W8a8DenseScales{});
+gemm_w8a8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA_min,
+                 const __grid_constant__ CUtensorMap tmB, const GemmParams p, const float* __restrict__ a_scale) {
+  w8a8_body<EPI, false>(&tmA, &tmA_min, &tmB, &tmB, &tmB, p, a_scale, W8a8DenseScales{});
 }
 
 template <int EPI>
@@ -466,7 +495,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_w8a8_dense_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
                        const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmParams p,
                        const float* __restrict__ a_scale, const W8a8DenseScales b_scale) {
-  w8a8_body<EPI, true>(&tmA, &tmB0, &tmB1, &tmB2, p, a_scale, b_scale);
+  w8a8_body<EPI, true>(&tmA, &tmA, &tmB0, &tmB1, &tmB2, p, a_scale, b_scale);
 }
 
 }  // namespace aria
@@ -588,11 +617,18 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   const bool pair = !b_scale && d->b_layout == ARIA_B_NK && d->num_groups == 1 && !d->group_offsets &&
                     d->epilogue == ARIA_EPI_LINEAR && d->m >= PAIR_MIN_ROWS;
 
-  CUtensorMap tmA, tmB[3];
+  CUtensorMap tmA, tmA_min, tmB[3];
   // a_rows: rows of the A buffer when groups live in fixed-capacity regions (m is then the EXPECTED row count that the
   // kernel-selection heuristics above use; the tensor map must cover the whole buffer).  Pairs: one box is a 64-row half.
-  int rc = make_tmap_2d(&tmA, d->a, d->k, d->a_rows > 0 ? d->a_rows : d->m, d->lda * 2, BK, pair ? BM / 2 : BM);
+  // Grouped launches also take the map with the small box (tma_load_a_rows).
+  const uint64_t a_buf_rows = d->a_rows > 0 ? d->a_rows : d->m;
+  int rc = make_tmap_2d(&tmA, d->a, d->k, a_buf_rows, d->lda * 2, BK, pair ? BM / 2 : BM);
   if (rc) return rc;
+  tmA_min = tmA;
+  if (d->group_offsets) {
+    rc = make_tmap_2d(&tmA_min, d->a, d->k, a_buf_rows, d->lda * 2, BK, A_BOX_MIN);
+    if (rc) return rc;
+  }
   if (b_mn) {
     const uint64_t ncols = swiglu ? 2 * d->n : d->n;
     const uint64_t n_weights = d->group_mod > 0 ? d->group_mod : (d->group_mod < 0 ? d->num_groups / (-d->group_mod) : d->num_groups);
@@ -620,12 +656,12 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   if (pair) {
     const int64_t m_tiles = (d->m + BM - 1) / BM, pairs = (tiles / m_tiles + 1) / 2 * m_tiles;
     return launch_persistent_pairs<gemm_kernel<128, false, ARIA_EPI_LINEAR, false, true>>(
-        "gemm_kernel", GEMM_THREADS, gemm_smem_bytes<128>(), pairs, stream, tmA, tmB[0], tmB[1], tmB[2], p);
+        "gemm_kernel", GEMM_THREADS, gemm_smem_bytes<128>(), pairs, stream, tmA, tmA_min, tmB[0], tmB[1], tmB[2], p);
   }
 #define ARIA_LAUNCH(BN_, MN_, EPI_, ...)                                                                                     \
   return launch_persistent<gemm_kernel<BN_, MN_, EPI_, ##__VA_ARGS__>>("gemm_kernel", GEMM_THREADS,                          \
                                                                        gemm_smem_bytes<BN_, ##__VA_ARGS__>(), tiles, stream, \
-                                                                       tmA, tmB[0], tmB[1], tmB[2], p)
+                                                                       tmA, tmA_min, tmB[0], tmB[1], tmB[2], p)
   if (b_scale) {
     if (swiglu) ARIA_LAUNCH(128, true, ARIA_EPI_SWIGLU, true);
     ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR, true);
@@ -687,8 +723,10 @@ extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, c
   const GemmParams p = gemm_params(&d, b_scale);
 
   // UINT8 maps, 128-byte swizzle: a box row is one 128-element k-block
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmA_min, tmB;  // A: the whole tile's box and the small one (tma_load_a_rows)
   int rc = make_tmap_2d(&tmA, a_fp8, k, rows, k, W8_BK, BM, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
+  if (rc) return rc;
+  rc = make_tmap_2d(&tmA_min, a_fp8, k, rows, k, W8_BK, A_BOX_MIN, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_DATA_TYPE_UINT8);
   if (rc) return rc;
   rc = make_tmap_2d(&tmB, b_fp8_nk, k, num_groups * (swiglu ? 2 * n : n), k, W8_BK, 64, CU_TENSOR_MAP_SWIZZLE_128B,
                     CU_TENSOR_MAP_DATA_TYPE_UINT8);
@@ -699,9 +737,9 @@ extern "C" int aria_grouped_gemm_w8a8(const void* a_fp8, const float* a_scale, c
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (swiglu)
     return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_SWIGLU>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA,
-                                                                 tmB, p, a_scale);
-  return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_LINEAR>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA, tmB,
-                                                              p, a_scale);
+                                                                 tmA_min, tmB, p, a_scale);
+  return launch_persistent<gemm_w8a8_kernel<ARIA_EPI_LINEAR>>("gemm_w8a8_kernel", GEMM_THREADS, SMEM, tiles, stream, tmA,
+                                                              tmA_min, tmB, p, a_scale);
 }
 
 extern "C" int aria_gemm_w8a8(const aria_gemm_desc_t* d, const float* a_scale, const float* const b_scale[3],

@@ -96,6 +96,32 @@ ARIA_DEVICE int tile_b_col(int x, int n_idx, int N) {
   else return n_idx * BN + x;
 }
 
+// Grouped launches (group_offsets != NULL) pack the groups' rows back to back, so a BM-row A box of a group's last m-tile would
+// mostly fetch other groups' rows: at 72 rows per expert 56 of 128, at batch-32 decode 125 of 128, again for every n-tile of
+// the group.  Their producer loads only the rows the group owns, rounded up to the smaller box of a second tensor map.
+constexpr int A_BOX_MIN = 16;
+ARIA_DEVICE int tile_a_rows(int rows, int m_idx) { return min(BM, (rows - m_idx * BM + A_BOX_MIN - 1) & ~(A_BOX_MIN - 1)); }
+
+// Loads the first n_rows (a multiple of A_BOX_MIN: tile_a_rows, or BM for a dense launch) rows of the A tile at row `row`
+// into the stage at `sa`, n_rows * 128 bytes on the mbarrier: a whole tile as the one box of `full`, a shorter one as boxes of
+// `small` (A_BOX_MIN rows).  SW128 swizzles by shared-memory address and a small box is two whole 1 KB swizzle atoms, so the
+// boxes compose to the bytes the BM-row box would have put there.  (A 64-row box in front of the small ones measured the same
+// as small boxes alone, DESIGN §6.)
+// INVARIANT: the stage's rows past n_rows keep whatever an earlier tile left there, and the consumers still multiply them.
+// That is safe only because row r of the accumulator depends on row r of A alone, and every epilogue a grouped launch
+// reaches (LINEAR, SWIGLU: one thread per row, stores under row_ok) neither stores a row at or past the group's end nor
+// reads another row's values for a row it stores.
+ARIA_DEVICE void tma_load_a_rows(uint32_t sa, const CUtensorMap* full, const CUtensorMap* small, uint32_t bar_addr, int c0,
+                                 int row, int n_rows) {
+  if (n_rows == BM) return tma_load_2d_addr(sa, full, bar_addr, c0, row);
+  for (int r = 0; r < n_rows; r += A_BOX_MIN) tma_load_2d_addr(sa + r * 128, small, bar_addr, c0, row + r);
+}
+
+// Whether a consumer warp skips a tile.  The condition is the same in every lane, which the compiler cannot see; taken from
+// lane 0 it is uniform to it as well.  Otherwise it treats the skip as a divergent branch and puts a warp re-convergence in
+// front of every k-block's first wgmma, which cost the compute-bound fp8 launches 2-4 % (H100 SXM, 700 W).
+ARIA_DEVICE bool sits_out(bool cond) { return __shfl_sync(0xffffffffu, cond ? 1 : 0, 0) != 0; }
+
 // A consumer thread: its place in the wgmma accumulator fragment of its warpgroup's 64 rows (cw: warpgroup 1 or 2 -> 0 / 1),
 // and the row it finishes in the epilogue with its `half` of the columns
 struct ConsumerThread {
