@@ -14,6 +14,8 @@ constexpr int FP8_LAND_STAGES = 3;
 constexpr int FP8_CONVERT_WARPS = 3;
 // Fewest rows of a dense LINEAR GEMM that runs as CTA pairs (gemm_run)
 constexpr int PAIR_MIN_ROWS = 2048;
+// Shortest reduction of a wide LINEAR GEMM that runs as CTA pairs (gemm_run)
+constexpr int WIDE_PAIR_MIN_K = 2048;
 template <int BN, bool B_FP8 = false>
 constexpr int gemm_smem_bytes() {
   return 1024 /*align*/ + GEMM_STAGES * (A_STAGE_BYTES + BN * BK * 2) + BM * acc_ld(BN) * 4 + 256 /*barriers*/ +
@@ -299,6 +301,275 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       stage_and_epilogue<BN, EPI, B_FP8 ? AccScale::COL : AccScale::NONE>(p, stg, ct, acc, bsc, 1.f, 1.f, n_out_total, grp,
                                                                            m_idx, n_idx, row0, rows);
     }
+  }
+  if constexpr (PAIR) cluster_sync();
+}
+
+// Wide dense GEMM for the 4,900-row ViT and projector launches (gemm_run): bf16, nn.Linear weights, LINEAR or HEADS without
+// RoPE.  128 x 192 tiles (1152 = 6 x 192), each consumer warpgroup one wgmma m64n192k16 per k16 step on its 64 rows.  The
+// epilogue runs on the accumulator registers: each thread rounds and activates its fragment exactly as epilogue_tile /
+// heads_store_tile do and writes it as bf16 into its warpgroup's 64 x 192 half of an output tile in shared memory (three
+// 64 x 64 SW128 boxes, 24 KB).  Without the fp32 staging tile of gemm_kernel the ring keeps four 40 KB stages.
+//   * LINEAR: one thread per warpgroup stores the half with TMA and does not wait for it; it waits for the store to have
+//     read the half during the next tile's first k-block.  With a residual, the producer TMA-loads the tile's residual rows
+//     into the half once that wait is over (out_free), on a barrier of its own (res_full), and the consumers add them at
+//     their fragment positions: out = bf16(x + res).
+//   * HEADS: the warpgroup reads its half back in 16-byte chunks and scatters them head-major with heads_store_tile's
+//     mapping; a 192-wide tile spans 2 2/3 heads of 72, so TMA cannot store it.
+// A half with no row of the launch is neither computed nor stored.  PAIR: the A-multicast CTA pairs of gemm_kernel (same
+// protocol, same phantom tile).
+constexpr int WIDE_BN = 192;
+constexpr int WIDE_STAGE_BYTES = A_STAGE_BYTES + WIDE_BN * BK * 2;  // 16 + 24 KB
+constexpr int WIDE_BOX_BYTES = 64 * 64 * 2;                         // one 64-row x 64-column bf16 SW128 box of the output
+constexpr int WIDE_HALF_BYTES = 3 * WIDE_BOX_BYTES;                 // a consumer warpgroup's 64 output rows
+constexpr int gemm_wide_smem_bytes() {
+  return 1024 /*align*/ + GEMM_STAGES * WIDE_STAGE_BYTES + 2 * WIDE_HALF_BYTES + 256 /*barriers*/;
+}
+static_assert(gemm_wide_smem_bytes() <= 232448, "wide GEMM must fit the opt-in shared memory of a block");
+
+// Byte offset of bf16 column c (even) of row r in a warpgroup's output half: box c / 64, its 16-byte chunk swizzled as TMA's
+// 128-byte swizzle places it
+ARIA_DEVICE uint32_t wide_out_offset(int r, int c) {
+  return (c >> 6) * WIDE_BOX_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
+}
+
+template <int EPI, bool PAIR>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
+                 const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2,
+                 const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmRes, const GemmParams p) {
+  constexpr int BN = WIDE_BN;
+  constexpr int STAGES = GEMM_STAGES;
+  static_assert(EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_HEADS, "wide GEMM epilogues");
+
+  uint8_t* smem = smem_1024();
+  uint8_t* out_tile = smem + STAGES * WIDE_STAGE_BYTES;  // [2 warpgroups][3 boxes][64 rows][128 B]
+  const BarrierRing<STAGES> bar(out_tile + 2 * WIDE_HALF_BYTES);
+  uint64_t* res_full = bar.empty + STAGES;  // [2]: the residual rows of a warpgroup's half have landed in it
+  uint64_t* out_free = res_full + 2;        // [2]: a warpgroup's previous TMA store has read its half
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
+  const bool res = EPI == ARIA_EPI_LINEAR && p.residual != nullptr;
+
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tmA);
+    prefetch_tmap(&tmB0);
+    if (p.n_seg > 1) prefetch_tmap(&tmB1);
+    if (p.n_seg > 2) prefetch_tmap(&tmB2);
+    if (EPI == ARIA_EPI_LINEAR) prefetch_tmap(&tmOut);
+    if (res) prefetch_tmap(&tmRes);
+    bar.init(1, PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(&res_full[h], 1);
+      mbar_init(&out_free[h], 1);
+    }
+    fence_mbar_init();
+  }
+  if constexpr (PAIR) cluster_sync();
+  else __syncthreads();
+
+  const int n_out_total = p.N * p.n_seg;
+  const int n_tiles = (n_out_total + BN - 1) / BN;
+  const int k_blocks = (p.K + BK - 1) / BK;
+  const uint32_t smem_base = smem_u32(smem);
+  const uint32_t full0 = smem_u32(bar.full), empty0 = smem_u32(bar.empty);
+  // output boxes of a tile that hold a column of the launch (fc1's 80-column tail tile: 2)
+  auto tile_boxes = [&](int col0) { return min(3, (n_out_total - col0 + 63) / 64); };
+
+  if (wg == 0) {
+    // =========================== TMA producer ===========================
+    setmaxnreg_dec<56>();  // the residual loads and the pair rank need more than 40
+    if (warp == 0 && elect_one()) {
+      const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+      TileSched sched;
+      sched.init(p, pair_sched_n<PAIR>(n_tiles));
+      RingPos<STAGES> rp;
+      uint32_t out_phase = 0;  // bit h: the phase of out_free[h] to wait for
+      for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
+        int grp, m_idx, n_idx, row0, rows;
+        if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+        if constexpr (PAIR) n_idx = 2 * n_idx + rank;
+        const bool phantom = PAIR && n_idx >= n_tiles;
+        const int a_row = m_idx * BM;
+        // PAIR: this CTA's half of the A tile, moved onto the first half when it lies wholly past the last row (gemm_kernel)
+        const int a_half_row = a_row + (a_row + static_cast<int>(rank) * (BM / 2) < rows ? rank * (BM / 2) : 0);
+        const int col0 = n_idx * BN;
+        const int seg = col0 / p.N;
+        const CUtensorMap* tb = seg == 0 ? &tmB0 : (seg == 1 ? &tmB1 : &tmB2);
+        const int b_row = col0 - seg * p.N;
+        // the residual goes in once the ring is full: by then the consumers are at this tile's first k-block, where they
+        // release the output tile
+        const int res_kb = min(STAGES - 1, k_blocks - 1);
+        for (int kb = 0; kb < k_blocks; ++kb) {
+          const uint32_t fb = full0 + rp.stage * 8;
+          const uint32_t sa = smem_base + rp.stage * WIDE_STAGE_BYTES;
+          mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
+          if constexpr (PAIR) {
+            mbar_arrive_expect_tx_addr(fb, phantom ? A_STAGE_BYTES : WIDE_STAGE_BYTES);
+            tma_load_2d_multicast_addr(sa + rank * (A_STAGE_BYTES / 2), &tmA, fb, kb * BK, a_half_row, 0b11);
+            if (phantom) {
+              rp.next();
+              continue;
+            }
+          } else {
+            mbar_arrive_expect_tx_addr(fb, WIDE_STAGE_BYTES);
+            tma_load_2d_addr(sa, &tmA, fb, kb * BK, a_row);
+          }
+          tma_load_2d_addr(sa + A_STAGE_BYTES, tb, fb, kb * BK, b_row);
+          rp.next();
+          if (res && kb == res_kb) {
+            const int nbox = tile_boxes(col0);
+            for (int h = 0; h < 2; ++h) {
+              if (a_row + 64 * h >= rows) continue;  // a half past the last row: no consumer waits for it
+              mbar_wait(&out_free[h], (out_phase >> h) & 1);
+              out_phase ^= 1u << h;
+              mbar_arrive_expect_tx(&res_full[h], nbox * WIDE_BOX_BYTES);
+              for (int c = 0; c < nbox; ++c)
+                tma_load_2d(out_tile + h * WIDE_HALF_BYTES + c * WIDE_BOX_BYTES, &tmRes, &res_full[h], col0 + 64 * c,
+                            a_row + 64 * h);
+            }
+          }
+        }
+      }
+    }
+  } else {
+    // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
+    setmaxnreg_inc<224>();
+    const int cw = wg - 1;
+    const uint64_t da0 = make_smem_desc(smem_base + cw * 64 * 128, 16, 1024);
+    const uint64_t db0 = make_smem_desc(smem_base + A_STAGE_BYTES, 16, 1024);
+    const ConsumerThread ct = consumer_thread(cw, lane);
+    const int fr = ct.frag_row - 64 * cw;  // fragment rows fr and fr + 8 of the warpgroup's half
+    const bool leader = (threadIdx.x & 127) == 0;
+    uint8_t* half = out_tile + cw * WIDE_HALF_BYTES;
+    const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+    TileSched sched;
+    sched.init(p, pair_sched_n<PAIR>(n_tiles));
+    RingPos<STAGES> rp;
+    uint32_t res_phase = 0;
+    auto release = [&](int s) {
+      if (lane == 0) {
+        mbar_arrive(&bar.empty[s]);
+        if constexpr (PAIR) mbar_arrive_cluster(&bar.empty[s], rank ^ 1);
+      }
+    };
+    auto pass_tile = [&] {
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+        release(rp.stage);
+        rp.next();
+      }
+    };
+    for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
+      int grp, m_idx, n_idx, row0, rows;
+      if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+      if constexpr (PAIR) n_idx = 2 * n_idx + rank;
+      // a phantom tile, or no row of the launch in this warpgroup's half (the 36-row last m-tile of 4,900)
+      if (sits_out((PAIR && n_idx >= n_tiles) || m_idx * BM + 64 * cw >= rows)) {
+        pass_tile();
+        continue;
+      }
+      const int col0 = n_idx * BN;
+      const int seg = col0 / p.N;
+      const int cseg0 = col0 - seg * p.N;
+      const __nv_bfloat16* bias = p.bias[seg];
+      // bias pairs of this thread's columns (8 j + frag_col, +1), fetched while the k-loop runs; columns past N get 0
+      uint32_t bias2[BN / 8];
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = cseg0 + 8 * j + ct.frag_col;
+        bias2[j] = (bias && c < p.N) ? __ldg(reinterpret_cast<const uint32_t*>(bias + c)) : 0u;
+      }
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb) {
+        mbar_wait_addr(full0 + rp.stage * 8, rp.phase);
+        const uint64_t da = da0 + rp.stage * (WIDE_STAGE_BYTES >> 4);
+        const uint64_t db = db0 + rp.stage * (WIDE_STAGE_BYTES >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) wgmma_m64n192_ss<0, 0>(acc, da + k * 2, db + k * 2, 1u);
+        wgmma_commit();
+        if (kb == 0 && leader) {
+          // the previous tile's store has read this half; with a residual the producer may now load this tile's
+          bulk_wait_group_read<0>();
+          if (res) mbar_arrive(&out_free[cw]);
+        }
+        wgmma_wait<1>();
+        if (prev >= 0) release(prev);
+        prev = static_cast<int>(rp.stage);
+        rp.next();
+      }
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (prev >= 0) release(prev);
+      if (res) {
+        mbar_wait(&res_full[cw], res_phase);
+        res_phase ^= 1;
+      }
+      // the leader has seen the previous store read the half (LINEAR), every thread has read its last chunks back (HEADS)
+      named_bar_sync(1 + cw, 128);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + ct.frag_col;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
+          uint32_t* dst = reinterpret_cast<uint32_t*>(half + wide_out_offset(fr + 8 * i, c));
+          float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
+          if (bias) {
+            x0 += bf16_lo(bias2[j]);
+            x1 += bf16_hi(bias2[j]);
+          }
+          if constexpr (EPI == ARIA_EPI_LINEAR) {
+            x0 = bf16r(x0);
+            x1 = bf16r(x1);
+            if (p.act != ARIA_ACT_NONE) {
+              x0 = bf16r(act_apply(x0, p.act));
+              x1 = bf16r(act_apply(x1, p.act));
+            }
+            if (res) {
+              const uint32_t r = *dst;
+              x0 += bf16_lo(r);
+              x1 += bf16_hi(r);
+            }
+          }
+          *dst = pack_bf16(x0, x1);
+        }
+        // one 64-column box at a time: hoisting all 48 residual loads ahead of the arithmetic spilled registers
+        if (j % 8 == 7) asm volatile("" ::: "memory");
+      }
+      if constexpr (EPI == ARIA_EPI_LINEAR) {
+        fence_proxy_async_smem();
+        named_bar_sync(1 + cw, 128);
+        if (leader) {
+          const int nbox = tile_boxes(col0);
+          for (int c = 0; c < nbox; ++c)
+            tma_store_2d_addr(&tmOut, smem_u32(half + c * WIDE_BOX_BYTES), col0 + 64 * c, m_idx * BM + 64 * cw);
+          bulk_commit_group();
+        }
+      } else {
+        named_bar_sync(1 + cw, 128);
+        // heads_store_tile's mapping: consecutive threads on consecutive 8-column chunks of a row
+        constexpr int CH = BN / 8;
+#pragma unroll 1
+        for (int i = threadIdx.x & 127; i < 64 * CH; i += 128) {
+          const int r = i / CH, c = (i % CH) * 8;
+          const int r_in_grp = m_idx * BM + 64 * cw + r;
+          const int cs = cseg0 + c;
+          if (r_in_grp >= rows || cs + 8 > p.N) continue;
+          const uint4 v = *reinterpret_cast<const uint4*>(half + wide_out_offset(r, c));
+          const int b = r_in_grp / p.rows_per_batch, tok = r_in_grp - b * p.rows_per_batch;
+          const int head = cs / p.head_dim, d = cs - head * p.head_dim;
+          *reinterpret_cast<uint4*>(p.out[seg] + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld +
+                                    head * p.stride_h + d) = v;
+        }
+      }
+    }
+    if (leader) bulk_wait_group_read<0>();  // no CTA leaves while a store still reads its shared memory
   }
   if constexpr (PAIR) cluster_sync();
 }
@@ -611,18 +882,27 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
     if (d->n_seg > 1 && !swiglu) ARIA_CHECK_ARG(d->n % BN == 0);
   }
 
-  // Dense bf16 LINEAR GEMMs with nn.Linear weights and at least PAIR_MIN_ROWS rows run as CTA pairs that share their A tile
-  // (gemm_kernel<.., PAIR>).  Measured on an H100 SXM at 700 W (DESIGN §6): the ViT's 4,900-row o_proj / fc1 / fc2 gain
-  // 3-12 %, while the LM's 768-row GEMMs and the 144-wide HEADS tiles lose 5-16 %, so those keep the one-CTA kernel.
-  const bool pair = !b_scale && d->b_layout == ARIA_B_NK && d->num_groups == 1 && !d->group_offsets &&
-                    d->epilogue == ARIA_EPI_LINEAR && d->m >= PAIR_MIN_ROWS;
+  // Dense bf16 GEMMs with nn.Linear weights and at least PAIR_MIN_ROWS rows, LINEAR or HEADS without RoPE (the ViT's four
+  // GEMMs, the projector's 4,900-row k / v and in-projections) run on gemm_wide_kernel; tiles must not straddle two weights.
+  // Measured on an H100 SXM at 700 W (DESIGN §6), µs before -> after: q/k/v heads 102.5 -> 83-85, o_proj 44.2 -> 34-36,
+  // fc1 149-152 -> 127, fc2 122.5 -> 95-96.  Only fc2, whose 68 k-blocks make the mainloop the cost, gains from CTA pairs
+  // (95 against 105 µs); o_proj, fc1 and the projector's k / v lose 10-25 % as pairs and q/k/v gains nothing, so pairs are
+  // selected for LINEAR at K >= WIDE_PAIR_MIN_K only.  Other dense LINEAR launches of PAIR_MIN_ROWS rows and more (several
+  // weights whose N is no multiple of 192) keep the 128-wide CTA pairs of gemm_kernel; the 768-row LM GEMMs lose 5-16 % as
+  // pairs and keep the one-CTA kernel.
+  const bool dense = !b_scale && d->b_layout == ARIA_B_NK && d->num_groups == 1 && !d->group_offsets;
+  const bool wide = dense && d->m >= PAIR_MIN_ROWS && (d->n_seg == 1 || d->n % WIDE_BN == 0) &&
+                    (d->epilogue == ARIA_EPI_HEADS ? !d->rope_mask : d->epilogue == ARIA_EPI_LINEAR);
+  const bool wide_pair = wide && d->epilogue == ARIA_EPI_LINEAR && d->k >= WIDE_PAIR_MIN_K;
+  const bool pair = !wide && dense && d->epilogue == ARIA_EPI_LINEAR && d->m >= PAIR_MIN_ROWS;
+  const bool half_a = wide_pair || pair;
 
   CUtensorMap tmA, tmA_min, tmB[3];
   // a_rows: rows of the A buffer when groups live in fixed-capacity regions (m is then the EXPECTED row count that the
   // kernel-selection heuristics above use; the tensor map must cover the whole buffer).  Pairs: one box is a 64-row half.
   // Grouped launches also take the map with the small box (tma_load_a_rows).
   const uint64_t a_buf_rows = d->a_rows > 0 ? d->a_rows : d->m;
-  int rc = make_tmap_2d(&tmA, d->a, d->k, a_buf_rows, d->lda * 2, BK, pair ? BM / 2 : BM);
+  int rc = make_tmap_2d(&tmA, d->a, d->k, a_buf_rows, d->lda * 2, BK, half_a ? BM / 2 : BM);
   if (rc) return rc;
   tmA_min = tmA;
   if (d->group_offsets) {
@@ -642,7 +922,7 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   } else {
     const int nb = swiglu ? 2 : d->n_seg;
     // rows of B staged per TMA box: the whole tile; SwiGLU splits gate | up
-    const uint32_t box_rows = swiglu ? BN / 2 : BN;
+    const uint32_t box_rows = swiglu ? BN / 2 : (wide ? WIDE_BN : BN);
     for (int s = 0; s < 3; ++s) {
       const void* ptr = s < nb ? d->b[s] : d->b[0];
       const uint64_t b_rows = b_gnk ? static_cast<uint64_t>(d->group_mod > 0 ? d->group_mod : (d->group_mod < 0 ? d->num_groups / (-d->group_mod) : d->num_groups)) * d->n : d->n;
@@ -652,6 +932,30 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   }
 
   const GemmParams p = gemm_params(d, b_scale);
+  if (wide) {
+    // out / residual: 64 x 64 boxes of the [m, n_seg n] row-major buffers
+    CUtensorMap tmOut = tmA, tmRes = tmA;
+    const uint64_t n_out = d->n * d->n_seg;
+    if (d->epilogue == ARIA_EPI_LINEAR) {
+      rc = make_tmap_2d(&tmOut, d->out[0], n_out, d->m, d->ldo * 2, 64, 64);
+      if (rc) return rc;
+      if (d->residual) {
+        rc = make_tmap_2d(&tmRes, d->residual, n_out, d->m, d->ldr * 2, 64, 64);
+        if (rc) return rc;
+      }
+    }
+    const int64_t m_tiles = (d->m + BM - 1) / BM, n_tiles = (n_out + WIDE_BN - 1) / WIDE_BN;
+    if (wide_pair)
+      return launch_persistent_pairs<gemm_wide_kernel<ARIA_EPI_LINEAR, true>>("gemm_wide_kernel", GEMM_THREADS,
+                                                                              gemm_wide_smem_bytes(), (n_tiles + 1) / 2 * m_tiles,
+                                                                              stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p);
+#define ARIA_LAUNCH_WIDE(EPI_)                                                                                                \
+  return launch_persistent<gemm_wide_kernel<EPI_, false>>("gemm_wide_kernel", GEMM_THREADS, gemm_wide_smem_bytes(),         \
+                                                          n_tiles * m_tiles, stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p)
+    if (d->epilogue == ARIA_EPI_HEADS) ARIA_LAUNCH_WIDE(ARIA_EPI_HEADS);
+    ARIA_LAUNCH_WIDE(ARIA_EPI_LINEAR);
+#undef ARIA_LAUNCH_WIDE
+  }
   const int64_t tiles = max_tiles(d, BN, d->num_groups > 1 ? d->num_groups : 0);
   if (pair) {
     const int64_t m_tiles = (d->m + BM - 1) / BM, pairs = (tiles / m_tiles + 1) / 2 * m_tiles;
