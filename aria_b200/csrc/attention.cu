@@ -17,6 +17,9 @@
 // lies in [0, 256] and is rounded to bf16 at that scale, which measured closer to transformers' eager attention (the reference
 // of the ViT path) than rounding P relative to the exact running max, and it skips most rescales of O.
 //
+// aria_attention_fwd_varlen: causal attention over sequences packed along one row (padding-free fine-tuning), on the
+//   shared-prefix prefill's pipeline with no prefix; each sequence bit-identical to aria_attention_fwd_lse on it alone.
+//
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
 // aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
@@ -132,7 +135,7 @@ template <int HD, bool CAUSAL, bool LSE, bool SHARED>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                               const CUtensorMap& tmK16, const CUtensorMap& tmV16, const CUtensorMap& tmPK,
                                               const CUtensorMap& tmPV, const AttnParams& p, const SharedPrefixParams& sp) {
-  static_assert(!SHARED || (HD == 128 && !CAUSAL && !LSE), "the shared-prefix prefill runs at head dim 128 with its own mask");
+  static_assert(!SHARED || (HD == 128 && !CAUSAL), "the shared-prefix prefill runs at head dim 128 with its own mask");
   constexpr int S = AttnCfg<HD>::STAGES, KVT = AttnCfg<HD>::KV_TILE, NO = AttnCfg<HD>::NO;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -489,12 +492,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 }
 
 // One CTA per (head, 128 packed queries): tmQ / tmK / tmV map the packed suffix [1, H, S_tot, 128], tmPK / tmPV the prefix
-// cache [1, H, P, 128] (rows past P are outside the map: never read)
+// cache [1, H, P, 128] (rows past P are outside the map: never read).  With P = 0 this is the varlen causal forward
+// (aria_attention_fwd_varlen): every key tile is aligned at its segment's start; LSE adds the logsumexp store [H, S_tot].
+template <bool LSE>
 __global__ void __launch_bounds__(AT_THREADS, 1)
 attn_prefill_shared_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmPK,
                                   const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const SharedPrefixParams sp) {
-  attn_fwd_body<128, false, false, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, sp);
+  attn_fwd_body<128, false, LSE, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, sp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1096,9 +1101,52 @@ extern "C" int aria_attention_prefill_shared_prefix(const void* q, const void* k
   const SharedPrefixParams sp{cu_seqlens, B, P};
   constexpr int smem = AttnCfg<128>::SMEM;
   static bool attr_set[kMaxDevices] = {};
-  if (ensure_dynamic_smem(attr_set, attn_prefill_shared_prefix_kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
-  attn_prefill_shared_prefix_kernel<<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
+  if (ensure_dynamic_smem(attr_set, attn_prefill_shared_prefix_kernel<false>, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_prefill_shared_prefix_kernel<false><<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
       tmQ, tmK, tmV, tmPK, tmPV, p, sp);
+  return check_launch("attn_prefill_shared_prefix_kernel");
+}
+
+extern "C" int aria_attention_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int32_t* cu_seqlens,
+                                         int32_t n_seg, int32_t H, int32_t N, int64_t q_stride_h, int64_t kv_stride_h, float scale,
+                                         aria_stream_t stream_) {
+  ARIA_CHECK_ARG(q && k && v && out && cu_seqlens);
+  ARIA_CHECK_ARG(n_seg > 0 && H > 0 && N >= n_seg);
+  ARIA_CHECK_ARG(q_stride_h >= static_cast<int64_t>(N) * AT_D && kv_stride_h >= static_cast<int64_t>(N) * AT_D);
+  ARIA_CHECK_ARG(q_stride_h % 8 == 0 && kv_stride_h % 8 == 0);
+  ARIA_CHECK_ARG(!lse || (reinterpret_cast<uintptr_t>(lse) & 3) == 0);
+  const int n_q_tiles = (N + AT_BM - 1) / AT_BM;
+  ARIA_CHECK_ARG(static_cast<int64_t>(H) * n_q_tiles < (1ll << 31));
+  // the shared-prefix pipeline with no prefix: the prefix maps are never read
+  CUtensorMap tmQ, tmK, tmV;
+  int rc = make_tmap_heads(&tmQ, q, N, H, 1, q_stride_h * H, q_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmK, k, N, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmV, v, N, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  AttnParams p{};
+  p.B = 1;
+  p.H = H;
+  p.Tq = N;
+  p.Tk = N;
+  p.out_hd = AT_D;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.lse = lse;
+  p.n_q_tiles = n_q_tiles;
+  const SharedPrefixParams sp{cu_seqlens, n_seg, 0};
+  constexpr int smem = AttnCfg<128>::SMEM;
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (lse) {
+    static bool attr_set[kMaxDevices] = {};
+    if (ensure_dynamic_smem(attr_set, attn_prefill_shared_prefix_kernel<true>, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+    attn_prefill_shared_prefix_kernel<true><<<H * n_q_tiles, AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, tmK, tmV, p, sp);
+  } else {
+    static bool attr_set[kMaxDevices] = {};
+    if (ensure_dynamic_smem(attr_set, attn_prefill_shared_prefix_kernel<false>, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+    attn_prefill_shared_prefix_kernel<false><<<H * n_q_tiles, AT_THREADS, smem, stream>>>(tmQ, tmK, tmV, tmK, tmV, p, sp);
+  }
   return check_launch("attn_prefill_shared_prefix_kernel");
 }
 

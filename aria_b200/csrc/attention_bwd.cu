@@ -20,6 +20,15 @@
 //   attn_bwd_post  dQ = bf16(scale * accumulator).
 // dK and dV are each produced by exactly one CTA in a fixed order: bit-reproducible.  dQ sums the key tiles' contributions with
 // fp32 atomics, so its low bits depend on their arrival order.
+//
+// aria_attention_bwd_varlen: the same three kernels over n_seg causal segments packed along one row axis (B = 1), segment s =
+// rows [cu[s], cu[s+1]).  attn_bwd_varlen_tiles first lists the segments' 128-key tiles, each aligned at its segment's start,
+// heaviest (most query rows) first; attn_bwd_kernel<true, true> takes one tile per CTA and walks 64-row query steps from the
+// tile's first row to the segment's end.  Query rows at or past the segment's end get P = 0 (and so add exact zeros to dQ);
+// keys past it are masked by causality for the segment's own queries, and their dK / dV rows are not stored.  Per segment the
+// tiles, the query steps and their order are those of aria_attention_bwd on the segment alone, so dK and dV are bit-identical
+// to it.  The statistics and the dQ accumulator carry one extra 64-row step past N (lse2 = +inf), so a step that starts at an
+// unaligned row never leaves them.
 #include "common.cuh"
 #include "ptx.cuh"
 
@@ -40,6 +49,9 @@ constexpr int AB_SMEM = 1024 + 2 * AB_KV + AB_STAGES * 2 * AB_QT + 2 * AB_DS + 2
 // workspace: dq_acc [B*H][Tq_pad][128] fp32, then lse2 and delta [B*H][Tq_pad] fp32 (query rows padded to the 64-row step, so
 // the main kernel reads statistics and adds dQ without bounds checks: pad rows carry lse2 = +inf, i.e. P = 0)
 static int64_t bwd_tq_pad(int32_t Tq) { return (static_cast<int64_t>(Tq) + AB_BM - 1) / AB_BM * AB_BM; }
+// varlen: query steps start at any row, so one more step of padding; and at most ceil(N / 128) + n_seg key tiles
+static int64_t bwd_varlen_pad(int32_t N) { return bwd_tq_pad(N) + AB_BM; }
+static int64_t bwd_varlen_slots(int32_t n_seg, int32_t N) { return (static_cast<int64_t>(N) + AB_BN - 1) / AB_BN + n_seg; }
 
 struct AttnBwdParams {
   int B, H, Tq, Tk, Tq_pad;
@@ -51,7 +63,43 @@ struct AttnBwdParams {
   __nv_bfloat16* dk;        // head-major, kv strides
   __nv_bfloat16* dv;
   int64_t kv_stride_b, kv_stride_h;
+  const int2* tiles;        // varlen: [slots] {first key row, segment end} per key tile, heaviest first; {-1, 0} = idle slot
 };
+
+// Varlen key-tile list (one block): tile t of segment s is {cu[s] + 128 t, cu[s+1]}; a counting sort on the number of 64-row
+// query steps it walks puts the heaviest first (as the batched launch's tile order does), then the unused slots are idled.
+// Boundaries are clamped to [0, N] and at most `slots` tiles are listed, so malformed boundaries (not nondecreasing from 0 to
+// N) give wrong gradients but never a read or write outside q / k / v, dq / dk / dv or the workspace.
+constexpr int AB_WEIGHTS = 1024;  // sort classes: query steps, capped (longer tiles are all "heaviest")
+__global__ void __launch_bounds__(1024) attn_bwd_varlen_tiles(const int32_t* __restrict__ cu, int n_seg, int N, int slots,
+                                                                int2* __restrict__ tiles) {
+  __shared__ int slot[AB_WEIGHTS];
+  __shared__ int total;
+  auto weight = [](int rows) { return min((rows + AB_BM - 1) / AB_BM, AB_WEIGHTS - 1); };
+  for (int w = threadIdx.x; w < AB_WEIGHTS; w += blockDim.x) slot[w] = 0;
+  __syncthreads();
+  auto start = [&](int s) { return min(max(cu[s], 0), N); };
+  auto end = [&](int s) { return min(max(cu[s + 1], 0), N); };
+  for (int s = threadIdx.x; s < n_seg; s += blockDim.x)
+    for (int k0 = start(s), e = end(s); k0 < e; k0 += AB_BN) atomicAdd(&slot[weight(e - k0)], 1);
+  __syncthreads();
+  if (threadIdx.x == 0) {  // first slot of each class, heaviest class first
+    int run = 0;
+    for (int w = AB_WEIGHTS - 1; w >= 0; --w) {
+      const int n = slot[w];
+      slot[w] = run;
+      run += n;
+    }
+    total = min(run, slots);
+  }
+  __syncthreads();
+  for (int s = threadIdx.x; s < n_seg; s += blockDim.x)
+    for (int k0 = start(s), e = end(s); k0 < e; k0 += AB_BN) {
+      const int i = atomicAdd(&slot[weight(e - k0)], 1);
+      if (i < slots) tiles[i] = make_int2(k0, e);
+    }
+  for (int i = total + threadIdx.x; i < slots; i += blockDim.x) tiles[i] = make_int2(-1, 0);
+}
 
 // one warp per (b, h, padded query row)
 __global__ void __launch_bounds__(256) attn_bwd_pre(const __nv_bfloat16* __restrict__ out, const __nv_bfloat16* __restrict__ dout,
@@ -84,10 +132,12 @@ __global__ void __launch_bounds__(256) attn_bwd_pre(const __nv_bfloat16* __restr
   }
 }
 
-template <bool CAUSAL>
+// VARLEN (causal, B = 1): the CTA's key tile and its segment's end come from p.tiles; see the header
+template <bool CAUSAL, bool VARLEN>
 __global__ void __launch_bounds__(AB_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO, const AttnBwdParams p) {
+  static_assert(!VARLEN || CAUSAL, "packed segments are causal");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sK = smem;                             // [2 chunks][128 keys][64]
@@ -104,10 +154,20 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int bh = blockIdx.x % BH;
   const int k_tile = blockIdx.x / BH;             // causal: the earliest keys are seen by the most queries
   const int b = bh / p.H, h = bh % p.H;
-  const int k0 = k_tile * AB_BN;
+  int k0 = k_tile * AB_BN;
   const int pos_off = p.Tk - p.Tq;
-  const int n_m = (p.Tq + AB_BM - 1) / AB_BM;
-  const int m_begin = CAUSAL ? max(0, k0 - pos_off) / AB_BM : 0;  // earlier query tiles see none of these keys
+  int n_m = (p.Tq + AB_BM - 1) / AB_BM;
+  int m_begin = CAUSAL ? max(0, k0 - pos_off) / AB_BM : 0;  // earlier query tiles see none of these keys
+  int m_base = 0;                                 // row of query step 0 (varlen: the key tile's first row)
+  int seg_end = p.Tk;                             // keys and query rows at or past it are dead
+  if constexpr (VARLEN) {
+    const int2 t = p.tiles[k_tile];
+    if (t.x < 0) return;                          // idle slot: the grid is an upper bound on the tile count
+    k0 = m_base = t.x;
+    seg_end = t.y;
+    m_begin = 0;
+    n_m = (seg_end - k0 + AB_BM - 1) / AB_BM;
+  }
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmQ);
@@ -123,10 +183,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // Q and dO tiles of query tile i into ring stage s
   auto load_qd = [&](int i, int s) {
     mbar_arrive_expect_tx(&qd_full[s], 2 * AB_QT);
-    tma_load_4d(sQ + s * AB_QT, &tmQ, &qd_full[s], 0, i * AB_BM, h, b);
-    tma_load_4d(sQ + s * AB_QT + AB_QT_HALF, &tmQ, &qd_full[s], 64, i * AB_BM, h, b);
-    tma_load_3d(sdO + s * AB_QT, &tmdO, &qd_full[s], h * AB_D, i * AB_BM, b);
-    tma_load_3d(sdO + s * AB_QT + AB_QT_HALF, &tmdO, &qd_full[s], h * AB_D + 64, i * AB_BM, b);
+    const int m0 = m_base + i * AB_BM;
+    tma_load_4d(sQ + s * AB_QT, &tmQ, &qd_full[s], 0, m0, h, b);
+    tma_load_4d(sQ + s * AB_QT + AB_QT_HALF, &tmQ, &qd_full[s], 64, m0, h, b);
+    tma_load_3d(sdO + s * AB_QT, &tmdO, &qd_full[s], h * AB_D, m0, b);
+    tma_load_3d(sdO + s * AB_QT + AB_QT_HALF, &tmdO, &qd_full[s], h * AB_D + 64, m0, b);
   };
   const bool loader = threadIdx.x == 0;
   if (loader) {
@@ -144,8 +205,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int key_lo = k0 + cw * 64 + kr, key_hi = key_lo + 8;
   const int kq = 2 * (lane & 3);                  // column offset of this thread in an 8-wide block
   const uint8_t* km = p.key_mask ? p.key_mask + static_cast<int64_t>(b) * p.Tk : nullptr;
-  const bool dead_lo = key_lo >= p.Tk || (km && km[key_lo]);
-  const bool dead_hi = key_hi >= p.Tk || (km && km[key_hi]);
+  const bool dead_lo = key_lo >= seg_end || (km && km[key_lo]);
+  const bool dead_hi = key_hi >= seg_end || (km && km[key_hi]);
   const uint32_t sKa = smem_u32(sK), sVa = smem_u32(sV), sQa = smem_u32(sQ), sdOa = smem_u32(sdO), sdSa = smem_u32(sdS);
   // K-major k-step kk (16 head dims): chunk kk / 4, +32 B per step inside the chunk
   auto kv_kmaj = [](int kk) { return static_cast<uint32_t>((kk >> 2) * AB_KV_HALF + (kk & 3) * 32); };
@@ -163,7 +224,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
   for (int i = m_begin; i < n_m; ++i) {
     const int it = i - m_begin, s = it % AB_STAGES;
-    const int m0 = i * AB_BM;
+    const int m0 = m_base + i * AB_BM;
     const uint32_t sQs = sQa + s * AB_QT, sdOs = sdOa + s * AB_QT;
     float st[32], dp[32];
     mbar_wait(&qd_full[s], (it / AB_STAGES) & 1);
@@ -184,21 +245,25 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     // P^T: row = key, column = query m0 + 8 jj + kq + e
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
-      const float2 l2 = *reinterpret_cast<const float2*>(lse2 + m0 + 8 * jj + kq);
+      // varlen steps start at any row: two 4-byte loads where the pair may be 8-byte misaligned
+      const float2 l2 = VARLEN ? make_float2(lse2[m0 + 8 * jj + kq], lse2[m0 + 8 * jj + kq + 1])
+                               : *reinterpret_cast<const float2*>(lse2 + m0 + 8 * jj + kq);
       st[4 * jj] = fast_ex2(fmaf(st[4 * jj], p.scale_log2, -l2.x));
       st[4 * jj + 1] = fast_ex2(fmaf(st[4 * jj + 1], p.scale_log2, -l2.y));
       st[4 * jj + 2] = fast_ex2(fmaf(st[4 * jj + 2], p.scale_log2, -l2.x));
       st[4 * jj + 3] = fast_ex2(fmaf(st[4 * jj + 3], p.scale_log2, -l2.y));
     }
-    const bool need_mask = km != nullptr || k0 + AB_BN > p.Tk || (CAUSAL && k0 + cw * 64 + 63 > pos_off + m0);
-    if (need_mask) {  // diagonal / key tail / padded keys
+    const bool need_mask = km != nullptr || k0 + AB_BN > seg_end || (CAUSAL && k0 + cw * 64 + 63 > pos_off + m0) ||
+                           (VARLEN && m0 + AB_BM > seg_end);
+    if (need_mask) {  // diagonal / key tail / padded keys / (varlen) query rows past the segment
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int qpos = pos_off + m0 + 8 * jj + kq + e;
-          if (dead_lo || (CAUSAL && key_lo > qpos)) st[4 * jj + e] = 0.f;
-          if (dead_hi || (CAUSAL && key_hi > qpos)) st[4 * jj + 2 + e] = 0.f;
+          const bool qdead = VARLEN && qpos >= seg_end;
+          if (dead_lo || qdead || (CAUSAL && key_lo > qpos)) st[4 * jj + e] = 0.f;
+          if (dead_hi || qdead || (CAUSAL && key_hi > qpos)) st[4 * jj + 2 + e] = 0.f;
         }
       }
     }
@@ -218,7 +283,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 
 #pragma unroll
     for (int jj = 0; jj < 8; ++jj) {
-      const float2 dd = *reinterpret_cast<const float2*>(delta + m0 + 8 * jj + kq);
+      const float2 dd = VARLEN ? make_float2(delta[m0 + 8 * jj + kq], delta[m0 + 8 * jj + kq + 1])
+                               : *reinterpret_cast<const float2*>(delta + m0 + 8 * jj + kq);
       dp[4 * jj] = st[4 * jj] * (dp[4 * jj] - dd.x);
       dp[4 * jj + 1] = st[4 * jj + 1] * (dp[4 * jj + 1] - dd.y);
       dp[4 * jj + 2] = st[4 * jj + 2] * (dp[4 * jj + 2] - dd.x);
@@ -274,7 +340,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 #pragma unroll
   for (int hrow = 0; hrow < 2; ++hrow) {
     const int key = hrow ? key_hi : key_lo;
-    if (key >= p.Tk) continue;
+    if (key >= seg_end) continue;
     __nv_bfloat16* dkr = p.dk + base + static_cast<int64_t>(key) * AB_D;
     __nv_bfloat16* dvr = p.dv + base + static_cast<int64_t>(key) * AB_D;
 #pragma unroll
@@ -309,10 +375,10 @@ static int make_tmap_heads_box(CUtensorMap* tm, const void* ptr, int T, int H, i
   return make_tmap_bf16(tm, ptr, 4, dims, str, box);
 }
 
-template <bool CAUSAL>
+template <bool CAUSAL, bool VARLEN = false>
 static int launch_attn_bwd(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV, const CUtensorMap& tmdO,
                            const AttnBwdParams& p, int64_t grid, cudaStream_t stream) {
-  auto kern = attn_bwd_kernel<CAUSAL>;
+  auto kern = attn_bwd_kernel<CAUSAL, VARLEN>;
   static bool attr_set[kMaxDevices] = {};
   if (ensure_dynamic_smem(attr_set, kern, AB_SMEM) != cudaSuccess) return ARIA_ERR_CUDA;
   kern<<<static_cast<int>(grid), AB_THREADS, AB_SMEM, stream>>>(tmQ, tmK, tmV, tmdO, p);
@@ -392,5 +458,82 @@ extern "C" int aria_attention_bwd(const void* q, const void* k, const void* v, c
   if (rc) return rc;
   attn_bwd_post<<<static_cast<int>((post_n + 255) / 256), 256, 0, stream>>>(ws, static_cast<__nv_bfloat16*>(dq), H, Tq,
                                                                             static_cast<int>(Tq_pad), q_stride_b, q_stride_h, scale, post_n);
+  return check_launch("attn_bwd_post");
+}
+
+extern "C" int64_t aria_attention_bwd_varlen_workspace_bytes(int32_t n_seg, int32_t H, int32_t N) {
+  if (n_seg <= 0 || H <= 0 || N < n_seg) return 0;
+  const int64_t slots = (bwd_varlen_slots(n_seg, N) * static_cast<int64_t>(sizeof(int2)) + 15) / 16 * 16;
+  return static_cast<int64_t>(H) * bwd_varlen_pad(N) * (AB_D + 2) * static_cast<int64_t>(sizeof(float)) + slots;
+}
+
+extern "C" int aria_attention_bwd_varlen(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
+                                         void* dq, void* dk, void* dv, const int32_t* cu_seqlens, int32_t n_seg, int32_t H, int32_t N,
+                                         int64_t q_stride_h, int64_t kv_stride_h, float scale, void* workspace, int64_t workspace_bytes,
+                                         aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && k && v && out && dout && lse && dq && dk && dv && cu_seqlens && workspace);
+  ARIA_CHECK_ARG(n_seg > 0 && H > 0 && N >= n_seg);
+  ARIA_CHECK_ARG(q_stride_h >= static_cast<int64_t>(N) * AB_D && kv_stride_h >= static_cast<int64_t>(N) * AB_D);
+  ARIA_CHECK_ARG(q_stride_h % 8 == 0 && kv_stride_h % 8 == 0);
+  auto aligned = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  ARIA_CHECK_ARG(aligned(q) && aligned(k) && aligned(v) && aligned(out) && aligned(dout) && aligned(dq) && aligned(dk) && aligned(dv) &&
+                 aligned(workspace) && (reinterpret_cast<uintptr_t>(lse) & 3) == 0 && (reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0);
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_bwd_varlen_workspace_bytes(n_seg, H, N));
+  const int64_t pad = bwd_varlen_pad(N);
+  const int64_t slots = bwd_varlen_slots(n_seg, N);
+  const int64_t grid = static_cast<int64_t>(H) * slots;
+  const int64_t pre_rows = static_cast<int64_t>(H) * pad;
+  const int64_t post_n = static_cast<int64_t>(H) * N * 32;
+  ARIA_CHECK_ARG(grid < (1ll << 31) && (pre_rows + 7) / 8 < (1ll << 31) && (post_n + 255) / 256 < (1ll << 31));
+  ARIA_CHECK_ARG(static_cast<int64_t>(H) * AB_D * 2 * N < (1ll << 40));
+
+  // one batch row: its stride is never stepped
+  CUtensorMap tmQ, tmK, tmV, tmdO;
+  int rc = make_tmap_heads_box(&tmQ, q, N, H, 1, q_stride_h * H, q_stride_h, AB_BM);
+  if (rc) return rc;
+  rc = make_tmap_heads_box(&tmK, k, N, H, 1, kv_stride_h * H, kv_stride_h, AB_BN);
+  if (rc) return rc;
+  rc = make_tmap_heads_box(&tmV, v, N, H, 1, kv_stride_h * H, kv_stride_h, AB_BN);
+  if (rc) return rc;
+  {  // dO is token-major [N, H*128]
+    uint64_t dims[3] = {static_cast<uint64_t>(H) * AB_D, static_cast<uint64_t>(N), 1};
+    uint64_t str[2] = {static_cast<uint64_t>(H) * AB_D * 2, static_cast<uint64_t>(H) * AB_D * 2 * N};
+    uint32_t box[3] = {64, AB_BM, 1};
+    rc = make_tmap_bf16(&tmdO, dout, 3, dims, str, box);
+    if (rc) return rc;
+  }
+
+  float* ws = static_cast<float*>(workspace);
+  AttnBwdParams p{};
+  p.B = 1;
+  p.H = H;
+  p.Tq = N;
+  p.Tk = N;
+  p.Tq_pad = static_cast<int>(pad);
+  p.scale = scale;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.dq_acc = ws;
+  p.lse2 = ws + pre_rows * AB_D;
+  p.delta = p.lse2 + pre_rows;
+  p.dk = static_cast<__nv_bfloat16*>(dk);
+  p.dv = static_cast<__nv_bfloat16*>(dv);
+  p.kv_stride_b = static_cast<int64_t>(H) * kv_stride_h;
+  p.kv_stride_h = kv_stride_h;
+  int2* tiles = reinterpret_cast<int2*>(ws + pre_rows * (AB_D + 2));
+  p.tiles = tiles;
+
+  attn_bwd_varlen_tiles<<<1, 1024, 0, stream>>>(cu_seqlens, n_seg, N, static_cast<int>(slots), tiles);
+  rc = check_launch("attn_bwd_varlen_tiles");
+  if (rc) return rc;
+  attn_bwd_pre<<<static_cast<int>((pre_rows + 7) / 8), 256, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(out), static_cast<const __nv_bfloat16*>(dout), lse, ws, ws + pre_rows * AB_D,
+      ws + pre_rows * AB_D + pre_rows, H, N, static_cast<int>(pad), pre_rows);
+  rc = check_launch("attn_bwd_pre");
+  if (rc) return rc;
+  rc = launch_attn_bwd<true, true>(tmQ, tmK, tmV, tmdO, p, grid, stream);
+  if (rc) return rc;
+  attn_bwd_post<<<static_cast<int>((post_n + 255) / 256), 256, 0, stream>>>(ws, static_cast<__nv_bfloat16*>(dq), H, N,
+                                                                            static_cast<int>(pad), 0, q_stride_h, scale, post_n);
   return check_launch("attn_bwd_post");
 }

@@ -1077,6 +1077,60 @@ def attention_prefill_shared_prefix(q: torch.Tensor, k: torch.Tensor, v: torch.T
     return out
 
 
+def _varlen_qkv(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens: torch.Tensor, N: Optional[int], what: str):
+    """Packed q / k / v [1,H,>=N,128] and cu_seqlens int32 [n_seg+1] -> (n_seg, H, N)."""
+    _attn_qkv_check(q, k, v, what)
+    N = q.shape[2] if N is None else N
+    n_seg = _packed_check(N, cu_seqlens, what)
+    H = q.shape[1]
+    if q.shape[0] != 1 or q.shape[2] < N or k.shape[:2] != (1, H) or k.shape[2] < N or v.shape != k.shape:
+        raise ValueError(f"{what}: q {tuple(q.shape)} / k {tuple(k.shape)} must be [1, H, >= {N}, 128]")
+    return n_seg, H, N
+
+
+def attention_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, cu_seqlens: torch.Tensor, scale: float,
+                     return_lse: bool = False, N: Optional[int] = None):
+    """Causal attention over packed sequences (padding-free batches).  q / k / v [1,H,>=N,128] head-major (first N rows used,
+    N = q.shape[2] by default; 128-element rows as in `attention`) hold n_seg sequences back to back: sequence s is rows
+    [cu_seqlens[s], cu_seqlens[s+1]) (cu_seqlens CUDA int32 [n_seg+1], nondecreasing from 0 to N, no empty sequence; not checked
+    here, see hf_attention).  The query at packed row r of sequence s sees the packed keys [cu_seqlens[s], r] -> out [N, H*128],
+    and with return_lse=True also lse [H, N] fp32.  Each sequence's out and lse are bit-identical to
+    `attention(..., causal=True, return_lse=True)` on that sequence alone.  See aria_attention_fwd_varlen."""
+    n_seg, H, N = _varlen_qkv(q, k, v, cu_seqlens, N, "attention_varlen")
+    out = torch.empty((N, H * 128), dtype=bf16, device=q.device)
+    lse = torch.empty((H, N), dtype=torch.float32, device=q.device) if return_lse else None
+    with torch.cuda.device(q.device):
+        L.check(L.load().aria_attention_fwd_varlen(_p(q), _p(k), _p(v), _p(out), _p(lse), _p(cu_seqlens), n_seg, H, N, q.stride(1),
+                                                   k.stride(1), scale, _stream(q)), "attention_fwd_varlen")
+    return (out, lse) if return_lse else out
+
+
+def attention_varlen_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, dout: torch.Tensor, lse: torch.Tensor,
+                         cu_seqlens: torch.Tensor, scale: float, N: Optional[int] = None):
+    """Backward of `attention_varlen(..., return_lse=True)`: q / k / v and cu_seqlens as there, out / dout [N, H*128] (or
+    [1, N, H*128]), lse [H, N] -> (dq, dk, dv) [1,H,N,128] bf16.  Per sequence, dk and dv are bit-identical to `attention_bwd`
+    (causal) on that sequence alone, dq equal to it up to the order of fp32 atomic additions."""
+    n_seg, H, N = _varlen_qkv(q, k, v, cu_seqlens, N, "attention_varlen_bwd")
+    _chk(out), _chk(dout), _chk(lse, torch.float32, align=4)
+    assert out.numel() == N * H * 128 and dout.shape == out.shape and lse.shape == (H, N)
+    dq = torch.empty((1, H, N, 128), dtype=bf16, device=q.device)
+    dk = torch.empty_like(dq)
+    dv = torch.empty_like(dq)
+    lib = L.load()
+    ws_bytes = lib.aria_attention_bwd_varlen_workspace_bytes(n_seg, H, N)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    # the kernel reads q with q's strides and writes dq with the same strides; k/v/dk/dv likewise share theirs
+    if q.stride() != dq.stride():
+        q = q[:, :, :N].contiguous()
+    if k.stride() != dk.stride():
+        k, v = k[:, :, :N].contiguous(), v[:, :, :N].contiguous()
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_bwd_varlen(_p(q), _p(k), _p(v), _p(out), _p(dout), _p(lse), _p(dq), _p(dk), _p(dv),
+                                              _p(cu_seqlens), n_seg, H, N, q.stride(1), k.stride(1), scale, _p(ws), ws_bytes,
+                                              _stream(q)), "attention_bwd_varlen")
+    return dq, dk, dv
+
+
 def kv_scatter_tails(k: torch.Tensor, v: torch.Tensor, S_tot: int, tail_k: torch.Tensor, tail_v: torch.Tensor,
                      cu_seqlens: torch.Tensor, group_size: int):
     """Copy packed suffix rows k / v [1,H,>=S_tot,128] (segments as in `attention_prefill_shared_prefix`) into the tails

@@ -366,6 +366,26 @@ int aria_attention_bwd(const void* q, const void* k, const void* v, const void* 
                        void* dq, void* dk, void* dv, const uint8_t* key_mask, int32_t B, int32_t H, int32_t Tq, int32_t Tk,
                        int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
                        int32_t causal, void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* Varlen (packed, padding-free) causal attention over n_seg segments packed along one sequence of N rows: segment s is rows
+ * [cu_seqlens[s], cu_seqlens[s+1]) (DEVICE int32 [n_seg+1], nondecreasing from 0 to N, every segment >= 1 row); the query at
+ * packed row r of segment s sees the packed keys [cu_seqlens[s], r].  q, k, v [1, H, >= N, 128] head-major (head strides
+ * q_stride_h / kv_stride_h, multiples of 8 elements, 128-element rows).  out [N, H*128] bf16; lse [H, N] fp32 natural-log
+ * logsumexp, or NULL.  The shared-prefix prefill's pipeline with no prefix: each segment's out and lse are bit-identical to
+ * aria_attention_fwd_lse (causal) on that segment alone.  No workspace. */
+int aria_attention_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int32_t* cu_seqlens,
+                              int32_t n_seg, int32_t H, int32_t N, int64_t q_stride_h, int64_t kv_stride_h, float scale,
+                              aria_stream_t stream);
+/* Backward of aria_attention_fwd_varlen (same segment convention; lse from it): q, dq at the q head stride, k, v, dk, dv at the
+ * kv head stride, out / dout [N, H*128].  One CTA per (head, 128-key tile aligned at its segment's start), heaviest tiles
+ * first.  Per segment, dk and dv are bit-identical to aria_attention_bwd (causal) on the segment alone and dq equals it up to
+ * the order of fp32 atomic additions; no segment's gradients read another segment's inputs.  Boundaries that break the
+ * convention give wrong gradients but no access outside the tensors and the workspace (they are clamped to [0, N]).
+ * workspace: aria_attention_bwd_varlen_workspace_bytes(...) bytes, 16-byte aligned.  Four kernel launches. */
+int64_t aria_attention_bwd_varlen_workspace_bytes(int32_t n_seg, int32_t H, int32_t N);
+int aria_attention_bwd_varlen(const void* q, const void* k, const void* v, const void* out, const void* dout, const float* lse,
+                              void* dq, void* dk, void* dv, const int32_t* cu_seqlens, int32_t n_seg, int32_t H, int32_t N,
+                              int64_t q_stride_h, int64_t kv_stride_h, float scale, void* workspace, int64_t workspace_bytes,
+                              aria_stream_t stream);
 /* Single-token decode against a KV cache (HBM-bound, split-KV): q element (b,h,:) at q + b*q_stride_b + h*q_stride_h
  * (128 contiguous bf16), cache [B,H,Tk_max,128], out [B, H*128].  workspace: B*H*splits*(128+2) floats.
  * key_mask [B, Tk] uint8 or NULL: 1 = key is masked OUT (padded batch: the HF 2-D attention_mask inverted). */
