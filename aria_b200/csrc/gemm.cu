@@ -307,17 +307,23 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
 // Wide dense GEMM for the 4,900-row ViT and projector launches (gemm_run): bf16, nn.Linear weights, LINEAR or HEADS without
 // RoPE.  128 x 192 tiles (1152 = 6 x 192), each consumer warpgroup one wgmma m64n192k16 per k16 step on its 64 rows.  The
-// epilogue runs on the accumulator registers: each thread rounds and activates its fragment exactly as epilogue_tile /
-// heads_store_tile do and writes it as bf16 into its warpgroup's 64 x 192 half of an output tile in shared memory (three
-// 64 x 64 SW128 boxes, 24 KB).  Without the fp32 staging tile of gemm_kernel the ring keeps four 40 KB stages.
-//   * LINEAR: one thread per warpgroup stores the half with TMA and does not wait for it; it waits for the store to have
-//     read the half during the next tile's first k-block.  With a residual, the producer TMA-loads the tile's residual rows
+// epilogue starts on the accumulator registers: each thread adds the bias to its fragment and rounds it exactly as
+// epilogue_tile / heads_store_tile do and writes it as bf16 into its warpgroup's 64 x 192 half of an output tile in shared
+// memory (three 64 x 64 SW128 boxes, 24 KB).  Without the fp32 staging tile of gemm_kernel the ring keeps four 40 KB stages.
+//   * LINEAR without a residual, and HEADS (hand-off): the consumers write bias + rounding only, arrive on out_full[cw] and
+//     go on to the next tile's k-loop; before writing the next tile's half they wait on out_free[cw].  The producer
+//     warpgroup's idle warps 1-3 (the epilogue warps) walk the same tiles: per half they wait on out_full, apply the
+//     activation in place (LINEAR; it sees bf16(x + bias) either way, so the bits are those of epilogue_tile), then one of
+//     them TMA-stores the half, waits for the store to have read it and arrives on out_free.  HEADS: they read the half back
+//     in 16-byte chunks and scatter them head-major with heads_store_tile's mapping (a 192-wide tile spans 2 2/3 heads of
+//     72, so TMA cannot store it), then arrive on out_free.  The tensor cores no longer idle through those epilogues.
+//   * LINEAR with a residual: one thread per warpgroup stores the half with TMA and does not wait for it; it waits for the
+//     store to have read the half during the next tile's first k-block.  The producer TMA-loads the tile's residual rows
 //     into the half once that wait is over (out_free), on a barrier of its own (res_full), and the consumers add them at
-//     their fragment positions: out = bf16(x + res).
-//   * HEADS: the warpgroup reads its half back in 16-byte chunks and scatters them head-major with heads_store_tile's
-//     mapping; a 192-wide tile spans 2 2/3 heads of 72, so TMA cannot store it.
-// A half with no row of the launch is neither computed nor stored.  PAIR: the A-multicast CTA pairs of gemm_kernel (same
-// protocol, same phantom tile).
+//     their fragment positions: out = bf16(x + res).  These launches' time is their mainloop (DESIGN §6).
+// HANDOFF selects the first protocol, per launch (gemm_run: no residual), so the residual instantiations carry no hand-off
+// code.  A half with no row of the launch is neither computed nor stored.  PAIR: the A-multicast CTA pairs of gemm_kernel
+// (same protocol, same phantom tile).
 constexpr int WIDE_BN = 192;
 constexpr int WIDE_STAGE_BYTES = A_STAGE_BYTES + WIDE_BN * BK * 2;  // 16 + 24 KB
 constexpr int WIDE_BOX_BYTES = 64 * 64 * 2;                         // one 64-row x 64-column bf16 SW128 box of the output
@@ -333,7 +339,33 @@ ARIA_DEVICE uint32_t wide_out_offset(int r, int c) {
   return (c >> 6) * WIDE_BOX_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
 }
 
-template <int EPI, bool PAIR>
+// Hand-off epilogue warps of gemm_wide_kernel: how many, and their named barrier (the consumer warpgroups use 1 and 2)
+constexpr int WIDE_EPI_THREADS = 96;
+constexpr uint32_t WIDE_EPI_BAR = 3;
+
+// The activation of the first n_chunks 16-byte chunks of an output half, in place: bf16(act(x)) of each bf16 x, as
+// epilogue_tile computes it.  Element-wise, so chunks go in address order whatever the swizzle; two per thread and
+// iteration, so each of the few epilogue warps has independent work in flight.
+template <int ACT>
+ARIA_DEVICE void wide_act_inplace(uint32_t half, int n_chunks, int et) {
+  auto act8 = [](uint4& v) {
+    uint32_t* w = reinterpret_cast<uint32_t*>(&v);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) w[e] = pack_bf16(bf16r(act_apply(bf16_lo(w[e]), ACT)), bf16r(act_apply(bf16_hi(w[e]), ACT)));
+  };
+#pragma unroll 1
+  for (int i = et; i < n_chunks; i += 2 * WIDE_EPI_THREADS) {
+    const uint32_t a0 = half + 16 * i, a1 = a0 + 16 * WIDE_EPI_THREADS;
+    const bool two = i + WIDE_EPI_THREADS < n_chunks;
+    uint4 v0 = ld_shared_v4(a0), v1 = two ? ld_shared_v4(a1) : make_uint4(0, 0, 0, 0);
+    act8(v0);
+    act8(v1);
+    st_shared_v4(a0, v0);
+    if (two) st_shared_v4(a1, v1);
+  }
+}
+
+template <int EPI, bool PAIR, bool HANDOFF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
                  const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2,
@@ -341,17 +373,20 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int BN = WIDE_BN;
   constexpr int STAGES = GEMM_STAGES;
   static_assert(EPI == ARIA_EPI_LINEAR || EPI == ARIA_EPI_HEADS, "wide GEMM epilogues");
+  static_assert(HANDOFF || EPI == ARIA_EPI_LINEAR, "HEADS launches hand off");
 
   uint8_t* smem = smem_1024();
   uint8_t* out_tile = smem + STAGES * WIDE_STAGE_BYTES;  // [2 warpgroups][3 boxes][64 rows][128 B]
   const BarrierRing<STAGES> bar(out_tile + 2 * WIDE_HALF_BYTES);
   uint64_t* res_full = bar.empty + STAGES;  // [2]: the residual rows of a warpgroup's half have landed in it
-  uint64_t* out_free = res_full + 2;        // [2]: a warpgroup's previous TMA store has read its half
+  uint64_t* out_free = res_full + 2;        // [2]: a warpgroup's previous tile has left its half (stored or scattered)
+  uint64_t* out_full = out_free + 2;        // [2]: hand-off: a warpgroup has written its tile into its half
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int wg = threadIdx.x >> 7;
-  const bool res = EPI == ARIA_EPI_LINEAR && p.residual != nullptr;
+  constexpr bool handoff = HANDOFF;
+  constexpr bool res = !HANDOFF;  // LINEAR with a residual
 
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmA);
@@ -364,6 +399,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int h = 0; h < 2; ++h) {
       mbar_init(&res_full[h], 1);
       mbar_init(&out_free[h], 1);
+      mbar_init(&out_full[h], 128);  // every consumer thread of the warpgroup
     }
     fence_mbar_init();
   }
@@ -433,6 +469,67 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           }
         }
       }
+    } else if (warp > 0 && handoff) {
+      // ================ epilogue warps (1-3): activation and store of each half the consumers hand off ================
+      const int et = threadIdx.x - 32;
+      const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+      TileSched sched;
+      sched.init(p, pair_sched_n<PAIR>(n_tiles));
+      uint32_t full_phase = 0;  // bit h: the phase of out_full[h] to wait for
+      for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
+        int grp, m_idx, n_idx, row0, rows;
+        if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+        if constexpr (PAIR) n_idx = 2 * n_idx + rank;
+        if (PAIR && n_idx >= n_tiles) continue;  // phantom tile
+        const int col0 = n_idx * BN;
+        const int seg = col0 / p.N;
+        const int cseg0 = col0 - seg * p.N;
+        for (int h = 0; h < 2; ++h) {
+          if (m_idx * BM + 64 * h >= rows) continue;  // the consumers sit this half out
+          mbar_wait(&out_full[h], (full_phase >> h) & 1);
+          full_phase ^= 1u << h;
+          const uint32_t half = smem_u32(out_tile) + h * WIDE_HALF_BYTES;
+          if constexpr (EPI == ARIA_EPI_LINEAR) {
+            const int nbox = tile_boxes(col0);
+            if (p.act == ARIA_ACT_GELU_TANH || p.act == ARIA_ACT_GELU_NEW) {
+              const int n_chunks = nbox * (WIDE_BOX_BYTES / 16);
+              if (p.act == ARIA_ACT_GELU_TANH) wide_act_inplace<ARIA_ACT_GELU_TANH>(half, n_chunks, et);
+              else wide_act_inplace<ARIA_ACT_GELU_NEW>(half, n_chunks, et);
+              fence_proxy_async_smem();
+            }
+            named_bar_sync(WIDE_EPI_BAR, WIDE_EPI_THREADS);
+            if (et == 0) {
+              fence_proxy_async_smem();
+              for (int c = 0; c < nbox; ++c)
+                tma_store_2d_addr(&tmOut, half + c * WIDE_BOX_BYTES, col0 + 64 * c, m_idx * BM + 64 * h);
+              bulk_commit_group();
+              bulk_wait_group_read<0>();
+              mbar_arrive(&out_free[h]);
+            }
+          } else {
+            // heads_store_tile's mapping, consecutive threads on consecutive 8-column chunks of a row.  96 threads are 4 rows
+            // of 24 chunks, so a thread keeps its column chunk (head, d) and steps 4 rows at a time.
+            constexpr int CH = BN / 8;
+            constexpr int ROW_STEP = WIDE_EPI_THREADS / CH;
+            static_assert(WIDE_EPI_THREADS % CH == 0, "a thread keeps its column chunk");
+            const int c = (et % CH) * 8, cs = cseg0 + c;
+            if (cs + 8 <= p.N) {
+              const int head = cs / p.head_dim, d = cs - head * p.head_dim;
+              __nv_bfloat16* col_base = p.out[seg] + head * p.stride_h + d;
+              int r = et / CH, r_in_grp = m_idx * BM + 64 * h + r;
+              int b = r_in_grp / p.rows_per_batch, tok = r_in_grp - b * p.rows_per_batch;
+#pragma unroll 1
+              for (; r < 64 && r_in_grp < rows; r += ROW_STEP, r_in_grp += ROW_STEP) {
+                st_global_v4(col_base + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld,
+                             ld_shared_v4(half + wide_out_offset(r, c)));
+                for (tok += ROW_STEP; tok >= p.rows_per_batch; tok -= p.rows_per_batch) ++b;
+              }
+            }
+            named_bar_sync(WIDE_EPI_BAR, WIDE_EPI_THREADS);  // every chunk of the half has been read
+            if (et == 0) mbar_arrive(&out_free[h]);
+          }
+        }
+      }
     }
   } else {
     // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
@@ -444,11 +541,12 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int fr = ct.frag_row - 64 * cw;  // fragment rows fr and fr + 8 of the warpgroup's half
     const bool leader = (threadIdx.x & 127) == 0;
     uint8_t* half = out_tile + cw * WIDE_HALF_BYTES;
+    const uint32_t half_s = smem_u32(half);
     const uint32_t rank = PAIR ? cluster_ctarank() : 0;
     TileSched sched;
     sched.init(p, pair_sched_n<PAIR>(n_tiles));
     RingPos<STAGES> rp;
-    uint32_t res_phase = 0;
+    uint32_t res_phase = 0, free_phase = 0;
     auto release = [&](int s) {
       if (lane == 0) {
         mbar_arrive(&bar.empty[s]);
@@ -494,10 +592,10 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k) wgmma_m64n192_ss<0, 0>(acc, da + k * 2, db + k * 2, 1u);
         wgmma_commit();
-        if (kb == 0 && leader) {
-          // the previous tile's store has read this half; with a residual the producer may now load this tile's
+        if (res && kb == 0 && leader) {
+          // the previous tile's store has read this half; the producer may now load this tile's residual
           bulk_wait_group_read<0>();
-          if (res) mbar_arrive(&out_free[cw]);
+          mbar_arrive(&out_free[cw]);
         }
         wgmma_wait<1>();
         if (prev >= 0) release(prev);
@@ -507,42 +605,57 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       fence_regs(acc);
       if (prev >= 0) release(prev);
-      if (res) {
+      if (handoff) {
+        // the epilogue warps have stored or scattered this warpgroup's previous tile and left its half
+        mbar_wait(&out_free[cw], free_phase ^ 1);
+        free_phase ^= 1;
+        // bias and rounding only, in a loop of its own: the residual loop below, with its per-element branches on the
+        // activation, unrolls to ~9k instructions, and fc1 measured 113-115 us through it, 89-94 us with this loop (DESIGN §6)
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
+            float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
+            if (bias) {
+              x0 += bf16_lo(bias2[j]);
+              x1 += bf16_hi(bias2[j]);
+            }
+            st_shared_u32(half_s + wide_out_offset(fr + 8 * i, 8 * j + ct.frag_col), pack_bf16(x0, x1));
+          }
+        }
+        if constexpr (EPI == ARIA_EPI_LINEAR) fence_proxy_async_smem();  // the epilogue warps' TMA store reads the half
+        mbar_arrive(&out_full[cw]);
+        continue;
+      }
+      if constexpr (EPI == ARIA_EPI_LINEAR) {  // with a residual
         mbar_wait(&res_full[cw], res_phase);
         res_phase ^= 1;
-      }
-      // the leader has seen the previous store read the half (LINEAR), every thread has read its last chunks back (HEADS)
-      named_bar_sync(1 + cw, 128);
+        named_bar_sync(1 + cw, 128);  // the leader has seen the previous store read the half
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int c = 8 * j + ct.frag_col;
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + ct.frag_col;
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
-          uint32_t* dst = reinterpret_cast<uint32_t*>(half + wide_out_offset(fr + 8 * i, c));
-          float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
-          if (bias) {
-            x0 += bf16_lo(bias2[j]);
-            x1 += bf16_hi(bias2[j]);
-          }
-          if constexpr (EPI == ARIA_EPI_LINEAR) {
+          for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
+            uint32_t* dst = reinterpret_cast<uint32_t*>(half + wide_out_offset(fr + 8 * i, c));
+            float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
+            if (bias) {
+              x0 += bf16_lo(bias2[j]);
+              x1 += bf16_hi(bias2[j]);
+            }
             x0 = bf16r(x0);
             x1 = bf16r(x1);
             if (p.act != ARIA_ACT_NONE) {
               x0 = bf16r(act_apply(x0, p.act));
               x1 = bf16r(act_apply(x1, p.act));
             }
-            if (res) {
-              const uint32_t r = *dst;
-              x0 += bf16_lo(r);
-              x1 += bf16_hi(r);
-            }
+            const uint32_t r = *dst;
+            x0 += bf16_lo(r);
+            x1 += bf16_hi(r);
+            *dst = pack_bf16(x0, x1);
           }
-          *dst = pack_bf16(x0, x1);
+          // one 64-column box at a time: hoisting all 48 residual loads ahead of the arithmetic spilled registers
+          if (j % 8 == 7) asm volatile("" ::: "memory");
         }
-        // one 64-column box at a time: hoisting all 48 residual loads ahead of the arithmetic spilled registers
-        if (j % 8 == 7) asm volatile("" ::: "memory");
-      }
-      if constexpr (EPI == ARIA_EPI_LINEAR) {
         fence_proxy_async_smem();
         named_bar_sync(1 + cw, 128);
         if (leader) {
@@ -550,22 +663,6 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int c = 0; c < nbox; ++c)
             tma_store_2d_addr(&tmOut, smem_u32(half + c * WIDE_BOX_BYTES), col0 + 64 * c, m_idx * BM + 64 * cw);
           bulk_commit_group();
-        }
-      } else {
-        named_bar_sync(1 + cw, 128);
-        // heads_store_tile's mapping: consecutive threads on consecutive 8-column chunks of a row
-        constexpr int CH = BN / 8;
-#pragma unroll 1
-        for (int i = threadIdx.x & 127; i < 64 * CH; i += 128) {
-          const int r = i / CH, c = (i % CH) * 8;
-          const int r_in_grp = m_idx * BM + 64 * cw + r;
-          const int cs = cseg0 + c;
-          if (r_in_grp >= rows || cs + 8 > p.N) continue;
-          const uint4 v = *reinterpret_cast<const uint4*>(half + wide_out_offset(r, c));
-          const int b = r_in_grp / p.rows_per_batch, tok = r_in_grp - b * p.rows_per_batch;
-          const int head = cs / p.head_dim, d = cs - head * p.head_dim;
-          *reinterpret_cast<uint4*>(p.out[seg] + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld +
-                                    head * p.stride_h + d) = v;
         }
       }
     }
@@ -885,9 +982,10 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   // Dense bf16 GEMMs with nn.Linear weights and at least PAIR_MIN_ROWS rows, LINEAR or HEADS without RoPE (the ViT's four
   // GEMMs, the projector's 4,900-row k / v and in-projections) run on gemm_wide_kernel; tiles must not straddle two weights.
   // Measured on an H100 SXM at 700 W (DESIGN §6), µs before -> after: q/k/v heads 102.5 -> 83-85, o_proj 44.2 -> 34-36,
-  // fc1 149-152 -> 127, fc2 122.5 -> 95-96.  Only fc2, whose 68 k-blocks make the mainloop the cost, gains from CTA pairs
-  // (95 against 105 µs); o_proj, fc1 and the projector's k / v lose 10-25 % as pairs and q/k/v gains nothing, so pairs are
-  // selected for LINEAR at K >= WIDE_PAIR_MIN_K only.  Other dense LINEAR launches of PAIR_MIN_ROWS rows and more (several
+  // fc1 149-152 -> 127, fc2 122.5 -> 95-96; then with the hand-off epilogue q/k/v 83-85 -> 73-76 and fc1 124-125 -> 84-89.
+  // Only fc2, whose 68 k-blocks make the mainloop the cost, gains from CTA pairs (95 against 105 µs); before the hand-off
+  // o_proj, fc1 and the projector's k / v lost 10-25 % as pairs and q/k/v gained nothing, so pairs are selected for LINEAR
+  // at K >= WIDE_PAIR_MIN_K only.  Other dense LINEAR launches of PAIR_MIN_ROWS rows and more (several
   // weights whose N is no multiple of 192) keep the 128-wide CTA pairs of gemm_kernel; the 768-row LM GEMMs lose 5-16 % as
   // pairs and keep the one-CTA kernel.
   const bool dense = !b_scale && d->b_layout == ARIA_B_NK && d->num_groups == 1 && !d->group_offsets;
@@ -945,15 +1043,22 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
       }
     }
     const int64_t m_tiles = (d->m + BM - 1) / BM, n_tiles = (n_out + WIDE_BN - 1) / WIDE_BN;
-    if (wide_pair)
-      return launch_persistent_pairs<gemm_wide_kernel<ARIA_EPI_LINEAR, true>>("gemm_wide_kernel", GEMM_THREADS,
-                                                                              gemm_wide_smem_bytes(), (n_tiles + 1) / 2 * m_tiles,
-                                                                              stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p);
-#define ARIA_LAUNCH_WIDE(EPI_)                                                                                                \
-  return launch_persistent<gemm_wide_kernel<EPI_, false>>("gemm_wide_kernel", GEMM_THREADS, gemm_wide_smem_bytes(),         \
-                                                          n_tiles * m_tiles, stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p)
-    if (d->epilogue == ARIA_EPI_HEADS) ARIA_LAUNCH_WIDE(ARIA_EPI_HEADS);
-    ARIA_LAUNCH_WIDE(ARIA_EPI_LINEAR);
+    // the hand-off epilogue (gemm_wide_kernel's HANDOFF) for every launch without a residual
+    if (wide_pair) {
+      const int64_t pairs = (n_tiles + 1) / 2 * m_tiles;
+      if (d->residual)
+        return launch_persistent_pairs<gemm_wide_kernel<ARIA_EPI_LINEAR, true, false>>(
+            "gemm_wide_kernel", GEMM_THREADS, gemm_wide_smem_bytes(), pairs, stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p);
+      return launch_persistent_pairs<gemm_wide_kernel<ARIA_EPI_LINEAR, true, true>>(
+          "gemm_wide_kernel", GEMM_THREADS, gemm_wide_smem_bytes(), pairs, stream, tmA, tmB[0], tmB[1], tmB[2], tmOut, tmRes, p);
+    }
+#define ARIA_LAUNCH_WIDE(EPI_, HANDOFF_)                                                                                      \
+  return launch_persistent<gemm_wide_kernel<EPI_, false, HANDOFF_>>("gemm_wide_kernel", GEMM_THREADS, gemm_wide_smem_bytes(), \
+                                                                    n_tiles * m_tiles, stream, tmA, tmB[0], tmB[1], tmB[2],   \
+                                                                    tmOut, tmRes, p)
+    if (d->epilogue == ARIA_EPI_HEADS) ARIA_LAUNCH_WIDE(ARIA_EPI_HEADS, true);
+    if (d->residual) ARIA_LAUNCH_WIDE(ARIA_EPI_LINEAR, false);
+    ARIA_LAUNCH_WIDE(ARIA_EPI_LINEAR, true);
 #undef ARIA_LAUNCH_WIDE
   }
   const int64_t tiles = max_tiles(d, BN, d->num_groups > 1 ? d->num_groups : 0);

@@ -11,6 +11,21 @@ namespace aria {
 #define ARIA_DEVICE __device__ __forceinline__
 
 ARIA_DEVICE uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
+// Shared-memory accesses by shared address.  Through a pointer derived from the aligned dynamic shared-memory base the
+// compiler cannot prove the address space and emits generic LD / ST, which cost the latency-bound epilogue loops.
+ARIA_DEVICE void st_shared_u32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+ARIA_DEVICE void st_shared_v4(uint32_t addr, uint4 v) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+// 16-byte global store (the compiler split a plain uint4 store of ld_shared_v4's result into four 4-byte ones)
+ARIA_DEVICE void st_global_v4(void* p, uint4 v) {
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+}
+ARIA_DEVICE uint4 ld_shared_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
 
 ARIA_DEVICE uint32_t elect_one() {
   uint32_t pred = 0;
