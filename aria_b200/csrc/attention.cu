@@ -22,6 +22,7 @@
 //
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
+// aria_attention_decode_paged: the devlen kernels over a paged KV cache (page pools and a block table, continuous batching).
 // aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
 // aria_attention_decode_shared_prefix: n rows per prompt decode against one shared prompt cache plus their own tail caches.
 // aria_attention_decode_multi: Q consecutive queries per row against its cache (prompt-lookup verification), each query
@@ -513,22 +514,40 @@ attn_prefill_shared_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const
 // sc_stride_b / sc_stride_h).  A lane widens its 4 codes per key exactly; the key scale multiplies the reduced dot product and
 // the value weight is pw * v_scale.  Split size, warp -> key assignment and update order are the bf16 kernel's, so with
 // power-of-two scales (both products exact) the result is bit-identical to the bf16 kernel run on the tensors code * scale.
+// PAGED (with DEVLEN, bf16): kc / vc are page pools [n_pages, H, DEC_SPLIT_KEYS, 128] (kv_stride_b is the page stride) and
+// split s of row b reads page block_table[b * bt_stride + s], which holds the row's keys [256 s, 256 s + 256).  A page is one
+// split, so every key is read by the warp, and updated in the order, of the contiguous kernel: row b is bit-identical to
+// the DEVLEN kernel on a cache that holds the same keys.  A live split whose entry is not a page of the pool reads no key.
 constexpr int DEC_SPLIT_KEYS = 256;
 
-template <bool DEVLEN, bool KV_FP8, typename KV = std::conditional_t<KV_FP8, uint8_t, __nv_bfloat16>>
+template <bool DEVLEN, bool KV_FP8, bool PAGED = false, typename KV = std::conditional_t<KV_FP8, uint8_t, __nv_bfloat16>>
 __device__ __forceinline__ void decode_partial(const __nv_bfloat16* __restrict__ q, const KV* __restrict__ kc,
                                                const KV* __restrict__ vc, const float* __restrict__ k_scale,
                                                const float* __restrict__ v_scale, const uint8_t* __restrict__ key_mask,
                                                float* __restrict__ ws, int H, int Tk, int64_t q_stride_b, int64_t q_stride_h,
                                                int64_t kv_stride_b, int64_t kv_stride_h, int64_t sc_stride_b, int64_t sc_stride_h,
-                                               float scale_log2, int splits, const int32_t* __restrict__ lens, int mask_stride) {
+                                               float scale_log2, int splits, const int32_t* __restrict__ lens, int mask_stride,
+                                               const int32_t* __restrict__ block_table = nullptr, int64_t bt_stride = 0,
+                                               int n_pages = 0) {
   const int bh = blockIdx.x, split = blockIdx.y;
   const int b = bh / H, h = bh % H;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int len = DEVLEN ? min(lens[b], Tk) : Tk;
-  const int k_begin = split * DEC_SPLIT_KEYS, k_end = min(len, k_begin + DEC_SPLIT_KEYS);
-  const KV* kbase = kc + b * kv_stride_b + h * kv_stride_h;
-  const KV* vbase = vc + b * kv_stride_b + h * kv_stride_h;
+  const int k_begin = split * DEC_SPLIT_KEYS;
+  int k_end = min(len, k_begin + DEC_SPLIT_KEYS);
+  const KV* kbase;
+  const KV* vbase;
+  if constexpr (PAGED) {
+    const int page = k_begin < k_end ? block_table[b * bt_stride + split] : 0;
+    if (page < 0 || page >= n_pages) k_end = k_begin;
+    // key kk of the split is row kk - k_begin of its page
+    const int64_t off = static_cast<int64_t>(page) * kv_stride_b + h * kv_stride_h - static_cast<int64_t>(k_begin) * AT_D;
+    kbase = kc + off;
+    vbase = vc + off;
+  } else {
+    kbase = kc + b * kv_stride_b + h * kv_stride_h;
+    vbase = vc + b * kv_stride_b + h * kv_stride_h;
+  }
   const uint8_t* km = key_mask ? key_mask + static_cast<int64_t>(b) * (DEVLEN ? mask_stride : Tk) : nullptr;
   const uint2 qv = *reinterpret_cast<const uint2*>(q + b * q_stride_b + h * q_stride_h + lane * 4);
   const float q0 = bf16_lo(qv.x) * scale_log2, q1 = bf16_hi(qv.x) * scale_log2, q2 = bf16_lo(qv.y) * scale_log2,
@@ -690,6 +709,18 @@ __global__ void __launch_bounds__(128) attn_decode_partial_fp8(const __nv_bfloat
                                                                const int32_t* __restrict__ lens, int mask_stride) {
   decode_partial<DEVLEN, true>(q, kc, vc, k_scale, v_scale, key_mask, ws, H, Tk, q_stride_b, q_stride_h, kv_stride_b, kv_stride_h,
                                sc_stride_b, sc_stride_h, scale_log2, splits, lens, mask_stride);
+}
+
+__global__ void __launch_bounds__(128) attn_decode_partial_paged(const __nv_bfloat16* __restrict__ q,
+                                                                 const __nv_bfloat16* __restrict__ k_pool,
+                                                                 const __nv_bfloat16* __restrict__ v_pool, float* __restrict__ ws,
+                                                                 int H, int Tk, int64_t q_stride_b, int64_t q_stride_h,
+                                                                 int64_t page_stride, int64_t pool_stride_h, float scale_log2,
+                                                                 int splits, const int32_t* __restrict__ lens,
+                                                                 const int32_t* __restrict__ block_table, int64_t bt_stride,
+                                                                 int n_pages) {
+  decode_partial<true, false, true>(q, k_pool, v_pool, nullptr, nullptr, nullptr, ws, H, Tk, q_stride_b, q_stride_h, page_stride,
+                                    pool_stride_h, 0, 0, scale_log2, splits, lens, 0, block_table, bt_stride, n_pages);
 }
 
 template <bool DEVLEN>
@@ -1192,6 +1223,29 @@ extern "C" int aria_attention_decode_devlen(const void* q, const void* k, const 
   if (rc) return rc;
   attn_decode_merge<true><<<B * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out), splits,
                                                      lens, H);
+  return check_launch("attn_decode_merge");
+}
+
+extern "C" int aria_attention_decode_paged(const void* q, const void* k_pool, const void* v_pool, const int32_t* block_table,
+                                           int64_t block_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* lens,
+                                           void* out, int32_t R, int32_t H, int64_t q_stride_b, int64_t q_stride_h,
+                                           int64_t page_stride, int64_t pool_stride_h, float scale, void* workspace,
+                                           int64_t workspace_bytes, aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && k_pool && v_pool && block_table && lens && out && workspace && R > 0 && H > 0 && n_pages > 0);
+  ARIA_CHECK_ARG(max_pages > 0 && max_pages <= 65535 && block_table_stride >= max_pages);  // splits are grid.y
+  ARIA_CHECK_ARG(q_stride_b % 4 == 0 && q_stride_h % 4 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  ARIA_CHECK_ARG(pool_stride_h >= DEC_SPLIT_KEYS * AT_D && page_stride >= pool_stride_h * H);  // pages do not overlap
+  const int T_max = max_pages * DEC_SPLIT_KEYS;
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(R, H, T_max));
+  attn_decode_partial_paged<<<dim3(R * H, max_pages), 128, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k_pool), static_cast<const __nv_bfloat16*>(v_pool),
+      static_cast<float*>(workspace), H, T_max, q_stride_b, q_stride_h, page_stride, pool_stride_h, scale * 1.4426950408889634f,
+      max_pages, lens, block_table, block_table_stride, n_pages);
+  int rc = check_launch("attn_decode_partial_paged");
+  if (rc) return rc;
+  attn_decode_merge<true><<<R * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out),
+                                                     max_pages, lens, H);
   return check_launch("attn_decode_merge");
 }
 

@@ -7,6 +7,12 @@
 // aria_decode_advance: after the sampler, feeds next_ids back as the next step's input, records the token, applies
 //   Hugging Face's EOS rule and advances the RoPE positions, the cache rows, the step index and the RNG offset.
 //
+// Continuous batching (serving.Engine) over a paged KV cache, pools [n_pages, H, 256, 128] and a block table [R, max_pages]:
+// aria_kv_append_paged: kv_append into the page block_table[r, write_pos[r] / 256], row write_pos[r] % 256.  A negative
+//   write_pos, or one outside the row's mapped pages, writes nothing: idle and finished slots never touch another's pages.
+// aria_kv_pages_store: copies rows [0, T) of a one-row prefill cache into a request's pages.
+// aria_decode_advance_slots: aria_decode_advance per slot: own output count, budget, RNG offset and finished flag.
+//
 // Prompt-lookup decoding (generate(prompt_lookup_num_tokens=K)): a step verifies Q = K + 1 tokens per row.
 // aria_kv_append_rows: kv_append for the Q rows of each row, at cache rows pos[b] + i.
 // aria_ngram_draft: Hugging Face's PromptLookupCandidateGenerator.get_candidates on each row's history, one CTA per row.
@@ -115,6 +121,88 @@ __global__ void __launch_bounds__(ADV_MAX_B) decode_advance_kernel(const Advance
     *p.rng_offset += 1;
     if (all && p.n_eos > 0 && *p.done_step < 0) *p.done_step = t;
   }
+}
+
+constexpr int PAGE_ROWS = 256;  // rows per KV page: the decode kernels' split size
+
+// The page holding row p of a slot whose table row is bt[0, max_pages), or -1 when p is not in a mapped page of the pool
+__device__ __forceinline__ int page_of(const int32_t* bt, int max_pages, int n_pages, int p) {
+  if (p < 0 || p / PAGE_ROWS >= max_pages) return -1;
+  const int page = bt[p / PAGE_ROWS];
+  return page < n_pages ? page : -1;
+}
+
+// One CTA per (slot r, head h)
+__global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_append_paged_kernel(const __nv_bfloat16* __restrict__ k_new,
+                                                                          const __nv_bfloat16* __restrict__ v_new, int64_t new_sb,
+                                                                          int64_t new_sh, __nv_bfloat16* __restrict__ kp,
+                                                                          __nv_bfloat16* __restrict__ vp, int64_t page_stride,
+                                                                          int64_t pool_sh, const int32_t* __restrict__ bt,
+                                                                          int64_t bt_stride, int max_pages, int n_pages,
+                                                                          const int32_t* __restrict__ pos, int H) {
+  const int r = blockIdx.x / H, h = blockIdx.x % H;
+  const int p = pos[r];
+  const int page = page_of(bt + r * bt_stride, max_pages, n_pages, p);
+  if (page < 0) return;
+  const bool is_v = threadIdx.x >= KV_ROW_VECS;
+  const int j = threadIdx.x % KV_ROW_VECS;
+  const __nv_bfloat16* src = (is_v ? v_new : k_new) + r * new_sb + h * new_sh;
+  __nv_bfloat16* dst = (is_v ? vp : kp) + page * page_stride + h * pool_sh + static_cast<int64_t>(p % PAGE_ROWS) * 128;
+  reinterpret_cast<uint4*>(dst)[j] = reinterpret_cast<const uint4*>(src)[j];
+}
+
+// One CTA per (row t, head h) of the prefill cache
+__global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_pages_store_kernel(const __nv_bfloat16* __restrict__ k,
+                                                                         const __nv_bfloat16* __restrict__ v, int64_t src_sh,
+                                                                         __nv_bfloat16* __restrict__ kp, __nv_bfloat16* __restrict__ vp,
+                                                                         int64_t page_stride, int64_t pool_sh,
+                                                                         const int32_t* __restrict__ pages, int max_pages,
+                                                                         int n_pages, int H) {
+  const int t = blockIdx.x / H, h = blockIdx.x % H;
+  const int page = page_of(pages, max_pages, n_pages, t);
+  if (page < 0) return;
+  const bool is_v = threadIdx.x >= KV_ROW_VECS;
+  const int j = threadIdx.x % KV_ROW_VECS;
+  const uint4 x = reinterpret_cast<const uint4*>((is_v ? v : k) + h * src_sh + static_cast<int64_t>(t) * 128)[j];
+  __nv_bfloat16* dst = (is_v ? vp : kp) + page * page_stride + h * pool_sh + static_cast<int64_t>(t % PAGE_ROWS) * 128;
+  reinterpret_cast<uint4*>(dst)[j] = x;
+}
+
+struct SlotAdvanceParams {
+  const int64_t* next_ids;
+  int64_t* ids_in;
+  int32_t* out_tokens;  // [R, out_stride]
+  int64_t out_stride;
+  int32_t* n_out;
+  const int32_t* max_new;
+  int32_t* rope_pos;
+  int32_t* write_pos;
+  int32_t* kv_len;
+  uint64_t* rng_offset;
+  uint8_t* finished;
+  int64_t eos[ADV_MAX_EOS];
+  int32_t n_eos;
+  int64_t pad;
+  int32_t R;
+};
+
+// Slot r emits its token n_out[r] (the one sampled at offset rng_offset[r] = n_out[r]) and finishes on an EOS id or when its
+// budget is spent; a finished slot keeps every value, and is fed pad, until the host retires it.
+__global__ void __launch_bounds__(ADV_MAX_B) decode_advance_slots_kernel(const SlotAdvanceParams p) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.R || p.finished[r]) return;
+  const int64_t tok = p.next_ids[r];
+  const int t = p.n_out[r];
+  if (t < p.out_stride) p.out_tokens[r * p.out_stride + t] = static_cast<int32_t>(tok);
+  bool fin = t + 1 >= p.max_new[r];
+  for (int e = 0; e < p.n_eos; ++e) fin |= tok == p.eos[e];
+  p.ids_in[r] = fin ? p.pad : tok;
+  p.n_out[r] = t + 1;
+  p.finished[r] = fin;
+  ++p.rope_pos[r];
+  ++p.write_pos[r];
+  ++p.kv_len[r];
+  ++p.rng_offset[r];
 }
 
 constexpr int LK_MAX_K = 15;  // drafts per row
@@ -328,6 +416,63 @@ extern "C" int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int
   const int threads = (B + 31) / 32 * 32;
   decode_advance_kernel<<<1, threads, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
   return check_launch("decode_advance_kernel");
+}
+
+extern "C" int aria_kv_append_paged(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_pool,
+                                    void* v_pool, int64_t page_stride, int64_t pool_stride_h, const int32_t* block_table,
+                                    int64_t block_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* write_pos,
+                                    int32_t R, int32_t H, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k_new && v_new && k_pool && v_pool && block_table && write_pos);
+  ARIA_CHECK_ARG(R > 0 && H > 0 && max_pages > 0 && n_pages > 0 && block_table_stride >= max_pages);
+  ARIA_CHECK_ARG(static_cast<int64_t>(R) * H < (1ll << 31) && static_cast<int64_t>(R) * block_table_stride < (1ll << 31));
+  ARIA_CHECK_ARG(pool_stride_h >= PAGE_ROWS * 128 && page_stride >= pool_stride_h * H);
+  ARIA_CHECK_ARG(new_stride_b % 8 == 0 && new_stride_h % 8 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  kv_append_paged_kernel<<<R * H, 2 * KV_ROW_VECS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __nv_bfloat16*>(k_new), static_cast<const __nv_bfloat16*>(v_new), new_stride_b, new_stride_h,
+      static_cast<__nv_bfloat16*>(k_pool), static_cast<__nv_bfloat16*>(v_pool), page_stride, pool_stride_h, block_table,
+      block_table_stride, max_pages, n_pages, write_pos, H);
+  return check_launch("kv_append_paged_kernel");
+}
+
+extern "C" int aria_kv_pages_store(const void* k, const void* v, int64_t src_stride_h, int32_t T, void* k_pool, void* v_pool,
+                                   int64_t page_stride, int64_t pool_stride_h, const int32_t* pages, int32_t max_pages,
+                                   int32_t n_pages, int32_t H, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k && v && k_pool && v_pool && pages);
+  ARIA_CHECK_ARG(T > 0 && H > 0 && n_pages > 0 && max_pages > 0 && T <= static_cast<int64_t>(max_pages) * PAGE_ROWS);
+  ARIA_CHECK_ARG(static_cast<int64_t>(T) * H < (1ll << 31) && src_stride_h >= static_cast<int64_t>(T) * 128);
+  ARIA_CHECK_ARG(pool_stride_h >= PAGE_ROWS * 128 && page_stride >= pool_stride_h * H);
+  ARIA_CHECK_ARG(src_stride_h % 8 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  kv_pages_store_kernel<<<T * H, 2 * KV_ROW_VECS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), src_stride_h, static_cast<__nv_bfloat16*>(k_pool),
+      static_cast<__nv_bfloat16*>(v_pool), page_stride, pool_stride_h, pages, max_pages, n_pages, H);
+  return check_launch("kv_pages_store_kernel");
+}
+
+extern "C" int aria_decode_advance_slots(const int64_t* next_ids, int64_t* ids_in, int32_t* out_tokens, int64_t out_stride,
+                                         int32_t* n_out, const int32_t* max_new, int32_t* rope_pos, int32_t* write_pos,
+                                         int32_t* kv_len, uint64_t* rng_offset, uint8_t* finished, const int64_t* eos_ids,
+                                         int32_t n_eos, int64_t pad_token_id, int32_t R, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(next_ids && ids_in && out_tokens && n_out && max_new && rope_pos && write_pos && kv_len && rng_offset && finished);
+  ARIA_CHECK_ARG(R > 0 && R <= ADV_MAX_B && out_stride > 0);
+  ARIA_CHECK_ARG(n_eos >= 0 && n_eos <= ADV_MAX_EOS && (n_eos == 0 || eos_ids));
+  SlotAdvanceParams p{};
+  p.next_ids = next_ids;
+  p.ids_in = ids_in;
+  p.out_tokens = out_tokens;
+  p.out_stride = out_stride;
+  p.n_out = n_out;
+  p.max_new = max_new;
+  p.rope_pos = rope_pos;
+  p.write_pos = write_pos;
+  p.kv_len = kv_len;
+  p.rng_offset = rng_offset;
+  p.finished = finished;
+  for (int e = 0; e < n_eos; ++e) p.eos[e] = eos_ids[e];  // host array, copied into the launch parameters
+  p.n_eos = n_eos;
+  p.pad = pad_token_id;
+  p.R = R;
+  decode_advance_slots_kernel<<<1, (R + 31) / 32 * 32, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
+  return check_launch("decode_advance_slots_kernel");
 }
 
 extern "C" int aria_kv_append_rows(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h,

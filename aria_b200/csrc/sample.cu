@@ -18,6 +18,8 @@
 //
 // aria_sample_tokens_rows: the same kernel with a noise row and an offset per logits row, so that logits row b * (K + 1) + i
 // of a prompt-lookup verification step draws the noise generation row b draws for its token n_out[b] + i.
+// aria_sample_tokens_slots: aria_sample_tokens_rows with the temperature, top_k, top_p and seed of each row also read from
+// device arrays (continuous batching: every slot samples with its own request's parameters).
 #include <float.h>
 #include <limits.h>
 
@@ -168,12 +170,33 @@ __device__ void find_bin(SampleSmem& sm, int need) {
   __syncthreads();
 }
 
+// Per-row sampling parameters of aria_sample_tokens_slots, device arrays [R]
+struct SlotSampling {
+  const float* temperature;
+  const int32_t* top_k;
+  const float* top_p;
+  const uint64_t* seed;
+};
+
 // ROWS (aria_sample_tokens_rows): logits row `row` draws the noise of row noise_rows[row] at offset offsets[row] instead of
-// (row, *p.rng_offset).  Everything else is the same code.
-template <bool ROWS>
-__device__ __forceinline__ void sample_body(const SampleParams p, const int32_t* __restrict__ noise_rows,
-                                            const uint64_t* __restrict__ offsets) {
+// (row, *p.rng_offset).  SLOTS (with ROWS): the row's temperature, top_k, top_p and seed come from `slots`, brought into the
+// ranges aria_sample_tokens accepts (a caller checks them; this keeps a bad entry from reading past shared memory).
+// Everything else is the same code.
+template <bool ROWS, bool SLOTS = false>
+__device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __restrict__ noise_rows,
+                                            const uint64_t* __restrict__ offsets, const SlotSampling slots = {}) {
   __shared__ SampleSmem sm;
+  if constexpr (SLOTS) {
+    const int r = blockIdx.x;
+    const float t = slots.temperature[r];
+    p.temperature = t > 0.f && t <= FLT_MAX ? t : 0.f;
+    p.top_k = min(max(slots.top_k[r], 0), SP_MAX_K);
+    const float tp = slots.top_p[r];
+    p.top_p = p.top_k > 0 && tp > 0.f && tp < 1.f ? tp : 1.f;
+    const uint64_t seed = slots.seed[r];
+    p.seed_lo = static_cast<uint32_t>(seed);
+    p.seed_hi = static_cast<uint32_t>(seed >> 32);
+  }
   const int tid = threadIdx.x, row = blockIdx.x, V = p.V;
   const uint16_t* x = p.logits + static_cast<int64_t>(row) * p.stride;
   float* probs = p.probs ? p.probs + static_cast<int64_t>(row) * V : nullptr;
@@ -347,6 +370,11 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_rows_kernel(const Sample
   sample_body<true>(p, noise_rows, offsets);
 }
 
+__global__ void __launch_bounds__(SP_THREADS, 1) sample_slots_kernel(const SampleParams p, const int32_t* __restrict__ noise_rows,
+                                                                     const uint64_t* __restrict__ offsets, const SlotSampling slots) {
+  sample_body<true, true>(p, noise_rows, offsets, slots);
+}
+
 }  // namespace aria
 
 using namespace aria;
@@ -393,4 +421,16 @@ extern "C" int aria_sample_tokens_rows(const void* logits, int64_t logits_stride
   if (rc) return rc;
   sample_rows_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p, noise_rows, offsets);
   return check_launch("sample_rows_kernel");
+}
+
+extern "C" int aria_sample_tokens_slots(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V,
+                                        const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seed,
+                                        const int32_t* noise_rows, const uint64_t* offsets, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(noise_rows && offsets && temperature && top_k && top_p && seed);
+  SampleParams p{};
+  const int rc = sample_params(p, logits, logits_stride, next_ids, nullptr, R, V, 0.f, 0, 1.f, 0, nullptr);
+  if (rc) return rc;
+  sample_slots_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p, noise_rows, offsets,
+                                                                                      SlotSampling{temperature, top_k, top_p, seed});
+  return check_launch("sample_slots_kernel");
 }

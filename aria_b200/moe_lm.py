@@ -539,6 +539,65 @@ class LookupDecodeState(DecodeState):
         self.qkv_k = torch.empty(3, B, H, K + 1, 128, dtype=bf16, device=device)
 
 
+class PagedKVCache:
+    """Paged KV cache of continuous batching (serving.Engine): per-layer page pools k[l] / v[l] [n_pages, H, 256, head_dim] bf16
+    and one block table [max_rows, max_pages] int32 shared by the layers, row r listing the pages of the request in slot r
+    (key 256 s + i of the request is row i of page block_table[r, s]; -1 = no page).  A page holds one decode split
+    (PAGE_SIZE = the split-KV kernels' 256 keys), so the paged decode reads exactly the keys, in the order, of the contiguous
+    one.  `width`: the table columns a decode step covers (its grid), set by the owner before a step is captured."""
+
+    PAGE_SIZE = 256
+
+    def __init__(self, n_layers, n_pages, H, hd, max_rows, max_pages, device):
+        self.k = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+        self.v = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+        # page 0 is the null page idle rows attend to (one key): zeros, so their attention output is 0 and not whatever the
+        # allocator left there; no request ever gets it, and the paged append never writes it for an idle row
+        for t in self.k + self.v:
+            t[0].zero_()
+        self.block_table = torch.full((max_rows, max_pages), -1, dtype=torch.int32, device=device)
+        self.n_pages = n_pages
+        self.width = max_pages
+        self.dtype = "bf16"
+
+
+class SlotDecodeState(DecodeState):
+    """DecodeState of continuous batching: one row per engine slot, max_batch rows, and what each slot's request needs on the
+    device: its sampling parameters (temperature, 0 = greedy; top_k; top_p; seed; noise row; RNG offset), its token budget
+    max_new, the count n_out and the tokens out_tokens [max_batch, max_out] (int32) it has emitted, its finished flag, and the
+    step's input ids_in and sampled next_ids.  A decode step over the first n slots reads rows(n); the other slots are idle."""
+
+    def __init__(self, max_batch, H, max_out, device):
+        super().__init__(max_batch, H, 0, device)
+        self.key_mask = None
+        i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
+        self.temperature = torch.zeros(max_batch, dtype=torch.float32, device=device)
+        self.top_k = torch.zeros(max_batch, **i32)
+        self.top_p = torch.ones(max_batch, dtype=torch.float32, device=device)
+        self.seed = torch.zeros(max_batch, **i64)
+        self.noise_row = torch.zeros(max_batch, **i32)
+        self.rng_offset = torch.zeros(max_batch, **i64)
+        self.max_new = torch.ones(max_batch, **i32)
+        self.n_out = torch.zeros(max_batch, **i32)
+        self.finished = torch.ones(max_batch, dtype=torch.uint8, device=device)
+        self.ids_in = torch.zeros(max_batch, 1, **i64)
+        self.next_ids = torch.zeros(max_batch, **i64)
+        self.out_tokens = torch.zeros(max_batch, max_out, **i32)
+
+    # the per-slot arrays, in the order a slot's row is copied when slots are compacted
+    SLOT_FIELDS = ("rope_pos", "write_pos", "kv_len", "temperature", "top_k", "top_p", "seed", "noise_row", "rng_offset",
+                   "max_new", "n_out", "finished", "ids_in", "next_ids", "out_tokens")
+
+    def rows(self, n):
+        """A DecodeState view of the first n slots (what decode_step and the sampler of a step over n slots read)."""
+        v = object.__new__(SlotDecodeState)
+        for f in self.SLOT_FIELDS:
+            setattr(v, f, getattr(self, f)[:n])
+        v.qkv = self.qkv[:, :n]
+        v.key_mask = None
+        return v
+
+
 class AriaAttention(nn.Module):
     """What `LLAMA_ATTENTION_CLASSES[config._attn_implementation]` provides at moe_lm.py:594: MHA, no bias,
     rotate-half RoPE, causal, KV cache.  q/k/v projections + RoPE + cache write are ONE GEMM launch."""
@@ -628,6 +687,11 @@ class AriaAttention(nn.Module):
         kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q, k, v = state.qkv[0], state.qkv[1], state.qkv[2]
         self._qkv(hidden_states, hq, [q, k, v], 1, 0, rope, state.rope_pos)
+        if isinstance(cache, PagedKVCache):
+            kp, vp, bt = cache.k[self.layer_idx], cache.v[self.layer_idx], cache.block_table[:, :cache.width]
+            ops.kv_append_paged(k[:, :, 0], v[:, :, 0], kp, vp, bt, state.write_pos)
+            o = ops.attention_decode_paged(q[:, :, 0], kp, vp, bt, state.kv_len, hd ** -0.5).view(B, 1, d)
+            return self._o_proj(o, residual)
         if isinstance(cache, SharedPrefixCache):
             tk, tv = cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx]
             ops.kv_append(k[:, :, 0], v[:, :, 0], tk, tv, state.write_pos)

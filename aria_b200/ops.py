@@ -1361,3 +1361,134 @@ def decode_advance(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: tor
                                              _p(write_pos), _p(kv_len), _p(rng_offset), _p(finished), _p(done_step),
                                              C.cast(arr, C.c_void_p), len(eos), int(pad_token_id), B, _stream(next_ids)),
                 "decode_advance")
+
+
+# ------------------------------------------------------------------------------------------- continuous batching (paged KV cache)
+def _paged_pool_check(k_pool: torch.Tensor, v_pool: torch.Tensor, what: str):
+    """Page pools k_pool / v_pool: CUDA bf16 [n_pages, H, 256, 128], contiguous and sharing one shape."""
+    for t in (k_pool, v_pool):
+        _chk(t)
+        if t.dim() != 4 or t.shape[2:] != (256, 128):
+            raise RuntimeError(f"{what}: page pools must be bf16 [n_pages, H, 256, 128], got {tuple(t.shape)}")
+    if k_pool.shape != v_pool.shape:
+        raise RuntimeError(f"{what}: k_pool and v_pool must share one shape")
+
+
+def _block_table_check(block_table: torch.Tensor, rows: int, what: str):
+    """Block table: CUDA int32 [>= rows, max_pages] with contiguous rows (any row stride)."""
+    if not (block_table.is_cuda and block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
+            and block_table.shape[0] >= rows and block_table.shape[1] >= 1):
+        raise RuntimeError(f"{what}: block_table must be CUDA int32 [>= {rows}, max_pages] with contiguous rows")
+
+
+def attention_decode_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, block_table: torch.Tensor,
+                           lens: torch.Tensor, scale: float) -> torch.Tensor:
+    """attention_decode_devlen over a paged cache: q [R, H, 128] (contiguous last dim), page pools [n_pages, H, 256, 128] bf16,
+    block_table int32 [>= R, max_pages] (row r's key 256 s + i is row i of page block_table[r, s]; its columns are the splits the
+    grid covers), lens int32 [R] -> out [R, H*128].  Row r is bit-identical to attention_decode_devlen on a contiguous cache
+    holding the same keys.  See aria_attention_decode_paged."""
+    _paged_pool_check(k_pool, v_pool, "attention_decode_paged")
+    _chk(lens, torch.int32, align=4)
+    if not (q.is_cuda and q.dtype == bf16 and q.dim() == 3 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
+        raise RuntimeError("attention_decode_paged: q must be a CUDA bf16 [R, H, 128] tensor with a contiguous last dim")
+    R, H = q.shape[0], q.shape[1]
+    _block_table_check(block_table, R, "attention_decode_paged")
+    if q.shape[2] != 128 or k_pool.shape[1] != H or lens.shape != (R,):
+        raise ValueError(f"attention_decode_paged: q {tuple(q.shape)}, pools {tuple(k_pool.shape)} and lens {tuple(lens.shape)} "
+                         "do not fit one another")
+    max_pages = block_table.shape[1]
+    lib = L.load()
+    ws_bytes = lib.aria_attention_decode_workspace_bytes(R, H, max_pages * 256)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
+    out = torch.empty((R, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(lib.aria_attention_decode_paged(_p(q), _p(k_pool), _p(v_pool), _p(block_table), block_table.stride(0), max_pages,
+                                                k_pool.shape[0], _p(lens), _p(out), R, H, q.stride(0), q.stride(1),
+                                                k_pool.stride(0), k_pool.stride(1), scale, _p(ws), ws_bytes, _stream(q)),
+                "attention_decode_paged")
+    return out
+
+
+def kv_append_paged(k_new: torch.Tensor, v_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                    block_table: torch.Tensor, write_pos: torch.Tensor):
+    """kv_append into a paged cache: k_new / v_new [R, H, 128] (128 contiguous, 16-byte aligned elements per row) go to row
+    write_pos[r] % 256 of page block_table[r, write_pos[r] // 256] (write_pos CUDA int32 [R]).  A negative write_pos, one past
+    the table's columns, or an entry outside the pool writes nothing.  See aria_kv_append_paged."""
+    _paged_pool_check(k_pool, v_pool, "kv_append_paged")
+    _chk(write_pos, torch.int32, align=4)
+    for t in (k_new, v_new):
+        if not (t.is_cuda and t.dtype == bf16 and t.dim() == 3 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0):
+            raise RuntimeError("kv_append_paged: new rows must be CUDA bf16 [R, H, 128] with a contiguous, 16-byte aligned last dim")
+    if k_new.stride() != v_new.stride() or k_new.shape != v_new.shape:
+        raise RuntimeError("kv_append_paged: k_new and v_new must share shape and strides")
+    R, H = k_new.shape[0], k_new.shape[1]
+    _block_table_check(block_table, R, "kv_append_paged")
+    if k_new.shape[2] != 128 or k_pool.shape[1] != H or write_pos.shape != (R,):
+        raise ValueError("kv_append_paged: the rows, pools and write_pos do not fit one another")
+    with torch.cuda.device(k_pool.device):
+        L.check(L.load().aria_kv_append_paged(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_pool), _p(v_pool),
+                                              k_pool.stride(0), k_pool.stride(1), _p(block_table), block_table.stride(0),
+                                              block_table.shape[1], k_pool.shape[0], _p(write_pos), R, H, _stream(k_pool)),
+                "kv_append_paged")
+
+
+def kv_pages_store(k: torch.Tensor, v: torch.Tensor, T: int, k_pool: torch.Tensor, v_pool: torch.Tensor, pages: torch.Tensor):
+    """Rows [0, T) of a one-row contiguous cache k / v [1, H, >= T, 128] (bf16, contiguous) into the pages of one request: row t
+    to row t % 256 of page pages[t // 256] (pages CUDA int32 [max_pages], e.g. a block-table row).  See aria_kv_pages_store."""
+    _paged_pool_check(k_pool, v_pool, "kv_pages_store")
+    _chk(k), _chk(v), _chk(pages, torch.int32, align=4)
+    H = k_pool.shape[1]
+    if (k.dim() != 4 or k.shape[0] != 1 or k.shape[1] != H or k.shape[3] != 128 or v.shape != k.shape or pages.dim() != 1
+            or not 0 < T <= min(k.shape[2], 256 * pages.numel())):
+        raise ValueError(f"kv_pages_store: {T} rows of {tuple(k.shape)} do not fit {pages.numel()} pages of {tuple(k_pool.shape)}")
+    with torch.cuda.device(k_pool.device):
+        L.check(L.load().aria_kv_pages_store(_p(k), _p(v), k.stride(1), int(T), _p(k_pool), _p(v_pool), k_pool.stride(0),
+                                             k_pool.stride(1), _p(pages), pages.numel(), k_pool.shape[0], H, _stream(k_pool)),
+                "kv_pages_store")
+
+
+def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                        seed: torch.Tensor, noise_rows: torch.Tensor, offsets: torch.Tensor,
+                        out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample_tokens_rows with every parameter per row, CUDA arrays [R]: temperature fp32 (0 = greedy), top_k int32, top_p fp32,
+    seed int64 (read as uint64), noise_rows int32, offsets int64 (read as uint64).  Row r equals sample_tokens on that row with
+    its own scalars, rng_offset = offsets[r], as row noise_rows[r].  out: int64 [R] (allocated when None).  The caller checks
+    the parameters as generate() does.  See aria_sample_tokens_slots."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(-1) == 1):
+        raise RuntimeError("sample_tokens_slots: logits must be CUDA bf16 [R, V] with a contiguous last dim")
+    R, V = logits.shape
+    if out is None:
+        out = torch.empty((R,), dtype=torch.int64, device=logits.device)
+    args = ((out, torch.int64), (temperature, torch.float32), (top_k, torch.int32), (top_p, torch.float32), (seed, torch.int64),
+            (noise_rows, torch.int32), (offsets, torch.int64))
+    for t, dt in args:
+        _chk(t, dt, align=4)
+        if t.shape != (R,):
+            raise ValueError(f"sample_tokens_slots: out and every per-row array must be [{R}], got {tuple(t.shape)}")
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_sample_tokens_slots(_p(logits), logits.stride(0), _p(out), R, V, _p(temperature), _p(top_k), _p(top_p),
+                                                  _p(seed), _p(noise_rows), _p(offsets), _stream(logits)), "sample_tokens_slots")
+    return out
+
+
+def decode_advance_slots(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: torch.Tensor, n_out: torch.Tensor,
+                         max_new: torch.Tensor, rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor,
+                         rng_offset: torch.Tensor, finished: torch.Tensor, eos_token_ids: Sequence[int] = (),
+                         pad_token_id: int = 0):
+    """decode_advance per slot, R = next_ids.numel() slots: an unfinished slot stores its token at out_tokens[r, n_out[r]]
+    (int32 [R, L]), finishes on an EOS id or at max_new[r] tokens, and moves n_out, its positions and its rng_offset (int64, read
+    as uint64) on by one; a finished slot changes nothing.  See aria_decode_advance_slots."""
+    R = next_ids.numel()
+    for t, dt in ((next_ids, torch.int64), (ids_in, torch.int64), (out_tokens, torch.int32), (n_out, torch.int32),
+                  (max_new, torch.int32), (rope_pos, torch.int32), (write_pos, torch.int32), (kv_len, torch.int32),
+                  (rng_offset, torch.int64), (finished, torch.uint8)):
+        _chk(t, dt, align=1)
+    if out_tokens.dim() != 2 or out_tokens.shape[0] != R or any(
+            t.numel() != R for t in (ids_in, n_out, max_new, rope_pos, write_pos, kv_len, rng_offset, finished)):
+        raise ValueError(f"decode_advance_slots: every slot array must have {R} entries and out_tokens [{R}, L]")
+    eos, n_eos = _eos_array(eos_token_ids)
+    with torch.cuda.device(next_ids.device):
+        L.check(L.load().aria_decode_advance_slots(_p(next_ids), _p(ids_in), _p(out_tokens), out_tokens.shape[1], _p(n_out),
+                                                   _p(max_new), _p(rope_pos), _p(write_pos), _p(kv_len), _p(rng_offset),
+                                                   _p(finished), C.cast(eos, C.c_void_p), n_eos, int(pad_token_id), R,
+                                                   _stream(next_ids)), "decode_advance_slots")

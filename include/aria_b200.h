@@ -401,6 +401,18 @@ int aria_attention_decode_devlen(const void* q, const void* k, const void* v, vo
                                  int64_t key_mask_stride, const int32_t* lens, int32_t B, int32_t H, int32_t T_max,
                                  int64_t q_stride_b, int64_t q_stride_h, int64_t kv_stride_b, int64_t kv_stride_h, float scale,
                                  void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* aria_attention_decode_devlen over a paged KV cache (continuous batching).  k_pool / v_pool [n_pages, H, 256, 128] bf16 (page
+ * stride page_stride, head stride pool_stride_h, 128-element rows); block_table int32 [R, >= max_pages] at row stride
+ * block_table_stride: row r's keys [256 s, 256 s + 256) are rows [0, 256) of page block_table[r, s].  Row r attends to its keys
+ * [0, min(lens[r], 256 max_pages)) (lens: DEVICE int32 [R]); q as aria_attention_decode's with R rows; out [R, H*128].
+ * The page size is the decode split, so split s reads exactly page s, with the contiguous kernel's key order and arithmetic:
+ * row r is bit-identical to aria_attention_decode_devlen on a contiguous cache holding the same keys.  Splits past
+ * ceil(lens[r] / 256) read no page and write (-inf, 0, 0); the merge reads the live splits only.  A live split whose entry is
+ * not in [0, n_pages) reads nothing.  workspace: aria_attention_decode_workspace_bytes(R, H, 256 * max_pages). */
+int aria_attention_decode_paged(const void* q, const void* k_pool, const void* v_pool, const int32_t* block_table,
+                                int64_t block_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* lens, void* out,
+                                int32_t R, int32_t H, int64_t q_stride_b, int64_t q_stride_h, int64_t page_stride,
+                                int64_t pool_stride_h, float scale, void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 /* aria_attention_decode / aria_attention_decode_devlen over an fp8 KV cache: k, v are e4m3 codes [B,H,T_max,128] (element = byte
  * strides kv_stride_b / kv_stride_h, multiples of 16), k_scale / v_scale fp32 [B,H,T_max] at scale_stride_b / scale_stride_h, one
  * scale per (row, head, token): key t of (b, h) is code * scale.  The key scale multiplies the reduced dot product q.code and the
@@ -532,6 +544,38 @@ int aria_kv_append_rows(const void* k_new, const void* v_new, int64_t new_stride
 int aria_sample_tokens_rows(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V, float temperature,
                             int32_t top_k, float top_p, uint64_t seed, const int32_t* noise_rows, const uint64_t* offsets,
                             aria_stream_t stream);
+/* Continuous batching over a paged KV cache (pools [n_pages, H, 256, 128] bf16 at page_stride / pool_stride_h, block table int32
+ * [R, >= max_pages] at row stride block_table_stride, as aria_attention_decode_paged's).
+ * aria_kv_append_paged: the k and v rows of slot r, k_new / v_new [R, H, 128] (strides new_stride_b / new_stride_h), go to row
+ * write_pos[r] % 256 of page block_table[r, write_pos[r] / 256] (write_pos: DEVICE int32 [R]).  Nothing is written for a
+ * negative write_pos, one at or past 256 * max_pages, or a table entry outside [0, n_pages): an idle or padding slot never
+ * writes into another request's pages.  Strides are multiples of 8 elements. */
+int aria_kv_append_paged(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_pool, void* v_pool,
+                         int64_t page_stride, int64_t pool_stride_h, const int32_t* block_table, int64_t block_table_stride,
+                         int32_t max_pages, int32_t n_pages, const int32_t* write_pos, int32_t R, int32_t H, aria_stream_t stream);
+/* Rows [0, T) of a one-row contiguous cache k / v [1, H, >= T, 128] (head stride src_stride_h) into the pages of one request:
+ * row t goes to row t % 256 of page pages[t / 256] (pages: DEVICE int32 [max_pages], a block-table row); a page entry outside
+ * [0, n_pages) is not written.  T <= 256 * max_pages. */
+int aria_kv_pages_store(const void* k, const void* v, int64_t src_stride_h, int32_t T, void* k_pool, void* v_pool,
+                        int64_t page_stride, int64_t pool_stride_h, const int32_t* pages, int32_t max_pages, int32_t n_pages,
+                        int32_t H, aria_stream_t stream);
+/* aria_sample_tokens_rows with every sampling parameter per row, from DEVICE arrays [R]: temperature (0 = greedy), top_k, top_p,
+ * seed (uint64), noise row and offset.  Row r is bit-identical to aria_sample_tokens run alone on that row with its scalars at
+ * rng_offset = offsets[r] as row noise_rows[r].  The caller checks the parameters as aria_sample_tokens does; out-of-range
+ * entries are brought into range (a non-positive or non-finite temperature is greedy, top_k is clamped to [0, 1024], and top_p
+ * is 1 without a top_k) rather than read past the kernel's buffers.  R <= 2^20, V <= 2^24. */
+int aria_sample_tokens_slots(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V,
+                             const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seed,
+                             const int32_t* noise_rows, const uint64_t* offsets, aria_stream_t stream);
+/* aria_decode_advance per slot (continuous batching).  For each slot r < R that is not finished: its token next_ids[r] is stored
+ * at out_tokens[r, n_out[r]] ([R, out_stride] int32) and n_out[r] + 1; the slot finishes when the token is one of the n_eos <= 8
+ * EOS ids (HOST array, copied into the launch) or n_out reaches max_new[r]; ids_in[r] <- the token (pad_token_id once
+ * finished); rope_pos, write_pos, kv_len and rng_offset[r] (uint64) + 1.  A finished slot (idle slots are finished) changes
+ * nothing.  R <= 1024, one launch. */
+int aria_decode_advance_slots(const int64_t* next_ids, int64_t* ids_in, int32_t* out_tokens, int64_t out_stride, int32_t* n_out,
+                              const int32_t* max_new, int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len, uint64_t* rng_offset,
+                              uint8_t* finished, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t R,
+                              aria_stream_t stream);
 /* Drafts from each row's history hist [B, hist_stride] int64 (its first hist_len[b] entries: the prompt after its left padding,
  * then the tokens emitted so far), Hugging Face's PromptLookupCandidateGenerator.get_candidates per row: for n = min(M, len - 1)
  * down to 1, the earliest occurrence of the last n tokens that has a non-empty continuation; the continuation, at most K tokens
