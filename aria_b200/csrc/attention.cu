@@ -126,17 +126,31 @@ struct SharedTileWalk {
   }
 };
 
+// Prefill over a paged prefix (aria_attention_prefill_paged_prefix): the shared-prefix prefill whose prefix is P keys
+// (a multiple of 256) held in pool pages, key 256 i + r at row r of page pages[i].
+struct PagedPrefixParams {
+  const int32_t* cu;     // [n_seg + 1] device segment starts of the packed suffixes
+  int n_seg;
+  int P;
+  const int32_t* pages;  // [>= P / 256] device page list of the prefix
+};
+
 // HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM); LSE: also store the row logsumexp
 // (what the backward needs to recompute P).  tmK16 / tmV16: 16-column SW32 boxes of columns 64-79 (HD = 80 only).
 // SHARED (HD = 128): the shared-prefix suffix prefill; the keys walk the prefix (tmPK / tmPV, rows [0, sp.P)) and then the
 // query tile's segments of the packed suffix (tmK / tmV), SharedTileWalk; a query sees the prefix and its own segment up to
 // itself.  A key masked for a row adds exact zeros to that row, so each row's arithmetic is: the prefix tiles, then its own
 // segment's tiles, whatever else shares its query tile.
-template <int HD, bool CAUSAL, bool LSE, bool SHARED>
+// PAGED (with SHARED): tmPK / tmPV map a page pool [n_pages, H, 256, 128] and prefix tile j (keys 128 j ..) is rows
+// 128 (j & 1) .. of page pages[j >> 1]; only the producer reads the page list.  The tiles, and so every row's arithmetic, are
+// those of the contiguous prefix.
+template <int HD, bool CAUSAL, bool LSE, bool SHARED, bool PAGED = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                               const CUtensorMap& tmK16, const CUtensorMap& tmV16, const CUtensorMap& tmPK,
-                                              const CUtensorMap& tmPV, const AttnParams& p, const SharedPrefixParams& sp) {
+                                              const CUtensorMap& tmPV, const AttnParams& p, const SharedPrefixParams& sp,
+                                              const int32_t* pages = nullptr) {
   static_assert(!SHARED || (HD == 128 && !CAUSAL), "the shared-prefix prefill runs at head dim 128 with its own mask");
+  static_assert(!PAGED || SHARED, "a paged prefix is a shared-prefix prefill");
   constexpr int S = AttnCfg<HD>::STAGES, KVT = AttnCfg<HD>::KV_TILE, NO = AttnCfg<HD>::NO;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -199,14 +213,22 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
           walk.step(j);
           const CUtensorMap* mk = walk.seg_c < 0 ? &tmPK : &tmK;
           const CUtensorMap* mv = walk.seg_c < 0 ? &tmPV : &tmV;
+          int row = walk.k0, page = 0;
+          if constexpr (PAGED) {
+            // an entry outside the pool is an out-of-bounds box: TMA fills it with zeros
+            if (walk.seg_c < 0) {
+              row = (j & 1) * AT_BN;
+              page = pages[j >> 1];
+            }
+          }
           mbar_wait(&k_empty[s], ph);
           mbar_arrive_expect_tx(&k_full[s], KVT);
-          tma_load_4d(sK + s * KVT, mk, &k_full[s], 0, walk.k0, h, 0);
-          tma_load_4d(sK + s * KVT + AT_HALF, mk, &k_full[s], 64, walk.k0, h, 0);
+          tma_load_4d(sK + s * KVT, mk, &k_full[s], 0, row, h, page);
+          tma_load_4d(sK + s * KVT + AT_HALF, mk, &k_full[s], 64, row, h, page);
           mbar_wait(&v_empty[s], ph);
           mbar_arrive_expect_tx(&v_full[s], KVT);
-          tma_load_4d(sV + s * KVT, mv, &v_full[s], 0, walk.k0, h, 0);
-          tma_load_4d(sV + s * KVT + AT_HALF, mv, &v_full[s], 64, walk.k0, h, 0);
+          tma_load_4d(sV + s * KVT, mv, &v_full[s], 0, row, h, page);
+          tma_load_4d(sV + s * KVT + AT_HALF, mv, &v_full[s], 64, row, h, page);
           continue;
         }
         mbar_wait(&k_empty[s], ph);
@@ -501,6 +523,16 @@ attn_prefill_shared_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const
                                   const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmPK,
                                   const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const SharedPrefixParams sp) {
   attn_fwd_body<128, false, LSE, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, sp);
+}
+
+// One CTA per (head, 128 packed queries): tmQ / tmK / tmV map the packed suffix [1, H, S_tot, 128] as above, tmPK / tmPV the
+// layer's page pools [n_pages, H, 256, 128].
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_prefill_paged_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmPK,
+                                 const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const PagedPrefixParams pp) {
+  attn_fwd_body<128, false, false, true, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, SharedPrefixParams{pp.cu, pp.n_seg, pp.P},
+                                               pp.pages);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1136,6 +1168,48 @@ extern "C" int aria_attention_prefill_shared_prefix(const void* q, const void* k
   attn_prefill_shared_prefix_kernel<false><<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
       tmQ, tmK, tmV, tmPK, tmPV, p, sp);
   return check_launch("attn_prefill_shared_prefix_kernel");
+}
+
+extern "C" int aria_attention_prefill_paged_prefix(const void* q, const void* k, const void* v, const void* k_pool,
+                                                   const void* v_pool, const int32_t* pages, int32_t n_pages_list, int32_t n_pages,
+                                                   const int32_t* cu_seqlens, void* out, int32_t B, int32_t H, int32_t S_tot,
+                                                   int32_t P, int64_t q_stride_h, int64_t kv_stride_h, int64_t page_stride,
+                                                   int64_t pool_stride_h, float scale, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(q && k && v && k_pool && v_pool && cu_seqlens && out && (pages || P == 0));
+  ARIA_CHECK_ARG(B > 0 && H > 0 && S_tot >= B && n_pages > 0 && n_pages_list >= 0);
+  ARIA_CHECK_ARG(P >= 0 && P % DEC_SPLIT_KEYS == 0 && P / DEC_SPLIT_KEYS <= n_pages_list);
+  ARIA_CHECK_ARG(q_stride_h >= static_cast<int64_t>(S_tot) * AT_D && kv_stride_h >= static_cast<int64_t>(S_tot) * AT_D);
+  ARIA_CHECK_ARG(pool_stride_h >= DEC_SPLIT_KEYS * AT_D && page_stride >= pool_stride_h * H);  // pages do not overlap
+  ARIA_CHECK_ARG(q_stride_h % 8 == 0 && kv_stride_h % 8 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  const int n_q_tiles = (S_tot + AT_BM - 1) / AT_BM;
+  ARIA_CHECK_ARG(static_cast<int64_t>(H) * n_q_tiles < (1ll << 31));
+  CUtensorMap tmQ, tmK, tmV, tmPK, tmPV;
+  int rc = make_tmap_heads(&tmQ, q, S_tot, H, 1, q_stride_h * H, q_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmK, k, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmV, v, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPK, k_pool, DEC_SPLIT_KEYS, H, n_pages, page_stride, pool_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPV, v_pool, DEC_SPLIT_KEYS, H, n_pages, page_stride, pool_stride_h);
+  if (rc) return rc;
+  AttnParams p{};
+  p.B = 1;
+  p.H = H;
+  p.Tq = S_tot;
+  p.Tk = S_tot;
+  p.out_hd = AT_D;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.n_q_tiles = n_q_tiles;
+  const PagedPrefixParams pp{cu_seqlens, B, P, pages};
+  constexpr int smem = AttnCfg<128>::SMEM;
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, attn_prefill_paged_prefix_kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_prefill_paged_prefix_kernel<<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      tmQ, tmK, tmV, tmPK, tmPV, p, pp);
+  return check_launch("attn_prefill_paged_prefix_kernel");
 }
 
 extern "C" int aria_attention_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int32_t* cu_seqlens,

@@ -736,6 +736,20 @@ class AriaAttention(nn.Module):
         ops.kv_scatter_tails(k, v, S, cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx], cu_seqlens, n)
         return self._o_proj(o.view(1, S, d), residual)
 
+    def prefill_paged(self, hidden_states, cache: PagedKVCache, rope, row, P, cu_seqlens, position_ids, residual=None, hq=None):
+        """The S prompt tokens after a P-token prefix held in pages (AriaMoELMModel.prefill_paged): the fused projection writes q,
+        k, v to a staging buffer (RoPE at position_ids), the tokens attend to the prefix pages row[: P / 256] and to themselves
+        (ops.attention_prefill_paged_prefix), and their k, v rows are stored into the pages row[P / 256:]."""
+        _, S, d = hidden_states.shape
+        H, hd = self.num_heads, self.head_dim
+        stage = torch.empty(3, 1, H, S, hd, dtype=bf16, device=hidden_states.device)
+        q, k, v = stage[0], stage[1], stage[2]
+        self._qkv(hidden_states, hq, [q, k, v], S, 0, rope, position_ids)
+        kp, vp = cache.k[self.layer_idx], cache.v[self.layer_idx]
+        o = ops.attention_prefill_paged_prefix(q, k, v, S, kp, vp, row, P, cu_seqlens, hd ** -0.5)
+        ops.kv_pages_store(k, v, S, kp, vp, row[P // PagedKVCache.PAGE_SIZE:])
+        return self._o_proj(o.view(1, S, d), residual)
+
 
 class MoEDecoderLayer(nn.Module):
     """moe_lm.py:580-602: x + attn(rms(x)); h + moe(rms(h)).  The MoE residual add is deferred into the next
@@ -790,6 +804,13 @@ class MoEDecoderLayer(nn.Module):
         """forward() for packed suffixes over a shared prefix (AriaAttention.prefill_suffixes)."""
         h, hq, x = self._attn_input(x, pending)
         x = self.self_attn.prefill_suffixes(h, cache, rope, cu_seqlens, position_ids, residual=x, hq=hq)
+        h = self.post_attention_layernorm(x)
+        return x, self.mlp(h)
+
+    def prefill_paged(self, x, pending, cache, rope, row, P, cu_seqlens, position_ids):
+        """forward() for a prompt's tokens after a prefix held in pages (AriaAttention.prefill_paged)."""
+        h, hq, x = self._attn_input(x, pending)
+        x = self.self_attn.prefill_paged(h, cache, rope, row, P, cu_seqlens, position_ids, residual=x, hq=hq)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
@@ -861,6 +882,30 @@ class AriaMoELMModel(nn.Module):
             x, pending = layer.prefill_suffixes(x, pending, cache, rope, cu_seqlens, position_ids)
         return x, pending
 
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, row, P, position_ids):
+        """Prefill the S prompt tokens that follow a P-token prefix whose keys and values are already in the pages of one
+        request (prefix caching, serving.Engine).  inputs_embeds [1, S, d]; row: the request's block-table row (CUDA int32
+        [max_pages]), whose first P / 256 pages hold the prefix (P a multiple of 256; 0 = no prefix); position_ids CUDA int32
+        [S], the RoPE positions P .. P + S - 1.  The tokens attend to the prefix and causally to themselves, and their keys and
+        values go to the pages row[P / 256:], as forward() on the whole prompt would have stored them.  Every row's output is
+        the one forward() gives that position on the whole prompt, bit for bit.  Returns (x, pending) as forward() does."""
+        if not isinstance(cache, PagedKVCache):
+            raise ValueError("prefill_paged needs a PagedKVCache")
+        if inputs_embeds.dim() != 3 or inputs_embeds.shape[0] != 1 or inputs_embeds.shape[1] < 1:
+            raise ValueError(f"prefill_paged: inputs_embeds must be [1, S >= 1, d], got {tuple(inputs_embeds.shape)}")
+        S = inputs_embeds.shape[1]
+        max_pages = row.numel()
+        if not isinstance(P, int) or P < 0 or P % cache.PAGE_SIZE or P + S > max_pages * cache.PAGE_SIZE:
+            raise ValueError(f"prefill_paged: P = {P!r} must be a multiple of {cache.PAGE_SIZE} and P + {S} tokens must fit "
+                             f"{max_pages} pages")
+        dev = inputs_embeds.device
+        rope = self.rope_tables(cache.block_table.shape[1] * cache.PAGE_SIZE, dev)
+        cu = torch.tensor([0, S], dtype=torch.int32).to(dev, non_blocking=True)
+        x, pending = inputs_embeds, None
+        for layer in self.layers:
+            x, pending = layer.prefill_paged(x, pending, cache, rope, row, P, cu, position_ids)
+        return x, pending
+
 
 class AriaMoELMForCausalLM(nn.Module):
     """moe_lm.py:639-679."""
@@ -911,6 +956,13 @@ class AriaMoELMForCausalLM(nn.Module):
             pending = pending[:, -num_logits_to_keep:, :].contiguous()
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h), cache
+
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, row, P, position_ids):
+        """AriaMoELMModel.prefill_paged, then the final norm and lm_head on the last row -> logits [1, 1, V], those of
+        forward(num_logits_to_keep=1) on the whole prompt."""
+        x, pending = self.model.prefill_paged(inputs_embeds, cache, row, P, position_ids)
+        h, _ = self.model.norm(x[:, -1:, :].contiguous(), residual=pending[:, -1:, :].contiguous())
+        return self.lm_head(h)
 
     def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
         """inputs_embeds [B, 1, d] -> logits [B, 1, V] for one decode step driven by device positions (graph-replayable)."""

@@ -1447,6 +1447,40 @@ def kv_pages_store(k: torch.Tensor, v: torch.Tensor, T: int, k_pool: torch.Tenso
                 "kv_pages_store")
 
 
+def attention_prefill_paged_prefix(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, S_tot: int, k_pool: torch.Tensor,
+                                   v_pool: torch.Tensor, pages: Optional[torch.Tensor], P: int, cu_seqlens: torch.Tensor,
+                                   scale: float) -> torch.Tensor:
+    """attention_prefill_shared_prefix with the prefix read from pool pages (prefix caching): q / k / v, S_tot and cu_seqlens as
+    there; the prefix is P keys (a multiple of 256), key 256 i + r at row r of page pages[i] (pages CUDA int32 [>= P / 256]) of the
+    pools [n_pages, H, 256, 128].  P = 0 is no prefix (pages may be None): the varlen causal forward -> out [S_tot, H*128].  Every
+    row is bit-identical to attention_prefill_shared_prefix on a contiguous copy of the prefix (P = 0: attention_varlen).  A page
+    entry outside the pool reads zeros.  See aria_attention_prefill_paged_prefix."""
+    what = "attention_prefill_paged_prefix"
+    _attn_qkv_check(q, k, v, what)
+    _paged_pool_check(k_pool, v_pool, what)
+    B = _packed_check(S_tot, cu_seqlens, what)
+    H = q.shape[1]
+    if q.shape[0] != 1 or q.shape[2] < S_tot or k.shape[:2] != (1, H) or k.shape[2] < S_tot or v.shape != k.shape:
+        raise ValueError(f"{what}: q {tuple(q.shape)} / k {tuple(k.shape)} must be [1, H, >= {S_tot}, 128]")
+    if k_pool.shape[1] != H:
+        raise ValueError(f"{what}: pools {tuple(k_pool.shape)} do not have the {H} heads of q")
+    n_list = 0
+    if pages is not None:
+        _chk(pages, torch.int32, align=4)
+        if pages.dim() != 1:
+            raise ValueError(f"{what}: pages must be int32 [n], got {tuple(pages.shape)}")
+        n_list = pages.numel()
+    if not isinstance(P, int) or P < 0 or P % 256 or P // 256 > n_list:
+        raise ValueError(f"{what}: P must be a multiple of 256 in [0, 256 x {n_list} listed pages], got {P!r}")
+    out = torch.empty((S_tot, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(L.load().aria_attention_prefill_paged_prefix(_p(q), _p(k), _p(v), _p(k_pool), _p(v_pool), _p(pages), n_list,
+                                                             k_pool.shape[0], _p(cu_seqlens), _p(out), B, H, S_tot, P,
+                                                             q.stride(1), k.stride(1), k_pool.stride(0), k_pool.stride(1), scale,
+                                                             _stream(q)), what)
+    return out
+
+
 def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
                         seed: torch.Tensor, noise_rows: torch.Tensor, offsets: torch.Tensor,
                         out: Optional[torch.Tensor] = None) -> torch.Tensor:

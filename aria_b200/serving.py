@@ -10,9 +10,9 @@ Every request's result equals model.generate(ids[None], pixel_values, pixel_mask
 eos_token_id=E, pad_token_id=P)[0] bit for bit: the prompt ids, then the generated tokens up to and including the first EOS.
 It does not depend on max_batch, poll_every, when the request arrived, its slot or the other requests, because
 
-  - admission is generate()'s batch-1 prefill (eager forward(), ViT included) into a one-row staging cache, whose rows are then
-    copied into the request's pages (ops.kv_pages_store), and its first token comes from its own sampling parameters at
-    RNG offset 0;
+  - admission is generate()'s batch-1 prefill (the ViT, then the prompt through every layer) written straight into the
+    request's pages (moe_lm.AriaMoELMForCausalLM.prefill_paged), and its first token comes from its own sampling parameters
+    at RNG offset 0;
   - a decode step reads every row's keys from its own pages with the arithmetic of the contiguous decode kernel
     (ops.attention_decode_paged: a page is one split), samples each row with its own parameters, noise row 0 and offset =
     tokens emitted (ops.sample_tokens_slots), and the other kernels of the step compute each row on its own.
@@ -24,12 +24,22 @@ for the smallest power of two >= n (and the smallest power of two of table colum
 n are idle: finished, one key on the reserved null page 0, and no write position, so they never write into a request's pages.
 The host looks at the finished flags every poll_every steps.
 
-The scheduler (Scheduler, PageAllocator) is plain host code with no device calls.  GPU only; bf16 KV pages; no expert
+Prefix caching: the full 256-token pages of a prompt that a prefill wrote are kept, keyed by a hash chain over the prompt's
+ids and images (page_keys), until their page is needed for something else.  A request whose prompt starts with keyed pages
+(the same image, system prompt or earlier turn) holds them instead of computing them: its prefill starts at the first page
+that is not cached (AriaMoELMModel.prefill_paged reads the earlier keys from the pages) and the ViT runs only on the images
+that have tokens from there on.  The hit stops before the prompt's last token, which is always prefilled for the first
+token's logits.  A page's keys and values do not depend on what follows it in the prompt, and the paged-prefix prefill
+attends to 256-key-aligned pages with the tile order of a prefill of the whole prompt, so a hit changes no result bit.
+Pages written by decode steps are never keyed: their keys and values come from the decode arithmetic, not the prefill's.
+
+The scheduler (Scheduler, PageAllocator) and the page keys are plain host code with no device calls.  GPU only; bf16 KV pages; no expert
 parallelism.  Fp8 or bf16 expert and dense weights are fine (they live inside the layers).
 """
 from __future__ import annotations
 
 import collections
+import hashlib
 import time
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
@@ -53,26 +63,137 @@ def _pow2_at_least(n: int, cap: int) -> int:
     return min(p, cap)
 
 
+def _hash(*parts) -> bytes:
+    """128 bits of SHA-256 over the parts (bytes or contiguous buffers; SHA-256 has CPU instructions on current hosts and ran
+    twice as fast as BLAKE2b on an image)."""
+    h = hashlib.sha256()
+    for p in parts:
+        h.update(p)
+    return h.digest()[:16]
+
+
+def _pixel_row_digest(pixels: torch.Tensor, mask: Optional[torch.Tensor]) -> bytes:
+    """128-bit digest of one pixel row: its bf16 bytes (what the ViT reads), its shape and its pixel_mask row."""
+    x = pixels.detach().to("cpu", torch.bfloat16).contiguous()
+    m = b"-" if mask is None else mask.detach().to("cpu", torch.bool).contiguous().numpy().tobytes()
+    return _hash(repr(tuple(x.shape)).encode(), x.view(torch.int16).numpy(), m)
+
+
+def page_keys(ids: torch.Tensor, pixel_values: Optional[torch.Tensor] = None, pixel_mask: Optional[torch.Tensor] = None,
+              image_token: Optional[int] = None) -> List[bytes]:
+    """Keys of the full 256-token pages of a prompt (host int64 ids [T]): page i (256 (i + 1) <= T) has key
+    H(key of page i - 1 | its ids | the digests of the pixel rows whose image tokens fall in it), so two prompts share page i's key
+    only if they agree on every token and image up to its end.  Pixel row r owns the image tokens r n .. r n + n - 1 in order,
+    n = image tokens / pixel rows; a prompt whose image-token count is not a positive multiple of its pixel rows gets no keys
+    (its admission fails as forward() would)."""
+    n_full = ids.numel() // PAGE
+    if n_full == 0:
+        return []
+    ids_np = ids.numpy()
+    rows_in_page: List[List[int]] = [[] for _ in range(n_full)]
+    digest: Dict[int, bytes] = {}
+    if pixel_values is not None:
+        pos = (ids == image_token).nonzero().flatten().tolist()
+        R = pixel_values.shape[0]
+        if not pos or R == 0 or len(pos) % R:
+            return []
+        n = len(pos) // R
+        for k, t in enumerate(pos):
+            i = t // PAGE
+            if i < n_full and (not rows_in_page[i] or rows_in_page[i][-1] != k // n):
+                rows_in_page[i].append(k // n)
+        needed = sorted({r for rows in rows_in_page for r in rows})
+        digest = {r: _pixel_row_digest(pixel_values[r], None if pixel_mask is None else pixel_mask[r]) for r in needed}
+    keys, prev = [], b""
+    for i in range(n_full):
+        prev = _hash(prev, ids_np[i * PAGE:(i + 1) * PAGE].tobytes(), *(digest[r] for r in rows_in_page[i]))
+        keys.append(prev)
+    return keys
+
+
 class PageAllocator:
-    """Free list of the pool's pages 1 .. n_pages - 1; page 0 is the null page idle slots point at, never handed out."""
+    """The pool's pages 1 .. n_pages - 1 with reference counts and a cache of keyed pages; page 0 is the null page idle slots
+    point at, never handed out.
+
+    A page is held by every live request that lists it (hold / alloc add one holder, free removes one).  A page no request
+    holds is free: uncached, or cached (it has a key) and idle, kept in the order it was released.  n_free counts both.  alloc
+    hands out uncached free pages first (the lowest first), then idle cached pages, least recently released first, dropping
+    their keys (an eviction, counted in n_evicted).  A held page is never handed out."""
 
     def __init__(self, n_pages: int):
         if n_pages < 2:
             raise ValueError(f"a page pool needs the null page and at least one more, got {n_pages} pages")
         self.n_pages = n_pages
-        self._free = list(range(n_pages - 1, 0, -1))   # pop() hands out the lowest page first
+        self._free = list(range(n_pages - 1, 0, -1))   # uncached free pages; pop() hands out the lowest page first
+        self._refs = [0] * n_pages
+        self._idle: "collections.OrderedDict[int, None]" = collections.OrderedDict()   # cached, unheld; oldest release first
+        self._page_of: Dict[bytes, int] = {}
+        self._key_of: Dict[int, bytes] = {}
+        self.n_evicted = 0
 
     @property
     def n_free(self) -> int:
-        return len(self._free)
+        return len(self._free) + len(self._idle)
+
+    @property
+    def n_cached(self) -> int:
+        return len(self._key_of)
+
+    def refs(self, page: int) -> int:
+        return self._refs[page]
 
     def alloc(self, n: int) -> List[int]:
-        if n > len(self._free):
-            raise RuntimeError(f"page pool: {n} pages asked, {len(self._free)} free")
-        return [self._free.pop() for _ in range(n)]
+        if n > self.n_free:
+            raise RuntimeError(f"page pool: {n} pages asked, {self.n_free} free")
+        out = []
+        for _ in range(n):
+            if self._free:
+                p = self._free.pop()
+            else:
+                p, _ = self._idle.popitem(last=False)
+                del self._page_of[self._key_of.pop(p)]
+                self.n_evicted += 1
+            self._refs[p] = 1
+            out.append(p)
+        return out
 
     def free(self, pages: List[int]) -> None:
-        self._free.extend(reversed(pages))
+        """Remove one holder from each page, the last page first: a prompt's later pages become least recently released, so
+        they are evicted before its earlier ones."""
+        for p in reversed(pages):
+            if self._refs[p] < 1:
+                raise RuntimeError(f"page pool: page {p} freed but not held")
+            self._refs[p] -= 1
+            if self._refs[p] == 0:
+                if p in self._key_of:
+                    self._idle[p] = None
+                else:
+                    self._free.append(p)
+
+    def lookup(self, keys: List[bytes]) -> List[int]:
+        """The cached pages of the longest run of keys[0], keys[1], ... that are all cached."""
+        out = []
+        for k in keys:
+            p = self._page_of.get(k)
+            if p is None:
+                break
+            out.append(p)
+        return out
+
+    def hold(self, pages: List[int]) -> None:
+        """Add one holder to each of these cached pages (a hit)."""
+        for p in pages:
+            if self._refs[p] == 0:
+                del self._idle[p]
+            self._refs[p] += 1
+
+    def register(self, page: int, key: bytes) -> None:
+        """Key a held page, unless the key or the page is keyed already."""
+        if key in self._page_of or page in self._key_of:
+            return
+        assert self._refs[page] > 0, "only a held page's contents are known"
+        self._page_of[key] = page
+        self._key_of[page] = key
 
 
 @dataclass
@@ -84,6 +205,8 @@ class Request:
     pixel_values: Optional[torch.Tensor] = None
     pixel_mask: Optional[torch.Tensor] = None
     pages: List[int] = field(default_factory=list)
+    keys: List[bytes] = field(default_factory=list)    # page_keys of the prompt's full pages
+    prefix_len: int = 0                                 # prompt tokens found in cached pages at admission (a multiple of 256)
 
     @property
     def n_pages(self) -> int:
@@ -94,7 +217,11 @@ class Scheduler:
     """FIFO admission without overcommit, dense slots, no preemption.  slots[s] is the request in slot s (s < n_active).
 
     admit() admits the queue's head while a slot is free and its pages are free, reserving them; retire(s) frees the pages of
-    slot s and moves the last active slot into s, returning that move (src, dst) or None when s was the last slot."""
+    slot s and moves the last active slot into s, returning that move (src, dst) or None when s was the last slot.
+    Prefix caching: admission first follows the head's page keys through the cache, at most floor((T - 1) / 256) pages (the
+    prompt's last token is always prefilled); the hit pages come first in req.pages and req.prefix_len = 256 x hits.  The
+    head is admitted when a slot is free and its other pages fit the free pages that are not among its hits.  register(req),
+    after a successful admission, keys its full prompt pages that are not cached yet."""
 
     def __init__(self, max_batch: int, n_pages: int):
         self.max_batch = max_batch
@@ -113,12 +240,25 @@ class Scheduler:
 
     def admit_one(self) -> Optional[tuple]:
         """-> (slot, request) for the queue's head, its pages reserved, when a slot and its pages are free; else None."""
-        if not (self.queue and len(self.slots) < self.max_batch and self.queue[0].n_pages <= self.pages.n_free):
+        if not (self.queue and len(self.slots) < self.max_batch):
             return None
-        req = self.queue.popleft()
-        req.pages = self.pages.alloc(req.n_pages)
+        req = self.queue[0]
+        hits = self.pages.lookup(req.keys[:(req.input_ids.numel() - 1) // PAGE])
+        idle_hits = sum(1 for p in hits if self.pages.refs(p) == 0)
+        if req.n_pages - len(hits) > self.pages.n_free - idle_hits:
+            return None
+        self.queue.popleft()
+        self.pages.hold(hits)                     # before alloc, which may evict idle cached pages
+        req.pages = hits + self.pages.alloc(req.n_pages - len(hits))
+        req.prefix_len = PAGE * len(hits)
         self.slots.append(req)
         return len(self.slots) - 1, req
+
+    def register(self, req: Request) -> None:
+        """Key req's full prompt pages that are not cached yet (their prefill is in flight on the admission stream, so a
+        later admission on that stream reads them finished)."""
+        for page, key in zip(req.pages, req.keys):
+            self.pages.register(page, key)
 
     def admit(self) -> List[tuple]:
         """-> [(slot, request)] admitted, in FIFO order, their pages reserved."""
@@ -151,7 +291,8 @@ class Engine:
     output row per slot as long as the pool, since a request may spend the whole pool on its budget: 4 x max_batch x
     256 ceil(max_kv_tokens / 256) bytes (32 MiB at the defaults, 4 GiB at 1024 slots and a 2^20-token pool).
     `stats`: graphs captured, decode steps replayed, slot-steps of active requests (mean occupancy = active_slot_steps /
-    (steps * max_batch)), host seconds spent waiting in polls.  `times[rid]`: host clock (time.perf_counter) when its first
+    (steps * max_batch)), host seconds spent waiting in polls; prefix caching: prompt tokens admitted, those found in cached
+    pages (prefix_hit_tokens), pixel rows the ViT ran on and skipped, cached pages evicted.  `times[rid]`: host clock (time.perf_counter) when its first
     token and its last token were known done (first poll after admission, poll that saw it finish)."""
 
     def __init__(self, model, max_batch: int = 64, max_kv_tokens: int = 131072, eos_token_id=None, pad_token_id=None,
@@ -182,7 +323,6 @@ class Engine:
         self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev)
         self._idle(0, max_batch)
         self.rope = lm.model.rope_tables(self.max_pages * PAGE, dev)   # held here: the graphs read these tables
-        self._staging = None                                            # one-row prefill cache, grown by 256-row buckets
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._pool = torch.cuda.graph_pool_handle()
         self._fin_host = torch.ones(max_batch, dtype=torch.uint8).pin_memory()
@@ -191,7 +331,8 @@ class Engine:
         self._next_rid = 0
         self._undelivered: Dict[int, torch.Tensor] = {}
         self._first_seen = set()
-        self.stats = {"graphs_captured": 0, "steps": 0, "active_slot_steps": 0, "poll_host_s": 0.0, "polls": 0}
+        self.stats = {"graphs_captured": 0, "steps": 0, "active_slot_steps": 0, "poll_host_s": 0.0, "polls": 0,
+                      "prompt_tokens": 0, "prefix_hit_tokens": 0, "vit_rows_run": 0, "vit_rows_skipped": 0, "pages_evicted": 0}
         self.times: Dict[int, list] = {}
 
     # ------------------------------------------------------------------------------------------------ public API
@@ -199,7 +340,7 @@ class Engine:
                     temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0) -> int:
         """Queue one request (input_ids [T] or [1, T]; pixel inputs as generate()'s for that one row) -> its id.  Arguments are
         checked as generate() checks them, and a request that needs more pages than the pool has is refused, here, before
-        any device work."""
+        any device work.  The prompt's page keys (page_keys) are computed here, on the host."""
         if not isinstance(input_ids, torch.Tensor) or input_ids.dim() not in (1, 2):
             raise ValueError("input_ids must be a tensor [T] or [1, T]")
         ids = input_ids.reshape(1, -1) if input_ids.dim() == 1 else input_ids
@@ -209,6 +350,8 @@ class Engine:
                                         self.pad, seed, self.poll_every)
         sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
         req = Request(self._next_rid, ids[0].to("cpu", torch.int64), max_new_tokens, sampling, pixel_values, pixel_mask)
+        image_token = None if pixel_values is None else self.model.config.image_token_index
+        req.keys = page_keys(req.input_ids, pixel_values, pixel_mask, image_token)
         self.sched.submit(req)
         self._next_rid += 1
         return req.rid
@@ -246,6 +389,7 @@ class Engine:
                 self._idle(s, s + 1)
                 self._undelivered = done
                 raise
+            self.sched.register(req)
         return done
 
     def run(self) -> Dict[int, torch.Tensor]:
@@ -307,23 +451,49 @@ class Engine:
         return g
 
     def _admit(self, s: int, req: Request) -> None:
-        """generate()'s batch-1 prefill into the staging cache, its rows into the request's pages, then slot s's state and its
-        first token (sampled at offset 0 and recorded by the slot advance, as generate() records its first token)."""
+        """generate()'s batch-1 prefill of the prompt past its cached prefix (req.prefix_len tokens, 0 on a miss), written into
+        the request's pages, then slot s's state and its first token (sampled at offset 0 and recorded by the slot advance, as
+        generate() records its first token).
+
+        Image features are merged from the first uncached image token on: the ViT and the projector run on the pixel rows from
+        the first one with a token at or past the prefix, and each pixel row's features do not depend on the rows that share
+        its launch."""
         m, lm = self.model, self.model.language_model
-        T = req.input_ids.numel()
-        bucket = _pages_for(T) * PAGE
-        if self._staging is None or self._staging.T_max < bucket:
-            self._staging = None
-            self._staging = lm.new_cache(1, bucket, self.dev)
-        cache = self._staging
-        cache.seq_len = 0
-        out = m.forward(req.input_ids[None], req.pixel_values, req.pixel_mask, past_key_values=cache, num_logits_to_keep=1)
+        ids, P = req.input_ids, req.prefix_len
+        T = ids.numel()
+        pv, pm = req.pixel_values, req.pixel_mask
+        if pv is not None:
+            # forward()'s image-token check, on the host and before any device work: pixel rows x queries per row
+            cfg = m.config
+            n_patch = (pv.shape[-1] // cfg.vision_config.patch_size) ** 2
+            n_query = cfg.projector_patch_to_query_dict.get(n_patch)
+            assert n_query is not None, f"Query number for {n_patch} patches is not provided"
+            img = (ids == cfg.image_token_index).nonzero().flatten()
+            if img.numel() != pv.shape[0] * n_query:
+                raise ValueError(f"Image features and image tokens do not match: tokens: {img.numel()}, features "
+                                 f"{pv.shape[0] * n_query}")
         row = torch.full((self.max_pages,), -1, dtype=torch.int32)
         row[:len(req.pages)] = torch.tensor(req.pages, dtype=torch.int32)
         bt = self.cache.block_table[s]
         bt.copy_(row)
-        for kc, vc, kp, vp in zip(cache.k, cache.v, self.cache.k, self.cache.v):
-            ops.kv_pages_store(kc, vc, T, kp, vp, bt)
+        ids_dev = ids[P:].to(self.dev, non_blocking=True)
+        emb = ops.embedding(ids_dev[None], lm.get_input_embeddings().weight)
+        if pv is not None:
+            k0 = int((img < P).sum())                  # image tokens inside the cached prefix
+            r0 = k0 // n_query                         # first pixel row with a token at or past P
+            if r0 < pv.shape[0]:
+                pix = pv[r0:].to(self.dev, non_blocking=True).to(torch.bfloat16)
+                feats, image_attn_mask = m.vision_tower(pix, None if pm is None else pm[r0:])
+                feats = m.multi_modal_projector(feats, image_attn_mask)
+                ops.merge_image_features(ids_dev, m.config.image_token_index,
+                                         feats.reshape(-1, feats.shape[-1])[k0 - r0 * n_query:], emb.view(-1, emb.shape[-1]))
+            self.stats["vit_rows_run"] += pv.shape[0] - r0
+            self.stats["vit_rows_skipped"] += r0
+        pos = torch.arange(P, T, dtype=torch.int32, device=self.dev)
+        logits = lm.prefill_paged(emb, self.cache, bt, P, pos)
+        self.stats["prompt_tokens"] += T
+        self.stats["prefix_hit_tokens"] += P
+        self.stats["pages_evicted"] = self.sched.pages.n_evicted
         t, k, p, seed = req.sampling
         st = self.state
         st.rope_pos[s] = T - 1
@@ -338,7 +508,7 @@ class Engine:
         st.max_new[s] = req.max_new_tokens
         st.n_out[s] = 0
         st.finished[s] = 0
-        self._sample_and_advance(_slot_rows(st, s), out.logits[:, -1])
+        self._sample_and_advance(_slot_rows(st, s), logits[:, -1])
 
     def _poll_and_retire(self) -> Dict[int, torch.Tensor]:
         t0 = time.perf_counter()

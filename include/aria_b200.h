@@ -559,6 +559,18 @@ int aria_kv_append_paged(const void* k_new, const void* v_new, int64_t new_strid
 int aria_kv_pages_store(const void* k, const void* v, int64_t src_stride_h, int32_t T, void* k_pool, void* v_pool,
                         int64_t page_stride, int64_t pool_stride_h, const int32_t* pages, int32_t max_pages, int32_t n_pages,
                         int32_t H, aria_stream_t stream);
+/* aria_attention_prefill_shared_prefix whose prefix is read from pool pages (prefix caching): key 256 i + r of the prefix is row
+ * r of page pages[i] (pages: DEVICE int32 [n_pages_list]) of k_pool / v_pool [n_pages, H, 256, 128] (page_stride /
+ * pool_stride_h as aria_attention_decode_paged's).  P is a multiple of 256 with P / 256 <= n_pages_list; P = 0 is no prefix
+ * (then pages may be NULL), the varlen forward.  q, k, v, cu_seqlens, out, B, S_tot and the head strides as there.  Every
+ * output row is bit-identical to aria_attention_prefill_shared_prefix on a contiguous copy of the same prefix (P = 0:
+ * aria_attention_fwd_varlen).  A page entry outside [0, n_pages) reads zeros; packed rows at or past S_tot are never read.
+ * No workspace. */
+int aria_attention_prefill_paged_prefix(const void* q, const void* k, const void* v, const void* k_pool, const void* v_pool,
+                                        const int32_t* pages, int32_t n_pages_list, int32_t n_pages, const int32_t* cu_seqlens,
+                                        void* out, int32_t B, int32_t H, int32_t S_tot, int32_t P, int64_t q_stride_h,
+                                        int64_t kv_stride_h, int64_t page_stride, int64_t pool_stride_h, float scale,
+                                        aria_stream_t stream);
 /* aria_sample_tokens_rows with every sampling parameter per row, from DEVICE arrays [R]: temperature (0 = greedy), top_k, top_p,
  * seed (uint64), noise row and offset.  Row r is bit-identical to aria_sample_tokens run alone on that row with its scalars at
  * rng_offset = offsets[r] as row noise_rows[r].  The caller checks the parameters as aria_sample_tokens does; out-of-range
