@@ -128,6 +128,9 @@ SIGNATURES = {
     "aria_kv_pages_store": (i32, [vp, vp, i64, i32, vp, vp, i64, i64, vp, i32, i32, i32, vp]),
     "aria_attention_prefill_paged_prefix": (i32, [vp, vp, vp, vp, vp, vp, i32, i32, vp, vp, i32, i32, i32, i32, i64, i64, i64, i64,
                                                   f32, vp]),
+    "aria_attention_prefill_paged_varlen": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, vp, i32, i32, i32, i64, i64, i64, i64,
+                                                  f32, vp]),
+    "aria_kv_pages_store_varlen": (i32, [vp, vp, i64, i32, vp, vp, i64, i64, vp, i64, i32, i32, vp, vp, i32, i32, vp]),
     "aria_sample_tokens_slots": (i32, [vp, i64, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
     "aria_decode_advance_slots": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp]),
 }

@@ -19,6 +19,8 @@
 //
 // aria_attention_fwd_varlen: causal attention over sequences packed along one row (padding-free fine-tuning), on the
 //   shared-prefix prefill's pipeline with no prefix; each sequence bit-identical to aria_attention_fwd_lse on it alone.
+// aria_attention_prefill_paged_varlen: packed prompt segments, each after a paged prefix of its own (batched admission in the
+//   serving engine); each segment bit-identical to aria_attention_prefill_paged_prefix on it alone.
 //
 // aria_attention_decode: single-query attention against the KV cache; HBM-bound, CUDA cores, split-KV.
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
@@ -135,6 +137,16 @@ struct PagedPrefixParams {
   const int32_t* pages;  // [>= P / 256] device page list of the prefix
 };
 
+// Prefill of packed segments over paged prefixes of their own (aria_attention_prefill_paged_varlen): segment b is packed rows
+// [cu[b], cu[b + 1]) and attends to its prefix_lens[b] keys (a multiple of 256) in pages page_table[b * table_stride + i].
+struct PagedVarlenParams {
+  const int32_t* cu;           // [n_seg + 1] device segment starts
+  const int32_t* prefix_lens;  // [n_seg] device
+  const int32_t* page_table;   // [n_seg, table_stride] device
+  int64_t table_stride;
+  int n_seg;
+};
+
 // HD = head dim contracted by QK^T (80 for the 72-wide ViT heads, 128 for the LM); LSE: also store the row logsumexp
 // (what the backward needs to recompute P).  tmK16 / tmV16: 16-column SW32 boxes of columns 64-79 (HD = 80 only).
 // SHARED (HD = 128): the shared-prefix suffix prefill; the keys walk the prefix (tmPK / tmPV, rows [0, sp.P)) and then the
@@ -144,13 +156,19 @@ struct PagedPrefixParams {
 // PAGED (with SHARED): tmPK / tmPV map a page pool [n_pages, H, 256, 128] and prefix tile j (keys 128 j ..) is rows
 // 128 (j & 1) .. of page pages[j >> 1]; only the producer reads the page list.  The tiles, and so every row's arithmetic, are
 // those of the contiguous prefix.
-template <int HD, bool CAUSAL, bool LSE, bool SHARED, bool PAGED = false>
+// SEGS (with PAGED): every segment has a prefix of its own (PagedVarlenParams).  Query tiles do not cross segments: the
+// 128-query tiles of segment b are aligned at its start, and tile index q_tile counts the tiles of the segments before it, so
+// a CTA is the CTA of the same tile in aria_attention_prefill_paged_prefix run on segment b alone (n_seg = 1, its P and page
+// list) and computes the same arithmetic; the rows of its tile past the segment's end are not stored.  Tile indices past the
+// last tile (the grid is sized for an upper bound) exit at once.
+template <int HD, bool CAUSAL, bool LSE, bool SHARED, bool PAGED = false, bool SEGS = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                                               const CUtensorMap& tmK16, const CUtensorMap& tmV16, const CUtensorMap& tmPK,
                                               const CUtensorMap& tmPV, const AttnParams& p, const SharedPrefixParams& sp,
-                                              const int32_t* pages = nullptr) {
+                                              const int32_t* pages = nullptr, const PagedVarlenParams* vl = nullptr) {
   static_assert(!SHARED || (HD == 128 && !CAUSAL), "the shared-prefix prefill runs at head dim 128 with its own mask");
   static_assert(!PAGED || SHARED, "a paged prefix is a shared-prefix prefill");
+  static_assert(!SEGS || (PAGED && !LSE), "per-segment prefixes are paged");
   constexpr int S = AttnCfg<HD>::STAGES, KVT = AttnCfg<HD>::KV_TILE, NO = AttnCfg<HD>::NO;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -169,13 +187,30 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
   const int bh = blockIdx.x % BH;
   const int q_tile = p.n_q_tiles - 1 - blockIdx.x / BH;  // heaviest (latest rows) first
   const int b = bh / p.H, h = bh % p.H;
-  const int q0 = q_tile * AT_BM;
+  int q0 = q_tile * AT_BM;
+  int q_stop = p.Tq;  // rows at or past q_stop are not stored
+  [[maybe_unused]] SharedPrefixParams seg_sp{};
+  [[maybe_unused]] const int32_t* seg_pages = pages;
+  if constexpr (SEGS) {
+    int sg = 0, t = q_tile, c = vl->cu[0], e = vl->cu[1];
+    while (t >= (e - c + AT_BM - 1) / AT_BM) {
+      t -= (e - c + AT_BM - 1) / AT_BM;
+      if (++sg == vl->n_seg) return;  // past the last tile: the whole CTA leaves before any barrier
+      c = e;
+      e = vl->cu[sg + 1];
+    }
+    q0 = c + t * AT_BM;
+    q_stop = min(q0 + AT_BM, e);
+    seg_sp = SharedPrefixParams{vl->cu + sg, 1, vl->prefix_lens[sg]};
+    seg_pages = vl->page_table + sg * vl->table_stride;
+  }
+  const SharedPrefixParams& spx = SEGS ? seg_sp : sp;
   const int pos_off = p.Tk - p.Tq;
   int n_kv = (p.Tk + AT_BN - 1) / AT_BN;
   if (CAUSAL) n_kv = min(n_kv, (pos_off + min(q0 + AT_BM, p.Tq) - 1) / AT_BN + 1);
   SharedTileWalk walk;
   if constexpr (SHARED) {
-    walk.init(sp, q0, min(q0 + AT_BM, p.Tq));
+    walk.init(spx, q0, min(q0 + AT_BM, q_stop));
     n_kv = walk.count();
   }
 
@@ -218,7 +253,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
             // an entry outside the pool is an out-of-bounds box: TMA fills it with zeros
             if (walk.seg_c < 0) {
               row = (j & 1) * AT_BN;
-              page = pages[j >> 1];
+              page = seg_pages[j >> 1];
             }
           }
           mbar_wait(&k_empty[s], ph);
@@ -256,8 +291,8 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
   const uint8_t* km = p.key_mask ? p.key_mask + static_cast<int64_t>(b) * p.Tk : nullptr;
   int c_lo = 0, c_hi = 0;  // SHARED: segment starts of this thread's two rows
   if constexpr (SHARED) {
-    c_lo = sp.cu[packed_segment(sp.cu, sp.n_seg, r_lo)];
-    c_hi = sp.cu[packed_segment(sp.cu, sp.n_seg, r_lo + 8)];
+    c_lo = spx.cu[packed_segment(spx.cu, spx.n_seg, r_lo)];
+    c_hi = spx.cu[packed_segment(spx.cu, spx.n_seg, r_lo + 8)];
   }
   const uint32_t sQa = smem_u32(sQ) + cw * 64 * 128, sKa = smem_u32(sK), sVa = smem_u32(sV);
   const uint32_t my_turn = AT_BAR_TURN + cw, other_turn = AT_BAR_TURN + (cw ^ 1);
@@ -309,14 +344,14 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
     if constexpr (SHARED) {
       // prefix tile: -inf on rows at or past P; suffix tile: -inf unless the key is in the row's segment, at or before it
       const int k0 = walk.k0, sc_ = walk.seg_c;
-      if (sc_ >= 0 || k0 + AT_BN > sp.P) {
+      if (sc_ >= 0 || k0 + AT_BN > spx.P) {
 #pragma unroll
         for (int jj = 0; jj < 16; ++jj) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int kc = k0 + 8 * jj + kq + e;
-            if (sc_ < 0 ? kc >= sp.P : (sc_ != c_lo || kc > r_lo)) sc[4 * jj + e] = -INFINITY;
-            if (sc_ < 0 ? kc >= sp.P : (sc_ != c_hi || kc > r_lo + 8)) sc[4 * jj + 2 + e] = -INFINITY;
+            if (sc_ < 0 ? kc >= spx.P : (sc_ != c_lo || kc > r_lo)) sc[4 * jj + e] = -INFINITY;
+            if (sc_ < 0 ? kc >= spx.P : (sc_ != c_hi || kc > r_lo + 8)) sc[4 * jj + 2 + e] = -INFINITY;
           }
         }
       }
@@ -494,7 +529,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tmQ, const CUte
 #pragma unroll
   for (int hrow = 0; hrow < 2; ++hrow) {
     const int q = r_lo + 8 * hrow;
-    if (q >= p.Tq) continue;
+    if (q >= q_stop) continue;
     const float l = hrow ? l_hi : l_lo;
     const float inv_l = l > 0.f ? 1.0f / l : 0.f;
     __nv_bfloat16* orow = p.out + (static_cast<int64_t>(b) * p.Tq + q) * ld + h * p.out_hd;
@@ -533,6 +568,15 @@ attn_prefill_paged_prefix_kernel(const __grid_constant__ CUtensorMap tmQ, const 
                                  const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const PagedPrefixParams pp) {
   attn_fwd_body<128, false, false, true, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, SharedPrefixParams{pp.cu, pp.n_seg, pp.P},
                                                pp.pages);
+}
+
+// One CTA per (head, query tile of one segment): tmQ / tmK / tmV map the packed rows [1, H, S_tot, 128], tmPK / tmPV the
+// layer's page pools [n_pages, H, 256, 128]; p.n_q_tiles bounds the segments' tile count.
+__global__ void __launch_bounds__(AT_THREADS, 1)
+attn_prefill_paged_varlen_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                                 const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmPK,
+                                 const __grid_constant__ CUtensorMap tmPV, const AttnParams p, const PagedVarlenParams vl) {
+  attn_fwd_body<128, false, false, true, true, true>(tmQ, tmK, tmV, tmK, tmV, tmPK, tmPV, p, SharedPrefixParams{}, nullptr, &vl);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1210,6 +1254,48 @@ extern "C" int aria_attention_prefill_paged_prefix(const void* q, const void* k,
   attn_prefill_paged_prefix_kernel<<<H * n_q_tiles, AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
       tmQ, tmK, tmV, tmPK, tmPV, p, pp);
   return check_launch("attn_prefill_paged_prefix_kernel");
+}
+
+extern "C" int aria_attention_prefill_paged_varlen(const void* q, const void* k, const void* v, const void* k_pool,
+                                                   const void* v_pool, const int32_t* page_table, int64_t page_table_stride,
+                                                   int32_t n_pages, const int32_t* prefix_lens, const int32_t* cu_seqlens, void* out,
+                                                   int32_t n_seg, int32_t H, int32_t S_tot, int64_t q_stride_h, int64_t kv_stride_h,
+                                                   int64_t page_stride, int64_t pool_stride_h, float scale, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(q && k && v && k_pool && v_pool && page_table && prefix_lens && cu_seqlens && out);
+  ARIA_CHECK_ARG(n_seg > 0 && H > 0 && S_tot >= n_seg && n_pages > 0 && page_table_stride > 0);
+  ARIA_CHECK_ARG(q_stride_h >= static_cast<int64_t>(S_tot) * AT_D && kv_stride_h >= static_cast<int64_t>(S_tot) * AT_D);
+  ARIA_CHECK_ARG(pool_stride_h >= DEC_SPLIT_KEYS * AT_D && page_stride >= pool_stride_h * H);  // pages do not overlap
+  ARIA_CHECK_ARG(q_stride_h % 8 == 0 && kv_stride_h % 8 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  // each segment of len rows has ceil(len / 128) tiles <= (len + 127) / 128, and the lens sum to S_tot
+  const int64_t n_q_tiles = (static_cast<int64_t>(S_tot) + static_cast<int64_t>(AT_BM - 1) * n_seg) / AT_BM;
+  ARIA_CHECK_ARG(static_cast<int64_t>(H) * n_q_tiles < (1ll << 31) && static_cast<int64_t>(n_seg) * page_table_stride < (1ll << 31));
+  CUtensorMap tmQ, tmK, tmV, tmPK, tmPV;
+  int rc = make_tmap_heads(&tmQ, q, S_tot, H, 1, q_stride_h * H, q_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmK, k, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmV, v, S_tot, H, 1, kv_stride_h * H, kv_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPK, k_pool, DEC_SPLIT_KEYS, H, n_pages, page_stride, pool_stride_h);
+  if (rc) return rc;
+  rc = make_tmap_heads(&tmPV, v_pool, DEC_SPLIT_KEYS, H, n_pages, page_stride, pool_stride_h);
+  if (rc) return rc;
+  AttnParams p{};
+  p.B = 1;
+  p.H = H;
+  p.Tq = S_tot;
+  p.Tk = S_tot;
+  p.out_hd = AT_D;
+  p.scale_log2 = scale * 1.4426950408889634f;
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.n_q_tiles = static_cast<int>(n_q_tiles);
+  const PagedVarlenParams vl{cu_seqlens, prefix_lens, page_table, page_table_stride, n_seg};
+  constexpr int smem = AttnCfg<128>::SMEM;
+  static bool attr_set[kMaxDevices] = {};
+  if (ensure_dynamic_smem(attr_set, attn_prefill_paged_varlen_kernel, smem) != cudaSuccess) return ARIA_ERR_CUDA;
+  attn_prefill_paged_varlen_kernel<<<static_cast<int>(H * n_q_tiles), AT_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      tmQ, tmK, tmV, tmPK, tmPV, p, vl);
+  return check_launch("attn_prefill_paged_varlen_kernel");
 }
 
 extern "C" int aria_attention_fwd_varlen(const void* q, const void* k, const void* v, void* out, float* lse, const int32_t* cu_seqlens,

@@ -11,6 +11,7 @@
 // aria_kv_append_paged: kv_append into the page block_table[r, write_pos[r] / 256], row write_pos[r] % 256.  A negative
 //   write_pos, or one outside the row's mapped pages, writes nothing: idle and finished slots never touch another's pages.
 // aria_kv_pages_store: copies rows [0, T) of a one-row prefill cache into a request's pages.
+// aria_kv_pages_store_varlen: the same for packed segments, each into its own pages after its own prefix.
 // aria_decode_advance_slots: aria_decode_advance per slot: own output count, budget, RNG offset and finished flag.
 //
 // Prompt-lookup decoding (generate(prompt_lookup_num_tokens=K)): a step verifies Q = K + 1 tokens per row.
@@ -165,6 +166,24 @@ __global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_pages_store_kernel(const _
   const int j = threadIdx.x % KV_ROW_VECS;
   const uint4 x = reinterpret_cast<const uint4*>((is_v ? v : k) + h * src_sh + static_cast<int64_t>(t) * 128)[j];
   __nv_bfloat16* dst = (is_v ? vp : kp) + page * page_stride + h * pool_sh + static_cast<int64_t>(t % PAGE_ROWS) * 128;
+  reinterpret_cast<uint4*>(dst)[j] = x;
+}
+
+// One CTA per (packed row t, head h): row t of segment b is position P_b + t - cu[b] of its request
+__global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_pages_store_varlen_kernel(
+    const __nv_bfloat16* __restrict__ k, const __nv_bfloat16* __restrict__ v, int64_t src_sh, __nv_bfloat16* __restrict__ kp,
+    __nv_bfloat16* __restrict__ vp, int64_t page_stride, int64_t pool_sh, const int32_t* __restrict__ page_table,
+    int64_t table_stride, int max_pages, int n_pages, const int32_t* __restrict__ prefix_lens, const int32_t* __restrict__ cu,
+    int n_seg, int H) {
+  const int t = blockIdx.x / H, h = blockIdx.x % H;
+  const int b = packed_segment(cu, n_seg, t);
+  const int pos = prefix_lens[b] + t - cu[b];
+  const int page = page_of(page_table + b * table_stride, max_pages, n_pages, pos);
+  if (page <= 0) return;  // unmapped, outside the pool, or the null page
+  const bool is_v = threadIdx.x >= KV_ROW_VECS;
+  const int j = threadIdx.x % KV_ROW_VECS;
+  const uint4 x = reinterpret_cast<const uint4*>((is_v ? v : k) + h * src_sh + static_cast<int64_t>(t) * 128)[j];
+  __nv_bfloat16* dst = (is_v ? vp : kp) + page * page_stride + h * pool_sh + static_cast<int64_t>(pos % PAGE_ROWS) * 128;
   reinterpret_cast<uint4*>(dst)[j] = x;
 }
 
@@ -446,6 +465,23 @@ extern "C" int aria_kv_pages_store(const void* k, const void* v, int64_t src_str
       static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), src_stride_h, static_cast<__nv_bfloat16*>(k_pool),
       static_cast<__nv_bfloat16*>(v_pool), page_stride, pool_stride_h, pages, max_pages, n_pages, H);
   return check_launch("kv_pages_store_kernel");
+}
+
+extern "C" int aria_kv_pages_store_varlen(const void* k, const void* v, int64_t src_stride_h, int32_t S_tot, void* k_pool,
+                                          void* v_pool, int64_t page_stride, int64_t pool_stride_h, const int32_t* page_table,
+                                          int64_t page_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* prefix_lens,
+                                          const int32_t* cu_seqlens, int32_t n_seg, int32_t H, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k && v && k_pool && v_pool && page_table && prefix_lens && cu_seqlens);
+  ARIA_CHECK_ARG(S_tot >= n_seg && n_seg > 0 && H > 0 && n_pages > 0 && max_pages > 0 && page_table_stride >= max_pages);
+  ARIA_CHECK_ARG(static_cast<int64_t>(S_tot) * H < (1ll << 31) && src_stride_h >= static_cast<int64_t>(S_tot) * 128);
+  ARIA_CHECK_ARG(static_cast<int64_t>(n_seg) * page_table_stride < (1ll << 31));
+  ARIA_CHECK_ARG(pool_stride_h >= PAGE_ROWS * 128 && page_stride >= pool_stride_h * H);
+  ARIA_CHECK_ARG(src_stride_h % 8 == 0 && page_stride % 8 == 0 && pool_stride_h % 8 == 0);
+  kv_pages_store_varlen_kernel<<<S_tot * H, 2 * KV_ROW_VECS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), src_stride_h, static_cast<__nv_bfloat16*>(k_pool),
+      static_cast<__nv_bfloat16*>(v_pool), page_stride, pool_stride_h, page_table, page_table_stride, max_pages, n_pages,
+      prefix_lens, cu_seqlens, n_seg, H);
+  return check_launch("kv_pages_store_varlen_kernel");
 }
 
 extern "C" int aria_decode_advance_slots(const int64_t* next_ids, int64_t* ids_in, int32_t* out_tokens, int64_t out_stride,

@@ -736,18 +736,19 @@ class AriaAttention(nn.Module):
         ops.kv_scatter_tails(k, v, S, cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx], cu_seqlens, n)
         return self._o_proj(o.view(1, S, d), residual)
 
-    def prefill_paged(self, hidden_states, cache: PagedKVCache, rope, row, P, cu_seqlens, position_ids, residual=None, hq=None):
-        """The S prompt tokens after a P-token prefix held in pages (AriaMoELMModel.prefill_paged): the fused projection writes q,
-        k, v to a staging buffer (RoPE at position_ids), the tokens attend to the prefix pages row[: P / 256] and to themselves
-        (ops.attention_prefill_paged_prefix), and their k, v rows are stored into the pages row[P / 256:]."""
+    def prefill_paged(self, hidden_states, cache: PagedKVCache, rope, page_table, seg, position_ids, residual=None, hq=None):
+        """Packed prompt segments, each after a prefix held in its own pages (AriaMoELMModel.prefill_paged): the fused projection
+        writes q, k, v to a staging buffer (RoPE at position_ids), segment b attends to the pages page_table[b, : P_b / 256] and
+        causally to itself (ops.attention_prefill_paged_varlen), and its k, v rows are stored after its prefix in its pages
+        (ops.kv_pages_store_varlen)."""
         _, S, d = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
         stage = torch.empty(3, 1, H, S, hd, dtype=bf16, device=hidden_states.device)
         q, k, v = stage[0], stage[1], stage[2]
         self._qkv(hidden_states, hq, [q, k, v], S, 0, rope, position_ids)
         kp, vp = cache.k[self.layer_idx], cache.v[self.layer_idx]
-        o = ops.attention_prefill_paged_prefix(q, k, v, S, kp, vp, row, P, cu_seqlens, hd ** -0.5)
-        ops.kv_pages_store(k, v, S, kp, vp, row[P // PagedKVCache.PAGE_SIZE:])
+        o = ops.attention_prefill_paged_varlen(q, k, v, kp, vp, page_table, seg, hd ** -0.5)
+        ops.kv_pages_store_varlen(k, v, kp, vp, page_table, seg)
         return self._o_proj(o.view(1, S, d), residual)
 
 
@@ -807,10 +808,10 @@ class MoEDecoderLayer(nn.Module):
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
-    def prefill_paged(self, x, pending, cache, rope, row, P, cu_seqlens, position_ids):
-        """forward() for a prompt's tokens after a prefix held in pages (AriaAttention.prefill_paged)."""
+    def prefill_paged(self, x, pending, cache, rope, page_table, seg, position_ids):
+        """forward() for packed prompt segments, each after a prefix held in its pages (AriaAttention.prefill_paged)."""
         h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.prefill_paged(h, cache, rope, row, P, cu_seqlens, position_ids, residual=x, hq=hq)
+        x = self.self_attn.prefill_paged(h, cache, rope, page_table, seg, position_ids, residual=x, hq=hq)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
@@ -882,28 +883,33 @@ class AriaMoELMModel(nn.Module):
             x, pending = layer.prefill_suffixes(x, pending, cache, rope, cu_seqlens, position_ids)
         return x, pending
 
-    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, row, P, position_ids):
-        """Prefill the S prompt tokens that follow a P-token prefix whose keys and values are already in the pages of one
-        request (prefix caching, serving.Engine).  inputs_embeds [1, S, d]; row: the request's block-table row (CUDA int32
-        [max_pages]), whose first P / 256 pages hold the prefix (P a multiple of 256; 0 = no prefix); position_ids CUDA int32
-        [S], the RoPE positions P .. P + S - 1.  The tokens attend to the prefix and causally to themselves, and their keys and
-        values go to the pages row[P / 256:], as forward() on the whole prompt would have stored them.  Every row's output is
-        the one forward() gives that position on the whole prompt, bit for bit.  Returns (x, pending) as forward() does."""
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids):
+        """Prefill prompt segments packed along one row, each continuing a prefix whose keys and values are already in the
+        pages of its request (batched and chunked admission, prefix caching: serving.Engine).  inputs_embeds [1, S_tot, d]; seg:
+        an ops.PackedSegments, segment b = packed rows [seg.cu[b], seg.cu[b + 1]) after a prefix of seg.prefix_lens[b] tokens (a
+        multiple of 256; 0 = no prefix); page_table: CUDA int32 [n_seg, width], row b the pages of segment b's request (its first
+        P_b / 256 hold the prefix); position_ids CUDA int32 [S_tot], the RoPE positions P_b .. P_b + len_b - 1 of each segment.
+        Each segment attends to its prefix and causally to itself, and its keys and values go to its pages after the prefix, as
+        forward() on its whole prompt would have stored them.  Every row's output is the one forward() gives that position on
+        its own prompt, bit for bit: attention keeps the segments apart and the rest of a layer computes each row on its own.
+        n_seg = 1 is one request's prefill.  Returns (x, pending) as forward() does."""
         if not isinstance(cache, PagedKVCache):
             raise ValueError("prefill_paged needs a PagedKVCache")
-        if inputs_embeds.dim() != 3 or inputs_embeds.shape[0] != 1 or inputs_embeds.shape[1] < 1:
-            raise ValueError(f"prefill_paged: inputs_embeds must be [1, S >= 1, d], got {tuple(inputs_embeds.shape)}")
-        S = inputs_embeds.shape[1]
-        max_pages = row.numel()
-        if not isinstance(P, int) or P < 0 or P % cache.PAGE_SIZE or P + S > max_pages * cache.PAGE_SIZE:
-            raise ValueError(f"prefill_paged: P = {P!r} must be a multiple of {cache.PAGE_SIZE} and P + {S} tokens must fit "
-                             f"{max_pages} pages")
-        dev = inputs_embeds.device
-        rope = self.rope_tables(cache.block_table.shape[1] * cache.PAGE_SIZE, dev)
-        cu = torch.tensor([0, S], dtype=torch.int32).to(dev, non_blocking=True)
+        if not isinstance(seg, ops.PackedSegments):
+            raise ValueError("prefill_paged: seg must be an ops.PackedSegments")
+        if inputs_embeds.dim() != 3 or inputs_embeds.shape[0] != 1 or inputs_embeds.shape[1] != seg.S_tot:
+            raise ValueError(f"prefill_paged: inputs_embeds must be [1, {seg.S_tot}, d], got {tuple(inputs_embeds.shape)}")
+        if position_ids.shape != (seg.S_tot,):
+            raise ValueError(f"prefill_paged: position_ids must be [{seg.S_tot}], got {tuple(position_ids.shape)}")
+        width = page_table.shape[-1]
+        for b, P in enumerate(seg.prefix_lens):
+            if P + seg.cu[b + 1] - seg.cu[b] > width * cache.PAGE_SIZE:
+                raise ValueError(f"prefill_paged: segment {b} (P = {P}, {seg.cu[b + 1] - seg.cu[b]} tokens) does not fit {width} "
+                                 "pages")
+        rope = self.rope_tables(cache.block_table.shape[1] * cache.PAGE_SIZE, inputs_embeds.device)
         x, pending = inputs_embeds, None
         for layer in self.layers:
-            x, pending = layer.prefill_paged(x, pending, cache, rope, row, P, cu, position_ids)
+            x, pending = layer.prefill_paged(x, pending, cache, rope, page_table, seg, position_ids)
         return x, pending
 
 
@@ -957,11 +963,21 @@ class AriaMoELMForCausalLM(nn.Module):
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h), cache
 
-    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, row, P, position_ids):
-        """AriaMoELMModel.prefill_paged, then the final norm and lm_head on the last row -> logits [1, 1, V], those of
-        forward(num_logits_to_keep=1) on the whole prompt."""
-        x, pending = self.model.prefill_paged(inputs_embeds, cache, row, P, position_ids)
-        h, _ = self.model.norm(x[:, -1:, :].contiguous(), residual=pending[:, -1:, :].contiguous())
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None):
+        """AriaMoELMModel.prefill_paged, then the final norm and lm_head on the last row of each segment listed in `ends`
+        (segment indices in increasing order, the segments that end a prompt; None = every segment) -> logits [1, len(ends), V],
+        row i those of forward(num_logits_to_keep=1) on the whole prompt of segment ends[i]."""
+        x, pending = self.model.prefill_paged(inputs_embeds, cache, page_table, seg, position_ids)
+        ends = range(seg.n_seg) if ends is None else ends
+        rows = [seg.cu[b + 1] - 1 for b in ends]
+        if not rows:                                         # only chunks that end no prompt: no logits
+            return x.new_empty((1, 0, self.vocab_size))
+        if rows == list(range(seg.S_tot - len(rows), seg.S_tot)):
+            x, pending = x[:, -len(rows):, :].contiguous(), pending[:, -len(rows):, :].contiguous()
+        else:
+            idx = torch.tensor(rows, dtype=torch.int64).to(x.device, non_blocking=True)
+            x, pending = x.index_select(1, idx), pending.index_select(1, idx)
+        h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h)
 
     def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):

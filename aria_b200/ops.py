@@ -1481,6 +1481,89 @@ def attention_prefill_paged_prefix(q: torch.Tensor, k: torch.Tensor, v: torch.Te
     return out
 
 
+class PackedSegments:
+    """n_seg prompt segments packed along one row, each after a paged prefix of its own: segment b is packed rows
+    [cu[b], cu[b + 1]) and follows prefix_lens[b] cached keys (a multiple of 256).  Holds the host lists, which the ops below
+    check before they launch, and one device int32 copy of both (cu_dev [n_seg + 1], prefix_dev [n_seg]), which the kernels
+    read.  Every segment has at least one row."""
+
+    def __init__(self, cu, prefix_lens, device):
+        cu, P = [int(c) for c in cu], [int(p) for p in prefix_lens]
+        if len(cu) < 2 or cu[0] != 0 or any(b <= a for a, b in zip(cu, cu[1:])) or len(P) != len(cu) - 1:
+            raise ValueError(f"PackedSegments: cu must increase from 0 with one prefix length per segment, got {cu} and {P}")
+        if any(p < 0 or p % 256 for p in P):
+            raise ValueError(f"PackedSegments: prefix lengths must be multiples of 256, got {P}")
+        self.cu, self.prefix_lens = cu, P
+        dev = torch.tensor(cu + P, dtype=torch.int32).pin_memory().to(device, non_blocking=True)
+        self.cu_dev, self.prefix_dev = dev[:len(cu)], dev[len(cu):]
+
+    @property
+    def n_seg(self) -> int:
+        return len(self.prefix_lens)
+
+    @property
+    def S_tot(self) -> int:
+        return self.cu[-1]
+
+
+def _page_table_check(page_table: torch.Tensor, seg: PackedSegments, rows_after_prefix: bool, what: str):
+    """page_table: CUDA int32 [n_seg, width] with contiguous rows; every prefix (and, rows_after_prefix, the segment's rows after
+    it) fits the width's pages."""
+    if not (page_table.is_cuda and page_table.dtype == torch.int32 and page_table.dim() == 2 and page_table.stride(1) == 1
+            and page_table.shape[0] == seg.n_seg and page_table.shape[1] >= 1 and page_table.data_ptr() % 4 == 0):
+        raise RuntimeError(f"{what}: page_table must be CUDA int32 [{seg.n_seg}, width] with contiguous rows")
+    W = page_table.shape[1]
+    for b, P in enumerate(seg.prefix_lens):
+        end = P + (seg.cu[b + 1] - seg.cu[b] if rows_after_prefix else 0)
+        if end > 256 * W:
+            raise ValueError(f"{what}: segment {b} needs {-(-end // 256)} pages; its page_table row lists {W}")
+
+
+def attention_prefill_paged_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
+                                   page_table: torch.Tensor, seg: PackedSegments, scale: float) -> torch.Tensor:
+    """attention_prefill_paged_prefix with a prefix per segment: q / k / v [1, H, >= seg.S_tot, 128] hold the packed segments
+    (seg), segment b attends to its seg.prefix_lens[b] keys, key 256 i + r at row r of page page_table[b, i] (CUDA int32
+    [n_seg, width]) of the pools [n_pages, H, 256, 128], and causally to its own rows -> out [S_tot, H*128].  Every row of segment
+    b is bit-identical to attention_prefill_paged_prefix on that segment alone, with its own page list and P.  A page entry
+    outside the pool reads zeros.  See aria_attention_prefill_paged_varlen."""
+    what = "attention_prefill_paged_varlen"
+    _attn_qkv_check(q, k, v, what)
+    _paged_pool_check(k_pool, v_pool, what)
+    S_tot, H = seg.S_tot, q.shape[1]
+    if q.shape[0] != 1 or q.shape[2] < S_tot or k.shape[:2] != (1, H) or k.shape[2] < S_tot or v.shape != k.shape:
+        raise ValueError(f"{what}: q {tuple(q.shape)} / k {tuple(k.shape)} must be [1, H, >= {S_tot}, 128]")
+    if k_pool.shape[1] != H:
+        raise ValueError(f"{what}: pools {tuple(k_pool.shape)} do not have the {H} heads of q")
+    _page_table_check(page_table, seg, False, what)
+    out = torch.empty((S_tot, H * 128), dtype=bf16, device=q.device)
+    with torch.cuda.device(q.device):
+        L.check(L.load().aria_attention_prefill_paged_varlen(_p(q), _p(k), _p(v), _p(k_pool), _p(v_pool), _p(page_table),
+                                                             page_table.stride(0), k_pool.shape[0], _p(seg.prefix_dev),
+                                                             _p(seg.cu_dev), _p(out), seg.n_seg, H, S_tot, q.stride(1), k.stride(1),
+                                                             k_pool.stride(0), k_pool.stride(1), scale, _stream(q)), what)
+    return out
+
+
+def kv_pages_store_varlen(k: torch.Tensor, v: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, page_table: torch.Tensor,
+                          seg: PackedSegments):
+    """kv_pages_store for packed segments: row t of segment b of k / v [1, H, >= S_tot, 128] (bf16, contiguous) is position
+    p = prefix_lens[b] + t - cu[b] of its request and goes to row p % 256 of page page_table[b, p // 256].  Writes nothing outside
+    the listed pages and never the null page 0; each segment's pages are those kv_pages_store gives it alone.
+    See aria_kv_pages_store_varlen."""
+    what = "kv_pages_store_varlen"
+    _paged_pool_check(k_pool, v_pool, what)
+    _chk(k), _chk(v)
+    H, S_tot = k_pool.shape[1], seg.S_tot
+    if k.dim() != 4 or k.shape[0] != 1 or k.shape[1] != H or k.shape[3] != 128 or v.shape != k.shape or k.shape[2] < S_tot:
+        raise ValueError(f"{what}: k {tuple(k.shape)} must be [1, {H}, >= {S_tot}, 128] like v")
+    _page_table_check(page_table, seg, True, what)
+    with torch.cuda.device(k_pool.device):
+        L.check(L.load().aria_kv_pages_store_varlen(_p(k), _p(v), k.stride(1), S_tot, _p(k_pool), _p(v_pool), k_pool.stride(0),
+                                                    k_pool.stride(1), _p(page_table), page_table.stride(0), page_table.shape[1],
+                                                    k_pool.shape[0], _p(seg.prefix_dev), _p(seg.cu_dev), seg.n_seg, H,
+                                                    _stream(k_pool)), what)
+
+
 def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
                         seed: torch.Tensor, noise_rows: torch.Tensor, offsets: torch.Tensor,
                         out: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -1,18 +1,22 @@
 """Continuous batching: an engine that admits and retires generation requests between graph-replayed decode steps.
 
-    eng = Engine(model, max_batch=64, max_kv_tokens=131072, eos_token_id=None, pad_token_id=None, poll_every=8)
+    eng = Engine(model, max_batch=64, max_kv_tokens=131072, eos_token_id=None, pad_token_id=None, poll_every=8,
+                 max_prefill_tokens=8192)
     rid = eng.add_request(input_ids, pixel_values=None, pixel_mask=None, max_new_tokens=16,
                           do_sample=False, temperature=1.0, top_k=50, top_p=1.0, seed=0)
-    done = eng.step()   # decode replays up to the next poll, retire, admit -> {rid: ids}
+    done = eng.step()   # decode replays up to the next poll, retire, admit and prefill -> {rid: ids}
     out = eng.run()     # until every request has finished -> {rid: ids}
 
 Every request's result equals model.generate(ids[None], pixel_values, pixel_mask, max_new_tokens=m, <its sampling arguments>,
 eos_token_id=E, pad_token_id=P)[0] bit for bit: the prompt ids, then the generated tokens up to and including the first EOS.
 It does not depend on max_batch, poll_every, when the request arrived, its slot or the other requests, because
 
-  - admission is generate()'s batch-1 prefill (the ViT, then the prompt through every layer) written straight into the
+  - admission is generate()'s prefill of the prompt (the ViT, then the prompt through every layer) written straight into the
     request's pages (moe_lm.AriaMoELMForCausalLM.prefill_paged), and its first token comes from its own sampling parameters
-    at RNG offset 0;
+    at RNG offset 0.  Several requests' prompts are packed into one prefill launch, and a long prompt is split into chunks
+    that end at multiples of 256 of its position; attention keeps every packed segment to its own pages
+    (ops.attention_prefill_paged_varlen: each segment exactly the one-request kernel), a later chunk reads the earlier ones
+    as a page-aligned prefix, and the rest of a layer computes each row on its own;
   - a decode step reads every row's keys from its own pages with the arithmetic of the contiguous decode kernel
     (ops.attention_decode_paged: a page is one split), samples each row with its own parameters, noise row 0 and offset =
     tokens emitted (ops.sample_tokens_slots), and the other kernels of the step compute each row on its own.
@@ -33,6 +37,15 @@ token's logits.  A page's keys and values do not depend on what follows it in th
 attends to 256-key-aligned pages with the tile order of a prefill of the whole prompt, so a hit changes no result bit.
 Pages written by decode steps are never keyed: their keys and values come from the decode arithmetic, not the prefill's.
 
+Batched and chunked admission: each step() prefills at most max_prefill_tokens prompt tokens past the cached prefixes (None:
+no limit), so a long prompt delays the running requests' decode by a bounded prefill, and short prompts share one pass over
+the expert weights.  It first continues the partly prefilled request, if any, then admits FIFO as before and packs the
+admitted requests' chunks into one launch.  A chunk that does not fit what is left of the budget ends at the last multiple
+of 256 of its absolute position the budget reaches (never a piece under 256 tokens but a prompt's last one), and admission
+stops there, so at most one request is partly prefilled.  It holds its slot and pages, its slot stays idle on the null page,
+no poll retires it, and its first token is sampled after its last chunk.  Pages are keyed as their chunk is staged; a head
+whose hit would read a page of a launch not yet run waits for that launch, so the hits are those of one-at-a-time admission.
+
 The scheduler (Scheduler, PageAllocator) and the page keys are plain host code with no device calls.  GPU only; bf16 KV pages; no expert
 parallelism.  Fp8 or bf16 expert and dense weights are fine (they live inside the layers).
 """
@@ -50,6 +63,7 @@ from . import ops
 
 PAGE = 256
 MAX_BATCH = 1024   # the slot advance runs one thread per slot in one CTA
+DEFAULT_PREFILL_TOKENS = 8192
 
 
 def _pages_for(tokens: int) -> int:
@@ -195,6 +209,13 @@ class PageAllocator:
         self._page_of[key] = page
         self._key_of[page] = key
 
+    def unregister(self, pages) -> None:
+        """Drop the keys of these pages: their prefill failed, so what they hold is not known."""
+        for p in pages:
+            key = self._key_of.pop(p, None)
+            if key is not None:
+                del self._page_of[key]
+
 
 @dataclass
 class Request:
@@ -207,6 +228,10 @@ class Request:
     pages: List[int] = field(default_factory=list)
     keys: List[bytes] = field(default_factory=list)    # page_keys of the prompt's full pages
     prefix_len: int = 0                                 # prompt tokens found in cached pages at admission (a multiple of 256)
+    chunk: tuple = (0, 0)                               # prompt positions [start, end) of its newest planned prefill chunk
+    feats: Optional[torch.Tensor] = None                # image features of pixel rows [feat_row, vit_rows) not merged yet
+    feat_row: int = 0
+    vit_rows: int = 0                                   # pixel rows the ViT has run on (rows inside the hit count as run)
 
     @property
     def n_pages(self) -> int:
@@ -221,13 +246,20 @@ class Scheduler:
     Prefix caching: admission first follows the head's page keys through the cache, at most floor((T - 1) / 256) pages (the
     prompt's last token is always prefilled); the hit pages come first in req.pages and req.prefix_len = 256 x hits.  The
     head is admitted when a slot is free and its other pages fit the free pages that are not among its hits.  register(req),
-    after a successful admission, keys its full prompt pages that are not cached yet."""
+    after a successful admission, keys its full prompt pages that are not cached yet, up to the end of its planned prefill.
+    Chunked admission: an admitted request's prompt past its hit is planned as one chunk, req.chunk = (prefix_len, T); plan()
+    cuts it to a step's budget of prompt tokens at a multiple of 256 of its absolute position, so the next chunk's prefix is
+    page-aligned, and the request stays `partial` until a chunk ends at T.  Admission is FIFO and stops at a partial request,
+    so at most one is partly prefilled; it holds its slot and pages meanwhile.  Pages keyed from chunks that are staged but not
+    launched yet are in `unlaunched`: a head that would hit one must wait for that launch (head_waits)."""
 
     def __init__(self, max_batch: int, n_pages: int):
         self.max_batch = max_batch
         self.pages = PageAllocator(n_pages)
         self.queue: collections.deque = collections.deque()
         self.slots: List[Request] = []
+        self.partial: Optional[Request] = None
+        self.unlaunched: set = set()
 
     @property
     def n_active(self) -> int:
@@ -243,7 +275,7 @@ class Scheduler:
         if not (self.queue and len(self.slots) < self.max_batch):
             return None
         req = self.queue[0]
-        hits = self.pages.lookup(req.keys[:(req.input_ids.numel() - 1) // PAGE])
+        hits = self._head_hits()
         idle_hits = sum(1 for p in hits if self.pages.refs(p) == 0)
         if req.n_pages - len(hits) > self.pages.n_free - idle_hits:
             return None
@@ -251,14 +283,50 @@ class Scheduler:
         self.pages.hold(hits)                     # before alloc, which may evict idle cached pages
         req.pages = hits + self.pages.alloc(req.n_pages - len(hits))
         req.prefix_len = PAGE * len(hits)
+        req.chunk = (req.prefix_len, req.input_ids.numel())
         self.slots.append(req)
         return len(self.slots) - 1, req
 
+    def _head_hits(self) -> List[int]:
+        req = self.queue[0]
+        return self.pages.lookup(req.keys[:(req.input_ids.numel() - 1) // PAGE])
+
     def register(self, req: Request) -> None:
-        """Key req's full prompt pages that are not cached yet (their prefill is in flight on the admission stream, so a
-        later admission on that stream reads them finished)."""
-        for page, key in zip(req.pages, req.keys):
+        """Key req's full prompt pages that are not cached yet and lie before the end of its planned prefill (their prefill is
+        staged or in flight on the admission stream, so a later launch on that stream reads them finished).  The pages of its
+        newest chunk join `unlaunched`."""
+        start, end = req.chunk
+        for i, (page, key) in enumerate(zip(req.pages[:end // PAGE], req.keys)):
             self.pages.register(page, key)
+            if i >= start // PAGE:
+                self.unlaunched.add(page)
+
+    @staticmethod
+    def chunk_end(T: int, start: int, budget: Optional[int]) -> int:
+        """End of the chunk of a T-token prompt that starts at `start` (a multiple of 256) within `budget` prompt tokens (None:
+        no limit): T when the rest fits, else the last multiple of 256 the budget reaches; `start` when not one page fits."""
+        if budget is None or T - start <= budget:
+            return T
+        return max(start, (start + budget) // PAGE * PAGE)
+
+    def head_fits(self, budget: Optional[int]) -> bool:
+        """Whether the queue's head, admitted now, would get a chunk within `budget`."""
+        req = self.queue[0]
+        start = PAGE * len(self._head_hits())
+        return self.chunk_end(req.input_ids.numel(), start, budget) > start
+
+    def head_waits(self) -> bool:
+        """Whether the queue's head would hit a page whose prefill is staged but not launched yet: launch it first."""
+        return bool(self.queue) and any(p in self.unlaunched for p in self._head_hits())
+
+    def plan(self, req: Request, start: int, budget: Optional[int]) -> int:
+        """Plan req's next chunk from prompt position `start` within `budget` -> its token count; req becomes (or stays)
+        `partial` unless the chunk reaches the end of its prompt."""
+        T = req.input_ids.numel()
+        end = self.chunk_end(T, start, budget)
+        req.chunk = (start, end)
+        self.partial = req if end < T else None
+        return end - start
 
     def admit(self) -> List[tuple]:
         """-> [(slot, request)] admitted, in FIFO order, their pages reserved."""
@@ -269,6 +337,8 @@ class Scheduler:
 
     def retire(self, s: int) -> Optional[tuple]:
         req = self.slots[s]
+        if req is self.partial:
+            self.partial = None
         self.pages.free(req.pages)
         req.pages = []
         last = len(self.slots) - 1
@@ -291,13 +361,22 @@ class Engine:
     output row per slot as long as the pool, since a request may spend the whole pool on its budget: 4 x max_batch x
     256 ceil(max_kv_tokens / 256) bytes (32 MiB at the defaults, 4 GiB at 1024 slots and a 2^20-token pool).
     `stats`: graphs captured, decode steps replayed, slot-steps of active requests (mean occupancy = active_slot_steps /
-    (steps * max_batch)), host seconds spent waiting in polls; prefix caching: prompt tokens admitted, those found in cached
-    pages (prefix_hit_tokens), pixel rows the ViT ran on and skipped, cached pages evicted.  `times[rid]`: host clock (time.perf_counter) when its first
-    token and its last token were known done (first poll after admission, poll that saw it finish)."""
+    (steps * max_batch); a partly prefilled request is not counted), host seconds spent waiting in polls; prefix caching: prompt tokens admitted, those found in cached
+    pages (prefix_hit_tokens), pixel rows the ViT ran on and skipped, cached pages evicted; admission: packed prefills run
+    (prefill_launches) and the segments among them that did not end a prompt (prefill_chunks).
+    max_prefill_tokens: the most prompt tokens one step() prefills (a multiple of 256; None = no limit; cached prefix tokens do
+    not count), so that a long admission delays the running requests' decode steps by a bounded prefill.
+    `times[rid]`: host clock (time.perf_counter) when its first token and its last token were known done (first poll after
+    its prompt was prefilled, poll that saw it finish)."""
+
+    max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS
 
     def __init__(self, model, max_batch: int = 64, max_kv_tokens: int = 131072, eos_token_id=None, pad_token_id=None,
-                 poll_every: int = 8):
+                 poll_every: int = 8, max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS):
         from .moe_lm import PagedKVCache, SlotDecodeState
+        if max_prefill_tokens is not None and (not isinstance(max_prefill_tokens, int) or max_prefill_tokens < PAGE
+                                               or max_prefill_tokens % PAGE):
+            raise ValueError(f"max_prefill_tokens must be None or a positive multiple of {PAGE}, got {max_prefill_tokens!r}")
         if not isinstance(max_batch, int) or max_batch < 1:
             raise ValueError(f"max_batch must be a positive int, got {max_batch!r}")
         if max_batch > MAX_BATCH:
@@ -312,7 +391,7 @@ class Engine:
         if getattr(model, "_ep_transport", None) is not None:
             raise NotImplementedError("Engine: expert parallelism is not supported")
         self.model, self.dev = model, dev
-        self.max_batch, self.poll_every = max_batch, poll_every
+        self.max_batch, self.poll_every, self.max_prefill_tokens = max_batch, poll_every, max_prefill_tokens
         self.eos, self.pad = eos, pad
         lm = model.language_model
         c = lm.config
@@ -332,7 +411,8 @@ class Engine:
         self._undelivered: Dict[int, torch.Tensor] = {}
         self._first_seen = set()
         self.stats = {"graphs_captured": 0, "steps": 0, "active_slot_steps": 0, "poll_host_s": 0.0, "polls": 0,
-                      "prompt_tokens": 0, "prefix_hit_tokens": 0, "vit_rows_run": 0, "vit_rows_skipped": 0, "pages_evicted": 0}
+                      "prompt_tokens": 0, "prefix_hit_tokens": 0, "vit_rows_run": 0, "vit_rows_skipped": 0, "pages_evicted": 0,
+                      "prefill_launches": 0, "prefill_chunks": 0}
         self.times: Dict[int, list] = {}
 
     # ------------------------------------------------------------------------------------------------ public API
@@ -365,31 +445,55 @@ class Engine:
         return len(self.sched.queue)
 
     def step(self) -> Dict[int, torch.Tensor]:
-        """Replay the decode step poll_every times over the active slots, poll, retire the finished requests, admit what fits
-        -> {rid: result [T + generated] int64 on the model's device} of the requests that finished.
-        A request whose admission raises (e.g. pixel inputs that do not match its image tokens, or running out of memory in its
-        prefill) is dropped, its slot and pages freed, and the error reaches the caller; the requests behind it stay queued,
-        and the results this call had retired come with the next call."""
+        """Replay the decode step poll_every times over the active slots, poll, retire the finished requests (neither when the
+        only active request is the partly prefilled one), then prefill up
+        to max_prefill_tokens prompt tokens -> {rid: result [T + generated] int64 on the model's device} of the requests that
+        finished.  The prefill first continues the partly prefilled request, if any, then admits FIFO what fits (a slot and all
+        its pages), and packs their chunks into as few packed prefills as it can (a head that would hit a page of a prefill
+        not launched yet waits for that launch).  A request whose admission raises (e.g. pixel inputs that do not match its
+        image tokens) is dropped, its slot and pages freed, after the requests packed ahead of it are prefilled, and the error
+        reaches the caller; a device error in a packed prefill drops every request of that launch and unkeys the pages it was to
+        write.  The requests behind stay queued, and the results this call had retired come with the next call."""
         done, self._undelivered = self._undelivered, {}
-        if self.sched.n_active:
+        decoding = self.sched.n_active - (self.sched.partial is not None)    # a partly prefilled request's slot is idle
+        if decoding:
             g = self._graph(_pow2_at_least(self.sched.n_active, self.max_batch),
                             _pow2_at_least(self.sched.width(), self.max_pages))
             for _ in range(self.poll_every):
                 g.replay()
             self.stats["steps"] += self.poll_every
-            self.stats["active_slot_steps"] += self.poll_every * self.sched.n_active
-        if self.sched.n_active:
+            self.stats["active_slot_steps"] += self.poll_every * decoding
             done.update(self._poll_and_retire())
-        while (a := self.sched.admit_one()) is not None:
-            s, req = a
-            try:
-                self._admit(s, req)
-            except BaseException:
-                self.sched.retire(s)                       # the last slot: nothing moves
-                self._idle(s, s + 1)
-                self._undelivered = done
-                raise
-            self.sched.register(req)
+        sched, budget = self.sched, self.max_prefill_tokens
+        self._staged = []
+        try:
+            if (req := sched.partial) is not None:
+                n = sched.plan(req, req.chunk[1], budget)
+                budget = None if budget is None else budget - n
+                self._staged.append(req)
+                sched.register(req)
+            while sched.partial is None and sched.queue and (budget is None or budget > 0):
+                if sched.head_waits():
+                    self._launch()
+                if not sched.head_fits(budget):
+                    break
+                a = sched.admit_one()
+                if a is None:
+                    break
+                s, req = a
+                n = sched.plan(req, req.prefix_len, budget)
+                try:
+                    self._admit(s, req)
+                except BaseException:
+                    self._launch()                             # the requests packed ahead of it
+                    self._drop(sched.slots.index(req))
+                    raise
+                budget = None if budget is None else budget - n
+                sched.register(req)
+            self._launch()
+        except BaseException:
+            self._undelivered = done
+            raise
         return done
 
     def run(self) -> Dict[int, torch.Tensor]:
@@ -451,49 +555,116 @@ class Engine:
         return g
 
     def _admit(self, s: int, req: Request) -> None:
-        """generate()'s batch-1 prefill of the prompt past its cached prefix (req.prefix_len tokens, 0 on a miss), written into
-        the request's pages, then slot s's state and its first token (sampled at offset 0 and recorded by the slot advance, as
-        generate() records its first token).
-
-        Image features are merged from the first uncached image token on: the ViT and the projector run on the pixel rows from
-        the first one with a token at or past the prefix, and each pixel row's features do not depend on the rows that share
-        its launch."""
-        m, lm = self.model, self.model.language_model
+        """Admit req into slot s: forward()'s image-token check, on the host and before any device work, then its first chunk
+        (req.chunk, from its cached prefix on) joins the packed prefill being staged."""
+        m = self.model
         ids, P = req.input_ids, req.prefix_len
-        T = ids.numel()
-        pv, pm = req.pixel_values, req.pixel_mask
+        pv = req.pixel_values
         if pv is not None:
-            # forward()'s image-token check, on the host and before any device work: pixel rows x queries per row
-            cfg = m.config
-            n_patch = (pv.shape[-1] // cfg.vision_config.patch_size) ** 2
-            n_query = cfg.projector_patch_to_query_dict.get(n_patch)
-            assert n_query is not None, f"Query number for {n_patch} patches is not provided"
-            img = (ids == cfg.image_token_index).nonzero().flatten()
-            if img.numel() != pv.shape[0] * n_query:
-                raise ValueError(f"Image features and image tokens do not match: tokens: {img.numel()}, features "
+            # forward()'s image-token check: pixel rows x queries per row
+            n_query = self._queries_per_row(pv)
+            n_img = int((ids == m.config.image_token_index).sum())
+            if n_img != pv.shape[0] * n_query:
+                raise ValueError(f"Image features and image tokens do not match: tokens: {n_img}, features "
                                  f"{pv.shape[0] * n_query}")
-        row = torch.full((self.max_pages,), -1, dtype=torch.int32)
-        row[:len(req.pages)] = torch.tensor(req.pages, dtype=torch.int32)
-        bt = self.cache.block_table[s]
-        bt.copy_(row)
-        ids_dev = ids[P:].to(self.dev, non_blocking=True)
-        emb = ops.embedding(ids_dev[None], lm.get_input_embeddings().weight)
-        if pv is not None:
-            k0 = int((img < P).sum())                  # image tokens inside the cached prefix
-            r0 = k0 // n_query                         # first pixel row with a token at or past P
-            if r0 < pv.shape[0]:
-                pix = pv[r0:].to(self.dev, non_blocking=True).to(torch.bfloat16)
-                feats, image_attn_mask = m.vision_tower(pix, None if pm is None else pm[r0:])
-                feats = m.multi_modal_projector(feats, image_attn_mask)
-                ops.merge_image_features(ids_dev, m.config.image_token_index,
-                                         feats.reshape(-1, feats.shape[-1])[k0 - r0 * n_query:], emb.view(-1, emb.shape[-1]))
-            self.stats["vit_rows_run"] += pv.shape[0] - r0
-            self.stats["vit_rows_skipped"] += r0
-        pos = torch.arange(P, T, dtype=torch.int32, device=self.dev)
-        logits = lm.prefill_paged(emb, self.cache, bt, P, pos)
-        self.stats["prompt_tokens"] += T
+            k0 = int((ids[:P] == m.config.image_token_index).sum())     # image tokens inside the cached prefix
+            req.vit_rows = req.feat_row = k0 // n_query                 # pixel rows wholly inside it are never run
+            self.stats["vit_rows_skipped"] += req.vit_rows
+        self.stats["prompt_tokens"] += ids.numel()
         self.stats["prefix_hit_tokens"] += P
         self.stats["pages_evicted"] = self.sched.pages.n_evicted
+        self._staged.append(req)
+
+    def _queries_per_row(self, pv) -> int:
+        cfg = self.model.config
+        n_patch = (pv.shape[-1] // cfg.vision_config.patch_size) ** 2
+        n_query = cfg.projector_patch_to_query_dict.get(n_patch)
+        assert n_query is not None, f"Query number for {n_patch} patches is not provided"
+        return n_query
+
+    def _launch(self) -> None:
+        """One packed prefill of the staged chunks (AriaMoELMForCausalLM.prefill_paged), each written into its request's pages;
+        then, for each request whose prompt it completes, slot state and its first token (sampled at offset 0 and recorded by
+        the slot advance, as generate() records its first token).  Nothing staged: no device work."""
+        staged, self._staged = self._staged, []
+        keyed, self.sched.unlaunched = self.sched.unlaunched, set()
+        if not staged:
+            return
+        try:
+            self._prefill(staged)
+        except BaseException:
+            # the pages this launch was to write were keyed when their chunks were staged; no other request holds them
+            # (head_waits), and their contents are now unknown, so they must not stay in the cache as their requests retire
+            self.sched.pages.unregister(keyed)
+            for s in sorted((self.sched.slots.index(r) for r in staged), reverse=True):
+                self._drop(s)
+            raise
+
+    def _prefill(self, staged: List[Request]) -> None:
+        lm = self.model.language_model
+        cu, starts, ends = [0], [], []
+        for req in staged:
+            start, end = req.chunk
+            cu.append(cu[-1] + end - start)
+            starts.append(start)
+            if end == req.input_ids.numel():
+                ends.append(len(starts) - 1)
+        ids = torch.cat([r.input_ids[r.chunk[0]:r.chunk[1]] for r in staged])
+        pos = torch.cat([torch.arange(r.chunk[0], r.chunk[1], dtype=torch.int32) for r in staged])
+        width = max(len(r.pages) for r in staged)
+        table = torch.full((len(staged), width), -1, dtype=torch.int32)
+        for b, r in enumerate(staged):
+            table[b, :len(r.pages)] = torch.tensor(r.pages, dtype=torch.int32)
+        host = torch.cat([ids, pos.to(torch.int64), table.flatten().to(torch.int64)]).pin_memory()
+        dev = host.to(self.dev, non_blocking=True)
+        S = ids.numel()
+        ids_dev, pos_dev, table_dev = dev[:S], dev[S:2 * S].to(torch.int32), dev[2 * S:].to(torch.int32).view(len(staged), width)
+        seg = ops.PackedSegments(cu, starts, self.dev)
+        emb = ops.embedding(ids_dev[None], lm.get_input_embeddings().weight)
+        for b, req in enumerate(staged):
+            if req.pixel_values is not None:
+                self._merge_images(req, ids_dev[cu[b]:cu[b + 1]], emb[0, cu[b]:cu[b + 1]])
+        logits = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends)
+        self.stats["prefill_launches"] += 1
+        self.stats["prefill_chunks"] += len(staged) - len(ends)
+        for i, b in enumerate(ends):
+            req = staged[b]
+            self._start_decode(self.sched.slots.index(req), req, logits[0, i:i + 1])
+
+    def _merge_images(self, req: Request, ids_dev, emb) -> None:
+        """Image features of the chunk req.chunk into its embedding rows: the ViT and the projector run on the pixel rows whose
+        first token past the cached prefix falls into this chunk, and the features of a row's tokens in later chunks are kept
+        with the request (req.feats, rows [req.feat_row, req.vit_rows)).  Each pixel row's features do not depend on the rows
+        that share its launch."""
+        m, pv, pm = self.model, req.pixel_values, req.pixel_mask
+        tok = m.config.image_token_index
+        n_query = self._queries_per_row(pv)
+        start, end = req.chunk
+        img = req.input_ids[:end] == tok
+        k0, k1 = int(img[:start].sum()), int(img.sum())       # the chunk's image tokens are k0 .. k1 - 1
+        if k1 == k0:
+            return
+        r_end = -(-k1 // n_query)                            # pixel rows the chunk reads features of: up to r_end
+        if r_end > req.vit_rows:
+            r0 = req.vit_rows
+            pix = pv[r0:r_end].to(self.dev, non_blocking=True).to(torch.bfloat16)
+            feats, image_attn_mask = m.vision_tower(pix, None if pm is None else pm[r0:r_end])
+            feats = m.multi_modal_projector(feats, image_attn_mask)
+            feats = feats.reshape(-1, feats.shape[-1])
+            req.feats = feats if req.feats is None else torch.cat([req.feats, feats])
+            req.vit_rows = r_end
+            self.stats["vit_rows_run"] += r_end - r0
+        ops.merge_image_features(ids_dev, tok, req.feats[k0 - req.feat_row * n_query:], emb)
+        keep = k1 // n_query                                  # rows wholly merged are dropped
+        req.feats = req.feats[(keep - req.feat_row) * n_query:] if keep < req.vit_rows else None
+        req.feat_row = keep
+
+    def _start_decode(self, s: int, req: Request, logits) -> None:
+        """Slot s's table row and state once req's prompt is prefilled, and its first token."""
+        row = torch.full((self.max_pages,), -1, dtype=torch.int32)
+        row[:len(req.pages)] = torch.tensor(req.pages, dtype=torch.int32)
+        self.cache.block_table[s].copy_(row)
+        T = req.input_ids.numel()
         t, k, p, seed = req.sampling
         st = self.state
         st.rope_pos[s] = T - 1
@@ -508,7 +679,20 @@ class Engine:
         st.max_new[s] = req.max_new_tokens
         st.n_out[s] = 0
         st.finished[s] = 0
-        self._sample_and_advance(_slot_rows(st, s), logits[:, -1])
+        self._sample_and_advance(_slot_rows(st, s), logits)
+
+    def _drop(self, s: int) -> None:
+        """Retire slot s without a result: the last active slot moves into s and the slot it left becomes idle."""
+        move = self.sched.retire(s)
+        if move is not None:
+            self._move_slot(*move)
+        self._idle(self.sched.n_active, self.sched.n_active + 1)
+
+    def _move_slot(self, src: int, dst: int) -> None:
+        for f in self.state.SLOT_FIELDS:
+            t = getattr(self.state, f)
+            t[dst].copy_(t[src])
+        self.cache.block_table[dst].copy_(self.cache.block_table[src])
 
     def _poll_and_retire(self) -> Dict[int, torch.Tensor]:
         t0 = time.perf_counter()
@@ -520,24 +704,21 @@ class Engine:
         fin = self._fin_host[:self.sched.n_active].tolist()
         n_out = self._nout_host[:self.sched.n_active].tolist()
         for req in self.sched.slots:
-            if req.rid not in self._first_seen:
+            if req is not self.sched.partial and req.rid not in self._first_seen:
                 self._first_seen.add(req.rid)
                 self.times[req.rid] = [now, None]
         done = {}
         for s in range(self.sched.n_active - 1, -1, -1):   # descending: the slot moved into s is always a live one
-            if not fin[s]:
-                continue
             req = self.sched.slots[s]
+            if not fin[s] or req is self.sched.partial:    # a partly prefilled request's slot is idle, not finished
+                continue
             done[req.rid] = torch.cat([req.input_ids.to(self.dev), self.state.out_tokens[s, :n_out[s]].to(torch.int64)])
             self.times[req.rid][1] = now
             self._first_seen.discard(req.rid)
             move = self.sched.retire(s)
             if move is not None:
                 src, dst = move
-                for f in self.state.SLOT_FIELDS:
-                    t = getattr(self.state, f)
-                    t[dst].copy_(t[src])
-                self.cache.block_table[dst].copy_(self.cache.block_table[src])
+                self._move_slot(src, dst)
                 fin[dst] = fin[src]
                 n_out[dst] = n_out[src]
             self._idle(self.sched.n_active, self.sched.n_active + 1)

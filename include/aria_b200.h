@@ -571,6 +571,26 @@ int aria_attention_prefill_paged_prefix(const void* q, const void* k, const void
                                         void* out, int32_t B, int32_t H, int32_t S_tot, int32_t P, int64_t q_stride_h,
                                         int64_t kv_stride_h, int64_t page_stride, int64_t pool_stride_h, float scale,
                                         aria_stream_t stream);
+/* aria_attention_prefill_paged_prefix over n_seg packed segments, each after a paged prefix of its own (batched admission):
+ * segment b is rows [cu_seqlens[b], cu_seqlens[b + 1]) of q / k / v [1, H, S_tot, 128] (DEVICE int32 [n_seg + 1], increasing
+ * from 0 to S_tot) and attends to its prefix_lens[b] cached keys (DEVICE int32 [n_seg], multiples of 256; key 256 i + r is row r
+ * of page page_table[b * page_table_stride + i], DEVICE int32, at least prefix_lens[b] / 256 entries per row) and causally to its
+ * own rows -> out [S_tot, H * 128].  Query tiles do not cross segments, so every row of segment b is bit-identical to
+ * aria_attention_prefill_paged_prefix run on segment b alone (B = 1) with its own page list and P.  The caller checks the device
+ * values; a page entry outside [0, n_pages) reads zeros.  Strides as aria_attention_prefill_paged_prefix's.  No workspace. */
+int aria_attention_prefill_paged_varlen(const void* q, const void* k, const void* v, const void* k_pool, const void* v_pool,
+                                        const int32_t* page_table, int64_t page_table_stride, int32_t n_pages,
+                                        const int32_t* prefix_lens, const int32_t* cu_seqlens, void* out, int32_t n_seg, int32_t H,
+                                        int32_t S_tot, int64_t q_stride_h, int64_t kv_stride_h, int64_t page_stride,
+                                        int64_t pool_stride_h, float scale, aria_stream_t stream);
+/* aria_kv_pages_store for packed segments: packed row t of segment b (cu_seqlens, prefix_lens and page_table as
+ * aria_attention_prefill_paged_varlen's, max_pages columns per table row) is position p = prefix_lens[b] + t - cu_seqlens[b] of
+ * its request and goes to row p % 256 of page page_table[b, p / 256].  Nothing is written for p past 256 * max_pages, a table
+ * entry outside [0, n_pages), or the null page 0.  Each segment's pages are bit-identical to aria_kv_pages_store on it alone. */
+int aria_kv_pages_store_varlen(const void* k, const void* v, int64_t src_stride_h, int32_t S_tot, void* k_pool, void* v_pool,
+                               int64_t page_stride, int64_t pool_stride_h, const int32_t* page_table, int64_t page_table_stride,
+                               int32_t max_pages, int32_t n_pages, const int32_t* prefix_lens, const int32_t* cu_seqlens,
+                               int32_t n_seg, int32_t H, aria_stream_t stream);
 /* aria_sample_tokens_rows with every sampling parameter per row, from DEVICE arrays [R]: temperature (0 = greedy), top_k, top_p,
  * seed (uint64), noise row and offset.  Row r is bit-identical to aria_sample_tokens run alone on that row with its scalars at
  * rng_offset = offsets[r] as row noise_rows[r].  The caller checks the parameters as aria_sample_tokens does; out-of-range
