@@ -969,6 +969,8 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
   if (d->epilogue == ARIA_EPI_HEADS) {
     ARIA_CHECK_ARG(d->head_dim > 0 && d->head_dim % 8 == 0 && d->head_ld >= d->head_dim && d->n % d->head_dim == 0);
     if (d->rope_mask) ARIA_CHECK_ARG(d->head_dim == 128 && d->rope_cos && d->rope_sin);
+    // the RoPE epilogue has no bias term: a rotated segment's bias would be dropped
+    for (int s = 0; s < d->n_seg; ++s) ARIA_CHECK_ARG(!((d->rope_mask >> s) & 1) || !d->bias[s]);
     if (d->n % 128 != 0) {
       ARIA_CHECK_ARG(!d->rope_mask && d->n % 144 == 0);
       BN = 144;

@@ -7,6 +7,8 @@ arithmetic of the kernel it checks (stated in each test's docstring), so a kerne
 import pytest
 import torch
 
+from gemm_ref import assert_gemm_close
+
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 bf16 = torch.bfloat16
@@ -214,26 +216,6 @@ def test_router_bwd_vs_fp64(T, E, k):
 
 
 # ------------------------------------------------------------------------------------------------ dense data-gradient GEMMs
-def assert_gemm_close(got, a, b, residual=None, what=""):
-    """got = a @ b (+ residual) per element:  |got - ref64| <= 2^-8 |ref| + 2^-12 (|a| @ |b|)   [+ 2^-8 (|ref| + |res|)].
-    2^-8 |ref| is one bf16 rounding of the output (bf16 keeps 8 significant bits, so a rounding moves a value by less
-    than 2^-8 of it); 2^-12 (|a| @ |b|) covers fp32 accumulation (under K 2^-24 of it for K <= 4096) and is far below
-    what a dropped or doubled 64-wide k-block moves (the |a||b| mass of 64 of the K products is about 64 / K of it, and
-    their sum is not small against 2^-12 of the whole).  With a residual the epilogue rounds the product to bf16 before
-    adding the residual and rounds again, so the first rounding adds 2^-8 |a @ b| <= 2^-8 (|ref| + |res|)."""
-    a64, b64 = a.to(f64), b.to(f64)
-    ref = a64 @ b64
-    bound = 2.0 ** -12 * (a64.abs() @ b64.abs())
-    if residual is not None:
-        ref = ref + residual.to(f64)
-        bound += 2.0 ** -8 * (ref.abs() + residual.to(f64).abs())
-    bound += 2.0 ** -8 * ref.abs()
-    err = (got.to(f64) - ref).abs()
-    bad = ~(err <= bound)
-    assert not bool(bad.any()), (f"{what}: {int(bad.sum())}/{bad.numel()} elements out of bound, first at "
-                                 f"{bad.nonzero()[0].tolist()}, worst err/bound {float((err / bound).max()):.3g}")
-
-
 GEMM_KN = [(3328, 2560), (2560, 3328), (200, 256)]   # cfg 5: dx from the shared expert's gate/up, dhs from down_w; K % 64 != 0
 
 
