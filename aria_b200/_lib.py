@@ -131,6 +131,12 @@ SIGNATURES = {
     "aria_attention_prefill_paged_varlen": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, vp, vp, vp, i32, i32, i32, i64, i64, i64, i64,
                                                   f32, vp]),
     "aria_kv_pages_store_varlen": (i32, [vp, vp, i64, i32, vp, vp, i64, i64, vp, i64, i32, i32, vp, vp, i32, i32, vp]),
+    "aria_attention_decode_paged_fp8": (i32, [vp, vp, vp, vp, vp, vp, i64, i32, i32, vp, vp, i32, i32, i64, i64, i64, i64, i64, i64,
+                                              f32, vp, i64, vp]),
+    "aria_kv_append_paged_fp8": (i32, [vp, vp, i64, i64, vp, vp, vp, vp, i64, i64, i64, i64, vp, i64, i32, i32, vp, i32, i32, vp]),
+    "aria_kv_pages_store_varlen_fp8": (i32, [vp, vp, i64, i32, vp, vp, vp, vp, i64, i64, i64, i64, vp, i64, i32, i32, vp, vp, i32, i32,
+                                             vp]),
+    "aria_kv_pages_load_fp8": (i32, [vp, vp, vp, vp, i64, i64, i64, i64, vp, i32, i32, vp, vp, i64, i64, i32, vp]),
     "aria_sample_tokens_slots": (i32, [vp, i64, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
     "aria_decode_advance_slots": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp]),
 }
@@ -159,7 +165,7 @@ def load():
 # kernels launched per C-ABI call (for bench.py's `gpu_launches`; memsets are not counted)
 KERNELS_PER_CALL = {"router_topk": 2, "attention_decode": 2, "attention_decode_devlen": 2, "attention_decode_fp8": 2,
                     "attention_decode_devlen_fp8": 2, "attention_decode_shared_prefix": 3,
-                    "attention_decode_multi": 2, "attention_decode_paged": 2, "attention_bwd": 3, "attention_bwd_varlen": 4, "moe_block_fwd": 9, "moe_block_fwd_fp8": 9,
+                    "attention_decode_multi": 2, "attention_decode_paged": 2, "attention_decode_paged_fp8": 2, "attention_bwd": 3, "attention_bwd_varlen": 4, "moe_block_fwd": 9, "moe_block_fwd_fp8": 9,
                     "moe_block_fwd_w8a8": 10, "quantize_fp8_cols": 2,
                     # W8A8 shared experts: two row quantisers join the shared branch's two GEMMs
                     "moe_block_fwd_bf16_shared_fp8": 11, "moe_block_fwd_fp8_shared_fp8": 11,

@@ -26,6 +26,7 @@
 // aria_attention_decode_devlen: the same kernels with the key count of each row read from device memory (graph replays).
 // aria_attention_decode_paged: the devlen kernels over a paged KV cache (page pools and a block table, continuous batching).
 // aria_attention_decode_fp8 / _devlen_fp8: the same split-KV kernels over an e4m3 KV cache with per-token scales.
+// aria_attention_decode_paged_fp8: the fp8 kernels over e4m3 page pools with per-token scale pools (fp8 KV pages).
 // aria_attention_decode_shared_prefix: n rows per prompt decode against one shared prompt cache plus their own tail caches.
 // aria_attention_decode_multi: Q consecutive queries per row against its cache (prompt-lookup verification), each query
 //   bit-identical to the devlen kernels.
@@ -590,10 +591,11 @@ attn_prefill_paged_varlen_kernel(const __grid_constant__ CUtensorMap tmQ, const 
 // sc_stride_b / sc_stride_h).  A lane widens its 4 codes per key exactly; the key scale multiplies the reduced dot product and
 // the value weight is pw * v_scale.  Split size, warp -> key assignment and update order are the bf16 kernel's, so with
 // power-of-two scales (both products exact) the result is bit-identical to the bf16 kernel run on the tensors code * scale.
-// PAGED (with DEVLEN, bf16): kc / vc are page pools [n_pages, H, DEC_SPLIT_KEYS, 128] (kv_stride_b is the page stride) and
+// PAGED (with DEVLEN): kc / vc are page pools [n_pages, H, DEC_SPLIT_KEYS, 128] (kv_stride_b is the page stride) and
 // split s of row b reads page block_table[b * bt_stride + s], which holds the row's keys [256 s, 256 s + 256).  A page is one
 // split, so every key is read by the warp, and updated in the order, of the contiguous kernel: row b is bit-identical to
 // the DEVLEN kernel on a cache that holds the same keys.  A live split whose entry is not a page of the pool reads no key.
+// With KV_FP8 the scales are pools [n_pages, H, DEC_SPLIT_KEYS] too (sc_stride_b is their page stride), read from the same page.
 constexpr int DEC_SPLIT_KEYS = 256;
 
 template <bool DEVLEN, bool KV_FP8, bool PAGED = false, typename KV = std::conditional_t<KV_FP8, uint8_t, __nv_bfloat16>>
@@ -613,8 +615,9 @@ __device__ __forceinline__ void decode_partial(const __nv_bfloat16* __restrict__
   int k_end = min(len, k_begin + DEC_SPLIT_KEYS);
   const KV* kbase;
   const KV* vbase;
+  [[maybe_unused]] int page = 0;
   if constexpr (PAGED) {
-    const int page = k_begin < k_end ? block_table[b * bt_stride + split] : 0;
+    page = k_begin < k_end ? block_table[b * bt_stride + split] : 0;
     if (page < 0 || page >= n_pages) k_end = k_begin;
     // key kk of the split is row kk - k_begin of its page
     const int64_t off = static_cast<int64_t>(page) * kv_stride_b + h * kv_stride_h - static_cast<int64_t>(k_begin) * AT_D;
@@ -667,8 +670,16 @@ __device__ __forceinline__ void decode_partial(const __nv_bfloat16* __restrict__
       }
     }
   } else {
-    const float* ksb = k_scale + b * sc_stride_b + h * sc_stride_h;
-    const float* vsb = v_scale + b * sc_stride_b + h * sc_stride_h;
+    const float* ksb;
+    const float* vsb;
+    if constexpr (PAGED) {  // the scale of key kk is entry kk - k_begin of its page's scale rows
+      const int64_t off = static_cast<int64_t>(page) * sc_stride_b + h * sc_stride_h - k_begin;
+      ksb = k_scale + off;
+      vsb = v_scale + off;
+    } else {
+      ksb = k_scale + b * sc_stride_b + h * sc_stride_h;
+      vsb = v_scale + b * sc_stride_b + h * sc_stride_h;
+    }
     // A lane reads 4 + 4 bytes per key, half of what the bf16 loop reads, so the loads of step k0 + 16 are issued before the
     // arithmetic of step k0 to keep as many bytes in flight per warp.
     uint32_t kn[4], vn[4];
@@ -797,6 +808,17 @@ __global__ void __launch_bounds__(128) attn_decode_partial_paged(const __nv_bflo
                                                                  int n_pages) {
   decode_partial<true, false, true>(q, k_pool, v_pool, nullptr, nullptr, nullptr, ws, H, Tk, q_stride_b, q_stride_h, page_stride,
                                     pool_stride_h, 0, 0, scale_log2, splits, lens, 0, block_table, bt_stride, n_pages);
+}
+
+__global__ void __launch_bounds__(128) attn_decode_partial_paged_fp8(
+    const __nv_bfloat16* __restrict__ q, const uint8_t* __restrict__ k_pool, const uint8_t* __restrict__ v_pool,
+    const float* __restrict__ k_scale, const float* __restrict__ v_scale, float* __restrict__ ws, int H, int Tk, int64_t q_stride_b,
+    int64_t q_stride_h, int64_t page_stride, int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h,
+    float scale_log2, int splits, const int32_t* __restrict__ lens, const int32_t* __restrict__ block_table, int64_t bt_stride,
+    int n_pages) {
+  decode_partial<true, true, true>(q, k_pool, v_pool, k_scale, v_scale, nullptr, ws, H, Tk, q_stride_b, q_stride_h, page_stride,
+                                   pool_stride_h, scale_page_stride, scale_stride_h, scale_log2, splits, lens, 0, block_table,
+                                   bt_stride, n_pages);
 }
 
 template <bool DEVLEN>
@@ -1525,4 +1547,30 @@ extern "C" int aria_attention_decode_devlen_fp8(const void* q, const void* k, co
   return attention_decode_fp8<true>(q, k, v, k_scale, v_scale, out, key_mask, key_mask_stride, lens, B, H, T_max, q_stride_b,
                                     q_stride_h, kv_stride_b, kv_stride_h, scale_stride_b, scale_stride_h, scale, workspace,
                                     workspace_bytes, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int aria_attention_decode_paged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale,
+                                               const float* v_scale, const int32_t* block_table, int64_t block_table_stride,
+                                               int32_t max_pages, int32_t n_pages, const int32_t* lens, void* out, int32_t R,
+                                               int32_t H, int64_t q_stride_b, int64_t q_stride_h, int64_t page_stride,
+                                               int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h, float scale,
+                                               void* workspace, int64_t workspace_bytes, aria_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  ARIA_CHECK_ARG(q && k_pool && v_pool && k_scale && v_scale && block_table && lens && out && workspace && R > 0 && H > 0 &&
+                 n_pages > 0);
+  ARIA_CHECK_ARG(max_pages > 0 && max_pages <= 65535 && block_table_stride >= max_pages);  // splits are grid.y
+  ARIA_CHECK_ARG(q_stride_b % 4 == 0 && q_stride_h % 4 == 0 && page_stride % 16 == 0 && pool_stride_h % 16 == 0);
+  ARIA_CHECK_ARG(pool_stride_h >= DEC_SPLIT_KEYS * AT_D && page_stride >= pool_stride_h * H);  // pages do not overlap
+  ARIA_CHECK_ARG(scale_stride_h >= DEC_SPLIT_KEYS && scale_page_stride >= scale_stride_h * H);
+  const int T_max = max_pages * DEC_SPLIT_KEYS;
+  ARIA_CHECK_ARG(workspace_bytes >= aria_attention_decode_workspace_bytes(R, H, T_max));
+  attn_decode_partial_paged_fp8<<<dim3(R * H, max_pages), 128, 0, stream>>>(
+      static_cast<const __nv_bfloat16*>(q), static_cast<const uint8_t*>(k_pool), static_cast<const uint8_t*>(v_pool), k_scale,
+      v_scale, static_cast<float*>(workspace), H, T_max, q_stride_b, q_stride_h, page_stride, pool_stride_h, scale_page_stride,
+      scale_stride_h, scale * 1.4426950408889634f, max_pages, lens, block_table, block_table_stride, n_pages);
+  int rc = check_launch("attn_decode_partial_paged_fp8");
+  if (rc) return rc;
+  attn_decode_merge<true><<<R * H, 128, 0, stream>>>(static_cast<const float*>(workspace), static_cast<__nv_bfloat16*>(out),
+                                                     max_pages, lens, H);
+  return check_launch("attn_decode_merge");
 }

@@ -202,6 +202,15 @@ __device__ __forceinline__ int packed_segment(const int32_t* cu, int n_seg, int 
   }
   return lo;
 }
+
+constexpr int PAGE_ROWS = 256;  // rows per KV page (serving.Engine's paged cache): the decode kernels' split size
+
+// The page holding row p of a slot whose table row is bt[0, max_pages), or -1 when p is not in a mapped page of the pool
+__device__ __forceinline__ int page_of(const int32_t* bt, int max_pages, int n_pages, int p) {
+  if (p < 0 || p / PAGE_ROWS >= max_pages) return -1;
+  const int page = bt[p / PAGE_ROWS];
+  return page < n_pages ? page : -1;
+}
 #endif
 
 }  // namespace aria

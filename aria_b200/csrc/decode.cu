@@ -124,15 +124,6 @@ __global__ void __launch_bounds__(ADV_MAX_B) decode_advance_kernel(const Advance
   }
 }
 
-constexpr int PAGE_ROWS = 256;  // rows per KV page: the decode kernels' split size
-
-// The page holding row p of a slot whose table row is bt[0, max_pages), or -1 when p is not in a mapped page of the pool
-__device__ __forceinline__ int page_of(const int32_t* bt, int max_pages, int n_pages, int p) {
-  if (p < 0 || p / PAGE_ROWS >= max_pages) return -1;
-  const int page = bt[p / PAGE_ROWS];
-  return page < n_pages ? page : -1;
-}
-
 // One CTA per (slot r, head h)
 __global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_append_paged_kernel(const __nv_bfloat16* __restrict__ k_new,
                                                                           const __nv_bfloat16* __restrict__ v_new, int64_t new_sb,

@@ -8,6 +8,8 @@
 // aria_kv_store_fp8: quantises bf16 rows [0, n) of a source into cache rows [row0, row0 + n) (prefill, host positions).
 // aria_kv_append_fp8: quantises one bf16 row per (b, h) into cache row pos[b] (device positions, the captured decode step).
 // aria_kv_load_fp8: dequantises cache rows [0, n) into bf16, bf16(code * scale) (a multi-token continuation attends bf16 K/V).
+// aria_kv_append_paged_fp8 / aria_kv_pages_store_varlen_fp8 / aria_kv_pages_load_fp8: the same quantiser and dequantiser over
+// the page pools of serving.Engine's fp8 KV pages (codes [n_pages, H, 256, 128], scales [n_pages, H, 256]).
 //
 // One half-warp per 128-wide row, 8 values per lane; a block covers 4 rows of k and the same 4 rows of v.
 #include <cuda_bf16.h>
@@ -21,10 +23,8 @@ namespace aria {
 constexpr int KVQ_D = 128;
 constexpr int KVQ_ROWS = 4;  // rows per 128-thread block: warp w takes row w, its low half-warp k and its high half-warp v
 
-// The one quantiser of both entries: lane j (of 16) holds elements [8j, 8j + 8) of the row
-__device__ __forceinline__ void quantize_row_e4m3(const __nv_bfloat16* __restrict__ src, uint8_t* __restrict__ dst,
-                                                  float* __restrict__ scale, int j) {
-  const uint4 v = *reinterpret_cast<const uint4*>(src + 8 * j);
+// The one quantiser of every entry: lane j (of 16) holds elements [8j, 8j + 8) of the row -> its 8 codes and the row's scale s
+__device__ __forceinline__ uint2 quantize8_e4m3(const uint4 v, float& s) {
   const uint32_t u[4] = {v.x, v.y, v.z, v.w};
   float m = 0.f;
 #pragma unroll
@@ -32,9 +32,26 @@ __device__ __forceinline__ void quantize_row_e4m3(const __nv_bfloat16* __restric
   const unsigned half = 0xFFFFu << (threadIdx.x & 16);
 #pragma unroll
   for (int o = 8; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(half, m, o));
-  const float s = m > 0.f ? __fdiv_rn(m, E4M3_MAX) : 1.f;
-  *reinterpret_cast<uint2*>(dst + 8 * j) = cast8_e4m3(v, s);
+  s = m > 0.f ? __fdiv_rn(m, E4M3_MAX) : 1.f;
+  return cast8_e4m3(v, s);
+}
+
+__device__ __forceinline__ void quantize_row_e4m3(const __nv_bfloat16* __restrict__ src, uint8_t* __restrict__ dst,
+                                                  float* __restrict__ scale, int j) {
+  float s;
+  *reinterpret_cast<uint2*>(dst + 8 * j) = quantize8_e4m3(*reinterpret_cast<const uint4*>(src + 8 * j), s);
   if (j == 0) *scale = s;
+}
+
+// The one dequantiser: 8 codes of scale s -> 8 bf16 values bf16(code * s)
+__device__ __forceinline__ uint4 dequantize8_e4m3(const uint2 c, float s) {
+  const float4 lo = e4m3x4_to_float4(c.x), hi = e4m3x4_to_float4(c.y);
+  uint4 o;
+  o.x = pack_bf16(lo.x * s, lo.y * s);
+  o.y = pack_bf16(lo.z * s, lo.w * s);
+  o.z = pack_bf16(hi.x * s, hi.y * s);
+  o.w = pack_bf16(hi.z * s, hi.w * s);
+  return o;
 }
 
 // DEV_POS: cache row pos[b] of source row 0 (n = 1); otherwise cache row row0 + r of source row r
@@ -69,13 +86,65 @@ __global__ void __launch_bounds__(32 * KVQ_ROWS) kv_load_kernel(const uint8_t* _
   const int j = threadIdx.x & 15;
   const uint2 c = *reinterpret_cast<const uint2*>((is_v ? vc : kc) + b * c_sb + h * c_sh + static_cast<int64_t>(r) * KVQ_D + 8 * j);
   const float s = (is_v ? vs : ks)[b * sc_sb + h * sc_sh + r];
-  const float4 lo = e4m3x4_to_float4(c.x), hi = e4m3x4_to_float4(c.y);
-  uint4 o;
-  o.x = pack_bf16(lo.x * s, lo.y * s);
-  o.y = pack_bf16(lo.z * s, lo.w * s);
-  o.z = pack_bf16(hi.x * s, hi.y * s);
-  o.w = pack_bf16(hi.z * s, hi.w * s);
-  *reinterpret_cast<uint4*>((is_v ? v_out : k_out) + b * o_sb + h * o_sh + static_cast<int64_t>(r) * KVQ_D + 8 * j) = o;
+  *reinterpret_cast<uint4*>((is_v ? v_out : k_out) + b * o_sb + h * o_sh + static_cast<int64_t>(r) * KVQ_D + 8 * j) =
+      dequantize8_e4m3(c, s);
+}
+
+// Paged fp8 pools (serving.Engine with kv_cache_dtype="fp8"): codes [n_pages, H, 256, 128] at (page_stride, pool_sh), scales
+// [n_pages, H, 256] at (sc_page_stride, sc_sh).  One warp per (row t, head h) item, its low half-warp k and its high half v.
+// VARLEN: item row t is packed row t of segment b, position prefix_lens[b] + t - cu[b] of its request (the varlen store); the
+// dequantised values bf16(code * scale) are written back over every source row.  Otherwise (the append) row t is slot t, at
+// position pos[t].  No page is written for an unmapped position, a table entry outside the pool, or the null page 0.
+template <bool VARLEN>
+__global__ void __launch_bounds__(32 * KVQ_ROWS) kv_quant_paged_kernel(
+    __nv_bfloat16* __restrict__ k_src, __nv_bfloat16* __restrict__ v_src, int64_t s_sb, int64_t s_sh, uint8_t* __restrict__ kp,
+    uint8_t* __restrict__ vp, float* __restrict__ ks, float* __restrict__ vs, int64_t page_stride, int64_t pool_sh,
+    int64_t sc_page_stride, int64_t sc_sh, const int32_t* __restrict__ table, int64_t table_stride, int max_pages, int n_pages,
+    const int32_t* __restrict__ pos, const int32_t* __restrict__ cu, int n_seg, int n_items, int H) {
+  const int item = blockIdx.x * KVQ_ROWS + (threadIdx.x >> 5);
+  if (item >= n_items) return;
+  const int t = item / H, h = item % H;
+  int row, p;
+  if constexpr (VARLEN) {
+    row = packed_segment(cu, n_seg, t);
+    p = pos[row] + t - cu[row];
+  } else {
+    row = t;
+    p = pos[t];
+  }
+  const int page = page_of(table + row * table_stride, max_pages, n_pages, p);
+  if (!VARLEN && page <= 0) return;
+  const bool is_v = threadIdx.x & 16;
+  const int j = threadIdx.x & 15;
+  __nv_bfloat16* src = (is_v ? v_src : k_src) + t * s_sb + h * s_sh + 8 * j;
+  float s;
+  const uint2 c = quantize8_e4m3(*reinterpret_cast<const uint4*>(src), s);
+  if (page > 0) {  // not unmapped, outside the pool, or the null page
+    const int r = p % PAGE_ROWS;
+    *reinterpret_cast<uint2*>((is_v ? vp : kp) + page * page_stride + h * pool_sh + static_cast<int64_t>(r) * KVQ_D + 8 * j) = c;
+    if (j == 0) (is_v ? vs : ks)[page * sc_page_stride + h * sc_sh + r] = s;
+  }
+  if constexpr (VARLEN) *reinterpret_cast<uint4*>(src) = dequantize8_e4m3(c, s);
+}
+
+// Page pages[i] of the fp8 pools -> page i of the bf16 pools out [n_list, H, 256, 128] (out_page_stride, out_sh), with the
+// dequantiser of kv_load_kernel; an entry outside [0, n_pages) gives zeros.  Block (i * H + h, 4 rows).
+__global__ void __launch_bounds__(32 * KVQ_ROWS) kv_pages_load_kernel(
+    const uint8_t* __restrict__ kp, const uint8_t* __restrict__ vp, const float* __restrict__ ks, const float* __restrict__ vs,
+    int64_t page_stride, int64_t pool_sh, int64_t sc_page_stride, int64_t sc_sh, const int32_t* __restrict__ pages, int n_pages,
+    __nv_bfloat16* __restrict__ k_out, __nv_bfloat16* __restrict__ v_out, int64_t out_page_stride, int64_t out_sh, int H) {
+  const int i = blockIdx.x / H, h = blockIdx.x % H;
+  const int r = blockIdx.y * KVQ_ROWS + (threadIdx.x >> 5);
+  const bool is_v = threadIdx.x & 16;
+  const int j = threadIdx.x & 15;
+  const int page = pages[i];
+  uint4 o = make_uint4(0u, 0u, 0u, 0u);
+  if (page >= 0 && page < n_pages) {
+    const uint2 c = *reinterpret_cast<const uint2*>((is_v ? vp : kp) + page * page_stride + h * pool_sh +
+                                                     static_cast<int64_t>(r) * KVQ_D + 8 * j);
+    o = dequantize8_e4m3(c, (is_v ? vs : ks)[page * sc_page_stride + h * sc_sh + r]);
+  }
+  *reinterpret_cast<uint4*>((is_v ? v_out : k_out) + i * out_page_stride + h * out_sh + static_cast<int64_t>(r) * KVQ_D + 8 * j) = o;
 }
 
 // what all three entries require of the cache: e4m3 rows of 16-byte alignment and non-negative scale strides
@@ -83,6 +152,13 @@ static bool cache_args_ok(const void* kc, const void* vc, const float* ks, const
                           int64_t sc_sb, int64_t sc_sh, int32_t B, int32_t H, int32_t T_max) {
   return kc && vc && ks && vs && c_sb % 16 == 0 && c_sh % 16 == 0 && sc_sb >= 0 && sc_sh >= 0 && B > 0 && H > 0 && T_max > 0 &&
          static_cast<int64_t>(B) * H < (1ll << 31);
+}
+
+// what the paged entries require of the pools: 16-byte code rows, pages that do not overlap, and scale strides to match
+static bool pool_args_ok(const void* kp, const void* vp, const float* ks, const float* vs, int64_t page_stride, int64_t pool_sh,
+                         int64_t sc_page_stride, int64_t sc_sh, int32_t n_pages, int32_t H) {
+  return kp && vp && ks && vs && n_pages > 0 && H > 0 && page_stride % 16 == 0 && pool_sh % 16 == 0 &&
+         pool_sh >= PAGE_ROWS * KVQ_D && page_stride >= pool_sh * H && sc_sh >= PAGE_ROWS && sc_page_stride >= sc_sh * H;
 }
 
 }  // namespace aria
@@ -135,4 +211,59 @@ extern "C" int aria_kv_load_fp8(const void* k_cache, const void* v_cache, const 
       scale_stride_b, scale_stride_h, static_cast<__nv_bfloat16*>(k_out), static_cast<__nv_bfloat16*>(v_out), out_stride_b,
       out_stride_h, n_rows, H);
   return check_launch("kv_load_kernel");
+}
+
+extern "C" int aria_kv_append_paged_fp8(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h,
+                                        void* k_pool, void* v_pool, float* k_scale, float* v_scale, int64_t page_stride,
+                                        int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h,
+                                        const int32_t* block_table, int64_t block_table_stride, int32_t max_pages, int32_t n_pages,
+                                        const int32_t* write_pos, int32_t R, int32_t H, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k_new && v_new && block_table && write_pos && new_stride_b % 8 == 0 && new_stride_h % 8 == 0);
+  ARIA_CHECK_ARG(pool_args_ok(k_pool, v_pool, k_scale, v_scale, page_stride, pool_stride_h, scale_page_stride, scale_stride_h,
+                              n_pages, H));
+  ARIA_CHECK_ARG(R > 0 && max_pages > 0 && block_table_stride >= max_pages);
+  ARIA_CHECK_ARG(static_cast<int64_t>(R) * H < (1ll << 31) && static_cast<int64_t>(R) * block_table_stride < (1ll << 31));
+  const int items = R * H;
+  kv_quant_paged_kernel<false><<<(items + KVQ_ROWS - 1) / KVQ_ROWS, 32 * KVQ_ROWS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(k_new)),
+      const_cast<__nv_bfloat16*>(static_cast<const __nv_bfloat16*>(v_new)), new_stride_b, new_stride_h,
+      static_cast<uint8_t*>(k_pool), static_cast<uint8_t*>(v_pool), k_scale, v_scale, page_stride, pool_stride_h, scale_page_stride,
+      scale_stride_h, block_table, block_table_stride, max_pages, n_pages, write_pos, nullptr, 0, items, H);
+  return check_launch("kv_quant_paged_kernel");
+}
+
+extern "C" int aria_kv_pages_store_varlen_fp8(void* k, void* v, int64_t src_stride_h, int32_t S_tot, void* k_pool, void* v_pool,
+                                              float* k_scale, float* v_scale, int64_t page_stride, int64_t pool_stride_h,
+                                              int64_t scale_page_stride, int64_t scale_stride_h, const int32_t* page_table,
+                                              int64_t page_table_stride, int32_t max_pages, int32_t n_pages,
+                                              const int32_t* prefix_lens, const int32_t* cu_seqlens, int32_t n_seg, int32_t H,
+                                              aria_stream_t stream_) {
+  ARIA_CHECK_ARG(k && v && page_table && prefix_lens && cu_seqlens);
+  ARIA_CHECK_ARG(pool_args_ok(k_pool, v_pool, k_scale, v_scale, page_stride, pool_stride_h, scale_page_stride, scale_stride_h,
+                              n_pages, H));
+  ARIA_CHECK_ARG(S_tot >= n_seg && n_seg > 0 && max_pages > 0 && page_table_stride >= max_pages);
+  ARIA_CHECK_ARG(static_cast<int64_t>(S_tot) * H < (1ll << 31) && src_stride_h >= static_cast<int64_t>(S_tot) * KVQ_D);
+  ARIA_CHECK_ARG(static_cast<int64_t>(n_seg) * page_table_stride < (1ll << 31) && src_stride_h % 8 == 0);
+  const int items = S_tot * H;
+  kv_quant_paged_kernel<true><<<(items + KVQ_ROWS - 1) / KVQ_ROWS, 32 * KVQ_ROWS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<__nv_bfloat16*>(k), static_cast<__nv_bfloat16*>(v), KVQ_D, src_stride_h, static_cast<uint8_t*>(k_pool),
+      static_cast<uint8_t*>(v_pool), k_scale, v_scale, page_stride, pool_stride_h, scale_page_stride, scale_stride_h, page_table,
+      page_table_stride, max_pages, n_pages, prefix_lens, cu_seqlens, n_seg, items, H);
+  return check_launch("kv_quant_paged_kernel");
+}
+
+extern "C" int aria_kv_pages_load_fp8(const void* k_pool, const void* v_pool, const float* k_scale, const float* v_scale,
+                                      int64_t page_stride, int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h,
+                                      const int32_t* pages, int32_t n_list, int32_t n_pages, void* k_out, void* v_out,
+                                      int64_t out_page_stride, int64_t out_stride_h, int32_t H, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(pool_args_ok(k_pool, v_pool, k_scale, v_scale, page_stride, pool_stride_h, scale_page_stride, scale_stride_h,
+                              n_pages, H));
+  ARIA_CHECK_ARG(pages && k_out && v_out && n_list > 0 && static_cast<int64_t>(n_list) * H < (1ll << 31));
+  ARIA_CHECK_ARG(out_stride_h % 8 == 0 && out_page_stride % 8 == 0 && out_stride_h >= PAGE_ROWS * KVQ_D &&
+                 out_page_stride >= out_stride_h * H);
+  kv_pages_load_kernel<<<dim3(n_list * H, PAGE_ROWS / KVQ_ROWS), 32 * KVQ_ROWS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const uint8_t*>(k_pool), static_cast<const uint8_t*>(v_pool), k_scale, v_scale, page_stride, pool_stride_h,
+      scale_page_stride, scale_stride_h, pages, n_pages, static_cast<__nv_bfloat16*>(k_out), static_cast<__nv_bfloat16*>(v_out),
+      out_page_stride, out_stride_h, H);
+  return check_launch("kv_pages_load_kernel");
 }

@@ -540,25 +540,45 @@ class LookupDecodeState(DecodeState):
 
 
 class PagedKVCache:
-    """Paged KV cache of continuous batching (serving.Engine): per-layer page pools k[l] / v[l] [n_pages, H, 256, head_dim] bf16
+    """Paged KV cache of continuous batching (serving.Engine): per-layer page pools k[l] / v[l] [n_pages, H, 256, head_dim]
     and one block table [max_rows, max_pages] int32 shared by the layers, row r listing the pages of the request in slot r
     (key 256 s + i of the request is row i of page block_table[r, s]; -1 = no page).  A page holds one decode split
     (PAGE_SIZE = the split-KV kernels' 256 keys), so the paged decode reads exactly the keys, in the order, of the contiguous
-    one.  `width`: the table columns a decode step covers (its grid), set by the owner before a step is captured."""
+    one.  `width`: the table columns a decode step covers (its grid), set by the owner before a step is captured.
+
+    dtype "bf16": the pools are bf16.
+    dtype "fp8":  the pools are float8_e4m3fn codes, with fp32 scale pools k_scale[l] / v_scale[l] [n_pages, H, 256], one per
+                  (page, head, row), quantized as KVCache(dtype="fp8") quantizes its rows (ops.kv_append_paged,
+                  ops.kv_pages_store_varlen)."""
 
     PAGE_SIZE = 256
 
-    def __init__(self, n_layers, n_pages, H, hd, max_rows, max_pages, device):
-        self.k = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=bf16, device=device) for _ in range(n_layers)]
-        self.v = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+    def __init__(self, n_layers, n_pages, H, hd, max_rows, max_pages, device, dtype="bf16"):
+        if dtype not in KV_CACHE_DTYPES:
+            raise ValueError(f"KV cache dtype must be 'bf16' or 'fp8', got {dtype!r}")
+        kv_dt = torch.float8_e4m3fn if dtype == "fp8" else bf16
+        self.k = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=kv_dt, device=device) for _ in range(n_layers)]
+        self.v = [torch.empty(n_pages, H, self.PAGE_SIZE, hd, dtype=kv_dt, device=device) for _ in range(n_layers)]
         # page 0 is the null page idle rows attend to (one key): zeros, so their attention output is 0 and not whatever the
         # allocator left there; no request ever gets it, and the paged append never writes it for an idle row
         for t in self.k + self.v:
-            t[0].zero_()
+            t[0].view(torch.uint8).zero_()
+        if dtype == "fp8":
+            # the null page's codes are 0 and its scales 1: its key scores 0 and its value is 0, as in the bf16 pools
+            self.k_scale = [torch.empty(n_pages, H, self.PAGE_SIZE, dtype=torch.float32, device=device) for _ in range(n_layers)]
+            self.v_scale = [torch.empty(n_pages, H, self.PAGE_SIZE, dtype=torch.float32, device=device) for _ in range(n_layers)]
+            for t in self.k_scale + self.v_scale:
+                t[0].fill_(1.0)
         self.block_table = torch.full((max_rows, max_pages), -1, dtype=torch.int32, device=device)
         self.n_pages = n_pages
         self.width = max_pages
-        self.dtype = "bf16"
+        self.dtype = dtype
+
+    def scales(self, layer):
+        """(k_scale, v_scale) of a layer's fp8 pools, (None, None) for bf16 ones: the ops' k_scale= / v_scale= arguments."""
+        if self.dtype == "fp8":
+            return self.k_scale[layer], self.v_scale[layer]
+        return None, None
 
 
 class SlotDecodeState(DecodeState):
@@ -689,8 +709,9 @@ class AriaAttention(nn.Module):
         self._qkv(hidden_states, hq, [q, k, v], 1, 0, rope, state.rope_pos)
         if isinstance(cache, PagedKVCache):
             kp, vp, bt = cache.k[self.layer_idx], cache.v[self.layer_idx], cache.block_table[:, :cache.width]
-            ops.kv_append_paged(k[:, :, 0], v[:, :, 0], kp, vp, bt, state.write_pos)
-            o = ops.attention_decode_paged(q[:, :, 0], kp, vp, bt, state.kv_len, hd ** -0.5).view(B, 1, d)
+            ks, vs = cache.scales(self.layer_idx)
+            ops.kv_append_paged(k[:, :, 0], v[:, :, 0], kp, vp, bt, state.write_pos, k_scale=ks, v_scale=vs)
+            o = ops.attention_decode_paged(q[:, :, 0], kp, vp, bt, state.kv_len, hd ** -0.5, k_scale=ks, v_scale=vs).view(B, 1, d)
             return self._o_proj(o, residual)
         if isinstance(cache, SharedPrefixCache):
             tk, tv = cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx]
@@ -736,17 +757,32 @@ class AriaAttention(nn.Module):
         ops.kv_scatter_tails(k, v, S, cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx], cu_seqlens, n)
         return self._o_proj(o.view(1, S, d), residual)
 
-    def prefill_paged(self, hidden_states, cache: PagedKVCache, rope, page_table, seg, position_ids, residual=None, hq=None):
+    def prefill_paged(self, hidden_states, cache: PagedKVCache, rope, page_table, seg, position_ids, residual=None, hq=None,
+                      prefix=None):
         """Packed prompt segments, each after a prefix held in its own pages (AriaMoELMModel.prefill_paged): the fused projection
         writes q, k, v to a staging buffer (RoPE at position_ids), segment b attends to the pages page_table[b, : P_b / 256] and
         causally to itself (ops.attention_prefill_paged_varlen), and its k, v rows are stored after its prefix in its pages
-        (ops.kv_pages_store_varlen)."""
+        (ops.kv_pages_store_varlen).
+        fp8 pages: every query attends to every key as bf16(code * scale), its own segment's included, so a result does not
+        depend on where a prompt was split or which pages were cached.  The rows are stored first, which rewrites the staging
+        rows with their dequantized values.  prefix = (pages, table, k_scratch, v_scratch) of AriaMoELMModel.prefill_paged:
+        the launch's distinct prefix pages (pages: CUDA int32, or None when no segment has a prefix) are dequantized into the
+        bf16 scratch pools (ops.kv_pages_load_fp8), and `table`, the page table renumbered to the scratch, is what attention
+        reads in page_table's place."""
         _, S, d = hidden_states.shape
         H, hd = self.num_heads, self.head_dim
         stage = torch.empty(3, 1, H, S, hd, dtype=bf16, device=hidden_states.device)
         q, k, v = stage[0], stage[1], stage[2]
         self._qkv(hidden_states, hq, [q, k, v], S, 0, rope, position_ids)
         kp, vp = cache.k[self.layer_idx], cache.v[self.layer_idx]
+        if cache.dtype == "fp8":
+            ks, vs = cache.scales(self.layer_idx)
+            pages, table, k_scr, v_scr = prefix
+            ops.kv_pages_store_varlen(k, v, kp, vp, page_table, seg, k_scale=ks, v_scale=vs)
+            if pages is not None:
+                ops.kv_pages_load_fp8(kp, vp, ks, vs, pages, k_scr, v_scr)
+            o = ops.attention_prefill_paged_varlen(q, k, v, k_scr, v_scr, table, seg, hd ** -0.5)
+            return self._o_proj(o.view(1, S, d), residual)
         o = ops.attention_prefill_paged_varlen(q, k, v, kp, vp, page_table, seg, hd ** -0.5)
         ops.kv_pages_store_varlen(k, v, kp, vp, page_table, seg)
         return self._o_proj(o.view(1, S, d), residual)
@@ -808,10 +844,10 @@ class MoEDecoderLayer(nn.Module):
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
-    def prefill_paged(self, x, pending, cache, rope, page_table, seg, position_ids):
+    def prefill_paged(self, x, pending, cache, rope, page_table, seg, position_ids, prefix=None):
         """forward() for packed prompt segments, each after a prefix held in its pages (AriaAttention.prefill_paged)."""
         h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.prefill_paged(h, cache, rope, page_table, seg, position_ids, residual=x, hq=hq)
+        x = self.self_attn.prefill_paged(h, cache, rope, page_table, seg, position_ids, residual=x, hq=hq, prefix=prefix)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
@@ -883,7 +919,7 @@ class AriaMoELMModel(nn.Module):
             x, pending = layer.prefill_suffixes(x, pending, cache, rope, cu_seqlens, position_ids)
         return x, pending
 
-    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids):
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, page_table_host=None):
         """Prefill prompt segments packed along one row, each continuing a prefix whose keys and values are already in the
         pages of its request (batched and chunked admission, prefix caching: serving.Engine).  inputs_embeds [1, S_tot, d]; seg:
         an ops.PackedSegments, segment b = packed rows [seg.cu[b], seg.cu[b + 1]) after a prefix of seg.prefix_lens[b] tokens (a
@@ -892,7 +928,10 @@ class AriaMoELMModel(nn.Module):
         Each segment attends to its prefix and causally to itself, and its keys and values go to its pages after the prefix, as
         forward() on its whole prompt would have stored them.  Every row's output is the one forward() gives that position on
         its own prompt, bit for bit: attention keeps the segments apart and the rest of a layer computes each row on its own.
-        n_seg = 1 is one request's prefill.  Returns (x, pending) as forward() does."""
+        n_seg = 1 is one request's prefill.  Returns (x, pending) as forward() does.
+        fp8 pages (AriaAttention.prefill_paged): one bf16 scratch pair holding the launch's distinct prefix pages is allocated
+        here and shared by the layers, each layer dequantizing its own pages into it; page_table_host, a CPU copy of
+        page_table, spares reading the prefix pages back from the device."""
         if not isinstance(cache, PagedKVCache):
             raise ValueError("prefill_paged needs a PagedKVCache")
         if not isinstance(seg, ops.PackedSegments):
@@ -907,10 +946,31 @@ class AriaMoELMModel(nn.Module):
                 raise ValueError(f"prefill_paged: segment {b} (P = {P}, {seg.cu[b + 1] - seg.cu[b]} tokens) does not fit {width} "
                                  "pages")
         rope = self.rope_tables(cache.block_table.shape[1] * cache.PAGE_SIZE, inputs_embeds.device)
+        prefix = self._prefix_scratch(cache, page_table, seg, page_table_host) if cache.dtype == "fp8" else None
         x, pending = inputs_embeds, None
         for layer in self.layers:
-            x, pending = layer.prefill_paged(x, pending, cache, rope, page_table, seg, position_ids)
+            x, pending = layer.prefill_paged(x, pending, cache, rope, page_table, seg, position_ids, prefix)
         return x, pending
+
+    @staticmethod
+    def _prefix_scratch(cache: PagedKVCache, page_table, seg, page_table_host=None):
+        """(pages, table, k_scratch, v_scratch) for an fp8 prefill_paged: the distinct prefix pages of the launch in order of
+        first use (CUDA int32, None without a prefix), the page table renumbered to them ([n_seg, max prefix pages]) and the
+        bf16 scratch pools [max(1, n), H, 256, 128] they are dequantized into."""
+        host = page_table.cpu() if page_table_host is None else page_table_host
+        index, table = {}, []
+        for b, P in enumerate(seg.prefix_lens):
+            table.append([index.setdefault(int(host[b, i]), len(index)) for i in range(P // cache.PAGE_SIZE)])
+        width = max(1, max(len(r) for r in table))
+        renum = torch.zeros(len(table), width, dtype=torch.int32)
+        for b, r in enumerate(table):
+            renum[b, :len(r)] = torch.tensor(r, dtype=torch.int32)
+        dev = torch.cat([torch.tensor(list(index), dtype=torch.int32), renum.flatten()]).pin_memory().to(page_table.device,
+                                                                                                         non_blocking=True)
+        n = len(index)
+        _, H, rows, hd = cache.k[0].shape
+        scratch = torch.empty(2, max(1, n), H, rows, hd, dtype=bf16, device=page_table.device)
+        return (dev[:n] if n else None), dev[n:].view(len(table), width), scratch[0], scratch[1]
 
 
 class AriaMoELMForCausalLM(nn.Module):
@@ -963,11 +1023,11 @@ class AriaMoELMForCausalLM(nn.Module):
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h), cache
 
-    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None):
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None, page_table_host=None):
         """AriaMoELMModel.prefill_paged, then the final norm and lm_head on the last row of each segment listed in `ends`
         (segment indices in increasing order, the segments that end a prompt; None = every segment) -> logits [1, len(ends), V],
         row i those of forward(num_logits_to_keep=1) on the whole prompt of segment ends[i]."""
-        x, pending = self.model.prefill_paged(inputs_embeds, cache, page_table, seg, position_ids)
+        x, pending = self.model.prefill_paged(inputs_embeds, cache, page_table, seg, position_ids, page_table_host)
         ends = range(seg.n_seg) if ends is None else ends
         rows = [seg.cu[b + 1] - 1 for b in ends]
         if not rows:                                         # only chunks that end no prompt: no logits

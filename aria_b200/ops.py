@@ -1374,6 +1374,23 @@ def _paged_pool_check(k_pool: torch.Tensor, v_pool: torch.Tensor, what: str):
         raise RuntimeError(f"{what}: k_pool and v_pool must share one shape")
 
 
+def _paged_fp8_pool_check(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scale: Optional[torch.Tensor],
+                          v_scale: Optional[torch.Tensor], what: str):
+    """fp8 KV pages: e4m3 code pools k_pool / v_pool [n_pages, H, 256, 128] and fp32 scale pools k_scale / v_scale
+    [n_pages, H, 256], each contiguous, the code pools sharing one shape and the scale pools theirs."""
+    if k_scale is None or v_scale is None:
+        raise ValueError(f"{what}: fp8 (float8_e4m3fn) page pools need k_scale= and v_scale=")
+    for t in (k_pool, v_pool):
+        if not (t.is_cuda and t.dtype == fp8 and t.dim() == 4 and t.shape[2:] == (256, 128) and t.is_contiguous()
+                and t.data_ptr() % 16 == 0):
+            raise RuntimeError(f"{what}: fp8 page pools must be contiguous CUDA float8_e4m3fn [n_pages, H, 256, 128]")
+    for t in (k_scale, v_scale):
+        if not (t.is_cuda and t.dtype == torch.float32 and t.shape == k_pool.shape[:3] and t.is_contiguous()):
+            raise RuntimeError(f"{what}: k_scale / v_scale must be contiguous CUDA float32 [n_pages, H, 256]")
+    if k_pool.shape != v_pool.shape:
+        raise RuntimeError(f"{what}: k_pool and v_pool must share one shape")
+
+
 def _block_table_check(block_table: torch.Tensor, rows: int, what: str):
     """Block table: CUDA int32 [>= rows, max_pages] with contiguous rows (any row stride)."""
     if not (block_table.is_cuda and block_table.dtype == torch.int32 and block_table.dim() == 2 and block_table.stride(1) == 1
@@ -1382,12 +1399,19 @@ def _block_table_check(block_table: torch.Tensor, rows: int, what: str):
 
 
 def attention_decode_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, block_table: torch.Tensor,
-                           lens: torch.Tensor, scale: float) -> torch.Tensor:
+                           lens: torch.Tensor, scale: float, k_scale: Optional[torch.Tensor] = None,
+                           v_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """attention_decode_devlen over a paged cache: q [R, H, 128] (contiguous last dim), page pools [n_pages, H, 256, 128] bf16,
     block_table int32 [>= R, max_pages] (row r's key 256 s + i is row i of page block_table[r, s]; its columns are the splits the
     grid covers), lens int32 [R] -> out [R, H*128].  Row r is bit-identical to attention_decode_devlen on a contiguous cache
-    holding the same keys.  See aria_attention_decode_paged."""
-    _paged_pool_check(k_pool, v_pool, "attention_decode_paged")
+    holding the same keys.  With fp8 pools (float8_e4m3fn) k_scale / v_scale [n_pages, H, 256] fp32 are required and the fp8
+    kernel runs, bit-identical to the fp8 attention_decode_devlen on the same codes and scales.  See
+    aria_attention_decode_paged(_fp8)."""
+    is_fp8 = k_pool.dtype == fp8
+    if is_fp8:
+        _paged_fp8_pool_check(k_pool, v_pool, k_scale, v_scale, "attention_decode_paged")
+    else:
+        _paged_pool_check(k_pool, v_pool, "attention_decode_paged")
     _chk(lens, torch.int32, align=4)
     if not (q.is_cuda and q.dtype == bf16 and q.dim() == 3 and q.stride(-1) == 1 and q.data_ptr() % 8 == 0):
         raise RuntimeError("attention_decode_paged: q must be a CUDA bf16 [R, H, 128] tensor with a contiguous last dim")
@@ -1402,6 +1426,13 @@ def attention_decode_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.
     ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=q.device)
     out = torch.empty((R, H * 128), dtype=bf16, device=q.device)
     with torch.cuda.device(q.device):
+        if is_fp8:
+            L.check(lib.aria_attention_decode_paged_fp8(_p(q), _p(k_pool), _p(v_pool), _p(k_scale), _p(v_scale), _p(block_table),
+                                                        block_table.stride(0), max_pages, k_pool.shape[0], _p(lens), _p(out), R, H,
+                                                        q.stride(0), q.stride(1), k_pool.stride(0), k_pool.stride(1),
+                                                        k_scale.stride(0), k_scale.stride(1), scale, _p(ws), ws_bytes, _stream(q)),
+                    "attention_decode_paged_fp8")
+            return out
         L.check(lib.aria_attention_decode_paged(_p(q), _p(k_pool), _p(v_pool), _p(block_table), block_table.stride(0), max_pages,
                                                 k_pool.shape[0], _p(lens), _p(out), R, H, q.stride(0), q.stride(1),
                                                 k_pool.stride(0), k_pool.stride(1), scale, _p(ws), ws_bytes, _stream(q)),
@@ -1410,11 +1441,18 @@ def attention_decode_paged(q: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.
 
 
 def kv_append_paged(k_new: torch.Tensor, v_new: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor,
-                    block_table: torch.Tensor, write_pos: torch.Tensor):
+                    block_table: torch.Tensor, write_pos: torch.Tensor, k_scale: Optional[torch.Tensor] = None,
+                    v_scale: Optional[torch.Tensor] = None):
     """kv_append into a paged cache: k_new / v_new [R, H, 128] (128 contiguous, 16-byte aligned elements per row) go to row
     write_pos[r] % 256 of page block_table[r, write_pos[r] // 256] (write_pos CUDA int32 [R]).  A negative write_pos, one past
-    the table's columns, or an entry outside the pool writes nothing.  See aria_kv_append_paged."""
-    _paged_pool_check(k_pool, v_pool, "kv_append_paged")
+    the table's columns, or an entry outside the pool writes nothing.  With fp8 pools (k_scale / v_scale [n_pages, H, 256]
+    required) the rows are quantized as kv_append_fp8 quantizes them, and the null page 0 is never written either.  See
+    aria_kv_append_paged(_fp8)."""
+    is_fp8 = k_pool.dtype == fp8
+    if is_fp8:
+        _paged_fp8_pool_check(k_pool, v_pool, k_scale, v_scale, "kv_append_paged")
+    else:
+        _paged_pool_check(k_pool, v_pool, "kv_append_paged")
     _chk(write_pos, torch.int32, align=4)
     for t in (k_new, v_new):
         if not (t.is_cuda and t.dtype == bf16 and t.dim() == 3 and t.stride(-1) == 1 and t.data_ptr() % 16 == 0):
@@ -1426,6 +1464,13 @@ def kv_append_paged(k_new: torch.Tensor, v_new: torch.Tensor, k_pool: torch.Tens
     if k_new.shape[2] != 128 or k_pool.shape[1] != H or write_pos.shape != (R,):
         raise ValueError("kv_append_paged: the rows, pools and write_pos do not fit one another")
     with torch.cuda.device(k_pool.device):
+        if is_fp8:
+            L.check(L.load().aria_kv_append_paged_fp8(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_pool),
+                                                      _p(v_pool), _p(k_scale), _p(v_scale), k_pool.stride(0), k_pool.stride(1),
+                                                      k_scale.stride(0), k_scale.stride(1), _p(block_table), block_table.stride(0),
+                                                      block_table.shape[1], k_pool.shape[0], _p(write_pos), R, H, _stream(k_pool)),
+                    "kv_append_paged_fp8")
+            return
         L.check(L.load().aria_kv_append_paged(_p(k_new), _p(v_new), k_new.stride(0), k_new.stride(1), _p(k_pool), _p(v_pool),
                                               k_pool.stride(0), k_pool.stride(1), _p(block_table), block_table.stride(0),
                                               block_table.shape[1], k_pool.shape[0], _p(write_pos), R, H, _stream(k_pool)),
@@ -1545,23 +1590,54 @@ def attention_prefill_paged_varlen(q: torch.Tensor, k: torch.Tensor, v: torch.Te
 
 
 def kv_pages_store_varlen(k: torch.Tensor, v: torch.Tensor, k_pool: torch.Tensor, v_pool: torch.Tensor, page_table: torch.Tensor,
-                          seg: PackedSegments):
+                          seg: PackedSegments, k_scale: Optional[torch.Tensor] = None, v_scale: Optional[torch.Tensor] = None):
     """kv_pages_store for packed segments: row t of segment b of k / v [1, H, >= S_tot, 128] (bf16, contiguous) is position
     p = prefix_lens[b] + t - cu[b] of its request and goes to row p % 256 of page page_table[b, p // 256].  Writes nothing outside
     the listed pages and never the null page 0; each segment's pages are those kv_pages_store gives it alone.
-    See aria_kv_pages_store_varlen."""
+    With fp8 pools (k_scale / v_scale [n_pages, H, 256] required) the rows are quantized as kv_store_fp8 quantizes them, and
+    rows [0, S_tot) of k / v are overwritten in place with bf16(code * scale), the values a later read of the pages gives
+    (kv_pages_load_fp8).  See aria_kv_pages_store_varlen(_fp8)."""
     what = "kv_pages_store_varlen"
-    _paged_pool_check(k_pool, v_pool, what)
+    is_fp8 = k_pool.dtype == fp8
+    if is_fp8:
+        _paged_fp8_pool_check(k_pool, v_pool, k_scale, v_scale, what)
+    else:
+        _paged_pool_check(k_pool, v_pool, what)
     _chk(k), _chk(v)
     H, S_tot = k_pool.shape[1], seg.S_tot
     if k.dim() != 4 or k.shape[0] != 1 or k.shape[1] != H or k.shape[3] != 128 or v.shape != k.shape or k.shape[2] < S_tot:
         raise ValueError(f"{what}: k {tuple(k.shape)} must be [1, {H}, >= {S_tot}, 128] like v")
     _page_table_check(page_table, seg, True, what)
     with torch.cuda.device(k_pool.device):
+        if is_fp8:
+            L.check(L.load().aria_kv_pages_store_varlen_fp8(_p(k), _p(v), k.stride(1), S_tot, _p(k_pool), _p(v_pool), _p(k_scale),
+                                                            _p(v_scale), k_pool.stride(0), k_pool.stride(1), k_scale.stride(0),
+                                                            k_scale.stride(1), _p(page_table), page_table.stride(0),
+                                                            page_table.shape[1], k_pool.shape[0], _p(seg.prefix_dev),
+                                                            _p(seg.cu_dev), seg.n_seg, H, _stream(k_pool)), what + "_fp8")
+            return
         L.check(L.load().aria_kv_pages_store_varlen(_p(k), _p(v), k.stride(1), S_tot, _p(k_pool), _p(v_pool), k_pool.stride(0),
                                                     k_pool.stride(1), _p(page_table), page_table.stride(0), page_table.shape[1],
                                                     k_pool.shape[0], _p(seg.prefix_dev), _p(seg.cu_dev), seg.n_seg, H,
                                                     _stream(k_pool)), what)
+
+
+def kv_pages_load_fp8(k_pool: torch.Tensor, v_pool: torch.Tensor, k_scale: torch.Tensor, v_scale: torch.Tensor,
+                      pages: torch.Tensor, k_out: torch.Tensor, v_out: torch.Tensor):
+    """Dequantize pages pages[i] (CUDA int32 [n]) of fp8 page pools into page i of bf16 pools k_out / v_out [>= n, H, 256, 128]
+    (contiguous): bf16(code.float() * scale), the values kv_load_fp8 gives the same rows.  An entry outside the pool gives zeros.
+    See aria_kv_pages_load_fp8."""
+    what = "kv_pages_load_fp8"
+    _paged_fp8_pool_check(k_pool, v_pool, k_scale, v_scale, what)
+    _paged_pool_check(k_out, v_out, what)
+    _chk(pages, torch.int32, align=4)
+    H = k_pool.shape[1]
+    if pages.dim() != 1 or pages.numel() < 1 or k_out.shape[0] < pages.numel() or k_out.shape[1] != H:
+        raise ValueError(f"{what}: {tuple(pages.shape)} pages of {tuple(k_pool.shape)} do not fit {tuple(k_out.shape)}")
+    with torch.cuda.device(k_pool.device):
+        L.check(L.load().aria_kv_pages_load_fp8(_p(k_pool), _p(v_pool), _p(k_scale), _p(v_scale), k_pool.stride(0), k_pool.stride(1),
+                                                k_scale.stride(0), k_scale.stride(1), _p(pages), pages.numel(), k_pool.shape[0],
+                                                _p(k_out), _p(v_out), k_out.stride(0), k_out.stride(1), H, _stream(k_pool)), what)
 
 
 def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,

@@ -46,7 +46,14 @@ stops there, so at most one request is partly prefilled.  It holds its slot and 
 no poll retires it, and its first token is sampled after its last chunk.  Pages are keyed as their chunk is staged; a head
 whose hit would read a page of a launch not yet run waits for that launch, so the hits are those of one-at-a-time admission.
 
-The scheduler (Scheduler, PageAllocator) and the page keys are plain host code with no device calls.  GPU only; bf16 KV pages; no expert
+FP8 KV pages (kv_cache_dtype="fp8"): the pages hold e4m3 keys and values with one fp32 scale per (page, head, row), quantized
+as generate()'s fp8 KV cache quantizes them, so the same pool holds about twice the tokens.  Every query attends to every key as
+bf16(code * scale), the keys of its own prefill chunk included: a prefill stores its rows into the pages first and attends to
+their dequantized values, and reads a cached prefix, or its prompt's earlier chunks, as the same values.  A result therefore
+does not depend on chunking or cache hits either.  It equals generate(kv_cache_dtype="fp8") with that one rule applied to its
+prefill; decode steps use the contiguous fp8 decode arithmetic (ops.attention_decode_paged: a page is one split).
+
+The scheduler (Scheduler, PageAllocator) and the page keys are plain host code with no device calls.  GPU only; no expert
 parallelism.  Fp8 or bf16 expert and dense weights are fine (they live inside the layers).
 """
 from __future__ import annotations
@@ -357,9 +364,13 @@ class Engine:
     max_batch: decode slots (<= 1024).  max_kv_tokens: KV cache capacity in tokens, rounded up to 256-token pages (plus the
     null page); a request needs ceil((prompt + max_new_tokens) / 256) pages.  eos_token_id / pad_token_id: as generate()'s, for
     every request.  poll_every: decode steps between two looks at the finished flags.
-    Memory: the page pools (2 x layers x heads x 128 bf16 values per token of max_kv_tokens, plus the null page), and one int32
+    kv_cache_dtype: "bf16" (default) or "fp8" KV pages (see the module docstring); max_kv_tokens counts tokens either way.
+    Memory: the page pools (2 x layers x heads x 128 bf16 values per token of max_kv_tokens, plus the null page; with fp8 pages
+    2 x layers x heads x (128 one-byte codes + one 4-byte scale) per token, 132 bytes where bf16 takes 256), and one int32
     output row per slot as long as the pool, since a request may spend the whole pool on its budget: 4 x max_batch x
-    256 ceil(max_kv_tokens / 256) bytes (32 MiB at the defaults, 4 GiB at 1024 slots and a 2^20-token pool).
+    256 ceil(max_kv_tokens / 256) bytes (32 MiB at the defaults, 4 GiB at 1024 slots and a 2^20-token pool).  An fp8 prefill
+    whose segments have a cached prefix also holds, while it runs, a bf16 scratch copy of the launch's distinct prefix pages:
+    2 x heads x 256 x 128 x 2 bytes per page (2.6 MB at 20 heads), shared by the layers.
     `stats`: graphs captured, decode steps replayed, slot-steps of active requests (mean occupancy = active_slot_steps /
     (steps * max_batch); a partly prefilled request is not counted), host seconds spent waiting in polls; prefix caching: prompt tokens admitted, those found in cached
     pages (prefix_hit_tokens), pixel rows the ViT ran on and skipped, cached pages evicted; admission: packed prefills run
@@ -372,8 +383,10 @@ class Engine:
     max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS
 
     def __init__(self, model, max_batch: int = 64, max_kv_tokens: int = 131072, eos_token_id=None, pad_token_id=None,
-                 poll_every: int = 8, max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS):
-        from .moe_lm import PagedKVCache, SlotDecodeState
+                 poll_every: int = 8, max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS, kv_cache_dtype: str = "bf16"):
+        from .moe_lm import KV_CACHE_DTYPES, PagedKVCache, SlotDecodeState
+        if not isinstance(kv_cache_dtype, str) or kv_cache_dtype not in KV_CACHE_DTYPES:
+            raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
         if max_prefill_tokens is not None and (not isinstance(max_prefill_tokens, int) or max_prefill_tokens < PAGE
                                                or max_prefill_tokens % PAGE):
             raise ValueError(f"max_prefill_tokens must be None or a positive multiple of {PAGE}, got {max_prefill_tokens!r}")
@@ -398,7 +411,9 @@ class Engine:
         self.max_pages = _pages_for(max_kv_tokens)
         n_pages = self.max_pages + 1
         self.sched = Scheduler(max_batch, n_pages)
-        self.cache = PagedKVCache(c.num_hidden_layers, n_pages, c.num_attention_heads, c.head_dim, max_batch, self.max_pages, dev)
+        self.kv_cache_dtype = kv_cache_dtype
+        self.cache = PagedKVCache(c.num_hidden_layers, n_pages, c.num_attention_heads, c.head_dim, max_batch, self.max_pages, dev,
+                                  kv_cache_dtype)
         self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev)
         self._idle(0, max_batch)
         self.rope = lm.model.rope_tables(self.max_pages * PAGE, dev)   # held here: the graphs read these tables
@@ -624,7 +639,7 @@ class Engine:
         for b, req in enumerate(staged):
             if req.pixel_values is not None:
                 self._merge_images(req, ids_dev[cu[b]:cu[b + 1]], emb[0, cu[b]:cu[b + 1]])
-        logits = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends)
+        logits = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends, page_table_host=table)
         self.stats["prefill_launches"] += 1
         self.stats["prefill_chunks"] += len(staged) - len(ends)
         for i, b in enumerate(ends):

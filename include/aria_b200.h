@@ -413,6 +413,16 @@ int aria_attention_decode_paged(const void* q, const void* k_pool, const void* v
                                 int64_t block_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* lens, void* out,
                                 int32_t R, int32_t H, int64_t q_stride_b, int64_t q_stride_h, int64_t page_stride,
                                 int64_t pool_stride_h, float scale, void* workspace, int64_t workspace_bytes, aria_stream_t stream);
+/* aria_attention_decode_paged over fp8 KV pages: k_pool / v_pool e4m3 codes [n_pages, H, 256, 128] (element = byte strides
+ * page_stride / pool_stride_h, multiples of 16) and k_scale / v_scale fp32 [n_pages, H, 256] (strides scale_page_stride /
+ * scale_stride_h), one scale per (page, head, row).  Split s of row r reads page block_table[r, s] and its scale rows, with the
+ * arithmetic of aria_attention_decode_devlen_fp8: row r is bit-identical to that entry on a contiguous cache holding the same
+ * codes and scales (no key mask).  Same block table, lens, q, out and workspace contracts as aria_attention_decode_paged. */
+int aria_attention_decode_paged_fp8(const void* q, const void* k_pool, const void* v_pool, const float* k_scale, const float* v_scale,
+                                    const int32_t* block_table, int64_t block_table_stride, int32_t max_pages, int32_t n_pages,
+                                    const int32_t* lens, void* out, int32_t R, int32_t H, int64_t q_stride_b, int64_t q_stride_h,
+                                    int64_t page_stride, int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h,
+                                    float scale, void* workspace, int64_t workspace_bytes, aria_stream_t stream);
 /* aria_attention_decode / aria_attention_decode_devlen over an fp8 KV cache: k, v are e4m3 codes [B,H,T_max,128] (element = byte
  * strides kv_stride_b / kv_stride_h, multiples of 16), k_scale / v_scale fp32 [B,H,T_max] at scale_stride_b / scale_stride_h, one
  * scale per (row, head, token): key t of (b, h) is code * scale.  The key scale multiplies the reduced dot product q.code and the
@@ -591,6 +601,32 @@ int aria_kv_pages_store_varlen(const void* k, const void* v, int64_t src_stride_
                                int64_t page_stride, int64_t pool_stride_h, const int32_t* page_table, int64_t page_table_stride,
                                int32_t max_pages, int32_t n_pages, const int32_t* prefix_lens, const int32_t* cu_seqlens,
                                int32_t n_seg, int32_t H, aria_stream_t stream);
+/* fp8 KV pages: e4m3 code pools k_pool / v_pool [n_pages, H, 256, 128] and fp32 scale pools k_scale / v_scale [n_pages, H, 256]
+ * (strides as aria_attention_decode_paged_fp8's), with the quantiser and dequantiser of aria_kv_store_fp8 / aria_kv_load_fp8.
+ * aria_kv_append_paged_fp8: aria_kv_append_paged that quantises: row r of k_new / v_new goes to row write_pos[r] % 256 of page
+ *   block_table[r, write_pos[r] / 256] with the codes and scale aria_kv_append_fp8 gives it.  Nothing is written for a negative
+ *   write_pos, one at or past 256 * max_pages, a table entry outside [0, n_pages), or the null page 0. */
+int aria_kv_append_paged_fp8(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_pool,
+                             void* v_pool, float* k_scale, float* v_scale, int64_t page_stride, int64_t pool_stride_h,
+                             int64_t scale_page_stride, int64_t scale_stride_h, const int32_t* block_table,
+                             int64_t block_table_stride, int32_t max_pages, int32_t n_pages, const int32_t* write_pos, int32_t R,
+                             int32_t H, aria_stream_t stream);
+/* aria_kv_pages_store_varlen that quantises: packed row t of segment b (k / v [1, H, >= S_tot, 128] bf16, head stride
+ * src_stride_h) goes to the page row aria_kv_pages_store_varlen gives it, as codes and a scale, and bf16(code * scale) is written
+ * back over the source row in place (every row), so attention over k / v then reads what the pages hold.  Never writes the null
+ * page 0 nor a page that is not listed. */
+int aria_kv_pages_store_varlen_fp8(void* k, void* v, int64_t src_stride_h, int32_t S_tot, void* k_pool, void* v_pool, float* k_scale,
+                                   float* v_scale, int64_t page_stride, int64_t pool_stride_h, int64_t scale_page_stride,
+                                   int64_t scale_stride_h, const int32_t* page_table, int64_t page_table_stride, int32_t max_pages,
+                                   int32_t n_pages, const int32_t* prefix_lens, const int32_t* cu_seqlens, int32_t n_seg, int32_t H,
+                                   aria_stream_t stream);
+/* Dequantise pages pages[i] (DEVICE int32 [n_list]) of the fp8 pools into page i of bf16 pools k_out / v_out [n_list, H, 256, 128]
+ * (strides out_page_stride / out_stride_h, multiples of 8): bf16(code * scale), aria_kv_load_fp8's values.  An entry outside
+ * [0, n_pages) gives zeros. */
+int aria_kv_pages_load_fp8(const void* k_pool, const void* v_pool, const float* k_scale, const float* v_scale, int64_t page_stride,
+                           int64_t pool_stride_h, int64_t scale_page_stride, int64_t scale_stride_h, const int32_t* pages,
+                           int32_t n_list, int32_t n_pages, void* k_out, void* v_out, int64_t out_page_stride,
+                           int64_t out_stride_h, int32_t H, aria_stream_t stream);
 /* aria_sample_tokens_rows with every sampling parameter per row, from DEVICE arrays [R]: temperature (0 = greedy), top_k, top_p,
  * seed (uint64), noise row and offset.  Row r is bit-identical to aria_sample_tokens run alone on that row with its scalars at
  * rng_offset = offsets[r] as row noise_rows[r].  The caller checks the parameters as aria_sample_tokens does; out-of-range
