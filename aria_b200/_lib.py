@@ -139,6 +139,7 @@ SIGNATURES = {
     "aria_kv_pages_load_fp8": (i32, [vp, vp, vp, vp, i64, i64, i64, i64, vp, i32, i32, vp, vp, i64, i64, i32, vp]),
     "aria_sample_tokens_slots": (i32, [vp, i64, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
     "aria_decode_advance_slots": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp]),
+    "aria_token_logprobs": (i32, [vp, i64, vp, i32, i32, i32, vp, vp, i32, i32, vp, i32, vp, vp, vp, i32, vp]),
 }
 
 _lib = None

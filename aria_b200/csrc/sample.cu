@@ -20,6 +20,9 @@
 // of a prompt-lookup verification step draws the noise generation row b draws for its token n_out[b] + i.
 // aria_sample_tokens_slots: aria_sample_tokens_rows with the temperature, top_k, top_p and seed of each row also read from
 // device arrays (continuous batching: every slot samples with its own request's parameters).
+//
+// aria_token_logprobs: the log-probability of a token under a row's raw distribution and the row's top n (n <= 20) by (value
+// desc, id asc), one CTA per row, reusing the radix select above (see token_logprobs_kernel).
 #include <float.h>
 #include <limits.h>
 
@@ -361,6 +364,237 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
   if (tid == 0) p.next_ids[row] = bi;
 }
 
+// ---------------------------------------------------------------------------------------------------- token log-probabilities
+constexpr int LP_MAX_N = 20;
+
+struct LogprobParams {
+  const uint16_t* logits;  // bf16 bits, row r at logits + r * stride
+  int64_t stride;
+  const int64_t* tokens;   // [R]
+  const int32_t* n_row;    // [R] or NULL (every row n_max); -1 skips the row
+  const int32_t* col;      // output column: col[r] (col_per_row) or col[0]; NULL: column 0
+  int col_per_row;
+  int ring;                // > 0: column col mod ring
+  const uint8_t* finished; // [R] or NULL
+  int finished_fill;       // finished rows: 1 write the filler, 0 leave untouched
+  float* lp;               // [R, cols]
+  int32_t* top_ids;        // [R, cols, n_max]
+  float* top_lp;           // [R, cols, n_max]
+  int cols, n_max, V;
+};
+
+// (m, s) <- the pair over the union; an empty side has m = -inf.  The compiler may contract one of the two products into an
+// FMA, so the two lanes of a butterfly exchange can round differently: the caller takes one lane's result (lp_pass1).  expf,
+// not __expf: the sum decides every logprob's last bits.
+__device__ __forceinline__ void lp_merge(float& m, float& s, float m2, float s2) {
+  if (m2 == -INFINITY) return;
+  if (m == -INFINITY) {
+    m = m2;
+    s = s2;
+    return;
+  }
+  const float M = fmaxf(m, m2);
+  s = s * expf(m - M) + s2 * expf(m2 - M);
+  m = M;
+}
+
+// one 8-element chunk of the row into the thread's (max, sum of exp) and, with HIST, the high-byte key histogram
+template <bool HIST>
+__device__ __forceinline__ void lp_add8(float& m, float& s, const uint32_t (&u)[8], int valid, SampleSmem& sm) {
+  float x[8];
+  float vm = -INFINITY;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    x[j] = j < valid ? __uint_as_float(u[j] << 16) : -INFINITY;
+    vm = fmaxf(vm, x[j]);
+    if (HIST && j < valid) atomicAdd(&sm.hist[bf16_key(u[j]) >> 8], 1u);
+  }
+  if (vm == -INFINITY) return;  // nothing to add (also keeps -inf - -inf out of the exponents)
+  if (vm > m) {
+    s *= expf(m - vm);          // m = -inf: s is 0 already
+    m = vm;
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) s += expf(x[j] - m);
+}
+
+// Chunk c (elements 8c .. 8c + 7) of a row always belongs to thread c mod SP_THREADS and is added in increasing c, whether it
+// is read with one 128-bit load (a 16-byte aligned row) or with scalar loads, so the sum does not depend on the row's address.
+template <bool HIST>
+__device__ void lp_pass1(const uint16_t* __restrict__ x, int V, float& m, float& s, SampleSmem& sm) {
+  const int tid = threadIdx.x, n_full = V >> 3;
+  m = -INFINITY;
+  s = 0.f;
+  uint32_t u[8];
+  if ((reinterpret_cast<uintptr_t>(x) & 15) == 0) {
+    const uint4* row = reinterpret_cast<const uint4*>(x);
+    int c = tid;
+    for (; c + 3 * SP_THREADS < n_full; c += 4 * SP_THREADS) {
+      uint4 q[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) q[i] = __ldg(row + c + i * SP_THREADS);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const uint32_t a[4] = {q[i].x, q[i].y, q[i].z, q[i].w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) u[2 * j] = a[j] & 0xFFFFu, u[2 * j + 1] = a[j] >> 16;
+        lp_add8<HIST>(m, s, u, 8, sm);
+      }
+    }
+    for (; c < n_full; c += SP_THREADS) {
+      const uint4 q = __ldg(row + c);
+      const uint32_t a[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) u[2 * j] = a[j] & 0xFFFFu, u[2 * j + 1] = a[j] >> 16;
+      lp_add8<HIST>(m, s, u, 8, sm);
+    }
+  } else {
+    for (int c = tid; c < n_full; c += SP_THREADS) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) u[j] = x[8 * c + j];
+      lp_add8<HIST>(m, s, u, 8, sm);
+    }
+  }
+  if ((V & 7) && tid == n_full % SP_THREADS) {  // the scalar tail, the last chunk of its thread
+#pragma unroll
+    for (int j = 0; j < 8; ++j) u[j] = 8 * n_full + j < V ? x[8 * n_full + j] : 0u;
+    lp_add8<HIST>(m, s, u, V & 7, sm);
+  }
+  // fixed-order merge: xor butterfly in each warp, then the same over the warps' pairs
+#pragma unroll
+  for (int o = 16; o; o >>= 1) lp_merge(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+  const int lane = tid & 31, warp = tid >> 5;
+  __syncthreads();
+  if (lane == 0) sm.red_f[warp] = m, sm.red_i[warp] = __float_as_int(s);
+  __syncthreads();
+  m = lane < SP_WARPS ? sm.red_f[lane] : -INFINITY;
+  s = lane < SP_WARPS ? __int_as_float(sm.red_i[lane]) : 0.f;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) lp_merge(m, s, __shfl_xor_sync(0xffffffffu, m, o), __shfl_xor_sync(0xffffffffu, s, o));
+  // lane 0 of every warp ran the same operations on the same values: its pair is the row's, in every thread, so the token's
+  // logprob (thread 0) and each top entry's (thread j) use the same m and log(s)
+  m = __shfl_sync(0xffffffffu, m, 0);
+  s = __shfl_sync(0xffffffffu, s, 0);
+}
+
+// logprob of token t in row x: (x_t - m) - log(s), the row's raw distribution.  Top n: the n largest logits by (value desc, id
+// asc), found by the radix select of sample_body (find_bin on the high, then the low byte of the 16-bit key); the keys above
+// the pivot (< n of them) and the lowest-id pivot ties are compacted and bitonic-sorted.  A row's result depends only on its
+// logits, its token and its n.
+__global__ void __launch_bounds__(SP_THREADS, 1) token_logprobs_kernel(const LogprobParams p) {
+  __shared__ SampleSmem sm;
+  const int tid = threadIdx.x, row = blockIdx.x, V = p.V;
+  int n = p.n_max;
+  if (p.n_row) {
+    n = p.n_row[row];
+    if (n < 0) return;
+    n = min(n, p.n_max);
+  }
+  int c = 0;
+  if (p.col) {
+    c = p.col[p.col_per_row ? row : 0];
+    if (p.ring > 0) c = ((c % p.ring) + p.ring) % p.ring;
+    if (c < 0 || c >= p.cols) return;
+  }
+  const int64_t o = static_cast<int64_t>(row) * p.cols + c;
+  float* top_lp = p.top_lp + o * p.n_max;
+  int32_t* top_ids = p.top_ids + o * p.n_max;
+  if (p.finished && p.finished[row]) {
+    if (!p.finished_fill) return;
+    if (tid == 0) p.lp[o] = 0.f;
+    for (int j = tid; j < p.n_max; j += SP_THREADS) top_ids[j] = -1, top_lp[j] = -INFINITY;
+    return;
+  }
+  const uint16_t* x = p.logits + static_cast<int64_t>(row) * p.stride;
+  const int ne = min(n, V);  // real top entries; [ne, n_max) get the filler
+  if (ne > 0)
+    for (int i = tid; i < 256; i += SP_THREADS) sm.hist[i] = 0;
+  if (tid == 0) sm.n_list = 0;
+  __syncthreads();
+  float m, s;
+  if (ne > 0)
+    lp_pass1<true>(x, V, m, s, sm);
+  else
+    lp_pass1<false>(x, V, m, s, sm);
+  const float log_s = logf(s);  // s >= 1: the maximum contributes exp(0)
+  if (tid == 0) {
+    const int64_t t = p.tokens[row];
+    p.lp[o] = t >= 0 && t < V ? (__uint_as_float(static_cast<uint32_t>(x[t]) << 16) - m) - log_s : __int_as_float(0x7fc00000);
+  }
+  for (int j = ne + tid; j < p.n_max; j += SP_THREADS) top_ids[j] = -1, top_lp[j] = -INFINITY;
+  if (ne == 0) return;
+
+  // ---- the ne-th largest key: high byte (histogram filled by pass 1), then the low byte within it
+  find_bin(sm, ne);
+  const uint32_t hb = sm.bin;
+  const int above_hi = sm.above;
+  for (int i = tid; i < 256; i += SP_THREADS) sm.hist[i] = 0;
+  __syncthreads();
+  for (int i = tid; i < V; i += SP_THREADS) {
+    const uint32_t key = bf16_key(x[i]);
+    if ((key >> 8) == hb) atomicAdd(&sm.hist[key & 0xFF], 1u);
+  }
+  find_bin(sm, ne - above_hi);
+  const uint32_t pivot = (hb << 8) | sm.bin;
+  const int n_gt = above_hi + sm.above;        // < ne
+  const int n_tie = static_cast<int>(sm.hist[sm.bin]);
+  const int need = ne - n_gt;                  // pivot ties taken, the lowest ids first
+  // ---- compact: entries (~key << 32 | id) sort ascending as (value desc, id asc)
+  const bool all_ties = n_tie <= SP_MAX_K - LP_MAX_N;  // else only the first `need` ties in id order, by an ordered scan
+  for (int i = tid; i < V; i += SP_THREADS) {
+    const uint32_t key = bf16_key(x[i]);
+    if (key > pivot || (all_ties && key == pivot))
+      sm.list[atomicAdd(&sm.n_list, 1)] = (static_cast<unsigned long long>(0xFFFFu - key) << 32) | static_cast<uint32_t>(i);
+  }
+  int total = n_gt + n_tie;
+  if (!all_ties) {
+    total = ne;
+    const int lane = tid & 31, warp = tid >> 5;
+    const unsigned long long piv = static_cast<unsigned long long>(0xFFFFu - pivot) << 32;
+    int base = 0;
+    for (int i0 = 0; i0 < V && base < need; i0 += SP_THREADS) {
+      const int i = i0 + tid;
+      const bool t = i < V && bf16_key(x[i]) == pivot;
+      const unsigned bal = __ballot_sync(0xffffffffu, t);
+      __syncthreads();
+      if (lane == 0) sm.red_i[warp] = __popc(bal);
+      __syncthreads();
+      int before = base + __popc(bal & ((1u << lane) - 1u)), sum = 0;
+      for (int w = 0; w < SP_WARPS; ++w) {
+        const int cnt = sm.red_i[w];
+        if (w < warp) before += cnt;
+        sum += cnt;
+      }
+      if (t && before < need) sm.list[n_gt + before] = piv | static_cast<uint32_t>(i);
+      base += sum;
+    }
+  }
+  __syncthreads();
+  int P = 1;
+  while (P < total) P <<= 1;
+  for (int i = total + tid; i < P; i += SP_THREADS) sm.list[i] = ~0ull;
+  for (int size = 2; size <= P; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      __syncthreads();
+      const int i = tid, j = tid ^ stride;
+      if (i < P && j > i) {
+        const unsigned long long a = sm.list[i], b = sm.list[j];
+        if ((a > b) == ((i & size) == 0)) {
+          sm.list[i] = b;
+          sm.list[j] = a;
+        }
+      }
+    }
+  }
+  __syncthreads();
+  if (tid < ne) {
+    const unsigned long long e = sm.list[tid];
+    const uint32_t key = 0xFFFFu - static_cast<uint32_t>(e >> 32);
+    top_ids[tid] = static_cast<int32_t>(e & 0xFFFFFFFFu);
+    top_lp[tid] = (key_to_float(key) - m) - log_s;
+  }
+}
+
 __global__ void __launch_bounds__(SP_THREADS, 1) sample_kernel(const SampleParams p) {
   sample_body<false>(p, nullptr, nullptr);
 }
@@ -433,4 +667,33 @@ extern "C" int aria_sample_tokens_slots(const void* logits, int64_t logits_strid
   sample_slots_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p, noise_rows, offsets,
                                                                                       SlotSampling{temperature, top_k, top_p, seed});
   return check_launch("sample_slots_kernel");
+}
+
+extern "C" int aria_token_logprobs(const void* logits, int64_t logits_stride, const int64_t* tokens, int32_t R, int32_t V,
+                                   int32_t n_max, const int32_t* n_row, const int32_t* col, int32_t col_per_row, int32_t ring,
+                                   const uint8_t* finished, int32_t finished_fill, float* logprobs, int32_t* top_ids,
+                                   float* top_logprobs, int32_t cols, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(logits && tokens && logprobs);
+  ARIA_CHECK_ARG(R > 0 && R <= SP_MAX_ROWS && V > 0 && V <= SP_MAX_VOCAB && logits_stride >= 0);
+  ARIA_CHECK_ARG(n_max >= 0 && n_max <= LP_MAX_N && (n_max == 0 || (top_ids && top_logprobs)));
+  ARIA_CHECK_ARG(cols >= 1 && ring >= 0 && ring <= cols && (col || (ring == 0 && col_per_row == 0)));
+  ARIA_CHECK_ARG(finished_fill == 0 || finished_fill == 1);
+  LogprobParams p{};
+  p.logits = static_cast<const uint16_t*>(logits);
+  p.stride = logits_stride;
+  p.tokens = tokens;
+  p.n_row = n_row;
+  p.col = col;
+  p.col_per_row = col_per_row != 0;
+  p.ring = ring;
+  p.finished = finished;
+  p.finished_fill = finished_fill;
+  p.lp = logprobs;
+  p.top_ids = top_ids;
+  p.top_lp = top_logprobs;
+  p.cols = cols;
+  p.n_max = n_max;
+  p.V = V;
+  token_logprobs_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
+  return check_launch("token_logprobs_kernel");
 }

@@ -9,12 +9,13 @@ autograd through this class (inference hot path; training = moe_train / lora), t
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 import torch.nn as nn
 
 from . import ops
+from .ops import MAX_LOGPROBS
 from .moe_lm import KV_CACHE_DTYPES, AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16
 from .projector import AriaProjector
 from .vision_encoder import AriaVisionConfig, AriaVisionModel
@@ -343,7 +344,8 @@ class AriaForConditionalGeneration(nn.Module):
                  do_sample: bool = False, temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, eos_token_id=None,
                  pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16",
                  num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None,
-                 prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None):
+                 prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None,
+                 output_logprobs: Optional[int] = None):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -375,12 +377,20 @@ class AriaForConditionalGeneration(nn.Module):
         the logits and the sampling noise of the plain step that would emit that token.  Not combined with
         num_return_sequences > 1, shared_prefix_len or the fp8 KV cache; B * (K + 1) <= 1024; GPU only.  The host waits for every
         step (poll_every does not apply); the call's counters are in self.prompt_lookup_stats.
-        Returns [B * n, T + generated] int64 on the model's device (prompt ids first)."""
+        output_logprobs k (None, or an int in [0, 20]): also the log-probability of every generated token under the model's raw
+        distribution (before temperature, top-k and top-p) and the k most likely tokens of each step, ties to the lowest id
+        (ops.token_logprobs, run inside the captured step).  Positions after a row's EOS hold logprob 0, ids -1 and logprobs
+        -inf, so a row's logprobs sum to the log-likelihood of its sequence up to and including EOS.  GPU only; not combined
+        with prompt_lookup_num_tokens.
+        Returns [B * n, T + generated] int64 on the model's device (prompt ids first); with output_logprobs a GenerateOutput
+        (sequences: that tensor; logprobs [B * n, L] fp32, top_ids [B * n, L, k] int64, top_logprobs [B * n, L, k] fp32, L the
+        generated length)."""
         B, T, eos, pad = self._check_generate_args(input_ids, max_new_tokens, attention_mask, do_sample, temperature, top_k,
                                                    top_p, eos_token_id, pad_token_id, seed, poll_every, kv_cache_dtype,
                                                    num_return_sequences, shared_prefix_len)
         n_seq = num_return_sequences
         dev = self.device
+        self._check_output_logprobs(output_logprobs, prompt_lookup_num_tokens, dev)
         if prompt_lookup_num_tokens is not None:
             K, M = self._check_prompt_lookup(B, prompt_lookup_num_tokens, max_matching_ngram_size, n_seq, shared_prefix_len,
                                              kv_cache_dtype, dev)
@@ -394,7 +404,7 @@ class AriaForConditionalGeneration(nn.Module):
                 raise NotImplementedError("aria_b200: shared_prefix_len runs on the GPU only")
             sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
             return self._generate_shared_prefix(input_ids, ids_host, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos,
-                                                pad, poll_every, n_seq, shared_prefix_len)
+                                                pad, poll_every, n_seq, shared_prefix_len, output_logprobs)
         if dev.type != "cuda":
             if do_sample or eos:
                 raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
@@ -410,9 +420,10 @@ class AriaForConditionalGeneration(nn.Module):
         T_max = -(-(T if n_seq > 1 else T + max_new_tokens) // 256) * 256
         key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, None, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
-            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype, n_seq)
+            g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype, n_seq,
+                                                   logprobs=output_logprobs)
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
                                                     attention_mask=mask, num_logits_to_keep=1)
@@ -426,10 +437,10 @@ class AriaForConditionalGeneration(nn.Module):
         if n_seq == 1:
             g.cache.seq_len = T + n             # a shared cache keeps the prompt's T; the tails hold the rest
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
-        return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
+        return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
 
     def _generate_shared_prefix(self, input_ids, ids, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos, pad,
-                                poll_every, n_seq, P):
+                                poll_every, n_seq, P, output_logprobs=None):
         """generate(shared_prefix_len=P) on checked arguments (ids: the host copy of input_ids, lens: each row's real length,
         from _check_shared_prefix): ViT + prefix prefill (forward()) into a SharedPrefixCache of one prompt row, the packed
         suffix prefill (AriaMoELMModel.prefill_suffixes), the first token from each suffix's last position, then the graphed
@@ -448,10 +459,10 @@ class AriaForConditionalGeneration(nn.Module):
         N_max = -(-(max(S) + max_new_tokens) // 256) * 256
         key = (1, T_max, max_new_tokens, sampling, eos, pad, dev, B * n_seq, N_max, "bf16")
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs:
             self._decode_graph = g = None
             g = self._decode_graph = GraphedDecode(self, 1, T_max, max_new_tokens, sampling, eos, pad, "bf16", B * n_seq,
-                                                   N_max=N_max)
+                                                   N_max=N_max, logprobs=output_logprobs)
         g.cache.seq_len = 0
         self.forward(prefix, pixel_values, pixel_mask, past_key_values=g.cache, num_logits_to_keep=1)
         cu_dev = cu.to(dev, non_blocking=True)
@@ -464,7 +475,7 @@ class AriaForConditionalGeneration(nn.Module):
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         _, L = g.run(max_new_tokens, poll_every)
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
-        return torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1)
+        return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
 
     def _generate_prompt_lookup(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask, sampling, eos, pad,
                                 K, M):
@@ -564,6 +575,19 @@ class AriaForConditionalGeneration(nn.Module):
         return B, T, eos, pad_token_id
 
     @staticmethod
+    def _check_output_logprobs(k, prompt_lookup_num_tokens, device):
+        """generate(output_logprobs=k)'s checks after _check_generate_args', on the host: k (ValueError), then prompt lookup and
+        a CPU device (NotImplementedError)."""
+        if k is None:
+            return
+        if not isinstance(k, int) or isinstance(k, bool) or not 0 <= k <= MAX_LOGPROBS:
+            raise ValueError(f"output_logprobs must be None or an int in [0, {MAX_LOGPROBS}], got {k!r}")
+        if prompt_lookup_num_tokens is not None:
+            raise NotImplementedError("output_logprobs with prompt_lookup_num_tokens is not supported")
+        if torch.device(device).type != "cuda":
+            raise NotImplementedError("aria_b200: output_logprobs runs on the GPU only")
+
+    @staticmethod
     def _check_prompt_lookup(B, K, M, n, shared_prefix_len, kv_cache_dtype, device):
         """generate(prompt_lookup_num_tokens=K, max_matching_ngram_size=M)'s checks after _check_generate_args', in this order:
         K, M (ValueError), then num_return_sequences > 1, shared_prefix_len, the fp8 KV cache, a CPU device and B * (K + 1) > 1024
@@ -621,6 +645,17 @@ class AriaForConditionalGeneration(nn.Module):
         return ids, lens
 
 
+class GenerateOutput(NamedTuple):
+    """generate(output_logprobs=k)'s result: `sequences` as generate() returns it without logprobs ([B * n, T + L] int64), and
+    per generated position the token's logprob under the raw distribution, logprobs [B * n, L] fp32, with the k most likely
+    tokens, top_ids [B * n, L, k] int64 and top_logprobs [B * n, L, k] fp32 (ops.token_logprobs).  Positions after a row's EOS
+    hold 0, -1 and -inf."""
+    sequences: torch.Tensor
+    logprobs: torch.Tensor
+    top_ids: torch.Tensor
+    top_logprobs: torch.Tensor
+
+
 class GraphedDecode:
     """One decode step captured as a CUDA graph and replayed token after token (AriaForConditionalGeneration.generate).
 
@@ -633,10 +668,13 @@ class GraphedDecode:
     group_size n > 1: B prompts decoded n times each.  The cache is a SharedPrefixCache of B prompt rows of T_max (the prompt
     bucket) and B * n tails of max_new_tokens rounded up to 256; the state, tokens and logits have B * n rows.
     N_max (generate(shared_prefix_len=...)): a SharedPrefixCache whose tails hold N_max rows (a multiple of 256), each row's
-    own prompt tokens and then its generated ones, for any group size."""
+    own prompt tokens and then its generated ones, for any group size.
+    logprobs k (generate(output_logprobs=k)): the step also runs ops.token_logprobs on the sampled tokens between the sampler and
+    the advance, into column `step` of lp [B, max_new_tokens], top_ids and top_lp [B, max_new_tokens, k]; rows finished before
+    the step get the filler.  None: the step is exactly the one without logprobs."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
-                 kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None):
+                 kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None, logprobs: Optional[int] = None):
         from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
         dev = model.device
         lm = model.language_model
@@ -665,6 +703,11 @@ class GraphedDecode:
         self.done_step = torch.full((1,), -1, dtype=torch.int32, device=dev)
         self.finished = torch.zeros(B, dtype=torch.uint8, device=dev)
         self.out_tokens = torch.zeros(B, max_new_tokens, dtype=torch.int64, device=dev)
+        self.n_logprobs = logprobs
+        if logprobs is not None:
+            self.lp = torch.zeros(B, max_new_tokens, dtype=torch.float32, device=dev)
+            self.top_ids = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.int32, device=dev)
+            self.top_lp = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.float32, device=dev)
         self.done_host = torch.full((1,), -1, dtype=torch.int32).pin_memory()
         self.event = torch.cuda.Event()
         self.dev = dev
@@ -689,10 +732,19 @@ class GraphedDecode:
         """Sample from logits [B, V] into next_ids, then advance the state (also the eager first token after the prefill)."""
         t, k, p, seed = self.sampling
         ops.sample_tokens(logits, t, k, p, seed, self.rng_offset, out=self.next_ids)
+        if self.n_logprobs is not None:
+            ops.token_logprobs(logits, self.next_ids, self.n_logprobs, col=self.step, finished=self.finished,
+                               out=(self.lp, self.top_ids, self.top_lp))
         st = self.state
         ops.decode_advance(self.next_ids, self.ids, self.out_tokens, self.step, st.rope_pos, st.write_pos, st.kv_len,
                            self.rng_offset, self.finished, self.done_step, self.eos, self.pad)
         self.done_host.copy_(self.done_step, non_blocking=True)
+
+    def result(self, sequences: torch.Tensor, L: int):
+        """generate()'s return value: sequences alone, or with logprobs a GenerateOutput of the first L columns."""
+        if self.n_logprobs is None:
+            return sequences
+        return GenerateOutput(sequences, self.lp[:, :L].clone(), self.top_ids[:, :L].to(torch.int64), self.top_lp[:, :L].clone())
 
     def start(self, T: int, mask: Optional[torch.Tensor]):
         """Reset the state for a prompt of T tokens (mask: host [B, T] padding mask or None) already prefilled into

@@ -585,9 +585,12 @@ class SlotDecodeState(DecodeState):
     """DecodeState of continuous batching: one row per engine slot, max_batch rows, and what each slot's request needs on the
     device: its sampling parameters (temperature, 0 = greedy; top_k; top_p; seed; noise row; RNG offset), its token budget
     max_new, the count n_out and the tokens out_tokens [max_batch, max_out] (int32) it has emitted, its finished flag, and the
-    step's input ids_in and sampled next_ids.  A decode step over the first n slots reads rows(n); the other slots are idle."""
+    step's input ids_in and sampled next_ids.  A decode step over the first n slots reads rows(n); the other slots are idle.
+    Log-probabilities (serving.Engine's logprobs): lp_n, the slot's top-n (-1: none), and rings of lp_ring entries that the step
+    writes at n_out mod lp_ring: lp_ring_lp [max_batch, lp_ring] fp32, lp_ring_ids [max_batch, lp_ring, 20] int32 and
+    lp_ring_top [max_batch, lp_ring, 20] fp32."""
 
-    def __init__(self, max_batch, H, max_out, device):
+    def __init__(self, max_batch, H, max_out, device, lp_ring: int = 1):
         super().__init__(max_batch, H, 0, device)
         self.key_mask = None
         i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
@@ -603,10 +606,15 @@ class SlotDecodeState(DecodeState):
         self.ids_in = torch.zeros(max_batch, 1, **i64)
         self.next_ids = torch.zeros(max_batch, **i64)
         self.out_tokens = torch.zeros(max_batch, max_out, **i32)
+        self.lp_n = torch.full((max_batch,), -1, **i32)
+        self.lp_ring_lp = torch.zeros(max_batch, lp_ring, dtype=torch.float32, device=device)
+        self.lp_ring_ids = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, **i32)
+        self.lp_ring_top = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, dtype=torch.float32, device=device)
 
     # the per-slot arrays, in the order a slot's row is copied when slots are compacted
     SLOT_FIELDS = ("rope_pos", "write_pos", "kv_len", "temperature", "top_k", "top_p", "seed", "noise_row", "rng_offset",
-                   "max_new", "n_out", "finished", "ids_in", "next_ids", "out_tokens")
+                   "max_new", "n_out", "finished", "ids_in", "next_ids", "out_tokens", "lp_n", "lp_ring_lp", "lp_ring_ids",
+                   "lp_ring_top")
 
     def rows(self, n):
         """A DecodeState view of the first n slots (what decode_step and the sampler of a step over n slots read)."""
@@ -1023,11 +1031,24 @@ class AriaMoELMForCausalLM(nn.Module):
         h, _ = self.model.norm(x, residual=pending)
         return self.lm_head(h), cache
 
-    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None, page_table_host=None):
+    def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None, page_table_host=None,
+                      hidden_rows=None):
         """AriaMoELMModel.prefill_paged, then the final norm and lm_head on the last row of each segment listed in `ends`
         (segment indices in increasing order, the segments that end a prompt; None = every segment) -> logits [1, len(ends), V],
-        row i those of forward(num_logits_to_keep=1) on the whole prompt of segment ends[i]."""
+        row i those of forward(num_logits_to_keep=1) on the whole prompt of segment ends[i].
+        hidden_rows (host ints, packed row indices): also the final-norm hidden states of those rows -> (logits, h [n, d]), row
+        i what forward() feeds lm_head at that position (prompt logprobs: serving.Engine)."""
         x, pending = self.model.prefill_paged(inputs_embeds, cache, page_table, seg, position_ids, page_table_host)
+        if hidden_rows is None:
+            return self._end_logits(x, pending, seg, ends)
+        if len(hidden_rows):
+            idx = torch.tensor(hidden_rows, dtype=torch.int64).to(x.device, non_blocking=True)
+            h, _ = self.model.norm(x.index_select(1, idx)[0], residual=pending.index_select(1, idx)[0])
+        else:
+            h = x.new_empty((0, x.shape[-1]))
+        return self._end_logits(x, pending, seg, ends), h
+
+    def _end_logits(self, x, pending, seg, ends):
         ends = range(seg.n_seg) if ends is None else ends
         rows = [seg.cu[b + 1] - 1 for b in ends]
         if not rows:                                         # only chunks that end no prompt: no logits

@@ -1664,6 +1664,62 @@ def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: 
     return out
 
 
+MAX_LOGPROBS = 20
+
+
+def token_logprobs(logits: torch.Tensor, tokens: torch.Tensor, n_max: int, *, n_row: Optional[torch.Tensor] = None,
+                   col: Optional[torch.Tensor] = None, ring: int = 0, finished: Optional[torch.Tensor] = None,
+                   finished_fill: bool = True, out: Optional[tuple] = None) -> tuple:
+    """Log-probabilities of `tokens` (CUDA int64 [R]) under the raw distribution of each row of bf16 logits [R, V] (contiguous
+    last dim, any row stride): lp = (x_t - max) - log(sum exp(x - max)) in fp32, and the n_max (0..20) largest logits of the row
+    by (value desc, id asc) with their logprobs.  -> (logprobs, top_ids int32, top_logprobs), allocated as [R], [R, n_max],
+    [R, n_max] when out is None; else out = (logprobs [R] or [R, cols] fp32, top_ids [R(, cols), n_max] int32, top_logprobs
+    likewise fp32) and row r writes column c of its output row:
+      col: None -> c = 0; a CUDA int32 [1] (every row) or [R] (one per row) -> c = col, or col mod ring when ring > 0; rows
+      whose column falls outside [0, cols) write nothing.
+      n_row: CUDA int32 [R], the row's n (-1: the row writes nothing); entries past it, or past V, hold id -1 / logprob -inf.
+      finished: CUDA uint8 [R]; a finished row writes the filler (0, -1, -inf) if finished_fill, else nothing.
+    A row's result depends only on its own logits, token and n (not on R, its index, the stride or where it is written).
+    See aria_token_logprobs."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(-1) == 1):
+        raise RuntimeError("token_logprobs: logits must be CUDA bf16 [R, V] with a contiguous last dim")
+    if not isinstance(n_max, int) or isinstance(n_max, bool) or not 0 <= n_max <= MAX_LOGPROBS:
+        raise ValueError(f"token_logprobs: n_max must be an int in [0, {MAX_LOGPROBS}], got {n_max!r}")
+    R, V = logits.shape
+    _chk(tokens, torch.int64, align=8)
+    if tokens.shape != (R,):
+        raise ValueError(f"token_logprobs: tokens must be [{R}], got {tuple(tokens.shape)}")
+    if out is None:
+        out = (torch.empty((R,), dtype=torch.float32, device=logits.device),
+               torch.empty((R, n_max), dtype=torch.int32, device=logits.device),
+               torch.empty((R, n_max), dtype=torch.float32, device=logits.device))
+    lp, ids, tlp = out
+    _chk(lp, torch.float32, align=4), _chk(ids, torch.int32, align=4), _chk(tlp, torch.float32, align=4)
+    cols = 1 if lp.dim() == 1 else lp.shape[1]
+    if lp.shape[0] != R or lp.dim() not in (1, 2) or ids.shape != lp.shape + (n_max,) or tlp.shape != ids.shape:
+        raise ValueError(f"token_logprobs: out must be [{R}(, cols)], [{R}(, cols), {n_max}] x 2, got "
+                         f"{[tuple(t.shape) for t in out]}")
+    if col is not None:
+        _chk(col, torch.int32, align=4)
+        if col.numel() not in (1, R):
+            raise ValueError(f"token_logprobs: col must have 1 or {R} entries, got {col.numel()}")
+    elif ring:
+        raise ValueError("token_logprobs: ring needs col")
+    if not isinstance(ring, int) or not 0 <= ring <= cols:
+        raise ValueError(f"token_logprobs: ring must be an int in [0, {cols}], got {ring!r}")
+    for t, dt, name in ((n_row, torch.int32, "n_row"), (finished, torch.uint8, "finished")):
+        if t is not None:
+            _chk(t, dt, align=1)
+            if t.shape != (R,):
+                raise ValueError(f"token_logprobs: {name} must be [{R}], got {tuple(t.shape)}")
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_token_logprobs(_p(logits), logits.stride(0), _p(tokens), R, V, n_max, _p(n_row), _p(col),
+                                             int(col is not None and col.numel() == R and R > 1), int(ring), _p(finished),
+                                             int(bool(finished_fill)), _p(lp), _p(ids), _p(tlp), cols, _stream(logits)),
+                "token_logprobs")
+    return lp, ids, tlp
+
+
 def decode_advance_slots(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: torch.Tensor, n_out: torch.Tensor,
                          max_new: torch.Tensor, rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor,
                          rng_offset: torch.Tensor, finished: torch.Tensor, eos_token_ids: Sequence[int] = (),

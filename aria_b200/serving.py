@@ -67,6 +67,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import ops
+from .ops import MAX_LOGPROBS
 
 PAGE = 256
 MAX_BATCH = 1024   # the slot advance runs one thread per slot in one CTA
@@ -225,6 +226,35 @@ class PageAllocator:
 
 
 @dataclass
+class Logprobs:
+    """A finished request's log-probabilities (Engine.logprobs[rid]), host tensors under the model's raw distribution
+    (ops.token_logprobs), None where not asked: token_logprobs [n_gen] fp32, top_ids [n_gen, k] int64 and top_logprobs [n_gen, k]
+    fp32 for its generated tokens (k = logprobs); prompt_logprobs [T - 1], prompt_top_ids and prompt_top_logprobs [T - 1, k] for
+    prompt positions 1 .. T - 1 (k = prompt_logprobs)."""
+    token_logprobs: Optional[torch.Tensor] = None
+    top_ids: Optional[torch.Tensor] = None
+    top_logprobs: Optional[torch.Tensor] = None
+    prompt_logprobs: Optional[torch.Tensor] = None
+    prompt_top_ids: Optional[torch.Tensor] = None
+    prompt_top_logprobs: Optional[torch.Tensor] = None
+
+
+def ring_entries(drained: int, n_out: int, ring: int) -> List[int]:
+    """Ring indices of a slot's generated tokens [drained, n_out), token i at i mod ring.  Between two polls a slot emits at
+    most ring = poll_every + 1 tokens (its first token from the admission prefill, then one per replay of the poll_every
+    replays), so the ring never overwrites an entry the host has not copied; a count past that is an engine bug and raises."""
+    n = n_out - drained
+    if not 0 <= n <= ring:
+        raise RuntimeError(f"logprob ring: {n} tokens since the last poll, the ring holds {ring}")
+    return [(drained + i) % ring for i in range(n)]
+
+
+def _check_logprobs_arg(name: str, k) -> None:
+    if k is not None and (not isinstance(k, int) or isinstance(k, bool) or not 0 <= k <= MAX_LOGPROBS):
+        raise ValueError(f"{name} must be None or an int in [0, {MAX_LOGPROBS}], got {k!r}")
+
+
+@dataclass
 class Request:
     rid: int
     input_ids: torch.Tensor            # host int64 [T]
@@ -239,6 +269,11 @@ class Request:
     feats: Optional[torch.Tensor] = None                # image features of pixel rows [feat_row, vit_rows) not merged yet
     feat_row: int = 0
     vit_rows: int = 0                                   # pixel rows the ViT has run on (rows inside the hit count as run)
+    logprobs: Optional[int] = None                      # top-n of the generated tokens' logprobs (None: none)
+    prompt_logprobs: Optional[int] = None               # top-n of the prompt tokens' logprobs (None: none; no prefix-cache hit)
+    lp_drained: int = 0                                 # generated tokens whose logprobs the host has copied out of the ring
+    lp_parts: list = field(default_factory=list)        # host (logprob [m], ids [m, k], logprobs [m, k]) pieces, in order
+    plp_parts: list = field(default_factory=list)       # device pieces of the prompt logprobs, in order
 
     @property
     def n_pages(self) -> int:
@@ -295,7 +330,11 @@ class Scheduler:
         return len(self.slots) - 1, req
 
     def _head_hits(self) -> List[int]:
+        """The cached pages the queue's head would hold; none for a request that wants its prompt logprobs, whose every prompt
+        row must be computed (its pages are still keyed for others)."""
         req = self.queue[0]
+        if req.prompt_logprobs is not None:
+            return []
         return self.pages.lookup(req.keys[:(req.input_ids.numel() - 1) // PAGE])
 
     def register(self, req: Request) -> None:
@@ -378,7 +417,12 @@ class Engine:
     max_prefill_tokens: the most prompt tokens one step() prefills (a multiple of 256; None = no limit; cached prefix tokens do
     not count), so that a long admission delays the running requests' decode steps by a bounded prefill.
     `times[rid]`: host clock (time.perf_counter) when its first token and its last token were known done (first poll after
-    its prompt was prefilled, poll that saw it finish)."""
+    its prompt was prefilled, poll that saw it finish).
+    Log-probabilities: `logprobs[rid]`, a Logprobs for each finished request that asked for logprobs or prompt_logprobs.  The
+    decode step writes each asking slot's entries into per-slot rings of poll_every + 1 entries (SlotDecodeState.lp_ring_*),
+    copied to the host at each poll, so the device memory does not grow with the pool (4 x 41 x max_batch x (poll_every + 1)
+    bytes).  A step with no asking slot replays a graph without the logprob kernel.  Prompt logprobs are computed from the
+    prefill's final hidden states in chunks of at most 1024 rows (a logits scratch of 2 x 1024 x V bytes)."""
 
     max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS
 
@@ -414,13 +458,16 @@ class Engine:
         self.kv_cache_dtype = kv_cache_dtype
         self.cache = PagedKVCache(c.num_hidden_layers, n_pages, c.num_attention_heads, c.head_dim, max_batch, self.max_pages, dev,
                                   kv_cache_dtype)
-        self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev)
+        self.lp_ring = poll_every + 1
+        self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev, self.lp_ring)
         self._idle(0, max_batch)
         self.rope = lm.model.rope_tables(self.max_pages * PAGE, dev)   # held here: the graphs read these tables
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._pool = torch.cuda.graph_pool_handle()
         self._fin_host = torch.ones(max_batch, dtype=torch.uint8).pin_memory()
         self._nout_host = torch.zeros(max_batch, dtype=torch.int32).pin_memory()
+        st = self.state
+        self._lp_host = [torch.empty_like(t, device="cpu").pin_memory() for t in (st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top)]
         self._event = torch.cuda.Event()
         self._next_rid = 0
         self._undelivered: Dict[int, torch.Tensor] = {}
@@ -429,13 +476,18 @@ class Engine:
                       "prompt_tokens": 0, "prefix_hit_tokens": 0, "vit_rows_run": 0, "vit_rows_skipped": 0, "pages_evicted": 0,
                       "prefill_launches": 0, "prefill_chunks": 0}
         self.times: Dict[int, list] = {}
+        self.logprobs: Dict[int, Logprobs] = {}
 
     # ------------------------------------------------------------------------------------------------ public API
     def add_request(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, do_sample: bool = False,
-                    temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0) -> int:
+                    temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, logprobs: Optional[int] = None,
+                    prompt_logprobs: Optional[int] = None) -> int:
         """Queue one request (input_ids [T] or [1, T]; pixel inputs as generate()'s for that one row) -> its id.  Arguments are
         checked as generate() checks them, and a request that needs more pages than the pool has is refused, here, before
-        any device work.  The prompt's page keys (page_keys) are computed here, on the host."""
+        any device work.  The prompt's page keys (page_keys) are computed here, on the host.
+        logprobs / prompt_logprobs (None, or an int k in [0, 20]): the logprob of each generated / prompt token under the model's
+        raw distribution and its k most likely tokens, in self.logprobs[rid] once it finishes (Logprobs); the generated ones are
+        generate(output_logprobs=k)'s bit for bit.  A request with prompt_logprobs takes no prefix-cache hit."""
         if not isinstance(input_ids, torch.Tensor) or input_ids.dim() not in (1, 2):
             raise ValueError("input_ids must be a tensor [T] or [1, T]")
         ids = input_ids.reshape(1, -1) if input_ids.dim() == 1 else input_ids
@@ -443,8 +495,11 @@ class Engine:
             raise ValueError(f"add_request takes one prompt, got input_ids {tuple(input_ids.shape)}")
         self.model._check_generate_args(ids, max_new_tokens, None, do_sample, temperature, top_k, top_p, list(self.eos),
                                         self.pad, seed, self.poll_every)
+        _check_logprobs_arg("logprobs", logprobs)
+        _check_logprobs_arg("prompt_logprobs", prompt_logprobs)
         sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
-        req = Request(self._next_rid, ids[0].to("cpu", torch.int64), max_new_tokens, sampling, pixel_values, pixel_mask)
+        req = Request(self._next_rid, ids[0].to("cpu", torch.int64), max_new_tokens, sampling, pixel_values, pixel_mask,
+                      logprobs=logprobs, prompt_logprobs=prompt_logprobs)
         image_token = None if pixel_values is None else self.model.config.image_token_index
         req.keys = page_keys(req.input_ids, pixel_values, pixel_mask, image_token)
         self.sched.submit(req)
@@ -472,8 +527,8 @@ class Engine:
         done, self._undelivered = self._undelivered, {}
         decoding = self.sched.n_active - (self.sched.partial is not None)    # a partly prefilled request's slot is idle
         if decoding:
-            g = self._graph(_pow2_at_least(self.sched.n_active, self.max_batch),
-                            _pow2_at_least(self.sched.width(), self.max_pages))
+            n, width = _pow2_at_least(self.sched.n_active, self.max_batch), _pow2_at_least(self.sched.width(), self.max_pages)
+            g = self._graph(n, width, True) if self._any_logprobs() else self._graph(n, width)
             for _ in range(self.poll_every):
                 g.replay()
             self.stats["steps"] += self.poll_every
@@ -527,28 +582,38 @@ class Engine:
         st.write_pos[lo:hi] = -1
         st.rope_pos[lo:hi] = 0
         st.n_out[lo:hi] = 0
+        st.lp_n[lo:hi] = -1
         st.temperature[lo:hi] = 0.0
         self.cache.block_table[lo:hi] = -1
         self.cache.block_table[lo:hi, 0] = 0
 
-    def _step(self, n: int) -> None:
+    def _any_logprobs(self) -> bool:
+        return any(r.logprobs is not None for r in self.sched.slots)
+
+    def _step(self, n: int, lp: bool) -> None:
         lm = self.model.language_model
         st = self.state.rows(n)
         emb = ops.embedding(st.ids_in, lm.get_input_embeddings().weight)
         logits = lm.decode_step(emb, self.cache, st, self.rope)
-        self._sample_and_advance(st, logits[:, -1])
+        self._sample_and_advance(st, logits[:, -1], lp)
         self._fin_host.copy_(self.state.finished, non_blocking=True)
         self._nout_host.copy_(self.state.n_out, non_blocking=True)
 
-    def _sample_and_advance(self, st, logits) -> None:
+    def _sample_and_advance(self, st, logits, lp: bool) -> None:
+        """Sample, then with lp the logprobs of the slots with lp_n >= 0 into ring entry n_out mod lp_ring (finished slots
+        untouched), then advance."""
         ops.sample_tokens_slots(logits, st.temperature, st.top_k, st.top_p, st.seed, st.noise_row, st.rng_offset, out=st.next_ids)
+        if lp:
+            ops.token_logprobs(logits, st.next_ids, MAX_LOGPROBS, n_row=st.lp_n, col=st.n_out, ring=self.lp_ring,
+                               finished=st.finished, finished_fill=False, out=(st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top))
         ops.decode_advance_slots(st.next_ids, st.ids_in, st.out_tokens, st.n_out, st.max_new, st.rope_pos, st.write_pos,
                                  st.kv_len, st.rng_offset, st.finished, self.eos, self.pad)
 
-    def _graph(self, n: int, width: int) -> torch.cuda.CUDAGraph:
-        """The captured step over slots [0, n) and table columns [0, width), captured on first use.  The warm-up run before the
-        capture computes the very step the next replay computes; the slot rows it advanced are put back afterwards."""
-        key = (n, width)
+    def _graph(self, n: int, width: int, lp: bool = False) -> torch.cuda.CUDAGraph:
+        """The captured step over slots [0, n) and table columns [0, width), with the logprob kernel when lp, captured on first
+        use; its key is (n, width), and (n, width, True) with the logprob kernel.  The warm-up run before the capture computes
+        the very step the next replay computes; the slot rows it advanced are put back afterwards."""
+        key = (n, width, True) if lp else (n, width)
         g = self._graphs.get(key)
         if g is not None:
             return g
@@ -558,13 +623,13 @@ class Engine:
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):
-            self._step(n)
+            self._step(n, lp)
         cur.wait_stream(side)
         for f, t in keep.items():
             getattr(self.state, f).copy_(t)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, pool=self._pool):
-            self._step(n)
+            self._step(n, lp)
         self._graphs[key] = g
         self.stats["graphs_captured"] += 1
         return g
@@ -639,12 +704,49 @@ class Engine:
         for b, req in enumerate(staged):
             if req.pixel_values is not None:
                 self._merge_images(req, ids_dev[cu[b]:cu[b + 1]], emb[0, cu[b]:cu[b + 1]])
-        logits = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends, page_table_host=table)
+        # prompt logprobs: rows [start, min(end, T - 1)) of each asking chunk give positions start + 1 .. min(end, T - 1); the
+        # last prompt row's logits are the first generated token's
+        want = [(b, r, min(r.chunk[1], r.input_ids.numel() - 1) - r.chunk[0]) for b, r in enumerate(staged)
+                if r.prompt_logprobs is not None]
+        if want:
+            rows = [i for b, _, n in want for i in range(cu[b], cu[b] + n)]
+            logits, h = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends, page_table_host=table, hidden_rows=rows)
+            self._prompt_logprobs(want, h)
+        else:
+            logits = lm.prefill_paged(emb, self.cache, table_dev, seg, pos_dev, ends, page_table_host=table)
         self.stats["prefill_launches"] += 1
         self.stats["prefill_chunks"] += len(staged) - len(ends)
         for i, b in enumerate(ends):
             req = staged[b]
             self._start_decode(self.sched.slots.index(req), req, logits[0, i:i + 1])
+
+    PROMPT_LP_ROWS = 1024   # lm_head rows per prompt-logprob chunk: a logits scratch of 2 x 1024 x V bytes (205 MB at V = 100,352)
+
+    def _prompt_logprobs(self, want, h) -> None:
+        """Prompt logprobs of the staged chunks in `want` [(packed segment, request, rows)] from their final hidden states h
+        [sum rows, d]: lm_head and ops.token_logprobs over at most PROMPT_LP_ROWS rows at a time, targets the next prompt ids.
+        The results stay on the device with their request until it retires."""
+        N = h.shape[0]
+        if N == 0:
+            return
+        lm = self.model.language_model
+        tgt = torch.cat([r.input_ids[r.chunk[0] + 1:r.chunk[0] + 1 + n] for _, r, n in want])
+        nrow = torch.cat([torch.full((n,), r.prompt_logprobs, dtype=torch.int64) for _, r, n in want])
+        host = torch.cat([tgt, nrow]).pin_memory()
+        dev = host.to(self.dev, non_blocking=True)
+        tgt_dev, nrow_dev = dev[:N], dev[N:].to(torch.int32)
+        k = max(r.prompt_logprobs for _, r, _ in want)
+        lp = torch.empty(N, dtype=torch.float32, device=self.dev)
+        ids = torch.empty(N, k, dtype=torch.int32, device=self.dev)
+        top = torch.empty(N, k, dtype=torch.float32, device=self.dev)
+        for i in range(0, N, self.PROMPT_LP_ROWS):
+            j = min(N, i + self.PROMPT_LP_ROWS)
+            ops.token_logprobs(lm.lm_head(h[i:j]), tgt_dev[i:j], k, n_row=nrow_dev[i:j], out=(lp[i:j], ids[i:j], top[i:j]))
+        o = 0
+        for _, r, n in want:       # each request's own copy, so the launch's buffers go when this call returns
+            k = r.prompt_logprobs
+            r.plp_parts.append((lp[o:o + n].clone(), ids[o:o + n, :k].clone(), top[o:o + n, :k].clone()))
+            o += n
 
     def _merge_images(self, req: Request, ids_dev, emb) -> None:
         """Image features of the chunk req.chunk into its embedding rows: the ViT and the projector run on the pixel rows whose
@@ -694,7 +796,8 @@ class Engine:
         st.max_new[s] = req.max_new_tokens
         st.n_out[s] = 0
         st.finished[s] = 0
-        self._sample_and_advance(_slot_rows(st, s), logits)
+        st.lp_n[s] = -1 if req.logprobs is None else req.logprobs
+        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None)
 
     def _drop(self, s: int) -> None:
         """Retire slot s without a result: the last active slot moves into s and the slot it left becomes idle."""
@@ -711,6 +814,12 @@ class Engine:
 
     def _poll_and_retire(self) -> Dict[int, torch.Tensor]:
         t0 = time.perf_counter()
+        n_act = self.sched.n_active
+        lp = self._any_logprobs()
+        if lp:      # the rings of the active slots, queued before the event the host waits on
+            st = self.state
+            for h, t in zip(self._lp_host, (st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top)):
+                h[:n_act].copy_(t[:n_act], non_blocking=True)
         self._event.record(torch.cuda.current_stream(self.dev))
         self._event.synchronize()
         now = time.perf_counter()
@@ -722,6 +831,10 @@ class Engine:
             if req is not self.sched.partial and req.rid not in self._first_seen:
                 self._first_seen.add(req.rid)
                 self.times[req.rid] = [now, None]
+        if lp:
+            for s, req in enumerate(self.sched.slots):
+                if req.logprobs is not None and req is not self.sched.partial:
+                    self._drain(req, s, n_out[s])
         done = {}
         for s in range(self.sched.n_active - 1, -1, -1):   # descending: the slot moved into s is always a live one
             req = self.sched.slots[s]
@@ -729,6 +842,8 @@ class Engine:
                 continue
             done[req.rid] = torch.cat([req.input_ids.to(self.dev), self.state.out_tokens[s, :n_out[s]].to(torch.int64)])
             self.times[req.rid][1] = now
+            if req.logprobs is not None or req.prompt_logprobs is not None:
+                self.logprobs[req.rid] = self._logprobs_result(req)
             self._first_seen.discard(req.rid)
             move = self.sched.retire(s)
             if move is not None:
@@ -738,6 +853,32 @@ class Engine:
                 n_out[dst] = n_out[src]
             self._idle(self.sched.n_active, self.sched.n_active + 1)
         return done
+
+    def _drain(self, req: Request, s: int, n_out: int) -> None:
+        """Copy slot s's ring entries [req.lp_drained, n_out) out of the pinned copy of the rings into req.lp_parts."""
+        idx = torch.tensor(ring_entries(req.lp_drained, n_out, self.lp_ring), dtype=torch.int64)
+        if idx.numel():
+            lp, ids, top = self._lp_host
+            k = req.logprobs
+            req.lp_parts.append((lp[s, idx].clone(), ids[s, idx, :k].to(torch.int64), top[s, idx, :k].clone()))
+        req.lp_drained = n_out
+
+    @staticmethod
+    def _logprobs_result(req: Request) -> Logprobs:
+        out = Logprobs()
+        if req.logprobs is not None:
+            k = req.logprobs
+            parts = req.lp_parts or [(torch.empty(0), torch.empty(0, k, dtype=torch.int64), torch.empty(0, k))]
+            out.token_logprobs, out.top_ids, out.top_logprobs = (torch.cat(t) for t in zip(*parts))
+        if req.prompt_logprobs is not None:
+            k = req.prompt_logprobs
+            if req.plp_parts:
+                lp, ids, top = (torch.cat(t).cpu() for t in zip(*req.plp_parts))
+                out.prompt_logprobs, out.prompt_top_ids, out.prompt_top_logprobs = lp, ids.to(torch.int64), top
+            else:   # a one-token prompt
+                out.prompt_logprobs, out.prompt_top_ids, out.prompt_top_logprobs = (
+                    torch.empty(0), torch.empty(0, k, dtype=torch.int64), torch.empty(0, k))
+        return out
 
 
 def _slot_rows(st, s: int):

@@ -635,6 +635,19 @@ int aria_kv_pages_load_fp8(const void* k_pool, const void* v_pool, const float* 
 int aria_sample_tokens_slots(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V,
                              const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seed,
                              const int32_t* noise_rows, const uint64_t* offsets, aria_stream_t stream);
+/* Token log-probabilities of bf16 logits [R, V] (row r at logits + r * logits_stride, contiguous within a row), one CTA per row,
+ * under the row's raw distribution: lp(t) = (x_t - m) - log(sum_i exp(x_i - m)), m = max_i x_i, in fp32 summed in a fixed order.
+ * Row r writes output entry o = r * cols + c: logprobs[o] = lp(tokens[r]) (NaN for a token outside [0, V)), and its n largest
+ * logits by (value desc, id asc) to top_ids[o * n_max + j] / top_logprobs[o * n_max + j], j < n; entries n .. n_max - 1 (also
+ * those past V) get id -1 and logprob -inf.  n = n_row[r] (DEVICE int32 [R], -1 skips the row; clamped to n_max) or n_max when
+ * n_row is NULL; 0 <= n_max <= 20.  Column c: col NULL -> 0; else col[r] (col_per_row) or col[0], taken mod ring when ring > 0;
+ * a column outside [0, cols) skips the row.  finished (DEVICE uint8 [R] or NULL): a finished row gets the filler (logprob 0,
+ * ids -1, logprobs -inf) when finished_fill, else is left untouched.  A row's result depends only on its logits, token and n.
+ * R <= 2^20, V <= 2^24. */
+int aria_token_logprobs(const void* logits, int64_t logits_stride, const int64_t* tokens, int32_t R, int32_t V, int32_t n_max,
+                        const int32_t* n_row, const int32_t* col, int32_t col_per_row, int32_t ring, const uint8_t* finished,
+                        int32_t finished_fill, float* logprobs, int32_t* top_ids, float* top_logprobs, int32_t cols,
+                        aria_stream_t stream);
 /* aria_decode_advance per slot (continuous batching).  For each slot r < R that is not finished: its token next_ids[r] is stored
  * at out_tokens[r, n_out[r]] ([R, out_stride] int32) and n_out[r] + 1; the slot finishes when the token is one of the n_eos <= 8
  * EOS ids (HOST array, copied into the launch) or n_out reaches max_new[r]; ids_in[r] <- the token (pad_token_id once
