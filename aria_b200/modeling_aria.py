@@ -718,7 +718,7 @@ class GraphedDecode:
             self._step()
         cur.wait_stream(side)
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with ops.graph_capture(self.graph):
             self.logits = self._step()
 
     def _step(self):
@@ -870,10 +870,10 @@ class GraphedLookupDecode:
             self._step_1()
         cur.wait_stream(side)
         self.graph_k = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph_k):
+        with ops.graph_capture(self.graph_k):
             self._step_k()
         self.graph_1 = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph_1):
+        with ops.graph_capture(self.graph_1):
             self._step_1()
 
     def _sample(self, logits, noise, offsets, out):
@@ -986,7 +986,7 @@ class GraphedPrefill:
                 model(self.ids_dev, self.pv_dev, None, **kw)
         torch.cuda.current_stream(dev).wait_stream(side)
         self.graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(self.graph):
+        with ops.graph_capture(self.graph):
             self.logits = model(self.ids_dev, self.pv_dev, None, **kw).logits
 
     def replay(self) -> torch.Tensor:

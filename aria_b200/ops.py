@@ -5,7 +5,9 @@ All wrappers launch on the current stream of the input's device and never synchr
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
+import gc
 from typing import Optional, Sequence
 
 import torch
@@ -21,6 +23,22 @@ def _p(t: Optional[torch.Tensor]):
 
 def _stream(t: torch.Tensor):
     return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
+
+
+@contextlib.contextmanager
+def graph_capture(graph: torch.cuda.CUDAGraph, pool=None):
+    """torch.cuda.graph(graph, pool) with Python's garbage collector paused.  A collection during the capture can run the
+    destructor of a dead object that holds CUDA resources (another CUDA graph, its memory pool), whose release is not
+    allowed while a stream captures, and the process aborts; torch.cuda.graph no longer collects before it captures.
+    The garbage is collected after the capture instead."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(graph, pool=pool):
+            yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 def _chk(t: torch.Tensor, dtype=bf16, align: int = 16):

@@ -628,7 +628,7 @@ class Engine:
         for f, t in keep.items():
             getattr(self.state, f).copy_(t)
         g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, pool=self._pool):
+        with ops.graph_capture(g, pool=self._pool):
             self._step(n, lp)
         self._graphs[key] = g
         self.stats["graphs_captured"] += 1

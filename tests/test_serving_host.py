@@ -196,3 +196,37 @@ def test_failed_admission_frees_its_slot_and_pages_and_keeps_the_queue(monkeypat
     assert [r.rid for r in eng.sched.queue] == [2, 3]         # the requests behind it are still queued, in order
     eng.sched.retire(0)                                      # (request 0 done) so that this host-only step has nothing to replay
     assert eng.step() == {} and admitted[1:] == [(0, 2), (1, 3)] and eng.sched.pages.n_free == 6
+
+
+def test_graph_capture_pauses_garbage_collection(monkeypatch):
+    """Graph captures (the engine's step graphs, generate()'s decode graphs) run with the garbage collector paused, so a
+    collection cannot release a dead object's CUDA graph or memory pool mid-capture; it is re-enabled afterwards, also when
+    the capture raises, and stays off if it was off."""
+    import contextlib
+    import gc
+
+    from aria_b200 import ops
+    seen = []
+
+    @contextlib.contextmanager
+    def fake_graph(graph, pool=None):
+        seen.append((graph, pool, gc.isenabled()))
+        yield
+
+    monkeypatch.setattr(torch.cuda, "graph", fake_graph)
+    was = gc.isenabled()
+    try:
+        gc.enable()
+        with ops.graph_capture("g", pool="p"):
+            assert not gc.isenabled()
+        assert seen == [("g", "p", False)] and gc.isenabled()
+        with pytest.raises(RuntimeError):
+            with ops.graph_capture("g"):
+                raise RuntimeError("capture failed")
+        assert gc.isenabled()
+        gc.disable()
+        with ops.graph_capture("g"):
+            pass
+        assert not gc.isenabled()
+    finally:
+        (gc.enable if was else gc.disable)()
