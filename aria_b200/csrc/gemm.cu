@@ -7,6 +7,10 @@ namespace aria {
 
 // four k-blocks in flight: the ring takes what the fp32 staging tile of the epilogue leaves of the 227 KB per block
 constexpr int GEMM_STAGES = 4;
+// gemm_kernel with the hand-off epilogue (HANDOFF): no staging tile, so up to six 32 KB stages fit beside the 32 KB bf16
+// output tile.  Six measured faster for the dense launches (nn.Linear weights: the LM's q/k/v, the shared gate/up), four for
+// the grouped expert launches ([E, K, N] weights), whose 196,608-row launches ran 2-3 % slower with six (DESIGN §6).
+constexpr int handoff_stages(bool b_mn) { return b_mn ? 4 : 6; }
 // fp8 B (B_FP8): TMA lands the e4m3 boxes in a ring of their own, the producer warpgroup's three idle warps widen them to bf16
 // in the SW128 layout of the bf16 ring, and the wgmma sequence is unchanged.  Three landing slots fit beside the four bf16
 // stages and the fp32 staging tile (DESIGN §3); a fourth would not.
@@ -16,12 +20,17 @@ constexpr int FP8_CONVERT_WARPS = 3;
 constexpr int PAIR_MIN_ROWS = 2048;
 // Shortest reduction of a wide LINEAR GEMM that runs as CTA pairs (gemm_run)
 constexpr int WIDE_PAIR_MIN_K = 2048;
-template <int BN, bool B_FP8 = false>
+// HANDOFF_RING: the ring's stages of a hand-off launch (handoff_stages), 0 for the staged epilogue (a CTA pair takes what
+// one CTA takes)
+template <int BN, bool B_FP8 = false, bool PAIR = false, int HANDOFF_RING = 0>
 constexpr int gemm_smem_bytes() {
-  return 1024 /*align*/ + GEMM_STAGES * (A_STAGE_BYTES + BN * BK * 2) + BM * acc_ld(BN) * 4 + 256 /*barriers*/ +
+  return 1024 /*align*/ + (HANDOFF_RING ? HANDOFF_RING : GEMM_STAGES) * (A_STAGE_BYTES + BN * BK * 2) +
+         (HANDOFF_RING ? 2 * 2 * OUT_BOX_BYTES : BM * acc_ld(BN) * 4) + 256 /*barriers*/ +
          (B_FP8 ? FP8_LAND_STAGES * BN * BK : 0);
 }
 static_assert(gemm_smem_bytes<128, true>() <= 232448, "fp8 landing ring must fit the opt-in shared memory of a block");
+static_assert(gemm_smem_bytes<128, false, false, handoff_stages(false)>() <= 232448,
+              "hand-off ring must fit the opt-in shared memory of a block");
 
 // 16 e4m3 values (one 16-byte landing chunk, columns in address order) -> 16 bf16 in two 16-byte chunks; every e4m3 value,
 // subnormals and -0 included, is exact in fp16, fp32 and bf16
@@ -41,11 +50,115 @@ ARIA_DEVICE void e4m3x16_to_bf16(const uint4 v, uint4& lo, uint4& hi) {
   hi = make_uint4(o[4], o[5], o[6], o[7]);
 }
 
-// The persistent loop of a CTA: tiles blockIdx.x, + gridDim.x, ...  PAIR: both CTAs of a cluster walk the same pair indices,
-// so their trip counts are identical, and the scheduler's n-tiles are n-pairs
-template <bool PAIR> ARIA_DEVICE int first_tile() { return PAIR ? blockIdx.x >> 1 : blockIdx.x; }
-template <bool PAIR> ARIA_DEVICE int tile_step() { return PAIR ? gridDim.x >> 1 : gridDim.x; }
-template <bool PAIR> ARIA_DEVICE int pair_sched_n(int n_tiles) { return PAIR ? (n_tiles + 1) / 2 : n_tiles; }
+// The epilogue warps' part of gemm_kernel's hand-off (HANDOFF): half h of a 128-wide tile, which holds what epilogue_tile
+// rounds first — bf16(x + bias) (LINEAR; HEADS without RoPE), bf16(gate) | bf16(up) in the two 64-column boxes (SWIGLU),
+// bf16(x) (HEADS, a RoPE segment) — is finished with epilogue_tile's arithmetic and stored, consecutive threads on
+// consecutive 16-byte chunks of a row so that each warp store covers whole row segments.  The row checks are
+// epilogue_tile's: no row at or past the group's end (it belongs to the next group), per-group destinations, head-major
+// rows in their own batch.  Ends with the one arrival on out_free.
+template <int EPI>
+ARIA_DEVICE void handoff_finish_half(const GemmParams& p, uint32_t half, uint64_t* out_free, int et, int h, int grp,
+                                     int m_idx, int n_idx, int row0, int rows, int n_out_total) {
+  const int r_base = m_idx * BM + 64 * h;  // row of the group at row 0 of the half
+  if constexpr (EPI == ARIA_EPI_SWIGLU) {
+    // out = bf16(bf16(silu(g)) * u) into 64 output columns: 8 chunks per row, 12 rows per step
+    constexpr int CH = 8, ROW_STEP = EPI_THREADS / CH;
+    const int c = (et % CH) * 8, col = n_idx * (BM / 2) + c;
+    if (col + 8 <= p.N) {
+      __nv_bfloat16* out = p.out[0] + col;
+#pragma unroll 1
+      for (int r = et / CH; r < 64 && r_base + r < rows; r += ROW_STEP) {
+        const uint4 gv = ld_shared_v4(half + out_half_offset(r, c)), uv = ld_shared_v4(half + out_half_offset(r, 64 + c));
+        const uint32_t g[4] = {gv.x, gv.y, gv.z, gv.w}, u[4] = {uv.x, uv.y, uv.z, uv.w};
+        uint32_t o[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          float s0 = fast_silu(bf16_lo(g[e])), s1 = fast_silu(bf16_hi(g[e]));
+          bf16r2(s0, s1);
+          o[e] = pack_bf16(s0 * bf16_lo(u[e]), s1 * bf16_hi(u[e]));
+        }
+        st_global_v4(out + static_cast<int64_t>(row0 + r_base + r) * p.ldo, make_uint4(o[0], o[1], o[2], o[3]));
+      }
+    }
+  } else if constexpr (EPI == ARIA_EPI_LINEAR) {
+    // the activation, then the store: 16 chunks per row, 6 rows per step
+    constexpr int CH = 16, ROW_STEP = EPI_THREADS / CH;
+    const int c = (et % CH) * 8, col = n_idx * BM + c;
+    if (col + 8 <= n_out_total) {
+#pragma unroll 1
+      for (int r = et / CH; r < 64 && r_base + r < rows; r += ROW_STEP) {
+        const int r_in_grp = r_base + r;
+        uint4 v = ld_shared_v4(half + out_half_offset(r, c));
+        if (p.act == ARIA_ACT_GELU_TANH) act_bf16x8<ARIA_ACT_GELU_TANH>(v);
+        else if (p.act == ARIA_ACT_GELU_NEW) act_bf16x8<ARIA_ACT_GELU_NEW>(v);
+        // per-group destination: possibly a peer GPU's memory, the stores then travel over NVLink
+        __nv_bfloat16* orow = p.out_group_base ? reinterpret_cast<__nv_bfloat16*>(p.out_group_base[grp]) +
+                                                     static_cast<int64_t>(p.out_group_row0[grp] + r_in_grp) * p.ldo
+                                               : p.out[0] + static_cast<int64_t>(row0 + r_in_grp) * p.ldo;
+        st_global_v4(orow + col, v);
+      }
+    }
+  } else {
+    const int col0 = n_idx * BM, seg = col0 / p.N, cseg0 = col0 - seg * p.N;
+    if ((p.rope_mask >> seg) & 1) {
+      // the tile is one whole head (head_dim 128): rotate-half RoPE with op-by-op bf16 rounding,
+      // out = bf16(bf16(x*cos) + bf16(rotate_half(x)*sin)); a thread takes a chunk of the low 64 columns and its partner 64
+      // further on, 12 rows per step
+      constexpr int CH = 8, ROW_STEP = EPI_THREADS / CH;
+      const int c = (et % CH) * 8;
+      __nv_bfloat16* head = p.out[seg] + (cseg0 / p.head_dim) * p.stride_h + c;
+#pragma unroll 1
+      for (int r = et / CH; r < 64 && r_base + r < rows; r += ROW_STEP) {
+        const int grow = row0 + r_base + r;
+        const int b = grow / p.rows_per_batch, tok = grow - b * p.rows_per_batch;
+        const int pos = p.position_ids ? p.position_ids[grow] : p.pos0 + tok;
+        const __nv_bfloat16* cs = p.rope_cos + static_cast<int64_t>(pos) * p.head_dim + c;
+        const __nv_bfloat16* sn = p.rope_sin + static_cast<int64_t>(pos) * p.head_dim + c;
+        const uint4 xlv = ld_shared_v4(half + out_half_offset(r, c)), xhv = ld_shared_v4(half + out_half_offset(r, 64 + c));
+        const uint32_t xl[4] = {xlv.x, xlv.y, xlv.z, xlv.w}, xh[4] = {xhv.x, xhv.y, xhv.z, xhv.w};
+        __nv_bfloat16* dst = head + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld;
+        // the low columns, x_lo cos_lo - x_hi sin_lo, then the high ones, x_hi cos_hi + x_lo sin_hi: one pair of table
+        // vectors live at a time
+#pragma unroll
+        for (int part = 0; part < 2; ++part) {
+          const uint4 cv = __ldg(reinterpret_cast<const uint4*>(cs + 64 * part));
+          const uint4 sv = __ldg(reinterpret_cast<const uint4*>(sn + 64 * part));
+          const uint32_t cw4[4] = {cv.x, cv.y, cv.z, cv.w}, sw4[4] = {sv.x, sv.y, sv.z, sv.w};
+          const uint32_t* x0 = part ? xh : xl;  // times cos
+          const uint32_t* x1 = part ? xl : xh;  // times sin, negated for the low columns
+          uint32_t o[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            float a0 = bf16_lo(x0[e]) * bf16_lo(cw4[e]), b0 = bf16_hi(x0[e]) * bf16_hi(cw4[e]);
+            float a1 = (part ? bf16_lo(x1[e]) : -bf16_lo(x1[e])) * bf16_lo(sw4[e]);
+            float b1 = (part ? bf16_hi(x1[e]) : -bf16_hi(x1[e])) * bf16_hi(sw4[e]);
+            bf16r2(a0, a1);
+            bf16r2(b0, b1);
+            o[e] = pack_bf16(a0 + a1, b0 + b1);
+          }
+          st_global_v4(dst + 64 * part, make_uint4(o[0], o[1], o[2], o[3]));
+        }
+      }
+    } else {
+      // heads_store_tile's scatter of bf16(x + bias): 16 chunks per row, 6 rows per step
+      constexpr int CH = 16, ROW_STEP = EPI_THREADS / CH;
+      const int c = (et % CH) * 8, cs = cseg0 + c;
+      if (cs + 8 <= p.N) {
+        const int hd = cs / p.head_dim;
+        __nv_bfloat16* col_base = p.out[seg] + hd * p.stride_h + (cs - hd * p.head_dim);
+#pragma unroll 1
+        for (int r = et / CH; r < 64 && r_base + r < rows; r += ROW_STEP) {
+          const int grow = row0 + r_base + r;
+          const int b = grow / p.rows_per_batch, tok = grow - b * p.rows_per_batch;
+          st_global_v4(col_base + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld,
+                       ld_shared_v4(half + out_half_offset(r, c)));
+        }
+      }
+    }
+  }
+  named_bar_sync(EPI_BAR, EPI_THREADS);  // every chunk of the half has been read
+  if (et == 0) mbar_arrive(out_free);
+}
 
 template <int BN, bool B_MN>
 ARIA_DEVICE void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) {
@@ -63,24 +176,33 @@ ARIA_DEVICE void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db) 
 //     and releases every stage like the others, and loads no B, issues no MMA and stores nothing.
 //   * cluster barriers after the barrier init (before any remote access) and before exit (no CTA leaves while its peer can
 //     still write its shared memory or arrive on its barriers).
-template <int BN, bool B_MN, int EPI, bool B_FP8 = false, bool PAIR = false>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA_min,
-            const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
-            const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+// HANDOFF (gemm_handoff_kernel; gemm_run: grouped launches without a residual, SwiGLU, HEADS with RoPE; bf16 B, one CTA):
+// the hand-off protocol of gemm_common.cuh in place of stage_and_epilogue.  The consumers write their fragment into a
+// 64 x 128 bf16 half (what epilogue_tile rounds first, so the stored bits are unchanged) and start the next tile's k-loop;
+// the epilogue warps finish the half (handoff_finish_half).  A warpgroup with no row of the tile in its half sits out, on
+// both sides.  Without the 64 KB fp32 staging tile the ring has up to six stages (handoff_stages).
+template <int BN, bool B_MN, int EPI, bool B_FP8, bool PAIR, bool HANDOFF>
+ARIA_DEVICE void gemm_body(const CUtensorMap* tmA, const CUtensorMap* tmA_min, const CUtensorMap* tmB0,
+                           const CUtensorMap* tmB1, const CUtensorMap* tmB2, const GemmParams& p) {
   constexpr int B_STAGE_BYTES = BN * BK * 2;
   constexpr int STAGE_BYTES = A_STAGE_BYTES + B_STAGE_BYTES;
-  constexpr int STAGES = GEMM_STAGES;
+  constexpr int STAGES = HANDOFF ? handoff_stages(B_MN) : GEMM_STAGES;
   constexpr int ACC_LD = acc_ld(BN);
   constexpr int OUT_BN = (EPI == ARIA_EPI_SWIGLU) ? BN / 2 : BN;  // output columns per tile
+  constexpr int HALF_BYTES = 2 * OUT_BOX_BYTES;                   // HANDOFF: a consumer warpgroup's 64 x 128 bf16 half
   static_assert(BN == 128 || BN == 144, "tile widths with a wgmma wrapper");
   static_assert(!B_FP8 || (B_MN && BN == 128 && EPI != ARIA_EPI_HEADS), "fp8 B: grouped [G, K, N] weights, 128-wide tiles");
   static_assert(!PAIR || (!B_MN && !B_FP8), "CTA pairs: dense K-major bf16 B");
+  static_assert(!HANDOFF || (BN == 128 && !B_FP8 && !PAIR), "hand-off: one-CTA bf16 launches, 128-wide tiles");
   constexpr int LAND_BYTES = BN * BK;  // one k-block of fp8 B: BN/64 boxes of 64 k-rows x 64 bytes, unswizzled
 
   uint8_t* smem = smem_1024();
-  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);  // [BM][ACC_LD] fp32 accumulator staging
-  const BarrierRing<STAGES> bar(stg + BM * ACC_LD);
+  // HANDOFF: the bf16 output tile, [2 warpgroups][2 boxes][64 rows][128 B]; otherwise the fp32 accumulator staging tile,
+  // [BM][ACC_LD]
+  float* stg = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);
+  const uint32_t out_tile = smem_u32(stg);
+  const BarrierRing<STAGES> bar(smem + STAGES * STAGE_BYTES + (HANDOFF ? 2 * HALF_BYTES : BM * ACC_LD * 4));
+  const HandoffBars hb(bar.empty + STAGES);  // HANDOFF
   // B_FP8: e4m3 landing ring after the barrier block; its full barriers complete on the TMA bytes, its empty ones once per
   // converter warp
   const BarrierRing<FP8_LAND_STAGES> land_bar(bar.empty + STAGES);
@@ -91,14 +213,15 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   const int wg = threadIdx.x >> 7;
 
   if (warp == 0 && lane == 0) {
-    prefetch_tmap(&tmA);
-    if (p.group_offsets) prefetch_tmap(&tmA_min);
-    prefetch_tmap(&tmB0);
-    if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(&tmB1);
-    if (p.n_seg > 2) prefetch_tmap(&tmB2);
+    prefetch_tmap(tmA);
+    if (p.group_offsets) prefetch_tmap(tmA_min);
+    prefetch_tmap(tmB0);
+    if (p.n_seg > 1 || EPI == ARIA_EPI_SWIGLU) prefetch_tmap(tmB1);
+    if (p.n_seg > 2) prefetch_tmap(tmB2);
     // B_FP8: a stage is full once A has landed AND every converter warp has written its share of B
     bar.init(B_FP8 ? 1 + FP8_CONVERT_WARPS : 1, PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
     if constexpr (B_FP8) land_bar.init(1, FP8_CONVERT_WARPS);
+    if constexpr (HANDOFF) hb.init();
     fence_mbar_init();
   }
   if constexpr (PAIR) cluster_sync();
@@ -114,7 +237,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (wg == 0) {
     // =========================== TMA producer ===========================
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<HANDOFF ? 80 : 40>();  // the epilogue warps: HEADS (RoPE) spilled at 56 to 72; 128 x 80 + 256 x 208 <= 64 K
     if (warp == 0 && elect_one()) {
       const uint32_t rank = PAIR ? cluster_ctarank() : 0;
       TileSched sched;
@@ -134,8 +257,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int bgrp = weight_block(p, grp);
         // B coordinates of this tile (k-invariant part)
         int b_c0 = 0, b_c1 = 0;          // K-major: row (n) coordinate of the two boxes; MN-major: base k row
-        const CUtensorMap* tb0 = &tmB0;
-        const CUtensorMap* tb1 = &tmB1;
+        const CUtensorMap* tb0 = tmB0;
+        const CUtensorMap* tb1 = tmB1;
         if constexpr (B_MN) {
           b_c0 = bgrp * p.K;
         } else if constexpr (EPI == ARIA_EPI_SWIGLU) {
@@ -143,7 +266,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         } else {
           const int col = n_idx * BN;
           const int seg = col / p.N;
-          tb0 = seg == 0 ? &tmB0 : (seg == 1 ? &tmB1 : &tmB2);
+          tb0 = seg == 0 ? tmB0 : (seg == 1 ? tmB1 : tmB2);
           b_c0 = col - seg * p.N + bgrp * p.b_group_rows;
         }
         for (int kb = 0; kb < k_blocks; ++kb) {
@@ -153,14 +276,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           mbar_wait_addr(empty0 + rp.stage * 8, rp.phase ^ 1);
           if constexpr (PAIR) {
             mbar_arrive_expect_tx_addr(fb, phantom ? A_STAGE_BYTES : STAGE_BYTES);
-            tma_load_2d_multicast_addr(sa + rank * (A_STAGE_BYTES / 2), &tmA, fb, kb * BK, a_half_row, 0b11);
+            tma_load_2d_multicast_addr(sa + rank * (A_STAGE_BYTES / 2), tmA, fb, kb * BK, a_half_row, 0b11);
             if (phantom) {
               rp.next();
               continue;
             }
           } else {
             mbar_arrive_expect_tx_addr(fb, a_rows * (BK * 2) + (B_FP8 ? 0 : B_STAGE_BYTES));
-            tma_load_a_rows(sa, &tmA, &tmA_min, fb, kb * BK, a_row, a_rows);
+            tma_load_a_rows(sa, tmA, tmA_min, fb, kb * BK, a_row, a_rows);
           }
           if constexpr (B_MN) {
             // B = [G*K, Ncols] rows k, N contiguous; one box = 64 k-rows x 64 n, BN/64 boxes per stage
@@ -177,7 +300,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             const int krow = b_c0 + kb * BK;
 #pragma unroll
             for (int c = 0; c < BN / 64; ++c)
-              tma_load_2d_addr(dst + c * box_bytes, &tmB0, bar_addr, tile_b_col<BN, EPI>(c * 64, n_idx, p.N), krow);
+              tma_load_2d_addr(dst + c * box_bytes, tmB0, bar_addr, tile_b_col<BN, EPI>(c * 64, n_idx, p.N), krow);
             if constexpr (B_FP8) lp.next();
           } else if constexpr (EPI == ARIA_EPI_SWIGLU) {
             tma_load_2d_addr(sb, tb0, fb, kb * BK, b_c0);
@@ -227,10 +350,19 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           }
         }
       }
+    } else if constexpr (HANDOFF) {
+      if (warp > 0) {
+        // ================ epilogue warps (1-3): finish and store each half the consumers hand off ================
+        const int et = threadIdx.x - 32;
+        handoff_walk<false>(p, n_tiles, hb, [&](int h, int grp, int m_idx, int n_idx, int row0, int rows) {
+          handoff_finish_half<EPI>(p, out_tile + h * HALF_BYTES, &hb.out_free[h], et, h, grp, m_idx, n_idx, row0, rows,
+                                   n_out_total);
+        });
+      }
     }
   } else {
     // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<HANDOFF ? 208 : 232>();
     const int cw = wg - 1;
     constexpr uint32_t b_lbo = B_MN ? 64 * BK * 2 : 16;
     constexpr uint32_t b_sbo = 1024;
@@ -244,6 +376,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     TileSched sched;
     sched.init(p, pair_sched_n<PAIR>(n_tiles));
     RingPos<STAGES> rp;
+    uint32_t free_phase = 0;  // HANDOFF: the phase of out_free[cw] to wait for, inverted
+    const uint32_t half = out_tile + cw * HALF_BYTES;
+    const int fr = ct.frag_row - 64 * cw;  // fragment rows fr and fr + 8 of the warpgroup's half
     // a stage is released to this CTA's producer and, PAIR, to the peer's, whose A half also lands in it
     auto release = [&](int s) {
       if (lane == 0) {
@@ -270,8 +405,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
       // grouped: no row of the group in rows [64, 128) of the tile, which are then not loaded either.  A whole warpgroup sits
-      // out, so the named barrier of its stage_and_epilogue stays consistent.
-      if (sits_out(grouped && cw == 1 && rows - m_idx * BM <= BM / 2)) {
+      // out, so the named barrier of its stage_and_epilogue stays consistent.  HANDOFF: no row of the launch or group in
+      // the warpgroup's half, as the epilogue warps' walk (handoff_walk) assumes.
+      if (sits_out(HANDOFF ? m_idx * BM + 64 * cw >= rows : grouped && cw == 1 && rows - m_idx * BM <= BM / 2)) {
         pass_tile();
         continue;
       }
@@ -280,6 +416,20 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       float2 bsc[BN / 8];
       if constexpr (B_FP8) load_col_scales<BN, EPI>(p, grp, n_idx, ct.frag_col, bsc);
+      // HANDOFF, LINEAR and HEADS: bias pairs of this thread's columns (8 j + frag_col, +1), fetched while the k-loop runs; a
+      // tile lies in one segment, columns past N get 0 and are never stored.  SwiGLU and RoPE segments have no bias.
+      uint32_t bias2[BN / 8];
+      bool has_bias = false;  // no bias: nothing is added, so a -0 stays -0 as in epilogue_tile
+      if constexpr (HANDOFF && EPI != ARIA_EPI_SWIGLU) {
+        const int col0 = n_idx * BN, seg = col0 / p.N, cseg0 = col0 - seg * p.N;
+        const __nv_bfloat16* bias = p.bias[seg];
+        has_bias = bias != nullptr;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = cseg0 + 8 * j + ct.frag_col;
+          bias2[j] = (bias && c < p.N) ? __ldg(reinterpret_cast<const uint32_t*>(bias + c)) : 0u;
+        }
+      }
       // one k-block's wgmma group stays in flight while the next one is issued; a stage is released once its group retired
       int prev = -1;
       for (int kb = 0; kb < k_blocks; ++kb) {
@@ -298,11 +448,48 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       wgmma_wait<0>();
       fence_regs(acc);
       if (prev >= 0) release(prev);
+      if constexpr (HANDOFF) {
+        // the epilogue warps have finished this warpgroup's previous tile and left its half
+        mbar_wait(&hb.out_free[cw], free_phase ^ 1);
+        free_phase ^= 1;
+        // what epilogue_tile rounds first: bf16(x + bias) (LINEAR, HEADS; SwiGLU: bf16(gate) | bf16(up), RoPE: bf16(x))
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
+            float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
+            if (has_bias) {
+              x0 += bf16_lo(bias2[j]);
+              x1 += bf16_hi(bias2[j]);
+            }
+            st_shared_u32(half + out_half_offset(fr + 8 * i, 8 * j + ct.frag_col), pack_bf16(x0, x1));
+          }
+        }
+        mbar_arrive(&hb.out_full[cw]);
+        continue;
+      }
       stage_and_epilogue<BN, EPI, B_FP8 ? AccScale::COL : AccScale::NONE>(p, stg, ct, acc, bsc, 1.f, 1.f, n_out_total, grp,
                                                                            m_idx, n_idx, row0, rows);
     }
   }
   if constexpr (PAIR) cluster_sync();
+}
+
+template <int BN, bool B_MN, int EPI, bool B_FP8 = false, bool PAIR = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA_min,
+            const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
+            const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+  gemm_body<BN, B_MN, EPI, B_FP8, PAIR, false>(&tmA, &tmA_min, &tmB0, &tmB1, &tmB2, p);
+}
+
+// gemm_kernel with the hand-off epilogue (HANDOFF above): 128-wide tiles, bf16 B, one CTA
+template <bool B_MN, int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_handoff_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA_min,
+                    const __grid_constant__ CUtensorMap tmB0, const __grid_constant__ CUtensorMap tmB1,
+                    const __grid_constant__ CUtensorMap tmB2, const GemmParams p) {
+  gemm_body<128, B_MN, EPI, false, false, true>(&tmA, &tmA_min, &tmB0, &tmB1, &tmB2, p);
 }
 
 // Wide dense GEMM for the 4,900-row ViT and projector launches (gemm_run): bf16, nn.Linear weights, LINEAR or HEADS without
@@ -326,44 +513,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 // (same protocol, same phantom tile).
 constexpr int WIDE_BN = 192;
 constexpr int WIDE_STAGE_BYTES = A_STAGE_BYTES + WIDE_BN * BK * 2;  // 16 + 24 KB
-constexpr int WIDE_BOX_BYTES = 64 * 64 * 2;                         // one 64-row x 64-column bf16 SW128 box of the output
-constexpr int WIDE_HALF_BYTES = 3 * WIDE_BOX_BYTES;                 // a consumer warpgroup's 64 output rows
+constexpr int WIDE_HALF_BYTES = 3 * OUT_BOX_BYTES;  // a consumer warpgroup's 64 output rows: three boxes
 constexpr int gemm_wide_smem_bytes() {
   return 1024 /*align*/ + GEMM_STAGES * WIDE_STAGE_BYTES + 2 * WIDE_HALF_BYTES + 256 /*barriers*/;
 }
 static_assert(gemm_wide_smem_bytes() <= 232448, "wide GEMM must fit the opt-in shared memory of a block");
-
-// Byte offset of bf16 column c (even) of row r in a warpgroup's output half: box c / 64, its 16-byte chunk swizzled as TMA's
-// 128-byte swizzle places it
-ARIA_DEVICE uint32_t wide_out_offset(int r, int c) {
-  return (c >> 6) * WIDE_BOX_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
-}
-
-// Hand-off epilogue warps of gemm_wide_kernel: how many, and their named barrier (the consumer warpgroups use 1 and 2)
-constexpr int WIDE_EPI_THREADS = 96;
-constexpr uint32_t WIDE_EPI_BAR = 3;
-
-// The activation of the first n_chunks 16-byte chunks of an output half, in place: bf16(act(x)) of each bf16 x, as
-// epilogue_tile computes it.  Element-wise, so chunks go in address order whatever the swizzle; two per thread and
-// iteration, so each of the few epilogue warps has independent work in flight.
-template <int ACT>
-ARIA_DEVICE void wide_act_inplace(uint32_t half, int n_chunks, int et) {
-  auto act8 = [](uint4& v) {
-    uint32_t* w = reinterpret_cast<uint32_t*>(&v);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) w[e] = pack_bf16(bf16r(act_apply(bf16_lo(w[e]), ACT)), bf16r(act_apply(bf16_hi(w[e]), ACT)));
-  };
-#pragma unroll 1
-  for (int i = et; i < n_chunks; i += 2 * WIDE_EPI_THREADS) {
-    const uint32_t a0 = half + 16 * i, a1 = a0 + 16 * WIDE_EPI_THREADS;
-    const bool two = i + WIDE_EPI_THREADS < n_chunks;
-    uint4 v0 = ld_shared_v4(a0), v1 = two ? ld_shared_v4(a1) : make_uint4(0, 0, 0, 0);
-    act8(v0);
-    act8(v1);
-    st_shared_v4(a0, v0);
-    if (two) st_shared_v4(a1, v1);
-  }
-}
 
 template <int EPI, bool PAIR, bool HANDOFF>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -378,9 +532,10 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint8_t* smem = smem_1024();
   uint8_t* out_tile = smem + STAGES * WIDE_STAGE_BYTES;  // [2 warpgroups][3 boxes][64 rows][128 B]
   const BarrierRing<STAGES> bar(out_tile + 2 * WIDE_HALF_BYTES);
-  uint64_t* res_full = bar.empty + STAGES;  // [2]: the residual rows of a warpgroup's half have landed in it
-  uint64_t* out_free = res_full + 2;        // [2]: a warpgroup's previous tile has left its half (stored or scattered)
-  uint64_t* out_full = out_free + 2;        // [2]: hand-off: a warpgroup has written its tile into its half
+  // out_free[2]: a warpgroup's previous tile has left its half (stored or scattered); out_full[2]: hand-off only
+  const HandoffBars hb(bar.empty + STAGES);
+  uint64_t* out_free = hb.out_free;
+  uint64_t* res_full = out_free + 2;  // [2]: the residual rows of a warpgroup's half have landed in it
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -396,11 +551,8 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (EPI == ARIA_EPI_LINEAR) prefetch_tmap(&tmOut);
     if (res) prefetch_tmap(&tmRes);
     bar.init(1, PAIR ? 2 * CONSUMER_WARPS : CONSUMER_WARPS);
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(&res_full[h], 1);
-      mbar_init(&out_free[h], 1);
-      mbar_init(&out_full[h], 128);  // every consumer thread of the warpgroup
-    }
+    hb.init();
+    for (int h = 0; h < 2; ++h) mbar_init(&res_full[h], 1);
     fence_mbar_init();
   }
   if constexpr (PAIR) cluster_sync();
@@ -461,9 +613,9 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               if (a_row + 64 * h >= rows) continue;  // a half past the last row: no consumer waits for it
               mbar_wait(&out_free[h], (out_phase >> h) & 1);
               out_phase ^= 1u << h;
-              mbar_arrive_expect_tx(&res_full[h], nbox * WIDE_BOX_BYTES);
+              mbar_arrive_expect_tx(&res_full[h], nbox * OUT_BOX_BYTES);
               for (int c = 0; c < nbox; ++c)
-                tma_load_2d(out_tile + h * WIDE_HALF_BYTES + c * WIDE_BOX_BYTES, &tmRes, &res_full[h], col0 + 64 * c,
+                tma_load_2d(out_tile + h * WIDE_HALF_BYTES + c * OUT_BOX_BYTES, &tmRes, &res_full[h], col0 + 64 * c,
                             a_row + 64 * h);
             }
           }
@@ -472,64 +624,51 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     } else if (warp > 0 && handoff) {
       // ================ epilogue warps (1-3): activation and store of each half the consumers hand off ================
       const int et = threadIdx.x - 32;
-      const uint32_t rank = PAIR ? cluster_ctarank() : 0;
-      TileSched sched;
-      sched.init(p, pair_sched_n<PAIR>(n_tiles));
-      uint32_t full_phase = 0;  // bit h: the phase of out_full[h] to wait for
-      for (int t = first_tile<PAIR>();; t += tile_step<PAIR>()) {
-        int grp, m_idx, n_idx, row0, rows;
-        if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
-        if constexpr (PAIR) n_idx = 2 * n_idx + rank;
-        if (PAIR && n_idx >= n_tiles) continue;  // phantom tile
+      handoff_walk<PAIR>(p, n_tiles, hb, [&](int h, int grp, int m_idx, int n_idx, int row0, int rows) {
         const int col0 = n_idx * BN;
         const int seg = col0 / p.N;
         const int cseg0 = col0 - seg * p.N;
-        for (int h = 0; h < 2; ++h) {
-          if (m_idx * BM + 64 * h >= rows) continue;  // the consumers sit this half out
-          mbar_wait(&out_full[h], (full_phase >> h) & 1);
-          full_phase ^= 1u << h;
-          const uint32_t half = smem_u32(out_tile) + h * WIDE_HALF_BYTES;
-          if constexpr (EPI == ARIA_EPI_LINEAR) {
-            const int nbox = tile_boxes(col0);
-            if (p.act == ARIA_ACT_GELU_TANH || p.act == ARIA_ACT_GELU_NEW) {
-              const int n_chunks = nbox * (WIDE_BOX_BYTES / 16);
-              if (p.act == ARIA_ACT_GELU_TANH) wide_act_inplace<ARIA_ACT_GELU_TANH>(half, n_chunks, et);
-              else wide_act_inplace<ARIA_ACT_GELU_NEW>(half, n_chunks, et);
-              fence_proxy_async_smem();
-            }
-            named_bar_sync(WIDE_EPI_BAR, WIDE_EPI_THREADS);
-            if (et == 0) {
-              fence_proxy_async_smem();
-              for (int c = 0; c < nbox; ++c)
-                tma_store_2d_addr(&tmOut, half + c * WIDE_BOX_BYTES, col0 + 64 * c, m_idx * BM + 64 * h);
-              bulk_commit_group();
-              bulk_wait_group_read<0>();
-              mbar_arrive(&out_free[h]);
-            }
-          } else {
-            // heads_store_tile's mapping, consecutive threads on consecutive 8-column chunks of a row.  96 threads are 4 rows
-            // of 24 chunks, so a thread keeps its column chunk (head, d) and steps 4 rows at a time.
-            constexpr int CH = BN / 8;
-            constexpr int ROW_STEP = WIDE_EPI_THREADS / CH;
-            static_assert(WIDE_EPI_THREADS % CH == 0, "a thread keeps its column chunk");
-            const int c = (et % CH) * 8, cs = cseg0 + c;
-            if (cs + 8 <= p.N) {
-              const int head = cs / p.head_dim, d = cs - head * p.head_dim;
-              __nv_bfloat16* col_base = p.out[seg] + head * p.stride_h + d;
-              int r = et / CH, r_in_grp = m_idx * BM + 64 * h + r;
-              int b = r_in_grp / p.rows_per_batch, tok = r_in_grp - b * p.rows_per_batch;
-#pragma unroll 1
-              for (; r < 64 && r_in_grp < rows; r += ROW_STEP, r_in_grp += ROW_STEP) {
-                st_global_v4(col_base + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld,
-                             ld_shared_v4(half + wide_out_offset(r, c)));
-                for (tok += ROW_STEP; tok >= p.rows_per_batch; tok -= p.rows_per_batch) ++b;
-              }
-            }
-            named_bar_sync(WIDE_EPI_BAR, WIDE_EPI_THREADS);  // every chunk of the half has been read
-            if (et == 0) mbar_arrive(&out_free[h]);
+        const uint32_t half = smem_u32(out_tile) + h * WIDE_HALF_BYTES;
+        if constexpr (EPI == ARIA_EPI_LINEAR) {
+          const int nbox = tile_boxes(col0);
+          if (p.act == ARIA_ACT_GELU_TANH || p.act == ARIA_ACT_GELU_NEW) {
+            const int n_chunks = nbox * (OUT_BOX_BYTES / 16);
+            if (p.act == ARIA_ACT_GELU_TANH) act_inplace<ARIA_ACT_GELU_TANH>(half, n_chunks, et);
+            else act_inplace<ARIA_ACT_GELU_NEW>(half, n_chunks, et);
+            fence_proxy_async_smem();
           }
+          named_bar_sync(EPI_BAR, EPI_THREADS);
+          if (et == 0) {
+            fence_proxy_async_smem();
+            for (int c = 0; c < nbox; ++c)
+              tma_store_2d_addr(&tmOut, half + c * OUT_BOX_BYTES, col0 + 64 * c, m_idx * BM + 64 * h);
+            bulk_commit_group();
+            bulk_wait_group_read<0>();
+            mbar_arrive(&out_free[h]);
+          }
+        } else {
+          // heads_store_tile's mapping, consecutive threads on consecutive 8-column chunks of a row.  96 threads are 4 rows
+          // of 24 chunks, so a thread keeps its column chunk (head, d) and steps 4 rows at a time.
+          constexpr int CH = BN / 8;
+          constexpr int ROW_STEP = EPI_THREADS / CH;
+          static_assert(EPI_THREADS % CH == 0, "a thread keeps its column chunk");
+          const int c = (et % CH) * 8, cs = cseg0 + c;
+          if (cs + 8 <= p.N) {
+            const int head = cs / p.head_dim, d = cs - head * p.head_dim;
+            __nv_bfloat16* col_base = p.out[seg] + head * p.stride_h + d;
+            int r = et / CH, r_in_grp = m_idx * BM + 64 * h + r;
+            int b = r_in_grp / p.rows_per_batch, tok = r_in_grp - b * p.rows_per_batch;
+#pragma unroll 1
+            for (; r < 64 && r_in_grp < rows; r += ROW_STEP, r_in_grp += ROW_STEP) {
+              st_global_v4(col_base + b * p.stride_b + static_cast<int64_t>(p.pos0 + tok) * p.head_ld,
+                           ld_shared_v4(half + out_half_offset(r, c)));
+              for (tok += ROW_STEP; tok >= p.rows_per_batch; tok -= p.rows_per_batch) ++b;
+            }
+          }
+          named_bar_sync(EPI_BAR, EPI_THREADS);  // every chunk of the half has been read
+          if (et == 0) mbar_arrive(&out_free[h]);
         }
-      }
+      });
     }
   } else {
     // =========================== consumers: MMA + epilogue of rows [64 cw, +64) of each tile ===========================
@@ -620,11 +759,11 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               x0 += bf16_lo(bias2[j]);
               x1 += bf16_hi(bias2[j]);
             }
-            st_shared_u32(half_s + wide_out_offset(fr + 8 * i, 8 * j + ct.frag_col), pack_bf16(x0, x1));
+            st_shared_u32(half_s + out_half_offset(fr + 8 * i, 8 * j + ct.frag_col), pack_bf16(x0, x1));
           }
         }
         if constexpr (EPI == ARIA_EPI_LINEAR) fence_proxy_async_smem();  // the epilogue warps' TMA store reads the half
-        mbar_arrive(&out_full[cw]);
+        mbar_arrive(&hb.out_full[cw]);
         continue;
       }
       if constexpr (EPI == ARIA_EPI_LINEAR) {  // with a residual
@@ -636,7 +775,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int c = 8 * j + ct.frag_col;
 #pragma unroll
           for (int i = 0; i < 2; ++i) {  // rows fr and fr + 8
-            uint32_t* dst = reinterpret_cast<uint32_t*>(half + wide_out_offset(fr + 8 * i, c));
+            uint32_t* dst = reinterpret_cast<uint32_t*>(half + out_half_offset(fr + 8 * i, c));
             float x0 = acc[4 * j + 2 * i], x1 = acc[4 * j + 2 * i + 1];
             if (bias) {
               x0 += bf16_lo(bias2[j]);
@@ -661,7 +800,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         if (leader) {
           const int nbox = tile_boxes(col0);
           for (int c = 0; c < nbox; ++c)
-            tma_store_2d_addr(&tmOut, smem_u32(half + c * WIDE_BOX_BYTES), col0 + 64 * c, m_idx * BM + 64 * cw);
+            tma_store_2d_addr(&tmOut, smem_u32(half + c * OUT_BOX_BYTES), col0 + 64 * c, m_idx * BM + 64 * cw);
           bulk_commit_group();
         }
       }
@@ -1077,16 +1216,31 @@ static int gemm_run(const aria_gemm_desc_t* d, const float* b_scale, cudaStream_
     if (swiglu) ARIA_LAUNCH(128, true, ARIA_EPI_SWIGLU, true);
     ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR, true);
   }
+  // the hand-off epilogue (gemm_kernel's HANDOFF) for the launches whose epilogue is long next to their tiles' mainloop: the
+  // grouped expert GEMMs without a residual (fc1 + SwiGLU, fc2; expert-parallel regions and per-group destinations
+  // included), dense SwiGLU (the shared experts' gate/up) and HEADS with RoPE (the LM's q/k/v).  Dense LINEAR launches and
+  // the ViT / projector heads without RoPE below 2,048 rows keep the staged epilogue: their gain was not measured apart
+  // from run-to-run noise (DESIGN §6).
+#define ARIA_LAUNCH_HANDOFF(MN_, EPI_)                                                                                \
+  return launch_persistent<gemm_handoff_kernel<MN_, EPI_>>("gemm_handoff_kernel", GEMM_THREADS,                      \
+                                                           gemm_smem_bytes<128, false, false, handoff_stages(MN_)>(), \
+                                                           tiles, stream, tmA, tmA_min, tmB[0], tmB[1], tmB[2], p)
   if (d->epilogue == ARIA_EPI_HEADS) {
+    if (BN == 128 && d->rope_mask) ARIA_LAUNCH_HANDOFF(false, ARIA_EPI_HEADS);
     if (BN == 128) ARIA_LAUNCH(128, false, ARIA_EPI_HEADS);
     ARIA_LAUNCH(144, false, ARIA_EPI_HEADS);
   }
   if (swiglu) {
-    if (b_mn) ARIA_LAUNCH(128, true, ARIA_EPI_SWIGLU);
-    ARIA_LAUNCH(128, false, ARIA_EPI_SWIGLU);
+    if (b_mn) ARIA_LAUNCH_HANDOFF(true, ARIA_EPI_SWIGLU);
+    ARIA_LAUNCH_HANDOFF(false, ARIA_EPI_SWIGLU);
+  }
+  if (d->group_offsets && !d->residual) {
+    if (b_mn) ARIA_LAUNCH_HANDOFF(true, ARIA_EPI_LINEAR);
+    ARIA_LAUNCH_HANDOFF(false, ARIA_EPI_LINEAR);
   }
   if (b_mn) ARIA_LAUNCH(128, true, ARIA_EPI_LINEAR);
   ARIA_LAUNCH(128, false, ARIA_EPI_LINEAR);
+#undef ARIA_LAUNCH_HANDOFF
 #undef ARIA_LAUNCH
 }
 

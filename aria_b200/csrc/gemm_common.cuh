@@ -480,4 +480,90 @@ ARIA_DEVICE void stage_and_epilogue(const GemmParams& p, float* stg, const Consu
   epilogue_tile<BN, EPI>(p, stg + ct.epi_row * ACC_LD, n_out_total, n_idx, grow, row_ok, ct.half, grp, r_in_grp);
 }
 
+// The persistent loop of a CTA: tiles blockIdx.x, + gridDim.x, ...  PAIR: both CTAs of a cluster walk the same pair indices,
+// so their trip counts are identical, and the scheduler's n-tiles are n-pairs
+template <bool PAIR> ARIA_DEVICE int first_tile() { return PAIR ? blockIdx.x >> 1 : blockIdx.x; }
+template <bool PAIR> ARIA_DEVICE int tile_step() { return PAIR ? gridDim.x >> 1 : gridDim.x; }
+template <bool PAIR> ARIA_DEVICE int pair_sched_n(int n_tiles) { return PAIR ? (n_tiles + 1) / 2 : n_tiles; }
+
+// ---- Hand-off epilogue (gemm_kernel and gemm_wide_kernel with HANDOFF) ----
+// After a tile's last MMA each consumer warpgroup writes its 64 rows as bf16 into its half of an output tile in shared
+// memory (64-row x 64-column SW128 boxes), arrives on out_full[cw] and goes on to the next tile's k-loop; it waits on
+// out_free[cw] only before it writes its next tile's half.  The producer warpgroup's warps 1-3, which issue no TMA, are the
+// epilogue warps: they walk the same tiles (handoff_walk), wait on out_full for each half, finish it (activation, SwiGLU,
+// RoPE, scatter, stores) and arrive on out_free.  So the tensor cores do not idle through the epilogue.
+constexpr int OUT_BOX_BYTES = 64 * 64 * 2;  // one 64-row x 64-column bf16 SW128 box of an output half
+constexpr int EPI_THREADS = 96;             // the epilogue warps
+constexpr uint32_t EPI_BAR = 3;             // their named barrier (the consumer warpgroups use 1 and 2)
+
+// Byte offset of bf16 column c (even) of row r in an output half: box c / 64, its 16-byte chunk swizzled as TMA's 128-byte
+// swizzle places it
+ARIA_DEVICE uint32_t out_half_offset(int r, int c) {
+  return (c >> 6) * OUT_BOX_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
+}
+
+// out_full[2]: warpgroup cw has written its tile into half cw (all 128 threads arrive); out_free[2]: the epilogue warps
+// have left half cw (one arrival).  init() runs on one thread before the block's first barrier.
+struct HandoffBars {
+  uint64_t* out_full;
+  uint64_t* out_free;
+  ARIA_DEVICE explicit HandoffBars(uint64_t* at) : out_full(at), out_free(at + 2) {}
+  ARIA_DEVICE void init() const {
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(&out_full[h], 128);
+      mbar_init(&out_free[h], 1);
+    }
+  }
+};
+
+// bf16(act(x)) of the eight bf16 values of a 16-byte chunk, as epilogue_tile computes it from bf16(x + bias)
+template <int ACT>
+ARIA_DEVICE void act_bf16x8(uint4& v) {
+  uint32_t* w = reinterpret_cast<uint32_t*>(&v);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) w[e] = pack_bf16(bf16r(act_apply(bf16_lo(w[e]), ACT)), bf16r(act_apply(bf16_hi(w[e]), ACT)));
+}
+
+// The activation of the first n_chunks 16-byte chunks of an output half, in place.  Element-wise, so chunks go in address
+// order whatever the swizzle; two per thread and iteration, so each of the few epilogue warps has independent work in flight.
+template <int ACT>
+ARIA_DEVICE void act_inplace(uint32_t half, int n_chunks, int et) {
+#pragma unroll 1
+  for (int i = et; i < n_chunks; i += 2 * EPI_THREADS) {
+    const uint32_t a0 = half + 16 * i, a1 = a0 + 16 * EPI_THREADS;
+    const bool two = i + EPI_THREADS < n_chunks;
+    uint4 v0 = ld_shared_v4(a0), v1 = two ? ld_shared_v4(a1) : make_uint4(0, 0, 0, 0);
+    act_bf16x8<ACT>(v0);
+    act_bf16x8<ACT>(v1);
+    st_shared_v4(a0, v0);
+    if (two) st_shared_v4(a1, v1);
+  }
+}
+
+// The epilogue warps' walk: the consumers' tile sequence, without the phantom tiles of a pair and the halves with no row
+// of the tile (the consumers sit those out); finish(h, grp, m_idx, n_idx, row0, rows) runs once half h is full and must
+// end with one arrival on out_free[h].
+template <bool PAIR, class Finish>
+ARIA_DEVICE void handoff_walk(const GemmParams& p, int n_tiles, const HandoffBars& hb, Finish&& finish) {
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+  TileSched sched;
+  sched.init(p, pair_sched_n<PAIR>(n_tiles));
+  uint32_t full_phase = 0;  // bit h: the phase of out_full[h] to wait for
+  // the step is read from %nctaid each tile: held in a register across the tile, it was the one value ptxas spilled under
+  // the epilogue warps' register budget (HEADS, gemm_kernel)
+  for (int t = first_tile<PAIR>();; t += PAIR ? nctaid_x() >> 1 : nctaid_x()) {
+    int grp, m_idx, n_idx, row0, rows;
+    if (!sched.decode(t, grp, m_idx, n_idx, row0, rows)) break;
+    if constexpr (PAIR) n_idx = 2 * n_idx + rank;
+    if (PAIR && n_idx >= n_tiles) continue;  // phantom tile
+#pragma unroll 1  // one copy of finish: unrolled, the epilogue warps' HEADS finish spilled under setmaxnreg
+    for (int h = 0; h < 2; ++h) {
+      if (m_idx * BM + 64 * h >= rows) continue;  // the consumers sit this half out
+      mbar_wait(&hb.out_full[h], (full_phase >> h) & 1);
+      full_phase ^= 1u << h;
+      finish(h, grp, m_idx, n_idx, row0, rows);
+    }
+  }
+}
+
 }  // namespace aria

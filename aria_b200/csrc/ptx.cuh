@@ -27,6 +27,13 @@ ARIA_DEVICE uint4 ld_shared_v4(uint32_t addr) {
   return v;
 }
 
+// gridDim.x, read from the special register where it is used (the compiler cannot hoist a volatile read into a register)
+ARIA_DEVICE int nctaid_x() {
+  int n;
+  asm volatile("mov.u32 %0, %%nctaid.x;" : "=r"(n));
+  return n;
+}
+
 ARIA_DEVICE uint32_t elect_one() {
   uint32_t pred = 0;
   asm volatile(
