@@ -140,6 +140,9 @@ SIGNATURES = {
     "aria_sample_tokens_slots": (i32, [vp, i64, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]),
     "aria_decode_advance_slots": (i32, [vp, vp, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp]),
     "aria_token_logprobs": (i32, [vp, i64, vp, i32, i32, i32, vp, vp, i32, i32, vp, i32, vp, vp, vp, i32, vp]),
+    "aria_sample_tokens_processed": (i32, [vp, i64, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, vp,
+                                           i32, vp]),
+    "aria_presence_set": (i32, [vp, i64, i32, i32, vp, i32, vp, i32, vp]),
 }
 
 _lib = None

@@ -21,6 +21,16 @@
 // aria_sample_tokens_slots: aria_sample_tokens_rows with the temperature, top_k, top_p and seed of each row also read from
 // device arrays (continuous batching: every slot samples with its own request's parameters).
 //
+// aria_sample_tokens_processed: aria_sample_tokens_slots behind Hugging Face's logits processors, each row with its own:
+//   RepetitionPenaltyLogitsProcessor -> MinNewTokensLengthLogitsProcessor -> (sampling) the warpers above -> MinPLogitsWarper.
+//   Every score is the fp32 value of the bf16 logit, divided (IEEE, __fdiv_rn) or multiplied by the penalty when the id is set in
+//   the row's presence bitmap (loaded to shared memory), or -inf for an EOS id while fewer than min_new tokens are out.  Such
+//   scores are no longer bf16 values, so the select, the top-p list and the argmax run on the 32-bit order-preserving key of the
+//   fp32 score (four 8-bit histogram passes); for a bf16-valued score it orders exactly as the 16-bit key, so a row whose
+//   processors are off gets aria_sample_tokens' token and probabilities bit for bit.  Min-p is a cut in the final pass: kept
+//   entries with p < min_p * p_max, p over the top-k / top-p survivors, are removed (the largest has p_max).
+// aria_presence_set: the bits of an id matrix into those bitmaps.
+//
 // aria_token_logprobs: the log-probability of a token under a row's raw distribution and the row's top n (n <= 20) by (value
 // desc, id asc), one CTA per row, reusing the radix select above (see token_logprobs_kernel).
 #include <float.h>
@@ -35,6 +45,8 @@ constexpr int SP_WARPS = SP_THREADS / 32;
 constexpr int SP_MAX_K = 1024;
 constexpr int32_t SP_MAX_ROWS = 1 << 20;
 constexpr int32_t SP_MAX_VOCAB = 1 << 24;
+constexpr int32_t SP_PROC_MAX_VOCAB = 1 << 18;  // the presence bitmap (V / 32 words) fits the shared memory left beside SampleSmem
+constexpr int SP_MAX_EOS = 8;
 
 struct SampleParams {
   const uint16_t* logits;  // bf16 bits, row r at logits + r * stride
@@ -55,6 +67,12 @@ __device__ __forceinline__ float key_to_float(uint32_t k) {
   const uint32_t u = (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu);
   return __uint_as_float(u << 16);
 }
+// the same for an fp32 value: the 32-bit key of the processed scores
+__device__ __forceinline__ uint32_t f32_key(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float f32_key_to_float(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
 
 // Philox4x32-10 (Salmon et al., SC'11); the first output word
 __device__ __forceinline__ uint32_t philox_x0(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1) {
@@ -86,6 +104,7 @@ struct SampleSmem {
   unsigned long long list[SP_MAX_K];  // (key << 32) | index, keys strictly above the pivot
   float red_f[SP_WARPS];
   int red_i[SP_WARPS];
+  unsigned long long red_u[SP_WARPS];
   int n_list;
   int bin, above;
   int cut;
@@ -123,6 +142,20 @@ __device__ void block_argmax(float& s, int& i, SampleSmem& sm) {
     const int oi = __shfl_xor_sync(0xffffffffu, i, o);
     if (arg_better(os, oi, s, i)) s = os, i = oi;
   }
+}
+
+// Block maximum of (key << 32) | ~index entries: the largest key, ties to the lowest index.
+__device__ unsigned long long block_max_u64(unsigned long long v, SampleSmem& sm) {
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();
+  if (lane == 0) sm.red_u[warp] = v;
+  __syncthreads();
+  v = lane < SP_WARPS ? sm.red_u[lane] : 0ull;
+#pragma unroll
+  for (int o = 16; o; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
 }
 
 // Inclusive scan over the block in thread order.
@@ -181,14 +214,28 @@ struct SlotSampling {
   const uint64_t* seed;
 };
 
+// Per-row logits processors of aria_sample_tokens_processed
+struct Processing {
+  const float* min_p;          // [R]
+  const float* penalty;        // [R], repetition penalty
+  const int32_t* min_new;      // [R]
+  const uint32_t* presence;    // [R, words] bitmaps
+  const int32_t* n_emitted;    // [R] (emitted_per_row) or [1]: tokens the row has emitted
+  int emitted_per_row, offset_per_row, words, n_eos;
+  int eos[SP_MAX_EOS];         // EOS ids inside [0, V)
+};
+
 // ROWS (aria_sample_tokens_rows): logits row `row` draws the noise of row noise_rows[row] at offset offsets[row] instead of
 // (row, *p.rng_offset).  SLOTS (with ROWS): the row's temperature, top_k, top_p and seed come from `slots`, brought into the
 // ranges aria_sample_tokens accepts (a caller checks them; this keeps a bad entry from reading past shared memory).
-// Everything else is the same code.
-template <bool ROWS, bool SLOTS = false>
+// PROC (with SLOTS): the row's scores are its processed logits (`proc`), keyed by 32 bits; the noise row is noise_rows[row] or
+// row when noise_rows is NULL, the offset offsets[row] or offsets[0].  Everything else is the same code.
+template <bool ROWS, bool SLOTS = false, bool PROC = false>
 __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __restrict__ noise_rows,
-                                            const uint64_t* __restrict__ offsets, const SlotSampling slots = {}) {
+                                            const uint64_t* __restrict__ offsets, const SlotSampling slots = {},
+                                            const Processing& proc = {}) {
   __shared__ SampleSmem sm;
+  extern __shared__ uint32_t presence_sm[];  // PROC: the row's presence bitmap
   if constexpr (SLOTS) {
     const int r = blockIdx.x;
     const float t = slots.temperature[r];
@@ -204,14 +251,53 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
   const uint16_t* x = p.logits + static_cast<int64_t>(row) * p.stride;
   float* probs = p.probs ? p.probs + static_cast<int64_t>(row) * V : nullptr;
 
-  if (p.temperature == 0.f) {  // greedy
-    float bs = -INFINITY;
-    int bi = INT_MAX;
-    for (int i = tid; i < V; i += SP_THREADS) {
-      const float k = static_cast<float>(bf16_key(x[i]));  // keys < 2^16 are exact in fp32
-      if (arg_better(k, i, bs, bi)) bs = k, bi = i;
+  float penalty = 1.f, min_p = 0.f;
+  bool no_eos = false;
+  if constexpr (PROC) {
+    const float pen = proc.penalty[row], mp = proc.min_p[row];
+    penalty = pen > 0.f && pen <= FLT_MAX ? pen : 1.f;
+    min_p = mp > 0.f && mp <= 1.f ? mp : 0.f;
+    no_eos = proc.n_eos > 0 && proc.n_emitted[proc.emitted_per_row ? row : 0] < proc.min_new[row];
+    if (penalty != 1.f) {
+      const uint32_t* src = proc.presence + static_cast<int64_t>(row) * proc.words;
+      for (int w = tid; w < proc.words; w += SP_THREADS) presence_sm[w] = src[w];
     }
-    block_argmax(bs, bi, sm);
+    __syncthreads();
+  }
+  // the score of id i (Hugging Face's fp32 copy of the logit, processed) and its order-preserving key; key_value inverts it
+  auto score = [&](int i) -> float {
+    float v = __uint_as_float(static_cast<uint32_t>(x[i]) << 16);
+    if constexpr (PROC) {
+      if (penalty != 1.f && ((presence_sm[i >> 5] >> (i & 31)) & 1u)) v = v < 0.f ? __fmul_rn(v, penalty) : __fdiv_rn(v, penalty);
+      if (no_eos) {
+#pragma unroll
+        for (int e = 0; e < SP_MAX_EOS; ++e)
+          if (e < proc.n_eos && i == proc.eos[e]) v = -INFINITY;
+      }
+    }
+    return v;
+  };
+  auto key_at = [&](int i) -> uint32_t {
+    if constexpr (PROC) return f32_key(score(i));
+    else return bf16_key(x[i]);
+  };
+  auto key_value = [&](uint32_t key) -> float {
+    if constexpr (PROC) return f32_key_to_float(key);
+    else return key_to_float(key);
+  };
+  // the largest key of the row, ties to the lowest id -> (key, id)
+  auto argmax_key = [&](uint32_t& key, int& id) {
+    unsigned long long b = 0;
+    for (int i = tid; i < V; i += SP_THREADS) b = max(b, (static_cast<unsigned long long>(key_at(i)) << 32) | (0xFFFFFFFFu - i));
+    b = block_max_u64(b, sm);
+    key = static_cast<uint32_t>(b >> 32);
+    id = static_cast<int>(0xFFFFFFFFu - static_cast<uint32_t>(b));
+  };
+
+  if (p.temperature == 0.f) {  // greedy
+    uint32_t bk;
+    int bi;
+    argmax_key(bk, bi);
     if (tid == 0) p.next_ids[row] = bi;
     if (probs)
       for (int i = tid; i < V; i += SP_THREADS) probs[i] = i == bi ? 1.f : 0.f;
@@ -228,27 +314,25 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
   unsigned long long fk_comp = 0;     // (key, index) of the smallest kept list entry
 
   if (k > 0) {
-    // ---- radix select of the k-th largest key: high byte, then low byte
-    for (int i = tid; i < 256; i += SP_THREADS) sm.hist[i] = 0;
+    // ---- radix select of the k-th largest key, one byte at a time from the top (16-bit keys: two passes, 32-bit: four)
+    constexpr int KEY_BITS = PROC ? 32 : 16;
     if (tid == 0) sm.n_list = 0;
-    __syncthreads();
-    for (int i = tid; i < V; i += SP_THREADS) atomicAdd(&sm.hist[bf16_key(x[i]) >> 8], 1u);
-    find_bin(sm, k);
-    const uint32_t hb = sm.bin;
-    const int above_hi = sm.above;
-    for (int i = tid; i < 256; i += SP_THREADS) sm.hist[i] = 0;
-    __syncthreads();
-    for (int i = tid; i < V; i += SP_THREADS) {
-      const uint32_t key = bf16_key(x[i]);
-      if ((key >> 8) == hb) atomicAdd(&sm.hist[key & 0xFF], 1u);
+#pragma unroll
+    for (int shift = KEY_BITS - 8; shift >= 0; shift -= 8) {
+      for (int i = tid; i < 256; i += SP_THREADS) sm.hist[i] = 0;
+      __syncthreads();
+      for (int i = tid; i < V; i += SP_THREADS) {
+        const uint32_t key = key_at(i);
+        if (shift == KEY_BITS - 8 || (key >> (shift + 8)) == pivot) atomicAdd(&sm.hist[(key >> shift) & 0xFF], 1u);
+      }
+      find_bin(sm, k - n_gt);
+      pivot = (pivot << 8) | sm.bin;  // the key prefix selected so far
+      n_gt += sm.above;
     }
-    find_bin(sm, k - above_hi);
-    pivot = (hb << 8) | sm.bin;
-    n_gt = above_hi + sm.above;
     n_tie = static_cast<int>(sm.hist[sm.bin]);
     // ---- compact the keys above the pivot (n_gt < k of them) and sort them ascending by (key, index)
     for (int i = tid; i < V; i += SP_THREADS) {
-      const uint32_t key = bf16_key(x[i]);
+      const uint32_t key = key_at(i);
       if (key > pivot) sm.list[atomicAdd(&sm.n_list, 1)] = (static_cast<unsigned long long>(key) << 32) | static_cast<uint32_t>(i);
     }
     __syncthreads();
@@ -270,10 +354,10 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
     }
     __syncthreads();
     // ---- softmax over the top-k set: pivot ties (probability q_piv each) first, then the sorted list
-    const float s_piv = key_to_float(pivot) / temp;
+    const float s_piv = key_value(pivot) / temp;
     const bool mine = tid < n_gt;
-    const float s_t = mine ? key_to_float(static_cast<uint32_t>(sm.list[tid] >> 32)) / temp : -INFINITY;
-    m = n_gt > 0 ? key_to_float(static_cast<uint32_t>(sm.list[n_gt - 1] >> 32)) / temp : s_piv;
+    const float s_t = mine ? key_value(static_cast<uint32_t>(sm.list[tid] >> 32)) / temp : -INFINITY;
+    m = n_gt > 0 ? key_value(static_cast<uint32_t>(sm.list[n_gt - 1] >> 32)) / temp : s_piv;
     const float e_t = mine ? expf(s_t - m) : 0.f;
     const float e_piv = expf(s_piv - m);
     const float cum_t = block_scan(e_t, sm);
@@ -299,7 +383,7 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
         int base = 0;
         for (int i0 = 0; i0 < V && base < r_tie; i0 += SP_THREADS) {
           const int i = i0 + tid;
-          const bool t = i < V && bf16_key(x[i]) == pivot;
+          const bool t = i < V && key_at(i) == pivot;
           const unsigned bal = __ballot_sync(0xffffffffu, t);
           __syncthreads();
           if (lane == 0) sm.red_i[warp] = __popc(bal);
@@ -323,36 +407,55 @@ __device__ __forceinline__ void sample_body(SampleParams p, const int32_t* __res
     z_kept = (n_tie - r_tie) * e_piv + block_sum(tid >= fk ? e_t : 0.f, sm);
   } else {
     // ---- no top-k (then p == 1): the full softmax
-    float bs = -INFINITY;
-    int bi = INT_MAX;
-    for (int i = tid; i < V; i += SP_THREADS) {
-      const float kf = static_cast<float>(bf16_key(x[i]));
-      if (arg_better(kf, i, bs, bi)) bs = kf, bi = i;
-    }
-    block_argmax(bs, bi, sm);
-    m = key_to_float(static_cast<uint32_t>(bs)) / temp;
+    uint32_t bk;
+    int bi;
+    argmax_key(bk, bi);
+    m = key_value(bk) / temp;
     float zs = 0.f;
-    for (int i = tid; i < V; i += SP_THREADS) zs += expf(__uint_as_float(static_cast<uint32_t>(x[i]) << 16) / temp - m);
+    for (int i = tid; i < V; i += SP_THREADS) zs += expf(score(i) / temp - m);
     z_kept = block_sum(zs, sm);
   }
 
   // ---- Gumbel-max over the kept set; the normalised distribution to probs_out
-  const uint64_t off = ROWS ? offsets[row] : p.rng_offset ? *p.rng_offset : 0ull;
-  const uint32_t noise_row = ROWS ? static_cast<uint32_t>(noise_rows[row]) : static_cast<uint32_t>(row);
+  uint64_t off;
+  uint32_t noise_row;
+  if constexpr (PROC) {
+    off = offsets[proc.offset_per_row ? row : 0];
+    noise_row = noise_rows ? static_cast<uint32_t>(noise_rows[row]) : static_cast<uint32_t>(row);
+  } else {
+    off = ROWS ? offsets[row] : p.rng_offset ? *p.rng_offset : 0ull;
+    noise_row = ROWS ? static_cast<uint32_t>(noise_rows[row]) : static_cast<uint32_t>(row);
+  }
   const float inv_z = 1.f / z_kept;
+  // whether id i (key `key`) is in the final set; then s = its scaled score and e = exp(s - m).  Min-p: p = e / z_kept over the
+  // top-k / top-p set, whose largest entry has e = 1, so p < min_p * p_max is e * inv_z < min_p * inv_z (never with min_p 0)
+  auto kept = [&](int i, uint32_t key, float& s, float& e) -> bool {
+    if (k > 0) {
+      const unsigned long long comp = (static_cast<unsigned long long>(key) << 32) | static_cast<uint32_t>(i);
+      if (!(key > pivot ? comp >= fk_comp : (key == pivot && i > idx_cut))) return false;
+    }
+    s = key_value(key) / temp;
+    e = expf(s - m);
+    if constexpr (PROC) return !(e * inv_z < min_p * inv_z);
+    return true;
+  };
+  float inv_zp = inv_z;  // the normaliser of probs_out: min-p renormalises over what it keeps
+  if constexpr (PROC) {
+    if (probs && min_p > 0.f) {
+      float zs = 0.f;
+      for (int i = tid; i < V; i += SP_THREADS) {
+        float s, e;
+        if (kept(i, key_at(i), s, e)) zs += e;
+      }
+      inv_zp = 1.f / block_sum(zs, sm);
+    }
+  }
   float bs = -INFINITY;
   int bi = INT_MAX;
   for (int i = tid; i < V; i += SP_THREADS) {
-    const uint32_t key = bf16_key(x[i]);
-    bool keep = true;
-    if (k > 0) {
-      const unsigned long long comp = (static_cast<unsigned long long>(key) << 32) | static_cast<uint32_t>(i);
-      keep = key > pivot ? comp >= fk_comp : (key == pivot && i > idx_cut);
-    }
-    float pr = 0.f;
-    if (keep) {
-      const float s = key_to_float(key) / temp;
-      pr = expf(s - m) * inv_z;
+    float pr = 0.f, s, e;
+    if (kept(i, key_at(i), s, e)) {
+      pr = e * inv_zp;
       const float g = gumbel(philox_x0(static_cast<uint32_t>(i), noise_row, static_cast<uint32_t>(off),
                                        static_cast<uint32_t>(off >> 32), p.seed_lo, p.seed_hi));
       const float sc = s + g;
@@ -609,6 +712,31 @@ __global__ void __launch_bounds__(SP_THREADS, 1) sample_slots_kernel(const Sampl
   sample_body<true, true>(p, noise_rows, offsets, slots);
 }
 
+__global__ void __launch_bounds__(SP_THREADS, 1) sample_processed_kernel(const SampleParams p, const int32_t* __restrict__ noise_rows,
+                                                                         const uint64_t* __restrict__ offsets,
+                                                                         const SlotSampling slots, const Processing proc) {
+  sample_body<true, true, true>(p, noise_rows, offsets, slots, proc);
+}
+
+// One CTA per row: optionally clear the row's bitmap, then set the bits of its first n ids (ids outside [0, V) are skipped).
+constexpr int PS_THREADS = 256;
+__global__ void __launch_bounds__(PS_THREADS) presence_set_kernel(const int64_t* __restrict__ ids, int64_t ids_stride, int32_t T,
+                                                                  const int32_t* __restrict__ lengths, int32_t clear,
+                                                                  uint32_t* __restrict__ bitmap, int32_t V, int32_t words) {
+  const int r = blockIdx.x;
+  uint32_t* bm = bitmap + static_cast<int64_t>(r) * words;
+  if (clear) {
+    for (int w = threadIdx.x; w < words; w += PS_THREADS) bm[w] = 0u;
+    __syncthreads();
+  }
+  const int n = lengths ? min(max(lengths[r], 0), T) : T;
+  const int64_t* row = ids + static_cast<int64_t>(r) * ids_stride;
+  for (int t = threadIdx.x; t < n; t += PS_THREADS) {
+    const int64_t id = row[t];
+    if (id >= 0 && id < V) atomicOr(bm + (id >> 5), 1u << (id & 31));
+  }
+}
+
 }  // namespace aria
 
 using namespace aria;
@@ -667,6 +795,45 @@ extern "C" int aria_sample_tokens_slots(const void* logits, int64_t logits_strid
   sample_slots_kernel<<<R, SP_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p, noise_rows, offsets,
                                                                                       SlotSampling{temperature, top_k, top_p, seed});
   return check_launch("sample_slots_kernel");
+}
+
+extern "C" int aria_sample_tokens_processed(const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out,
+                                            int32_t R, int32_t V, const float* temperature, const int32_t* top_k, const float* top_p,
+                                            const float* min_p, const uint64_t* seed, const float* repetition_penalty,
+                                            const int32_t* min_new_tokens, const uint32_t* presence, const int32_t* noise_rows,
+                                            const uint64_t* rng_offset, int32_t offset_per_row, const int32_t* n_emitted,
+                                            int32_t emitted_per_row, const int64_t* eos_ids, int32_t n_eos, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(temperature && top_k && top_p && min_p && seed && repetition_penalty && min_new_tokens && presence && rng_offset &&
+                 n_emitted);
+  ARIA_CHECK_ARG(V > 0 && V <= SP_PROC_MAX_VOCAB);
+  ARIA_CHECK_ARG(n_eos >= 0 && n_eos <= SP_MAX_EOS && (n_eos == 0 || eos_ids));
+  SampleParams p{};
+  const int rc = sample_params(p, logits, logits_stride, next_ids, probs_out, R, V, 0.f, 0, 1.f, 0, nullptr);
+  if (rc) return rc;
+  Processing proc{};
+  proc.min_p = min_p;
+  proc.penalty = repetition_penalty;
+  proc.min_new = min_new_tokens;
+  proc.presence = presence;
+  proc.n_emitted = n_emitted;
+  proc.emitted_per_row = emitted_per_row != 0;
+  proc.offset_per_row = offset_per_row != 0;
+  proc.words = (V + 31) / 32;
+  for (int e = 0; e < n_eos; ++e)  // host array; an id outside the vocabulary has no score to mask
+    if (eos_ids[e] >= 0 && eos_ids[e] < V) proc.eos[proc.n_eos++] = static_cast<int>(eos_ids[e]);
+  const size_t smem = sizeof(uint32_t) * proc.words;
+  sample_processed_kernel<<<R, SP_THREADS, smem, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      p, noise_rows, rng_offset, SlotSampling{temperature, top_k, top_p, seed}, proc);
+  return check_launch("sample_processed_kernel");
+}
+
+extern "C" int aria_presence_set(const int64_t* ids, int64_t ids_stride, int32_t R, int32_t T, const int32_t* lengths,
+                                 int32_t clear, uint32_t* bitmap, int32_t V, aria_stream_t stream_) {
+  ARIA_CHECK_ARG(ids && bitmap);
+  ARIA_CHECK_ARG(R > 0 && R <= SP_MAX_ROWS && T > 0 && ids_stride >= 0 && V > 0 && V <= SP_PROC_MAX_VOCAB);
+  presence_set_kernel<<<R, PS_THREADS, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(ids, ids_stride, T, lengths, clear != 0,
+                                                                                     bitmap, V, (V + 31) / 32);
+  return check_launch("presence_set_kernel");
 }
 
 extern "C" int aria_token_logprobs(const void* logits, int64_t logits_stride, const int64_t* tokens, int32_t R, int32_t V,

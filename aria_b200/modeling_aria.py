@@ -345,7 +345,8 @@ class AriaForConditionalGeneration(nn.Module):
                  pad_token_id=None, seed: int = 0, poll_every: int = 8, kv_cache_dtype: str = "bf16",
                  num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None,
                  prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None,
-                 output_logprobs: Optional[int] = None):
+                 output_logprobs: Optional[int] = None, repetition_penalty: float = 1.0, min_p: float = 0.0,
+                 min_new_tokens: int = 0):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -382,6 +383,14 @@ class AriaForConditionalGeneration(nn.Module):
         (ops.token_logprobs, run inside the captured step).  Positions after a row's EOS hold logprob 0, ids -1 and logprobs
         -inf, so a row's logprobs sum to the log-likelihood of its sequence up to and including EOS.  GPU only; not combined
         with prompt_lookup_num_tokens.
+        repetition_penalty (> 0, 1 = off), min_new_tokens (>= 0) and min_p (in [0, 1], 0 = off): Hugging Face's logits
+        processors, in GenerationMixin's order, applied inside the sampling kernel of the captured step
+        (ops.sample_tokens_processed) to an fp32 copy of the logits.  Every id anywhere in the row so far (left padding, image
+        tokens, prompt, generated tokens) gets x < 0 ? x * penalty : x / penalty; while a row has emitted fewer than
+        min_new_tokens tokens its EOS ids get -inf; greedy takes the argmax of those scores, and sampling runs temperature, top-k
+        and top-p on them, then min-p (a survivor with p < min_p * max p is removed; min_p also works with top_k = 0).  Each row
+        keeps a bitmap of the ids it has seen (ops.presence_set), V / 8 bytes.  Logprobs stay those of the raw distribution.
+        GPU only; not combined with prompt_lookup_num_tokens.  Without them, the captured step is the one above.
         Returns [B * n, T + generated] int64 on the model's device (prompt ids first); with output_logprobs a GenerateOutput
         (sequences: that tensor; logprobs [B * n, L] fp32, top_ids [B * n, L, k] int64, top_logprobs [B * n, L, k] fp32, L the
         generated length)."""
@@ -390,6 +399,7 @@ class AriaForConditionalGeneration(nn.Module):
                                                    num_return_sequences, shared_prefix_len)
         n_seq = num_return_sequences
         dev = self.device
+        processors = self._check_logits_processors(repetition_penalty, min_p, min_new_tokens, prompt_lookup_num_tokens, dev)
         self._check_output_logprobs(output_logprobs, prompt_lookup_num_tokens, dev)
         if prompt_lookup_num_tokens is not None:
             K, M = self._check_prompt_lookup(B, prompt_lookup_num_tokens, max_matching_ngram_size, n_seq, shared_prefix_len,
@@ -404,7 +414,7 @@ class AriaForConditionalGeneration(nn.Module):
                 raise NotImplementedError("aria_b200: shared_prefix_len runs on the GPU only")
             sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
             return self._generate_shared_prefix(input_ids, ids_host, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos,
-                                                pad, poll_every, n_seq, shared_prefix_len, output_logprobs)
+                                                pad, poll_every, n_seq, shared_prefix_len, output_logprobs, processors)
         if dev.type != "cuda":
             if do_sample or eos:
                 raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
@@ -420,10 +430,10 @@ class AriaForConditionalGeneration(nn.Module):
         T_max = -(-(T if n_seq > 1 else T + max_new_tokens) // 256) * 256
         key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, None, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key or g.n_logprobs != output_logprobs:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
             g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype, n_seq,
-                                                   logprobs=output_logprobs)
+                                                   logprobs=output_logprobs, processors=processors)
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
                                                     attention_mask=mask, num_logits_to_keep=1)
@@ -431,6 +441,8 @@ class AriaForConditionalGeneration(nn.Module):
         inputs["past_key_values"] = g.cache
         out = self.forward(**inputs)
         g.start(T, mask)
+        if processors is not None:
+            g.start_presence(input_ids.to(dev) if n_seq == 1 else input_ids.to(dev).repeat_interleave(n_seq, 0))
         first = out.logits[:, -1]
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         n, L = g.run(max_new_tokens, poll_every)
@@ -440,7 +452,7 @@ class AriaForConditionalGeneration(nn.Module):
         return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
 
     def _generate_shared_prefix(self, input_ids, ids, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos, pad,
-                                poll_every, n_seq, P, output_logprobs=None):
+                                poll_every, n_seq, P, output_logprobs=None, processors=None):
         """generate(shared_prefix_len=P) on checked arguments (ids: the host copy of input_ids, lens: each row's real length,
         from _check_shared_prefix): ViT + prefix prefill (forward()) into a SharedPrefixCache of one prompt row, the packed
         suffix prefill (AriaMoELMModel.prefill_suffixes), the first token from each suffix's last position, then the graphed
@@ -459,10 +471,10 @@ class AriaForConditionalGeneration(nn.Module):
         N_max = -(-(max(S) + max_new_tokens) // 256) * 256
         key = (1, T_max, max_new_tokens, sampling, eos, pad, dev, B * n_seq, N_max, "bf16")
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key or g.n_logprobs != output_logprobs:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors:
             self._decode_graph = g = None
             g = self._decode_graph = GraphedDecode(self, 1, T_max, max_new_tokens, sampling, eos, pad, "bf16", B * n_seq,
-                                                   N_max=N_max, logprobs=output_logprobs)
+                                                   N_max=N_max, logprobs=output_logprobs, processors=processors)
         g.cache.seq_len = 0
         self.forward(prefix, pixel_values, pixel_mask, past_key_values=g.cache, num_logits_to_keep=1)
         cu_dev = cu.to(dev, non_blocking=True)
@@ -472,6 +484,8 @@ class AriaForConditionalGeneration(nn.Module):
         h, _ = lm.model.norm(x[0, last].contiguous(), residual=pending[0, last].contiguous())
         first = lm.lm_head(h)                       # [B, V]
         g.start_suffixes(P, S, n_seq)
+        if processors is not None:      # each row's own left-padded ids, as the repeated-image batch has them
+            g.start_presence(input_ids.to(dev).repeat_interleave(n_seq, 0))
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         _, L = g.run(max_new_tokens, poll_every)
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
@@ -575,6 +589,28 @@ class AriaForConditionalGeneration(nn.Module):
         return B, T, eos, pad_token_id
 
     @staticmethod
+    def _check_logits_processors(repetition_penalty, min_p, min_new_tokens, prompt_lookup_num_tokens, device):
+        """generate()'s and Engine.add_request()'s checks of the logits processors, on the host after _check_generate_args':
+        repetition_penalty, min_p, min_new_tokens (ValueError), then, when one of them is on, prompt lookup and a CPU device
+        (NotImplementedError).  -> None when every one is off, else (penalty, min_p, min_new_tokens)."""
+        import math
+        def real(v):
+            return isinstance(v, (int, float)) and not isinstance(v, bool)
+        if not (real(repetition_penalty) and math.isfinite(repetition_penalty) and repetition_penalty > 0):
+            raise ValueError(f"repetition_penalty must be a strictly positive finite float, got {repetition_penalty!r}")
+        if not (real(min_p) and 0 <= min_p <= 1):
+            raise ValueError(f"min_p must be a float in [0, 1], got {min_p!r}")
+        if not isinstance(min_new_tokens, int) or isinstance(min_new_tokens, bool) or min_new_tokens < 0:
+            raise ValueError(f"min_new_tokens must be a non-negative int, got {min_new_tokens!r}")
+        if repetition_penalty == 1 and min_p == 0 and min_new_tokens == 0:
+            return None
+        if prompt_lookup_num_tokens is not None:
+            raise NotImplementedError("repetition_penalty, min_p and min_new_tokens with prompt_lookup_num_tokens are not supported")
+        if torch.device(device).type != "cuda":
+            raise NotImplementedError("aria_b200: repetition_penalty, min_p and min_new_tokens run on the GPU only")
+        return float(repetition_penalty), float(min_p), int(min_new_tokens)
+
+    @staticmethod
     def _check_output_logprobs(k, prompt_lookup_num_tokens, device):
         """generate(output_logprobs=k)'s checks after _check_generate_args', on the host: k (ValueError), then prompt lookup and
         a CPU device (NotImplementedError)."""
@@ -671,10 +707,15 @@ class GraphedDecode:
     own prompt tokens and then its generated ones, for any group size.
     logprobs k (generate(output_logprobs=k)): the step also runs ops.token_logprobs on the sampled tokens between the sampler and
     the advance, into column `step` of lp [B, max_new_tokens], top_ids and top_lp [B, max_new_tokens, k]; rows finished before
-    the step get the filler.  None: the step is exactly the one without logprobs."""
+    the step get the filler.  None: the step is exactly the one without logprobs.
+    processors (penalty, min_p, min_new_tokens) (generate(repetition_penalty=..., min_p=..., min_new_tokens=...)): the sampler is
+    ops.sample_tokens_processed, which reads each row's presence bitmap [B, V / 32] (start_presence) and counts its emitted
+    tokens by `step`, and the advance is followed by ops.presence_set of the tokens it wrote to `ids`.  generate() rebuilds the
+    graph when they change, as it does for logprobs.  None: the step is exactly the one without them."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
-                 kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None, logprobs: Optional[int] = None):
+                 kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None, logprobs: Optional[int] = None,
+                 processors: Optional[tuple] = None):
         from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
         dev = model.device
         lm = model.language_model
@@ -708,6 +749,19 @@ class GraphedDecode:
             self.lp = torch.zeros(B, max_new_tokens, dtype=torch.float32, device=dev)
             self.top_ids = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.int32, device=dev)
             self.top_lp = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.float32, device=dev)
+        self.processors = processors
+        if processors is not None:
+            t, k, p, seed = sampling
+            penalty, min_p, min_new = processors
+            f32, i32 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int32, device=dev)
+            # per-row arrays of the processed sampler, in its argument order: temperature, top_k, top_p, min_p, seed, penalty,
+            # min_new_tokens
+            self.proc_rows = (torch.full((B,), t, **f32), torch.full((B,), k, **i32), torch.full((B,), p, **f32),
+                              torch.full((B,), min_p, **f32),
+                              torch.full((B,), seed - 2 ** 64 if seed >= 2 ** 63 else seed, dtype=torch.int64, device=dev),
+                              torch.full((B,), penalty, **f32), torch.full((B,), min_new, **i32))
+            self.V = c.vocab_size
+            self.presence = torch.zeros(B, ops.presence_words(self.V), **i32)
         self.done_host = torch.full((1,), -1, dtype=torch.int32).pin_memory()
         self.event = torch.cuda.Event()
         self.dev = dev
@@ -731,14 +785,24 @@ class GraphedDecode:
     def sample_and_advance(self, logits: torch.Tensor):
         """Sample from logits [B, V] into next_ids, then advance the state (also the eager first token after the prefill)."""
         t, k, p, seed = self.sampling
-        ops.sample_tokens(logits, t, k, p, seed, self.rng_offset, out=self.next_ids)
+        if self.processors is None:
+            ops.sample_tokens(logits, t, k, p, seed, self.rng_offset, out=self.next_ids)
+        else:
+            ops.sample_tokens_processed(logits, *self.proc_rows, self.presence, self.rng_offset, self.step, self.eos,
+                                        out=self.next_ids)
         if self.n_logprobs is not None:
             ops.token_logprobs(logits, self.next_ids, self.n_logprobs, col=self.step, finished=self.finished,
                                out=(self.lp, self.top_ids, self.top_lp))
         st = self.state
         ops.decode_advance(self.next_ids, self.ids, self.out_tokens, self.step, st.rope_pos, st.write_pos, st.kv_len,
                            self.rng_offset, self.finished, self.done_step, self.eos, self.pad)
+        if self.processors is not None:
+            ops.presence_set(self.ids, self.presence, self.V)
         self.done_host.copy_(self.done_step, non_blocking=True)
+
+    def start_presence(self, ids: torch.Tensor):
+        """Every row's presence bitmap from its ids [B, T] on the device (the prompt as the row has it, padding included)."""
+        ops.presence_set(ids, self.presence, self.V, clear=True)
 
     def result(self, sequences: torch.Tensor, L: int):
         """generate()'s return value: sequences alone, or with logprobs a GenerateOutput of the first L columns."""

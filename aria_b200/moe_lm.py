@@ -588,9 +588,11 @@ class SlotDecodeState(DecodeState):
     step's input ids_in and sampled next_ids.  A decode step over the first n slots reads rows(n); the other slots are idle.
     Log-probabilities (serving.Engine's logprobs): lp_n, the slot's top-n (-1: none), and rings of lp_ring entries that the step
     writes at n_out mod lp_ring: lp_ring_lp [max_batch, lp_ring] fp32, lp_ring_ids [max_batch, lp_ring, 20] int32 and
-    lp_ring_top [max_batch, lp_ring, 20] fp32."""
+    lp_ring_top [max_batch, lp_ring, 20] fp32.
+    Logits processors (serving.Engine's repetition_penalty, min_p, min_new_tokens): the slot's rep_penalty (1: off), min_p (0:
+    off) and min_new, and presence [max_batch, ceil(vocab / 32)] int32, the bitmap of the ids its request has seen."""
 
-    def __init__(self, max_batch, H, max_out, device, lp_ring: int = 1):
+    def __init__(self, max_batch, H, max_out, device, lp_ring: int = 1, vocab: int = 1):
         super().__init__(max_batch, H, 0, device)
         self.key_mask = None
         i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
@@ -610,11 +612,15 @@ class SlotDecodeState(DecodeState):
         self.lp_ring_lp = torch.zeros(max_batch, lp_ring, dtype=torch.float32, device=device)
         self.lp_ring_ids = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, **i32)
         self.lp_ring_top = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, dtype=torch.float32, device=device)
+        self.rep_penalty = torch.ones(max_batch, dtype=torch.float32, device=device)
+        self.min_p = torch.zeros(max_batch, dtype=torch.float32, device=device)
+        self.min_new = torch.zeros(max_batch, **i32)
+        self.presence = torch.zeros(max_batch, ops.presence_words(vocab), **i32)
 
     # the per-slot arrays, in the order a slot's row is copied when slots are compacted
     SLOT_FIELDS = ("rope_pos", "write_pos", "kv_len", "temperature", "top_k", "top_p", "seed", "noise_row", "rng_offset",
                    "max_new", "n_out", "finished", "ids_in", "next_ids", "out_tokens", "lp_n", "lp_ring_lp", "lp_ring_ids",
-                   "lp_ring_top")
+                   "lp_ring_top", "rep_penalty", "min_p", "min_new", "presence")
 
     def rows(self, n):
         """A DecodeState view of the first n slots (what decode_step and the sampler of a step over n slots read)."""

@@ -1682,6 +1682,81 @@ def sample_tokens_slots(logits: torch.Tensor, temperature: torch.Tensor, top_k: 
     return out
 
 
+PROCESSED_MAX_VOCAB = 1 << 18   # the presence bitmap of a row is staged in the sampler's shared memory
+
+
+def presence_words(V: int) -> int:
+    """int32 words of one row's token-presence bitmap over a vocabulary of V ids."""
+    return (V + 31) // 32
+
+
+def sample_tokens_processed(logits: torch.Tensor, temperature: torch.Tensor, top_k: torch.Tensor, top_p: torch.Tensor,
+                            min_p: torch.Tensor, seed: torch.Tensor, repetition_penalty: torch.Tensor,
+                            min_new_tokens: torch.Tensor, presence: torch.Tensor, rng_offset: torch.Tensor,
+                            n_emitted: torch.Tensor, eos_token_ids: Sequence[int] = (), noise_rows: Optional[torch.Tensor] = None,
+                            out: Optional[torch.Tensor] = None, probs_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """sample_tokens_slots behind Hugging Face's repetition penalty, min_new_tokens and min-p, every parameter per row, CUDA
+    arrays [R]: temperature fp32 (0 = greedy), top_k int32, top_p fp32, min_p fp32 (0 = off), seed int64 (read as uint64),
+    repetition_penalty fp32 (1 = off), min_new_tokens int32.  presence: int32 [R, presence_words(V)], the ids each row has seen
+    (presence_set).  rng_offset int64 and n_emitted int32 (tokens the row has emitted): [R], or [1] for every row.  noise_rows:
+    int32 [R], or None for row r.  eos_token_ids: at most 8 ids, masked while a row has emitted fewer than its min_new_tokens.
+    out: int64 [R] (allocated when None); probs_out: fp32 [R, V], the final distribution.  The caller checks the parameters as
+    generate() does.  See aria_sample_tokens_processed."""
+    if not (logits.is_cuda and logits.dtype == bf16 and logits.dim() == 2 and logits.stride(-1) == 1):
+        raise RuntimeError("sample_tokens_processed: logits must be CUDA bf16 [R, V] with a contiguous last dim")
+    R, V = logits.shape
+    if out is None:
+        out = torch.empty((R,), dtype=torch.int64, device=logits.device)
+    args = ((out, torch.int64), (temperature, torch.float32), (top_k, torch.int32), (top_p, torch.float32), (min_p, torch.float32),
+            (seed, torch.int64), (repetition_penalty, torch.float32), (min_new_tokens, torch.int32))
+    if noise_rows is not None:
+        args += ((noise_rows, torch.int32),)
+    for t, dt in args:
+        _chk(t, dt, align=4)
+        if t.shape != (R,):
+            raise ValueError(f"sample_tokens_processed: out and every per-row array must be [{R}], got {tuple(t.shape)}")
+    for t, dt, name in ((rng_offset, torch.int64, "rng_offset"), (n_emitted, torch.int32, "n_emitted")):
+        _chk(t, dt, align=4)
+        if t.shape not in ((1,), (R,)):
+            raise ValueError(f"sample_tokens_processed: {name} must be [1] or [{R}], got {tuple(t.shape)}")
+    _chk(presence, torch.int32, align=4)
+    if presence.shape != (R, presence_words(V)):
+        raise ValueError(f"sample_tokens_processed: presence must be [{R}, {presence_words(V)}], got {tuple(presence.shape)}")
+    if probs_out is not None:
+        _chk(probs_out, torch.float32, align=4)
+        if probs_out.shape != (R, V):
+            raise ValueError(f"sample_tokens_processed: probs_out must be [{R}, {V}], got {tuple(probs_out.shape)}")
+    eos, n_eos = _eos_array(eos_token_ids)
+    with torch.cuda.device(logits.device):
+        L.check(L.load().aria_sample_tokens_processed(
+            _p(logits), logits.stride(0), _p(out), _p(probs_out), R, V, _p(temperature), _p(top_k), _p(top_p), _p(min_p), _p(seed),
+            _p(repetition_penalty), _p(min_new_tokens), _p(presence), _p(noise_rows), _p(rng_offset),
+            int(rng_offset.numel() == R and R > 1), _p(n_emitted), int(n_emitted.numel() == R and R > 1),
+            C.cast(eos, C.c_void_p), n_eos, _stream(logits)), "sample_tokens_processed")
+    return out
+
+
+def presence_set(ids: torch.Tensor, presence: torch.Tensor, V: int, lengths: Optional[torch.Tensor] = None,
+                 clear: bool = False) -> torch.Tensor:
+    """Set bit id of presence row r (int32 [R, presence_words(V)]) for every id of ids row r (CUDA int64 [R, T], contiguous
+    last dim, any row stride), only its first lengths[r] (CUDA int32 [R]) when given; ids outside [0, V) are skipped.  clear:
+    zero each row first.  -> presence.  See aria_presence_set."""
+    if not (ids.is_cuda and ids.dtype == torch.int64 and ids.dim() == 2 and ids.stride(-1) == 1):
+        raise RuntimeError("presence_set: ids must be CUDA int64 [R, T] with a contiguous last dim")
+    R, T = ids.shape
+    _chk(presence, torch.int32, align=4)
+    if presence.shape != (R, presence_words(V)):
+        raise ValueError(f"presence_set: presence must be [{R}, {presence_words(V)}], got {tuple(presence.shape)}")
+    if lengths is not None:
+        _chk(lengths, torch.int32, align=4)
+        if lengths.shape != (R,):
+            raise ValueError(f"presence_set: lengths must be [{R}], got {tuple(lengths.shape)}")
+    with torch.cuda.device(ids.device):
+        L.check(L.load().aria_presence_set(_p(ids), ids.stride(0), R, T, _p(lengths), int(bool(clear)), _p(presence), int(V),
+                                           _stream(ids)), "presence_set")
+    return presence
+
+
 MAX_LOGPROBS = 20
 
 

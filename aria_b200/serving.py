@@ -273,6 +273,7 @@ class Request:
     prompt_logprobs: Optional[int] = None               # top-n of the prompt tokens' logprobs (None: none; no prefix-cache hit)
     lp_drained: int = 0                                 # generated tokens whose logprobs the host has copied out of the ring
     lp_parts: list = field(default_factory=list)        # host (logprob [m], ids [m, k], logprobs [m, k]) pieces, in order
+    processors: Optional[tuple] = None                  # (repetition_penalty, min_p, min_new_tokens), None when all are off
     plp_parts: list = field(default_factory=list)       # device pieces of the prompt logprobs, in order
 
     @property
@@ -409,7 +410,9 @@ class Engine:
     output row per slot as long as the pool, since a request may spend the whole pool on its budget: 4 x max_batch x
     256 ceil(max_kv_tokens / 256) bytes (32 MiB at the defaults, 4 GiB at 1024 slots and a 2^20-token pool).  An fp8 prefill
     whose segments have a cached prefix also holds, while it runs, a bf16 scratch copy of the launch's distinct prefix pages:
-    2 x heads x 256 x 128 x 2 bytes per page (2.6 MB at 20 heads), shared by the layers.
+    2 x heads x 256 x 128 x 2 bytes per page (2.6 MB at 20 heads), shared by the layers.  Logits processors: a token-presence
+    bitmap of ceil(V / 32) int32 words per slot, 12.5 KB at V = 100,352 (0.8 MB at 64 slots, 12.3 MiB at 1024), and 12 bytes
+    of parameters.
     `stats`: graphs captured, decode steps replayed, slot-steps of active requests (mean occupancy = active_slot_steps /
     (steps * max_batch); a partly prefilled request is not counted), host seconds spent waiting in polls; prefix caching: prompt tokens admitted, those found in cached
     pages (prefix_hit_tokens), pixel rows the ViT ran on and skipped, cached pages evicted; admission: packed prefills run
@@ -459,7 +462,7 @@ class Engine:
         self.cache = PagedKVCache(c.num_hidden_layers, n_pages, c.num_attention_heads, c.head_dim, max_batch, self.max_pages, dev,
                                   kv_cache_dtype)
         self.lp_ring = poll_every + 1
-        self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev, self.lp_ring)
+        self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev, self.lp_ring, c.vocab_size)
         self._idle(0, max_batch)
         self.rope = lm.model.rope_tables(self.max_pages * PAGE, dev)   # held here: the graphs read these tables
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
@@ -481,13 +484,16 @@ class Engine:
     # ------------------------------------------------------------------------------------------------ public API
     def add_request(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, do_sample: bool = False,
                     temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, logprobs: Optional[int] = None,
-                    prompt_logprobs: Optional[int] = None) -> int:
+                    prompt_logprobs: Optional[int] = None, repetition_penalty: float = 1.0, min_p: float = 0.0,
+                    min_new_tokens: int = 0) -> int:
         """Queue one request (input_ids [T] or [1, T]; pixel inputs as generate()'s for that one row) -> its id.  Arguments are
         checked as generate() checks them, and a request that needs more pages than the pool has is refused, here, before
         any device work.  The prompt's page keys (page_keys) are computed here, on the host.
         logprobs / prompt_logprobs (None, or an int k in [0, 20]): the logprob of each generated / prompt token under the model's
         raw distribution and its k most likely tokens, in self.logprobs[rid] once it finishes (Logprobs); the generated ones are
-        generate(output_logprobs=k)'s bit for bit.  A request with prompt_logprobs takes no prefix-cache hit."""
+        generate(output_logprobs=k)'s bit for bit.  A request with prompt_logprobs takes no prefix-cache hit.
+        repetition_penalty / min_p / min_new_tokens: generate()'s logits processors; the request's tokens are batch-1 generate()'s
+        with the same arguments bit for bit.  A decode step runs the processed sampler only when some active slot asks for one."""
         if not isinstance(input_ids, torch.Tensor) or input_ids.dim() not in (1, 2):
             raise ValueError("input_ids must be a tensor [T] or [1, T]")
         ids = input_ids.reshape(1, -1) if input_ids.dim() == 1 else input_ids
@@ -495,11 +501,13 @@ class Engine:
             raise ValueError(f"add_request takes one prompt, got input_ids {tuple(input_ids.shape)}")
         self.model._check_generate_args(ids, max_new_tokens, None, do_sample, temperature, top_k, top_p, list(self.eos),
                                         self.pad, seed, self.poll_every)
+        from .modeling_aria import AriaForConditionalGeneration
+        processors = AriaForConditionalGeneration._check_logits_processors(repetition_penalty, min_p, min_new_tokens, None, "cuda")
         _check_logprobs_arg("logprobs", logprobs)
         _check_logprobs_arg("prompt_logprobs", prompt_logprobs)
         sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
         req = Request(self._next_rid, ids[0].to("cpu", torch.int64), max_new_tokens, sampling, pixel_values, pixel_mask,
-                      logprobs=logprobs, prompt_logprobs=prompt_logprobs)
+                      logprobs=logprobs, prompt_logprobs=prompt_logprobs, processors=processors)
         image_token = None if pixel_values is None else self.model.config.image_token_index
         req.keys = page_keys(req.input_ids, pixel_values, pixel_mask, image_token)
         self.sched.submit(req)
@@ -528,7 +536,10 @@ class Engine:
         decoding = self.sched.n_active - (self.sched.partial is not None)    # a partly prefilled request's slot is idle
         if decoding:
             n, width = _pow2_at_least(self.sched.n_active, self.max_batch), _pow2_at_least(self.sched.width(), self.max_pages)
-            g = self._graph(n, width, True) if self._any_logprobs() else self._graph(n, width)
+            if self._any_processors():
+                g = self._graph(n, width, self._any_logprobs(), True)
+            else:
+                g = self._graph(n, width, True) if self._any_logprobs() else self._graph(n, width)
             for _ in range(self.poll_every):
                 g.replay()
             self.stats["steps"] += self.poll_every
@@ -584,36 +595,51 @@ class Engine:
         st.n_out[lo:hi] = 0
         st.lp_n[lo:hi] = -1
         st.temperature[lo:hi] = 0.0
+        st.rep_penalty[lo:hi] = 1.0
+        st.min_p[lo:hi] = 0.0
+        st.min_new[lo:hi] = 0
         self.cache.block_table[lo:hi] = -1
         self.cache.block_table[lo:hi, 0] = 0
 
     def _any_logprobs(self) -> bool:
         return any(r.logprobs is not None for r in self.sched.slots)
 
-    def _step(self, n: int, lp: bool) -> None:
+    def _any_processors(self) -> bool:
+        return any(r.processors is not None for r in self.sched.slots)
+
+    def _step(self, n: int, lp: bool, proc: bool = False) -> None:
         lm = self.model.language_model
         st = self.state.rows(n)
         emb = ops.embedding(st.ids_in, lm.get_input_embeddings().weight)
         logits = lm.decode_step(emb, self.cache, st, self.rope)
-        self._sample_and_advance(st, logits[:, -1], lp)
+        self._sample_and_advance(st, logits[:, -1], lp, proc)
         self._fin_host.copy_(self.state.finished, non_blocking=True)
         self._nout_host.copy_(self.state.n_out, non_blocking=True)
 
-    def _sample_and_advance(self, st, logits, lp: bool) -> None:
-        """Sample, then with lp the logprobs of the slots with lp_n >= 0 into ring entry n_out mod lp_ring (finished slots
-        untouched), then advance."""
-        ops.sample_tokens_slots(logits, st.temperature, st.top_k, st.top_p, st.seed, st.noise_row, st.rng_offset, out=st.next_ids)
+    def _sample_and_advance(self, st, logits, lp: bool, proc: bool = False) -> None:
+        """Sample (with proc, through each slot's logits processors), then with lp the logprobs of the slots with lp_n >= 0 into
+        ring entry n_out mod lp_ring (finished slots untouched), then advance; with proc, each slot's new input id then joins
+        its presence bitmap."""
+        if proc:
+            ops.sample_tokens_processed(logits, st.temperature, st.top_k, st.top_p, st.min_p, st.seed, st.rep_penalty, st.min_new,
+                                        st.presence, st.rng_offset, st.n_out, self.eos, noise_rows=st.noise_row, out=st.next_ids)
+        else:
+            ops.sample_tokens_slots(logits, st.temperature, st.top_k, st.top_p, st.seed, st.noise_row, st.rng_offset,
+                                    out=st.next_ids)
         if lp:
             ops.token_logprobs(logits, st.next_ids, MAX_LOGPROBS, n_row=st.lp_n, col=st.n_out, ring=self.lp_ring,
                                finished=st.finished, finished_fill=False, out=(st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top))
         ops.decode_advance_slots(st.next_ids, st.ids_in, st.out_tokens, st.n_out, st.max_new, st.rope_pos, st.write_pos,
                                  st.kv_len, st.rng_offset, st.finished, self.eos, self.pad)
+        if proc:
+            ops.presence_set(st.ids_in, st.presence, self.model.language_model.config.vocab_size)
 
-    def _graph(self, n: int, width: int, lp: bool = False) -> torch.cuda.CUDAGraph:
-        """The captured step over slots [0, n) and table columns [0, width), with the logprob kernel when lp, captured on first
-        use; its key is (n, width), and (n, width, True) with the logprob kernel.  The warm-up run before the capture computes
-        the very step the next replay computes; the slot rows it advanced are put back afterwards."""
-        key = (n, width, True) if lp else (n, width)
+    def _graph(self, n: int, width: int, lp: bool = False, proc: bool = False) -> torch.cuda.CUDAGraph:
+        """The captured step over slots [0, n) and table columns [0, width), with the logprob kernel when lp and the processed
+        sampler when proc, captured on first use; its key is (n, width), (n, width, True) with the logprob kernel, and
+        (n, width, lp, "processors") with the processed sampler.  The warm-up run before the capture computes the very step the
+        next replay computes; the slot rows it advanced are put back afterwards."""
+        key = (n, width, lp, "processors") if proc else (n, width, True) if lp else (n, width)
         g = self._graphs.get(key)
         if g is not None:
             return g
@@ -623,13 +649,13 @@ class Engine:
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):
-            self._step(n, lp)
+            self._step(n, lp, proc)
         cur.wait_stream(side)
         for f, t in keep.items():
             getattr(self.state, f).copy_(t)
         g = torch.cuda.CUDAGraph()
         with ops.graph_capture(g, pool=self._pool):
-            self._step(n, lp)
+            self._step(n, lp, proc)
         self._graphs[key] = g
         self.stats["graphs_captured"] += 1
         return g
@@ -797,7 +823,14 @@ class Engine:
         st.n_out[s] = 0
         st.finished[s] = 0
         st.lp_n[s] = -1 if req.logprobs is None else req.logprobs
-        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None)
+        pen, min_p, min_new = (1.0, 0.0, 0) if req.processors is None else req.processors
+        st.rep_penalty[s] = pen
+        st.min_p[s] = min_p
+        st.min_new[s] = min_new
+        if req.processors is not None:      # the prompt's ids, before the first token is sampled
+            ops.presence_set(req.input_ids.to(self.dev)[None], st.presence[s:s + 1], self.model.language_model.config.vocab_size,
+                             clear=True)
+        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None, req.processors is not None)
 
     def _drop(self, s: int) -> None:
         """Retire slot s without a result: the last active slot moves into s and the slot it left becomes idle."""

@@ -635,6 +635,33 @@ int aria_kv_pages_load_fp8(const void* k_pool, const void* v_pool, const float* 
 int aria_sample_tokens_slots(const void* logits, int64_t logits_stride, int64_t* next_ids, int32_t R, int32_t V,
                              const float* temperature, const int32_t* top_k, const float* top_p, const uint64_t* seed,
                              const int32_t* noise_rows, const uint64_t* offsets, aria_stream_t stream);
+/* aria_sample_tokens_slots behind Hugging Face's logits processors (transformers' GenerationMixin order), every parameter per
+ * row from DEVICE arrays [R]: temperature, top_k, top_p and seed as there, min_p (fp32, 0 = off), repetition_penalty (fp32,
+ * 1 = off) and min_new_tokens (int32).  Row r's scores are the fp32 values of its bf16 logits where
+ *   - an id set in its presence bitmap (DEVICE uint32 [R, ceil(V / 32)], bit i of word i / 32; aria_presence_set) becomes
+ *     x < 0 ? x * penalty : x / penalty, IEEE-rounded (RepetitionPenaltyLogitsProcessor);
+ *   - while the row has emitted fewer than min_new_tokens tokens, every EOS id (HOST array of n_eos <= 8 ids, copied at the
+ *     call) becomes -inf (MinNewTokensLengthLogitsProcessor);
+ * then greedy takes their argmax (ties to the lowest id), and sampling runs temperature -> top-k -> top-p as aria_sample_tokens
+ * does, then min-p: a survivor with p < min_p * max p, p the softmax over the survivors, is removed (MinPLogitsWarper; the
+ * largest always stays).  min_p also applies with top_k = 0.  probs_out [R, V] or NULL: the final distribution, renormalised
+ * over what min-p keeps.  Row r draws the noise of row noise_rows[r] (DEVICE int32 [R], or NULL for row r) at offset
+ * rng_offset[r] (offset_per_row) or rng_offset[0] (DEVICE uint64); n_emitted (DEVICE int32) is likewise per row or one value.
+ * A row whose processors are off (penalty 1, min_p 0, min_new_tokens 0) gets aria_sample_tokens_slots' token and
+ * aria_sample_tokens' probs_out bit for bit.  Out-of-range entries are brought into range as there (a non-positive or
+ * non-finite penalty is 1, a min_p outside (0, 1] is 0).  R <= 2^20, V <= 2^18 (the bitmap is staged in shared memory). */
+int aria_sample_tokens_processed(const void* logits, int64_t logits_stride, int64_t* next_ids, float* probs_out, int32_t R,
+                                 int32_t V, const float* temperature, const int32_t* top_k, const float* top_p, const float* min_p,
+                                 const uint64_t* seed, const float* repetition_penalty, const int32_t* min_new_tokens,
+                                 const uint32_t* presence, const int32_t* noise_rows, const uint64_t* rng_offset,
+                                 int32_t offset_per_row, const int32_t* n_emitted, int32_t emitted_per_row, const int64_t* eos_ids,
+                                 int32_t n_eos, aria_stream_t stream);
+/* Token-presence bitmaps for aria_sample_tokens_processed: for each row r < R, bitmap row r (uint32 [R, ceil(V / 32)]) is
+ * cleared first when `clear`, then bit id is set for each of the row's first n ids, ids + r * ids_stride (DEVICE int64),
+ * n = lengths[r] clamped to [0, T] (DEVICE int32 [R]) or T when lengths is NULL.  Ids outside [0, V) are skipped.
+ * R <= 2^20, V <= 2^18, one CTA per row. */
+int aria_presence_set(const int64_t* ids, int64_t ids_stride, int32_t R, int32_t T, const int32_t* lengths, int32_t clear,
+                      uint32_t* bitmap, int32_t V, aria_stream_t stream);
 /* Token log-probabilities of bf16 logits [R, V] (row r at logits + r * logits_stride, contiguous within a row), one CTA per row,
  * under the row's raw distribution: lp(t) = (x_t - m) - log(sum_i exp(x_i - m)), m = max_i x_i, in fp32 summed in a fixed order.
  * Row r writes output entry o = r * cols + c: logprobs[o] = lp(tokens[r]) (NaN for a token outside [0, V)), and its n largest
