@@ -143,6 +143,8 @@ SIGNATURES = {
     "aria_sample_tokens_processed": (i32, [vp, i64, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, vp,
                                            i32, vp]),
     "aria_presence_set": (i32, [vp, i64, i32, i32, vp, i32, vp, i32, vp]),
+    "aria_stop_check": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, vp]),
+    "aria_stop_check_slots": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp, i64, i32, vp]),
 }
 
 _lib = None

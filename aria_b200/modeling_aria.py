@@ -14,7 +14,7 @@ from typing import NamedTuple, Optional
 import torch
 import torch.nn as nn
 
-from . import ops
+from . import ops, stopping
 from .ops import MAX_LOGPROBS
 from .moe_lm import KV_CACHE_DTYPES, AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16
 from .projector import AriaProjector
@@ -346,7 +346,7 @@ class AriaForConditionalGeneration(nn.Module):
                  num_return_sequences: int = 1, shared_prefix_len: Optional[int] = None,
                  prompt_lookup_num_tokens: Optional[int] = None, max_matching_ngram_size: Optional[int] = None,
                  output_logprobs: Optional[int] = None, repetition_penalty: float = 1.0, min_p: float = 0.0,
-                 min_new_tokens: int = 0):
+                 min_new_tokens: int = 0, stop_strings=None, tokenizer=None):
         """Greedy or sampled generation (the reference goes through HF GenerationMixin, modeling_aria.py:125,337-365).
 
         Eager prefill with the image, the first token sampled from its logits, then one CUDA-graph replay per token of a
@@ -391,6 +391,14 @@ class AriaForConditionalGeneration(nn.Module):
         and top-p on them, then min-p (a survivor with p < min_p * max p is removed; min_p also works with top_k = 0).  Each row
         keeps a bitmap of the ids it has seen (ops.presence_set), V / 8 bytes.  Logprobs stay those of the raw distribution.
         GPU only; not combined with prompt_lookup_num_tokens.  Without them, the captured step is the one above.
+        stop_strings (a str or up to 16 of them, 1..128 characters each) with tokenizer: Hugging Face's StopStringCriteria,
+        checked inside the captured step after every token, the first one included (ops.stop_check, aria_b200.stopping).  A
+        row stops once the token it just emitted completes a string against the row's ids so far (left padding, image tokens
+        and prompt included), as the tokenizer's cleaned vocabulary spells them; it is then finished exactly as after an EOS
+        (the token is kept, pad_token_id follows, logprob filler), and min_new_tokens does not delay it.  A stopped row is
+        always padded, also without EOS ids (Hugging Face then keeps sampling into it), so stop_strings without eos_token_id
+        needs pad_token_id.  GPU only; not combined with prompt_lookup_num_tokens.  The step captured for one set of strings
+        serves any other set with the same vocabulary; without stop_strings it is the one above.
         Returns [B * n, T + generated] int64 on the model's device (prompt ids first); with output_logprobs a GenerateOutput
         (sequences: that tensor; logprobs [B * n, L] fp32, top_ids [B * n, L, k] int64, top_logprobs [B * n, L, k] fp32, L the
         generated length)."""
@@ -401,6 +409,8 @@ class AriaForConditionalGeneration(nn.Module):
         dev = self.device
         processors = self._check_logits_processors(repetition_penalty, min_p, min_new_tokens, prompt_lookup_num_tokens, dev)
         self._check_output_logprobs(output_logprobs, prompt_lookup_num_tokens, dev)
+        stops = self._check_stop_strings(stop_strings, tokenizer, eos, pad_token_id, prompt_lookup_num_tokens, dev)
+        table = None if stops is None else stopping.vocab_table(tokenizer)
         if prompt_lookup_num_tokens is not None:
             K, M = self._check_prompt_lookup(B, prompt_lookup_num_tokens, max_matching_ngram_size, n_seq, shared_prefix_len,
                                              kv_cache_dtype, dev)
@@ -414,7 +424,8 @@ class AriaForConditionalGeneration(nn.Module):
                 raise NotImplementedError("aria_b200: shared_prefix_len runs on the GPU only")
             sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
             return self._generate_shared_prefix(input_ids, ids_host, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos,
-                                                pad, poll_every, n_seq, shared_prefix_len, output_logprobs, processors)
+                                                pad, poll_every, n_seq, shared_prefix_len, output_logprobs, processors,
+                                                stops, table)
         if dev.type != "cuda":
             if do_sample or eos:
                 raise NotImplementedError("aria_b200: sampling and EOS run on the GPU only")
@@ -430,10 +441,10 @@ class AriaForConditionalGeneration(nn.Module):
         T_max = -(-(T if n_seq > 1 else T + max_new_tokens) // 256) * 256
         key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, n_seq, None, kv_cache_dtype)
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors or g.stop is not table:
             self._decode_graph = g = None   # release the old graph and cache before building the new one
             g = self._decode_graph = GraphedDecode(self, B, T_max, max_new_tokens, sampling, eos, pad, kv_cache_dtype, n_seq,
-                                                   logprobs=output_logprobs, processors=processors)
+                                                   logprobs=output_logprobs, processors=processors, stop=table)
         mask = None if attention_mask is None else attention_mask.to("cpu", torch.long)
         inputs = self.prepare_inputs_for_generation(input_ids, None, pixel_values=pixel_values, pixel_mask=pixel_mask,
                                                     attention_mask=mask, num_logits_to_keep=1)
@@ -443,6 +454,8 @@ class AriaForConditionalGeneration(nn.Module):
         g.start(T, mask)
         if processors is not None:
             g.start_presence(input_ids.to(dev) if n_seq == 1 else input_ids.to(dev).repeat_interleave(n_seq, 0))
+        if stops is not None:
+            g.start_stops(stops, input_ids.repeat_interleave(n_seq, 0))
         first = out.logits[:, -1]
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         n, L = g.run(max_new_tokens, poll_every)
@@ -452,7 +465,7 @@ class AriaForConditionalGeneration(nn.Module):
         return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
 
     def _generate_shared_prefix(self, input_ids, ids, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos, pad,
-                                poll_every, n_seq, P, output_logprobs=None, processors=None):
+                                poll_every, n_seq, P, output_logprobs=None, processors=None, stops=None, table=None):
         """generate(shared_prefix_len=P) on checked arguments (ids: the host copy of input_ids, lens: each row's real length,
         from _check_shared_prefix): ViT + prefix prefill (forward()) into a SharedPrefixCache of one prompt row, the packed
         suffix prefill (AriaMoELMModel.prefill_suffixes), the first token from each suffix's last position, then the graphed
@@ -471,10 +484,10 @@ class AriaForConditionalGeneration(nn.Module):
         N_max = -(-(max(S) + max_new_tokens) // 256) * 256
         key = (1, T_max, max_new_tokens, sampling, eos, pad, dev, B * n_seq, N_max, "bf16")
         g = getattr(self, "_decode_graph", None)
-        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors:
+        if g is None or g.key != key or g.n_logprobs != output_logprobs or g.processors != processors or g.stop is not table:
             self._decode_graph = g = None
             g = self._decode_graph = GraphedDecode(self, 1, T_max, max_new_tokens, sampling, eos, pad, "bf16", B * n_seq,
-                                                   N_max=N_max, logprobs=output_logprobs, processors=processors)
+                                                   N_max=N_max, logprobs=output_logprobs, processors=processors, stop=table)
         g.cache.seq_len = 0
         self.forward(prefix, pixel_values, pixel_mask, past_key_values=g.cache, num_logits_to_keep=1)
         cu_dev = cu.to(dev, non_blocking=True)
@@ -486,6 +499,8 @@ class AriaForConditionalGeneration(nn.Module):
         g.start_suffixes(P, S, n_seq)
         if processors is not None:      # each row's own left-padded ids, as the repeated-image batch has them
             g.start_presence(input_ids.to(dev).repeat_interleave(n_seq, 0))
+        if stops is not None:
+            g.start_stops(stops, input_ids.repeat_interleave(n_seq, 0))
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         _, L = g.run(max_new_tokens, poll_every)
         prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
@@ -611,6 +626,22 @@ class AriaForConditionalGeneration(nn.Module):
         return float(repetition_penalty), float(min_p), int(min_new_tokens)
 
     @staticmethod
+    def _check_stop_strings(stop_strings, tokenizer, eos, pad_token_id, prompt_lookup_num_tokens, device):
+        """generate()'s checks of stop_strings after _check_output_logprobs', on the host: the strings and the tokenizer
+        (stopping.check_stop_strings), then prompt lookup and a CPU device (NotImplementedError), then no EOS id and no
+        pad_token_id (ValueError).  -> None, or the strings as a tuple."""
+        stops = stopping.check_stop_strings(stop_strings, tokenizer)
+        if stops is None:
+            return None
+        if prompt_lookup_num_tokens is not None:
+            raise NotImplementedError("stop_strings with prompt_lookup_num_tokens is not supported")
+        if torch.device(device).type != "cuda":
+            raise NotImplementedError("aria_b200: stop_strings run on the GPU only")
+        if not eos and pad_token_id is None:
+            raise ValueError("stop_strings without eos_token_id needs pad_token_id: a stopped row is padded with it")
+        return stops
+
+    @staticmethod
     def _check_output_logprobs(k, prompt_lookup_num_tokens, device):
         """generate(output_logprobs=k)'s checks after _check_generate_args', on the host: k (ValueError), then prompt lookup and
         a CPU device (NotImplementedError)."""
@@ -711,11 +742,14 @@ class GraphedDecode:
     processors (penalty, min_p, min_new_tokens) (generate(repetition_penalty=..., min_p=..., min_new_tokens=...)): the sampler is
     ops.sample_tokens_processed, which reads each row's presence bitmap [B, V / 32] (start_presence) and counts its emitted
     tokens by `step`, and the advance is followed by ops.presence_set of the tokens it wrote to `ids`.  generate() rebuilds the
-    graph when they change, as it does for logprobs.  None: the step is exactly the one without them."""
+    graph when they change, as it does for logprobs.  None: the step is exactly the one without them.
+    stop (generate(stop_strings=..., tokenizer=...)): the tokenizer's stopping.StopVocab; the advance is followed by
+    ops.stop_check on static buffers, the stop set and each row's prompt tail, that start_stops() rewrites, so one capture
+    serves every set of strings.  None: the step is exactly the one without it."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
                  kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None, logprobs: Optional[int] = None,
-                 processors: Optional[tuple] = None):
+                 processors: Optional[tuple] = None, stop: Optional[stopping.StopVocab] = None):
         from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
         dev = model.device
         lm = model.language_model
@@ -762,6 +796,15 @@ class GraphedDecode:
                               torch.full((B,), penalty, **f32), torch.full((B,), min_new, **i32))
             self.V = c.vocab_size
             self.presence = torch.zeros(B, ops.presence_words(self.V), **i32)
+        self.stop = stop
+        if stop is not None:
+            self.stop_vocab = stop.device(dev)
+            self.stop_bytes = torch.zeros(stopping.MAX_STRINGS, stopping.MAX_BYTES, dtype=torch.uint8, device=dev)
+            self.stop_lens = torch.zeros(stopping.MAX_STRINGS, dtype=torch.int32, device=dev)
+            self.stop_lookback = torch.zeros(1, dtype=torch.int32, device=dev)
+            self.stop_tail = torch.zeros(B, stopping.TAIL, dtype=torch.int64, device=dev)
+            self.stop_tail_len = torch.zeros(B, dtype=torch.int32, device=dev)
+            self.stop_counter = torch.zeros(1, dtype=torch.int32, device=dev)
         self.done_host = torch.full((1,), -1, dtype=torch.int32).pin_memory()
         self.event = torch.cuda.Event()
         self.dev = dev
@@ -798,11 +841,24 @@ class GraphedDecode:
                            self.rng_offset, self.finished, self.done_step, self.eos, self.pad)
         if self.processors is not None:
             ops.presence_set(self.ids, self.presence, self.V)
+        if self.stop is not None:
+            ops.stop_check(*self.stop_vocab, self.stop_bytes, self.stop_lens, self.stop_lookback, self.stop_tail,
+                           self.stop_tail_len, self.out_tokens, self.step, self.finished, self.done_step, self.stop_counter)
         self.done_host.copy_(self.done_step, non_blocking=True)
 
     def start_presence(self, ids: torch.Tensor):
         """Every row's presence bitmap from its ids [B, T] on the device (the prompt as the row has it, padding included)."""
         ops.presence_set(ids, self.presence, self.V, clear=True)
+
+    def start_stops(self, strings, ids: torch.Tensor):
+        """The stop set of strings, and every row's prompt tail from its ids [B, T] (as the row has them, padding included)."""
+        data, lens, lookback = stopping.encode_stop_set(strings)
+        tail, n = stopping.prompt_tail(ids)
+        self.stop_bytes.copy_(data)
+        self.stop_lens.copy_(lens)
+        self.stop_lookback.fill_(lookback)
+        self.stop_tail.copy_(tail)
+        self.stop_tail_len.fill_(n)
 
     def result(self, sequences: torch.Tensor, L: int):
         """generate()'s return value: sequences alone, or with logprobs a GenerateOutput of the first L columns."""
@@ -857,15 +913,16 @@ class GraphedDecode:
         self.done_host.fill_(-1)
 
     def run(self, max_new_tokens: int, poll_every: int):
-        """Replay the step until max_new_tokens tokens are out (the first one is sampled before) or, with EOS ids, every row has
-        finished; the host polls every poll_every steps.  -> (steps replayed, tokens to keep per row)."""
+        """Replay the step until max_new_tokens tokens are out (the first one is sampled before) or, with EOS ids or stop
+        strings, every row has finished; the host polls every poll_every steps.  -> (steps replayed, tokens to keep per row)."""
         n = 0
+        poll = bool(self.eos) or self.stop is not None
         while n < max_new_tokens - 1:
-            if self.eos and n % poll_every == 0 and self.done():
+            if poll and n % poll_every == 0 and self.done():
                 break
             self.graph.replay()
             n += 1
-        done = int(self.done_step.item())       # synchronises; -1 when no EOS stopped the batch
+        done = int(self.done_step.item())       # synchronises; -1 when no EOS or stop string stopped the batch
         return n, (done + 1 if done >= 0 else max_new_tokens)
 
     def done(self) -> bool:

@@ -590,7 +590,10 @@ class SlotDecodeState(DecodeState):
     writes at n_out mod lp_ring: lp_ring_lp [max_batch, lp_ring] fp32, lp_ring_ids [max_batch, lp_ring, 20] int32 and
     lp_ring_top [max_batch, lp_ring, 20] fp32.
     Logits processors (serving.Engine's repetition_penalty, min_p, min_new_tokens): the slot's rep_penalty (1: off), min_p (0:
-    off) and min_new, and presence [max_batch, ceil(vocab / 32)] int32, the bitmap of the ids its request has seen."""
+    off) and min_new, and presence [max_batch, ceil(vocab / 32)] int32, the bitmap of the ids its request has seen.
+    Stops (serving.Engine's stop_strings, stop_token_ids): the slot's stop set stop_bytes [max_batch, 16, 512] uint8, stop_lens
+    [max_batch, 16] int32 and stop_lookback (0: no strings), its stop ids stop_ids [max_batch, 8] int64 (the first n_stop_ids),
+    and its prompt tail stop_tail [max_batch, 128] int64, the last stop_tail_len ids right-aligned (ops.stop_check_slots)."""
 
     def __init__(self, max_batch, H, max_out, device, lp_ring: int = 1, vocab: int = 1):
         super().__init__(max_batch, H, 0, device)
@@ -616,11 +619,19 @@ class SlotDecodeState(DecodeState):
         self.min_p = torch.zeros(max_batch, dtype=torch.float32, device=device)
         self.min_new = torch.zeros(max_batch, **i32)
         self.presence = torch.zeros(max_batch, ops.presence_words(vocab), **i32)
+        self.stop_bytes = torch.zeros(max_batch, ops.STOP_MAX_STRINGS, ops.STOP_MAX_BYTES, dtype=torch.uint8, device=device)
+        self.stop_lens = torch.zeros(max_batch, ops.STOP_MAX_STRINGS, **i32)
+        self.stop_lookback = torch.zeros(max_batch, **i32)
+        self.stop_ids = torch.zeros(max_batch, ops.STOP_MAX_IDS, **i64)
+        self.n_stop_ids = torch.zeros(max_batch, **i32)
+        self.stop_tail = torch.zeros(max_batch, ops.STOP_MAX_TOKENS, **i64)
+        self.stop_tail_len = torch.zeros(max_batch, **i32)
 
     # the per-slot arrays, in the order a slot's row is copied when slots are compacted
     SLOT_FIELDS = ("rope_pos", "write_pos", "kv_len", "temperature", "top_k", "top_p", "seed", "noise_row", "rng_offset",
                    "max_new", "n_out", "finished", "ids_in", "next_ids", "out_tokens", "lp_n", "lp_ring_lp", "lp_ring_ids",
-                   "lp_ring_top", "rep_penalty", "min_p", "min_new", "presence")
+                   "lp_ring_top", "rep_penalty", "min_p", "min_new", "presence", "stop_bytes", "stop_lens", "stop_lookback",
+                   "stop_ids", "n_stop_ids", "stop_tail", "stop_tail_len")
 
     def rows(self, n):
         """A DecodeState view of the first n slots (what decode_step and the sampler of a step over n slots read)."""

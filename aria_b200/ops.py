@@ -1834,3 +1834,61 @@ def decode_advance_slots(next_ids: torch.Tensor, ids_in: torch.Tensor, out_token
                                                    _p(max_new), _p(rope_pos), _p(write_pos), _p(kv_len), _p(rng_offset),
                                                    _p(finished), C.cast(eos, C.c_void_p), n_eos, int(pad_token_id), R,
                                                    _stream(next_ids)), "decode_advance_slots")
+
+
+# ------------------------------------------------------------------------------------------- stop strings
+STOP_MAX_STRINGS, STOP_MAX_BYTES, STOP_MAX_TOKENS, STOP_MAX_IDS = 16, 512, 128, 8
+
+
+def stop_check(vocab_bytes: torch.Tensor, vocab_offsets: torch.Tensor, stop_bytes: torch.Tensor, stop_lens: torch.Tensor,
+               lookback: torch.Tensor, prompt_tail: torch.Tensor, tail_len: torch.Tensor, out_tokens: torch.Tensor,
+               step: torch.Tensor, finished: torch.Tensor, done_step: torch.Tensor, counter: torch.Tensor):
+    """Hugging Face's StopStringCriteria on B rows, after decode_advance: a row that is not finished and whose history
+    (prompt_tail int64 [B, 128], its last tail_len[b] ids right-aligned, then out_tokens[b, :step]) ends by completing one of
+    the stop set's strings gets finished[b] = 1; when that leaves every row finished, done_step = step - 1 (if still < 0).
+    The vocabulary table: uint8 bytes and int32 offsets [V + 1] (stopping.StopVocab); the stop set: uint8 [16, 512], int32
+    byte lengths [16] and int32 lookback [1] (stopping.encode_stop_set).  counter: int32 [1], zero.  See aria_stop_check."""
+    B = finished.numel()
+    for t, dt in ((vocab_bytes, torch.uint8), (vocab_offsets, torch.int32), (stop_bytes, torch.uint8), (stop_lens, torch.int32),
+                  (lookback, torch.int32), (prompt_tail, torch.int64), (tail_len, torch.int32), (out_tokens, torch.int64),
+                  (step, torch.int32), (finished, torch.uint8), (done_step, torch.int32), (counter, torch.int32)):
+        _chk(t, dt, align=1)
+    if vocab_offsets.dim() != 1 or vocab_offsets.numel() < 2:
+        raise ValueError(f"stop_check: vocab_offsets must be [V + 1] with V >= 1, got {tuple(vocab_offsets.shape)}")
+    if stop_bytes.shape != (STOP_MAX_STRINGS, STOP_MAX_BYTES) or stop_lens.shape != (STOP_MAX_STRINGS,) or lookback.numel() != 1:
+        raise ValueError("stop_check: the stop set must be [16, 512], [16] and [1]")
+    if prompt_tail.shape != (B, STOP_MAX_TOKENS) or tail_len.shape != (B,) or out_tokens.dim() != 2 or out_tokens.shape[0] != B:
+        raise ValueError(f"stop_check: prompt_tail [{B}, 128], tail_len [{B}] and out_tokens [{B}, L] expected")
+    with torch.cuda.device(finished.device):
+        L.check(L.load().aria_stop_check(_p(vocab_bytes), _p(vocab_offsets), vocab_offsets.numel() - 1, _p(stop_bytes),
+                                         _p(stop_lens), _p(lookback), _p(prompt_tail), _p(tail_len), _p(out_tokens),
+                                         out_tokens.shape[1], _p(step), _p(finished), _p(done_step), _p(counter), B,
+                                         _stream(finished)), "stop_check")
+
+
+def stop_check_slots(vocab_bytes: torch.Tensor, vocab_offsets: torch.Tensor, stop_bytes: torch.Tensor, stop_lens: torch.Tensor,
+                     lookback: torch.Tensor, stop_ids: torch.Tensor, n_stop_ids: torch.Tensor, prompt_tail: torch.Tensor,
+                     tail_len: torch.Tensor, out_tokens: torch.Tensor, n_out: torch.Tensor, finished: torch.Tensor,
+                     ids_in: torch.Tensor, pad_token_id: int):
+    """stop_check per slot, after decode_advance_slots: slot r has its own stop set (stop_bytes uint8 [R, 16, 512], stop_lens
+    int32 [R, 16], lookback int32 [R], 0 = no strings) and its own stop ids (stop_ids int64 [R, 8], the first n_stop_ids[r]);
+    its history is its prompt tail (int64 [R, 128], tail_len [R]), then out_tokens[r, :n_out[r]] (int32).  A slot that is not
+    finished and stops gets finished[r] = 1 and ids_in[r] = pad_token_id.  See aria_stop_check_slots."""
+    R = finished.numel()
+    for t, dt in ((vocab_bytes, torch.uint8), (vocab_offsets, torch.int32), (stop_bytes, torch.uint8), (stop_lens, torch.int32),
+                  (lookback, torch.int32), (stop_ids, torch.int64), (n_stop_ids, torch.int32), (prompt_tail, torch.int64),
+                  (tail_len, torch.int32), (out_tokens, torch.int32), (n_out, torch.int32), (finished, torch.uint8),
+                  (ids_in, torch.int64)):
+        _chk(t, dt, align=1)
+    if vocab_offsets.dim() != 1 or vocab_offsets.numel() < 2:
+        raise ValueError(f"stop_check_slots: vocab_offsets must be [V + 1] with V >= 1, got {tuple(vocab_offsets.shape)}")
+    if (stop_bytes.shape != (R, STOP_MAX_STRINGS, STOP_MAX_BYTES) or stop_lens.shape != (R, STOP_MAX_STRINGS)
+            or lookback.shape != (R,) or stop_ids.shape != (R, STOP_MAX_IDS) or n_stop_ids.shape != (R,)
+            or prompt_tail.shape != (R, STOP_MAX_TOKENS) or tail_len.shape != (R,) or out_tokens.dim() != 2
+            or out_tokens.shape[0] != R or n_out.shape != (R,) or ids_in.numel() != R):
+        raise ValueError(f"stop_check_slots: every slot array must have {R} rows")
+    with torch.cuda.device(finished.device):
+        L.check(L.load().aria_stop_check_slots(_p(vocab_bytes), _p(vocab_offsets), vocab_offsets.numel() - 1, _p(stop_bytes),
+                                               _p(stop_lens), _p(lookback), _p(stop_ids), _p(n_stop_ids), _p(prompt_tail),
+                                               _p(tail_len), _p(out_tokens), out_tokens.shape[1], _p(n_out), _p(finished),
+                                               _p(ids_in), int(pad_token_id), R, _stream(finished)), "stop_check_slots")

@@ -66,7 +66,7 @@ from typing import Dict, List, Optional
 
 import torch
 
-from . import ops
+from . import ops, stopping
 from .ops import MAX_LOGPROBS
 
 PAGE = 256
@@ -274,6 +274,8 @@ class Request:
     lp_drained: int = 0                                 # generated tokens whose logprobs the host has copied out of the ring
     lp_parts: list = field(default_factory=list)        # host (logprob [m], ids [m, k], logprobs [m, k]) pieces, in order
     processors: Optional[tuple] = None                  # (repetition_penalty, min_p, min_new_tokens), None when all are off
+    stop_strings: Optional[tuple] = None                # the request's stop strings (None: none)
+    stop_token_ids: tuple = ()                          # its own ids that finish it like EOS
     plp_parts: list = field(default_factory=list)       # device pieces of the prompt logprobs, in order
 
     @property
@@ -425,12 +427,17 @@ class Engine:
     decode step writes each asking slot's entries into per-slot rings of poll_every + 1 entries (SlotDecodeState.lp_ring_*),
     copied to the host at each poll, so the device memory does not grow with the pool (4 x 41 x max_batch x (poll_every + 1)
     bytes).  A step with no asking slot replays a graph without the logprob kernel.  Prompt logprobs are computed from the
-    prefill's final hidden states in chunks of at most 1024 rows (a logits scratch of 2 x 1024 x V bytes)."""
+    prefill's final hidden states in chunks of at most 1024 rows (a logits scratch of 2 x 1024 x V bytes).
+    tokenizer: the tokenizer whose cleaned vocabulary spells the tokens for add_request(stop_strings=...) (its table is built
+    here, stopping.vocab_table; None: no request may ask for stop strings).  Stops: 9.4 KB of per-slot state (a stop set of
+    16 x 512 bytes, eight stop ids, a 128-id prompt tail); a step with no stopping slot replays a graph without the check."""
 
     max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS
+    tokenizer = None
 
     def __init__(self, model, max_batch: int = 64, max_kv_tokens: int = 131072, eos_token_id=None, pad_token_id=None,
-                 poll_every: int = 8, max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS, kv_cache_dtype: str = "bf16"):
+                 poll_every: int = 8, max_prefill_tokens: Optional[int] = DEFAULT_PREFILL_TOKENS, kv_cache_dtype: str = "bf16",
+                 tokenizer=None):
         from .moe_lm import KV_CACHE_DTYPES, PagedKVCache, SlotDecodeState
         if not isinstance(kv_cache_dtype, str) or kv_cache_dtype not in KV_CACHE_DTYPES:
             raise ValueError(f"kv_cache_dtype must be 'bf16' or 'fp8', got {kv_cache_dtype!r}")
@@ -453,6 +460,9 @@ class Engine:
         self.model, self.dev = model, dev
         self.max_batch, self.poll_every, self.max_prefill_tokens = max_batch, poll_every, max_prefill_tokens
         self.eos, self.pad = eos, pad
+        self.tokenizer = tokenizer
+        # without a tokenizer only stop ids can stop a request, and the check reads a one-id table no slot's strings use
+        self.stop_vocab = (stopping.StopVocab({0: ""}) if tokenizer is None else stopping.vocab_table(tokenizer)).device(dev)
         lm = model.language_model
         c = lm.config
         self.max_pages = _pages_for(max_kv_tokens)
@@ -485,7 +495,7 @@ class Engine:
     def add_request(self, input_ids, pixel_values=None, pixel_mask=None, max_new_tokens: int = 16, do_sample: bool = False,
                     temperature: float = 1.0, top_k: int = 50, top_p: float = 1.0, seed: int = 0, logprobs: Optional[int] = None,
                     prompt_logprobs: Optional[int] = None, repetition_penalty: float = 1.0, min_p: float = 0.0,
-                    min_new_tokens: int = 0) -> int:
+                    min_new_tokens: int = 0, stop_strings=None, stop_token_ids=None) -> int:
         """Queue one request (input_ids [T] or [1, T]; pixel inputs as generate()'s for that one row) -> its id.  Arguments are
         checked as generate() checks them, and a request that needs more pages than the pool has is refused, here, before
         any device work.  The prompt's page keys (page_keys) are computed here, on the host.
@@ -493,7 +503,12 @@ class Engine:
         raw distribution and its k most likely tokens, in self.logprobs[rid] once it finishes (Logprobs); the generated ones are
         generate(output_logprobs=k)'s bit for bit.  A request with prompt_logprobs takes no prefix-cache hit.
         repetition_penalty / min_p / min_new_tokens: generate()'s logits processors; the request's tokens are batch-1 generate()'s
-        with the same arguments bit for bit.  A decode step runs the processed sampler only when some active slot asks for one."""
+        with the same arguments bit for bit.  A decode step runs the processed sampler only when some active slot asks for one.
+        stop_strings (generate()'s, with the engine's tokenizer) and stop_token_ids (an id or a list of ids that finish this
+        request like an EOS; with the engine's EOS ids at most 8): the result is batch-1 generate(ids, ..., stop_strings=...,
+        tokenizer=tokenizer, eos_token_id=eos + stop_token_ids, pad_token_id=pad)[0] bit for bit.  stop_token_ids is a stopping
+        criterion only, so it is not combined with min_new_tokens > 0 (which masks EOS ids).  A decode step runs the stop check
+        only when some active slot has stops."""
         if not isinstance(input_ids, torch.Tensor) or input_ids.dim() not in (1, 2):
             raise ValueError("input_ids must be a tensor [T] or [1, T]")
         ids = input_ids.reshape(1, -1) if input_ids.dim() == 1 else input_ids
@@ -505,14 +520,34 @@ class Engine:
         processors = AriaForConditionalGeneration._check_logits_processors(repetition_penalty, min_p, min_new_tokens, None, "cuda")
         _check_logprobs_arg("logprobs", logprobs)
         _check_logprobs_arg("prompt_logprobs", prompt_logprobs)
+        stops, stop_ids = self._check_stops(stop_strings, stop_token_ids, min_new_tokens)
         sampling = (float(temperature), int(top_k), float(top_p), int(seed)) if do_sample else (0.0, 0, 1.0, 0)
         req = Request(self._next_rid, ids[0].to("cpu", torch.int64), max_new_tokens, sampling, pixel_values, pixel_mask,
-                      logprobs=logprobs, prompt_logprobs=prompt_logprobs, processors=processors)
+                      logprobs=logprobs, prompt_logprobs=prompt_logprobs, processors=processors, stop_strings=stops,
+                      stop_token_ids=stop_ids)
         image_token = None if pixel_values is None else self.model.config.image_token_index
         req.keys = page_keys(req.input_ids, pixel_values, pixel_mask, image_token)
         self.sched.submit(req)
         self._next_rid += 1
         return req.rid
+
+    def _check_stops(self, stop_strings, stop_token_ids, min_new_tokens):
+        """add_request's checks of its stops, after the logprob checks, in this order: the strings and the engine's tokenizer
+        (stopping.check_stop_strings), then stop_token_ids: its type, then more than 8 ids with the engine's EOS ids
+        (ValueError), then min_new_tokens > 0 (NotImplementedError).  -> (strings or None, ids tuple)."""
+        stops = stopping.check_stop_strings(stop_strings, self.tokenizer)
+        if stop_token_ids is None:
+            return stops, ()
+        ids = (stop_token_ids,) if isinstance(stop_token_ids, int) else stop_token_ids
+        if (not isinstance(ids, (list, tuple)) or not ids
+                or not all(isinstance(e, int) and not isinstance(e, bool) for e in ids)):
+            raise ValueError(f"stop_token_ids must be an int or a non-empty list of ints, got {stop_token_ids!r}")
+        if len(self.eos) + len(ids) > stopping.MAX_IDS:
+            raise ValueError(f"stop_token_ids: the engine's {len(self.eos)} EOS ids and the request's {len(ids)} stop ids are "
+                             f"more than {stopping.MAX_IDS}")
+        if min_new_tokens > 0:
+            raise NotImplementedError("stop_token_ids with min_new_tokens > 0 is not supported")
+        return stops, tuple(ids)
 
     @property
     def n_active(self) -> int:
@@ -536,7 +571,9 @@ class Engine:
         decoding = self.sched.n_active - (self.sched.partial is not None)    # a partly prefilled request's slot is idle
         if decoding:
             n, width = _pow2_at_least(self.sched.n_active, self.max_batch), _pow2_at_least(self.sched.width(), self.max_pages)
-            if self._any_processors():
+            if self._any_stops():
+                g = self._graph(n, width, self._any_logprobs(), self._any_processors(), True)
+            elif self._any_processors():
                 g = self._graph(n, width, self._any_logprobs(), True)
             else:
                 g = self._graph(n, width, True) if self._any_logprobs() else self._graph(n, width)
@@ -598,6 +635,8 @@ class Engine:
         st.rep_penalty[lo:hi] = 1.0
         st.min_p[lo:hi] = 0.0
         st.min_new[lo:hi] = 0
+        st.stop_lookback[lo:hi] = 0
+        st.n_stop_ids[lo:hi] = 0
         self.cache.block_table[lo:hi] = -1
         self.cache.block_table[lo:hi, 0] = 0
 
@@ -607,19 +646,22 @@ class Engine:
     def _any_processors(self) -> bool:
         return any(r.processors is not None for r in self.sched.slots)
 
-    def _step(self, n: int, lp: bool, proc: bool = False) -> None:
+    def _any_stops(self) -> bool:
+        return any(r.stop_strings is not None or r.stop_token_ids for r in self.sched.slots)
+
+    def _step(self, n: int, lp: bool, proc: bool = False, stop: bool = False) -> None:
         lm = self.model.language_model
         st = self.state.rows(n)
         emb = ops.embedding(st.ids_in, lm.get_input_embeddings().weight)
         logits = lm.decode_step(emb, self.cache, st, self.rope)
-        self._sample_and_advance(st, logits[:, -1], lp, proc)
+        self._sample_and_advance(st, logits[:, -1], lp, proc, stop)
         self._fin_host.copy_(self.state.finished, non_blocking=True)
         self._nout_host.copy_(self.state.n_out, non_blocking=True)
 
-    def _sample_and_advance(self, st, logits, lp: bool, proc: bool = False) -> None:
+    def _sample_and_advance(self, st, logits, lp: bool, proc: bool = False, stop: bool = False) -> None:
         """Sample (with proc, through each slot's logits processors), then with lp the logprobs of the slots with lp_n >= 0 into
         ring entry n_out mod lp_ring (finished slots untouched), then advance; with proc, each slot's new input id then joins
-        its presence bitmap."""
+        its presence bitmap; with stop, each slot's stop ids and strings are checked against its new token."""
         if proc:
             ops.sample_tokens_processed(logits, st.temperature, st.top_k, st.top_p, st.min_p, st.seed, st.rep_penalty, st.min_new,
                                         st.presence, st.rng_offset, st.n_out, self.eos, noise_rows=st.noise_row, out=st.next_ids)
@@ -633,13 +675,17 @@ class Engine:
                                  st.kv_len, st.rng_offset, st.finished, self.eos, self.pad)
         if proc:
             ops.presence_set(st.ids_in, st.presence, self.model.language_model.config.vocab_size)
+        if stop:
+            ops.stop_check_slots(*self.stop_vocab, st.stop_bytes, st.stop_lens, st.stop_lookback, st.stop_ids, st.n_stop_ids,
+                                 st.stop_tail, st.stop_tail_len, st.out_tokens, st.n_out, st.finished, st.ids_in, self.pad)
 
-    def _graph(self, n: int, width: int, lp: bool = False, proc: bool = False) -> torch.cuda.CUDAGraph:
+    def _graph(self, n: int, width: int, lp: bool = False, proc: bool = False, stop: bool = False) -> torch.cuda.CUDAGraph:
         """The captured step over slots [0, n) and table columns [0, width), with the logprob kernel when lp and the processed
         sampler when proc, captured on first use; its key is (n, width), (n, width, True) with the logprob kernel, and
-        (n, width, lp, "processors") with the processed sampler.  The warm-up run before the capture computes the very step the
+        (n, width, lp, "processors") with the processed sampler, and (n, width, lp, proc, "stops") with the stop check.  The warm-up run before the capture computes the very step the
         next replay computes; the slot rows it advanced are put back afterwards."""
-        key = (n, width, lp, "processors") if proc else (n, width, True) if lp else (n, width)
+        key = ((n, width, lp, proc, "stops") if stop else (n, width, lp, "processors") if proc else (n, width, True) if lp
+               else (n, width))
         g = self._graphs.get(key)
         if g is not None:
             return g
@@ -649,13 +695,13 @@ class Engine:
         side = torch.cuda.Stream(device=self.dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):
-            self._step(n, lp, proc)
+            self._step(n, lp, proc, stop)
         cur.wait_stream(side)
         for f, t in keep.items():
             getattr(self.state, f).copy_(t)
         g = torch.cuda.CUDAGraph()
         with ops.graph_capture(g, pool=self._pool):
-            self._step(n, lp, proc)
+            self._step(n, lp, proc, stop)
         self._graphs[key] = g
         self.stats["graphs_captured"] += 1
         return g
@@ -830,7 +876,23 @@ class Engine:
         if req.processors is not None:      # the prompt's ids, before the first token is sampled
             ops.presence_set(req.input_ids.to(self.dev)[None], st.presence[s:s + 1], self.model.language_model.config.vocab_size,
                              clear=True)
-        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None, req.processors is not None)
+        stop = req.stop_strings is not None or bool(req.stop_token_ids)
+        if stop:            # the prompt's tail and the request's stops, before the first token is checked
+            data, lens, lookback = stopping.encode_stop_set(req.stop_strings or ())
+            tail, n = stopping.prompt_tail(req.input_ids[None])
+            ids = torch.zeros(stopping.MAX_IDS, dtype=torch.int64)
+            ids[:len(req.stop_token_ids)] = torch.tensor(req.stop_token_ids, dtype=torch.int64)
+            st.stop_bytes[s].copy_(data)
+            st.stop_lens[s].copy_(lens)
+            st.stop_lookback[s] = lookback
+            st.stop_ids[s].copy_(ids)
+            st.n_stop_ids[s] = len(req.stop_token_ids)
+            st.stop_tail[s].copy_(tail[0])
+            st.stop_tail_len[s] = n
+        else:
+            st.stop_lookback[s] = 0
+            st.n_stop_ids[s] = 0
+        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None, req.processors is not None, stop)
 
     def _drop(self, s: int) -> None:
         """Retire slot s without a result: the last active slot moves into s and the slot it left becomes idle."""

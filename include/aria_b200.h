@@ -710,6 +710,34 @@ int aria_lookup_accept_advance(const int64_t* targets, const int64_t* step_ids, 
                                int32_t* status, uint64_t* counters, const int64_t* eos_ids, int32_t n_eos, int32_t B,
                                aria_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Stop strings (Hugging Face's StopStringCriteria), checked after the decode advance
+ * ------------------------------------------------------------------------------------------------ */
+/* The vocabulary table: token id i's cleaned string is vocab_bytes[vocab_offsets[i], vocab_offsets[i + 1]) (UTF-8), for
+ * 0 <= i < V; ids outside [0, V) match nothing.  A stop set is up to 16 strings of stop_bytes [16, 512] (UTF-8) with byte
+ * lengths stop_lens [16] (0 = unused), and *lookback: the tokens HF looks at, the characters of the longest string (<= 128).
+ * Every array is DEVICE memory.  A row stops after its final token when that token completes a string: some byte prefix of
+ * it ends with the string's last bytes (or holds the whole string), and the tokens before it, walking back within the
+ * lookback window, cover the rest of the string, the earliest one allowed to run off its start.  One warp per row. */
+/* One stop set for B <= 1024 rows.  The history of row b is its last tail_len[b] <= 128 prompt ids, right-aligned in
+ * prompt_tail [B, 128] int64, then out_tokens[b, 0 .. *step) ([B, max_steps] int64).  A row that is not finished and stops gets finished[b] = 1;
+ * then if every row is finished, *step > 0 and *done_step < 0, *done_step = *step - 1.  counter (int32) is 0 before the launch and after
+ * it. */
+int aria_stop_check(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
+                    const int32_t* stop_lens, const int32_t* lookback, const int64_t* prompt_tail,
+                    const int32_t* tail_len, const int64_t* out_tokens, int32_t max_steps, const int32_t* step, uint8_t* finished,
+                    int32_t* done_step, int32_t* counter, int32_t B, aria_stream_t stream);
+/* The serving engine's flavour, R <= 1024 slots, slot r with its own stop set (stop_bytes [R, 16, 512], stop_lens [R, 16],
+ * lookback [R]; lookback 0 = no strings) and its own stop ids (stop_ids [R, 8] int64, the first n_stop_ids[r] of them).  Its
+ * history is its prompt tail as above, then out_tokens[r, 0 .. n_out[r]) ([R, out_stride] int32).  A slot that is not
+ * finished and whose final token is one of its stop ids or completes one of its strings gets finished[r] = 1 and
+ * ids_in[r] = pad_token_id. */
+int aria_stop_check_slots(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
+                          const int32_t* stop_lens, const int32_t* lookback, const int64_t* stop_ids, const int32_t* n_stop_ids,
+                          const int64_t* prompt_tail, const int32_t* tail_len, const int32_t* out_tokens, int64_t out_stride,
+                          const int32_t* n_out, uint8_t* finished, int64_t* ids_in, int64_t pad_token_id, int32_t R,
+                          aria_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
