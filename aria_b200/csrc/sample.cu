@@ -2,6 +2,7 @@
 //
 // aria_sample_tokens: Hugging Face's warper chain on an fp32 copy of bf16 logits, one CTA of 1024 threads per row:
 //   TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper -> softmax -> multinomial.
+//   Values compare as torch compares them: -0 and +0 are one value, tied like any other equal logits.
 //   top-k: radix select on the 16-bit order-preserving key of each bf16 logit (two 8-bit histogram passes).  Division by a
 //     positive temperature is monotone, so the k-th largest scaled logit is the scaled k-th largest bf16 logit; every logit
 //     equal to it (the pivot) is kept, as TopKLogitsWarper keeps ties.
@@ -61,15 +62,20 @@ struct SampleParams {
   const uint64_t* rng_offset;  // device, or NULL (offset 0)
 };
 
-// order-preserving 16-bit key of a bf16 bit pattern (larger key = larger value) and its inverse
-__device__ __forceinline__ uint32_t bf16_key(uint32_t u) { return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u); }
+// order-preserving 16-bit key of a bf16 bit pattern (larger key = larger value) and its inverse.  -0 is keyed as +0: the two
+// compare equal in torch and transformers, so they tie (argmax and top-k ties, the stable top-p order, the top-n list).
+__device__ __forceinline__ uint32_t bf16_key(uint32_t u) {
+  u = u == 0x8000u ? 0u : u;
+  return (u & 0x8000u) ? (~u & 0xFFFFu) : (u | 0x8000u);
+}
 __device__ __forceinline__ float key_to_float(uint32_t k) {
   const uint32_t u = (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu);
   return __uint_as_float(u << 16);
 }
-// the same for an fp32 value: the 32-bit key of the processed scores
+// the same for an fp32 value: the 32-bit key of the processed scores (-0 keyed as +0 here too)
 __device__ __forceinline__ uint32_t f32_key(float f) {
-  const uint32_t u = __float_as_uint(f);
+  uint32_t u = __float_as_uint(f);
+  u = u == 0x80000000u ? 0u : u;
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 __device__ __forceinline__ float f32_key_to_float(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }

@@ -18,11 +18,12 @@ def _ops():
 
 
 def _rows(R, V, seed):
-    """R rows cycling through: randn at scale 1 and 30, a peaked row, a constant row, rows quantized to 4 values."""
+    """R rows cycling through: randn at scale 1 and 30, a peaked row, a constant row, rows quantized to 4 values, and rows
+    whose top entries are -0 and +0 ties in mixed order below three larger logits (the pivot of n = 5 among them)."""
     g = torch.Generator().manual_seed(seed)
     out = torch.empty(R, V)
     for r in range(R):
-        kind = r % 5
+        kind = r % 6
         if kind == 0:
             x = torch.randn(V, generator=g)
         elif kind == 1:
@@ -32,8 +33,14 @@ def _rows(R, V, seed):
             x[int(torch.randint(V, (1,), generator=g))] += 60
         elif kind == 3:
             x = torch.full((V,), 0.75)
-        else:
+        elif kind == 4:
             x = torch.randint(0, 4, (V,), generator=g).float() - 1.5
+        else:
+            x = -1 - torch.rand(V, generator=g)
+            p = torch.randperm(V, generator=g)
+            x[p[:3]] = 2.0
+            z = p[3:15].sort().values
+            x[z] = torch.tensor([-0.0, 0.0] * 6)[:z.numel()]
         out[r] = x
     return out.bfloat16()
 
