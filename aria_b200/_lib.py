@@ -115,7 +115,6 @@ SIGNATURES = {
     "aria_kv_store_fp8": (i32, [vp, vp, i64, i64, vp, vp, vp, vp, i64, i64, i64, i64, i32, i32, i32, i32, i32, vp]),
     "aria_kv_append_fp8": (i32, [vp, vp, i64, i64, vp, vp, vp, vp, i64, i64, i64, i64, vp, i32, i32, i32, vp]),
     "aria_kv_load_fp8": (i32, [vp, vp, vp, vp, i64, i64, i64, i64, vp, vp, i64, i64, i32, i32, i32, i32, vp]),
-    "aria_decode_advance": (i32, [vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, i64, i32, vp]),
     "aria_attention_decode_multi": (i32, [vp, vp, vp, vp, vp, i64, vp, i32, i32, i32, i32, i64, i64, i64, i64, i64, f32, vp, i64,
                                           vp]),
     "aria_kv_append_rows": (i32, [vp, vp, i64, i64, i64, vp, vp, i64, i64, vp, i32, i32, i32, i32, vp]),
@@ -143,7 +142,6 @@ SIGNATURES = {
     "aria_sample_tokens_processed": (i32, [vp, i64, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, vp,
                                            i32, vp]),
     "aria_presence_set": (i32, [vp, i64, i32, i32, vp, i32, vp, i32, vp]),
-    "aria_stop_check": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, i32, vp]),
     "aria_stop_check_slots": (i32, [vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp, vp, vp, i64, i32, vp]),
 }
 

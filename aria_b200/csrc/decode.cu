@@ -4,15 +4,14 @@
 // aria_kv_append: copies the step's k and v rows ([B, H, 128] staging rows written by the q/k/v projection) into the cache
 //   at the device row pos[b].
 // aria_kv_scatter_tails: copies the packed suffix k and v rows of a shared-prefix prefill into the n tails of each prompt.
-// aria_decode_advance: after the sampler, feeds next_ids back as the next step's input, records the token, applies
-//   Hugging Face's EOS rule and advances the RoPE positions, the cache rows, the step index and the RNG offset.
+// aria_decode_advance_slots: after the sampler, feeds each row's token back as the next step's input, records it, applies
+//   Hugging Face's EOS rule and the row's budget, and advances the row's RoPE position, cache row, output count and RNG offset.
 //
 // Continuous batching (serving.Engine) over a paged KV cache, pools [n_pages, H, 256, 128] and a block table [R, max_pages]:
 // aria_kv_append_paged: kv_append into the page block_table[r, write_pos[r] / 256], row write_pos[r] % 256.  A negative
 //   write_pos, or one outside the row's mapped pages, writes nothing: idle and finished slots never touch another's pages.
 // aria_kv_pages_store: copies rows [0, T) of a one-row prefill cache into a request's pages.
 // aria_kv_pages_store_varlen: the same for packed segments, each into its own pages after its own prefix.
-// aria_decode_advance_slots: aria_decode_advance per slot: own output count, budget, RNG offset and finished flag.
 //
 // Prompt-lookup decoding (generate(prompt_lookup_num_tokens=K)): a step verifies Q = K + 1 tokens per row.
 // aria_kv_append_rows: kv_append for the Q rows of each row, at cache rows pos[b] + i.
@@ -79,50 +78,6 @@ __global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_append_rows_kernel(const _
 
 constexpr int ADV_MAX_EOS = 8;
 constexpr int ADV_MAX_B = 1024;
-
-struct AdvanceParams {
-  const int64_t* next_ids;
-  int64_t* ids_in;
-  int64_t* out_tokens;  // [B, max_steps]
-  int32_t max_steps;
-  int32_t* step;
-  int32_t* rope_pos;
-  int32_t* write_pos;
-  int32_t* kv_len;
-  uint64_t* rng_offset;
-  uint8_t* finished;
-  int32_t* done_step;
-  int64_t eos[ADV_MAX_EOS];
-  int32_t n_eos;
-  int64_t pad;
-  int32_t B;
-};
-
-__global__ void __launch_bounds__(ADV_MAX_B) decode_advance_kernel(const AdvanceParams p) {
-  const int b = threadIdx.x;
-  const int t = *p.step;
-  bool fin = true;
-  if (b < p.B) {
-    // GenerationMixin._sample: a finished row emits pad; a row finishes when the token it emits is an EOS id
-    const bool was = p.finished[b] != 0;
-    const int64_t tok = was ? p.pad : p.next_ids[b];
-    if (t < p.max_steps) p.out_tokens[static_cast<int64_t>(b) * p.max_steps + t] = tok;
-    p.ids_in[b] = tok;
-    bool now = was;
-    for (int e = 0; e < p.n_eos; ++e) now |= tok == p.eos[e];
-    p.finished[b] = now;
-    fin = now;
-    ++p.rope_pos[b];
-    ++p.write_pos[b];
-    ++p.kv_len[b];
-  }
-  const bool all = __syncthreads_and(fin);  // every thread has read *p.step
-  if (b == 0) {
-    *p.step = t + 1;
-    *p.rng_offset += 1;
-    if (all && p.n_eos > 0 && *p.done_step < 0) *p.done_step = t;
-  }
-}
 
 // One CTA per (slot r, head h)
 __global__ void __launch_bounds__(2 * KV_ROW_VECS) kv_append_paged_kernel(const __nv_bfloat16* __restrict__ k_new,
@@ -398,34 +353,6 @@ extern "C" int aria_kv_scatter_tails(const void* k, const void* v, int64_t src_s
       static_cast<const __nv_bfloat16*>(k), static_cast<const __nv_bfloat16*>(v), src_stride_h, static_cast<__nv_bfloat16*>(tail_k),
       static_cast<__nv_bfloat16*>(tail_v), tail_stride_b, tail_stride_h, cu_seqlens, B, n, H, N_max);
   return check_launch("kv_scatter_tails_kernel");
-}
-
-extern "C" int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int64_t* out_tokens, int32_t max_steps, int32_t* step,
-                                   int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len, uint64_t* rng_offset, uint8_t* finished,
-                                   int32_t* done_step, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t B,
-                                   aria_stream_t stream_) {
-  ARIA_CHECK_ARG(next_ids && ids_in && out_tokens && step && rope_pos && write_pos && kv_len && rng_offset && finished && done_step);
-  ARIA_CHECK_ARG(B > 0 && B <= ADV_MAX_B && max_steps > 0);
-  ARIA_CHECK_ARG(n_eos >= 0 && n_eos <= ADV_MAX_EOS && (n_eos == 0 || eos_ids));
-  AdvanceParams p{};
-  p.next_ids = next_ids;
-  p.ids_in = ids_in;
-  p.out_tokens = out_tokens;
-  p.max_steps = max_steps;
-  p.step = step;
-  p.rope_pos = rope_pos;
-  p.write_pos = write_pos;
-  p.kv_len = kv_len;
-  p.rng_offset = rng_offset;
-  p.finished = finished;
-  p.done_step = done_step;
-  for (int e = 0; e < n_eos; ++e) p.eos[e] = eos_ids[e];  // host array, copied into the launch parameters
-  p.n_eos = n_eos;
-  p.pad = pad_token_id;
-  p.B = B;
-  const int threads = (B + 31) / 32 * 32;
-  decode_advance_kernel<<<1, threads, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
-  return check_launch("decode_advance_kernel");
 }
 
 extern "C" int aria_kv_append_paged(const void* k_new, const void* v_new, int64_t new_stride_b, int64_t new_stride_h, void* k_pool,

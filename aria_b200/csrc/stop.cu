@@ -1,9 +1,7 @@
 // Stop strings inside the captured decode step: Hugging Face's StopStringCriteria, run on each row's history right after the
 // decode advance has written the row's new token.
 //
-// aria_stop_check: generate()'s flavour; one stop set for every row, whose history is its prompt tail plus
-//   out_tokens[:, :*step]; the last row to stop sets done_step.
-// aria_stop_check_slots: the serving engine's flavour; every slot has its own stop set, stop ids, prompt tail and output row.
+// aria_stop_check_slots: every row has its own stop set, stop ids, prompt tail and output row.
 //
 // A row stops when its final token completes one of its stop strings S (L bytes) in HF's sense.  For every byte prefix T0[:m]
 // of the final token that ends with S's last min(m, L) bytes (m > L: S lies whole inside T0[:m], a match at once), the walk
@@ -79,55 +77,6 @@ __device__ bool warp_row_stops(const StopVocab& v, const uint8_t* S_all, const i
   return any;
 }
 
-struct StopParams {
-  StopVocab v;
-  const uint8_t* stop_bytes;  // [16, 512]
-  const int32_t* stop_lens;   // [16] bytes, 0 = no string
-  const int32_t* lookback;    // [1] tokens
-  const int64_t* tail;      // [B, 128]: row b's last tail_len[b] prompt ids, right-aligned
-  const int32_t* tail_len;  // [B]
-  const int64_t* out_tokens;  // [B, max_steps]
-  int32_t max_steps;
-  const int32_t* step;
-  uint8_t* finished;
-  int32_t* done_step;
-  int32_t* counter;         // 0 between launches
-  int32_t B;
-};
-
-__global__ void __launch_bounds__(STOP_WARPS * 32) stop_check_kernel(const StopParams p) {
-  __shared__ int s_off[STOP_WARPS][STOP_MAX_TOKENS], s_len[STOP_WARPS][STOP_MAX_TOKENS];
-  __shared__ bool s_last;
-  const int warp = threadIdx.x / 32;
-  const int b = blockIdx.x * STOP_WARPS + warp;
-  const int n_gen = min(*p.step, p.max_steps);
-  if (b < p.B && n_gen > 0 && !p.finished[b]) {
-    const int64_t* out = p.out_tokens + static_cast<int64_t>(b) * p.max_steps;
-    const int64_t* tail = p.tail + static_cast<int64_t>(b) * STOP_MAX_TOKENS;
-    const auto hist = [&](int j) -> int64_t { return j < n_gen ? out[n_gen - 1 - j] : tail[STOP_MAX_TOKENS - 1 - (j - n_gen)]; };
-    const int n_hist = n_gen + min(max(p.tail_len[b], 0), STOP_MAX_TOKENS);
-    if (warp_row_stops(p.v, p.stop_bytes, p.stop_lens, *p.lookback, n_hist, hist, s_off[warp], s_len[warp]) &&
-        threadIdx.x % 32 == 0)
-      p.finished[b] = 1;
-  }
-  // the last CTA to finish sees every row's flag: when they are all set, generation ends after this step
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    s_last = atomicAdd(p.counter, 1) == static_cast<int>(gridDim.x) - 1;
-  }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();  // acquire: the other CTAs' flags, released by their fence before the counter
-  bool fin = true;
-  for (int r = threadIdx.x; r < p.B; r += blockDim.x) fin &= __ldcg(p.finished + r) != 0;
-  const bool all = __syncthreads_and(fin);
-  if (threadIdx.x == 0) {
-    if (all && n_gen > 0 && *p.done_step < 0) *p.done_step = n_gen - 1;
-    *p.counter = 0;
-  }
-}
-
 struct SlotStopParams {
   StopVocab v;
   const uint8_t* stop_bytes;  // [R, 16, 512]
@@ -174,31 +123,6 @@ __global__ void __launch_bounds__(STOP_WARPS * 32) stop_check_slots_kernel(const
 }  // namespace aria
 
 using namespace aria;
-
-extern "C" int aria_stop_check(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
-                               const int32_t* stop_lens, const int32_t* lookback, const int64_t* prompt_tail,
-                               const int32_t* tail_len, const int64_t* out_tokens, int32_t max_steps, const int32_t* step,
-                               uint8_t* finished, int32_t* done_step, int32_t* counter, int32_t B, aria_stream_t stream_) {
-  ARIA_CHECK_ARG(vocab_bytes && vocab_offsets && stop_bytes && stop_lens && lookback && prompt_tail && tail_len && out_tokens);
-  ARIA_CHECK_ARG(step && finished && done_step && counter);
-  ARIA_CHECK_ARG(V > 0 && B > 0 && B <= STOP_MAX_ROWS && max_steps > 0);
-  StopParams p{};
-  p.v = {vocab_bytes, vocab_offsets, V};
-  p.stop_bytes = stop_bytes;
-  p.stop_lens = stop_lens;
-  p.lookback = lookback;
-  p.tail = prompt_tail;
-  p.tail_len = tail_len;
-  p.out_tokens = out_tokens;
-  p.max_steps = max_steps;
-  p.step = step;
-  p.finished = finished;
-  p.done_step = done_step;
-  p.counter = counter;
-  p.B = B;
-  stop_check_kernel<<<(B + STOP_WARPS - 1) / STOP_WARPS, STOP_WARPS * 32, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(p);
-  return check_launch("stop_check_kernel");
-}
 
 extern "C" int aria_stop_check_slots(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
                                      const int32_t* stop_lens, const int32_t* lookback, const int64_t* stop_ids,

@@ -16,7 +16,7 @@ import torch.nn as nn
 
 from . import ops, stopping
 from .ops import MAX_LOGPROBS
-from .moe_lm import KV_CACHE_DTYPES, AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16
+from .moe_lm import KV_CACHE_DTYPES, AriaMoELMConfig, AriaMoELMForCausalLM, KVCache, bf16, sample_and_advance, start_rows
 from .projector import AriaProjector
 from .vision_encoder import AriaVisionConfig, AriaVisionModel
 
@@ -392,7 +392,7 @@ class AriaForConditionalGeneration(nn.Module):
         keeps a bitmap of the ids it has seen (ops.presence_set), V / 8 bytes.  Logprobs stay those of the raw distribution.
         GPU only; not combined with prompt_lookup_num_tokens.  Without them, the captured step is the one above.
         stop_strings (a str or up to 16 of them, 1..128 characters each) with tokenizer: Hugging Face's StopStringCriteria,
-        checked inside the captured step after every token, the first one included (ops.stop_check, aria_b200.stopping).  A
+        checked inside the captured step after every token, the first one included (ops.stop_check_slots, aria_b200.stopping).  A
         row stops once the token it just emitted completes a string against the row's ids so far (left padding, image tokens
         and prompt included), as the tokenizer's cleaned vocabulary spells them; it is then finished exactly as after an EOS
         (the token is kept, pad_token_id follows, logprob filler), and min_new_tokens does not delay it.  A stopped row is
@@ -461,8 +461,7 @@ class AriaForConditionalGeneration(nn.Module):
         n, L = g.run(max_new_tokens, poll_every)
         if n_seq == 1:
             g.cache.seq_len = T + n             # a shared cache keeps the prompt's T; the tails hold the rest
-        prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
-        return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
+        return g.result(input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0), L)
 
     def _generate_shared_prefix(self, input_ids, ids, lens, pixel_values, pixel_mask, max_new_tokens, sampling, eos, pad,
                                 poll_every, n_seq, P, output_logprobs=None, processors=None, stops=None, table=None):
@@ -503,8 +502,7 @@ class AriaForConditionalGeneration(nn.Module):
             g.start_stops(stops, input_ids.repeat_interleave(n_seq, 0))
         g.sample_and_advance(first if n_seq == 1 else first.repeat_interleave(n_seq, 0))
         _, L = g.run(max_new_tokens, poll_every)
-        prompt = input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0)
-        return g.result(torch.cat([prompt.to(dev), g.out_tokens[:, :L]], dim=1), L)
+        return g.result(input_ids if n_seq == 1 else input_ids.repeat_interleave(n_seq, 0), L)
 
     def _generate_prompt_lookup(self, input_ids, pixel_values, pixel_mask, max_new_tokens, attention_mask, sampling, eos, pad,
                                 K, M):
@@ -726,37 +724,38 @@ class GenerateOutput(NamedTuple):
 class GraphedDecode:
     """One decode step captured as a CUDA graph and replayed token after token (AriaForConditionalGeneration.generate).
 
-    The step is embedding -> every layer (AriaMoELMForCausalLM.decode_step) -> norm -> lm_head -> sample_tokens ->
-    decode_advance.  Nothing in it is a host integer: the step's input ids, RoPE positions, cache rows and key counts
-    (`state`), the RNG offset, the finished flags, the step index and the output tokens all live in static device buffers,
-    and decode_advance moves them on at the end of every replay.  The KV cache belongs to the graph: generate() prefills
-    into it with forward(past_key_values=g.cache), then calls start() and sample_and_advance() for the first token.
-    `logits` is the last replayed step's logits [B, 1, V].
+    The step is embedding -> every layer (AriaMoELMForCausalLM.decode_step) -> norm -> lm_head -> moe_lm.sample_and_advance,
+    the serving engine's step tail: a batch of generate() is a set of rows that all start together and share parameters.
+    Nothing in it is a host integer: every row's input id, RoPE position, cache rows and key count, its sampling parameters,
+    RNG offset, output count, finished flag and output tokens live in static device buffers on `state` (moe_lm.add_token_fields),
+    and the advance moves an unfinished row on at the end of every replay.  Row r draws the Philox noise of row r at offset
+    n_out[r], as sample_tokens does for row r of the batch; the rows share `sampling`, so the sampler takes it as scalars.
+    The KV cache belongs to the graph: generate() prefills into it with forward(past_key_values=g.cache), then calls start()
+    and sample_and_advance() for the first token.  `logits` is the last replayed step's logits [B, 1, V].
     group_size n > 1: B prompts decoded n times each.  The cache is a SharedPrefixCache of B prompt rows of T_max (the prompt
     bucket) and B * n tails of max_new_tokens rounded up to 256; the state, tokens and logits have B * n rows.
     N_max (generate(shared_prefix_len=...)): a SharedPrefixCache whose tails hold N_max rows (a multiple of 256), each row's
     own prompt tokens and then its generated ones, for any group size.
-    logprobs k (generate(output_logprobs=k)): the step also runs ops.token_logprobs on the sampled tokens between the sampler and
-    the advance, into column `step` of lp [B, max_new_tokens], top_ids and top_lp [B, max_new_tokens, k]; rows finished before
-    the step get the filler.  None: the step is exactly the one without logprobs.
-    processors (penalty, min_p, min_new_tokens) (generate(repetition_penalty=..., min_p=..., min_new_tokens=...)): the sampler is
-    ops.sample_tokens_processed, which reads each row's presence bitmap [B, V / 32] (start_presence) and counts its emitted
-    tokens by `step`, and the advance is followed by ops.presence_set of the tokens it wrote to `ids`.  generate() rebuilds the
-    graph when they change, as it does for logprobs.  None: the step is exactly the one without them.
-    stop (generate(stop_strings=..., tokenizer=...)): the tokenizer's stopping.StopVocab; the advance is followed by
-    ops.stop_check on static buffers, the stop set and each row's prompt tail, that start_stops() rewrites, so one capture
-    serves every set of strings.  None: the step is exactly the one without it."""
+    logprobs k (generate(output_logprobs=k)): the step also writes each token's logprobs into rings of max_new_tokens entries,
+    k wide, so entry n_out of every row; start() fills them with the filler (0, -1, -inf) that finished rows keep.
+    processors (penalty, min_p, min_new_tokens) (generate(repetition_penalty=..., min_p=..., min_new_tokens=...)): the step
+    samples through them on each row's presence bitmap (start_presence).  generate() rebuilds the graph when they change, as it
+    does for logprobs.
+    stop (generate(stop_strings=..., tokenizer=...)): the tokenizer's stopping.StopVocab; the step checks every row's stop set
+    and prompt tail, which start_stops() rewrites, so one capture serves every set of strings.
+    Without logprobs, processors or stop, the step runs none of their kernels."""
 
     def __init__(self, model: "AriaForConditionalGeneration", B: int, T_max: int, max_new_tokens: int, sampling, eos, pad,
                  kv_cache_dtype: str = "bf16", group_size: int = 1, N_max: Optional[int] = None, logprobs: Optional[int] = None,
                  processors: Optional[tuple] = None, stop: Optional[stopping.StopVocab] = None):
-        from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache
+        from .moe_lm import DecodeState, SharedDecodeState, SharedPrefixCache, add_token_fields
         dev = model.device
         lm = model.language_model
         c = lm.config
         self.key = (B, T_max, max_new_tokens, sampling, eos, pad, dev, group_size, N_max, kv_cache_dtype)
         self.group_size = group_size
         self.T_max = T_max
+        self.max_new = max_new_tokens
         self.sampling, self.eos, self.pad = sampling, eos, pad
         if group_size == 1 and N_max is None:
             self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
@@ -771,41 +770,14 @@ class GraphedDecode:
             B = B * group_size
         self.model, self.B = model, B
         self.rope = lm.model.rope_tables(n_pos, dev)   # held here: the graph reads these tables
-        self.ids = torch.zeros(B, 1, dtype=torch.int64, device=dev)
-        self.next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
-        self.rng_offset = torch.zeros(1, dtype=torch.int64, device=dev)   # read as uint64 by the kernels
-        self.step = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.done_step = torch.full((1,), -1, dtype=torch.int32, device=dev)
-        self.finished = torch.zeros(B, dtype=torch.uint8, device=dev)
-        self.out_tokens = torch.zeros(B, max_new_tokens, dtype=torch.int64, device=dev)
-        self.n_logprobs = logprobs
-        if logprobs is not None:
-            self.lp = torch.zeros(B, max_new_tokens, dtype=torch.float32, device=dev)
-            self.top_ids = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.int32, device=dev)
-            self.top_lp = torch.zeros(B, max_new_tokens, logprobs, dtype=torch.float32, device=dev)
-        self.processors = processors
-        if processors is not None:
-            t, k, p, seed = sampling
-            penalty, min_p, min_new = processors
-            f32, i32 = dict(dtype=torch.float32, device=dev), dict(dtype=torch.int32, device=dev)
-            # per-row arrays of the processed sampler, in its argument order: temperature, top_k, top_p, min_p, seed, penalty,
-            # min_new_tokens
-            self.proc_rows = (torch.full((B,), t, **f32), torch.full((B,), k, **i32), torch.full((B,), p, **f32),
-                              torch.full((B,), min_p, **f32),
-                              torch.full((B,), seed - 2 ** 64 if seed >= 2 ** 63 else seed, dtype=torch.int64, device=dev),
-                              torch.full((B,), penalty, **f32), torch.full((B,), min_new, **i32))
-            self.V = c.vocab_size
-            self.presence = torch.zeros(B, ops.presence_words(self.V), **i32)
-        self.stop = stop
-        if stop is not None:
-            self.stop_vocab = stop.device(dev)
-            self.stop_bytes = torch.zeros(stopping.MAX_STRINGS, stopping.MAX_BYTES, dtype=torch.uint8, device=dev)
-            self.stop_lens = torch.zeros(stopping.MAX_STRINGS, dtype=torch.int32, device=dev)
-            self.stop_lookback = torch.zeros(1, dtype=torch.int32, device=dev)
-            self.stop_tail = torch.zeros(B, stopping.TAIL, dtype=torch.int64, device=dev)
-            self.stop_tail_len = torch.zeros(B, dtype=torch.int32, device=dev)
-            self.stop_counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.done_host = torch.full((1,), -1, dtype=torch.int32).pin_memory()
+        self.n_logprobs, self.processors, self.stop = logprobs, processors, stop
+        self.V = c.vocab_size
+        st = self.state
+        add_token_fields(st, B, max_new_tokens, dev, lp_ring=1 if logprobs is None else max_new_tokens, lp_width=logprobs or 0,
+                         vocab=1 if processors is None else self.V, stops=stop is not None)
+        st.noise_row.copy_(torch.arange(B, dtype=torch.int32))
+        self.stop_vocab = None if stop is None else stop.device(dev)
+        self.fin_host = torch.ones(B, dtype=torch.uint8).pin_memory()
         self.event = torch.cuda.Event()
         self.dev = dev
         cur = torch.cuda.current_stream(dev)
@@ -820,51 +792,41 @@ class GraphedDecode:
 
     def _step(self):
         lm = self.model.language_model
-        emb = ops.embedding(self.ids, lm.get_input_embeddings().weight)
+        emb = ops.embedding(self.state.ids_in, lm.get_input_embeddings().weight)
         logits = lm.decode_step(emb, self.cache, self.state, self.rope)
         self.sample_and_advance(logits[:, -1])
         return logits
 
     def sample_and_advance(self, logits: torch.Tensor):
-        """Sample from logits [B, V] into next_ids, then advance the state (also the eager first token after the prefill)."""
-        t, k, p, seed = self.sampling
-        if self.processors is None:
-            ops.sample_tokens(logits, t, k, p, seed, self.rng_offset, out=self.next_ids)
-        else:
-            ops.sample_tokens_processed(logits, *self.proc_rows, self.presence, self.rng_offset, self.step, self.eos,
-                                        out=self.next_ids)
-        if self.n_logprobs is not None:
-            ops.token_logprobs(logits, self.next_ids, self.n_logprobs, col=self.step, finished=self.finished,
-                               out=(self.lp, self.top_ids, self.top_lp))
-        st = self.state
-        ops.decode_advance(self.next_ids, self.ids, self.out_tokens, self.step, st.rope_pos, st.write_pos, st.kv_len,
-                           self.rng_offset, self.finished, self.done_step, self.eos, self.pad)
-        if self.processors is not None:
-            ops.presence_set(self.ids, self.presence, self.V)
-        if self.stop is not None:
-            ops.stop_check(*self.stop_vocab, self.stop_bytes, self.stop_lens, self.stop_lookback, self.stop_tail,
-                           self.stop_tail_len, self.out_tokens, self.step, self.finished, self.done_step, self.stop_counter)
-        self.done_host.copy_(self.done_step, non_blocking=True)
+        """Sample from logits [B, V] and advance the state (also the eager first token after the prefill)."""
+        sample_and_advance(self.state, logits, self.eos, self.pad, self.stop_vocab, self.n_logprobs is not None,
+                           self.processors is not None, self.stop is not None, self.sampling)
+        self.fin_host.copy_(self.state.finished, non_blocking=True)
 
     def start_presence(self, ids: torch.Tensor):
         """Every row's presence bitmap from its ids [B, T] on the device (the prompt as the row has it, padding included)."""
-        ops.presence_set(ids, self.presence, self.V, clear=True)
+        ops.presence_set(ids, self.state.presence, self.V, clear=True)
 
     def start_stops(self, strings, ids: torch.Tensor):
-        """The stop set of strings, and every row's prompt tail from its ids [B, T] (as the row has them, padding included)."""
+        """Every row's stop set of strings, and its prompt tail from its ids [B, T] (as the row has them, padding included)."""
         data, lens, lookback = stopping.encode_stop_set(strings)
         tail, n = stopping.prompt_tail(ids)
-        self.stop_bytes.copy_(data)
-        self.stop_lens.copy_(lens)
-        self.stop_lookback.fill_(lookback)
-        self.stop_tail.copy_(tail)
-        self.stop_tail_len.fill_(n)
+        st = self.state
+        st.stop_bytes.copy_(data)          # broadcast to every row
+        st.stop_lens.copy_(lens)
+        st.stop_lookback.fill_(lookback)
+        st.stop_tail.copy_(tail)
+        st.stop_tail_len.fill_(n)
 
-    def result(self, sequences: torch.Tensor, L: int):
-        """generate()'s return value: sequences alone, or with logprobs a GenerateOutput of the first L columns."""
+    def result(self, prompt: torch.Tensor, L: int):
+        """generate()'s return value: the prompt ids [B, T] then the first L generated tokens of every row, with logprobs a
+        GenerateOutput of the first L columns."""
+        st = self.state
+        sequences = torch.cat([prompt.to(self.dev), st.out_tokens[:, :L].to(torch.int64)], dim=1)
         if self.n_logprobs is None:
             return sequences
-        return GenerateOutput(sequences, self.lp[:, :L].clone(), self.top_ids[:, :L].to(torch.int64), self.top_lp[:, :L].clone())
+        return GenerateOutput(sequences, st.lp_ring_lp[:, :L].clone(), st.lp_ring_ids[:, :L].to(torch.int64),
+                              st.lp_ring_top[:, :L].clone())
 
     def start(self, T: int, mask: Optional[torch.Tensor]):
         """Reset the state for a prompt of T tokens (mask: host [B, T] padding mask or None) already prefilled into
@@ -906,15 +868,19 @@ class GraphedDecode:
         self._reset()
 
     def _reset(self):
-        self.rng_offset.zero_()
-        self.step.zero_()
-        self.done_step.fill_(-1)
-        self.finished.zero_()
-        self.done_host.fill_(-1)
+        """Every row starts its token stream; a row that finishes keeps the pad tokens and logprob filler written here."""
+        st = self.state
+        start_rows(st, slice(None), self.sampling, self.max_new, self.n_logprobs, self.processors)
+        st.out_tokens.fill_(self.pad)
+        st.lp_ring_lp.zero_()
+        st.lp_ring_ids.fill_(-1)
+        st.lp_ring_top.fill_(float("-inf"))
+        self.fin_host.zero_()
 
     def run(self, max_new_tokens: int, poll_every: int):
         """Replay the step until max_new_tokens tokens are out (the first one is sampled before) or, with EOS ids or stop
-        strings, every row has finished; the host polls every poll_every steps.  -> (steps replayed, tokens to keep per row)."""
+        strings, every row has finished; the host polls every poll_every steps.  -> (steps replayed, tokens to keep per row:
+        the longest row, as every row has finished by then, at an EOS id, a stop string or its budget)."""
         n = 0
         poll = bool(self.eos) or self.stop is not None
         while n < max_new_tokens - 1:
@@ -922,14 +888,13 @@ class GraphedDecode:
                 break
             self.graph.replay()
             n += 1
-        done = int(self.done_step.item())       # synchronises; -1 when no EOS or stop string stopped the batch
-        return n, (done + 1 if done >= 0 else max_new_tokens)
+        return n, int(self.state.n_out.max())       # synchronises
 
     def done(self) -> bool:
-        """Whether every row has finished, from the pinned copy of done_step (waits for the work queued so far)."""
+        """Whether every row has finished, from the pinned copy of the finished flags (waits for the work queued so far)."""
         self.event.record(torch.cuda.current_stream(self.dev))
         self.event.synchronize()
-        return int(self.done_host[0]) >= 0
+        return bool(self.fin_host.all())
 
 
 class GraphedLookupDecode:

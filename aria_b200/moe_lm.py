@@ -488,7 +488,8 @@ class DecodeState:
     """Device-resident positions of a decode step that is captured once and replayed token after token
     (modeling_aria.GraphedDecode): nothing in the step reads `KVCache.seq_len` or any other host integer.
     The step's token has RoPE position rope_pos[b], its k/v land in cache row write_pos[b], and it attends to cache rows
-    [0, kv_len[b]) minus the padded prompt keys of key_mask (1 = masked out).  aria_decode_advance moves all three on."""
+    [0, kv_len[b]) minus the padded prompt keys of key_mask (1 = masked out).  The advance at the end of the step
+    (sample_and_advance) moves all three on for every row that has not finished."""
 
     def __init__(self, B, H, T_max, device):
         i32 = dict(dtype=torch.int32, device=device)
@@ -581,51 +582,111 @@ class PagedKVCache:
         return None, None
 
 
+def add_token_fields(st, R, max_out, device, lp_ring: int = 1, lp_width: int = ops.MAX_LOGPROBS, vocab: int = 1,
+                     stops: bool = True):
+    """Put on st (a DecodeState of R rows) what each row's token stream needs on the device, for sample_and_advance: its
+    sampling parameters (temperature, 0 = greedy; top_k; top_p; seed; noise row; RNG offset), its token budget max_new, the
+    count n_out and the tokens out_tokens [R, max_out] (int32) it has emitted, its finished flag (set: the row is idle until
+    start_rows), and the step's input ids_in [R, 1] and sampled next_ids.
+    Log-probabilities: lp_n, the row's top-n (-1: none), and rings of lp_ring entries that the step writes at n_out mod
+    lp_ring: lp_ring_lp [R, lp_ring] fp32, lp_ring_ids [R, lp_ring, lp_width] int32 and lp_ring_top [R, lp_ring, lp_width] fp32.
+    Logits processors: the row's rep_penalty (1: off), min_p (0: off) and min_new, and presence [R, ceil(vocab / 32)] int32,
+    the bitmap of the ids the row has seen.
+    Stops (only with stops): the row's stop set stop_bytes [R, 16, 512] uint8, stop_lens [R, 16] int32 and stop_lookback (0:
+    no strings), its stop ids stop_ids [R, 8] int64 (the first n_stop_ids), and its prompt tail stop_tail [R, 128] int64, the
+    last stop_tail_len ids right-aligned (ops.stop_check_slots)."""
+    i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
+    f32 = dict(dtype=torch.float32, device=device)
+    st.temperature = torch.zeros(R, **f32)
+    st.top_k = torch.zeros(R, **i32)
+    st.top_p = torch.ones(R, **f32)
+    st.seed = torch.zeros(R, **i64)
+    st.noise_row = torch.zeros(R, **i32)
+    st.rng_offset = torch.zeros(R, **i64)
+    st.max_new = torch.ones(R, **i32)
+    st.n_out = torch.zeros(R, **i32)
+    st.finished = torch.ones(R, dtype=torch.uint8, device=device)
+    st.ids_in = torch.zeros(R, 1, **i64)
+    st.next_ids = torch.zeros(R, **i64)
+    st.out_tokens = torch.zeros(R, max_out, **i32)
+    st.lp_n = torch.full((R,), -1, **i32)
+    st.lp_ring_lp = torch.zeros(R, lp_ring, **f32)
+    st.lp_ring_ids = torch.zeros(R, lp_ring, lp_width, **i32)
+    st.lp_ring_top = torch.zeros(R, lp_ring, lp_width, **f32)
+    st.rep_penalty = torch.ones(R, **f32)
+    st.min_p = torch.zeros(R, **f32)
+    st.min_new = torch.zeros(R, **i32)
+    st.presence = torch.zeros(R, ops.presence_words(vocab), **i32)
+    if stops:
+        st.stop_bytes = torch.zeros(R, ops.STOP_MAX_STRINGS, ops.STOP_MAX_BYTES, dtype=torch.uint8, device=device)
+        st.stop_lens = torch.zeros(R, ops.STOP_MAX_STRINGS, **i32)
+        st.stop_lookback = torch.zeros(R, **i32)
+        st.stop_ids = torch.zeros(R, ops.STOP_MAX_IDS, **i64)
+        st.n_stop_ids = torch.zeros(R, **i32)
+        st.stop_tail = torch.zeros(R, ops.STOP_MAX_TOKENS, **i64)
+        st.stop_tail_len = torch.zeros(R, **i32)
+
+
+def start_rows(st, rows, sampling, max_new: int, logprobs: Optional[int] = None, processors: Optional[tuple] = None):
+    """Start the token streams of rows (an index or a slice of st's rows): sampling (temperature, top_k, top_p, seed), the
+    budget max_new, logprobs (None or the top-n) and processors (None or (repetition_penalty, min_p, min_new_tokens)); no token
+    out, RNG offset 0, not finished.  The noise row, the output row and the stops are the caller's."""
+    t, k, p, seed = sampling
+    st.temperature[rows] = t
+    st.top_k[rows] = k
+    st.top_p[rows] = p
+    st.seed[rows] = seed - 2 ** 64 if seed >= 2 ** 63 else seed    # int64 storage of the uint64 seed
+    st.rng_offset[rows] = 0
+    st.max_new[rows] = max_new
+    st.n_out[rows] = 0
+    st.finished[rows] = 0
+    st.lp_n[rows] = -1 if logprobs is None else logprobs
+    pen, min_p, min_new = (1.0, 0.0, 0) if processors is None else processors
+    st.rep_penalty[rows] = pen
+    st.min_p[rows] = min_p
+    st.min_new[rows] = min_new
+
+
+def sample_and_advance(st, logits, eos, pad: int, stop_vocab=None, logprobs: bool = False, processors: bool = False,
+                       stops: bool = False, sampling: Optional[tuple] = None) -> None:
+    """The tail of a decode step on the per-row token state st (add_token_fields), logits [R, V] -> next token of every row:
+    sample (with processors, through each row's logits processors; row r draws the Philox noise of row noise_row[r] at offset
+    rng_offset[r]; sampling: (temperature, top_k, top_p, seed) when every row has these, which the sampler then takes as
+    launch arguments instead of loading the row's own, the same token either way), then with logprobs the logprobs of the rows with lp_n >= 0 into ring entry n_out mod lp_ring (finished rows
+    untouched), then advance (ops.decode_advance_slots: an unfinished row records its token, finishes on an EOS id or its
+    budget, and moves on; a finished row keeps its positions and is fed pad); with processors, each row's new input id then
+    joins its presence bitmap; with stops, each row's stop ids and strings are checked against its new token (stop_vocab: the
+    device vocabulary table, stopping.StopVocab.device).  eos: the EOS ids (at most 8); pad: what a finished row is fed."""
+    if processors:
+        ops.sample_tokens_processed(logits, st.temperature, st.top_k, st.top_p, st.min_p, st.seed, st.rep_penalty, st.min_new,
+                                    st.presence, st.rng_offset, st.n_out, eos, noise_rows=st.noise_row, out=st.next_ids)
+    elif sampling is not None:
+        ops.sample_tokens_rows(logits, *sampling, st.noise_row, st.rng_offset, out=st.next_ids)
+    else:
+        ops.sample_tokens_slots(logits, st.temperature, st.top_k, st.top_p, st.seed, st.noise_row, st.rng_offset,
+                                out=st.next_ids)
+    if logprobs:
+        ops.token_logprobs(logits, st.next_ids, st.lp_ring_ids.shape[-1], n_row=st.lp_n, col=st.n_out,
+                           ring=st.lp_ring_lp.shape[1], finished=st.finished, finished_fill=False,
+                           out=(st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top))
+    ops.decode_advance_slots(st.next_ids, st.ids_in, st.out_tokens, st.n_out, st.max_new, st.rope_pos, st.write_pos, st.kv_len,
+                             st.rng_offset, st.finished, eos, pad)
+    if processors:
+        ops.presence_set(st.ids_in, st.presence, logits.shape[-1])
+    if stops:
+        ops.stop_check_slots(*stop_vocab, st.stop_bytes, st.stop_lens, st.stop_lookback, st.stop_ids, st.n_stop_ids,
+                             st.stop_tail, st.stop_tail_len, st.out_tokens, st.n_out, st.finished, st.ids_in, pad)
+
+
 class SlotDecodeState(DecodeState):
-    """DecodeState of continuous batching: one row per engine slot, max_batch rows, and what each slot's request needs on the
-    device: its sampling parameters (temperature, 0 = greedy; top_k; top_p; seed; noise row; RNG offset), its token budget
-    max_new, the count n_out and the tokens out_tokens [max_batch, max_out] (int32) it has emitted, its finished flag, and the
-    step's input ids_in and sampled next_ids.  A decode step over the first n slots reads rows(n); the other slots are idle.
-    Log-probabilities (serving.Engine's logprobs): lp_n, the slot's top-n (-1: none), and rings of lp_ring entries that the step
-    writes at n_out mod lp_ring: lp_ring_lp [max_batch, lp_ring] fp32, lp_ring_ids [max_batch, lp_ring, 20] int32 and
-    lp_ring_top [max_batch, lp_ring, 20] fp32.
-    Logits processors (serving.Engine's repetition_penalty, min_p, min_new_tokens): the slot's rep_penalty (1: off), min_p (0:
-    off) and min_new, and presence [max_batch, ceil(vocab / 32)] int32, the bitmap of the ids its request has seen.
-    Stops (serving.Engine's stop_strings, stop_token_ids): the slot's stop set stop_bytes [max_batch, 16, 512] uint8, stop_lens
-    [max_batch, 16] int32 and stop_lookback (0: no strings), its stop ids stop_ids [max_batch, 8] int64 (the first n_stop_ids),
-    and its prompt tail stop_tail [max_batch, 128] int64, the last stop_tail_len ids right-aligned (ops.stop_check_slots)."""
+    """DecodeState of continuous batching: one row per engine slot, max_batch rows, each with the token fields of
+    add_token_fields (logprob rings of lp_ring entries, 20 wide; presence bitmaps over vocab ids; stops).  A decode step over
+    the first n slots reads rows(n); the other slots are idle."""
 
     def __init__(self, max_batch, H, max_out, device, lp_ring: int = 1, vocab: int = 1):
         super().__init__(max_batch, H, 0, device)
         self.key_mask = None
-        i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
-        self.temperature = torch.zeros(max_batch, dtype=torch.float32, device=device)
-        self.top_k = torch.zeros(max_batch, **i32)
-        self.top_p = torch.ones(max_batch, dtype=torch.float32, device=device)
-        self.seed = torch.zeros(max_batch, **i64)
-        self.noise_row = torch.zeros(max_batch, **i32)
-        self.rng_offset = torch.zeros(max_batch, **i64)
-        self.max_new = torch.ones(max_batch, **i32)
-        self.n_out = torch.zeros(max_batch, **i32)
-        self.finished = torch.ones(max_batch, dtype=torch.uint8, device=device)
-        self.ids_in = torch.zeros(max_batch, 1, **i64)
-        self.next_ids = torch.zeros(max_batch, **i64)
-        self.out_tokens = torch.zeros(max_batch, max_out, **i32)
-        self.lp_n = torch.full((max_batch,), -1, **i32)
-        self.lp_ring_lp = torch.zeros(max_batch, lp_ring, dtype=torch.float32, device=device)
-        self.lp_ring_ids = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, **i32)
-        self.lp_ring_top = torch.zeros(max_batch, lp_ring, ops.MAX_LOGPROBS, dtype=torch.float32, device=device)
-        self.rep_penalty = torch.ones(max_batch, dtype=torch.float32, device=device)
-        self.min_p = torch.zeros(max_batch, dtype=torch.float32, device=device)
-        self.min_new = torch.zeros(max_batch, **i32)
-        self.presence = torch.zeros(max_batch, ops.presence_words(vocab), **i32)
-        self.stop_bytes = torch.zeros(max_batch, ops.STOP_MAX_STRINGS, ops.STOP_MAX_BYTES, dtype=torch.uint8, device=device)
-        self.stop_lens = torch.zeros(max_batch, ops.STOP_MAX_STRINGS, **i32)
-        self.stop_lookback = torch.zeros(max_batch, **i32)
-        self.stop_ids = torch.zeros(max_batch, ops.STOP_MAX_IDS, **i64)
-        self.n_stop_ids = torch.zeros(max_batch, **i32)
-        self.stop_tail = torch.zeros(max_batch, ops.STOP_MAX_TOKENS, **i64)
-        self.stop_tail_len = torch.zeros(max_batch, **i32)
+        add_token_fields(self, max_batch, max_out, device, lp_ring, vocab=vocab)
 
     # the per-slot arrays, in the order a slot's row is copied when slots are compacted
     SLOT_FIELDS = ("rope_pos", "write_pos", "kv_len", "temperature", "top_k", "top_p", "seed", "noise_row", "rng_offset",

@@ -1360,27 +1360,6 @@ def kv_load_fp8(k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Ten
                                           k_out.stride(1), n, B, H, T_max, _stream(k_cache)), "kv_load_fp8")
 
 
-def decode_advance(next_ids: torch.Tensor, ids_in: torch.Tensor, out_tokens: torch.Tensor, step: torch.Tensor,
-                   rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor, rng_offset: torch.Tensor,
-                   finished: torch.Tensor, done_step: torch.Tensor, eos_token_ids: Sequence[int] = (), pad_token_id: int = 0):
-    """One launch after sample_tokens: out_tokens[:, step] <- next_ids (pad for finished rows), ids_in <- the same tokens,
-    EOS bookkeeping (finished, done_step), positions / step / rng offset + 1.  Every argument is a device tensor; the EOS ids
-    (at most 8) and the pad id are baked into the launch.  See aria_decode_advance."""
-    B = next_ids.numel()
-    for t, dt in ((next_ids, torch.int64), (ids_in, torch.int64), (out_tokens, torch.int64), (step, torch.int32),
-                  (rope_pos, torch.int32), (write_pos, torch.int32), (kv_len, torch.int32), (rng_offset, torch.int64),
-                  (finished, torch.uint8), (done_step, torch.int32)):
-        _chk(t, dt, align=1)
-    assert ids_in.numel() == B and out_tokens.shape[0] == B and finished.numel() == B and rope_pos.numel() == B
-    eos = list(eos_token_ids)
-    arr = (C.c_int64 * max(1, len(eos)))(*eos)
-    with torch.cuda.device(next_ids.device):
-        L.check(L.load().aria_decode_advance(_p(next_ids), _p(ids_in), _p(out_tokens), out_tokens.shape[1], _p(step), _p(rope_pos),
-                                             _p(write_pos), _p(kv_len), _p(rng_offset), _p(finished), _p(done_step),
-                                             C.cast(arr, C.c_void_p), len(eos), int(pad_token_id), B, _stream(next_ids)),
-                "decode_advance")
-
-
 # ------------------------------------------------------------------------------------------- continuous batching (paged KV cache)
 def _paged_pool_check(k_pool: torch.Tensor, v_pool: torch.Tensor, what: str):
     """Page pools k_pool / v_pool: CUDA bf16 [n_pages, H, 256, 128], contiguous and sharing one shape."""
@@ -1817,9 +1796,10 @@ def decode_advance_slots(next_ids: torch.Tensor, ids_in: torch.Tensor, out_token
                          max_new: torch.Tensor, rope_pos: torch.Tensor, write_pos: torch.Tensor, kv_len: torch.Tensor,
                          rng_offset: torch.Tensor, finished: torch.Tensor, eos_token_ids: Sequence[int] = (),
                          pad_token_id: int = 0):
-    """decode_advance per slot, R = next_ids.numel() slots: an unfinished slot stores its token at out_tokens[r, n_out[r]]
-    (int32 [R, L]), finishes on an EOS id or at max_new[r] tokens, and moves n_out, its positions and its rng_offset (int64, read
-    as uint64) on by one; a finished slot changes nothing.  See aria_decode_advance_slots."""
+    """One launch after the sampler, R = next_ids.numel() rows: an unfinished row stores its token at out_tokens[r, n_out[r]]
+    (int32 [R, L]) and feeds it back as ids_in[r], finishes on an EOS id (at most 8, baked into the launch) or at max_new[r]
+    tokens (then ids_in[r] = pad_token_id), and moves n_out, its positions and its rng_offset (int64, read as uint64) on by one;
+    a finished row changes nothing.  See aria_decode_advance_slots."""
     R = next_ids.numel()
     for t, dt in ((next_ids, torch.int64), (ids_in, torch.int64), (out_tokens, torch.int32), (n_out, torch.int32),
                   (max_new, torch.int32), (rope_pos, torch.int32), (write_pos, torch.int32), (kv_len, torch.int32),
@@ -1840,40 +1820,16 @@ def decode_advance_slots(next_ids: torch.Tensor, ids_in: torch.Tensor, out_token
 STOP_MAX_STRINGS, STOP_MAX_BYTES, STOP_MAX_TOKENS, STOP_MAX_IDS = 16, 512, 128, 8
 
 
-def stop_check(vocab_bytes: torch.Tensor, vocab_offsets: torch.Tensor, stop_bytes: torch.Tensor, stop_lens: torch.Tensor,
-               lookback: torch.Tensor, prompt_tail: torch.Tensor, tail_len: torch.Tensor, out_tokens: torch.Tensor,
-               step: torch.Tensor, finished: torch.Tensor, done_step: torch.Tensor, counter: torch.Tensor):
-    """Hugging Face's StopStringCriteria on B rows, after decode_advance: a row that is not finished and whose history
-    (prompt_tail int64 [B, 128], its last tail_len[b] ids right-aligned, then out_tokens[b, :step]) ends by completing one of
-    the stop set's strings gets finished[b] = 1; when that leaves every row finished, done_step = step - 1 (if still < 0).
-    The vocabulary table: uint8 bytes and int32 offsets [V + 1] (stopping.StopVocab); the stop set: uint8 [16, 512], int32
-    byte lengths [16] and int32 lookback [1] (stopping.encode_stop_set).  counter: int32 [1], zero.  See aria_stop_check."""
-    B = finished.numel()
-    for t, dt in ((vocab_bytes, torch.uint8), (vocab_offsets, torch.int32), (stop_bytes, torch.uint8), (stop_lens, torch.int32),
-                  (lookback, torch.int32), (prompt_tail, torch.int64), (tail_len, torch.int32), (out_tokens, torch.int64),
-                  (step, torch.int32), (finished, torch.uint8), (done_step, torch.int32), (counter, torch.int32)):
-        _chk(t, dt, align=1)
-    if vocab_offsets.dim() != 1 or vocab_offsets.numel() < 2:
-        raise ValueError(f"stop_check: vocab_offsets must be [V + 1] with V >= 1, got {tuple(vocab_offsets.shape)}")
-    if stop_bytes.shape != (STOP_MAX_STRINGS, STOP_MAX_BYTES) or stop_lens.shape != (STOP_MAX_STRINGS,) or lookback.numel() != 1:
-        raise ValueError("stop_check: the stop set must be [16, 512], [16] and [1]")
-    if prompt_tail.shape != (B, STOP_MAX_TOKENS) or tail_len.shape != (B,) or out_tokens.dim() != 2 or out_tokens.shape[0] != B:
-        raise ValueError(f"stop_check: prompt_tail [{B}, 128], tail_len [{B}] and out_tokens [{B}, L] expected")
-    with torch.cuda.device(finished.device):
-        L.check(L.load().aria_stop_check(_p(vocab_bytes), _p(vocab_offsets), vocab_offsets.numel() - 1, _p(stop_bytes),
-                                         _p(stop_lens), _p(lookback), _p(prompt_tail), _p(tail_len), _p(out_tokens),
-                                         out_tokens.shape[1], _p(step), _p(finished), _p(done_step), _p(counter), B,
-                                         _stream(finished)), "stop_check")
-
-
 def stop_check_slots(vocab_bytes: torch.Tensor, vocab_offsets: torch.Tensor, stop_bytes: torch.Tensor, stop_lens: torch.Tensor,
                      lookback: torch.Tensor, stop_ids: torch.Tensor, n_stop_ids: torch.Tensor, prompt_tail: torch.Tensor,
                      tail_len: torch.Tensor, out_tokens: torch.Tensor, n_out: torch.Tensor, finished: torch.Tensor,
                      ids_in: torch.Tensor, pad_token_id: int):
-    """stop_check per slot, after decode_advance_slots: slot r has its own stop set (stop_bytes uint8 [R, 16, 512], stop_lens
-    int32 [R, 16], lookback int32 [R], 0 = no strings) and its own stop ids (stop_ids int64 [R, 8], the first n_stop_ids[r]);
-    its history is its prompt tail (int64 [R, 128], tail_len [R]), then out_tokens[r, :n_out[r]] (int32).  A slot that is not
-    finished and stops gets finished[r] = 1 and ids_in[r] = pad_token_id.  See aria_stop_check_slots."""
+    """Hugging Face's StopStringCriteria on R rows, after decode_advance_slots: row r has its own stop set (stop_bytes uint8
+    [R, 16, 512], stop_lens int32 [R, 16], lookback int32 [R], 0 = no strings; stopping.encode_stop_set) and its own stop ids
+    (stop_ids int64 [R, 8], the first n_stop_ids[r]); its history is its prompt tail (int64 [R, 128], its last tail_len[r] ids
+    right-aligned), then out_tokens[r, :n_out[r]] (int32).  The vocabulary table: uint8 bytes and int32 offsets [V + 1]
+    (stopping.StopVocab).  A row that is not finished and stops gets finished[r] = 1 and ids_in[r] = pad_token_id.  See
+    aria_stop_check_slots."""
     R = finished.numel()
     for t, dt in ((vocab_bytes, torch.uint8), (vocab_offsets, torch.int32), (stop_bytes, torch.uint8), (stop_lens, torch.int32),
                   (lookback, torch.int32), (stop_ids, torch.int64), (n_stop_ids, torch.int32), (prompt_tail, torch.int64),

@@ -67,6 +67,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import ops, stopping
+from .moe_lm import sample_and_advance, start_rows
 from .ops import MAX_LOGPROBS
 
 PAGE = 256
@@ -654,30 +655,9 @@ class Engine:
         st = self.state.rows(n)
         emb = ops.embedding(st.ids_in, lm.get_input_embeddings().weight)
         logits = lm.decode_step(emb, self.cache, st, self.rope)
-        self._sample_and_advance(st, logits[:, -1], lp, proc, stop)
+        sample_and_advance(st, logits[:, -1], self.eos, self.pad, self.stop_vocab, lp, proc, stop)
         self._fin_host.copy_(self.state.finished, non_blocking=True)
         self._nout_host.copy_(self.state.n_out, non_blocking=True)
-
-    def _sample_and_advance(self, st, logits, lp: bool, proc: bool = False, stop: bool = False) -> None:
-        """Sample (with proc, through each slot's logits processors), then with lp the logprobs of the slots with lp_n >= 0 into
-        ring entry n_out mod lp_ring (finished slots untouched), then advance; with proc, each slot's new input id then joins
-        its presence bitmap; with stop, each slot's stop ids and strings are checked against its new token."""
-        if proc:
-            ops.sample_tokens_processed(logits, st.temperature, st.top_k, st.top_p, st.min_p, st.seed, st.rep_penalty, st.min_new,
-                                        st.presence, st.rng_offset, st.n_out, self.eos, noise_rows=st.noise_row, out=st.next_ids)
-        else:
-            ops.sample_tokens_slots(logits, st.temperature, st.top_k, st.top_p, st.seed, st.noise_row, st.rng_offset,
-                                    out=st.next_ids)
-        if lp:
-            ops.token_logprobs(logits, st.next_ids, MAX_LOGPROBS, n_row=st.lp_n, col=st.n_out, ring=self.lp_ring,
-                               finished=st.finished, finished_fill=False, out=(st.lp_ring_lp, st.lp_ring_ids, st.lp_ring_top))
-        ops.decode_advance_slots(st.next_ids, st.ids_in, st.out_tokens, st.n_out, st.max_new, st.rope_pos, st.write_pos,
-                                 st.kv_len, st.rng_offset, st.finished, self.eos, self.pad)
-        if proc:
-            ops.presence_set(st.ids_in, st.presence, self.model.language_model.config.vocab_size)
-        if stop:
-            ops.stop_check_slots(*self.stop_vocab, st.stop_bytes, st.stop_lens, st.stop_lookback, st.stop_ids, st.n_stop_ids,
-                                 st.stop_tail, st.stop_tail_len, st.out_tokens, st.n_out, st.finished, st.ids_in, self.pad)
 
     def _graph(self, n: int, width: int, lp: bool = False, proc: bool = False, stop: bool = False) -> torch.cuda.CUDAGraph:
         """The captured step over slots [0, n) and table columns [0, width), with the logprob kernel when lp and the processed
@@ -854,25 +834,12 @@ class Engine:
         row[:len(req.pages)] = torch.tensor(req.pages, dtype=torch.int32)
         self.cache.block_table[s].copy_(row)
         T = req.input_ids.numel()
-        t, k, p, seed = req.sampling
         st = self.state
         st.rope_pos[s] = T - 1
         st.write_pos[s] = T - 1
         st.kv_len[s] = T
-        st.temperature[s] = t
-        st.top_k[s] = k
-        st.top_p[s] = p
-        st.seed[s] = seed - 2 ** 64 if seed >= 2 ** 63 else seed    # int64 storage of the uint64 seed
+        start_rows(st, s, req.sampling, req.max_new_tokens, req.logprobs, req.processors)
         st.noise_row[s] = 0
-        st.rng_offset[s] = 0
-        st.max_new[s] = req.max_new_tokens
-        st.n_out[s] = 0
-        st.finished[s] = 0
-        st.lp_n[s] = -1 if req.logprobs is None else req.logprobs
-        pen, min_p, min_new = (1.0, 0.0, 0) if req.processors is None else req.processors
-        st.rep_penalty[s] = pen
-        st.min_p[s] = min_p
-        st.min_new[s] = min_new
         if req.processors is not None:      # the prompt's ids, before the first token is sampled
             ops.presence_set(req.input_ids.to(self.dev)[None], st.presence[s:s + 1], self.model.language_model.config.vocab_size,
                              clear=True)
@@ -892,7 +859,8 @@ class Engine:
         else:
             st.stop_lookback[s] = 0
             st.n_stop_ids[s] = 0
-        self._sample_and_advance(_slot_rows(st, s), logits, req.logprobs is not None, req.processors is not None, stop)
+        sample_and_advance(_slot_rows(st, s), logits, self.eos, self.pad, self.stop_vocab, req.logprobs is not None,
+                           req.processors is not None, stop)
 
     def _drop(self, s: int) -> None:
         """Retire slot s without a result: the last active slot moves into s and the slot it left becomes idle."""

@@ -1,6 +1,6 @@
 """Stop strings: the host side of generate(stop_strings=..., tokenizer=...) and Engine.add_request(stop_strings=...).
 
-Hugging Face's StopStringCriteria, checked on the GPU by ops.stop_check / ops.stop_check_slots.  The kernels read two things
+Hugging Face's StopStringCriteria, checked on the GPU by ops.stop_check_slots.  The kernel reads two things
 built here: the vocabulary table, every token's cleaned string (StopStringCriteria.clean_tokenizer_vocab: the string the
 token really yields, with "Ġ" / "▁" / byte-fallback spellings resolved) as UTF-8 bytes with int32 offsets, and a stop set,
 up to 16 strings of at most 128 characters in fixed-size buffers with the lookback window HF uses (the characters of the

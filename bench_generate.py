@@ -135,7 +135,7 @@ def run_b32(model, cfg, args, dev):
     for t in g.cache.k + g.cache.v:
         t.normal_()
     gen = torch.Generator(device=dev).manual_seed(5)
-    g.ids.copy_(torch.randint(10, cfg["text_config"]["vocab_size"], (B, 1), generator=gen, device=dev))
+    g.state.ids_in.copy_(torch.randint(10, cfg["text_config"]["vocab_size"], (B, 1), generator=gen, device=dev))
     timed_replays(g, T, n - 1)                  # warm
     ms = sorted(timed_replays(g, T, n - 1) for _ in range(args.runs))[args.runs // 2]
     return {"protocol": "batch 32, 2048-token text prompts (cache rows random), 64 new tokens, greedy; median of runs",

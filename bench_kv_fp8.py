@@ -136,7 +136,7 @@ def _decode(model, B, T, n, kv, w8a8, args, dev):
     else:
         for t in c.k + c.v:
             t.normal_(generator=gen)
-    g.ids.copy_(torch.randint(10, model.config.text_config.vocab_size, (B, 1), generator=gen, device=dev))
+    g.state.ids_in.copy_(torch.randint(10, model.config.text_config.vocab_size, (B, 1), generator=gen, device=dev))
     BG.timed_replays(g, T, n - 1)
     ms = _median([BG.timed_replays(g, T, n - 1) for _ in range(args.runs)])
     tc = model.config.text_config

@@ -98,7 +98,7 @@ def bench_generate(model, Vm, dev, iters=3):
                 t.normal_()
             gen = torch.Generator(device=dev).manual_seed(5)
             prompt = torch.randint(10, Vm, (B, T), generator=gen, device=dev)
-            g.ids.copy_(prompt[:, -1:])
+            g.state.ids_in.copy_(prompt[:, -1:])
 
             def replays():
                 g.start(T, None)

@@ -62,7 +62,7 @@ def bench_generate(model, V, dev, iters=3):
             for t in g.cache.k + g.cache.v:
                 t.normal_()
             gen = torch.Generator(device=dev).manual_seed(5)
-            g.ids.copy_(torch.randint(10, V, (B, 1), generator=gen, device=dev))
+            g.state.ids_in.copy_(torch.randint(10, V, (B, 1), generator=gen, device=dev))
 
             def replays():
                 g.start(T, None)

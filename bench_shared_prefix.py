@@ -136,7 +136,7 @@ def repeated_decode(model, ids, pv, n, new, kw):
     g.sample_and_advance(out.logits[:, -1].expand(n, -1))     # row stride 0: every row samples the same logits
     for _ in range(new - 1):
         g.graph.replay()
-    return g, g.out_tokens.clone()
+    return g, g.state.out_tokens.to(torch.int64)
 
 
 def run_b32(model, cfg, args, kw):

@@ -4,9 +4,9 @@
 
   table_build_s   host seconds of the first vocabulary-table build (stopping.vocab_table) for a byte-level BPE tokenizer of
                   100,352 ids, and of a second, cached call.
-  stop_check      the kernel's own time per launch: --iters ops.stop_check launches captured in one CUDA graph, the graph
-                  replayed and timed with CUDA events, at 1, 32, 256 and 1,024 rows, with 1 and 16 strings of 10 and 128
-                  characters, on random 64-token histories that never stop (every row is checked).
+  stop_check_slots  the kernel's own time per launch: --iters ops.stop_check_slots launches captured in one CUDA graph, the
+                  graph replayed and timed with CUDA events, at 1, 32, 256 and 1,024 rows, each with the same 1 or 16 strings
+                  of 10 or 128 characters and no stop ids, on random 64-token histories that never stop (every row is checked).
   generate        generate()'s decode ms per step, greedy, at batch 1 from a 16-token prompt and at batch 32 from 2K-token
                   prompts, without and with stop_strings=["<|im_end|>"] (the captured step replayed, CUDA events, as
                   bench_logits_processors.py times it).
@@ -52,22 +52,24 @@ def bench_kernel(ops, table, dev, iters):
                                enumerate(torch.randint(0, 500, (chars,), generator=g))) for _ in range(n)]
             data, lens, lookback = stopping.encode_stop_set(strings)
             tail, k = stopping.prompt_tail(hist[:, :32])
-            args = (vb, vo, data.to(dev), lens.to(dev), torch.tensor([lookback], dtype=torch.int32, device=dev), tail.to(dev),
-                    torch.full((R,), k, dtype=torch.int32, device=dev), hist[:, 32:].contiguous().to(dev),
-                    torch.tensor([32], dtype=torch.int32, device=dev), torch.zeros(R, dtype=torch.uint8, device=dev),
-                    torch.full((1,), -1, dtype=torch.int32, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
-            ops.stop_check(*args)
+            i32 = dict(dtype=torch.int32, device=dev)
+            fin = torch.zeros(R, dtype=torch.uint8, device=dev)
+            args = (vb, vo, data.repeat(R, 1, 1).to(dev), lens.repeat(R, 1).to(dev), torch.full((R,), lookback, **i32),
+                    torch.zeros(R, 8, dtype=torch.int64, device=dev), torch.zeros(R, **i32), tail.to(dev),
+                    torch.full((R,), k, **i32), hist[:, 32:].to(dev, torch.int32), torch.full((R,), 32, **i32), fin,
+                    torch.zeros(R, dtype=torch.int64, device=dev), 0)
+            ops.stop_check_slots(*args)
             graph = torch.cuda.CUDAGraph()
             with ops.graph_capture(graph):
                 for _ in range(iters):
-                    ops.stop_check(*args)
+                    ops.stop_check_slots(*args)
             graph.replay()
             a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             a.record()
             graph.replay()
             b.record()
             b.synchronize()
-            assert not bool(args[9].any())
+            assert not bool(fin.any())
             out[f"R{R}_{n}x{chars}_us"] = round(a.elapsed_time(b) / iters * 1e3, 2)
     return out
 
@@ -86,7 +88,7 @@ def bench_generate(model, Vm, table, dev, iters=3):
                     t.normal_()
                 gen = torch.Generator(device=dev).manual_seed(5)
                 prompt = torch.randint(10, Vm, (B, T), generator=gen, device=dev)
-                g.ids.copy_(prompt[:, -1:])
+                g.state.ids_in.copy_(prompt[:, -1:])
 
                 def replays():
                     g.start(T, None)
@@ -157,7 +159,7 @@ def main():
                           text=True).stdout.strip()
     tok, table, build = bench_table()
     result = {"bench": "stop_strings", "V": V, "card": card, "table_build_s": build,
-              "stop_check": bench_kernel(ops, table, dev, args.iters)}
+              "stop_check_slots": bench_kernel(ops, table, dev, args.iters)}
     if not args.kernel_only:
         from aria_b200 import configs as C
         from aria_b200.modeling_aria import AriaConfig, AriaForConditionalGeneration, init_random_

@@ -520,15 +520,6 @@ int aria_kv_load_fp8(const void* k_cache, const void* v_cache, const float* k_sc
                      int64_t cache_stride_h, int64_t scale_stride_b, int64_t scale_stride_h, void* k_out, void* v_out,
                      int64_t out_stride_b, int64_t out_stride_h, int32_t n_rows, int32_t B, int32_t H, int32_t T_max,
                      aria_stream_t stream);
-/* Decode-state advance after aria_sample_tokens, one launch (B <= 1024), all state in device memory:
- *   t = *step; tok[b] = finished[b] ? pad_token_id : next_ids[b]; out_tokens[b * max_steps + t] = tok[b] (if t < max_steps);
- *   ids_in[b] = tok[b]; finished[b] |= tok[b] is one of eos_ids (HOST array of n_eos <= 8 ids, copied at the call);
- *   ++rope_pos[b], ++write_pos[b], ++kv_len[b]; *step = t + 1; *rng_offset += 1;
- *   and when n_eos > 0, every row is finished and *done_step < 0: *done_step = t (GenerationMixin stops after that token). */
-int aria_decode_advance(const int64_t* next_ids, int64_t* ids_in, int64_t* out_tokens, int32_t max_steps, int32_t* step,
-                        int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len, uint64_t* rng_offset, uint8_t* finished,
-                        int32_t* done_step, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t B,
-                        aria_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Prompt-lookup decoding: a step verifies Q = K + 1 tokens per row (the last token, then K drafts from the row's history)
@@ -675,11 +666,11 @@ int aria_token_logprobs(const void* logits, int64_t logits_stride, const int64_t
                         const int32_t* n_row, const int32_t* col, int32_t col_per_row, int32_t ring, const uint8_t* finished,
                         int32_t finished_fill, float* logprobs, int32_t* top_ids, float* top_logprobs, int32_t cols,
                         aria_stream_t stream);
-/* aria_decode_advance per slot (continuous batching).  For each slot r < R that is not finished: its token next_ids[r] is stored
- * at out_tokens[r, n_out[r]] ([R, out_stride] int32) and n_out[r] + 1; the slot finishes when the token is one of the n_eos <= 8
- * EOS ids (HOST array, copied into the launch) or n_out reaches max_new[r]; ids_in[r] <- the token (pad_token_id once
- * finished); rope_pos, write_pos, kv_len and rng_offset[r] (uint64) + 1.  A finished slot (idle slots are finished) changes
- * nothing.  R <= 1024, one launch. */
+/* Decode-state advance after the sampler, per row (generate() and continuous batching).  For each row r < R that is not
+ * finished: its token next_ids[r] is stored at out_tokens[r, n_out[r]] ([R, out_stride] int32) and n_out[r] + 1; the row
+ * finishes when the token is one of the n_eos <= 8 EOS ids (HOST array, copied into the launch) or n_out reaches max_new[r];
+ * ids_in[r] <- the token (pad_token_id once finished); rope_pos, write_pos, kv_len and rng_offset[r] (uint64) + 1.  A finished
+ * row (idle slots are finished) changes nothing.  R <= 1024, one launch. */
 int aria_decode_advance_slots(const int64_t* next_ids, int64_t* ids_in, int32_t* out_tokens, int64_t out_stride, int32_t* n_out,
                               const int32_t* max_new, int32_t* rope_pos, int32_t* write_pos, int32_t* kv_len, uint64_t* rng_offset,
                               uint8_t* finished, const int64_t* eos_ids, int32_t n_eos, int64_t pad_token_id, int32_t R,
@@ -719,19 +710,11 @@ int aria_lookup_accept_advance(const int64_t* targets, const int64_t* step_ids, 
  * Every array is DEVICE memory.  A row stops after its final token when that token completes a string: some byte prefix of
  * it ends with the string's last bytes (or holds the whole string), and the tokens before it, walking back within the
  * lookback window, cover the rest of the string, the earliest one allowed to run off its start.  One warp per row. */
-/* One stop set for B <= 1024 rows.  The history of row b is its last tail_len[b] <= 128 prompt ids, right-aligned in
- * prompt_tail [B, 128] int64, then out_tokens[b, 0 .. *step) ([B, max_steps] int64).  A row that is not finished and stops gets finished[b] = 1;
- * then if every row is finished, *step > 0 and *done_step < 0, *done_step = *step - 1.  counter (int32) is 0 before the launch and after
- * it. */
-int aria_stop_check(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
-                    const int32_t* stop_lens, const int32_t* lookback, const int64_t* prompt_tail,
-                    const int32_t* tail_len, const int64_t* out_tokens, int32_t max_steps, const int32_t* step, uint8_t* finished,
-                    int32_t* done_step, int32_t* counter, int32_t B, aria_stream_t stream);
-/* The serving engine's flavour, R <= 1024 slots, slot r with its own stop set (stop_bytes [R, 16, 512], stop_lens [R, 16],
- * lookback [R]; lookback 0 = no strings) and its own stop ids (stop_ids [R, 8] int64, the first n_stop_ids[r] of them).  Its
- * history is its prompt tail as above, then out_tokens[r, 0 .. n_out[r]) ([R, out_stride] int32).  A slot that is not
- * finished and whose final token is one of its stop ids or completes one of its strings gets finished[r] = 1 and
- * ids_in[r] = pad_token_id. */
+/* R <= 1024 rows, row r with its own stop set (stop_bytes [R, 16, 512], stop_lens [R, 16], lookback [R]; lookback 0 = no
+ * strings) and its own stop ids (stop_ids [R, 8] int64, the first n_stop_ids[r] of them).  Its history is its last
+ * tail_len[r] <= 128 prompt ids, right-aligned in prompt_tail [R, 128] int64, then out_tokens[r, 0 .. n_out[r]) ([R, out_stride]
+ * int32).  A row that is not finished and whose final token is one of its stop ids or completes one of its strings gets
+ * finished[r] = 1 and ids_in[r] = pad_token_id. */
 int aria_stop_check_slots(const uint8_t* vocab_bytes, const int32_t* vocab_offsets, int32_t V, const uint8_t* stop_bytes,
                           const int32_t* stop_lens, const int32_t* lookback, const int64_t* stop_ids, const int32_t* n_stop_ids,
                           const int64_t* prompt_tail, const int32_t* tail_len, const int32_t* out_tokens, int64_t out_stride,

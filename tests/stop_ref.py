@@ -1,4 +1,4 @@
-"""Stop strings on the host: the stop-check kernels' algorithm restated in plain Python (stops), and the offline tokenizers the
+"""Stop strings on the host: the stop-check kernel's algorithm restated in plain Python (stops), and the offline tokenizers the
 tests check it with (byte_level_tokenizer, sentencepiece_tokenizer), built in-process with the `tokenizers` library."""
 import random
 
@@ -7,7 +7,7 @@ from aria_b200 import stopping
 
 def stops(table: "stopping.StopVocab", strings, history) -> bool:
     """Whether a row whose ids so far are `history` (prompt and generated, oldest first) stops after its last id: what
-    ops.stop_check computes for one row, byte for byte (see csrc/stop.cu)."""
+    ops.stop_check_slots computes for one row with these strings and no stop ids, byte for byte (see csrc/stop.cu)."""
     data, offsets = bytes(table.data.numpy()), table.offsets.tolist()
     W = min(max(len(s) for s in strings), stopping.TAIL)
     window = list(history)[::-1][:W]

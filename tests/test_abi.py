@@ -33,7 +33,8 @@ def test_exports_every_declared_symbol(lib):
 
 
 def test_abi_version_3_and_arch(lib):
-    """Version 3: `aria_gemm_desc_t` without the descriptor debug fields, and 41 entries (no round-1 peer transport)."""
+    """Version 3: `aria_gemm_desc_t` without the descriptor debug fields, and 89 entries (no round-1 peer transport, no batch-wide
+    decode advance or stop check)."""
     assert lib.aria_abi_version() == 3
     assert lib.aria_build_arch() == b"sm_90a"
 

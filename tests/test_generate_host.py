@@ -36,7 +36,7 @@ def test_sample_tokens_validation(lib):
     assert f(fake, 1000, fake, None, 1, 1000, 1.0, 0, 0.9, 0, None, None) == UNSUPPORTED   # full-vocabulary nucleus
 
 
-def test_decode_devlen_kv_append_advance_validation(lib):
+def test_decode_devlen_kv_append_slot_advance_validation(lib):
     a = lib.aria_attention_decode_devlen
     ws = lib.aria_attention_decode_workspace_bytes(2, 4, 512)
     args = [fake, fake, fake, fake, None, 0, fake, 2, 4, 512, 4 * 512 * 128, 512 * 128, 4 * 512 * 128, 512 * 128, 0.1, fake, ws, None]
@@ -59,7 +59,7 @@ def test_decode_devlen_kv_append_advance_validation(lib):
     assert k(fake, fake, 512, 100, fake, fake, 4 * 512 * 128, 512 * 128, fake, 2, 4, 512, None) == BAD   # stride % 8
     assert k(fake, fake, 512, 128, fake, fake, 4 * 512 * 128, 512 * 128, fake, 2, 4, 0, None) == BAD     # T_max = 0
 
-    d = lib.aria_decode_advance
+    d = lib.aria_decode_advance_slots
     ok = [fake] * 3 + [16] + [fake] * 7 + [None, 0, 0, 4, None]
     for i in (0, 1, 2, 4, 5, 6, 7, 8, 9, 10):
         bad = list(ok)

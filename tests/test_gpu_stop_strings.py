@@ -1,6 +1,6 @@
-"""GPU: stop strings.  ops.stop_check against transformers' StopStringCriteria row for row on adversarial histories (both
-tokenizer styles, at a small vocabulary and at V = 100,352, at 1, 33 and 1,024 rows), with finished rows left alone and
-done_step set exactly when the last row stops; generate(stop_strings=...) on the tiny model against its own unconstrained
+"""GPU: stop strings.  ops.stop_check_slots with one stop set in every row against transformers' StopStringCriteria row for
+row on adversarial histories (both tokenizer styles, at a small vocabulary and at V = 100,352, at 1, 33 and 1,024 rows), with
+finished rows left alone and stopped rows fed pad; generate(stop_strings=...) on the tiny model against its own unconstrained
 run cut where StopStringCriteria first fires, across the paths generate() has; and the captured step kept without stop
 strings and shared between sets of strings."""
 import random
@@ -29,28 +29,30 @@ def _tok(kind, V):
     return _TOKS[kind, V]
 
 
-def _launch(table, strings, hist, n_gen, finished=None, done_step=-1):
-    """ops.stop_check on histories [R, H] whose last n_gen ids are the generated ones -> (finished, done_step)."""
+def _launch(table, strings, hist, n_gen, finished=None):
+    """ops.stop_check_slots with the stop set of strings in every row (no stop ids) on histories [R, H] whose last n_gen ids
+    are the generated ones -> finished; every row it stops, and no other, is fed pad."""
     from aria_b200 import ops, stopping
     R, H = hist.shape
     data, lens, lookback = stopping.encode_stop_set(strings)
     tail, n = stopping.prompt_tail(hist[:, :H - n_gen]) if H > n_gen else (torch.zeros(R, 128, dtype=torch.int64), 0)
-    out = torch.full((R, n_gen + 3), -5, dtype=torch.int64)
+    out = torch.full((R, n_gen + 3), -5, dtype=torch.int32)
     out[:, :n_gen] = hist[:, H - n_gen:]
     fin = torch.zeros(R, dtype=torch.uint8) if finished is None else finished.clone()
     d = dict(device=DEV)
-    dev_fin, dev_done = fin.to(DEV), torch.tensor([done_step], dtype=torch.int32, **d)
-    counter = torch.zeros(1, dtype=torch.int32, **d)
-    ops.stop_check(*table.device(DEV), data.to(DEV), lens.to(DEV), torch.tensor([lookback], dtype=torch.int32, **d),
-                   tail.to(DEV), torch.full((R,), n, dtype=torch.int32, **d), out.to(DEV),
-                   torch.tensor([n_gen], dtype=torch.int32, **d), dev_fin, dev_done, counter)
-    assert int(counter.item()) == 0
-    return dev_fin.cpu(), int(dev_done.item())
+    i32 = dict(dtype=torch.int32, **d)
+    dev_fin, ids_in = fin.to(DEV), torch.full((R,), 99, dtype=torch.int64, **d)
+    ops.stop_check_slots(*table.device(DEV), data.repeat(R, 1, 1).to(DEV), lens.repeat(R, 1).to(DEV),
+                         torch.full((R,), lookback, **i32), torch.zeros(R, 8, dtype=torch.int64, **d), torch.zeros(R, **i32),
+                         tail.to(DEV), torch.full((R,), n, **i32), out.to(DEV), torch.full((R,), n_gen, **i32), dev_fin, ids_in, 3)
+    got = dev_fin.cpu()
+    assert ids_in.cpu().tolist() == [3 if a and not b else 99 for a, b in zip(got.tolist(), fin.tolist())]
+    return got
 
 
 @pytest.mark.parametrize("kind", ["byte", "sp"])
 @pytest.mark.parametrize("V", [1000, 100352])
-def test_kernel_equals_hf(kind, V):
+def test_kernel_one_set_in_every_row_equals_hf(kind, V):
     from aria_b200 import stopping
     tok = _tok(kind, V)
     table = stopping.vocab_table(tok)
@@ -62,33 +64,29 @@ def test_kernel_equals_hf(kind, V):
         for R in (1, 33, 1024):
             idx = torch.tensor([rng.randrange(hist.shape[0]) for _ in range(R)])
             n_gen = rng.randint(1, hist.shape[1])
-            fin, done = _launch(table, strings, hist[idx], n_gen)
+            fin = _launch(table, strings, hist[idx], n_gen)
             assert torch.equal(fin, want[idx]), (strings, n_gen)
-            assert done == (n_gen - 1 if bool(want[idx].all()) else -1)
             stopped += int(want[idx].sum())
             total += R
     assert 0.05 * total < stopped < 0.95 * total
 
 
-def test_kernel_leaves_finished_rows_and_keeps_done_step():
+def test_kernel_leaves_finished_rows_and_feeds_stopped_rows_pad():
     from aria_b200 import stopping
     tok = _tok("byte", 1000)
     table = stopping.vocab_table(tok)
     v = tok.get_vocab()
     st, op, x = v["st"], v["op"], v["s"]
     hist = torch.tensor([[x, st, op], [x, x, st], [x, st, op], [x, x, x]])
-    # rows 0 and 2 stop; row 1 finished before (an EOS), row 3 not finished: done_step stays -1
-    fin, done = _launch(table, ["stop"], hist, 2, finished=torch.tensor([0, 1, 0, 0], dtype=torch.uint8))
-    assert fin.tolist() == [1, 1, 1, 0] and done == -1
-    # row 3 finished too: the stop of rows 0 and 2 ends the batch at this step
-    fin, done = _launch(table, ["stop"], hist, 2, finished=torch.tensor([0, 1, 0, 1], dtype=torch.uint8))
-    assert fin.tolist() == [1, 1, 1, 1] and done == 1
-    # an earlier done_step (the EOS advance set it) is kept
-    fin, done = _launch(table, ["stop"], hist, 2, finished=torch.tensor([0, 1, 0, 1], dtype=torch.uint8), done_step=0)
-    assert done == 0
-    # every row finished already: nothing is checked, done_step is kept as it is
-    fin, done = _launch(table, ["stop"], hist, 2, finished=torch.ones(4, dtype=torch.uint8), done_step=0)
-    assert fin.tolist() == [1, 1, 1, 1] and done == 0
+    # rows 0 and 2 stop; row 1 finished before (an EOS) and is left alone, row 3 does not stop
+    fin = _launch(table, ["stop"], hist, 2, finished=torch.tensor([0, 1, 0, 0], dtype=torch.uint8))
+    assert fin.tolist() == [1, 1, 1, 0]
+    # row 3 finished before too: every row is finished after this step
+    fin = _launch(table, ["stop"], hist, 2, finished=torch.tensor([0, 1, 0, 1], dtype=torch.uint8))
+    assert fin.tolist() == [1, 1, 1, 1]
+    # every row finished already: nothing is checked (no row is fed pad)
+    fin = _launch(table, ["stop"], hist, 2, finished=torch.ones(4, dtype=torch.uint8))
+    assert fin.tolist() == [1, 1, 1, 1]
 
 
 # ------------------------------------------------------------------------------------------------ generate()
@@ -432,20 +430,20 @@ def test_kernel_slots_equal_hf():
 
 
 @pytest.mark.parametrize("R", [33, 1024])
-def test_kernel_done_step_over_many_ctas(R):
-    """Only stopping rows, or stopping rows and rows finished before: the last CTA sets done_step = step - 1 and leaves the
-    counter at zero; one row that does not stop keeps done_step at -1."""
+def test_kernel_finished_flags_over_many_ctas(R):
+    """Only stopping rows, or stopping rows and rows finished before, over many CTAs: every row ends finished; one row that
+    does not stop stays unfinished."""
     from aria_b200 import stopping
     tok = _tok("byte", 1000)
     table = stopping.vocab_table(tok)
     v = tok.get_vocab()
     stop_row = [v["s"], v["st"], v["op"]]
     hist = torch.tensor([stop_row] * R)
-    fin, done = _launch(table, ["stop"], hist, 2)
-    assert bool(fin.all()) and done == 1
+    fin = _launch(table, ["stop"], hist, 2)
+    assert bool(fin.all())
     pre = (torch.arange(R) % 3 == 0).to(torch.uint8)
-    fin, done = _launch(table, ["stop"], hist, 2, finished=pre)
-    assert bool(fin.all()) and done == 1
+    fin = _launch(table, ["stop"], hist, 2, finished=pre)
+    assert bool(fin.all())
     hist[R // 2, -1] = v["s"]
-    fin, done = _launch(table, ["stop"], hist, 2, finished=pre)
-    assert int(fin.sum()) == R - (0 if pre[R // 2] else 1) and done == -1
+    fin = _launch(table, ["stop"], hist, 2, finished=pre)
+    assert int(fin.sum()) == R - (0 if pre[R // 2] else 1)
