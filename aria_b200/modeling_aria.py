@@ -493,8 +493,7 @@ class AriaForConditionalGeneration(nn.Module):
         emb = ops.embedding(suffix.to(dev, non_blocking=True), lm.get_input_embeddings().weight)
         x, pending = lm.model.prefill_suffixes(emb, g.cache, cu_dev, pos.to(dev, non_blocking=True))
         last = (cu[1:] - 1).to(dev, torch.int64, non_blocking=True)
-        h, _ = lm.model.norm(x[0, last].contiguous(), residual=pending[0, last].contiguous())
-        first = lm.lm_head(h)                       # [B, V]
+        first = lm.head(x[0, last].contiguous(), pending[0, last].contiguous())   # [B, V]
         g.start_suffixes(P, S, n_seq)
         if processors is not None:      # each row's own left-padded ids, as the repeated-image batch has them
             g.start_presence(input_ids.to(dev).repeat_interleave(n_seq, 0))
@@ -760,16 +759,14 @@ class GraphedDecode:
         if group_size == 1 and N_max is None:
             self.cache = lm.new_cache(B, T_max, dev, kv_cache_dtype)
             self.state = DecodeState(B, c.num_attention_heads, T_max, dev)
-            n_pos = T_max
         else:
             if N_max is None:
                 N_max = -(-max_new_tokens // 256) * 256
             self.cache = SharedPrefixCache(c.num_hidden_layers, B, group_size, c.num_attention_heads, T_max, N_max, c.head_dim, dev)
             self.state = SharedDecodeState(B, group_size, c.num_attention_heads, T_max, dev)
-            n_pos = T_max + N_max
             B = B * group_size
         self.model, self.B = model, B
-        self.rope = lm.model.rope_tables(n_pos, dev)   # held here: the graph reads these tables
+        self.rope = lm.model.rope_tables(self.cache.n_positions, dev)   # held here: the graph reads these tables
         self.n_logprobs, self.processors, self.stop = logprobs, processors, stop
         self.V = c.vocab_size
         st = self.state
@@ -924,7 +921,7 @@ class GraphedLookupDecode:
         self.sampling, self.eos, self.pad = sampling, eos, pad
         self.cache = lm.new_cache(B, T_max, dev)
         self.state = LookupDecodeState(B, c.num_attention_heads, T_max, K, dev)
-        self.rope = lm.model.rope_tables(T_max, dev)
+        self.rope = lm.model.rope_tables(self.cache.n_positions, dev)
         i64, i32 = dict(dtype=torch.int64, device=dev), dict(dtype=torch.int32, device=dev)
         Q = K + 1
         self.ids1 = torch.zeros(B, 1, **i64)

@@ -483,6 +483,29 @@ class KVCache:
         self.seq_len = 0
         self.T_max = T_max
 
+    @property
+    def n_positions(self) -> int:
+        """The RoPE positions the cache spans: the length of the rope_tables its steps read."""
+        return self.T_max
+
+    def scales(self, layer):
+        """(k_scale, v_scale) of a layer's fp8 cache, (None, None) for a bf16 one: the ops' k_scale= / v_scale= arguments."""
+        if self.dtype == "fp8":
+            return self.k_scale[layer], self.v_scale[layer]
+        return None, None
+
+    def decode_attention(self, layer, q, k, v, state: "DecodeState", scale: float) -> torch.Tensor:
+        """One decode step of `layer` on this cache: the step's k, v rows [B, H, 128] are stored at cache row
+        state.write_pos[b] (quantized on an fp8 cache), then q [B, H, 128] attends to rows [0, state.kv_len[b]) minus
+        state.key_mask -> o [B, H*128]."""
+        kc, vc = self.k[layer], self.v[layer]
+        ks, vs = self.scales(layer)
+        if ks is None:
+            ops.kv_append(k, v, kc, vc, state.write_pos)
+        else:
+            ops.kv_append_fp8(k, v, kc, vc, ks, vs, state.write_pos)
+        return ops.attention_decode_devlen(q, kc, vc, state.kv_len, scale, key_mask=state.key_mask, k_scale=ks, v_scale=vs)
+
 
 class DecodeState:
     """Device-resident positions of a decode step that is captured once and replayed token after token
@@ -513,6 +536,19 @@ class SharedPrefixCache(KVCache):
         self.N_max = N_max
         self.tail_k = [torch.empty(G * n, H, N_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
         self.tail_v = [torch.empty(G * n, H, N_max, hd, dtype=bf16, device=device) for _ in range(n_layers)]
+
+    @property
+    def n_positions(self) -> int:
+        """A row's tail continues its prompt: the prompt bucket, then the tail."""
+        return self.T_max + self.N_max
+
+    def decode_attention(self, layer, q, k, v, state: "SharedDecodeState", scale: float) -> torch.Tensor:
+        """KVCache.decode_attention on the shared prompts: row r's k, v go to its tail row state.write_pos[r], then it attends
+        to its group's prompt (state.prefix_lens, state.prefix_mask) and to tail rows [0, state.kv_len[r])."""
+        tk, tv = self.tail_k[layer], self.tail_v[layer]
+        ops.kv_append(k, v, tk, tv, state.write_pos)
+        return ops.attention_decode_shared_prefix(q, self.k[layer], self.v[layer], state.prefix_lens, tk, tv, state.kv_len,
+                                                  self.group_size, scale, prefix_mask=state.prefix_mask)
 
 
 class SharedDecodeState(DecodeState):
@@ -575,11 +611,20 @@ class PagedKVCache:
         self.width = max_pages
         self.dtype = dtype
 
-    def scales(self, layer):
-        """(k_scale, v_scale) of a layer's fp8 pools, (None, None) for bf16 ones: the ops' k_scale= / v_scale= arguments."""
-        if self.dtype == "fp8":
-            return self.k_scale[layer], self.v_scale[layer]
-        return None, None
+    @property
+    def n_positions(self) -> int:
+        """The RoPE positions a request of max_pages pages spans."""
+        return self.block_table.shape[1] * self.PAGE_SIZE
+
+    scales = KVCache.scales
+
+    def decode_attention(self, layer, q, k, v, state: "SlotDecodeState", scale: float) -> torch.Tensor:
+        """KVCache.decode_attention on the pages: slot r's k, v go to its key state.write_pos[r], then it attends to its keys
+        [0, state.kv_len[r]), over the first `width` columns of the block table."""
+        kp, vp, bt = self.k[layer], self.v[layer], self.block_table[:, :self.width]
+        ks, vs = self.scales(layer)
+        ops.kv_append_paged(k, v, kp, vp, bt, state.write_pos, k_scale=ks, v_scale=vs)
+        return ops.attention_decode_paged(q, kp, vp, bt, state.kv_len, scale, k_scale=ks, v_scale=vs)
 
 
 def add_token_fields(st, R, max_out, device, lp_ring: int = 1, lp_width: int = ops.MAX_LOGPROBS, vocab: int = 1,
@@ -767,7 +812,7 @@ class AriaAttention(nn.Module):
             # fp8 cache: a single token is quantized into the cache and attends to it (as decode_step does); a multi-token
             # step attends in bf16 to the staging pair, holding the dequantized cached rows and its own rows, which are
             # quantized into the cache afterwards.  A one-chunk prefill thus gives the bf16 cache's logits bit for bit.
-            ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
+            ks, vs = cache.scales(self.layer_idx)
             k_st, v_st = cache.k_stage, cache.v_stage
             if T == 1:
                 ops.kv_store_fp8(k_st[:, :, pos0:Tk], v_st[:, :, pos0:Tk], kc, vc, ks, vs, pos0)
@@ -786,34 +831,13 @@ class AriaAttention(nn.Module):
 
     def decode_step(self, hidden_states, cache: KVCache, rope, state: DecodeState, residual=None, hq=None):
         """One token per row with every position on the device (graph-replayable): the fused projection writes q, k, v
-        to the state's staging rows (RoPE at state.rope_pos), kv_append moves k, v into the cache at state.write_pos, and
-        the decode attention reads state.kv_len keys.  Same kernels and arithmetic as forward() at T = 1."""
+        to the state's staging rows (RoPE at state.rope_pos), and the cache's decode_attention stores k, v at state.write_pos
+        and attends over state.kv_len keys.  Same kernels and arithmetic as forward() at T = 1."""
         B, T, d = hidden_states.shape
-        H, hd = self.num_heads, self.head_dim
-        kc, vc = cache.k[self.layer_idx], cache.v[self.layer_idx]
         q, k, v = state.qkv[0], state.qkv[1], state.qkv[2]
         self._qkv(hidden_states, hq, [q, k, v], 1, 0, rope, state.rope_pos)
-        if isinstance(cache, PagedKVCache):
-            kp, vp, bt = cache.k[self.layer_idx], cache.v[self.layer_idx], cache.block_table[:, :cache.width]
-            ks, vs = cache.scales(self.layer_idx)
-            ops.kv_append_paged(k[:, :, 0], v[:, :, 0], kp, vp, bt, state.write_pos, k_scale=ks, v_scale=vs)
-            o = ops.attention_decode_paged(q[:, :, 0], kp, vp, bt, state.kv_len, hd ** -0.5, k_scale=ks, v_scale=vs).view(B, 1, d)
-            return self._o_proj(o, residual)
-        if isinstance(cache, SharedPrefixCache):
-            tk, tv = cache.tail_k[self.layer_idx], cache.tail_v[self.layer_idx]
-            ops.kv_append(k[:, :, 0], v[:, :, 0], tk, tv, state.write_pos)
-            o = ops.attention_decode_shared_prefix(q[:, :, 0], kc, vc, state.prefix_lens, tk, tv, state.kv_len, cache.group_size,
-                                                   hd ** -0.5, prefix_mask=state.prefix_mask).view(B, 1, d)
-            return self._o_proj(o, residual)
-        if cache.dtype == "fp8":
-            ks, vs = cache.k_scale[self.layer_idx], cache.v_scale[self.layer_idx]
-            ops.kv_append_fp8(k[:, :, 0], v[:, :, 0], kc, vc, ks, vs, state.write_pos)
-            o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask, k_scale=ks,
-                                            v_scale=vs).view(B, 1, d)
-            return self._o_proj(o, residual)
-        ops.kv_append(k[:, :, 0], v[:, :, 0], kc, vc, state.write_pos)
-        o = ops.attention_decode_devlen(q[:, :, 0], kc, vc, state.kv_len, hd ** -0.5, key_mask=state.key_mask).view(B, 1, d)
-        return self._o_proj(o, residual)
+        o = cache.decode_attention(self.layer_idx, q[:, :, 0], k[:, :, 0], v[:, :, 0], state, self.head_dim ** -0.5)
+        return self._o_proj(o.view(B, 1, d), residual)
 
     def verify_step(self, hidden_states, cache: KVCache, rope, state: LookupDecodeState, residual=None, hq=None):
         """decode_step for Q tokens per row (a prompt-lookup verify step): hidden_states [B, Q, d]; the fused projection writes
@@ -902,38 +926,12 @@ class MoEDecoderLayer(nn.Module):
         h, x = norm(x, residual=pending)
         return h, None, x
 
-    def forward(self, x, pending, cache, rope, key_mask=None, position_ids=None):
-        """x: residual stream; pending: MoE output of the previous layer not yet added (or None)."""
+    def forward(self, x, pending, attend):
+        """x: residual stream; pending: MoE output of the previous layer not yet added (or None); attend(self_attn, h, hq,
+        residual): the step's attention, one of AriaAttention's forward, decode_step, verify_step, prefill_suffixes or
+        prefill_paged, returning the residual stream after it."""
         h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn(h, cache, rope, residual=x, key_mask=key_mask, position_ids=position_ids, hq=hq)
-        h = self.post_attention_layernorm(x)
-        return x, self.mlp(h)
-
-    def decode_step(self, x, pending, cache, rope, state: DecodeState):
-        """forward() for one token per row, positions from `state` (AriaAttention.decode_step)."""
-        h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.decode_step(h, cache, rope, state, residual=x, hq=hq)
-        h = self.post_attention_layernorm(x)
-        return x, self.mlp(h)
-
-    def verify_step(self, x, pending, cache, rope, state: LookupDecodeState):
-        """decode_step for Q tokens per row (AriaAttention.verify_step)."""
-        h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.verify_step(h, cache, rope, state, residual=x, hq=hq)
-        h = self.post_attention_layernorm(x)
-        return x, self.mlp(h)
-
-    def prefill_suffixes(self, x, pending, cache, rope, cu_seqlens, position_ids):
-        """forward() for packed suffixes over a shared prefix (AriaAttention.prefill_suffixes)."""
-        h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.prefill_suffixes(h, cache, rope, cu_seqlens, position_ids, residual=x, hq=hq)
-        h = self.post_attention_layernorm(x)
-        return x, self.mlp(h)
-
-    def prefill_paged(self, x, pending, cache, rope, page_table, seg, position_ids, prefix=None):
-        """forward() for packed prompt segments, each after a prefix held in its pages (AriaAttention.prefill_paged)."""
-        h, hq, x = self._attn_input(x, pending)
-        x = self.self_attn.prefill_paged(h, cache, rope, page_table, seg, position_ids, residual=x, hq=hq, prefix=prefix)
+        x = attend(self.self_attn, h, hq, x)
         h = self.post_attention_layernorm(x)
         return x, self.mlp(h)
 
@@ -962,27 +960,28 @@ class AriaMoELMModel(nn.Module):
         B, T, _ = inputs_embeds.shape
         if cache.seq_len + T > cache.T_max:
             raise RuntimeError(f"KV cache overflow: {cache.seq_len} cached + {T} new tokens > T_max = {cache.T_max}")
-        rope = self.rope_tables(cache.T_max, inputs_embeds.device)
-        x, pending = inputs_embeds, None
-        for layer in self.layers:
-            x, pending = layer(x, pending, cache, rope, key_mask, position_ids)
+        rope = self.rope_tables(cache.n_positions, inputs_embeds.device)
+        x, pending = self._run_layers(inputs_embeds, lambda a, h, hq, x: a(h, cache, rope, residual=x, key_mask=key_mask,
+                                                                           position_ids=position_ids, hq=hq))
         cache.seq_len += T
         return x, pending  # final residual add happens inside the final norm
 
-    def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
-        """One token per row through every layer with the positions of `state`; `cache.seq_len` is neither read nor
-        written (the caller owns it).  `rope`: the tables of rope_tables(cache.T_max), computed outside any graph capture."""
-        x, pending = inputs_embeds, None
+    def _run_layers(self, x, attend):
+        """Every layer on the residual stream x, each attending through attend (MoEDecoderLayer.forward) -> (x, pending)."""
+        pending = None
         for layer in self.layers:
-            x, pending = layer.decode_step(x, pending, cache, rope, state)
+            x, pending = layer(x, pending, attend)
         return x, pending
 
+    def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
+        """One token per row through every layer with the positions of `state`; `cache.seq_len` is neither read nor
+        written (the caller owns it).  `rope`: the tables of rope_tables(cache.n_positions), computed outside any graph
+        capture.  cache: a KVCache, SharedPrefixCache or PagedKVCache (its decode_attention)."""
+        return self._run_layers(inputs_embeds, lambda a, h, hq, x: a.decode_step(h, cache, rope, state, residual=x, hq=hq))
+
     def verify_step(self, inputs_embeds, cache: KVCache, state: LookupDecodeState, rope):
-        """decode_step for Q tokens per row, inputs_embeds [B, Q, d], positions from `state` (MoEDecoderLayer.verify_step)."""
-        x, pending = inputs_embeds, None
-        for layer in self.layers:
-            x, pending = layer.verify_step(x, pending, cache, rope, state)
-        return x, pending
+        """decode_step for Q tokens per row, inputs_embeds [B, Q, d], positions from `state` (AriaAttention.verify_step)."""
+        return self._run_layers(inputs_embeds, lambda a, h, hq, x: a.verify_step(h, cache, rope, state, residual=x, hq=hq))
 
     def prefill_suffixes(self, inputs_embeds, cache: SharedPrefixCache, cu_seqlens, position_ids):
         """Prefill B suffixes that continue the one prefix already in `cache` (a SharedPrefixCache of one prompt row whose
@@ -999,11 +998,9 @@ class AriaMoELMModel(nn.Module):
             raise ValueError(f"prefill_suffixes: inputs_embeds must be [1, S_tot, d], got {tuple(inputs_embeds.shape)}")
         if cache.seq_len < 1:
             raise ValueError("prefill_suffixes: the cache holds no prefix (seq_len 0)")
-        rope = self.rope_tables(cache.T_max + cache.N_max, inputs_embeds.device)
-        x, pending = inputs_embeds, None
-        for layer in self.layers:
-            x, pending = layer.prefill_suffixes(x, pending, cache, rope, cu_seqlens, position_ids)
-        return x, pending
+        rope = self.rope_tables(cache.n_positions, inputs_embeds.device)
+        return self._run_layers(inputs_embeds, lambda a, h, hq, x: a.prefill_suffixes(h, cache, rope, cu_seqlens, position_ids,
+                                                                                      residual=x, hq=hq))
 
     def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, page_table_host=None):
         """Prefill prompt segments packed along one row, each continuing a prefix whose keys and values are already in the
@@ -1031,12 +1028,10 @@ class AriaMoELMModel(nn.Module):
             if P + seg.cu[b + 1] - seg.cu[b] > width * cache.PAGE_SIZE:
                 raise ValueError(f"prefill_paged: segment {b} (P = {P}, {seg.cu[b + 1] - seg.cu[b]} tokens) does not fit {width} "
                                  "pages")
-        rope = self.rope_tables(cache.block_table.shape[1] * cache.PAGE_SIZE, inputs_embeds.device)
+        rope = self.rope_tables(cache.n_positions, inputs_embeds.device)
         prefix = self._prefix_scratch(cache, page_table, seg, page_table_host) if cache.dtype == "fp8" else None
-        x, pending = inputs_embeds, None
-        for layer in self.layers:
-            x, pending = layer.prefill_paged(x, pending, cache, rope, page_table, seg, position_ids, prefix)
-        return x, pending
+        return self._run_layers(inputs_embeds, lambda a, h, hq, x: a.prefill_paged(h, cache, rope, page_table, seg, position_ids,
+                                                                                   residual=x, hq=hq, prefix=prefix))
 
     @staticmethod
     def _prefix_scratch(cache: PagedKVCache, page_table, seg, page_table_host=None):
@@ -1106,8 +1101,13 @@ class AriaMoELMForCausalLM(nn.Module):
         if num_logits_to_keep:
             x = x[:, -num_logits_to_keep:, :].contiguous()
             pending = pending[:, -num_logits_to_keep:, :].contiguous()
+        return self.head(x, pending), cache
+
+    def head(self, x, pending):
+        """Logits of the layers' output (x, pending): the final norm, which adds the last layer's pending MoE output, then
+        lm_head."""
         h, _ = self.model.norm(x, residual=pending)
-        return self.lm_head(h), cache
+        return self.lm_head(h)
 
     def prefill_paged(self, inputs_embeds, cache: PagedKVCache, page_table, seg, position_ids, ends=None, page_table_host=None,
                       hidden_rows=None):
@@ -1136,18 +1136,13 @@ class AriaMoELMForCausalLM(nn.Module):
         else:
             idx = torch.tensor(rows, dtype=torch.int64).to(x.device, non_blocking=True)
             x, pending = x.index_select(1, idx), pending.index_select(1, idx)
-        h, _ = self.model.norm(x, residual=pending)
-        return self.lm_head(h)
+        return self.head(x, pending)
 
     def decode_step(self, inputs_embeds, cache: KVCache, state: DecodeState, rope):
         """inputs_embeds [B, 1, d] -> logits [B, 1, V] for one decode step driven by device positions (graph-replayable)."""
-        x, pending = self.model.decode_step(inputs_embeds, cache, state, rope)
-        h, _ = self.model.norm(x, residual=pending)
-        return self.lm_head(h)
+        return self.head(*self.model.decode_step(inputs_embeds, cache, state, rope))
 
     def verify_step(self, inputs_embeds, cache: KVCache, state: LookupDecodeState, rope):
         """inputs_embeds [B, Q, d] -> logits [B, Q, V]: decode_step for the Q tokens of a prompt-lookup verify step, each row's
         query i with the logits decode_step gives its token (graph-replayable)."""
-        x, pending = self.model.verify_step(inputs_embeds, cache, state, rope)
-        h, _ = self.model.norm(x, residual=pending)
-        return self.lm_head(h)
+        return self.head(*self.model.verify_step(inputs_embeds, cache, state, rope))

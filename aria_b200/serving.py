@@ -475,7 +475,7 @@ class Engine:
         self.lp_ring = poll_every + 1
         self.state = SlotDecodeState(max_batch, c.num_attention_heads, self.max_pages * PAGE, dev, self.lp_ring, c.vocab_size)
         self._idle(0, max_batch)
-        self.rope = lm.model.rope_tables(self.max_pages * PAGE, dev)   # held here: the graphs read these tables
+        self.rope = lm.model.rope_tables(self.cache.n_positions, dev)   # held here: the graphs read these tables
         self._graphs: Dict[tuple, torch.cuda.CUDAGraph] = {}
         self._pool = torch.cuda.graph_pool_handle()
         self._fin_host = torch.ones(max_batch, dtype=torch.uint8).pin_memory()
